@@ -1,4 +1,4 @@
-"""aloam-b200: B200-native (sm_100a) A-LOAM per-scan registration hot path.
+"""aloam-b200: H100-native (sm_90a) A-LOAM per-scan registration hot path.
 
 Python here is only a ctypes mirror of the C ABI in include/aloam_b200.h (the reference is C++; its host side is
 C++ inside libaloam_b200.so).  There is no CPU fallback: importing works anywhere (so the symbol table can be
@@ -138,7 +138,7 @@ def default_config(n_scans):
 
 
 class Aloam:
-    """One context = one caller thread = one CUDA stream on one B200 (mirrors `aloam_ctx`)."""
+    """One context = one caller thread = one CUDA stream on one GPU (mirrors `aloam_ctx`)."""
 
     def __init__(self, n_scans=64, device=0, max_points=None, **overrides):
         cfg = default_config(n_scans)

@@ -1,4 +1,4 @@
-"""Builds libaloam_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Builds libaloam_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
 -fmad=false everywhere: float32 results must match an x86-64 (no-FMA) build of the reference bit for bit.
 """
@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libaloam_b200.so")
 SOURCES = ["features.cu", "odometry.cu", "lm.cu", "mapping.cu", "comm.cu", "voxel.cu", "cubemap.cu", "capi.cu", "io.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # float32 decision kernels must not contract a*b+c (bit parity with an x86-64 no-FMA build of the reference);
 # lm.cu is double precision, compared at 1e-9, and keeps FMA.
@@ -35,7 +35,7 @@ def build(force=False, verbose=False):
         if r.returncode != 0:
             raise RuntimeError("nvcc failed on " + s)
         objs.append(o)
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", SO] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", SO] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

@@ -1,6 +1,6 @@
 // Host side of the C ABI (include/aloam_b200.h): context, device buffers, kernel sequencing.
 // The reference's host code around the hot path is C++ (the ROS node bodies), so this layer is C++ too.
-// No CPU fallback: every entry point runs the sm_100a kernels or returns an error.
+// No CPU fallback: every entry point runs the sm_90a kernels or returns an error.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -143,6 +143,7 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   const size_t mp = (size_t)c->max_points;
   const size_t mr = (size_t)c->max_ring;
 #define TRY(e) do { if ((e) != cudaSuccess) { fprintf(stderr, "[aloam_b200] %s failed: %s\n", #e, cudaGetErrorString(cudaGetLastError())); aloam_destroy(c); return ALOAM_ERR_CUDA; } } while (0)
+  TRY(cudaDeviceGetAttribute(&c->sms, cudaDevAttrMultiProcessorCount, cfg.device));
   TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   TRY(cudaEventCreate(&c->ev0)); TRY(cudaEventCreate(&c->ev1));
   for (cudaEvent_t& e : c->prof_ev) TRY(cudaEventCreate(&e));

@@ -1,4 +1,4 @@
-// Shared device/host definitions for the sm_100a kernels.  Everything in csrc/ is compiled with -fmad=false:
+// Shared device/host definitions for the sm_90a kernels.  Everything in csrc/ is compiled with -fmad=false:
 // the reference is an x86-64 baseline build (CMakeLists.txt:4-6, no -march => no FMA), and the discrete decisions
 // of the hot path (feature picks, nearest neighbours, voxel indices) depend on float32 results bit for bit.
 #pragma once

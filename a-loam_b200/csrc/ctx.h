@@ -55,6 +55,7 @@ struct aloam_ctx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int max_points = 0, nblocks_max = 0, max_ring = ALOAM_MAX_RING, n_lanes = 1;
+  int sms = 1;                     // SMs of cfg.device (grid-stride launch sizes)
   std::vector<Lane> lanes;
   float* d_curv = nullptr;         // debug outputs of the last extraction (lane 0 only)
   int8_t* d_label = nullptr;

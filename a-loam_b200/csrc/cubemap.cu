@@ -472,7 +472,7 @@ int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, 
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1), dim3(32), 0, 1, true, S, d_out7);
   // ---- insertion (:736-767)
   const int up = std::max(n_upper_c, n_upper_s);
-  launch_ex(c, KID_CUBES, k_cube_ids, dim3(std::max(1, std::min((up + 255) / 256, 148 * 2)), 2), dim3(256), 0, 1, true, (const Pt4*)c->d_stack_corner, (const Pt4*)c->d_stack_surf,
+  launch_ex(c, KID_CUBES, k_cube_ids, dim3(std::max(1, std::min((up + 255) / 256, c->sms * 2)), 2), dim3(256), 0, 1, true, (const Pt4*)c->d_stack_corner, (const Pt4*)c->d_stack_surf,
             (const MapperState*)S, m->d_world, m->d_cube, c->max_points);
   launch_ex(c, KID_CUBES, k_cube_insert, dim3(2), dim3(1024), 0, 1, true, (const Pt4*)m->d_world, (const int*)m->d_cube, c->max_points, S, m->d_pts[0], m->cap[0], m->d_pts[1], m->cap[1]);
   // ---- per-cube re-filter of the valid cubes (:770-801): one segmented pass over <= 150 cubes, in place

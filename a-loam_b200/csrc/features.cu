@@ -553,7 +553,7 @@ __device__ __forceinline__ void st_dsmem_s8(void* local, unsigned rank, int v) {
 
 // RFT = threads of a ring CTA: six warps walk the segments, all of them load, sort and sum.
 //   PAIR = false : one CTA does the whole ring (256 threads, two or three CTAs per SM): batches of trajectories, which fill the GPU.
-//   PAIR = true  : a single trajectory, where the kernel is a latency chain on 64 of 148 SMs.  A ring is processed by a CLUSTER
+//   PAIR = true  : a single trajectory, where the kernel is a latency chain on 64 of the GPU's SMs.  A ring is processed by a CLUSTER
 //                  OF TWO CTAs on two SMs: rank 0 = curvature, greedy picks, labels, the three picked clouds ; rank 1 = the voxel
 //                  sort of the ring, which is made INDEPENDENT of the picks: it sorts every in-range position by its absolute voxel
 //                  coordinates (floor(z/leaf), floor(y/leaf), floor(x/leaf)) -- the same order as PCL's index relative to the
@@ -695,8 +695,8 @@ __device__ __forceinline__ void ring_features_body(const Batch<RingFeatArgs>& B,
     else pick_segment<24>(curv, fb, sp, ep, spill_in, s_less[w], nl, s_flat[w], nf, so, dbg8 && w == 2);
     if (lane == 0) { s_nl[w] = nl; s_nf[w] = nf; s_spill[w] = so; }
   };
-  // Warps 1..6 walk the six segments.  NOT warp 0: it carries the thread that writes the debug stamps, and measured on B200 a
-  // segment walked by warp 0 took 30 k cycles against 9-13 k on any other warp (its REDUX go through the divergent-warp path).
+  // Warps 1..6 walk the six segments.  NOT warp 0: it carries the thread that writes the debug stamps, so its REDUX go
+  // through the divergent-warp path and a segment walk there is slower than on any other warp.
   if (warp >= 1 && warp <= 6) {
     if (dbg8 && lane == 0) g_dbg_pick[8 + 2 * (warp - 1)] = clock64();
     run_segment(warp - 1, 0u);

@@ -3,7 +3,7 @@
 // :106-138 plane-norm) and everything Ceres drives around them (AutoDiff Jacobians, HuberLoss(0.1) + Corrector,
 // EigenQuaternionParameterization, trust-region loop, DENSE_QR step).
 //
-// B200 shape: the whole solve is ONE launch of ONE thread-block cluster (8 CTAs x 288 threads, co-scheduled on one
+// Shape: the whole solve is ONE launch of ONE thread-block cluster (8 CTAs x 288 threads, co-scheduled on one
 // GPC) and never returns to the host.  Each pass evaluates every residual block with the closed-form tangent
 // Jacobian (SURVEY.md 8a "Residual math") and reduces the 28 numbers the 6-dof problem boils down to -- upper
 // triangle of J^T J (21), J^T r (6), cost (1) -- plus the two block counts:
@@ -667,8 +667,8 @@ __device__ __forceinline__ void lm_solve_body(const Batch<LmArgs>& B, const LmPa
       return;   // all remote stores into this CTA preceded the cluster barrier inside cluster_evaluate
     }
     // thread 0 of EVERY CTA takes the same decision from the same totals (no broadcast needed).  The step works on a LOCAL copy
-    // of the state (registers) and of nothing else in shared memory but the two totals vectors: measured, the step was 46 % of the
-    // solve (3.6 k cycles per pass) when every field access went to shared memory behind possibly-aliasing stores.
+    // of the state (registers) and of nothing else in shared memory but the two totals vectors: with every field access going to
+    // shared memory behind possibly-aliasing stores the step took a large share of the solve.
     if (tid == 0) {
       TrState t;
       int next = 0;   // 0: nothing to produce, 1: next candidate from the accepted totals, 2: from the totals just evaluated

@@ -81,8 +81,8 @@ __global__ void k_grid_clear(GridTable a, GridTable b) {
 }
 
 // blockIdx.y selects the cloud (0 = a, 1 = b).  (Grouping the lanes of a cell with __match_any so that one lane claims the slot for
-// the group was measured here: 34.0 us instead of 29.7 us at 1M points -- the vote costs more than the atomics it saves; the
-// fill below does profit from it, 31.8 -> 29.3 us.)
+// the group was tried here and was slower -- the vote costs more than the atomics it saves; the fill below does profit from
+// it.)
 __global__ void k_grid_insert(GridTable a, const Pt4* __restrict__ pa, GridTable b, const Pt4* __restrict__ pb, int shard_rank,
                               int shard_count) {
   pdl_launch_dependents();
@@ -113,7 +113,7 @@ __global__ void k_grid_insert(GridTable a, const Pt4* __restrict__ pa, GridTable
 }
 
 // per-cell storage: block-wide exclusive scan of the counts, ONE atomicAdd per CTA and table on the cursor (a per-slot
-// atomicAdd serialises ~500k updates of a single address: 324 us for a 1M-point map, ncu r01).  Writes the cell's START
+// atomicAdd serialises ~500k updates of a single address for a 1M-point map).  Writes the cell's START
 // into the `end` word; k_grid_fill advances it to the end.
 __global__ void __launch_bounds__(256) k_grid_alloc(GridTable a, GridTable b) {
   pdl_launch_dependents();
@@ -600,7 +600,7 @@ using namespace aloam;
 int comm_allreduce_int2(aloam_ctx* c, int* d_two);   // comm.cu
 
 namespace {
-constexpr int kGridCtas = 148 * 8;   // grid-stride launches: 8 resident CTAs of 256 threads per SM
+inline int grid_ctas(const aloam_ctx* c) { return c->sms * 8; }   // grid-stride launches: 8 resident CTAs of 256 threads per SM
 
 int ensure_map_buffers(aloam_ctx* c) {
   if (c->map_corner.grid.slots) return ALOAM_OK;
@@ -641,9 +641,9 @@ bool is_device_ptr(const void* p) {
 // K0 over two clouds already in device memory; their sizes are in the GridDyn records (host path: written by the caller;
 // mapping loop: k_grid_setup).  n_upper bounds the larger cloud (grid sizing only).
 void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n_upper) {
-  const int pb = std::max(1, std::min((std::max(n_upper, 1) + 255) / 256, kGridCtas));
+  const int pb = std::max(1, std::min((std::max(n_upper, 1) + 255) / 256, grid_ctas(c)));
   const unsigned slots_upper = grid_mask_for(std::max(n_upper, 1), (unsigned)c->map_slots) + 1;
-  const int tb = std::max(1, std::min((int)((slots_upper + 255) / 256), kGridCtas));
+  const int tb = std::max(1, std::min((int)((slots_upper + 255) / 256), grid_ctas(c)));
   launch_ex(c, KID_MAP_GRID, k_grid_clear, dim3(tb), dim3(256), 0, 1, true, c->map_corner.grid, c->map_surf.grid);
   launch_ex(c, KID_MAP_GRID, k_grid_insert, dim3(dim3(pb, 2)), dim3(256), 0, 1, true, c->map_corner.grid, d_corner, c->map_surf.grid, d_surf, c->shard_rank, c->shard_count);
   launch_ex(c, KID_MAP_GRID, k_grid_alloc, dim3(tb), dim3(256), 0, 1, true, c->map_corner.grid, c->map_surf.grid);
@@ -654,7 +654,7 @@ void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n
 void map_register_device(aloam_ctx* c, const Pt4* d_corner_stack, const Pt4* d_surf_stack, const int* d_counts3, int nq_upper,
                          double* d_pose, bool want_fits) {
   const LmParams lp = lm_params(c->cfg);
-  const int kb = std::max(1, std::min((nq_upper + 7) / 8, kGridCtas));
+  const int kb = std::max(1, std::min((nq_upper + 7) / 8, grid_ctas(c)));
   const int fb = std::max(1, (nq_upper + 31) / 32);   // one warp per CTA: a few thousand serial double-precision fits spread over all SMs
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
     launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb), dim3(256), 0, 1, it > 0, d_corner_stack, d_surf_stack, d_counts3, c->map_corner, c->map_surf,
@@ -847,7 +847,7 @@ int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_c
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
   const int nq = corner_stack.n + surf_stack.n;
   if (nq > 0) {
-    LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, kGridCtas), 256, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner,
+    LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, grid_ctas(c)), 256, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner,
            c->map_surf, c->d_map_pose, c->d_nbr, c->shard_rank, c->shard_count);
     LAUNCH(c, KID_MAP_FIT, k_map_fit, (nq + 31) / 32, 32, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->d_nbr, c->d_map_blocks, c->d_fits);
     CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));

@@ -119,8 +119,8 @@ __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B) {
 namespace {
 
 // The visitors below are written for CODE SIZE as much as for loads in flight: every call site of the visitor lambda is
-// inlined, the kernel runs for ~10 us on a cold instruction cache, and an earlier version with ~120 inlined copies of
-// the lambda (13 k SASS instructions) spent more time fetching instructions than data.  Each helper has exactly one
+// inlined, the kernel is short enough to run on a cold instruction cache, and an earlier version with ~120 inlined copies
+// of the lambda (13 k SASS instructions) spent more time fetching instructions than data.  Each helper has exactly one
 // batch of B inlined copies inside a loop that is not unrolled.
 //
 // f(x, y, z, packed) over gpts[e0, e1) with B coalesced float4 loads in flight per lane.  Out-of-range slots are clamped
@@ -142,8 +142,8 @@ __device__ __forceinline__ void visit_span(const float4* __restrict__ gpts, int 
 
 // Ring slice [r_lo, r_hi] of azimuth buckets bq-k and bq+k (the two coincide when 2k == NB): the growth step of a sweep
 // whose first interval was not enough (2 % of the queries).  (A variant that doubles the interval per step -- one
-// delimiter round per step instead of two per bucket -- was measured: it shortens the rare far sweeps but its extra
-// bookkeeping on the common path cost 2 us per launch on average (14.5 -> 16.6 us); bucket-by-bucket growth stays.)
+// delimiter round per step instead of two per bucket -- was tried: it shortens the rare far sweeps but its extra
+// bookkeeping on the common path made the average launch slower; bucket-by-bucket growth stays.)
 template <typename F>
 __device__ __forceinline__ void visit_ring_step(const RabIndex& g, int bq, int k, int r_lo, int r_hi, F&& f) {
   const int b0 = (bq - k + ALOAM_NB) % ALOAM_NB, b1 = (bq + k) % ALOAM_NB;

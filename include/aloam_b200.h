@@ -1,4 +1,4 @@
-/* aloam_b200.h -- C ABI of the B200-native A-LOAM per-scan registration hot path.
+/* aloam_b200.h -- C ABI of the H100-native A-LOAM per-scan registration hot path.
  *
  * The reference (HKUST-Aerial-Robotics/A-LOAM) has NO library / plugin / FFI boundary: the hot path is inline
  * code in three ROS node `main`s.  This header creates the boundary at exactly the seam between the node shells

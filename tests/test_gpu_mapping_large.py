@@ -94,7 +94,7 @@ def test_1m_map_knn_exact(ctx1m, map1m, orc, synth):
 
 
 def test_8m_map_one_gpu(aloam, orc, synth):
-    """configs[3]'s 8M-point map (1.6M corner + 6.4M surf) on one B200: index build + association + register vs the oracle"""
+    """configs[3]'s 8M-point map (1.6M corner + 6.4M surf) on one GPU: index build + association + register vs the oracle"""
     cmap, smap = synth.build_map(_features(orc, synth), 8_000_000)
     m = orc.Mapping(); m.set_map(cmap, smap)
     c = aloam.Aloam(n_scans=64, max_points=200000, max_map_points=6_400_000)

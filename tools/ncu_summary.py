@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One line per kernel launch of an .ncu-rep: duration, DRAM bytes, occupancy, issue activity (for profiles/*.md).
+"""One line per kernel launch of an .ncu-rep: duration, DRAM bytes, occupancy, issue activity.
 usage: python tools/ncu_summary.py <file.ncu-rep>"""
 import csv
 import io
