@@ -15,9 +15,6 @@
 
 extern "C" {
 
-void aloam_map_free_impl(aloam_ctx* c);
-void aloam_comm_free_impl(aloam_ctx* c);
-void aloam_mapper_free_impl(aloam_ctx* c);
 int aloam_map_knn_impl(aloam_ctx* c, int which, aloam_cloud_view queries, int k, int* idx, float* sqdist);
 
 void aloam_default_config(aloam_config* cfg, int n_scans) {
@@ -50,55 +47,11 @@ const char* aloam_strerror(int code) {
   }
 }
 
-static void free_lane(Lane& L) {
-  void* dev[] = {L.d_raw[0], L.d_raw[1], L.d_ring, L.d_hist, L.d_offsets, L.d_scan_start, L.d_scan_end, L.d_ring_start[0], L.d_ring_start[1], L.d_sc,
-                 L.d_full[0], L.d_full[1], L.st_sharp[0], L.st_sharp[1], L.st_less_sharp[0], L.st_less_sharp[1], L.st_flat[0], L.st_flat[1],
-                 L.st_less_flat[0], L.st_less_flat[1], L.st_counts[0], L.st_counts[1], L.d_blocks, L.d_corr, L.d_pose, L.d_world, L.d_summary};
-  for (void* p : dev) if (p) cudaFree(p);
-  for (FeatBuf& f : L.feat) {
-    void* fp[] = {f.sharp, f.less_sharp, f.flat, f.less_flat, f.counts, f.rs_ls, f.rs_lf};
-    for (void* p : fp) if (p) cudaFree(p);
-    for (RabIndex* g : {&f.g_ls, &f.g_lf}) {
-      void* gp[] = {g->cnt, g->start, g->cell_of, g->rank_of, g->gpts};
-      for (void* p : gp) if (p) cudaFree(p);
-    }
-  }
-}
-
 int aloam_destroy(aloam_ctx* c) {
   if (!c) return ALOAM_OK;
   cudaSetDevice(c->cfg.device);
-  cudaStream_t* side[] = {&c->s_ext, &c->s_h2d, &c->s_exa, &c->s_idx, &c->s_map};
-  if (c->stream) cudaStreamSynchronize(c->stream);
-  for (cudaStream_t* s : side) if (*s) { cudaStreamSynchronize(*s); cudaStreamDestroy(*s); }
-  for (cudaEvent_t e : c->ev_idx) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_a) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_b) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_cmp) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_feat) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_odo) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_mapdone) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_h2d) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->ev_rawfree) if (e) cudaEventDestroy(e);
-  if (c->h_poses) cudaFreeHost(c->h_poses);
-  if (c->h_scan_nfull) cudaFreeHost(c->h_scan_nfull);
-  for (Lane& L : c->lanes) free_lane(L);
-  void* dev[] = {c->d_poses, c->d_map_poses, c->d_scan_nfull, c->d_curv, c->d_label, c->d_out28, c->d_api_pose, c->d_packed, c->d_err, c->d_query, c->d_knn_idx, c->d_knn_d};
-  for (void* p : dev) if (p) cudaFree(p);
-  aloam_map_free_impl(c);
-  { void* vp[] = {c->d_vox_keys[0], c->d_vox_keys[1], c->d_vox_vals[0], c->d_vox_vals[1], c->d_vox_hist, c->d_vox_offs, c->d_vox_misc}; for (void* p : vp) if (p) cudaFree(p); }
-  aloam_comm_free_impl(c);
-  aloam_mapper_free_impl(c);
-  for (Pt4* p : c->h_out) if (p) cudaFreeHost(p);
-  if (c->h_vox_out) cudaFreeHost(c->h_vox_out);
-  if (c->h_ints) cudaFreeHost(c->h_ints);
-  if (c->h_dbl) cudaFreeHost(c->h_dbl);
-  if (c->h_summary) cudaFreeHost(c->h_summary);
-  if (c->h_sc) cudaFreeHost(c->h_sc);
-  for (cudaEvent_t e : c->prof_ev) if (e) cudaEventDestroy(e);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  if (c->stream) cudaStreamDestroy(c->stream);
+  for (cudaStream_t s : c->streams) cudaStreamSynchronize(s);
+  for (auto r = c->release.rbegin(); r != c->release.rend(); ++r) (*r)();
   delete c;
   return ALOAM_OK;
 }
@@ -129,6 +82,7 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_batch < 1 || cfg.max_batch > ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_ring_points < 64 || cfg.max_ring_points > ALOAM_MAX_RING_POINTS || cfg.max_ring_points % 32) return ALOAM_ERR_INVALID_ARG;
+  if (cfg.max_map_points > (1 << 30)) return ALOAM_ERR_INVALID_ARG;   // the map's hash-grid slot count is a 32-bit power of two
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return ALOAM_ERR_NO_DEVICE;
   if (cfg.device < 0 || cfg.device >= ndev) return ALOAM_ERR_INVALID_ARG;
@@ -144,58 +98,53 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   const size_t mr = (size_t)c->max_ring;
 #define TRY(e) do { if ((e) != cudaSuccess) { fprintf(stderr, "[aloam_b200] %s failed: %s\n", #e, cudaGetErrorString(cudaGetLastError())); aloam_destroy(c); return ALOAM_ERR_CUDA; } } while (0)
   TRY(cudaDeviceGetAttribute(&c->sms, cudaDevAttrMultiProcessorCount, cfg.device));
-  TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  TRY(cudaEventCreate(&c->ev0)); TRY(cudaEventCreate(&c->ev1));
-  for (cudaEvent_t& e : c->prof_ev) TRY(cudaEventCreate(&e));
-  for (cudaStream_t* s : {&c->s_ext, &c->s_h2d, &c->s_exa, &c->s_idx, &c->s_map}) TRY(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
-  for (cudaEvent_t& e : c->ev_idx) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_a) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_b) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_cmp) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_feat) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_odo) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_mapdone) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_h2d) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  for (cudaEvent_t& e : c->ev_rawfree) TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  TRY(halloc(&c->h_poses, (size_t)kMaxStreamScans * 14)); TRY(dalloc(&c->d_poses, (size_t)kMaxStreamScans * 7)); TRY(dalloc(&c->d_map_poses, (size_t)kMaxStreamScans * 7));
-  TRY(halloc(&c->h_scan_nfull, (size_t)kMaxStreamScans)); TRY(dalloc(&c->d_scan_nfull, (size_t)kMaxStreamScans));
-  TRY(dalloc(&c->d_curv, mp)); TRY(dalloc(&c->d_label, mp));
+  TRY(screate(c, &c->stream));
+  TRY(ecreate(c, &c->ev0, cudaEventDefault)); TRY(ecreate(c, &c->ev1, cudaEventDefault));
+  for (cudaEvent_t& e : c->prof_ev) TRY(ecreate(c, &e, cudaEventDefault));
+  for (cudaStream_t* s : {&c->s_ext, &c->s_h2d, &c->s_exa, &c->s_idx, &c->s_map}) TRY(screate(c, s));
+  const std::pair<cudaEvent_t*, int> scan_events[] = {{c->ev_idx, kFeatSlots}, {c->ev_a, 2}, {c->ev_b, 2}, {c->ev_cmp, 2}, {c->ev_feat, kFeatSlots},
+                                                      {c->ev_odo, kFeatSlots}, {c->ev_mapdone, kFeatSlots}, {c->ev_h2d, 2}, {c->ev_rawfree, 2}};
+  for (const auto& a : scan_events)
+    for (int i = 0; i < a.second; ++i) TRY(ecreate(c, &a.first[i], cudaEventDisableTiming));
+  TRY(halloc(c, &c->h_poses, (size_t)kMaxStreamScans * 14)); TRY(dalloc(c, &c->d_poses, (size_t)kMaxStreamScans * 7)); TRY(dalloc(c, &c->d_map_poses, (size_t)kMaxStreamScans * 7));
+  TRY(halloc(c, &c->h_scan_nfull, (size_t)kMaxStreamScans)); TRY(dalloc(c, &c->d_scan_nfull, (size_t)kMaxStreamScans));
+  TRY(dalloc(c, &c->d_curv, mp)); TRY(dalloc(c, &c->d_label, mp));
   c->lanes.resize(c->n_lanes);
   ScanScalars init[3];
   for (ScanScalars& s : init) { s.first_valid = INT32_MAX; s.last_valid = -1; s.half_idx = INT32_MAX; s.n_full = 0; s.start_ori = 0; s.end_ori = 0; s.error = 0; s.pad = 0; }
   for (Lane& L : c->lanes) {
     for (int b = 0; b < 2; ++b) {
-      TRY(dalloc(&L.d_raw[b], mp * 8)); TRY(dalloc(&L.d_full[b], mp)); TRY(dalloc(&L.d_ring_start[b], 72));
-      TRY(dalloc(&L.st_sharp[b], 64 * kMaxSharpPerRing)); TRY(dalloc(&L.st_less_sharp[b], 64 * kMaxLessSharpPerRing));
-      TRY(dalloc(&L.st_flat[b], 64 * kMaxFlatPerRing)); TRY(dalloc(&L.st_less_flat[b], (size_t)64 * mr));
-      TRY(dalloc(&L.st_counts[b], 64 * 4));
+      TRY(dalloc(c, &L.d_raw[b], mp * 8)); TRY(dalloc(c, &L.d_full[b], mp)); TRY(dalloc(c, &L.d_ring_start[b], 72));
+      TRY(dalloc(c, &L.st_sharp[b], 64 * kMaxSharpPerRing)); TRY(dalloc(c, &L.st_less_sharp[b], 64 * kMaxLessSharpPerRing));
+      TRY(dalloc(c, &L.st_flat[b], 64 * kMaxFlatPerRing)); TRY(dalloc(c, &L.st_less_flat[b], (size_t)64 * mr));
+      TRY(dalloc(c, &L.st_counts[b], 64 * 4));
     }
-    TRY(dalloc(&L.d_ring, mp));
-    TRY(dalloc(&L.d_hist, (size_t)c->nblocks_max * 64)); TRY(dalloc(&L.d_offsets, (size_t)c->nblocks_max * 64));
-    TRY(dalloc(&L.d_scan_start, 64)); TRY(dalloc(&L.d_scan_end, 64));
-    TRY(dalloc(&L.d_sc, 3));
+    TRY(dalloc(c, &L.d_ring, mp));
+    TRY(dalloc(c, &L.d_hist, (size_t)c->nblocks_max * 64)); TRY(dalloc(c, &L.d_offsets, (size_t)c->nblocks_max * 64));
+    TRY(dalloc(c, &L.d_scan_start, 64)); TRY(dalloc(c, &L.d_scan_end, 64));
+    TRY(dalloc(c, &L.d_sc, 3));
     TRY(cudaMemcpy(L.d_sc, init, sizeof(init), cudaMemcpyHostToDevice));
     for (FeatBuf& f : L.feat) {
-      TRY(dalloc(&f.sharp, kMaxQueries)); TRY(dalloc(&f.flat, kMaxQueries));
-      TRY(dalloc(&f.less_sharp, mp)); TRY(dalloc(&f.less_flat, mp));
-      TRY(dalloc(&f.counts, 4)); TRY(dalloc(&f.rs_ls, 72)); TRY(dalloc(&f.rs_lf, 72));
+      TRY(dalloc(c, &f.sharp, kMaxQueries)); TRY(dalloc(c, &f.flat, kMaxQueries));
+      TRY(dalloc(c, &f.less_sharp, mp)); TRY(dalloc(c, &f.less_flat, mp));
+      TRY(dalloc(c, &f.counts, 4)); TRY(dalloc(c, &f.rs_ls, 72)); TRY(dalloc(c, &f.rs_lf, 72));
       for (RabIndex* g : {&f.g_ls, &f.g_lf}) {
-        TRY(dalloc(&g->cnt, (size_t)ALOAM_NB * 64)); TRY(dalloc(&g->start, (size_t)ALOAM_NB * 64 + 8));
-        TRY(dalloc(&g->cell_of, mp)); TRY(dalloc(&g->rank_of, mp)); TRY(dalloc(&g->gpts, mp));
+        TRY(dalloc(c, &g->cnt, (size_t)ALOAM_NB * 64)); TRY(dalloc(c, &g->start, (size_t)ALOAM_NB * 64 + 8));
+        TRY(dalloc(c, &g->cell_of, mp)); TRY(dalloc(c, &g->rank_of, mp)); TRY(dalloc(c, &g->gpts, mp));
         TRY(cudaMemset(g->cnt, 0, (size_t)ALOAM_NB * 64 * 4)); TRY(cudaMemset(g->start, 0, ((size_t)ALOAM_NB * 64 + 8) * 4));
       }
       TRY(cudaMemset(f.counts, 0, 16)); TRY(cudaMemset(f.rs_ls, 0, 72 * 4)); TRY(cudaMemset(f.rs_lf, 0, 72 * 4));
     }
-    TRY(dalloc(&L.d_blocks, (size_t)2 * kMaxQueries)); TRY(dalloc(&L.d_corr, (size_t)2 * kMaxQueries * 4));
-    TRY(dalloc(&L.d_pose, 8)); TRY(dalloc(&L.d_world, 8)); TRY(dalloc(&L.d_summary, 4));
+    TRY(dalloc(c, &L.d_blocks, (size_t)2 * kMaxQueries)); TRY(dalloc(c, &L.d_corr, (size_t)2 * kMaxQueries * 4));
+    TRY(dalloc(c, &L.d_pose, 8)); TRY(dalloc(c, &L.d_world, 8)); TRY(dalloc(c, &L.d_summary, 4));
   }
-  TRY(dalloc(&c->d_out28, 32)); TRY(dalloc(&c->d_api_pose, 8));
-  TRY(dalloc(&c->d_packed, (size_t)2 * kMaxQueries * 11));
-  TRY(dalloc(&c->d_err, 4));
-  TRY(dalloc(&c->d_query, mp)); TRY(dalloc(&c->d_knn_idx, mp)); TRY(dalloc(&c->d_knn_d, mp));
-  for (int k = 0; k < 5; ++k) TRY(halloc(&c->h_out[k], k == 0 || k == 4 ? mp : (size_t)kMaxQueries));
-  TRY(halloc(&c->h_ints, 4096)); TRY(halloc(&c->h_dbl, 4096));
-  TRY(halloc(&c->h_summary, (size_t)4 * c->n_lanes)); TRY(halloc(&c->h_sc, (size_t)3 * c->n_lanes));
+  TRY(dalloc(c, &c->d_out28, 32)); TRY(dalloc(c, &c->d_api_pose, 8));
+  TRY(dalloc(c, &c->d_packed, (size_t)2 * kMaxQueries * 11));
+  TRY(dalloc(c, &c->d_err, 4));
+  TRY(dalloc(c, &c->d_query, mp)); TRY(dalloc(c, &c->d_knn_idx, mp)); TRY(dalloc(c, &c->d_knn_d, mp));
+  for (int k = 0; k < 5; ++k) TRY(halloc(c, &c->h_out[k], k == 0 || k == 4 ? mp : (size_t)kMaxQueries));
+  TRY(halloc(c, &c->pin, 1));
+  TRY(halloc(c, &c->h_summary, (size_t)4 * c->n_lanes)); TRY(halloc(c, &c->h_sc, (size_t)3 * c->n_lanes));
   TRY(cudaMemset(c->d_err, 0, 16));
   // function attributes are process-wide: always opt in to the largest ring capacity, whatever this context uses
   TRY(cudaFuncSetAttribute(k_ring_features, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring_features_smem_bytes(ALOAM_MAX_RING, true)));
@@ -347,7 +296,7 @@ int aloam_extract_features(aloam_ctx* c, aloam_cloud_view raw, aloam_cloud_view*
   const float* rp = L.d_raw[0];
   rc = run_features(c, 1, &rp, &raw.n, raw.stride_floats, kApiCur);
   if (rc) return rc;
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints, f.counts, 16, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->feat_counts, f.counts, 16, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_sc, L.d_sc + slot, sizeof(ScanScalars), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   if (c->h_sc->error) {
@@ -358,7 +307,8 @@ int aloam_extract_features(aloam_ctx* c, aloam_cloud_view raw, aloam_cloud_view*
   const int n_full = c->h_sc->n_full;
   c->last_n_full = n_full;
   if (c->h_sc->first_valid == INT32_MAX) return ALOAM_ERR_EMPTY_CLOUD;
-  const int n[5] = {n_full, c->h_ints[0], c->h_ints[1], c->h_ints[2], c->h_ints[3]};
+  const int* fc = c->pin->feat_counts;
+  const int n[5] = {n_full, fc[0], fc[1], fc[2], fc[3]};
   const Pt4* src[5] = {L.d_full[0], f.sharp, f.less_sharp, f.flat, f.less_flat};
   for (int k = 0; k < 5; ++k)
     if (n[k] > 0) CUDA_CHECK_RET(cudaMemcpyAsync(c->h_out[k], src[k], (size_t)n[k] * 16, cudaMemcpyDeviceToHost, c->stream));
@@ -392,18 +342,19 @@ int aloam_odometry_set_last(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cl
   FeatBuf& f = c->lanes[0].feat[kApiLast];
   rc = upload_cloud(c, corner_last, f.less_sharp, c->max_points); if (rc) return rc;
   rc = upload_cloud(c, surf_last, f.less_flat, c->max_points); if (rc) return rc;
-  c->h_ints[0] = 0; c->h_ints[1] = corner_last.n; c->h_ints[2] = 0; c->h_ints[3] = surf_last.n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, c->h_ints, 16, cudaMemcpyHostToDevice, c->stream));
+  int* lc = c->pin->last_counts;
+  lc[0] = 0; lc[1] = corner_last.n; lc[2] = 0; lc[3] = surf_last.n;
+  CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, lc, 16, cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(f.rs_ls, 0, 72 * 4, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(f.rs_lf, 0, 72 * 4, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
   if (corner_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (corner_last.n + 255) / 256, 256, 0, f.less_sharp, corner_last.n, f.rs_ls, c->d_err);
   if (surf_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (surf_last.n + 255) / 256, 256, 0, f.less_flat, surf_last.n, f.rs_lf, c->d_err);
   run_grid_build(c, 1, kApiLast, corner_last.n, surf_last.n);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 8, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
-  if (c->h_ints[8]) return ALOAM_ERR_NOT_RING_MAJOR;
+  if (c->pin->ring_err) return ALOAM_ERR_NOT_RING_MAJOR;
   c->have_last = true;
   return ALOAM_OK;
 }
@@ -413,8 +364,9 @@ static int upload_queries(aloam_ctx* c, aloam_cloud_view sharp, aloam_cloud_view
   rc = check_view(flat); if (rc) return rc;
   rc = upload_cloud(c, sharp, f.sharp, kMaxQueries); if (rc) return rc;
   rc = upload_cloud(c, flat, f.flat, kMaxQueries); if (rc) return rc;
-  c->h_ints[16] = sharp.n; c->h_ints[17] = 0; c->h_ints[18] = flat.n; c->h_ints[19] = 0;
-  CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, c->h_ints + 16, 16, cudaMemcpyHostToDevice, c->stream));
+  int* qc = c->pin->query_counts;
+  qc[0] = sharp.n; qc[1] = 0; qc[2] = flat.n; qc[3] = 0;
+  CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, qc, 16, cudaMemcpyHostToDevice, c->stream));
   return ALOAM_OK;
 }
 
@@ -425,19 +377,19 @@ int aloam_odometry_register(aloam_ctx* c, aloam_cloud_view sharp, aloam_cloud_vi
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   Lane& L = c->lanes[0];
   int rc = upload_queries(c, sharp, flat, L.feat[kApiCur]); if (rc) return rc;
-  for (int k = 0; k < 4; ++k) c->h_dbl[k] = q[k];
-  for (int k = 0; k < 3; ++k) c->h_dbl[4 + k] = t[k];
+  for (int k = 0; k < 4; ++k) c->pin->pose_in[k] = q[k];
+  for (int k = 0; k < 3; ++k) c->pin->pose_in[4 + k] = t[k];
   CUDA_CHECK_RET(cudaEventRecord(c->ev0, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   run_register(c, 1, kApiCur, kApiLast, sharp.n, flat.n, false, false, nullptr, c->d_api_pose);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 8, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   prof_collect(c);
-  for (int k = 0; k < 4; ++k) q[k] = c->h_dbl[8 + k];
-  for (int k = 0; k < 3; ++k) t[k] = c->h_dbl[12 + k];
+  for (int k = 0; k < 4; ++k) q[k] = c->pin->pose_out[k];
+  for (int k = 0; k < 3; ++k) t[k] = c->pin->pose_out[4 + k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   fill_stats(c, stats, c->cfg.outer_iters, 0, ms);
   return ALOAM_OK;
@@ -451,9 +403,9 @@ int aloam_odometry_associate(aloam_ctx* c, aloam_cloud_view sharp, aloam_cloud_v
   Lane& L = c->lanes[0];
   FeatBuf& cur = L.feat[kApiCur];
   int rc = upload_queries(c, sharp, flat, cur); if (rc) return rc;
-  for (int k = 0; k < 4; ++k) c->h_dbl[k] = q[k];
-  for (int k = 0; k < 3; ++k) c->h_dbl[4 + k] = t[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 4; ++k) c->pin->pose_in[k] = q[k];
+  for (int k = 0; k < 3; ++k) c->pin->pose_in[4 + k] = t[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   OdomParams op{c->cfg.dist_sq_thresh, c->cfg.nearby_scan, c->cfg.distortion};
   const int slots = sharp.n + flat.n;
   if (slots > 0) {
@@ -499,7 +451,7 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
     run_register(c, 1, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, nullptr);
   }
   CUDA_CHECK_RET(cudaEventRecord(c->ev_odo[cur], c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 16, L.d_world, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->world, L.d_world, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_sc, L.d_sc + slot, sizeof(ScanScalars), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
@@ -513,8 +465,8 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
   }
   if (c->h_sc->first_valid == INT32_MAX) return ALOAM_ERR_EMPTY_CLOUD;
   c->last_n_full = c->h_sc->n_full;
-  for (int k = 0; k < 4; ++k) q_w[k] = c->h_dbl[16 + k];
-  for (int k = 0; k < 3; ++k) t_w[k] = c->h_dbl[20 + k];
+  for (int k = 0; k < 4; ++k) q_w[k] = c->pin->world[k];
+  for (int k = 0; k < 3; ++k) t_w[k] = c->pin->world[4 + k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (c->frame == 0) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = flags; stats->ms_total = ms; } }
   else fill_stats(c, stats, c->cfg.outer_iters, flags, ms);
@@ -739,9 +691,9 @@ int aloam_transform_to_end(aloam_ctx* c, aloam_cloud_view in, const double q[4],
   out->data = reinterpret_cast<const float*>(c->h_out[0]); out->n = in.n; out->stride_floats = 4;
   if (in.n == 0) return ALOAM_OK;
   rc = upload_cloud(c, in, c->d_query, c->max_points); if (rc) return rc;
-  for (int k = 0; k < 4; ++k) c->h_dbl[k] = q[k];
-  for (int k = 0; k < 3; ++k) c->h_dbl[4 + k] = t[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_out28, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 4; ++k) c->pin->pose_in[k] = q[k];
+  for (int k = 0; k < 3; ++k) c->pin->pose_in[4 + k] = t[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_out28, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   Pt4* d_out = c->lanes[0].d_full[0];
   LAUNCH(c, KID_KNN_LAST, k_transform_to_end, (in.n + 255) / 256, 256, 0, c->d_query, in.n, c->d_out28, distortion, d_out);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_out[0], d_out, (size_t)in.n * 16, cudaMemcpyDeviceToHost, c->stream));
@@ -757,12 +709,12 @@ static int run_lm_api(aloam_ctx* c, const double* blocks, int n_blocks, const do
     CUDA_CHECK_RET(cudaMemcpyAsync(c->d_packed, blocks, (size_t)n_blocks * 11 * 8, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_PACK_BLOCKS, k_pack_blocks, (n_blocks + 255) / 256, 256, 0, c->d_packed, n_blocks, L.d_blocks);
   }
-  for (int k = 0; k < 7; ++k) c->h_dbl[k] = x[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   launch_lm(c, false, (const BlockRec*)L.d_blocks, (const int*)nullptr, n_blocks, c->d_api_pose, lm_params(c->cfg), L.d_summary, mode,
             c->d_out28, (double*)nullptr, 0, true /* blocks from the caller may carry any interpolation ratio */);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 8, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 32, c->d_out28, 28 * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->ne, c->d_out28, 28 * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -775,7 +727,7 @@ int aloam_normal_equations(aloam_ctx* c, const double* blocks, int n_blocks, con
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   int rc = run_lm_api(c, blocks, n_blocks, x, 1);
   if (rc) return rc;
-  const double* o = c->h_dbl + 32;
+  const double* o = c->pin->ne;
   int k = 0;
   for (int a = 0; a < 6; ++a)
     for (int b = a; b < 6; ++b) { JtJ[6 * a + b] = o[k]; JtJ[6 * b + a] = o[k]; ++k; }
@@ -790,7 +742,7 @@ int aloam_solve(aloam_ctx* c, const double* blocks, int n_blocks, double x[7], d
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   int rc = run_lm_api(c, blocks, n_blocks, x, 0);
   if (rc) return rc;
-  for (int k = 0; k < 7; ++k) x[k] = c->h_dbl[8 + k];
+  for (int k = 0; k < 7; ++k) x[k] = c->pin->pose_out[k];
   const LmSummary& s = c->h_summary[0];
   if (summary7) {
     summary7[0] = s.termination; summary7[1] = s.num_iterations; summary7[2] = s.num_successful; summary7[3] = s.num_jac_evals;

@@ -47,6 +47,22 @@ struct PeerState {
   void* opened[ALOAM_MAX_RANKS] = {};  // peers' mailboxes mapped into this process (cudaIpcOpenMemHandle)
 };
 
+// unmaps the peers' mailboxes, frees this rank's and forgets the peer state (back to the NCCL path)
+static void peer_drop(aloam_ctx* c) {
+  PeerState* ps = static_cast<PeerState*>(c->peer);
+  if (!ps) return;
+  for (void* p : ps->opened) if (p) cudaIpcCloseMemHandle(p);
+  if (ps->own) cudaFree(ps->own);
+  delete ps;
+  c->peer = nullptr;
+}
+
+// a device buffer that lives for one call
+template <typename T> struct DeviceTemp {
+  T* p = nullptr;
+  ~DeviceTemp() { if (p) cudaFree(p); }
+};
+
 void launch_lm_sharded(aloam_ctx* c, const BlockRec* blocks, const int* d_n, double* pose, const LmParams& lp, LmSummary* summary) {
   if (c->peer) {
     // ONE launch per solve: the cluster kernel of the single-GPU path with the all-reduce of every evaluation done inside it
@@ -82,24 +98,24 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
   if (getenv("ALOAM_NO_PEER") || world > ALOAM_MAX_RANKS || !g_nccl.AllGather) return false;
   PeerState* ps = new (std::nothrow) PeerState();
   if (!ps) return false;
+  c->peer = ps;
   const size_t box_bytes = (size_t)2 * world * 32 * 2 * sizeof(unsigned long long), flag_bytes = (size_t)2 * world * sizeof(unsigned);
   const size_t total = box_bytes + flag_bytes + 64 + 2 * 32 * sizeof(double) + 64;
   bool ok = cudaMalloc(&ps->own, total) == cudaSuccess && cudaMemset(ps->own, 0, total) == cudaSuccess;
   cudaIpcMemHandle_t mine;
   ok = ok && cudaIpcGetMemHandle(&mine, ps->own) == cudaSuccess;
-  cudaIpcMemHandle_t* d_all = nullptr;
+  DeviceTemp<cudaIpcMemHandle_t> d_all;
   std::vector<cudaIpcMemHandle_t> all(world);
-  ok = ok && cudaMalloc((void**)&d_all, sizeof(mine) * (world + 1)) == cudaSuccess;
+  ok = ok && cudaMalloc((void**)&d_all.p, sizeof(mine) * (world + 1)) == cudaSuccess;
   // every rank must take part in the gather even if its own setup failed: a zeroed handle marks the failure
   if (!ok) std::memset(&mine, 0, sizeof(mine));
   bool gathered = false;
-  if (d_all) {
-    cudaMemcpyAsync(d_all + world, &mine, sizeof(mine), cudaMemcpyHostToDevice, c->stream);
-    if (g_nccl.AllGather(d_all + world, d_all, sizeof(mine), ncclChar, (ncclComm_t)c->comm, c->stream) == ncclSuccess &&
-        cudaMemcpyAsync(all.data(), d_all, sizeof(mine) * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess &&
+  if (d_all.p) {
+    cudaMemcpyAsync(d_all.p + world, &mine, sizeof(mine), cudaMemcpyHostToDevice, c->stream);
+    if (g_nccl.AllGather(d_all.p + world, d_all.p, sizeof(mine), ncclChar, (ncclComm_t)c->comm, c->stream) == ncclSuccess &&
+        cudaMemcpyAsync(all.data(), d_all.p, sizeof(mine) * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess &&
         cudaStreamSynchronize(c->stream) == cudaSuccess)
       gathered = true;
-    cudaFree(d_all);
   }
   ok = ok && gathered;
   const cudaIpcMemHandle_t zero = {};
@@ -114,18 +130,16 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
   }
   if (!ok) {
     cudaGetLastError();
-    for (void* p : ps->opened) if (p) cudaIpcCloseMemHandle(p);
-    if (ps->own) cudaFree(ps->own);
-    delete ps;
+    peer_drop(c);
     fprintf(stderr, "[aloam_b200] peer-memory exchange unavailable on rank %d: the sharded LM uses ncclAllReduce\n", rank);
     return false;
   }
-  char* own = static_cast<char*>(ps->own);
-  ps->px.seq = reinterpret_cast<unsigned long long*>(own + box_bytes + flag_bytes);
-  ps->px.gtot = reinterpret_cast<double*>(own + box_bytes + flag_bytes + 64);
-  ps->px.err = reinterpret_cast<int*>(own + box_bytes + flag_bytes + 64 + 2 * 32 * sizeof(double));
+  char* mbox = static_cast<char*>(ps->own);
+  ps->px.seq = reinterpret_cast<unsigned long long*>(mbox + box_bytes + flag_bytes);
+  ps->px.gtot = reinterpret_cast<double*>(mbox + box_bytes + flag_bytes + 64);
+  ps->px.err = reinterpret_cast<int*>(mbox + box_bytes + flag_bytes + 64 + 2 * 32 * sizeof(double));
   ps->px.rank = rank; ps->px.world = world;
-  c->peer = ps;
+  own(c, [c] { peer_drop(c); });
   return true;
 }
 
@@ -138,20 +152,6 @@ int comm_allreduce_int2(aloam_ctx* c, int* d_two) {
 }
 
 extern "C" {
-
-void aloam_comm_free_impl(aloam_ctx* c) {
-  if (c->comm && g_nccl.CommDestroy) { g_nccl.CommDestroy((ncclComm_t)c->comm); c->comm = nullptr; }
-  if (c->peer) {
-    PeerState* ps = static_cast<PeerState*>(c->peer);
-    for (void* p : ps->opened) if (p) cudaIpcCloseMemHandle(p);
-    if (ps->own) cudaFree(ps->own);
-    delete ps;
-    c->peer = nullptr;
-  }
-  if (c->d_lm_tot) cudaFree(c->d_lm_tot);
-  if (c->d_lm_state) cudaFree(c->d_lm_state);
-  c->d_lm_tot = nullptr; c->d_lm_state = nullptr;
-}
 
 // rank 0 creates the 128-byte NCCL id; the caller ships it to the other ranks (e.g. torch.distributed.broadcast)
 int aloam_comm_unique_id(char out128[128]) {
@@ -178,28 +178,23 @@ int aloam_comm_init(aloam_ctx* c, int rank, int world, const char id128[128]) {
   ncclResult_t r = g_nccl.CommInitRank(&comm, world, id, rank);
   if (r != ncclSuccess) { fprintf(stderr, "[aloam_b200] ncclCommInitRank failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?"); return ALOAM_ERR_COMM; }
   c->comm = comm;
-  if (!c->d_lm_tot) CUDA_CHECK_RET(cudaMalloc((void**)&c->d_lm_tot, 64 * sizeof(double)));
-  if (!c->d_lm_state) CUDA_CHECK_RET(cudaMalloc(&c->d_lm_state, lm_state_bytes()));
+  own(c, [comm] { g_nccl.CommDestroy(comm); });   // an earlier communicator of this context lives on until aloam_destroy
+  if (!c->d_lm_tot) CUDA_CHECK_RET(dalloc(c, &c->d_lm_tot, 64));
+  if (!c->d_lm_state) CUDA_CHECK_RET(dalloc(c, reinterpret_cast<char**>(&c->d_lm_state), lm_state_bytes()));
   c->shard_rank = rank; c->shard_count = world;
   // the 256-byte exchange of every LM evaluation goes through NVLink peer memory inside the solve kernel when the ranks can map
   // each other's memory (all ranks decide alike: the outcome of the handle exchange is the same everywhere ... see below)
+  peer_drop(c);   // the peer path of an earlier communicator
   const bool mine_ok = peer_setup(c, rank, world);
   // agree on the path: one rank without peer access forces everybody onto NCCL
-  int* d_flag = nullptr;
-  CUDA_CHECK_RET(cudaMalloc((void**)&d_flag, 2 * sizeof(int)));
+  DeviceTemp<int> d_flag;
+  CUDA_CHECK_RET(cudaMalloc((void**)&d_flag.p, 2 * sizeof(int)));
   int h[2] = {mine_ok ? 0 : 1, 0};
-  CUDA_CHECK_RET(cudaMemcpyAsync(d_flag, h, 8, cudaMemcpyHostToDevice, c->stream));
-  if (g_nccl.AllReduce(d_flag, d_flag, 2, ncclInt32, ncclSum, (ncclComm_t)c->comm, c->stream) != ncclSuccess) { cudaFree(d_flag); return ALOAM_ERR_COMM; }
-  CUDA_CHECK_RET(cudaMemcpyAsync(h, d_flag, 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(d_flag.p, h, 8, cudaMemcpyHostToDevice, c->stream));
+  if (g_nccl.AllReduce(d_flag.p, d_flag.p, 2, ncclInt32, ncclSum, (ncclComm_t)c->comm, c->stream) != ncclSuccess) return ALOAM_ERR_COMM;
+  CUDA_CHECK_RET(cudaMemcpyAsync(h, d_flag.p, 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  cudaFree(d_flag);
-  if (h[0] != 0 && c->peer) {   // somebody failed: drop the peer path here too
-    PeerState* ps = static_cast<PeerState*>(c->peer);
-    for (void* p : ps->opened) if (p) cudaIpcCloseMemHandle(p);
-    if (ps->own) cudaFree(ps->own);
-    delete ps;
-    c->peer = nullptr;
-  }
+  if (h[0] != 0) peer_drop(c);   // somebody failed: drop the peer path here too
   return ALOAM_OK;
 }
 

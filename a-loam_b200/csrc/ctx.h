@@ -4,6 +4,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <vector>
 #include "../../include/aloam_b200.h"
@@ -48,6 +49,28 @@ struct Lane {
   LmSummary* d_summary = nullptr;                // [4]
 };
 
+// Pinned scratch of the synchronous entry points: one field per purpose.  The host->device copies from here are
+// asynchronous, so two uses that share a field before their synchronise would race.
+struct PinnedScratch {
+  int feat_counts[4];       // aloam_extract_features: n_sharp, n_less_sharp, n_flat, n_less_flat
+  int last_counts[4];       // aloam_odometry_set_last: counts of the "last" feature set
+  int ring_err;             // aloam_odometry_set_last: ring-order error word
+  int query_counts[4];      // sharp / flat query counts (odometry register / associate)
+  GridDyn grid[2];          // aloam_map_upload: corner, surf
+  int owned[2];             // sharded map upload: points in owned cells, summed over the ranks
+  int shard[3];             // aloam_map_upload_sharded: points kept (corner, surf), error word
+  int stack_counts[3];      // scan-to-map stacks: n_corner, n_surf, total
+  int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
+  int vox_init[6];          // aloam_voxel_filter: initial bounding box (ordered-int min xyz, max xyz)
+  int vox_n;                //                     input size
+  int vox_box[6];           //                     bounding box of the cloud
+  int vox_out_n;            //                     output size
+  double pose_in[7], pose_out[7];             // pose of the per-stage entry points
+  double world[7];                            // fused pipeline: world pose of the scan
+  double ne[28];                              // normal equations: J^T J upper 21, J^T r 6, cost
+  double mapper_pose_in[7], mapper_pose_out[7];
+};
+
 }  // namespace
 
 struct aloam_ctx {
@@ -80,6 +103,7 @@ struct aloam_ctx {
   int map_n[2] = {0, 0};          // points indexed on this rank (corner, surf)
   int map_global_n[2] = {0, 0};   // size of the whole submap (== map_n unless the map is sharded over ranks)
   bool have_map = false;
+  bool map_ready = false;         // every buffer of this group is allocated (set last by ensure_map_buffers)
   Pt4 *d_stack_corner = nullptr, *d_stack_surf = nullptr;
   int* d_stack_counts = nullptr;  // [4] {n_corner, n_surf, total} of the stacks being registered
   float4* d_nbr = nullptr;        // [queries][5] neighbours found by k_map_knn5 (x, y, z, index bits)
@@ -91,6 +115,7 @@ struct aloam_ctx {
   unsigned* d_vox_keys[2] = {nullptr, nullptr};
   int* d_vox_vals[2] = {nullptr, nullptr};
   int *d_vox_hist = nullptr, *d_vox_offs = nullptr, *d_vox_misc = nullptr;
+  bool vox_ready = false;         // every buffer of this group is allocated
   // pipelined scan stream: ring binning on s_exa, per-ring features on s_ext, compaction + index on s_idx, association + LM
   // on `stream`, host->device copies of the raw scans on s_h2d, scan-to-map on s_map; all chained by events
   cudaStream_t s_ext = nullptr, s_exa = nullptr, s_idx = nullptr, s_h2d = nullptr, s_map = nullptr;
@@ -103,8 +128,7 @@ struct aloam_ctx {
   // pinned host mirrors
   Pt4* h_out[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   Pt4* h_vox_out = nullptr;     // result of aloam_voxel_filter (never aliases the feature views)
-  int* h_ints = nullptr;        // scratch ints (counts etc.)
-  double* h_dbl = nullptr;      // scratch doubles
+  PinnedScratch* pin = nullptr;
   LmSummary* h_summary = nullptr;   // [n_lanes][4]
   ScanScalars* h_sc = nullptr;      // [n_lanes][3]
   // per-kernel profiler (bench.py roofline leg) + cumulative launch counter
@@ -121,6 +145,10 @@ struct aloam_ctx {
   int cur = 0;            // fused pipeline: feat[] slot of the most recent scan
   bool have_last = false; // API path: set_last called
   int last_n_full = 0;
+  // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
+  // runs `release` in reverse order of acquisition
+  std::vector<cudaStream_t> streams;
+  std::vector<std::function<void()>> release;
 };
 
 namespace {
@@ -192,8 +220,7 @@ inline void launch_lm(aloam_ctx* c, bool pdl, const BlockRec* blocks, const int*
 // sharded LM (comm.cu): per evaluation one kernel for the local blocks, one exchange of 32 doubles, one step kernel
 void launch_lm_sharded(aloam_ctx* c, const aloam::BlockRec* blocks, const int* d_n, double* pose, const aloam::LmParams& lp, aloam::LmSummary* summary);
 void vox_seg_filter(aloam_ctx* c, const aloam::SegFilter& f, aloam::SegBuffers& b, int S_upper, int n_upper, int per_seg_upper);
-int vox_seg_alloc(aloam::SegBuffers& b, size_t cap);
-void vox_seg_free(aloam::SegBuffers& b);
+int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, int n_upper_c, const Pt4* d_surf_last, const int* d_ns, int n_upper_s,
                        const double* d_odom7, double* d_out7);
 void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n_upper);
@@ -211,8 +238,28 @@ LmParams lm_params(const aloam_config& c) {
   return p;
 }
 
-template <typename T> cudaError_t dalloc(T** p, size_t n) { return cudaMalloc((void**)p, n * sizeof(T)); }
-template <typename T> cudaError_t halloc(T** p, size_t n) { return cudaMallocHost((void**)p, n * sizeof(T)); }
+// acquisition helpers: what they return belongs to the context and is released by aloam_destroy
+inline void own(aloam_ctx* c, std::function<void()> f) { c->release.push_back(std::move(f)); }
+template <typename T> cudaError_t dalloc(aloam_ctx* c, T** p, size_t n) {
+  const cudaError_t e = cudaMalloc((void**)p, n * sizeof(T));
+  if (e == cudaSuccess) { void* q = *p; own(c, [q] { cudaFree(q); }); }
+  return e;
+}
+template <typename T> cudaError_t halloc(aloam_ctx* c, T** p, size_t n) {
+  const cudaError_t e = cudaMallocHost((void**)p, n * sizeof(T));
+  if (e == cudaSuccess) { void* q = *p; own(c, [q] { cudaFreeHost(q); }); }
+  return e;
+}
+inline cudaError_t screate(aloam_ctx* c, cudaStream_t* s) {
+  const cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+  if (e == cudaSuccess) { const cudaStream_t q = *s; c->streams.push_back(q); own(c, [q] { cudaStreamDestroy(q); }); }
+  return e;
+}
+inline cudaError_t ecreate(aloam_ctx* c, cudaEvent_t* ev, unsigned flags) {
+  const cudaError_t e = cudaEventCreateWithFlags(ev, flags);
+  if (e == cudaSuccess) { const cudaEvent_t q = *ev; own(c, [q] { cudaEventDestroy(q); }); }
+  return e;
+}
 
 int upload_cloud(aloam_ctx* c, aloam_cloud_view v, Pt4* dst, int capacity) {
   if (v.n < 0 || (v.n > 0 && !v.data) || (v.stride_floats != 4 && v.stride_floats != 8 && v.n > 0)) return ALOAM_ERR_INVALID_ARG;

@@ -23,10 +23,7 @@
 #include "common.cuh"
 #include "ctx.h"
 
-extern "C" {
-void aloam_mapper_free_impl(aloam_ctx* c);
-int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
-}
+extern "C" int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
 
 namespace {
 
@@ -367,33 +364,33 @@ int ensure_mapper(aloam_ctx* c) {
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   Mapper* m = new (std::nothrow) Mapper();
   if (!m) return ALOAM_ERR_CUDA;
+  own(c, [m] { delete m; });
   m->cap[0] = std::min(16384, c->max_points);
   m->cap[1] = std::min(65536, c->max_points);
   m->max_sub = c->cfg.max_map_points;
   bool ok = true;
   for (int t = 0; t < 2 && ok; ++t) {
-    ok = ok && cudaMalloc((void**)&m->d_pts[t], (size_t)kPool * m->cap[t] * sizeof(Pt4)) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&m->d_sub[t], (size_t)m->max_sub * sizeof(Pt4)) == cudaSuccess;
-    ok = ok && cudaMalloc((void**)&m->d_in[t], (size_t)c->max_points * sizeof(Pt4)) == cudaSuccess;
+    ok = ok && dalloc(c, &m->d_pts[t], (size_t)kPool * m->cap[t]) == cudaSuccess;
+    ok = ok && dalloc(c, &m->d_sub[t], (size_t)m->max_sub) == cudaSuccess;
+    ok = ok && dalloc(c, &m->d_in[t], (size_t)c->max_points) == cudaSuccess;
   }
-  ok = ok && cudaMalloc((void**)&m->d_world, (size_t)2 * c->max_points * sizeof(Pt4)) == cudaSuccess;   // both stacks side by side
-  ok = ok && cudaMalloc((void**)&m->d_cube, (size_t)2 * c->max_points * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_state, sizeof(MapperState)) == cudaSuccess;
-  ok = ok && cudaMallocHost((void**)&m->h_state, sizeof(MapperState)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_segs, ALOAM_MAX_SEGS * sizeof(SegDesc)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_nseg, 16) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_off, (ALOAM_MAX_SEGS + 8) * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_rank0, (ALOAM_MAX_SEGS + 8) * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_bbox, ALOAM_MAX_SEGS * 6 * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_total, 16) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&m->d_pose_io, 16 * sizeof(double)) == cudaSuccess;
-  ok = ok && cudaStreamCreateWithFlags(&m->s_aux, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&m->ev_join, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_world, (size_t)2 * c->max_points) == cudaSuccess;   // both stacks side by side
+  ok = ok && dalloc(c, &m->d_cube, (size_t)2 * c->max_points) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
+  ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_segs, ALOAM_MAX_SEGS) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_nseg, 4) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_off, ALOAM_MAX_SEGS + 8) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_rank0, ALOAM_MAX_SEGS + 8) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_bbox, ALOAM_MAX_SEGS * 6) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_total, 4) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
+  ok = ok && screate(c, &m->s_aux) == cudaSuccess;
+  ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
   // the re-filter sorts every point of the valid cubes (<= the submap capacity per type), the stack filter two scan clouds
-  ok = ok && vox_seg_alloc(m->buf, std::max((size_t)2 * m->max_sub, (size_t)2 * c->max_points)) == ALOAM_OK;
-  if (!ok) {   // publish nothing half-built
+  ok = ok && vox_seg_alloc(c, m->buf, std::max((size_t)2 * m->max_sub, (size_t)2 * c->max_points)) == ALOAM_OK;
+  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
     cudaGetLastError();
-    c->mapper = m; aloam_mapper_free_impl(c);
     return ALOAM_ERR_CUDA;
   }
   c->mapper = m;
@@ -409,21 +406,6 @@ SegFilter make_filter(Mapper* m, int idx_bits) {
 
 }  // namespace
 
-extern "C" void aloam_mapper_free_impl(aloam_ctx* c) {
-  Mapper* m = static_cast<Mapper*>(c->mapper);
-  if (!m) return;
-  for (int t = 0; t < 2; ++t) { if (m->d_pts[t]) cudaFree(m->d_pts[t]); if (m->d_sub[t]) cudaFree(m->d_sub[t]); if (m->d_in[t]) cudaFree(m->d_in[t]); }
-  if (m->s_aux) { cudaStreamSynchronize(m->s_aux); cudaStreamDestroy(m->s_aux); }
-  if (m->ev_fork) cudaEventDestroy(m->ev_fork);
-  if (m->ev_join) cudaEventDestroy(m->ev_join);
-  void* ps[] = {m->d_world, m->d_cube, m->d_state, m->d_segs, m->d_nseg, m->d_off, m->d_rank0, m->d_bbox, m->d_total, m->d_pose_io};
-  for (void* p : ps) if (p) cudaFree(p);
-  if (m->h_state) cudaFreeHost(m->h_state);
-  vox_seg_free(m->buf);
-  delete m;
-  c->mapper = nullptr;
-}
-
 // One frame of alaserMapping's process() on the current stream, entirely on the device.  corner_last / surf_last and their
 // sizes, the odometry pose (7 doubles) and the output pose slot are device pointers; n_upper_* bound the cloud sizes.
 int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, int n_upper_c, const Pt4* d_surf_last, const int* d_ns, int n_upper_s,
@@ -432,7 +414,7 @@ int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, 
   Mapper* m = static_cast<Mapper*>(c->mapper);
   MapperState* S = m->d_state;
   // the registration buffers of mapping.cu (grids, stacks, blocks) are shared with the host API
-  if (!c->map_corner.grid.slots) {
+  if (!c->map_ready) {
     aloam_cloud_view none{nullptr, 0, 4};
     rc = aloam_map_upload_impl(c, none, none); if (rc) return rc;
   }
@@ -521,22 +503,22 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   // the inputs are uploaded to mapper-owned device buffers first: the views may alias any ctx-owned pinned buffer
   rc = upload_cloud(c, corner_last, m->d_in[0], c->max_points); if (rc) return rc;
   rc = upload_cloud(c, surf_last, m->d_in[1], c->max_points); if (rc) return rc;
-  c->h_ints[112] = corner_last.n; c->h_ints[113] = surf_last.n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state->in_counts, c->h_ints + 112, 8, cudaMemcpyHostToDevice, c->stream));
-  for (int k = 0; k < 4; ++k) c->h_dbl[64 + k] = q_wodom_curr[k];
-  for (int k = 0; k < 3; ++k) c->h_dbl[68 + k] = t_wodom_curr[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->h_dbl + 64, 56, cudaMemcpyHostToDevice, c->stream));
+  c->pin->mapper_counts[0] = corner_last.n; c->pin->mapper_counts[1] = surf_last.n;
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state->in_counts, c->pin->mapper_counts, 8, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 4; ++k) c->pin->mapper_pose_in[k] = q_wodom_curr[k];
+  for (int k = 0; k < 3; ++k) c->pin->mapper_pose_in[4 + k] = t_wodom_curr[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->pin->mapper_pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   rc = mapper_step_device(c, m->d_in[0], &m->d_state->in_counts[0], corner_last.n, m->d_in[1], &m->d_state->in_counts[1], surf_last.n, m->d_pose_io, m->d_pose_io + 7);
   if (rc) return rc;
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 72, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(&m->h_state->flags, &m->d_state->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   prof_collect(c);
-  for (int k = 0; k < 4; ++k) q_w_curr[k] = c->h_dbl[72 + k];
-  for (int k = 0; k < 3; ++k) t_w_curr[k] = c->h_dbl[76 + k];
+  for (int k = 0; k < 4; ++k) q_w_curr[k] = c->pin->mapper_pose_out[k];
+  for (int k = 0; k < 3; ++k) t_w_curr[k] = c->pin->mapper_pose_out[4 + k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (m->h_state->flags & ALOAM_FLAG_MAP_TOO_THIN) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = m->h_state->flags; stats->ms_total = ms; } }
   else fill_stats(c, stats, c->cfg.outer_iters, m->h_state->flags, ms);

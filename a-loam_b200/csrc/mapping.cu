@@ -635,18 +635,18 @@ namespace {
 inline int grid_ctas(const aloam_ctx* c) { return c->sms * 8; }   // grid-stride launches: 8 resident CTAs of 256 threads per SM
 
 int ensure_map_buffers(aloam_ctx* c) {
-  if (c->map_corner.grid.slots) return ALOAM_OK;
+  if (c->map_ready) return ALOAM_OK;
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   c->max_map = c->cfg.max_map_points;
   unsigned slots = 1024;
-  while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;
+  while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;   // ends: aloam_create bounds max_map_points by 2^30
   c->map_slots = (int)slots;
   const size_t mm = (size_t)c->max_map;
   for (int t = 0; t < 2; ++t) {
     MapCloud* m = t ? &c->map_surf : &c->map_corner;
     GridTable& g = m->grid;
-    if (cudaMalloc((void**)&c->d_map_pts[t], mm * 16) != cudaSuccess || cudaMalloc((void**)&g.slots, (size_t)slots * 16) != cudaSuccess ||
-        cudaMalloc((void**)&g.dyn, sizeof(GridDyn)) != cudaSuccess || cudaMalloc((void**)&g.gpts, mm * 16) != cudaSuccess)
+    if (dalloc(c, &c->d_map_pts[t], mm) != cudaSuccess || dalloc(c, &g.slots, slots) != cudaSuccess ||
+        dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, mm) != cudaSuccess)
       return ALOAM_ERR_CUDA;
     if (cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess) return ALOAM_ERR_CUDA;
     g.cap_slots = slots;
@@ -654,11 +654,12 @@ int ensure_map_buffers(aloam_ctx* c) {
     g.inv_cs = 1.0f / g.cs;
   }
   const size_t mp = (size_t)c->max_points;
-  if (cudaMalloc((void**)&c->d_stack_corner, mp * 16) != cudaSuccess || cudaMalloc((void**)&c->d_stack_surf, mp * 16) != cudaSuccess ||
-      cudaMalloc((void**)&c->d_fits, 2 * mp * 14 * 8) != cudaSuccess || cudaMalloc((void**)&c->d_map_blocks, 2 * mp * sizeof(BlockRec)) != cudaSuccess ||
-      cudaMalloc((void**)&c->d_nbr, 2 * mp * 5 * sizeof(float4)) != cudaSuccess || cudaMalloc((void**)&c->d_stack_counts, 4 * sizeof(int)) != cudaSuccess ||
-      cudaMalloc((void**)&c->d_map_pose, 8 * sizeof(double)) != cudaSuccess || cudaMalloc((void**)&c->d_map_summary, 4 * sizeof(LmSummary)) != cudaSuccess)
+  if (dalloc(c, &c->d_stack_corner, mp) != cudaSuccess || dalloc(c, &c->d_stack_surf, mp) != cudaSuccess ||
+      dalloc(c, &c->d_fits, 2 * mp * 14) != cudaSuccess || dalloc(c, &c->d_map_blocks, 2 * mp) != cudaSuccess ||
+      dalloc(c, &c->d_nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &c->d_stack_counts, 4) != cudaSuccess ||
+      dalloc(c, &c->d_map_pose, 8) != cudaSuccess || dalloc(c, &c->d_map_summary, 4) != cudaSuccess)
     return ALOAM_ERR_CUDA;
+  c->map_ready = true;
   return ALOAM_OK;
 }
 
@@ -726,16 +727,6 @@ int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_cor
 
 extern "C" {
 
-void aloam_map_free_impl(aloam_ctx* c) {
-  for (int t = 0; t < 2; ++t) {
-    MapCloud* m = t ? &c->map_surf : &c->map_corner;
-    void* ps[] = {c->d_map_pts[t], m->grid.slots, m->grid.dyn, m->grid.gpts};
-    for (void* p : ps) if (p) cudaFree(p);
-  }
-  void* qs[] = {c->d_stack_corner, c->d_stack_surf, c->d_fits, c->d_map_blocks, c->d_nbr, c->d_stack_counts, c->d_map_pose, c->d_map_summary};
-  for (void* p : qs) if (p) cudaFree(p);
-}
-
 int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map) {
   if (!c) return ALOAM_ERR_INVALID_ARG;
   int rc = check_view(corner_map); if (rc) return rc;
@@ -752,7 +743,7 @@ int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud
     if (views[t].n > 0 && views[t].stride_floats == 4 && is_device_ptr(views[t].data)) src[t] = reinterpret_cast<const Pt4*>(views[t].data);
     else { rc = upload_cloud(c, views[t], c->d_map_pts[t], c->max_map); if (rc) return rc; src[t] = c->d_map_pts[t]; }
   }
-  GridDyn* hd = reinterpret_cast<GridDyn*>(c->h_ints + 64);
+  GridDyn* hd = c->pin->grid;
   for (int t = 0; t < 2; ++t) { hd[t].n = views[t].n; hd[t].mask = grid_mask_for(views[t].n, (unsigned)c->map_slots); hd[t].cursor = 0; hd[t].owned = 0; }
   CUDA_CHECK_RET(cudaMemcpyAsync(c->map_corner.grid.dyn, &hd[0], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->map_surf.grid.dyn, &hd[1], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
@@ -766,11 +757,11 @@ int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map_corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map_surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
     rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 80, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
-  if (c->shard_count > 1) { c->map_global_n[0] = c->h_ints[80]; c->map_global_n[1] = c->h_ints[81]; }
+  if (c->shard_count > 1) { c->map_global_n[0] = c->pin->owned[0]; c->map_global_n[1] = c->pin->owned[1]; }
   prof_collect(c);
   c->have_map = true;
   return ALOAM_OK;
@@ -813,21 +804,21 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
   }
   LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, c->map_corner.grid, (const int*)d_cnt, c->map_surf.grid, (const int*)(d_cnt + 1));
   map_index_build(c, c->d_map_pts[0], c->d_map_pts[1], c->max_map);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 84, d_cnt, 12, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->shard, d_cnt, 12, cudaMemcpyDeviceToHost, c->stream));
   if (c->shard_count > 1) {
     int* d_two = d_cnt + 2;   // reuse after the error word has been copied out (stream order)
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map_corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map_surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
     rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 80, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   prof_collect(c);
-  if (c->h_ints[86]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points
-  c->map_n[0] = c->h_ints[84]; c->map_n[1] = c->h_ints[85];
-  c->map_global_n[0] = c->shard_count > 1 ? c->h_ints[80] : c->map_n[0];
-  c->map_global_n[1] = c->shard_count > 1 ? c->h_ints[81] : c->map_n[1];
+  if (c->pin->shard[2]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points
+  c->map_n[0] = c->pin->shard[0]; c->map_n[1] = c->pin->shard[1];
+  c->map_global_n[0] = c->shard_count > 1 ? c->pin->owned[0] : c->map_n[0];
+  c->map_global_n[1] = c->shard_count > 1 ? c->pin->owned[1] : c->map_n[1];
   c->have_map = true;
   return ALOAM_OK;
 }
@@ -835,8 +826,9 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
 static int upload_stacks(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack) {
   int rc = upload_cloud(c, corner_stack, c->d_stack_corner, c->max_points); if (rc) return rc;
   rc = upload_cloud(c, surf_stack, c->d_stack_surf, c->max_points); if (rc) return rc;
-  c->h_ints[96] = corner_stack.n; c->h_ints[97] = surf_stack.n; c->h_ints[98] = corner_stack.n + surf_stack.n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_stack_counts, c->h_ints + 96, 12, cudaMemcpyHostToDevice, c->stream));
+  int* sc = c->pin->stack_counts;
+  sc[0] = corner_stack.n; sc[1] = surf_stack.n; sc[2] = corner_stack.n + surf_stack.n;
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_stack_counts, sc, 12, cudaMemcpyHostToDevice, c->stream));
   return ALOAM_OK;
 }
 
@@ -852,16 +844,16 @@ int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, alo
   }
   CUDA_CHECK_RET(cudaEventRecord(c->ev0, c->stream));
   rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
-  for (int k = 0; k < 7; ++k) c->h_dbl[k] = x[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   map_register_device(c, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, corner_stack.n + surf_stack.n, c->d_map_pose, false);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_dbl + 8, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   prof_collect(c);
-  for (int k = 0; k < 7; ++k) x[k] = c->h_dbl[8 + k];
+  for (int k = 0; k < 7; ++k) x[k] = c->pin->pose_out[k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   fill_stats(c, stats, c->cfg.outer_iters, 0, ms);
   return ALOAM_OK;
@@ -875,8 +867,8 @@ int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_c
   rc = check_view(surf_stack); if (rc) return rc;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
-  for (int k = 0; k < 7; ++k) c->h_dbl[k] = x[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->h_dbl, 56, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   const int nq = corner_stack.n + surf_stack.n;
   if (nq > 0) {
     LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, grid_ctas(c)), 256, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner,

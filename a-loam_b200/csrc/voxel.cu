@@ -578,21 +578,16 @@ void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_up
   }
 }
 
-int vox_seg_alloc(SegBuffers& b, size_t cap) {
+int vox_seg_alloc(aloam_ctx* c, SegBuffers& b, size_t cap) {
   const size_t nb = (cap + VCH - 1) / VCH + 1;
   b.cap = cap;
-  if (cudaMalloc((void**)&b.keys[0], cap * 4) != cudaSuccess || cudaMalloc((void**)&b.keys[1], cap * 4) != cudaSuccess ||
-      cudaMalloc((void**)&b.vals[0], cap * 4) != cudaSuccess || cudaMalloc((void**)&b.vals[1], cap * 4) != cudaSuccess ||
-      cudaMalloc((void**)&b.hist, nb * 256 * 4) != cudaSuccess || cudaMalloc((void**)&b.offs, nb * 256 * 4) != cudaSuccess ||
-      cudaMalloc((void**)&b.block_heads, nb * 4) != cudaSuccess || cudaMalloc((void**)&b.heads_total, 16) != cudaSuccess ||
-      cudaMalloc((void**)&b.tmp, cap * sizeof(Pt4)) != cudaSuccess)
+  if (dalloc(c, &b.keys[0], cap) != cudaSuccess || dalloc(c, &b.keys[1], cap) != cudaSuccess ||
+      dalloc(c, &b.vals[0], cap) != cudaSuccess || dalloc(c, &b.vals[1], cap) != cudaSuccess ||
+      dalloc(c, &b.hist, nb * 256) != cudaSuccess || dalloc(c, &b.offs, nb * 256) != cudaSuccess ||
+      dalloc(c, &b.block_heads, nb) != cudaSuccess || dalloc(c, &b.heads_total, 4) != cudaSuccess ||
+      dalloc(c, &b.tmp, cap) != cudaSuccess)
     return ALOAM_ERR_CUDA;
   return ALOAM_OK;
-}
-void vox_seg_free(SegBuffers& b) {
-  void* ps[] = {b.keys[0], b.keys[1], b.vals[0], b.vals[1], b.hist, b.offs, b.block_heads, b.heads_total, b.tmp};
-  for (void* p : ps) if (p) cudaFree(p);
-  b = SegBuffers();
 }
 
 
@@ -603,34 +598,35 @@ extern "C" int aloam_voxel_filter_impl(aloam_ctx* c, aloam_cloud_view in, float 
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   // the result has its OWN pinned buffer: a caller may pass a view returned by aloam_extract_features (h_out[*]) straight
   // back in, so the output must not alias any other ctx-owned view
-  if (!c->h_vox_out) CUDA_CHECK_RET(cudaMallocHost((void**)&c->h_vox_out, (size_t)c->max_points * sizeof(Pt4)));
+  if (!c->h_vox_out) CUDA_CHECK_RET(halloc(c, &c->h_vox_out, (size_t)c->max_points));
   out->data = reinterpret_cast<const float*>(c->h_vox_out); out->n = 0; out->stride_floats = 4;
   if (in.n == 0) return ALOAM_OK;
   const int n = in.n;
-  if (!c->d_vox_keys[0]) {
+  if (!c->vox_ready) {
     const size_t mp = (size_t)c->max_points;
     const int nb_max = (c->max_points + VCH - 1) / VCH;
-    CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_keys[0], mp * 4)); CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_keys[1], mp * 4));
-    CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_vals[0], mp * 4)); CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_vals[1], mp * 4));
-    CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_hist, (size_t)nb_max * 256 * 4)); CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_offs, (size_t)nb_max * 256 * 4));
-    CUDA_CHECK_RET(cudaMalloc((void**)&c->d_vox_misc, 64 * 4 + (size_t)nb_max * 4));
+    CUDA_CHECK_RET(dalloc(c, &c->d_vox_keys[0], mp)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_keys[1], mp));
+    CUDA_CHECK_RET(dalloc(c, &c->d_vox_vals[0], mp)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_vals[1], mp));
+    CUDA_CHECK_RET(dalloc(c, &c->d_vox_hist, (size_t)nb_max * 256)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_offs, (size_t)nb_max * 256));
+    CUDA_CHECK_RET(dalloc(c, &c->d_vox_misc, 64 + (size_t)nb_max));
+    c->vox_ready = true;
   }
   Pt4* d_in = c->d_query;        // staging buffers that already exist in the context
   Pt4* d_out = c->lanes[0].d_full[0];
   rc = upload_cloud(c, in, d_in, c->max_points); if (rc) return rc;
   int* mm6 = c->d_vox_misc; int* d_total = c->d_vox_misc + 8; int* d_n = c->d_vox_misc + 9; int* block_heads = c->d_vox_misc + 64;
   const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-  std::memcpy(c->h_ints + 32, init, sizeof(init));
-  c->h_ints[38] = n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(mm6, c->h_ints + 32, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(d_n, c->h_ints + 38, 4, cudaMemcpyHostToDevice, c->stream));
+  std::memcpy(c->pin->vox_init, init, sizeof(init));
+  c->pin->vox_n = n;
+  CUDA_CHECK_RET(cudaMemcpyAsync(mm6, c->pin->vox_init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(d_n, &c->pin->vox_n, 4, cudaMemcpyHostToDevice, c->stream));
   LAUNCH(c, KID_VOXEL, k_vox_bbox, std::min((n + 255) / 256, 592), 256, 0, d_in, n, mm6);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 40, mm6, 24, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->vox_box, mm6, 24, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   // host replica of PCL's index-range computation (needs the box; also decides the number of radix passes)
   float mn[3], mx[3];
   for (int a = 0; a < 3; ++a) {
-    int lo = c->h_ints[40 + a], hi = c->h_ints[43 + a];
+    int lo = c->pin->vox_box[a], hi = c->pin->vox_box[3 + a];
     lo = lo >= 0 ? lo : (lo ^ 0x7fffffff); hi = hi >= 0 ? hi : (hi ^ 0x7fffffff);
     std::memcpy(&mn[a], &lo, 4); std::memcpy(&mx[a], &hi, 4);
   }
@@ -664,10 +660,10 @@ extern "C" int aloam_voxel_filter_impl(aloam_ctx* c, aloam_cloud_view in, float 
   LAUNCH(c, KID_VOXEL, k_vox_heads, nblk, VT, 0, c->d_vox_keys[cur], d_n, block_heads);
   LAUNCH(c, KID_VOXEL, k_vox_blockscan, 1, 1024, 0, block_heads, d_n, d_total);
   LAUNCH(c, KID_VOXEL, k_vox_emit, nblk, VT, 0, d_in, c->d_vox_keys[cur], c->d_vox_vals[cur], d_n, block_heads, d_out);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_ints + 48, d_total, 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->vox_out_n, d_total, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
-  const int m = c->h_ints[48];
+  const int m = c->pin->vox_out_n;
   if (m > 0) {
     CUDA_CHECK_RET(cudaMemcpyAsync(c->h_vox_out, d_out, (size_t)m * 16, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

@@ -64,7 +64,8 @@ typedef struct aloam_config {
   double nearby_scan;    /* 2.5 NEARBY_SCAN, laserOdometry.cpp:66 */
   int device;            /* CUDA device ordinal */
   int max_points;        /* capacity of one raw scan (reference: 400000 static arrays, scanRegistration.cpp:66-69) */
-  int max_map_points;    /* capacity of the uploaded submap, per cloud type (0 = mapping not used) */
+  int max_map_points;    /* capacity of the uploaded submap, per cloud type (0 = mapping not used); at most 2^30, larger
+                            values are rejected by aloam_create with ALOAM_ERR_INVALID_ARG */
   int max_batch;         /* trajectories a context can advance in lockstep (aloam_scan_stream_batch); 1..ALOAM_MAX_BATCH, default 1 */
   int distortion;        /* 0 (reference build) or 1: #define DISTORTION of laserOdometry.cpp:59 -- per-point interpolation ratio
                             s = (intensity - int(intensity)) / SCAN_PERIOD in TransformToStart (:113-118) and in the

@@ -47,6 +47,14 @@ def test_no_cpu_fallback(aloam):
     assert aloam.lib().aloam_strerror(-6).decode() == "no CUDA device"
 
 
+def test_map_capacity_above_2_30_is_rejected_before_the_device(aloam):
+    """the map's hash-grid slot count (next power of two above 1.25 x max_map_points) must fit 32 bits: a larger
+    max_map_points is an invalid argument, reported before any device is queried"""
+    with pytest.raises(aloam.AloamError) as e:
+        aloam.Aloam(n_scans=16, max_map_points=2**30 + 1)
+    assert e.value.code == -1
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "a-loam_b200")
     for dirpath, _, files in os.walk(pkg):
