@@ -22,7 +22,7 @@ EXPORTED_SYMBOLS = [
     "aloam_odometry_set_last", "aloam_odometry_register", "aloam_map_upload", "aloam_mapping_register",
     "aloam_voxel_filter", "aloam_scan_to_pose", "aloam_scan_to_pose_device", "aloam_reset_odometry", "aloam_knn",
     "aloam_odometry_associate", "aloam_normal_equations", "aloam_solve", "aloam_debug_features", "aloam_mapping_associate",
-    "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
+    "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_debug_seg_voxel_filter", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
 ]
 
 
@@ -85,6 +85,7 @@ def lib():
         L.aloam_mapper_step.argtypes = [C.c_void_p, cv, cv, dp, dp, dp, dp, C.POINTER(Stats)]
         L.aloam_mapper_debug_state.argtypes = [C.c_void_p, ip, ip, ip, dp, dp, C.POINTER(C.c_longlong)]
         L.aloam_mapper_debug_cube.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(cv)]
+        L.aloam_debug_seg_voxel_filter.argtypes = [C.c_void_p, C.POINTER(cv), fp, C.c_int, C.c_int, fp, ip, ip]
         L.aloam_scan_to_pose.argtypes = [C.c_void_p, cv, dp, dp, C.POINTER(Stats)]
         L.aloam_scan_to_pose_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, dp, C.POINTER(Stats)]
         L.aloam_reset_odometry.argtypes = [C.c_void_p]
@@ -253,6 +254,26 @@ class Aloam:
         out = CloudView()
         _check(lib().aloam_mapper_debug_cube(self._h, which, cube_index, C.byref(out)))
         return _out(out)
+
+    def seg_voxel_filter(self, segs, leaves, idx_bits=31):
+        """the mapper's segmented VoxelGrid over `segs` ((n, 4) float32 clouds, one leaf each) in one pass with `idx_bits`
+        voxel-index bits in the sort key -> (list of filtered clouds, error word)"""
+        keep = [_view(s) for s in segs]
+        n = len(keep)
+        views = (CloudView * max(n, 1))(*[v for v, _ in keep])
+        lv = np.ascontiguousarray(leaves, np.float32)
+        total = sum(v.n for v, _ in keep)
+        out = np.zeros((max(total, 1), 4), np.float32)
+        counts = np.zeros(max(n, 1), np.int32)
+        err = C.c_int(0)
+        fp, ip = C.POINTER(C.c_float), C.POINTER(C.c_int)
+        _check(lib().aloam_debug_seg_voxel_filter(self._h, views, lv.ctypes.data_as(fp), n, int(idx_bits), out.ctypes.data_as(fp),
+                                                  counts.ctypes.data_as(ip), C.byref(err)))
+        res, off = [], 0
+        for (v, _), k in zip(keep, counts):
+            res.append(out[off:off + k].copy())
+            off += v.n
+        return res, err.value
 
     def mapping_register(self, corner_stack, surf_stack, x):
         a, ka = _view(corner_stack)

@@ -527,6 +527,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     return code;
   };
 #define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return fail(ALOAM_ERR_CUDA); } } while (0)
+  if (map_poses) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c), 0, sizeof(int), s_main));   // the mapper's error bits of this call
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
   // everything issued on the main stream before this call (reset, earlier calls) is ordered before the side streams.
   // Waiting on an event that was never recorded, or whose work finished in an earlier call, is a no-op -- so the
@@ -614,6 +615,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   if (map_poses) {
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapdone[c->cur], 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
+    STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err, mapper_err_acc(c), sizeof(int), cudaMemcpyDeviceToHost, s_main));
   }
   for (int l = 0; l < nb; ++l) {
     STREAM_TRY(cudaMemcpyAsync(c->h_summary + 4 * l, c->lanes[l].d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, s_main));
@@ -641,6 +643,8 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
+  // as aloam_mapper_step: a voxel index range beyond the key width in any frame means its map results would be wrong
+  if (map_poses && (c->pin->mapper_err & 1)) return ALOAM_ERR_CAPACITY;
   return ALOAM_OK;
 }
 

@@ -61,6 +61,7 @@ struct PinnedScratch {
   int shard[3];             // aloam_map_upload_sharded: points kept (corner, surf), error word
   int stack_counts[3];      // scan-to-map stacks: n_corner, n_surf, total
   int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
+  int mapper_err;           // aloam_scan_stream_mapped: the mapper's error bits, OR over the call's frames
   int vox_init[6];          // aloam_voxel_filter: initial bounding box (ordered-int min xyz, max xyz)
   int vox_n;                //                     input size
   int vox_box[6];           //                     bounding box of the cloud
@@ -223,6 +224,7 @@ void vox_seg_filter(aloam_ctx* c, const aloam::SegFilter& f, aloam::SegBuffers& 
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, int n_upper_c, const Pt4* d_surf_last, const int* d_ns, int n_upper_s,
                        const double* d_odom7, double* d_out7);
+int* mapper_err_acc(aloam_ctx* c);
 void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n_upper);
 int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_corner, const Pt4* sub_surf, const int* n_surf, int n_upper, int* err_word);
 void map_register_device(aloam_ctx* c, const Pt4* d_corner_stack, const Pt4* d_surf_stack, const int* d_counts3, int nq_upper, double* d_pose, bool want_fits);

@@ -44,7 +44,10 @@ struct MapperState {
   int stack_counts[4];                       // filtered stack sizes: corner, surf, total used by the registration, raw total
   int in_counts[2];                          // sizes of the incoming less-sharp / less-flat clouds (host API path)
   int flags;                                 // ALOAM_FLAG_* of this frame
-  int err;                                   // bit 0: voxel index range, bit 1: slab overflow, bit 2: pool exhausted, bit 3: submap capacity
+  int frame_err;                             // `err` of the last completed frame (read back with `flags`)
+  int err;                                   // of the running frame -- bit 0: voxel index range, bit 1: slab overflow, bit 2: pool
+                                             // exhausted, bit 3: submap capacity; cleared when the frame ends
+  int err_acc;                               // OR of the frames' words over one aloam_scan_stream_mapped call
   int frames;
   int zero, sink;                            // always 0 (count of a cube without a slab) ; write-only dummy
   int free_top;                              // slabs [free_top, kPool) of free_list are free ... per type
@@ -68,6 +71,9 @@ struct Mapper {
   int *d_off = nullptr, *d_rank0 = nullptr, *d_bbox = nullptr, *d_total = nullptr;
   SegBuffers buf;
   double* d_pose_io = nullptr;              // [14] host API: odometry pose in, refined pose out
+  Pt4* d_dbg_pts = nullptr;                 // aloam_debug_seg_voxel_filter: segments back to back [buf.cap] ...
+  int* d_dbg_counts = nullptr;              //                                their sizes [ALOAM_MAX_SEGS]
+  int* d_dbg_err = nullptr;                 //                                private error word
   int max_sub = 0;
   cudaStream_t s_aux = nullptr;             // the stack filters run here, beside the submap gather + index build
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -256,8 +262,22 @@ __global__ void k_mapper_update(MapperState* S, double* __restrict__ out7) {
   S->q_wmap_wodom[0] = qn.x; S->q_wmap_wodom[1] = qn.y; S->q_wmap_wodom[2] = qn.z; S->q_wmap_wodom[3] = qn.w;
   S->t_wmap_wodom[0] = S->x[4] - r[0]; S->t_wmap_wodom[1] = S->x[5] - r[1]; S->t_wmap_wodom[2] = S->x[6] - r[2];
   if (out7) for (int k = 0; k < 7; ++k) out7[k] = S->x[k];
-  if (S->err & 6) S->flags |= ALOAM_FLAG_CUBE_OVERFLOW;
   S->frames++;
+}
+
+// end of the frame, after insertion and re-filter have set their error bits: slab overflow, pool exhaustion and submap
+// truncation become this frame's ALOAM_FLAG_CUBE_OVERFLOW, the frame's word joins the per-call accumulation, and `err` starts
+// the next frame clear (everything of the next frame -- the stack filter forked onto the auxiliary stream included -- is
+// ordered after this kernel)
+__global__ void k_mapper_finish(MapperState* S) {
+  pdl_launch_dependents();
+  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
+  if (threadIdx.x || blockIdx.x) return;
+  const int e = S->err;
+  if (e & 14) S->flags |= ALOAM_FLAG_CUBE_OVERFLOW;
+  S->frame_err = e;
+  S->err_acc |= e;
+  S->err = 0;
 }
 
 // pointAssociateToMap (:154-163) in double, stored as float, then the cube of the stored point (:741-758)
@@ -359,6 +379,12 @@ __global__ void __launch_bounds__(256) k_seg_cubes(MapperState* S, SegDesc* segs
   if (t == 0) { *n_seg = 2 * nv; S->zero = 0; }
 }
 
+// points one segmented filter can sort: the re-filter takes every point of the <= 75 valid cubes of each type, full slabs
+// included (the submap gather truncates only its own copy at max_map_points), the stack filter two scan clouds
+size_t refilter_bound(const Mapper* m, const aloam_ctx* c) {
+  return std::max((size_t)75 * (m->cap[0] + m->cap[1]), (size_t)2 * c->max_points);
+}
+
 int ensure_mapper(aloam_ctx* c) {
   if (c->mapper) return ALOAM_OK;
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
@@ -387,8 +413,7 @@ int ensure_mapper(aloam_ctx* c) {
   ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
   ok = ok && screate(c, &m->s_aux) == cudaSuccess;
   ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
-  // the re-filter sorts every point of the valid cubes (<= the submap capacity per type), the stack filter two scan clouds
-  ok = ok && vox_seg_alloc(c, m->buf, std::max((size_t)2 * m->max_sub, (size_t)2 * c->max_points)) == ALOAM_OK;
+  ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
   if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
     cudaGetLastError();
     return ALOAM_ERR_CUDA;
@@ -463,10 +488,14 @@ int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, 
   int cube_bits = 1;
   { const double side = std::floor(50.0 / std::min(c->cfg.line_res, c->cfg.plane_res)) + 3.0; const double cells = side * side * side;
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
-  vox_seg_filter(c, make_filter(m, cube_bits), m->buf, 2 * 75, (int)std::min(m->buf.cap, (size_t)2 * m->max_sub + (size_t)2 * c->max_points), m->cap[1]);
+  vox_seg_filter(c, make_filter(m, cube_bits), m->buf, 2 * 75, (int)m->buf.cap, m->cap[1]);   // buf.cap = refilter_bound
+  launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1), dim3(32), 0, 1, true, S);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
+
+// the per-call error accumulation of aloam_scan_stream_mapped (device word; the mapper must exist)
+int* mapper_err_acc(aloam_ctx* c) { return &static_cast<Mapper*>(c->mapper)->d_state->err_acc; }
 
 extern "C" {
 
@@ -522,7 +551,7 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (m->h_state->flags & ALOAM_FLAG_MAP_TOO_THIN) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = m->h_state->flags; stats->ms_total = ms; } }
   else fill_stats(c, stats, c->cfg.outer_iters, m->h_state->flags, ms);
-  if (m->h_state->err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
+  if (m->h_state->frame_err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
   return ALOAM_OK;
 }
 
@@ -555,6 +584,63 @@ int aloam_mapper_debug_cube(aloam_ctx* c, int which, int cube, aloam_cloud_view*
   const int n = s < 0 ? 0 : m->h_state->cnt[which][s];
   out->data = reinterpret_cast<const float*>(c->h_out[4]); out->n = n; out->stride_floats = 4;
   if (n > 0) CUDA_CHECK_RET(cudaMemcpy(c->h_out[4], m->d_pts[which] + (size_t)s * m->cap[which], (size_t)n * sizeof(Pt4), cudaMemcpyDeviceToHost));
+  return ALOAM_OK;
+}
+
+int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, const float* leaves, int n_segs, int idx_bits, float* out,
+                                 int* out_counts, int* err) {
+  if (!c || n_segs < 0 || (n_segs > 0 && (!segs || !leaves || !out_counts)) || !err || idx_bits < 1 || idx_bits > 31) return ALOAM_ERR_INVALID_ARG;
+  if (n_segs > ALOAM_MAX_SEGS) return ALOAM_ERR_CAPACITY;
+  size_t total = 0;
+  int per_seg = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    int rc = check_view(segs[s]); if (rc) return rc;
+    if (!(leaves[s] > 0.f)) return ALOAM_ERR_INVALID_ARG;
+    total += (size_t)segs[s].n;
+    per_seg = std::max(per_seg, segs[s].n);
+  }
+  if (total > 0 && !out) return ALOAM_ERR_INVALID_ARG;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const bool fresh = c->mapper == nullptr;
+  int rc = ensure_mapper(c); if (rc) return rc;
+  if (fresh) { rc = aloam_mapper_reset(c); if (rc) return rc; }
+  Mapper* m = static_cast<Mapper*>(c->mapper);
+  if (total > m->buf.cap) return ALOAM_ERR_CAPACITY;
+  if (!m->d_dbg_err) {   // first use; the pointer that marks the group as ready is allocated last
+    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_pts, m->buf.cap));
+    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_counts, ALOAM_MAX_SEGS));
+    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_err, 1));
+  }
+  // the segments back to back, filtered in place like the cubes of the re-filter; the mapper state is not touched (the
+  // descriptors, offsets and sort buffers are scratch that every frame rewrites before use)
+  SegDesc desc[ALOAM_MAX_SEGS];
+  int counts[ALOAM_MAX_SEGS];
+  size_t off = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    rc = upload_cloud(c, segs[s], m->d_dbg_pts + off, (int)(m->buf.cap - off)); if (rc) return rc;
+    desc[s] = SegDesc{m->d_dbg_pts + off, m->d_dbg_counts + s, leaves[s], m->d_dbg_pts + off, m->d_dbg_counts + s};
+    counts[s] = segs[s].n;
+    off += (size_t)segs[s].n;
+  }
+  if (n_segs > 0) {
+    CUDA_CHECK_RET(cudaMemcpyAsync(m->d_segs, desc, sizeof(SegDesc) * n_segs, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(m->d_dbg_counts, counts, sizeof(int) * n_segs, cudaMemcpyHostToDevice, c->stream));
+  }
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_nseg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemsetAsync(m->d_dbg_err, 0, sizeof(int), c->stream));
+  SegFilter f = make_filter(m, idx_bits);
+  f.err = m->d_dbg_err;
+  if (n_segs > 0) vox_seg_filter(c, f, m->buf, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
+  CUDA_CHECK_RET(cudaGetLastError());
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  if (n_segs > 0) CUDA_CHECK_RET(cudaMemcpy(out_counts, m->d_dbg_counts, sizeof(int) * n_segs, cudaMemcpyDeviceToHost));
+  CUDA_CHECK_RET(cudaMemcpy(err, m->d_dbg_err, sizeof(int), cudaMemcpyDeviceToHost));
+  off = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    if (out_counts[s] > 0)
+      CUDA_CHECK_RET(cudaMemcpy(out + 4 * off, m->d_dbg_pts + off, (size_t)out_counts[s] * sizeof(Pt4), cudaMemcpyDeviceToHost));
+    off += (size_t)segs[s].n;
+  }
   return ALOAM_OK;
 }
 

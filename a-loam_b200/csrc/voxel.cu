@@ -221,26 +221,29 @@ __global__ void __launch_bounds__(VT) k_radix_sort_all(unsigned* __restrict__ k0
   }
 }
 
-// number of voxel heads (first element of each run of equal keys) per block of VCH sorted elements
+// number of voxel heads (first element of each run of equal keys) per block of VCH sorted elements; the CTAs stride over
+// the blocks, so the grid may be smaller than the live block count
 __global__ void __launch_bounds__(VT) k_vox_heads(const unsigned* __restrict__ keys, const int* __restrict__ n_ptr, int* __restrict__ block_heads) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int n = *n_ptr;
-  if (blockIdx.x * VCH >= n) return;
   __shared__ int s_c;
-  if (threadIdx.x == 0) s_c = 0;
-  __syncthreads();
-  int c = 0;
+  for (int blk = blockIdx.x; blk * VCH < n; blk += gridDim.x) {
+    if (threadIdx.x == 0) s_c = 0;
+    __syncthreads();
+    int c = 0;
 #pragma unroll
-  for (int it = 0; it < VIT; ++it) {
-    const int i = blockIdx.x * VCH + it * VT + threadIdx.x;
-    if (i < n && (i == 0 || keys[i] != keys[i - 1])) ++c;
+    for (int it = 0; it < VIT; ++it) {
+      const int i = blk * VCH + it * VT + threadIdx.x;
+      if (i < n && (i == 0 || keys[i] != keys[i - 1])) ++c;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_c, c);
+    __syncthreads();
+    if (threadIdx.x == 0) block_heads[blk] = s_c;
+    __syncthreads();
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
-  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_c, c);
-  __syncthreads();
-  if (threadIdx.x == 0) block_heads[blockIdx.x] = s_c;
 }
 
 __global__ void __launch_bounds__(1024) k_vox_blockscan(int* __restrict__ block_heads, const int* __restrict__ n_ptr, int* __restrict__ total) {
@@ -449,74 +452,77 @@ __global__ void __launch_bounds__(32) k_seg_rank0(SegFilter f, const unsigned* _
   }
 }
 
-// every head sums its run in sorted order (float, like pcl::CentroidPoint); output slot = off[segment] + rank inside the segment
+// every head sums its run in sorted order (float, like pcl::CentroidPoint); output slot = off[segment] + rank inside the segment.
+// The CTAs stride over the blocks of VCH sorted keys (the grid is sized by a host bound, the live total is on the device).
 __global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __restrict__ keys, const int* __restrict__ vals,
                                                  const int* __restrict__ block_offsets, Pt4* __restrict__ tmp) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int n = *f.total;
-  if (blockIdx.x * VCH >= n) return;
   __shared__ int s_w[VT / 32];
   __shared__ Pt4 s_pts[VCH];        // the block's points in sorted order: the runs are summed from shared memory, the gather
   __shared__ unsigned s_keys[VCH];  // through vals[] is issued once, all loads in flight
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int b0 = blockIdx.x * VCH;
+  for (int blk = blockIdx.x; blk * VCH < n; blk += gridDim.x) {
+    const int b0 = blk * VCH;
 #pragma unroll
-  for (int k = 0; k < VIT; ++k) {
-    const int i = b0 + k * VT + tid;
-    if (i < n) {
-      const unsigned key = keys[i];
+    for (int k = 0; k < VIT; ++k) {
+      const int i = b0 + k * VT + tid;
+      if (i < n) {
+        const unsigned key = keys[i];
+        const int sgm = (int)(key >> f.idx_bits);
+        s_keys[k * VT + tid] = key;
+        s_pts[k * VT + tid] = f.seg[f.seg0 + sgm].src[vals[i] - f.off[sgm]];
+      }
+    }
+    __syncthreads();
+    const int base = b0 + tid * VIT;
+    int heads = 0;
+    bool is_head[VIT];
+#pragma unroll
+    for (int k = 0; k < VIT; ++k) {
+      const int i = base + k;
+      is_head[k] = i < n && (i == 0 || keys[i] != keys[i - 1]);
+      heads += is_head[k] ? 1 : 0;
+    }
+    int incl = heads;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { int u = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += u; }
+    if (lane == 31) s_w[w] = incl;
+    __syncthreads();
+    int wbase = 0;
+    for (int v = 0; v < w; ++v) wbase += s_w[v];
+    int rank = block_offsets[blk] + wbase + incl - heads;
+    const int bend = min(n, b0 + VCH);
+#pragma unroll
+    for (int k = 0; k < VIT; ++k) {
+      if (!is_head[k]) continue;
+      const int i = base + k;
+      const unsigned key = s_keys[i - b0];
       const int sgm = (int)(key >> f.idx_bits);
-      s_keys[k * VT + tid] = key;
-      s_pts[k * VT + tid] = f.seg[f.seg0 + sgm].src[vals[i] - f.off[sgm]];
-    }
-  }
-  __syncthreads();
-  const int base = b0 + tid * VIT;
-  int heads = 0;
-  bool is_head[VIT];
-#pragma unroll
-  for (int k = 0; k < VIT; ++k) {
-    const int i = base + k;
-    is_head[k] = i < n && (i == 0 || keys[i] != keys[i - 1]);
-    heads += is_head[k] ? 1 : 0;
-  }
-  int incl = heads;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { int u = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += u; }
-  if (lane == 31) s_w[w] = incl;
-  __syncthreads();
-  int wbase = 0;
-  for (int v = 0; v < w; ++v) wbase += s_w[v];
-  int rank = block_offsets[blockIdx.x] + wbase + incl - heads;
-  const int bend = min(n, b0 + VCH);
-#pragma unroll
-  for (int k = 0; k < VIT; ++k) {
-    if (!is_head[k]) continue;
-    const int i = base + k;
-    const unsigned key = s_keys[i - b0];
-    const int sgm = (int)(key >> f.idx_bits);
-    const int off = f.off[sgm];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-    int cnt = 0;
-    int j = i;
-    for (; j < bend && s_keys[j - b0] == key; ++j) {   // float accumulation in sorted order (pcl::CentroidPoint)
-      const Pt4 p = s_pts[j - b0];
-      sx += p.x; sy += p.y; sz += p.z; si += p.i;
-      ++cnt;
-    }
-    if (j == bend) {   // the run continues in the next block(s): finish it from global memory
-      const Pt4* __restrict__ src = f.seg[f.seg0 + sgm].src;
-      for (; j < n && keys[j] == key; ++j) {
-        const Pt4 p = src[vals[j] - off];
+      const int off = f.off[sgm];
+      float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
+      int cnt = 0;
+      int j = i;
+      for (; j < bend && s_keys[j - b0] == key; ++j) {   // float accumulation in sorted order (pcl::CentroidPoint)
+        const Pt4 p = s_pts[j - b0];
         sx += p.x; sy += p.y; sz += p.z; si += p.i;
         ++cnt;
       }
+      if (j == bend) {   // the run continues in the next block(s): finish it from global memory
+        const Pt4* __restrict__ src = f.seg[f.seg0 + sgm].src;
+        for (; j < n && keys[j] == key; ++j) {
+          const Pt4 p = src[vals[j] - off];
+          sx += p.x; sy += p.y; sz += p.z; si += p.i;
+          ++cnt;
+        }
+      }
+      const float nf = (float)cnt;
+      Pt4 o; o.x = sx / nf; o.y = sy / nf; o.z = sz / nf; o.i = si / nf;
+      tmp[off + (rank - f.rank0[sgm])] = o;
+      ++rank;
     }
-    const float nf = (float)cnt;
-    Pt4 o; o.x = sx / nf; o.y = sy / nf; o.z = sz / nf; o.i = si / nf;
-    tmp[off + (rank - f.rank0[sgm])] = o;
-    ++rank;
+    __syncthreads();   // s_w, s_pts and s_keys are refilled for the next block
   }
 }
 
@@ -537,10 +543,11 @@ __global__ void __launch_bounds__(256) k_seg_writeback(SegFilter f, const Pt4* _
 using namespace aloam;
 
 // segmented filter over up to S_upper segments; n_upper / per_seg_upper are host bounds for grid sizing (total points, points of
-// one segment).  A 32-bit key holds f.idx_bits index bits and the segment number: when S_upper segments do not fit beside the
+// one segment).  The caller guarantees that the live total never exceeds b.cap: nothing here clamps it.  A 32-bit key holds f.idx_bits index bits and the segment number: when S_upper segments do not fit beside the
 // index, the segments are processed in windows of 2^(32 - idx_bits).
 void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_upper, int n_upper, int per_seg_upper) {
   const int nblk = std::max(1, (n_upper + VCH - 1) / VCH);
+  const int grid_blk = std::min(nblk, 8 * c->sms);   // k_vox_heads / k_seg_emit stride over the blocks: one resident wave at most
   const int chunks = std::max(1, std::min((per_seg_upper + 255) / 256, S_upper > 8 ? 8 : 64));   // grid-stride inside a segment
   const int win = (int)std::min<long long>(1ll << std::max(0, 32 - f_in.idx_bits), ALOAM_MAX_SEGS);
   for (int s0 = 0; s0 < S_upper; s0 += win) {
@@ -570,10 +577,10 @@ void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_up
       prof_end(c);
     }
     const int cur = ((bits + 7) / 8) & 1;
-    launch_ex(c, KID_VOXEL, k_vox_heads, dim3(nblk), dim3(VT), 0, 1, true, b.keys[cur], f.total, b.block_heads);
+    launch_ex(c, KID_VOXEL, k_vox_heads, dim3(grid_blk), dim3(VT), 0, 1, true, b.keys[cur], f.total, b.block_heads);
     launch_ex(c, KID_VOXEL, k_vox_blockscan, dim3(1), dim3(1024), 0, 1, true, b.block_heads, f.total, b.heads_total);
     launch_ex(c, KID_VOXEL, k_seg_rank0, dim3(f.seg_cap + 1), dim3(32), 0, 1, true, f, b.keys[cur], b.block_heads);
-    launch_ex(c, KID_VOXEL, k_seg_emit, dim3(nblk), dim3(VT), 0, 1, true, f, b.keys[cur], b.vals[cur], b.block_heads, b.tmp);
+    launch_ex(c, KID_VOXEL, k_seg_emit, dim3(grid_blk), dim3(VT), 0, 1, true, f, b.keys[cur], b.vals[cur], b.block_heads, b.tmp);
     launch_ex(c, KID_VOXEL, k_seg_writeback, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f, b.tmp);
   }
 }

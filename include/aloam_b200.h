@@ -150,7 +150,9 @@ int aloam_scan_stream_batch(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_
  * per scan, on its own stream, overlapping the odometry of the following scans) -- what the reference ships over
  * /laser_cloud_corner_last, /laser_cloud_surf_last and /laser_odom_to_init (laserOdometry.cpp:570-591 ->
  * laserMapping.cpp:278-288, 142-152).  odom_poses / map_poses: n_scans x 7 doubles (q xyzw, t): laser_odom_to_init and
- * aft_mapped_to_init.  Identical to calling aloam_scan_to_pose + aloam_mapper_step per scan.  Needs cfg.max_map_points > 0.
+ * aft_mapped_to_init.  Identical to calling aloam_scan_to_pose + aloam_mapper_step per scan; if any scan's mapper step would
+ * have returned ALOAM_ERR_CAPACITY (a voxel index range beyond the sort key), the call fills both pose arrays and returns
+ * ALOAM_ERR_CAPACITY.  Needs cfg.max_map_points > 0.
  * After aloam_comm_init (every rank fed the same scans) the scan-to-map stage is sharded: each rank keeps the whole cube store,
  * indexes and searches only its x-slabs of the gathered submap, and the ranks meet in the all-reduce of the normal equations;
  * all ranks return the same poses (equal to a single-GPU run to rounding of the summation order). */
@@ -201,8 +203,10 @@ int aloam_mapping_associate(aloam_ctx* ctx, aloam_cloud_view corner_stack, aloam
  * cubes.  corner_last / surf_last are the less-sharp / less-flat clouds of the scan (what /laser_cloud_corner_last and
  * /laser_cloud_surf_last carry); the odometry pose is q_wodom_curr / t_wodom_curr; the refined pose is returned.
  * The call never fails half-way: a full cube slab, an exhausted pool or a submap beyond cfg.max_map_points drop the
- * overflow and set ALOAM_FLAG_CUBE_OVERFLOW in stats->flags; argument errors are reported before any state changes.
- * cfg.max_map_points must be > 0. */
+ * overflow and set ALOAM_FLAG_CUBE_OVERFLOW in stats->flags of the frame where it happened (the flags of every frame
+ * describe that frame only); argument errors are reported before any state changes.  A cube whose voxel index range does
+ * not fit the sort key is kept unfiltered and the frame returns ALOAM_ERR_CAPACITY after completing (pose and store are
+ * updated); the next frame starts clean.  cfg.max_map_points must be > 0. */
 int aloam_mapper_reset(aloam_ctx* ctx);
 int aloam_mapper_step(aloam_ctx* ctx, aloam_cloud_view corner_last, aloam_cloud_view surf_last,
                       const double q_wodom_curr[4], const double t_wodom_curr[3], double q_w_curr[4], double t_w_curr[3],
@@ -213,6 +217,14 @@ int aloam_mapper_step(aloam_ctx* ctx, aloam_cloud_view corner_last, aloam_cloud_
 int aloam_mapper_debug_state(aloam_ctx* ctx, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4],
                              double t_wmap_wodom[3], long long totals[2]);
 int aloam_mapper_debug_cube(aloam_ctx* ctx, int which, int cube_index, aloam_cloud_view* out);
+/* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
+ * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
+ * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
+ * written at its input offset (the sum of the sizes before it), out_counts[s] points.  err: bit 0 = a segment's index range
+ * needed more than idx_bits bits (that segment is returned unchanged).  n_segs > 160 or more points than the mapper's sort
+ * buffers hold: ALOAM_ERR_CAPACITY.  Creates the cube store if needed; never changes its state. */
+int aloam_debug_seg_voxel_filter(aloam_ctx* ctx, const aloam_cloud_view* segs, const float* leaves, int n_segs, int idx_bits,
+                                 float* out, int* out_counts, int* err);
 
 /* ---- multi-GPU scan-to-map (one process per GPU).  Rank 0 creates the 128-byte id and ships it to the others;
  * after aloam_comm_init each rank uploads only ITS shard of the submap (x-slabs of aloam_shard_slab_cells() cells of

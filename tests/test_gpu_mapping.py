@@ -124,3 +124,58 @@ def test_map_upload_accepts_device_memory(aloam, scene):
     x_dev, _ = c.mapping_register(cs, ss, x0)
     assert np.array_equal(x_host, x_dev)
     c.close()
+
+
+# ---- the single-cloud filter at its size limits: > 1024 blocks of 1024 keys (k_vox_blockscan strides), 1 to 4 radix
+# passes (an odd count leaves the sorted keys in the other buffer), runs across blocks, clouds near +-5 km
+
+def _radix_passes(cloud, leaf):
+    f = np.float32
+    inv = f(1) / f(leaf)
+    mn, mx = cloud[:, :3].min(0), cloud[:, :3].max(0)
+    cells = 1
+    for a in range(3):
+        cells *= int(np.floor(f(mx[a]) * inv)) - int(np.floor(f(mn[a]) * inv)) + 1
+    bits = 1
+    while bits < 32 and (1 << bits) < cells:
+        bits += 1
+    return (bits + 7) // 8
+
+
+@pytest.fixture(scope="module")
+def big_ctx(aloam):
+    c = aloam.Aloam(n_scans=16, max_points=1300000)
+    yield c
+    c.close()
+
+
+def _cube_cloud(rng, n, centre, side):
+    out = np.zeros((n, 4), np.float32)
+    out[:, :3] = np.asarray(centre) + rng.uniform(-side / 2, side / 2, size=(n, 3))
+    out[:, 3] = rng.uniform(0, 64, n)
+    return out
+
+
+@pytest.mark.parametrize("passes,side", [(1, 1.0), (2, 6.0), (3, 40.0), (4, 70.0)])
+def test_voxel_filter_radix_pass_counts(big_ctx, orc, passes, side):
+    rng = np.random.default_rng(passes)
+    cloud = _cube_cloud(rng, 200000, (-3.1, 7.7, 0.4), side)
+    assert _radix_passes(cloud, 0.2) == passes
+    ref = orc.voxel_grid(cloud, 0.2, orc.SORT_CANONICAL)
+    got = big_ctx.voxel_filter(cloud, 0.2)
+    assert got.shape == ref.shape and np.array_equal(got.view(np.uint32), ref.view(np.uint32))
+
+
+@pytest.mark.parametrize("sign", [1, -1])
+def test_voxel_filter_1_3_million_points_near_5_km(big_ctx, orc, sign):
+    """1.3 M points (1270 blocks of 1024 keys) around (+-4990, -+4990, 20) m; one voxel holds 5000 points, so its run
+    crosses several blocks"""
+    rng = np.random.default_rng(60 + sign)
+    centre = (sign * 4990.0, -sign * 4990.0, 20.0)
+    cloud = _cube_cloud(rng, 1300000, centre, 30.0)
+    run = _cube_cloud(rng, 5000, (0, 0, 0), 0.15)
+    run[:, :3] = np.floor(np.asarray(centre) / 0.4) * 0.4 + 0.2 + run[:, :3]
+    cloud[rng.choice(len(cloud), 5000, replace=False)] = run
+    ref = orc.voxel_grid(cloud, 0.4, orc.SORT_CANONICAL)
+    got = big_ctx.voxel_filter(cloud, 0.4)
+    assert got.shape == ref.shape and np.array_equal(got.view(np.uint32), ref.view(np.uint32))
