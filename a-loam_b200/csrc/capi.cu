@@ -793,12 +793,10 @@ int aloam_debug_feature_cycles(aloam_ctx* c, long long* out64x8) {
 // ------------------------------------------------------------------------------------------------ mapping (mapping.cu)
 int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
 int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats);
-int aloam_voxel_filter_impl(aloam_ctx* c, aloam_cloud_view in, float leaf, aloam_cloud_view* out);
 
 int aloam_map_upload(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map) { return aloam_map_upload_impl(c, corner_map, surf_map); }
 int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats) {
   return aloam_mapping_register_impl(c, corner_stack, surf_stack, x, stats);
 }
-int aloam_voxel_filter(aloam_ctx* c, aloam_cloud_view in, float leaf, aloam_cloud_view* out) { return aloam_voxel_filter_impl(c, in, leaf, out); }
 
 }  // extern "C"

@@ -62,10 +62,10 @@ struct PinnedScratch {
   int stack_counts[3];      // scan-to-map stacks: n_corner, n_surf, total
   int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
   int mapper_err;           // aloam_scan_stream_mapped: the mapper's error bits, OR over the call's frames
-  int vox_init[6];          // aloam_voxel_filter: initial bounding box (ordered-int min xyz, max xyz)
-  int vox_n;                //                     input size
-  int vox_box[6];           //                     bounding box of the cloud
-  int vox_out_n;            //                     output size
+  SegDesc vox_seg;          // aloam_voxel_filter: the cloud as the one segment of its filter
+  int vox_nseg;             //                     1
+  int vox_io[3];            //                     cloud size, filtered size, error word: {n, 0, 0}
+  int vox_out_n;            //                     filtered size
   double pose_in[7], pose_out[7];             // pose of the per-stage entry points
   double world[7];                            // fused pipeline: world pose of the scan
   double ne[28];                              // normal equations: J^T J upper 21, J^T r 6, cost
@@ -112,11 +112,10 @@ struct aloam_ctx {
   double* d_fits = nullptr;       // [queries][14] debug / test records of the line / plane fits
   BlockRec* d_map_blocks = nullptr;
   LmSummary* d_map_summary = nullptr;   // [4] summaries of the scan-to-map solves
-  // general voxel filter (voxel.cu): radix-sort ping-pong buffers, histograms, small scalars
-  unsigned* d_vox_keys[2] = {nullptr, nullptr};
-  int* d_vox_vals[2] = {nullptr, nullptr};
-  int *d_vox_hist = nullptr, *d_vox_offs = nullptr, *d_vox_misc = nullptr;
-  bool vox_ready = false;         // every buffer of this group is allocated
+  // aloam_voxel_filter (voxel.cu): a segmented filter of its own (cap = max_points), created on first use
+  SegBuffers vox_seg;
+  int* d_seg_io = nullptr;        // [3] the segment's size, its filtered size, the filter's error word
+  bool vox_seg_ready = false;     // every buffer of this group is allocated
   // pipelined scan stream: ring binning on s_exa, per-ring features on s_ext, compaction + index on s_idx, association + LM
   // on `stream`, host->device copies of the raw scans on s_h2d, scan-to-map on s_map; all chained by events
   cudaStream_t s_ext = nullptr, s_exa = nullptr, s_idx = nullptr, s_h2d = nullptr, s_map = nullptr;

@@ -66,10 +66,7 @@ struct Mapper {
   int* d_cube = nullptr;                    //                    their cube index (-1 = outside the ring buffer)
   MapperState* d_state = nullptr;
   MapperState* h_state = nullptr;           // pinned mirror (debug / host API read-back)
-  SegDesc* d_segs = nullptr;                // [ALOAM_MAX_SEGS]
-  int* d_nseg = nullptr;
-  int *d_off = nullptr, *d_rank0 = nullptr, *d_bbox = nullptr, *d_total = nullptr;
-  SegBuffers buf;
+  SegBuffers buf;                           // the segmented filter of the stack filters and the per-cube re-filter
   double* d_pose_io = nullptr;              // [14] host API: odometry pose in, refined pose out
   Pt4* d_dbg_pts = nullptr;                 // aloam_debug_seg_voxel_filter: segments back to back [buf.cap] ...
   int* d_dbg_counts = nullptr;              //                                their sizes [ALOAM_MAX_SEGS]
@@ -404,12 +401,6 @@ int ensure_mapper(aloam_ctx* c) {
   ok = ok && dalloc(c, &m->d_cube, (size_t)2 * c->max_points) == cudaSuccess;
   ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
   ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_segs, ALOAM_MAX_SEGS) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_nseg, 4) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_off, ALOAM_MAX_SEGS + 8) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_rank0, ALOAM_MAX_SEGS + 8) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_bbox, ALOAM_MAX_SEGS * 6) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_total, 4) == cudaSuccess;
   ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
   ok = ok && screate(c, &m->s_aux) == cudaSuccess;
   ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
@@ -420,13 +411,6 @@ int ensure_mapper(aloam_ctx* c) {
   }
   c->mapper = m;
   return ALOAM_OK;
-}
-
-SegFilter make_filter(Mapper* m, int idx_bits) {
-  SegFilter f;
-  f.seg = m->d_segs; f.n_seg = m->d_nseg; f.off = m->d_off; f.rank0 = m->d_rank0; f.bbox = m->d_bbox; f.total = m->d_total;
-  f.err = &m->d_state->err; f.idx_bits = idx_bits; f.seg0 = 0; f.seg_cap = ALOAM_MAX_SEGS;
-  return f;
 }
 
 }  // namespace
@@ -451,9 +435,9 @@ int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, 
     CUDA_CHECK_RET(cudaEventRecord(m->ev_fork, main_stream));
     CUDA_CHECK_RET(cudaStreamWaitEvent(m->s_aux, m->ev_fork, 0));
     c->stream = m->s_aux;
-    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1), dim3(32), 0, 1, false, m->d_segs, m->d_nseg, d_corner_last, d_nc, c->cfg.line_res, c->d_stack_corner, &S->stack_counts[0], d_surf_last, d_ns,
+    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1), dim3(32), 0, 1, false, m->buf.segs, m->buf.n_seg, d_corner_last, d_nc, c->cfg.line_res, c->d_stack_corner, &S->stack_counts[0], d_surf_last, d_ns,
               c->cfg.plane_res, c->d_stack_surf, &S->stack_counts[1]);
-    vox_seg_filter(c, make_filter(m, 31), m->buf, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
+    vox_seg_filter(c, seg_filter(m->buf, 31, &S->err), m->buf, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
     const cudaError_t e = cudaEventRecord(m->ev_join, m->s_aux);
     c->stream = main_stream;
     CUDA_CHECK_RET(e);
@@ -483,12 +467,12 @@ int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, 
             (const MapperState*)S, m->d_world, m->d_cube, c->max_points);
   launch_ex(c, KID_CUBES, k_cube_insert, dim3(2), dim3(1024), 0, 1, true, (const Pt4*)m->d_world, (const int*)m->d_cube, c->max_points, S, m->d_pts[0], m->cap[0], m->d_pts[1], m->cap[1]);
   // ---- per-cube re-filter of the valid cubes (:770-801): one segmented pass over <= 150 cubes, in place
-  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1), dim3(256), 0, 1, true, S, m->d_segs, m->d_nseg, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->cfg.line_res, c->cfg.plane_res);
+  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1), dim3(256), 0, 1, true, S, m->buf.segs, m->buf.n_seg, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->cfg.line_res, c->cfg.plane_res);
   // index bits of a 50 m cube at the finer leaf: (50 / leaf + 3)^3 voxels at most (PCL itself gives up beyond 2^31)
   int cube_bits = 1;
   { const double side = std::floor(50.0 / std::min(c->cfg.line_res, c->cfg.plane_res)) + 3.0; const double cells = side * side * side;
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
-  vox_seg_filter(c, make_filter(m, cube_bits), m->buf, 2 * 75, (int)m->buf.cap, m->cap[1]);   // buf.cap = refilter_bound
+  vox_seg_filter(c, seg_filter(m->buf, cube_bits, &S->err), m->buf, 2 * 75, (int)m->buf.cap, m->cap[1]);   // buf.cap = refilter_bound
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1), dim3(32), 0, 1, true, S);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
@@ -623,14 +607,12 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
     off += (size_t)segs[s].n;
   }
   if (n_segs > 0) {
-    CUDA_CHECK_RET(cudaMemcpyAsync(m->d_segs, desc, sizeof(SegDesc) * n_segs, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(m->buf.segs, desc, sizeof(SegDesc) * n_segs, cudaMemcpyHostToDevice, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(m->d_dbg_counts, counts, sizeof(int) * n_segs, cudaMemcpyHostToDevice, c->stream));
   }
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_nseg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->buf.n_seg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_dbg_err, 0, sizeof(int), c->stream));
-  SegFilter f = make_filter(m, idx_bits);
-  f.err = m->d_dbg_err;
-  if (n_segs > 0) vox_seg_filter(c, f, m->buf, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
+  if (n_segs > 0) vox_seg_filter(c, seg_filter(m->buf, idx_bits, m->d_dbg_err), m->buf, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
   CUDA_CHECK_RET(cudaGetLastError());
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   if (n_segs > 0) CUDA_CHECK_RET(cudaMemcpy(out_counts, m->d_dbg_counts, sizeof(int) * n_segs, cudaMemcpyDeviceToHost));

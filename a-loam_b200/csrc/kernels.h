@@ -108,7 +108,8 @@ __global__ void k_map_fit(const Pt4* corner_stack, const Pt4* surf_stack, const 
                           double* fits);
 __global__ void k_map_knn(MapCloud map, const Pt4* queries, int nq, int k, int* idx, float* sqd);
 
-// ---- voxel.cu: segmented, device-resident pcl::VoxelGrid (the scan-stack filters and the per-cube re-filter of the mapping loop)
+// ---- voxel.cu: segmented, device-resident pcl::VoxelGrid (aloam_voxel_filter, the scan-stack filters and the per-cube re-filter
+// of the mapping loop)
 #define ALOAM_MAX_SEGS 160
 struct SegDesc { const Pt4* src; const int* n_in; float leaf; Pt4* dst; int* n_out; };
 struct SegFilter {
@@ -118,12 +119,26 @@ struct SegFilter {
   int* rank0;           // [MAX_SEGS + 1] voxels before each segment
   int* bbox;            // [MAX_SEGS][6] ordered-int min / max
   int* total;           // points over all segments
+  int* pass;            // [MAX_SEGS] 1: the segment is returned unchanged (index overflow), set for every non-empty segment
   int* err;             // sticky error word (bit 0: a segment needs more than idx_bits index bits)
-  int idx_bits;         // bits of the voxel index inside a segment
+  int idx_bits;         // bits of the voxel index inside a segment, 1 .. 32 (32: one segment, the key is PCL's int index)
   int seg0, seg_cap;    // this pass handles segments seg0 .. seg0 + seg_cap - 1 (as many as fit beside idx_bits in a 32-bit key)
 };
-struct SegBuffers { unsigned* keys[2] = {nullptr, nullptr}; int* vals[2] = {nullptr, nullptr}; int *hist = nullptr, *offs = nullptr, *block_heads = nullptr, *heads_total = nullptr;
-                    Pt4* tmp = nullptr; size_t cap = 0; };
+// everything one segmented filter owns on the device (vox_seg_alloc); its calls run one after another on one stream
+struct SegBuffers {
+  SegDesc* segs = nullptr;   // [MAX_SEGS]
+  int* n_seg = nullptr;
+  int *off = nullptr, *rank0 = nullptr, *bbox = nullptr, *total = nullptr, *pass = nullptr;   // see SegFilter
+  unsigned* keys[2] = {nullptr, nullptr};
+  int* vals[2] = {nullptr, nullptr};
+  int *hist = nullptr, *block_heads = nullptr, *heads_total = nullptr;   // heads_total: k_vox_blockscan's voxel count (not read)
+  Pt4* tmp = nullptr;
+  size_t cap = 0;            // points over all segments of one call
+  int coop_grid = 1;         // CTAs of the cooperative radix sort: one per SM of the context's device
+};
+inline SegFilter seg_filter(const SegBuffers& b, int idx_bits, int* err) {
+  return SegFilter{b.segs, b.n_seg, b.off, b.rank0, b.bbox, b.total, b.pass, err, idx_bits, 0, ALOAM_MAX_SEGS};
+}
 
 // ---- lm.cu
 struct LmParams {

@@ -1,10 +1,15 @@
-// pcl::VoxelGrid<PointXYZI>::applyFilter on an arbitrary cloud -- the scan-stack filters of laserMapping.cpp:543-549
-// (downSizeFilterCorner / downSizeFilterSurf) as a general GPU routine (the per-ring 0.2 m instance of
-// scanRegistration.cpp:401-407 is fused into k_ring_features).  Semantics per SURVEY.md 8a "V":
+// pcl::VoxelGrid<PointXYZI>::applyFilter as one segmented, device-resident GPU routine: S independent clouds ("segments",
+// each with its own leaf size) are filtered by ONE sequence of launches -- a single cloud (aloam_voxel_filter), the two scan
+// stacks of a mapping frame (laserMapping.cpp:543-549, downSizeFilterCorner / downSizeFilterSurf), or all valid cubes of the
+// map after insertion (:787-801, up to 75 corner + 75 surf cubes).  The per-ring 0.2 m instance of scanRegistration.cpp:401-407
+// is fused into k_ring_features.  Semantics per SURVEY.md 8a "V", per segment:
 //   bounding box -> min_b / div_b -> voxel index (float multiply, floor) -> sort by index -> one output per occupied
 //   voxel in ascending index order = float32 centroid of x, y, z, intensity accumulated in sorted order.
-// PCL's std::sort is unstable; here ties are resolved by point index (a STABLE least-significant-digit radix sort on
-// the voxel index, 8 bits per pass, as many passes as the index range needs), which is the CANONICAL order of the oracle.
+// Key = segment << idx_bits | voxel index (PCL's index inside the segment's own bounding box), so one stable LSD radix sort
+// (8 bits per pass) orders every segment by voxel and keeps the segments apart.  PCL's std::sort is unstable; here ties are
+// resolved by point index, which is the CANONICAL order of the oracle.  Sizes live in device memory; nothing here
+// synchronises with the host.  A segment whose index range overflows int (PCL: "leaf size is too small", input returned
+// unchanged) or idx_bits (flagged) is returned as it is: its key is the position and the write-back copies the source.
 #include <climits>
 #include <cfloat>
 #include <cooperative_groups.h>
@@ -19,132 +24,11 @@ __device__ __forceinline__ int f2ord(float f) { int i = __float_as_int(f); retur
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : (i ^ 0x7fffffff)); }
 }  // namespace
 
-// mm6: ordered-int encoded [min x,y,z | max x,y,z], pre-set to +inf / -inf encodings
-__global__ void k_vox_bbox(const Pt4* __restrict__ pts, int n, int* __restrict__ mm6) {
-  float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const Pt4 p = pts[i];
-    lo[0] = fminf(lo[0], p.x); lo[1] = fminf(lo[1], p.y); lo[2] = fminf(lo[2], p.z);
-    hi[0] = fmaxf(hi[0], p.x); hi[1] = fmaxf(hi[1], p.y); hi[2] = fmaxf(hi[2], p.z);
-  }
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], d));
-      hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], d));
-    }
-    if ((threadIdx.x & 31) == 0) { atomicMin(&mm6[a], f2ord(lo[a])); atomicMax(&mm6[3 + a], f2ord(hi[a])); }
-  }
-}
-
-struct VoxParams { float inv; int min_b[3]; int div0, div01; };
-
-__global__ void k_vox_keys(const Pt4* __restrict__ pts, int n, VoxParams vp, unsigned* __restrict__ keys, int* __restrict__ vals) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const Pt4 p = pts[i];
-  const int i0 = (int)(floorf(p.x * vp.inv) - (float)vp.min_b[0]);
-  const int i1 = (int)(floorf(p.y * vp.inv) - (float)vp.min_b[1]);
-  const int i2 = (int)(floorf(p.z * vp.inv) - (float)vp.min_b[2]);
-  keys[i] = (unsigned)(i0 + i1 * vp.div0 + i2 * vp.div01);
-  vals[i] = i;
-}
-
-__global__ void __launch_bounds__(VT) k_radix_hist(const unsigned* __restrict__ keys, const int* __restrict__ n_ptr, int shift, int* __restrict__ hist) {
-  pdl_launch_dependents();
-  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
-  __shared__ int s_h[256];
-  const int tid = threadIdx.x;
-  const int n = *n_ptr;
-  if (blockIdx.x * VCH >= n) return;   // grids are sized by a host upper bound; the live size is on the device
-  s_h[tid] = 0;
-  __syncthreads();
-#pragma unroll
-  for (int it = 0; it < VIT; ++it) {
-    const int i = blockIdx.x * VCH + it * VT + tid;
-    if (i < n) atomicAdd(&s_h[(keys[i] >> shift) & 255u], 1);
-  }
-  __syncthreads();
-  hist[blockIdx.x * 256 + tid] = s_h[tid];
-}
-
-// one CTA, 1024 threads: thread (bin = t >> 2, quarter = t & 3) ; offsets are digit-major over all blocks
-__global__ void __launch_bounds__(1024) k_radix_scan(const int* __restrict__ hist, const int* __restrict__ n_ptr, int* __restrict__ offsets) {
-  pdl_launch_dependents();
-  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
-  const int nblocks = (*n_ptr + VCH - 1) / VCH;
-  __shared__ int s_tot[256];
-  __shared__ int s_start[257];
-  const int t = threadIdx.x, bin = t >> 2, q = t & 3;
-  const int per = (nblocks + 3) / 4;
-  const int b0 = min(nblocks, q * per), b1 = min(nblocks, b0 + per);
-  int local = 0;
-  for (int b = b0; b < b1; ++b) local += hist[b * 256 + bin];
-  int incl = local;
-#pragma unroll
-  for (int d = 1; d < 4; d <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, d, 4); if (q >= d) incl += v; }
-  if (q == 3) s_tot[bin] = incl;
-  __syncthreads();
-  if (t < 32) {  // exclusive scan of 256 bin totals, 8 per lane
-    int v[8], sum = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { v[k] = s_tot[t * 8 + k]; sum += v[k]; }
-    int inc = sum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { int u = __shfl_up_sync(0xffffffffu, inc, d); if (t >= d) inc += u; }
-    int run = inc - sum;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { s_start[t * 8 + k] = run; run += v[k]; }
-  }
-  __syncthreads();
-  int running = s_start[bin] + (incl - local);
-  for (int b = b0; b < b1; ++b) { offsets[b * 256 + bin] = running; running += hist[b * 256 + bin]; }
-}
-
-__global__ void __launch_bounds__(VT) k_radix_scatter(const unsigned* __restrict__ keys_in, const int* __restrict__ vals_in, const int* __restrict__ n_ptr,
-                                                      int shift, const int* __restrict__ offsets, unsigned* __restrict__ keys_out,
-                                                      int* __restrict__ vals_out) {
-  pdl_launch_dependents();
-  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
-  __shared__ int s_cnt[VIT * (VT / 32)][256];   // [slot = it*8 + warp][digit] -> exclusive prefix over slots
-  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
-  const int n = *n_ptr;
-  if (blockIdx.x * VCH >= n) return;
-  for (int k = tid; k < VIT * (VT / 32) * 256; k += VT) (&s_cnt[0][0])[k] = 0;
-  __syncthreads();
-  int dig[VIT], rank[VIT];
-#pragma unroll
-  for (int it = 0; it < VIT; ++it) {
-    const int i = blockIdx.x * VCH + it * VT + tid;
-    const int d = i < n ? (int)((keys_in[i] >> shift) & 255u) : -1;
-    dig[it] = d;
-    const unsigned grp = __match_any_sync(0xffffffffu, d);
-    rank[it] = __popc(grp & ((1u << lane) - 1u));
-    if (d >= 0 && rank[it] == 0) s_cnt[it * (VT / 32) + w][d] = __popc(grp);
-  }
-  __syncthreads();
-  {
-    int run = offsets[blockIdx.x * 256 + tid];
-#pragma unroll
-    for (int k = 0; k < VIT * (VT / 32); ++k) { const int c = s_cnt[k][tid]; s_cnt[k][tid] = run; run += c; }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int it = 0; it < VIT; ++it) {
-    if (dig[it] < 0) continue;
-    const int i = blockIdx.x * VCH + it * VT + tid;
-    const int dst = s_cnt[it * (VT / 32) + w][dig[it]] + rank[it];
-    keys_out[dst] = keys_in[i];
-    vals_out[dst] = vals_in[i];
-  }
-}
-
 // All passes of the LSD radix sort in ONE cooperative launch (the segmented filters of the mapper sort a few 10^4 keys: twelve
 // launches of a few microseconds each were launch latency, not work).  Tiles of VCH keys go round-robin over the CTAs; per pass:
 // tile histograms -> grid barrier -> every CTA derives the offsets of its own tiles from the histogram table (thread = digit:
 // digit totals over all tiles, block-wide exclusive scan, plus the running sum over the tiles before its own) and scatters ->
-// grid barrier.  Same stable order as k_radix_hist / k_radix_scan / k_radix_scatter; the result is in buffer (passes & 1).
+// grid barrier.  Within a digit the keys keep their order (stable); the result is in buffer (passes & 1).
 __global__ void __launch_bounds__(VT) k_radix_sort_all(unsigned* __restrict__ k0, int* __restrict__ v0, unsigned* __restrict__ k1, int* __restrict__ v1,
                                                        const int* __restrict__ n_ptr, int bits, int* __restrict__ hist) {
   namespace cg = cooperative_groups;
@@ -272,60 +156,9 @@ __global__ void __launch_bounds__(1024) k_vox_blockscan(int* __restrict__ block_
   for (int k = 0; k < per; ++k) { const int b = t * per + k; if (b < nblocks) { const int c = block_heads[b]; block_heads[b] = run; run += c; } }
 }
 
-// every head sums its run in sorted order (float, like pcl::CentroidPoint) and writes voxel number (block offset + local rank)
-__global__ void __launch_bounds__(VT) k_vox_emit(const Pt4* __restrict__ pts, const unsigned* __restrict__ keys, const int* __restrict__ vals,
-                                                 const int* __restrict__ n_ptr, const int* __restrict__ block_offsets, Pt4* __restrict__ out) {
-  const int n = *n_ptr;
-  if (blockIdx.x * VCH >= n) return;
-  __shared__ int s_w[VT / 32];
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int base = blockIdx.x * VCH + tid * VIT;   // this thread owns VIT consecutive sorted slots
-  int heads = 0;
-  bool is_head[VIT];
-#pragma unroll
-  for (int k = 0; k < VIT; ++k) {
-    const int i = base + k;
-    is_head[k] = i < n && (i == 0 || keys[i] != keys[i - 1]);
-    heads += is_head[k] ? 1 : 0;
-  }
-  int incl = heads;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { int u = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += u; }
-  if (lane == 31) s_w[w] = incl;
-  __syncthreads();
-  int wbase = 0;
-  for (int v = 0; v < w; ++v) wbase += s_w[v];
-  int slot = block_offsets[blockIdx.x] + wbase + incl - heads;
-#pragma unroll
-  for (int k = 0; k < VIT; ++k) {
-    if (!is_head[k]) continue;
-    const int i = base + k;
-    const unsigned key = keys[i];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-    int cnt = 0;
-    for (int j = i; j < n && keys[j] == key; ++j) {
-      const Pt4 p = pts[vals[j]];
-      sx += p.x; sy += p.y; sz += p.z; si += p.i;
-      ++cnt;
-    }
-    const float nf = (float)cnt;
-    Pt4 o; o.x = sx / nf; o.y = sy / nf; o.z = sz / nf; o.i = si / nf;
-    out[slot++] = o;
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------
-// Segmented, device-resident form: S independent clouds ("segments", each with its own leaf size) are filtered by ONE
-// sequence of launches -- the two scan stacks of a mapping frame (laserMapping.cpp:543-549), or all valid cubes of the map
-// after insertion (:787-801, up to 75 corner + 75 surf cubes).  Sizes live in device memory; nothing here synchronises
-// with the host.  Key = segment << idx_bits | voxel index (PCL's index inside the segment's own bounding box), so one
-// stable LSD radix sort orders every segment by voxel and keeps the segments apart; everything else is the single-cloud
-// algorithm above, per segment: same bounding-box rule, same float centroid accumulation in sorted order.
-// A segment whose index range overflows int (PCL: "leaf size is too small", input returned unchanged) or idx_bits keeps its
-// points as they are (key = position).
-
 __device__ __forceinline__ int seg_count(const SegFilter& f) { return min(max(*f.n_seg - f.seg0, 0), f.seg_cap); }
+// segment number of a key; idx_bits may be 32 (one segment), so the shift is done in 64 bits
+__device__ __forceinline__ int seg_of(unsigned key, int idx_bits) { return (int)((unsigned long long)key >> idx_bits); }
 
 __global__ void __launch_bounds__(256) k_seg_prep(SegFilter f) {
   pdl_launch_dependents();
@@ -406,10 +239,14 @@ __global__ void __launch_bounds__(256) k_seg_keys(SegFilter f, unsigned* __restr
   }
   const unsigned long long cells = (unsigned long long)div_b[0] * (unsigned long long)div_b[1] * (unsigned long long)div_b[2];
   const bool pcl_overflow = dxyz[0] * dxyz[1] * dxyz[2] > (long long)INT_MAX;   // PCL: "leaf size is too small", input returned unchanged
-  const bool key_overflow = !pcl_overflow && cells > (1ull << f.idx_bits);       // cannot be encoded: flagged, points kept as they are
+  // cannot be encoded: flagged, points kept as they are.  At 32 bits the key is PCL's own int index and wraps as PCL's does.
+  const bool key_overflow = !pcl_overflow && f.idx_bits < 32 && cells > (1ull << f.idx_bits);
   const bool pass = pcl_overflow || key_overflow;
-  if (key_overflow && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(f.err, 1);
-  const unsigned hi_bits = (unsigned)sgm << f.idx_bits;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    f.pass[sgm] = pass;
+    if (key_overflow) atomicOr(f.err, 1);
+  }
+  const unsigned hi_bits = (unsigned)((unsigned long long)sgm << f.idx_bits);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     unsigned idx;
     if (pass) idx = (unsigned)i;
@@ -470,7 +307,7 @@ __global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __
       const int i = b0 + k * VT + tid;
       if (i < n) {
         const unsigned key = keys[i];
-        const int sgm = (int)(key >> f.idx_bits);
+        const int sgm = seg_of(key, f.idx_bits);
         s_keys[k * VT + tid] = key;
         s_pts[k * VT + tid] = f.seg[f.seg0 + sgm].src[vals[i] - f.off[sgm]];
       }
@@ -499,7 +336,7 @@ __global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __
       if (!is_head[k]) continue;
       const int i = base + k;
       const unsigned key = s_keys[i - b0];
-      const int sgm = (int)(key >> f.idx_bits);
+      const int sgm = seg_of(key, f.idx_bits);
       const int off = f.off[sgm];
       float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
       int cnt = 0;
@@ -526,16 +363,19 @@ __global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __
   }
 }
 
-// grid (chunks, segments): filtered points back to their destination (which may be the source slab itself)
+// grid (chunks, segments): filtered points back to their destination (which may be the source slab itself).  A pass-through
+// segment is copied from its source, not from its one-point "centroids": (0.f + x) / 1.f would turn -0.f into +0.f.
 __global__ void __launch_bounds__(256) k_seg_writeback(SegFilter f, const Pt4* __restrict__ tmp) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int sgm = blockIdx.y;
   if (sgm >= seg_count(f)) return;
   const SegDesc d = f.seg[f.seg0 + sgm];
-  const int m = f.rank0[sgm + 1] - f.rank0[sgm];
-  const int off = f.off[sgm];
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) d.dst[i] = tmp[off + i];
+  const int m = f.rank0[sgm + 1] - f.rank0[sgm];   // a pass-through segment has one key per point: m is its size
+  const bool pass = f.pass[sgm];                   // not set for an empty segment, which has m = 0
+  if (pass && d.dst == d.src) return;
+  const Pt4* __restrict__ from = pass ? d.src : tmp + f.off[sgm];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) d.dst[i] = from[i];
 }
 
 }  // namespace aloam
@@ -544,7 +384,7 @@ using namespace aloam;
 
 // segmented filter over up to S_upper segments; n_upper / per_seg_upper are host bounds for grid sizing (total points, points of
 // one segment).  The caller guarantees that the live total never exceeds b.cap: nothing here clamps it.  A 32-bit key holds f.idx_bits index bits and the segment number: when S_upper segments do not fit beside the
-// index, the segments are processed in windows of 2^(32 - idx_bits).
+// index, the segments are processed in windows of 2^(32 - idx_bits) (idx_bits = 32: one segment, 32 key bits).
 void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_upper, int n_upper, int per_seg_upper) {
   const int nblk = std::max(1, (n_upper + VCH - 1) / VCH);
   const int grid_blk = std::min(nblk, 8 * c->sms);   // k_vox_heads / k_seg_emit stride over the blocks: one resident wave at most
@@ -559,17 +399,10 @@ void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_up
     launch_ex(c, KID_VOXEL, k_seg_bbox, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f);
     launch_ex(c, KID_VOXEL, k_seg_keys, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f, b.keys[0], b.vals[0]);
     // the radix passes: one cooperative launch (all CTAs co-resident, at most one per SM)
-    static int coop_cap = 0;
-    if (!coop_cap) {
-      int per_sm = 0, sms = 0;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort_all, VT, 0);
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->cfg.device);
-      coop_cap = std::max(1, std::min(sms, per_sm * sms));
-    }
     {
       prof_begin(c, KID_VOXEL);
       cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(std::min(nblk, coop_cap)); cfg.blockDim = dim3(VT); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
+      cfg.gridDim = dim3(std::min(nblk, b.coop_grid)); cfg.blockDim = dim3(VT); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
       cfg.attrs = at; cfg.numAttrs = 1;
@@ -587,18 +420,24 @@ void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_up
 
 int vox_seg_alloc(aloam_ctx* c, SegBuffers& b, size_t cap) {
   const size_t nb = (cap + VCH - 1) / VCH + 1;
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort_all, VT, 0);
   b.cap = cap;
-  if (dalloc(c, &b.keys[0], cap) != cudaSuccess || dalloc(c, &b.keys[1], cap) != cudaSuccess ||
+  b.coop_grid = std::max(1, std::min(c->sms, per_sm * c->sms));
+  if (dalloc(c, &b.segs, ALOAM_MAX_SEGS) != cudaSuccess || dalloc(c, &b.n_seg, 1) != cudaSuccess ||
+      dalloc(c, &b.off, ALOAM_MAX_SEGS + 8) != cudaSuccess || dalloc(c, &b.rank0, ALOAM_MAX_SEGS + 8) != cudaSuccess ||
+      dalloc(c, &b.bbox, ALOAM_MAX_SEGS * 6) != cudaSuccess || dalloc(c, &b.total, 1) != cudaSuccess ||
+      dalloc(c, &b.pass, ALOAM_MAX_SEGS) != cudaSuccess ||
+      dalloc(c, &b.keys[0], cap) != cudaSuccess || dalloc(c, &b.keys[1], cap) != cudaSuccess ||
       dalloc(c, &b.vals[0], cap) != cudaSuccess || dalloc(c, &b.vals[1], cap) != cudaSuccess ||
-      dalloc(c, &b.hist, nb * 256) != cudaSuccess || dalloc(c, &b.offs, nb * 256) != cudaSuccess ||
-      dalloc(c, &b.block_heads, nb) != cudaSuccess || dalloc(c, &b.heads_total, 4) != cudaSuccess ||
-      dalloc(c, &b.tmp, cap) != cudaSuccess)
+      dalloc(c, &b.hist, nb * 256) != cudaSuccess || dalloc(c, &b.block_heads, nb) != cudaSuccess ||
+      dalloc(c, &b.heads_total, 1) != cudaSuccess || dalloc(c, &b.tmp, cap) != cudaSuccess)
     return ALOAM_ERR_CUDA;
   return ALOAM_OK;
 }
 
-
-extern "C" int aloam_voxel_filter_impl(aloam_ctx* c, aloam_cloud_view in, float leaf, aloam_cloud_view* out) {
+// the general entry point: the cloud is the one segment of a segmented filter the context owns for it (not the mapper's)
+extern "C" int aloam_voxel_filter(aloam_ctx* c, aloam_cloud_view in, float leaf, aloam_cloud_view* out) {
   if (!c || !out || !(leaf > 0.f)) return ALOAM_ERR_INVALID_ARG;
   int rc = check_view(in); if (rc) return rc;
   if (in.n > c->max_points) return ALOAM_ERR_CAPACITY;
@@ -608,69 +447,31 @@ extern "C" int aloam_voxel_filter_impl(aloam_ctx* c, aloam_cloud_view in, float 
   if (!c->h_vox_out) CUDA_CHECK_RET(halloc(c, &c->h_vox_out, (size_t)c->max_points));
   out->data = reinterpret_cast<const float*>(c->h_vox_out); out->n = 0; out->stride_floats = 4;
   if (in.n == 0) return ALOAM_OK;
-  const int n = in.n;
-  if (!c->vox_ready) {
-    const size_t mp = (size_t)c->max_points;
-    const int nb_max = (c->max_points + VCH - 1) / VCH;
-    CUDA_CHECK_RET(dalloc(c, &c->d_vox_keys[0], mp)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_keys[1], mp));
-    CUDA_CHECK_RET(dalloc(c, &c->d_vox_vals[0], mp)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_vals[1], mp));
-    CUDA_CHECK_RET(dalloc(c, &c->d_vox_hist, (size_t)nb_max * 256)); CUDA_CHECK_RET(dalloc(c, &c->d_vox_offs, (size_t)nb_max * 256));
-    CUDA_CHECK_RET(dalloc(c, &c->d_vox_misc, 64 + (size_t)nb_max));
-    c->vox_ready = true;
+  if (!c->vox_seg_ready) {   // publish nothing half-built: what a failed attempt acquired belongs to the context until aloam_destroy
+    if (dalloc(c, &c->d_seg_io, 3) != cudaSuccess || vox_seg_alloc(c, c->vox_seg, (size_t)c->max_points) != ALOAM_OK) {
+      cudaGetLastError();
+      return ALOAM_ERR_CUDA;
+    }
+    c->vox_seg_ready = true;
   }
   Pt4* d_in = c->d_query;        // staging buffers that already exist in the context
   Pt4* d_out = c->lanes[0].d_full[0];
   rc = upload_cloud(c, in, d_in, c->max_points); if (rc) return rc;
-  int* mm6 = c->d_vox_misc; int* d_total = c->d_vox_misc + 8; int* d_n = c->d_vox_misc + 9; int* block_heads = c->d_vox_misc + 64;
-  const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-  std::memcpy(c->pin->vox_init, init, sizeof(init));
-  c->pin->vox_n = n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(mm6, c->pin->vox_init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(d_n, &c->pin->vox_n, 4, cudaMemcpyHostToDevice, c->stream));
-  LAUNCH(c, KID_VOXEL, k_vox_bbox, std::min((n + 255) / 256, 592), 256, 0, d_in, n, mm6);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->vox_box, mm6, 24, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  // host replica of PCL's index-range computation (needs the box; also decides the number of radix passes)
-  float mn[3], mx[3];
-  for (int a = 0; a < 3; ++a) {
-    int lo = c->pin->vox_box[a], hi = c->pin->vox_box[3 + a];
-    lo = lo >= 0 ? lo : (lo ^ 0x7fffffff); hi = hi >= 0 ? hi : (hi ^ 0x7fffffff);
-    std::memcpy(&mn[a], &lo, 4); std::memcpy(&mx[a], &hi, 4);
-  }
-  const float inv = 1.0f / leaf;
-  long long dxyz[3]; int min_b[3], div_b[3];
-  for (int a = 0; a < 3; ++a) {
-    dxyz[a] = (long long)((mx[a] - mn[a]) * inv) + 1;
-    min_b[a] = (int)std::floor(mn[a] * inv);
-    div_b[a] = (int)std::floor(mx[a] * inv) - min_b[a] + 1;
-  }
-  const int nblk = (n + VCH - 1) / VCH;
-  if (dxyz[0] * dxyz[1] * dxyz[2] > (long long)INT_MAX) {   // "leaf size is too small": PCL returns the input unchanged
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->h_vox_out, d_in, (size_t)n * 16, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-    out->n = n;
-    return ALOAM_OK;
-  }
-  VoxParams vp; vp.inv = inv; vp.min_b[0] = min_b[0]; vp.min_b[1] = min_b[1]; vp.min_b[2] = min_b[2];
-  vp.div0 = div_b[0]; vp.div01 = div_b[0] * div_b[1];
-  LAUNCH(c, KID_VOXEL, k_vox_keys, (n + 255) / 256, 256, 0, d_in, n, vp, c->d_vox_keys[0], c->d_vox_vals[0]);
-  const unsigned long long cells = (unsigned long long)div_b[0] * (unsigned long long)div_b[1] * (unsigned long long)div_b[2];
-  int bits = 1; while (bits < 32 && (1ull << bits) < cells) ++bits;
-  int cur = 0;
-  for (int shift = 0; shift < bits; shift += 8) {
-    LAUNCH(c, KID_VOXEL, k_radix_hist, nblk, VT, 0, c->d_vox_keys[cur], d_n, shift, c->d_vox_hist);
-    LAUNCH(c, KID_VOXEL, k_radix_scan, 1, 1024, 0, c->d_vox_hist, d_n, c->d_vox_offs);
-    LAUNCH(c, KID_VOXEL, k_radix_scatter, nblk, VT, 0, c->d_vox_keys[cur], c->d_vox_vals[cur], d_n, shift, c->d_vox_offs, c->d_vox_keys[cur ^ 1],
-           c->d_vox_vals[cur ^ 1]);
-    cur ^= 1;
-  }
-  LAUNCH(c, KID_VOXEL, k_vox_heads, nblk, VT, 0, c->d_vox_keys[cur], d_n, block_heads);
-  LAUNCH(c, KID_VOXEL, k_vox_blockscan, 1, 1024, 0, block_heads, d_n, d_total);
-  LAUNCH(c, KID_VOXEL, k_vox_emit, nblk, VT, 0, d_in, c->d_vox_keys[cur], c->d_vox_vals[cur], d_n, block_heads, d_out);
-  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->vox_out_n, d_total, 4, cudaMemcpyDeviceToHost, c->stream));
+  SegBuffers& b = c->vox_seg;
+  int* io = c->d_seg_io;     // cloud size, filtered size, error word
+  PinnedScratch* p = c->pin;
+  p->vox_seg = SegDesc{d_in, io, leaf, d_out, io + 1};
+  p->vox_nseg = 1;
+  p->vox_io[0] = in.n; p->vox_io[1] = 0; p->vox_io[2] = 0;
+  CUDA_CHECK_RET(cudaMemcpyAsync(b.segs, &p->vox_seg, sizeof(SegDesc), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(b.n_seg, &p->vox_nseg, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(io, p->vox_io, sizeof(p->vox_io), cudaMemcpyHostToDevice, c->stream));
+  // 32 index bits: the key is PCL's int index itself, so every cloud PCL filters is filtered here and the error word stays 0
+  vox_seg_filter(c, seg_filter(b, 32, io + 2), b, 1, in.n, in.n);
+  CUDA_CHECK_RET(cudaMemcpyAsync(&p->vox_out_n, io + 1, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
-  const int m = c->pin->vox_out_n;
+  const int m = p->vox_out_n;
   if (m > 0) {
     CUDA_CHECK_RET(cudaMemcpyAsync(c->h_vox_out, d_out, (size_t)m * 16, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

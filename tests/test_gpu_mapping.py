@@ -108,8 +108,10 @@ def test_voxel_filter_matches_pcl_restatement(ctx, orc, synth, scans, leaf):
 
 
 def test_voxel_filter_overflow_returns_input(ctx):
-    cloud = np.array([[0, 0, 0, 1], [3000, 3000, 3000, 2], [1, 1, 1, 3]], np.float32)
-    assert np.array_equal(ctx.voxel_filter(cloud, 0.2), cloud)
+    """PCL returns the input unchanged, bit for bit: -0.0 stays -0.0"""
+    cloud = np.array([[0, 0, 0, 1], [3000, 3000, 3000, 2], [1, 1, 1, 3], [-0.0, 1, -0.0, 4]], np.float32)
+    got = ctx.voxel_filter(cloud, 0.2)
+    assert np.array_equal(got, cloud) and np.array_equal(got.view(np.uint32), cloud.view(np.uint32))
 
 
 def test_map_upload_accepts_device_memory(aloam, scene):
@@ -126,10 +128,11 @@ def test_map_upload_accepts_device_memory(aloam, scene):
     c.close()
 
 
-# ---- the single-cloud filter at its size limits: > 1024 blocks of 1024 keys (k_vox_blockscan strides), 1 to 4 radix
-# passes (an odd count leaves the sorted keys in the other buffer), runs across blocks, clouds near +-5 km
+# ---- the single-cloud filter at its size limits: > 1024 blocks of 1024 keys (k_vox_blockscan strides), voxel indices of 1 to
+# 4 bytes (the sort always runs 4 passes over the 32-bit key; all-zero high digits leave a stable sort unchanged), runs across
+# blocks, clouds near +-5 km
 
-def _radix_passes(cloud, leaf):
+def _index_bytes(cloud, leaf):
     f = np.float32
     inv = f(1) / f(leaf)
     mn, mx = cloud[:, :3].min(0), cloud[:, :3].max(0)
@@ -156,11 +159,11 @@ def _cube_cloud(rng, n, centre, side):
     return out
 
 
-@pytest.mark.parametrize("passes,side", [(1, 1.0), (2, 6.0), (3, 40.0), (4, 70.0)])
-def test_voxel_filter_radix_pass_counts(big_ctx, orc, passes, side):
-    rng = np.random.default_rng(passes)
+@pytest.mark.parametrize("index_bytes,side", [(1, 1.0), (2, 6.0), (3, 40.0), (4, 70.0)])
+def test_voxel_filter_radix_pass_counts(big_ctx, orc, index_bytes, side):
+    rng = np.random.default_rng(index_bytes)
     cloud = _cube_cloud(rng, 200000, (-3.1, 7.7, 0.4), side)
-    assert _radix_passes(cloud, 0.2) == passes
+    assert _index_bytes(cloud, 0.2) == index_bytes
     ref = orc.voxel_grid(cloud, 0.2, orc.SORT_CANONICAL)
     got = big_ctx.voxel_filter(cloud, 0.2)
     assert got.shape == ref.shape and np.array_equal(got.view(np.uint32), ref.view(np.uint32))

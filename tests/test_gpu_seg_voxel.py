@@ -155,10 +155,12 @@ def test_coordinates_at_the_edges(ctx, orc):
 
 
 def test_pcl_overflow_segment_passes_through(ctx, orc):
-    """a segment whose index range overflows PCL's int comes back unchanged, without an error, between normal ones"""
+    """a segment whose index range overflows PCL's int comes back unchanged (bit for bit: -0.0 stays -0.0), without an
+    error, between normal ones"""
     rng = np.random.default_rng(29)
     huge = cluster_cloud(rng, 3000, side=4.0)
     huge[:2] = [[-2000.0, -2000.0, -2000.0, 1.0], [2000.0, 2000.0, 2000.0, 2.0]]
+    huge[2, 0] = huge[3, 1] = huge[4, 2] = np.float32(-0.0)
     assert index_range(huge, 0.1)[0] > INT_MAX
     segs = [cluster_cloud(rng, 2500, side=6.0), huge, cluster_cloud(rng, 1800, side=3.0)]
     for idx_bits in (31, 28):
@@ -169,8 +171,9 @@ def test_pcl_overflow_segment_passes_through(ctx, orc):
 @pytest.mark.parametrize("idx_bits", [31, 24])
 def test_key_overflow_segment_is_flagged(ctx, orc, idx_bits):
     """a segment whose voxel index needs more than idx_bits bits (but not more than PCL's int): err bit 0, that segment
-    unchanged, every other segment still exact.  For 31 bits: a 25.79 m box at leaf 0.02 off the voxel lattice gives
-    dxyz = 1290^3 <= INT_MAX but 1291^3 > 2^31 cells"""
+    unchanged (bit for bit: -0.0 stays -0.0), every other segment still exact.  For 31 bits: a 25.79 m box at leaf 0.02 off
+    the voxel lattice gives dxyz = 1290^3 <= INT_MAX but 1291^3 > 2^31 cells; aloam_voxel_filter, whose key is PCL's whole
+    32-bit index, filters that cloud exactly"""
     rng = np.random.default_rng(31 + idx_bits)
     if idx_bits == 31:
         leaf, lo = 0.02, np.float32(-12.887)
@@ -179,15 +182,22 @@ def test_key_overflow_segment_is_flagged(ctx, orc, idx_bits):
     else:
         leaf = 0.1
         bad = cluster_cloud(rng, 2000, side=30.0, leaf=leaf)
+    bad[2, 0] = bad[3, 1] = bad[4, 2] = np.float32(-0.0)
     dprod, cells = index_range(bad, leaf)
     assert dprod <= INT_MAX and cells > 2**idx_bits
     segs = [cluster_cloud(rng, 1200, side=5.0), bad, np.zeros((0, 4), np.float32), cluster_cloud(rng, 3000, side=8.0)]
     got = check(ctx, orc, segs, [0.2, leaf, 0.4, 0.1], idx_bits)
     assert np.array_equal(got[1], bad)
+    if idx_bits == 31:
+        assert cells <= 2**32
+        ref = orc.voxel_grid(bad, leaf, orc.SORT_CANONICAL)
+        one = ctx.voxel_filter(bad, leaf)
+        assert one.shape == ref.shape and np.array_equal(one.view(np.uint32), ref.view(np.uint32))
 
 
 def test_debug_filter_leaves_the_mapper_alone(aloam, orc):
-    """mapper_step frames with debug filter calls between them give the same results as without"""
+    """mapper_step frames with debug filter and voxel_filter calls between them give the same results as without, and
+    voxel_filter, which has a segmented filter of its own, stays exact between the mapper's filters"""
     rng = np.random.default_rng(37)
     frames = []
     for k in range(4):
@@ -200,7 +210,12 @@ def test_debug_filter_leaves_the_mapper_alone(aloam, orc):
         out = []
         for corner, surf, q, t in frames:
             if interleave:
+                one = c.voxel_filter(surf, 0.4)
                 c.seg_voxel_filter([cluster_cloud(rng, 5000, side=9.0), surf[:3000]], [0.1, 0.2], 28)
+                ref = orc.voxel_grid(surf, 0.4, orc.SORT_CANONICAL)
+                assert np.array_equal(one.view(np.uint32), ref.view(np.uint32))
+                ref = orc.voxel_grid(corner, 0.2, orc.SORT_CANONICAL)
+                assert np.array_equal(c.voxel_filter(corner, 0.2).view(np.uint32), ref.view(np.uint32))
             out.append(np.concatenate(c.mapper_step(corner, surf, q, t)[:2]))
         st = c.mapper_state()
         out.append(np.concatenate([st["q_wmap_wodom"], st["t_wmap_wodom"]]))
