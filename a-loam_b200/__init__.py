@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = [
     "aloam_voxel_filter", "aloam_scan_to_pose", "aloam_scan_to_pose_device", "aloam_reset_odometry", "aloam_knn",
     "aloam_odometry_associate", "aloam_normal_equations", "aloam_solve", "aloam_debug_features", "aloam_mapping_associate",
     "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_debug_seg_voxel_filter", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
+    "aloam_scan_stream_mapped_batch", "aloam_mapper_debug_state_lane", "aloam_mapper_debug_cube_lane",
 ]
 
 
@@ -85,6 +86,8 @@ def lib():
         L.aloam_mapper_step.argtypes = [C.c_void_p, cv, cv, dp, dp, dp, dp, C.POINTER(Stats)]
         L.aloam_mapper_debug_state.argtypes = [C.c_void_p, ip, ip, ip, dp, dp, C.POINTER(C.c_longlong)]
         L.aloam_mapper_debug_cube.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(cv)]
+        L.aloam_mapper_debug_state_lane.argtypes = [C.c_void_p, C.c_int, ip, ip, ip, dp, dp, C.POINTER(C.c_longlong)]
+        L.aloam_mapper_debug_cube_lane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(cv)]
         L.aloam_debug_seg_voxel_filter.argtypes = [C.c_void_p, C.POINTER(cv), fp, C.c_int, C.c_int, fp, ip, ip]
         L.aloam_scan_to_pose.argtypes = [C.c_void_p, cv, dp, dp, C.POINTER(Stats)]
         L.aloam_scan_to_pose_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, dp, C.POINTER(Stats)]
@@ -92,6 +95,7 @@ def lib():
         L.aloam_scan_stream.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, dp, C.POINTER(Stats)]
         L.aloam_scan_stream_batch.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, C.c_int, dp, C.POINTER(Stats)]
         L.aloam_scan_stream_mapped.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, dp, dp, C.POINTER(Stats)]
+        L.aloam_scan_stream_mapped_batch.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, C.c_int, dp, dp, C.POINTER(Stats)]
         L.aloam_transform_to_end.argtypes = [C.c_void_p, cv, dp, dp, C.c_int, C.POINTER(cv)]
         L.aloam_knn.argtypes = [C.c_void_p, C.c_int, cv, C.c_int, ip, fp]
         L.aloam_odometry_associate.argtypes = [C.c_void_p, cv, cv, dp, dp, ip, ip]
@@ -243,16 +247,17 @@ class Aloam:
         _check(lib().aloam_mapper_step(self._h, a, b, _dp(qo), _dp(to), _dp(q), _dp(t), C.byref(st)))
         return q, t, st.as_dict()
 
-    def mapper_state(self):
+    def mapper_state(self, lane=0):
+        """cube-store state of one mapper lane (lane 0: aloam_mapper_step and both mapped stream calls)"""
         cen = (C.c_int * 3)(); nv = C.c_int(0); valid = (C.c_int * 125)(); tot = (C.c_longlong * 2)()
         q = np.zeros(4); t = np.zeros(3)
-        _check(lib().aloam_mapper_debug_state(self._h, cen, C.byref(nv), valid, _dp(q), _dp(t), tot))
+        _check(lib().aloam_mapper_debug_state_lane(self._h, int(lane), cen, C.byref(nv), valid, _dp(q), _dp(t), tot))
         return {"centre": tuple(cen), "valid": list(valid[:nv.value]), "q_wmap_wodom": q, "t_wmap_wodom": t,
                 "total_corner": int(tot[0]), "total_surf": int(tot[1])}
 
-    def mapper_cube(self, which, cube_index):
+    def mapper_cube(self, which, cube_index, lane=0):
         out = CloudView()
-        _check(lib().aloam_mapper_debug_cube(self._h, which, cube_index, C.byref(out)))
+        _check(lib().aloam_mapper_debug_cube_lane(self._h, int(lane), which, cube_index, C.byref(out)))
         return _out(out)
 
     def seg_voxel_filter(self, segs, leaves, idx_bits=31):
@@ -373,6 +378,22 @@ class Aloam:
         _check(lib().aloam_scan_stream_batch(self._h, views, n, b, int(device_resident), _dp(poses), st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return poses
+
+    def scan_stream_mapped_batch(self, ptrs, counts, device_resident, stride=4):
+        """aloam_scan_stream_mapped_batch: ptrs / counts are (n_scans, batch) arrays as for scan_stream_batch; returns
+        (odom poses, map poses), (n_scans, batch, 7) each.  Every lane is bit-identical to its solo scan_stream_mapped run."""
+        ptrs = np.asarray(ptrs, np.uint64)
+        counts = np.asarray(counts, np.int64)
+        n, b = ptrs.shape
+        views = (CloudView * (n * b))()
+        for k in range(n):
+            for j in range(b):
+                views[k * b + j] = CloudView(C.cast(C.c_void_p(int(ptrs[k, j])), C.POINTER(C.c_float)), int(counts[k, j]), stride)
+        odom = np.zeros((n, b, 7)); mapped = np.zeros((n, b, 7))
+        st = (Stats * b)()
+        _check(lib().aloam_scan_stream_mapped_batch(self._h, views, n, b, int(device_resident), _dp(odom), _dp(mapped), st))
+        self.last_batch_stats = [s.as_dict() for s in st]
+        return odom, mapped
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

@@ -502,7 +502,7 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
 // and trajectory.  raws / poses are scan-major: entry k * nb + b.
 static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int nb, int device_resident, double* poses, aloam_stats* stats_last,
                             double* map_poses = nullptr) {
-  if (map_poses && (nb != 1 || !c || c->cfg.max_map_points <= 0)) return ALOAM_ERR_INVALID_ARG;
+  if (map_poses && (!c || c->cfg.max_map_points <= 0)) return ALOAM_ERR_INVALID_ARG;
   if (!c || !raws || !poses || n_scans < 1 || nb < 1 || nb > c->n_lanes || (long long)n_scans * nb > kMaxStreamScans) return ALOAM_ERR_INVALID_ARG;
   for (int k = 0; k < n_scans * nb; ++k) {
     int rc = check_view(raws[k]); if (rc) return rc;
@@ -512,7 +512,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
   }
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (map_poses && !c->mapper) { int rc = aloam_mapper_reset(c); if (rc) return rc; }   // creates the cube store
+  if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
   StreamGuard guard(c);
   cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
@@ -527,7 +527,8 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     return code;
   };
 #define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return fail(ALOAM_ERR_CUDA); } } while (0)
-  if (map_poses) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c), 0, sizeof(int), s_main));   // the mapper's error bits of this call
+  if (map_poses)   // the mappers' error bits of this call
+    for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
   // everything issued on the main stream before this call (reset, earlier calls) is ordered before the side streams.
   // Waiting on an event that was never recorded, or whose work finished in an earlier call, is a no-op -- so the
@@ -595,11 +596,16 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
       // ---- scan-to-map on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose go
       //      to the mapping stage on the device -- what the reference ships through /laser_cloud_corner_last, /laser_cloud_surf_last
       //      and /laser_odom_to_init (laserOdometry.cpp:570-591 -> laserMapping.cpp:278-288) never leaves HBM
+      //      One frame covers every trajectory: each launch of it serves all lanes, each lane with its own cube store.
       STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
       c->stream = c->s_map;
-      const FeatBuf& fc = c->lanes[0].feat[cur];
-      rc = mapper_step_device(c, fc.less_sharp, fc.counts + 1, 64 * kMaxLessSharpPerRing, fc.less_flat, fc.counts + 3, std::min(nmax, c->max_points),
-                              c->d_poses + (size_t)k * 7, c->d_map_poses + (size_t)k * 7);
+      MapperIn in[ALOAM_MAX_BATCH];
+      for (int l = 0; l < nb; ++l) {
+        const FeatBuf& fc = c->lanes[l].feat[cur];
+        const size_t slot = ((size_t)k * nb + l) * 7;
+        in[l] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot};
+      }
+      rc = mapper_step_device(c, nb, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
       if (rc) return fail(rc);
       STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
       c->stream = s_main;
@@ -615,7 +621,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   if (map_poses) {
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapdone[c->cur], 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
-    STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err, mapper_err_acc(c), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+    for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
   }
   for (int l = 0; l < nb; ++l) {
     STREAM_TRY(cudaMemcpyAsync(c->h_summary + 4 * l, c->lanes[l].d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, s_main));
@@ -643,8 +649,12 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
-  // as aloam_mapper_step: a voxel index range beyond the key width in any frame means its map results would be wrong
-  if (map_poses && (c->pin->mapper_err & 1)) return ALOAM_ERR_CAPACITY;
+  // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
+  if (map_poses) {
+    c->pin->mapper_err = 0;
+    for (int l = 0; l < nb; ++l) c->pin->mapper_err |= c->pin->mapper_err_lane[l];
+    if (c->pin->mapper_err & 1) return ALOAM_ERR_CAPACITY;
+  }
   return ALOAM_OK;
 }
 
@@ -661,6 +671,13 @@ int aloam_scan_stream_mapped(aloam_ctx* c, const aloam_cloud_view* raws, int n_s
 int aloam_scan_stream_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* poses,
                             aloam_stats* stats_last) {
   return scan_stream_impl(c, raws, n_scans, batch, device_resident, poses, stats_last);
+}
+
+int aloam_scan_stream_mapped_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* odom_poses,
+                                   double* map_poses, aloam_stats* stats_last) {
+  if (!map_poses) return ALOAM_ERR_INVALID_ARG;
+  if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  return scan_stream_impl(c, raws, n_scans, batch, device_resident, odom_poses, stats_last, map_poses);
 }
 
 // ------------------------------------------------------------------------------------------------ fine-grained

@@ -10,6 +10,37 @@
 #include "../../include/aloam_b200.h"
 #include "kernels.h"
 
+namespace aloam {
+// the buffers of one scan-to-map registration (mapping.cu): the two indexed submaps, the neighbours found by k_map_knn5, the
+// residual blocks and the solve summaries.  The context's set serves the host API and lane 0 of the mapper; every other lane
+// of aloam_scan_stream_mapped_batch owns a set of its own.
+struct MapReg {
+  MapCloud corner, surf;
+  float4* nbr;
+  BlockRec* blocks;
+  LmSummary* summary;   // [4]
+};
+// one lane of the mapper's index build (the submap clouds) and registration (the filtered stacks, their sizes
+// {n_corner, n_surf, total} and the pose being refined), all device pointers
+struct MapLaneIO {
+  MapReg reg;
+  const Pt4* sub[2];
+  const Pt4* stack[2];
+  const int* counts3;
+  double* pose;
+};
+// one lane's input to a mapper frame (cubemap.cu): the scan's less-sharp / less-flat clouds and their sizes, its odometry pose
+// and the slot of the refined pose, all device pointers
+struct MapperIn {
+  const Pt4* corner;
+  const int* nc;
+  const Pt4* surf;
+  const int* ns;
+  const double* odom7;
+  double* out7;
+};
+}  // namespace aloam
+
 using namespace aloam;
 
 namespace {
@@ -62,6 +93,7 @@ struct PinnedScratch {
   int stack_counts[3];      // scan-to-map stacks: n_corner, n_surf, total
   int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
   int mapper_err;           // aloam_scan_stream_mapped: the mapper's error bits, OR over the call's frames
+  int mapper_err_lane[ALOAM_MAX_BATCH];   // aloam_scan_stream_mapped_batch: the same per lane
   SegDesc vox_seg;          // aloam_voxel_filter: the cloud as the one segment of its filter
   int vox_nseg;             //                     1
   int vox_io[3];            //                     cloud size, filtered size, error word: {n, 0, 0}
@@ -96,7 +128,9 @@ struct aloam_ctx {
   void* peer = nullptr;          // peer-memory exchange of the sharded LM (comm.cu), when enabled
   double* d_lm_tot = nullptr;    // [64] all-reduced normal equations of one evaluation (sharded LM)
   void* d_lm_state = nullptr;    // device-resident trust-region state (sharded LM)
-  void* mapper = nullptr;        // map cube store (cubemap.cu), created on first use
+  // map cube store of every lane (cubemap.cu), each created on first use: lane 0 serves the host API and both mapped stream
+  // calls, lanes 1 .. max_batch-1 only aloam_scan_stream_mapped_batch
+  void* mapper[ALOAM_MAX_BATCH] = {};
   // scan-to-map: uploaded submap (corner, surf) with hash grids, stack queries, fit debug records
   MapCloud map_corner = {}, map_surf = {};
   Pt4* d_map_pts[2] = {nullptr, nullptr};   // staging for maps handed in as host views (device views are indexed in place)
@@ -219,14 +253,18 @@ inline void launch_lm(aloam_ctx* c, bool pdl, const BlockRec* blocks, const int*
 }  // namespace
 // sharded LM (comm.cu): per evaluation one kernel for the local blocks, one exchange of 32 doubles, one step kernel
 void launch_lm_sharded(aloam_ctx* c, const aloam::BlockRec* blocks, const int* d_n, double* pose, const aloam::LmParams& lp, aloam::LmSummary* summary);
-void vox_seg_filter(aloam_ctx* c, const aloam::SegFilter& f, aloam::SegBuffers& b, int S_upper, int n_upper, int per_seg_upper);
+void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper);
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
-int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, int n_upper_c, const Pt4* d_surf_last, const int* d_ns, int n_upper_s,
-                       const double* d_odom7, double* d_out7);
-int* mapper_err_acc(aloam_ctx* c);
-void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n_upper);
+int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
+int mapper_ensure_lanes(aloam_ctx* c, int nb);
+int* mapper_err_acc(aloam_ctx* c, int lane);
+MapReg ctx_map_reg(const aloam_ctx* c);
+MapLaneIO ctx_map_io(const aloam_ctx* c, const Pt4* sub_corner, const Pt4* sub_surf);
+Batch<GridArgs> grid_setup_args(const MapLaneIO& io, const int* na, const int* nb);
+int map_reg_alloc(aloam_ctx* c, MapReg* r, Pt4** stack_corner, Pt4** stack_surf);
+void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_corner, const Pt4* sub_surf, const int* n_surf, int n_upper, int* err_word);
-void map_register_device(aloam_ctx* c, const Pt4* d_corner_stack, const Pt4* d_surf_stack, const int* d_counts3, int nq_upper, double* d_pose, bool want_fits);
+void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, double* d_fits);
 namespace {
 
 LmParams lm_params(const aloam_config& c) {

@@ -72,8 +72,28 @@ struct Mapper {
   int* d_dbg_counts = nullptr;              //                                their sizes [ALOAM_MAX_SEGS]
   int* d_dbg_err = nullptr;                 //                                private error word
   int max_sub = 0;
+  MapReg reg = {};                          // lanes > 0: a registration set of their own (lane 0 uses the context's, shared with
+  Pt4* d_stack[2] = {nullptr, nullptr};     //            the host API) and the filtered corner / surf stacks
   cudaStream_t s_aux = nullptr;             // the stack filters run here, beside the submap gather + index build
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+};
+
+// what every kernel of a frame needs of one lane: the frame runs over all lanes at once, each launch taking one record per lane
+// (lane = blockIdx.z)
+struct MapperLane {
+  MapperState* S;
+  const double* odom7;   // odometry pose of this scan
+  double* out7;          // refined pose out (may be null)
+  Pt4* pts[2];           // slab pools
+  int cap[2];
+  Pt4* sub[2];           // gathered submap
+  const Pt4* in[2];      // less-sharp / less-flat clouds of the scan and their sizes
+  const int* n_in[2];
+  Pt4* stack[2];         // filtered stacks
+  Pt4* world;            // insertion scratch
+  int* cube;
+  SegDesc* segs;         // the lane's segmented filter
+  int* n_seg;
 };
 
 // ---- Eigen-order quaternion helpers (operation order of Eigen::Quaternion: the pose hand-off is compared bit for bit)
@@ -133,7 +153,7 @@ __device__ void rotate_line(MapperState* S, int axis, bool towards_high, int u, 
 }
 
 // transformAssociateToMap (:142-146), centre cube + shift (:314-509), valid cubes (:511-529), gather offsets
-__global__ void __launch_bounds__(1024) k_mapper_begin(MapperState* S, const double* __restrict__ odom7, int max_sub) {
+__device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   __shared__ int s_ctr[3], s_cen[3];
@@ -207,9 +227,15 @@ __global__ void __launch_bounds__(1024) k_mapper_begin(MapperState* S, const dou
     S->n_sub[ty] = off;
   }
 }
+// grid (1, 1, lanes)
+__global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub) {
+  const MapperLane& a = B.a[blockIdx.z];
+  mapper_begin_body(a.S, a.odom7, max_sub);
+}
+
 
 // grid (valid cubes, 2 types): slab -> submap (:531-539), device to device
-__global__ void __launch_bounds__(256) k_mapper_gather(const MapperState* __restrict__ S, const Pt4* __restrict__ p0, const Pt4* __restrict__ p1,
+__device__ __forceinline__ void mapper_gather_body(const MapperState* __restrict__ S, const Pt4* __restrict__ p0, const Pt4* __restrict__ p1,
                                                        int cap0, int cap1, Pt4* __restrict__ sub0, Pt4* __restrict__ sub1) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -222,9 +248,15 @@ __global__ void __launch_bounds__(256) k_mapper_gather(const MapperState* __rest
   Pt4* __restrict__ dst = (ty ? sub1 : sub0) + off;
   for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }
+// grid (valid cubes, 2 types, lanes)
+__global__ void __launch_bounds__(256) k_mapper_gather(const __grid_constant__ Batch<MapperLane> B) {
+  const MapperLane& a = B.a[blockIdx.z];
+  mapper_gather_body(a.S, a.pts[0], a.pts[1], a.cap[0], a.cap[1], a.sub[0], a.sub[1]);
+}
+
 
 // segment descriptors of the two scan-stack filters (:543-549)
-__global__ void k_seg_two(SegDesc* segs, int* n_seg, const Pt4* c_in, const int* nc, float c_leaf, Pt4* c_out, int* nc_out, const Pt4* s_in, const int* ns,
+__device__ __forceinline__ void seg_two_body(SegDesc* segs, int* n_seg, const Pt4* c_in, const int* nc, float c_leaf, Pt4* c_out, int* nc_out, const Pt4* s_in, const int* ns,
                           float s_leaf, Pt4* s_out, int* ns_out) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -234,9 +266,15 @@ __global__ void k_seg_two(SegDesc* segs, int* n_seg, const Pt4* c_in, const int*
     *n_seg = 2;
   }
 }
+// grid (1, 1, lanes)
+__global__ void k_seg_two(const __grid_constant__ Batch<MapperLane> B, float c_leaf, float s_leaf) {
+  const MapperLane& a = B.a[blockIdx.z];
+  seg_two_body(a.segs, a.n_seg, a.in[0], a.n_in[0], c_leaf, a.stack[0], &a.S->stack_counts[0], a.in[1], a.n_in[1], s_leaf, a.stack[1], &a.S->stack_counts[1]);
+}
+
 
 // after the stack filters: the map-too-thin test of :554 (on the gathered submap) -> number of queries the registration sees
-__global__ void k_mapper_prep(MapperState* S) {
+__device__ __forceinline__ void mapper_prep_body(MapperState* S) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (threadIdx.x || blockIdx.x) return;
@@ -246,9 +284,11 @@ __global__ void k_mapper_prep(MapperState* S) {
   if (!ok) S->flags |= ALOAM_FLAG_MAP_TOO_THIN;
   S->stack_counts[2] = ok ? total : 0;   // zero residual blocks: the solve leaves the pose untouched, like the skipped optimisation
 }
+__global__ void k_mapper_prep(const __grid_constant__ Batch<MapperLane> B) { mapper_prep_body(B.a[blockIdx.z].S); }   // grid (1, 1, lanes)
+
 
 // transformUpdate (:148-152) ; refined pose out
-__global__ void k_mapper_update(MapperState* S, double* __restrict__ out7) {
+__device__ __forceinline__ void mapper_update_body(MapperState* S, double* __restrict__ out7) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (threadIdx.x || blockIdx.x) return;
@@ -261,12 +301,17 @@ __global__ void k_mapper_update(MapperState* S, double* __restrict__ out7) {
   if (out7) for (int k = 0; k < 7; ++k) out7[k] = S->x[k];
   S->frames++;
 }
+__global__ void k_mapper_update(const __grid_constant__ Batch<MapperLane> B) {   // grid (1, 1, lanes)
+  const MapperLane& a = B.a[blockIdx.z];
+  mapper_update_body(a.S, a.out7);
+}
+
 
 // end of the frame, after insertion and re-filter have set their error bits: slab overflow, pool exhaustion and submap
 // truncation become this frame's ALOAM_FLAG_CUBE_OVERFLOW, the frame's word joins the per-call accumulation, and `err` starts
 // the next frame clear (everything of the next frame -- the stack filter forked onto the auxiliary stream included -- is
 // ordered after this kernel)
-__global__ void k_mapper_finish(MapperState* S) {
+__device__ __forceinline__ void mapper_finish_body(MapperState* S) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (threadIdx.x || blockIdx.x) return;
@@ -276,10 +321,12 @@ __global__ void k_mapper_finish(MapperState* S) {
   S->err_acc |= e;
   S->err = 0;
 }
+__global__ void k_mapper_finish(const __grid_constant__ Batch<MapperLane> B) { mapper_finish_body(B.a[blockIdx.z].S); }   // grid (1, 1, lanes)
+
 
 // pointAssociateToMap (:154-163) in double, stored as float, then the cube of the stored point (:741-758)
 // blockIdx.y = cloud (0 corner stack, 1 surf stack); the scratch of cloud 1 starts `scratch_stride` elements in
-__global__ void k_cube_ids(const Pt4* __restrict__ stack0, const Pt4* __restrict__ stack1, const MapperState* __restrict__ S, Pt4* __restrict__ world,
+__device__ __forceinline__ void cube_ids_body(const Pt4* __restrict__ stack0, const Pt4* __restrict__ stack1, const MapperState* __restrict__ S, Pt4* __restrict__ world,
                            int* __restrict__ cube, int scratch_stride) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -305,12 +352,18 @@ __global__ void k_cube_ids(const Pt4* __restrict__ stack0, const Pt4* __restrict
     cube[i] = (ci >= 0 && ci < CW && cj >= 0 && cj < CH && ck >= 0 && ck < CD) ? cube_index(ci, cj, ck) : -1;
   }
 }
+// grid (CTAs, 2 clouds, lanes)
+__global__ void k_cube_ids(const __grid_constant__ Batch<MapperLane> B, int scratch_stride) {
+  const MapperLane& a = B.a[blockIdx.z];
+  cube_ids_body(a.stack[0], a.stack[1], a.S, a.world, a.cube, scratch_stride);
+}
+
 
 // stable append of the stack points to their cubes (push_back order = stack order, :759-767).  ONE CTA per cloud (blockIdx.x: the
 // corner and the surf store are independent, the two appends run side by side): the stack is walked in
 // chunks of 1024; inside a chunk the warps take turns, the lanes of one cube form a group (__match_any) whose leader
 // advances the cube's running end in shared memory -- and takes a slab from the free list when the cube had none.
-__global__ void __launch_bounds__(1024) k_cube_insert(const Pt4* __restrict__ world, const int* __restrict__ cube, int scratch_stride, MapperState* S,
+__device__ __forceinline__ void cube_insert_body(const Pt4* __restrict__ world, const int* __restrict__ cube, int scratch_stride, MapperState* S,
                                                       Pt4* __restrict__ pts0, int cap0, Pt4* __restrict__ pts1, int cap1) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -360,9 +413,15 @@ __global__ void __launch_bounds__(1024) k_cube_insert(const Pt4* __restrict__ wo
   }
   for (int c = tid; c < NCUBE; c += blockDim.x) { const int s = s_slab[c]; if (s >= 0) { slab_of[c] = s; cnt[s] = min(s_end[c], cap); } }
 }
+// grid (2 clouds, 1, lanes): every CTA has its own shared cube tables and takes slabs from its lane's free list
+__global__ void __launch_bounds__(1024) k_cube_insert(const __grid_constant__ Batch<MapperLane> B, int scratch_stride) {
+  const MapperLane& a = B.a[blockIdx.z];
+  cube_insert_body(a.world, a.cube, scratch_stride, a.S, a.pts[0], a.cap[0], a.pts[1], a.cap[1]);
+}
+
 
 // segment descriptors of the per-cube re-filter (:770-801): every valid cube that has a slab, corner cubes then surf cubes, in place
-__global__ void __launch_bounds__(256) k_seg_cubes(MapperState* S, SegDesc* segs, int* n_seg, Pt4* p0, Pt4* p1, int cap0, int cap1, float leaf0, float leaf1) {
+__device__ __forceinline__ void seg_cubes_body(MapperState* S, SegDesc* segs, int* n_seg, Pt4* p0, Pt4* p1, int cap0, int cap1, float leaf0, float leaf1) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int t = threadIdx.x, nv = S->n_valid;
@@ -375,6 +434,12 @@ __global__ void __launch_bounds__(256) k_seg_cubes(MapperState* S, SegDesc* segs
   }
   if (t == 0) { *n_seg = 2 * nv; S->zero = 0; }
 }
+// grid (1, 1, lanes)
+__global__ void __launch_bounds__(256) k_seg_cubes(const __grid_constant__ Batch<MapperLane> B, float leaf0, float leaf1) {
+  const MapperLane& a = B.a[blockIdx.z];
+  seg_cubes_body(a.S, a.segs, a.n_seg, a.pts[0], a.pts[1], a.cap[0], a.cap[1], leaf0, leaf1);
+}
+
 
 // points one segmented filter can sort: the re-filter takes every point of the <= 75 valid cubes of each type, full slabs
 // included (the submap gather truncates only its own copy at max_map_points), the stack filter two scan clouds
@@ -382,8 +447,23 @@ size_t refilter_bound(const Mapper* m, const aloam_ctx* c) {
   return std::max((size_t)75 * (m->cap[0] + m->cap[1]), (size_t)2 * c->max_points);
 }
 
-int ensure_mapper(aloam_ctx* c) {
-  if (c->mapper) return ALOAM_OK;
+// the state of a fresh trajectory: identity T_wmap_wodom, centre cube (10, 10, 5), no slabs in use (laserMapping.cpp:74-117)
+int reset_lane(aloam_ctx* c, Mapper* m) {
+  MapperState* h = m->h_state;
+  std::memset(h, 0, sizeof(*h));
+  h->q_wmap_wodom[3] = 1.0;
+  h->cen[0] = 10; h->cen[1] = 10; h->cen[2] = 5;
+  for (int t = 0; t < 2; ++t) {
+    for (int i = 0; i < NCUBE; ++i) h->slab_of[t][i] = -1;
+    for (int i = 0; i < kPool; ++i) h->free_list[t][i] = i;
+  }
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state, h, sizeof(*h), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  return ALOAM_OK;
+}
+
+int ensure_mapper(aloam_ctx* c, int lane) {
+  if (c->mapper[lane]) return ALOAM_OK;
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   Mapper* m = new (std::nothrow) Mapper();
   if (!m) return ALOAM_ERR_CUDA;
@@ -405,99 +485,122 @@ int ensure_mapper(aloam_ctx* c) {
   ok = ok && screate(c, &m->s_aux) == cudaSuccess;
   ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
+  ok = ok && (lane == 0 || map_reg_alloc(c, &m->reg, &m->d_stack[0], &m->d_stack[1]) == ALOAM_OK);
   if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
     cudaGetLastError();
     return ALOAM_ERR_CUDA;
   }
-  c->mapper = m;
+  const int rc = reset_lane(c, m);   // a lane is published with the state of a fresh trajectory, never uninitialised
+  if (rc) return rc;
+  c->mapper[lane] = m;
   return ALOAM_OK;
 }
 
 }  // namespace
 
-// One frame of alaserMapping's process() on the current stream, entirely on the device.  corner_last / surf_last and their
-// sizes, the odometry pose (7 doubles) and the output pose slot are device pointers; n_upper_* bound the cloud sizes.
-int mapper_step_device(aloam_ctx* c, const Pt4* d_corner_last, const int* d_nc, int n_upper_c, const Pt4* d_surf_last, const int* d_ns, int n_upper_s,
-                       const double* d_odom7, double* d_out7) {
-  int rc = ensure_mapper(c); if (rc) return rc;
-  Mapper* m = static_cast<Mapper*>(c->mapper);
-  MapperState* S = m->d_state;
-  // the registration buffers of mapping.cu (grids, stacks, blocks) are shared with the host API
+// One frame of alaserMapping's process() for nb trajectories ("lanes") on the current stream, entirely on the device: every launch
+// covers all lanes, lane l in blockIdx.z, and each lane has its own cube store, stack filter buffers and registration set, so
+// lane l computes exactly what a frame of lane l alone computes.  in[l]: the lane's less-sharp / less-flat clouds and their
+// sizes, its odometry pose (7 doubles) and its output pose slot, all device pointers; n_upper_* bound the cloud sizes of every
+// lane.  Lane 0 registers with the buffers of mapping.cu that it shares with the host API.  A sharded job maps one lane.
+int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
+  if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && c->shard_count > 1)) return ALOAM_ERR_STATE;
+  int rc;
+  for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, l); if (rc) return rc; }
   if (!c->map_ready) {
     aloam_cloud_view none{nullptr, 0, 4};
     rc = aloam_map_upload_impl(c, none, none); if (rc) return rc;
   }
-  // ---- stack filters (:541-550): one segmented pass for both clouds.  They read only the scan's clouds, the gather + index
-  // build below only the cube store: two independent chains, the filters forked onto an auxiliary stream and joined before the
-  // registration.
-  {
-    cudaStream_t main_stream = c->stream;
-    CUDA_CHECK_RET(cudaEventRecord(m->ev_fork, main_stream));
-    CUDA_CHECK_RET(cudaStreamWaitEvent(m->s_aux, m->ev_fork, 0));
-    c->stream = m->s_aux;
-    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1), dim3(32), 0, 1, false, m->buf.segs, m->buf.n_seg, d_corner_last, d_nc, c->cfg.line_res, c->d_stack_corner, &S->stack_counts[0], d_surf_last, d_ns,
-              c->cfg.plane_res, c->d_stack_surf, &S->stack_counts[1]);
-    vox_seg_filter(c, seg_filter(m->buf, 31, &S->err), m->buf, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
-    const cudaError_t e = cudaEventRecord(m->ev_join, m->s_aux);
-    c->stream = main_stream;
-    CUDA_CHECK_RET(e);
-  }
-  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1), dim3(1024), 0, 1, true, S, d_odom7, m->max_sub);
-  launch_ex(c, KID_CUBES, k_mapper_gather, dim3(dim3(kMaxValid, 2)), dim3(256), 0, 1, true, (const MapperState*)S, (const Pt4*)m->d_pts[0], (const Pt4*)m->d_pts[1], m->cap[0], m->cap[1],
-         m->d_sub[0], m->d_sub[1]);
-  if (c->shard_count > 1) {
-    // A rank of a sharded job keeps the WHOLE cube store (the insertions below are replicated: the refined pose is bit-identical
-    // on every rank) but indexes and searches only its x-slabs (+ halo) of the submap; the ranks meet in the all-reduce of the
-    // normal equations inside the solve.  The too-thin test of k_mapper_prep is on the whole submap, the same on every rank.
-    rc = map_shard_index_device(c, m->d_sub[0], &S->n_sub[0], m->d_sub[1], &S->n_sub[1], m->max_sub, &S->err); if (rc) return rc;
-  } else {
-    launch_ex(c, KID_MAP_GRID, k_grid_setup, dim3(1), dim3(32), 0, 1, true, c->map_corner.grid, (const int*)&S->n_sub[0], c->map_surf.grid, (const int*)&S->n_sub[1]);
-    map_index_build(c, m->d_sub[0], m->d_sub[1], m->max_sub);
-  }
-  c->have_map = true;
-  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, m->ev_join, 0));   // join: the filtered stacks are ready
-  launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1), dim3(32), 0, 1, true, S);
-  // ---- optimisation (:554-733)
-  const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  map_register_device(c, c->d_stack_corner, c->d_stack_surf, S->stack_counts, nq_upper, S->x, false);
-  launch_ex(c, KID_CUBES, k_mapper_update, dim3(1), dim3(32), 0, 1, true, S, d_out7);
-  // ---- insertion (:736-767)
-  const int up = std::max(n_upper_c, n_upper_s);
-  launch_ex(c, KID_CUBES, k_cube_ids, dim3(std::max(1, std::min((up + 255) / 256, c->sms * 2)), 2), dim3(256), 0, 1, true, (const Pt4*)c->d_stack_corner, (const Pt4*)c->d_stack_surf,
-            (const MapperState*)S, m->d_world, m->d_cube, c->max_points);
-  launch_ex(c, KID_CUBES, k_cube_insert, dim3(2), dim3(1024), 0, 1, true, (const Pt4*)m->d_world, (const int*)m->d_cube, c->max_points, S, m->d_pts[0], m->cap[0], m->d_pts[1], m->cap[1]);
-  // ---- per-cube re-filter of the valid cubes (:770-801): one segmented pass over <= 150 cubes, in place
-  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1), dim3(256), 0, 1, true, S, m->buf.segs, m->buf.n_seg, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->cfg.line_res, c->cfg.plane_res);
+  Mapper* m0 = static_cast<Mapper*>(c->mapper[0]);
+  Batch<MapperLane> B = {};
+  MapLaneIO io[ALOAM_MAX_BATCH];
+  SegFilter stack_f[ALOAM_MAX_BATCH], cube_f[ALOAM_MAX_BATCH];
+  SegBuffers* bufs[ALOAM_MAX_BATCH];
+  Batch<GridArgs> gs = {};
   // index bits of a 50 m cube at the finer leaf: (50 / leaf + 3)^3 voxels at most (PCL itself gives up beyond 2^31)
   int cube_bits = 1;
   { const double side = std::floor(50.0 / std::min(c->cfg.line_res, c->cfg.plane_res)) + 3.0; const double cells = side * side * side;
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
-  vox_seg_filter(c, seg_filter(m->buf, cube_bits, &S->err), m->buf, 2 * 75, (int)m->buf.cap, m->cap[1]);   // buf.cap = refilter_bound
-  launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1), dim3(32), 0, 1, true, S);
+  for (int l = 0; l < nb; ++l) {
+    Mapper* m = static_cast<Mapper*>(c->mapper[l]);
+    MapperState* S = m->d_state;
+    const MapReg reg = l == 0 ? ctx_map_reg(c) : m->reg;
+    Pt4* const stack_corner = l == 0 ? c->d_stack_corner : m->d_stack[0];
+    Pt4* const stack_surf = l == 0 ? c->d_stack_surf : m->d_stack[1];
+    B.a[l] = MapperLane{S, in[l].odom7, in[l].out7, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, {m->d_sub[0], m->d_sub[1]}, {in[l].corner, in[l].surf},
+                        {in[l].nc, in[l].ns}, {stack_corner, stack_surf}, m->d_world, m->d_cube, m->buf.segs, m->buf.n_seg};
+    io[l] = MapLaneIO{reg, {m->d_sub[0], m->d_sub[1]}, {stack_corner, stack_surf}, S->stack_counts, S->x};
+    gs.a[l] = GridArgs{reg.corner.grid, m->d_sub[0], &S->n_sub[0], reg.surf.grid, m->d_sub[1], &S->n_sub[1]};
+    stack_f[l] = seg_filter(m->buf, 31, &S->err);
+    cube_f[l] = seg_filter(m->buf, cube_bits, &S->err);
+    bufs[l] = &m->buf;
+  }
+  const int max_sub = m0->max_sub, cap1 = m0->cap[1];
+  const int refilter_cap = (int)m0->buf.cap;   // refilter_bound: the same for every lane
+  // ---- stack filters (:541-550): one segmented pass for both clouds of every lane.  They read only the scans' clouds, the
+  // gather + index build below only the cube stores: two independent chains, the filters forked onto an auxiliary stream and
+  // joined before the registration.
+  {
+    cudaStream_t main_stream = c->stream;
+    CUDA_CHECK_RET(cudaEventRecord(m0->ev_fork, main_stream));
+    CUDA_CHECK_RET(cudaStreamWaitEvent(m0->s_aux, m0->ev_fork, 0));
+    c->stream = m0->s_aux;
+    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1, 1, nb), dim3(32), 0, 1, false, B, c->cfg.line_res, c->cfg.plane_res);
+    vox_seg_filter(c, nb, stack_f, bufs, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
+    const cudaError_t e = cudaEventRecord(m0->ev_join, m0->s_aux);
+    c->stream = main_stream;
+    CUDA_CHECK_RET(e);
+  }
+  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub);
+  launch_ex(c, KID_CUBES, k_mapper_gather, dim3(kMaxValid, 2, nb), dim3(256), 0, 1, true, B);
+  if (c->shard_count > 1) {
+    // A rank of a sharded job keeps the WHOLE cube store (the insertions below are replicated: the refined pose is bit-identical
+    // on every rank) but indexes and searches only its x-slabs (+ halo) of the submap; the ranks meet in the all-reduce of the
+    // normal equations inside the solve.  The too-thin test of k_mapper_prep is on the whole submap, the same on every rank.
+    MapperState* S = m0->d_state;
+    rc = map_shard_index_device(c, m0->d_sub[0], &S->n_sub[0], m0->d_sub[1], &S->n_sub[1], max_sub, &S->err); if (rc) return rc;
+  } else {
+    launch_ex(c, KID_MAP_GRID, k_grid_setup, dim3(1, 1, nb), dim3(32), 0, 1, true, gs);
+    map_index_build(c, nb, io, max_sub);
+  }
+  c->have_map = true;
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, m0->ev_join, 0));   // join: the filtered stacks are ready
+  launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  // ---- optimisation (:554-733)
+  const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
+  map_register_device(c, nb, io, nq_upper, nullptr);
+  launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  // ---- insertion (:736-767)
+  const int up = std::max(n_upper_c, n_upper_s);
+  launch_ex(c, KID_CUBES, k_cube_ids, dim3(std::max(1, std::min((up + 255) / 256, std::max(1, c->sms * 2 / nb))), 2, nb), dim3(256), 0, 1, true, B, c->max_points);
+  launch_ex(c, KID_CUBES, k_cube_insert, dim3(2, 1, nb), dim3(1024), 0, 1, true, B, c->max_points);
+  // ---- per-cube re-filter of the valid cubes (:770-801): one segmented pass over <= 150 cubes of every lane, in place
+  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1, 1, nb), dim3(256), 0, 1, true, B, c->cfg.line_res, c->cfg.plane_res);
+  vox_seg_filter(c, nb, cube_f, bufs, 2 * 75, refilter_cap, cap1);
+  launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
 
-// the per-call error accumulation of aloam_scan_stream_mapped (device word; the mapper must exist)
-int* mapper_err_acc(aloam_ctx* c) { return &static_cast<Mapper*>(c->mapper)->d_state->err_acc; }
+// the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
+int* mapper_err_acc(aloam_ctx* c, int lane) { return &static_cast<Mapper*>(c->mapper[lane])->d_state->err_acc; }
+
+// the cube stores of lanes 0 .. nb-1, each created on first use with the state of a fresh trajectory.  A failure leaves the
+// lanes that existed untouched.
+int mapper_ensure_lanes(aloam_ctx* c, int nb) {
+  for (int l = 0; l < nb; ++l) { int rc = ensure_mapper(c, l); if (rc) return rc; }
+  return ALOAM_OK;
+}
 
 extern "C" {
 
 int aloam_mapper_reset(aloam_ctx* c) {
   if (!c) return ALOAM_ERR_INVALID_ARG;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  int rc = ensure_mapper(c); if (rc) return rc;
-  Mapper* m = static_cast<Mapper*>(c->mapper);
-  MapperState* h = m->h_state;
-  std::memset(h, 0, sizeof(*h));
-  h->q_wmap_wodom[3] = 1.0;
-  h->cen[0] = 10; h->cen[1] = 10; h->cen[2] = 5;
-  for (int t = 0; t < 2; ++t) {
-    for (int i = 0; i < NCUBE; ++i) h->slab_of[t][i] = -1;
-    for (int i = 0; i < kPool; ++i) h->free_list[t][i] = i;
-  }
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state, h, sizeof(*h), cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  const bool fresh = c->mapper[0] == nullptr;
+  int rc = ensure_mapper(c, 0); if (rc) return rc;   // a new lane 0 is reset already
+  for (int l = fresh ? 1 : 0; l < ALOAM_MAX_BATCH; ++l)   // every lane that exists
+    if (c->mapper[l]) { rc = reset_lane(c, static_cast<Mapper*>(c->mapper[l])); if (rc) return rc; }
   return ALOAM_OK;
 }
 
@@ -508,10 +611,8 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   rc = check_view(surf_last); if (rc) return rc;
   if (corner_last.n > c->max_points || surf_last.n > c->max_points) return ALOAM_ERR_CAPACITY;   // before any state is touched
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  const bool fresh = c->mapper == nullptr;
-  rc = ensure_mapper(c); if (rc) return rc;
-  if (fresh) { rc = aloam_mapper_reset(c); if (rc) return rc; }
-  Mapper* m = static_cast<Mapper*>(c->mapper);
+  rc = mapper_ensure_lanes(c, 1); if (rc) return rc;
+  Mapper* m = static_cast<Mapper*>(c->mapper[0]);
   CUDA_CHECK_RET(cudaEventRecord(c->ev0, c->stream));
   // the inputs are uploaded to mapper-owned device buffers first: the views may alias any ctx-owned pinned buffer
   rc = upload_cloud(c, corner_last, m->d_in[0], c->max_points); if (rc) return rc;
@@ -521,7 +622,8 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   for (int k = 0; k < 4; ++k) c->pin->mapper_pose_in[k] = q_wodom_curr[k];
   for (int k = 0; k < 3; ++k) c->pin->mapper_pose_in[4 + k] = t_wodom_curr[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->pin->mapper_pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  rc = mapper_step_device(c, m->d_in[0], &m->d_state->in_counts[0], corner_last.n, m->d_in[1], &m->d_state->in_counts[1], surf_last.n, m->d_pose_io, m->d_pose_io + 7);
+  const MapperIn one{m->d_in[0], &m->d_state->in_counts[0], m->d_in[1], &m->d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7};
+  rc = mapper_step_device(c, 1, &one, corner_last.n, surf_last.n);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -539,10 +641,12 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   return ALOAM_OK;
 }
 
-int aloam_mapper_debug_state(aloam_ctx* c, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4], double t_wmap_wodom[3],
-                             long long totals[2]) {
-  if (!c || !c->mapper) return ALOAM_ERR_STATE;
-  Mapper* m = static_cast<Mapper*>(c->mapper);
+int aloam_mapper_debug_state_lane(aloam_ctx* c, int lane, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4],
+                                  double t_wmap_wodom[3], long long totals[2]) {
+  if (!c) return ALOAM_ERR_STATE;
+  if (lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
+  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
+  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
   const MapperState* h = m->h_state;
@@ -559,9 +663,15 @@ int aloam_mapper_debug_state(aloam_ctx* c, int centre[3], int* n_valid, int vali
   return ALOAM_OK;
 }
 
-int aloam_mapper_debug_cube(aloam_ctx* c, int which, int cube, aloam_cloud_view* out) {
-  if (!c || !c->mapper || !out || which < 0 || which > 1 || cube < 0 || cube >= NCUBE) return ALOAM_ERR_INVALID_ARG;
-  Mapper* m = static_cast<Mapper*>(c->mapper);
+int aloam_mapper_debug_state(aloam_ctx* c, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4], double t_wmap_wodom[3],
+                             long long totals[2]) {
+  return aloam_mapper_debug_state_lane(c, 0, centre, n_valid, valid, q_wmap_wodom, t_wmap_wodom, totals);
+}
+
+int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, aloam_cloud_view* out) {
+  if (!c || !out || which < 0 || which > 1 || cube < 0 || cube >= NCUBE || lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
+  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
+  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
   const int s = m->h_state->slab_of[which][cube];
@@ -569,6 +679,11 @@ int aloam_mapper_debug_cube(aloam_ctx* c, int which, int cube, aloam_cloud_view*
   out->data = reinterpret_cast<const float*>(c->h_out[4]); out->n = n; out->stride_floats = 4;
   if (n > 0) CUDA_CHECK_RET(cudaMemcpy(c->h_out[4], m->d_pts[which] + (size_t)s * m->cap[which], (size_t)n * sizeof(Pt4), cudaMemcpyDeviceToHost));
   return ALOAM_OK;
+}
+
+int aloam_mapper_debug_cube(aloam_ctx* c, int which, int cube, aloam_cloud_view* out) {
+  if (!c || !c->mapper[0]) return ALOAM_ERR_INVALID_ARG;
+  return aloam_mapper_debug_cube_lane(c, 0, which, cube, out);
 }
 
 int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, const float* leaves, int n_segs, int idx_bits, float* out,
@@ -585,10 +700,8 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
   }
   if (total > 0 && !out) return ALOAM_ERR_INVALID_ARG;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  const bool fresh = c->mapper == nullptr;
-  int rc = ensure_mapper(c); if (rc) return rc;
-  if (fresh) { rc = aloam_mapper_reset(c); if (rc) return rc; }
-  Mapper* m = static_cast<Mapper*>(c->mapper);
+  int rc = mapper_ensure_lanes(c, 1); if (rc) return rc;
+  Mapper* m = static_cast<Mapper*>(c->mapper[0]);
   if (total > m->buf.cap) return ALOAM_ERR_CAPACITY;
   if (!m->d_dbg_err) {   // first use; the pointer that marks the group as ready is allocated last
     CUDA_CHECK_RET(dalloc(c, &m->d_dbg_pts, m->buf.cap));
@@ -612,7 +725,11 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
   }
   CUDA_CHECK_RET(cudaMemcpyAsync(m->buf.n_seg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_dbg_err, 0, sizeof(int), c->stream));
-  if (n_segs > 0) vox_seg_filter(c, seg_filter(m->buf, idx_bits, m->d_dbg_err), m->buf, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
+  if (n_segs > 0) {
+    const SegFilter f = seg_filter(m->buf, idx_bits, m->d_dbg_err);
+    SegBuffers* bp = &m->buf;
+    vox_seg_filter(c, 1, &f, &bp, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
+  }
   CUDA_CHECK_RET(cudaGetLastError());
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   if (n_segs > 0) CUDA_CHECK_RET(cudaMemcpy(out_counts, m->d_dbg_counts, sizeof(int) * n_segs, cudaMemcpyDeviceToHost));

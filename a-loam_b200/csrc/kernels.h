@@ -95,17 +95,20 @@ struct GridTable {
 };
 struct MapCloud { GridTable grid; };
 unsigned grid_mask_for(int n, unsigned cap_slots);
-__global__ void k_grid_setup(GridTable a, const int* na, GridTable b, const int* nb);
-__global__ void k_grid_clear(GridTable a, GridTable b);
-__global__ void k_grid_insert(GridTable a, const Pt4* pa, GridTable b, const Pt4* pb, int shard_rank, int shard_count);
-__global__ void k_grid_alloc(GridTable a, GridTable b);
-__global__ void k_grid_fill(GridTable a, const Pt4* pa, GridTable b, const Pt4* pb);
+// the mapper's index build and association run over all lanes of aloam_scan_stream_mapped_batch at once: every kernel takes
+// one record per lane and finds its own in blockIdx.z (the host API is the batch of one)
+struct GridArgs { GridTable a; const Pt4* pa; const int* na; GridTable b; const Pt4* pb; const int* nb; };   // corner, surf
+__global__ void k_grid_setup(const __grid_constant__ Batch<GridArgs> B);    // na / nb -> GridDyn
+__global__ void k_grid_clear(const __grid_constant__ Batch<GridArgs> B);
+__global__ void k_grid_insert(const __grid_constant__ Batch<GridArgs> B, int shard_rank, int shard_count);
+__global__ void k_grid_alloc(const __grid_constant__ Batch<GridArgs> B);
+__global__ void k_grid_fill(const __grid_constant__ Batch<GridArgs> B);
 // 5-NN (warp per stack point) then line / plane fit + residual block (thread per stack point), laserMapping.cpp:577-687;
 // counts3 = {n_corner, n_surf, total} in device memory, queries = corner then surf
-__global__ void k_map_knn5(const Pt4* corner_stack, const Pt4* surf_stack, const int* counts3, MapCloud corner_map, MapCloud surf_map,
-                           const double* pose7, float4* nbr, int shard_rank, int shard_count);
-__global__ void k_map_fit(const Pt4* corner_stack, const Pt4* surf_stack, const int* counts3, const float4* nbr, BlockRec* blocks,
-                          double* fits);
+struct MapAssocArgs { const Pt4* corner_stack; const Pt4* surf_stack; const int* counts3; MapCloud corner_map, surf_map; const double* pose7;
+                      float4* nbr; BlockRec* blocks; double* fits; };
+__global__ void k_map_knn5(const __grid_constant__ Batch<MapAssocArgs> B, int shard_rank, int shard_count);
+__global__ void k_map_fit(const __grid_constant__ Batch<MapAssocArgs> B);
 __global__ void k_map_knn(MapCloud map, const Pt4* queries, int nq, int k, int* idx, float* sqd);
 
 // ---- voxel.cu: segmented, device-resident pcl::VoxelGrid (aloam_voxel_filter, the scan-stack filters and the per-cube re-filter
@@ -139,6 +142,9 @@ struct SegBuffers {
 inline SegFilter seg_filter(const SegBuffers& b, int idx_bits, int* err) {
   return SegFilter{b.segs, b.n_seg, b.off, b.rank0, b.bbox, b.total, b.pass, err, idx_bits, 0, ALOAM_MAX_SEGS};
 }
+// one lane of a segmented-filter launch over several lanes (the mapper's lanes each own a SegBuffers): the filter and its sort
+// buffers; every kernel of voxel.cu takes one per lane and finds its own in blockIdx.z
+struct VoxLane { SegFilter f; unsigned* keys[2]; int* vals[2]; int* hist; int* block_heads; int* heads_total; Pt4* tmp; };
 
 // ---- lm.cu
 struct LmParams {

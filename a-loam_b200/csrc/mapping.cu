@@ -61,7 +61,7 @@ unsigned grid_mask_for(int n, unsigned cap_slots) {
 }
 
 // device-resident sizes -> GridDyn (the mapping loop gathers the submap on the device; its size never visits the host)
-__global__ void k_grid_setup(GridTable a, const int* __restrict__ na, GridTable b, const int* __restrict__ nb) {
+__device__ __forceinline__ void grid_setup_body(GridTable a, const int* __restrict__ na, GridTable b, const int* __restrict__ nb) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -69,8 +69,11 @@ __global__ void k_grid_setup(GridTable a, const int* __restrict__ na, GridTable 
     b.dyn->n = *nb; b.dyn->mask = min(table_mask_for(*nb), b.cap_slots - 1); b.dyn->cursor = 0; b.dyn->owned = 0;
   }
 }
+// grid (1, 1, lanes)
+__global__ void k_grid_setup(const __grid_constant__ Batch<GridArgs> B) { const GridArgs& g = B.a[blockIdx.z]; grid_setup_body(g.a, g.na, g.b, g.nb); }
 
-__global__ void k_grid_clear(GridTable a, GridTable b) {
+
+__device__ __forceinline__ void grid_clear_body(GridTable a, GridTable b) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gstride = gridDim.x * blockDim.x;
@@ -79,11 +82,14 @@ __global__ void k_grid_clear(GridTable a, GridTable b) {
   for (int i = gtid; i <= ma; i += gstride) a.slots[i] = empty;
   for (int i = gtid; i <= mb; i += gstride) b.slots[i] = empty;
 }
+// grid (CTAs, 1, lanes)
+__global__ void k_grid_clear(const __grid_constant__ Batch<GridArgs> B) { const GridArgs& g = B.a[blockIdx.z]; grid_clear_body(g.a, g.b); }
+
 
 // blockIdx.y selects the cloud (0 = a, 1 = b).  (Grouping the lanes of a cell with __match_any so that one lane claims the slot for
 // the group was tried here and was slower -- the vote costs more than the atomics it saves; the fill below does profit from
 // it.)
-__global__ void k_grid_insert(GridTable a, const Pt4* __restrict__ pa, GridTable b, const Pt4* __restrict__ pb, int shard_rank,
+__device__ __forceinline__ void grid_insert_body(GridTable a, const Pt4* __restrict__ pa, GridTable b, const Pt4* __restrict__ pb, int shard_rank,
                               int shard_count) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -111,11 +117,17 @@ __global__ void k_grid_insert(GridTable a, const Pt4* __restrict__ pa, GridTable
     if ((threadIdx.x & 31) == 0 && owned) atomicAdd(&g.dyn->owned, owned);
   }
 }
+// grid (CTAs, 2 clouds, lanes)
+__global__ void k_grid_insert(const __grid_constant__ Batch<GridArgs> B, int shard_rank, int shard_count) {
+  const GridArgs& g = B.a[blockIdx.z];
+  grid_insert_body(g.a, g.pa, g.b, g.pb, shard_rank, shard_count);
+}
+
 
 // per-cell storage: block-wide exclusive scan of the counts, ONE atomicAdd per CTA and table on the cursor (a per-slot
 // atomicAdd serialises ~500k updates of a single address for a 1M-point map).  Writes the cell's START
 // into the `end` word; k_grid_fill advances it to the end.
-__global__ void __launch_bounds__(256) k_grid_alloc(GridTable a, GridTable b) {
+__device__ __forceinline__ void grid_alloc_body(GridTable a, GridTable b) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   __shared__ int s_w[2][8];
@@ -148,8 +160,11 @@ __global__ void __launch_bounds__(256) k_grid_alloc(GridTable a, GridTable b) {
     __syncthreads();
   }
 }
+// grid (CTAs, 1, lanes)
+__global__ void __launch_bounds__(256) k_grid_alloc(const __grid_constant__ Batch<GridArgs> B) { const GridArgs& g = B.a[blockIdx.z]; grid_alloc_body(g.a, g.b); }
 
-__global__ void k_grid_fill(GridTable a, const Pt4* __restrict__ pa, GridTable b, const Pt4* __restrict__ pb) {
+
+__device__ __forceinline__ void grid_fill_body(GridTable a, const Pt4* __restrict__ pa, GridTable b, const Pt4* __restrict__ pb) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const GridTable& g = blockIdx.y == 0 ? a : b;
@@ -178,6 +193,9 @@ __global__ void k_grid_fill(GridTable a, const Pt4* __restrict__ pa, GridTable b
     if (i < n) g.gpts[base + __popc(grp & ((1u << lane) - 1u))] = make_float4(p.x, p.y, p.z, __int_as_float(i));
   }
 }
+// grid (CTAs, 2 clouds, lanes)
+__global__ void k_grid_fill(const __grid_constant__ Batch<GridArgs> B) { const GridArgs& g = B.a[blockIdx.z]; grid_fill_body(g.a, g.pa, g.b, g.pb); }
+
 
 // ---- device-side shard split (SURVEY.md 8e): keeps the points of a cloud that fall in this rank's x-slabs or within one
 // cell of them (the halo), in their original order -- a stable stream compaction in three launches (per-block counts, scan of
@@ -471,7 +489,7 @@ __device__ __forceinline__ D3 cross3(const D3& a, const D3& b) { return {a.y * b
 // query w < n_corner is corner point w, else surf point w - n_corner.  nbr[5 w + j] = j-th neighbour (x, y, z, index bits);
 // nbr[5 w].w = -1 marks a query without an accepted neighbourhood (fewer than 5 points in reach, 5th farther than 1 m,
 // or -- sharded -- a cell another rank owns).
-__global__ void __launch_bounds__(256) k_map_knn5(const Pt4* __restrict__ corner_stack, const Pt4* __restrict__ surf_stack,
+__device__ __forceinline__ void map_knn5_body(const Pt4* __restrict__ corner_stack, const Pt4* __restrict__ surf_stack,
                                                   const int* __restrict__ counts3, MapCloud corner_map, MapCloud surf_map,
                                                   const double* __restrict__ pose7, float4* __restrict__ nbr, int shard_rank,
                                                   int shard_count) {
@@ -521,9 +539,15 @@ __global__ void __launch_bounds__(256) k_map_knn5(const Pt4* __restrict__ corner
     }
   }
 }
+// grid (CTAs, 1, lanes)
+__global__ void __launch_bounds__(256) k_map_knn5(const __grid_constant__ Batch<MapAssocArgs> B, int shard_rank, int shard_count) {
+  const MapAssocArgs& a = B.a[blockIdx.z];
+  map_knn5_body(a.corner_stack, a.surf_stack, a.counts3, a.corner_map, a.surf_map, a.pose7, a.nbr, shard_rank, shard_count);
+}
+
 
 // K6: one thread per stack point: line fit (:586-621) or plane fit (:650-686) on its five neighbours, residual block out.
-__global__ void __launch_bounds__(128) k_map_fit(const Pt4* __restrict__ corner_stack, const Pt4* __restrict__ surf_stack,
+__device__ __forceinline__ void map_fit_body(const Pt4* __restrict__ corner_stack, const Pt4* __restrict__ surf_stack,
                                                  const int* __restrict__ counts3, const float4* __restrict__ nbr,
                                                  BlockRec* __restrict__ blocks, double* __restrict__ fits) {
   pdl_launch_dependents();
@@ -592,6 +616,12 @@ __global__ void __launch_bounds__(128) k_map_fit(const Pt4* __restrict__ corner_
     }
   }
 }
+// grid (CTAs, 1, lanes)
+__global__ void __launch_bounds__(128) k_map_fit(const __grid_constant__ Batch<MapAssocArgs> B) {
+  const MapAssocArgs& a = B.a[blockIdx.z];
+  map_fit_body(a.corner_stack, a.surf_stack, a.counts3, a.nbr, a.blocks, a.fits);
+}
+
 
 // exact k-NN (k <= 8) against a map cloud: 27-cell block first; if its k-th distance is not inside the guaranteed
 // radius (one cell), a coalesced sweep over the whole (cell-sorted) cloud settles it
@@ -634,6 +664,20 @@ int comm_allreduce_int2(aloam_ctx* c, int* d_two);   // comm.cu
 namespace {
 inline int grid_ctas(const aloam_ctx* c) { return c->sms * 8; }   // grid-stride launches: 8 resident CTAs of 256 threads per SM
 
+// the two grid tables of one registration, sized for cfg.max_map_points (c->map_slots)
+bool alloc_grids(aloam_ctx* c, MapReg* r) {
+  for (int t = 0; t < 2; ++t) {
+    GridTable& g = (t ? r->surf : r->corner).grid;
+    if (dalloc(c, &g.slots, (size_t)c->map_slots) != cudaSuccess || dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, (size_t)c->max_map) != cudaSuccess)
+      return false;
+    if (cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess) return false;
+    g.cap_slots = (unsigned)c->map_slots;
+    g.cs = 1.0f * (1.0f + 1e-5f);   // > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
+    g.inv_cs = 1.0f / g.cs;
+  }
+  return true;
+}
+
 int ensure_map_buffers(aloam_ctx* c) {
   if (c->map_ready) return ALOAM_OK;
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
@@ -642,17 +686,9 @@ int ensure_map_buffers(aloam_ctx* c) {
   while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;   // ends: aloam_create bounds max_map_points by 2^30
   c->map_slots = (int)slots;
   const size_t mm = (size_t)c->max_map;
-  for (int t = 0; t < 2; ++t) {
-    MapCloud* m = t ? &c->map_surf : &c->map_corner;
-    GridTable& g = m->grid;
-    if (dalloc(c, &c->d_map_pts[t], mm) != cudaSuccess || dalloc(c, &g.slots, slots) != cudaSuccess ||
-        dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, mm) != cudaSuccess)
-      return ALOAM_ERR_CUDA;
-    if (cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess) return ALOAM_ERR_CUDA;
-    g.cap_slots = slots;
-    g.cs = 1.0f * (1.0f + 1e-5f);   // > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
-    g.inv_cs = 1.0f / g.cs;
-  }
+  MapReg r = {};
+  if (dalloc(c, &c->d_map_pts[0], mm) != cudaSuccess || dalloc(c, &c->d_map_pts[1], mm) != cudaSuccess || !alloc_grids(c, &r)) return ALOAM_ERR_CUDA;
+  c->map_corner = r.corner; c->map_surf = r.surf;
   const size_t mp = (size_t)c->max_points;
   if (dalloc(c, &c->d_stack_corner, mp) != cudaSuccess || dalloc(c, &c->d_stack_surf, mp) != cudaSuccess ||
       dalloc(c, &c->d_fits, 2 * mp * 14) != cudaSuccess || dalloc(c, &c->d_map_blocks, 2 * mp) != cudaSuccess ||
@@ -673,31 +709,67 @@ bool is_device_ptr(const void* p) {
 
 // K0 over two clouds already in device memory; their sizes are in the GridDyn records (host path: written by the caller;
 // mapping loop: k_grid_setup).  n_upper bounds the larger cloud (grid sizing only).
-void map_index_build(aloam_ctx* c, const Pt4* d_corner, const Pt4* d_surf, int n_upper) {
-  const int pb = std::max(1, std::min((std::max(n_upper, 1) + 255) / 256, grid_ctas(c)));
-  const unsigned slots_upper = grid_mask_for(std::max(n_upper, 1), (unsigned)c->map_slots) + 1;
-  const int tb = std::max(1, std::min((int)((slots_upper + 255) / 256), grid_ctas(c)));
-  launch_ex(c, KID_MAP_GRID, k_grid_clear, dim3(tb), dim3(256), 0, 1, true, c->map_corner.grid, c->map_surf.grid);
-  launch_ex(c, KID_MAP_GRID, k_grid_insert, dim3(dim3(pb, 2)), dim3(256), 0, 1, true, c->map_corner.grid, d_corner, c->map_surf.grid, d_surf, c->shard_rank, c->shard_count);
-  launch_ex(c, KID_MAP_GRID, k_grid_alloc, dim3(tb), dim3(256), 0, 1, true, c->map_corner.grid, c->map_surf.grid);
-  launch_ex(c, KID_MAP_GRID, k_grid_fill, dim3(dim3(pb, 2)), dim3(256), 0, 1, true, c->map_corner.grid, d_corner, c->map_surf.grid, d_surf);
+MapReg ctx_map_reg(const aloam_ctx* c) { return MapReg{c->map_corner, c->map_surf, c->d_nbr, c->d_map_blocks, c->d_map_summary}; }
+
+// the host API's lane: the context's registration set, its stacks, and the clouds to index
+MapLaneIO ctx_map_io(const aloam_ctx* c, const Pt4* sub_corner, const Pt4* sub_surf) {
+  return MapLaneIO{ctx_map_reg(c), {sub_corner, sub_surf}, {c->d_stack_corner, c->d_stack_surf}, nullptr, nullptr};
 }
 
-// outer_iters x (5-NN + fits + LM) with the stacks, their counts {n_corner, n_surf, total} and the pose all in device memory
-void map_register_device(aloam_ctx* c, const Pt4* d_corner_stack, const Pt4* d_surf_stack, const int* d_counts3, int nq_upper,
-                         double* d_pose, bool want_fits) {
+Batch<GridArgs> grid_setup_args(const MapLaneIO& io, const int* na, const int* nb) {
+  Batch<GridArgs> g = {};
+  g.a[0] = GridArgs{io.reg.corner.grid, io.sub[0], na, io.reg.surf.grid, io.sub[1], nb};
+  return g;
+}
+
+// a registration set of its own for a mapper lane other than 0 (the context's map buffers are created first: they fix the
+// table size), with the two stack buffers.  On failure what was acquired belongs to the context until aloam_destroy.
+int map_reg_alloc(aloam_ctx* c, MapReg* r, Pt4** stack_corner, Pt4** stack_surf) {
+  int rc = ensure_map_buffers(c); if (rc) return rc;
+  const size_t mp = (size_t)c->max_points;
+  *r = MapReg{};
+  if (!alloc_grids(c, r) || dalloc(c, &r->nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &r->blocks, 2 * mp) != cudaSuccess ||
+      dalloc(c, &r->summary, 4) != cudaSuccess || dalloc(c, stack_corner, mp) != cudaSuccess || dalloc(c, stack_surf, mp) != cudaSuccess)
+    return ALOAM_ERR_CUDA;
+  return ALOAM_OK;
+}
+
+// CTAs per lane of a grid-stride launch over nb lanes: one resident wave in all (8 CTAs of 256 threads per SM)
+inline int lane_ctas(const aloam_ctx* c, int nb) { return std::max(1, grid_ctas(c) / nb); }
+
+// K0 of nb lanes in one launch per phase: lane l indexes io[l].sub[0] / [1] into io[l].reg
+void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper) {
+  const int pb = std::max(1, std::min((std::max(n_upper, 1) + 255) / 256, lane_ctas(c, nb)));
+  const unsigned slots_upper = grid_mask_for(std::max(n_upper, 1), (unsigned)c->map_slots) + 1;
+  const int tb = std::max(1, std::min((int)((slots_upper + 255) / 256), lane_ctas(c, nb)));
+  Batch<GridArgs> g = {};
+  for (int l = 0; l < nb; ++l) g.a[l] = GridArgs{io[l].reg.corner.grid, io[l].sub[0], nullptr, io[l].reg.surf.grid, io[l].sub[1], nullptr};
+  launch_ex(c, KID_MAP_GRID, k_grid_clear, dim3(tb, 1, nb), dim3(256), 0, 1, true, g);
+  launch_ex(c, KID_MAP_GRID, k_grid_insert, dim3(pb, 2, nb), dim3(256), 0, 1, true, g, c->shard_rank, c->shard_count);
+  launch_ex(c, KID_MAP_GRID, k_grid_alloc, dim3(tb, 1, nb), dim3(256), 0, 1, true, g);
+  launch_ex(c, KID_MAP_GRID, k_grid_fill, dim3(pb, 2, nb), dim3(256), 0, 1, true, g);
+}
+
+// outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers io[l].stack[0] / [1] (sizes
+// io[l].counts3 = {n_corner, n_surf, total}) against io[l].reg at pose io[l].pose, all in device memory.  d_fits: lane 0 only.
+void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, double* d_fits) {
   const LmParams lp = lm_params(c->cfg);
-  const int kb = std::max(1, std::min((nq_upper + 7) / 8, grid_ctas(c)));
+  const int kb = std::max(1, std::min((nq_upper + 7) / 8, lane_ctas(c, nb)));
   const int fb = std::max(1, (nq_upper + 31) / 32);   // one warp per CTA: a few thousand serial double-precision fits spread over all SMs
+  Batch<MapAssocArgs> a = {};
+  for (int l = 0; l < nb; ++l)
+    a.a[l] = MapAssocArgs{io[l].stack[0], io[l].stack[1], io[l].counts3, io[l].reg.corner, io[l].reg.surf, io[l].pose, io[l].reg.nbr, io[l].reg.blocks,
+                          l == 0 ? d_fits : nullptr};
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
-    launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb), dim3(256), 0, 1, it > 0, d_corner_stack, d_surf_stack, d_counts3, c->map_corner, c->map_surf,
-              (const double*)d_pose, c->d_nbr, c->shard_rank, c->shard_count);
-    launch_ex(c, KID_MAP_FIT, k_map_fit, dim3(fb), dim3(32), 0, 1, true, d_corner_stack, d_surf_stack, d_counts3, (const float4*)c->d_nbr,
-              c->d_map_blocks, want_fits ? c->d_fits : (double*)nullptr);
-    if (c->shard_count <= 1)
-      launch_lm(c, true, (const BlockRec*)c->d_map_blocks, d_counts3 + 2, 0, d_pose, lp, c->d_map_summary + (it & 3), 0, (double*)nullptr, (double*)nullptr, 0);
-    else
-      launch_lm_sharded(c, c->d_map_blocks, d_counts3 + 2, d_pose, lp, c->d_map_summary + (it & 3));
+    launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb, 1, nb), dim3(256), 0, 1, it > 0, a, c->shard_rank, c->shard_count);
+    launch_ex(c, KID_MAP_FIT, k_map_fit, dim3(fb, 1, nb), dim3(32), 0, 1, true, a);
+    if (c->shard_count <= 1) {
+      Batch<LmArgs> lm = {};
+      for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
+      launch_lm_batch(c, true, lm, nb, lp, 0, 0);
+    } else {
+      launch_lm_sharded(c, io[0].reg.blocks, io[0].counts3 + 2, io[0].pose, lp, io[0].reg.summary + (it & 3));
+    }
   }
 }
 
@@ -719,8 +791,9 @@ int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_cor
     LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, reinterpret_cast<const float*>(subs[t]), 4, n_upper, ns[t], inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks,
            c->d_map_pts[t], c->max_map, err_word);
   }
-  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, c->map_corner.grid, (const int*)d_cnt, c->map_surf.grid, (const int*)(d_cnt + 1));
-  map_index_build(c, c->d_map_pts[0], c->d_map_pts[1], c->max_map);
+  const MapLaneIO io = ctx_map_io(c, c->d_map_pts[0], c->d_map_pts[1]);
+  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, grid_setup_args(io, d_cnt, d_cnt + 1));
+  map_index_build(c, 1, &io, c->max_map);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
@@ -747,7 +820,8 @@ int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud
   for (int t = 0; t < 2; ++t) { hd[t].n = views[t].n; hd[t].mask = grid_mask_for(views[t].n, (unsigned)c->map_slots); hd[t].cursor = 0; hd[t].owned = 0; }
   CUDA_CHECK_RET(cudaMemcpyAsync(c->map_corner.grid.dyn, &hd[0], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->map_surf.grid.dyn, &hd[1], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
-  map_index_build(c, src[0], src[1], std::max(corner_map.n, surf_map.n));
+  const MapLaneIO io = ctx_map_io(c, src[0], src[1]);
+  map_index_build(c, 1, &io, std::max(corner_map.n, surf_map.n));
   c->map_n[0] = corner_map.n; c->map_n[1] = surf_map.n;
   c->map_global_n[0] = corner_map.n; c->map_global_n[1] = surf_map.n;
   if (c->shard_count > 1) {
@@ -802,8 +876,9 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
       LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, src, stride, m, (const int*)nullptr, inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks, c->d_map_pts[t], c->max_map, d_cnt + 2);
     }
   }
-  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, c->map_corner.grid, (const int*)d_cnt, c->map_surf.grid, (const int*)(d_cnt + 1));
-  map_index_build(c, c->d_map_pts[0], c->d_map_pts[1], c->max_map);
+  const MapLaneIO io = ctx_map_io(c, c->d_map_pts[0], c->d_map_pts[1]);
+  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, grid_setup_args(io, d_cnt, d_cnt + 1));
+  map_index_build(c, 1, &io, c->max_map);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->shard, d_cnt, 12, cudaMemcpyDeviceToHost, c->stream));
   if (c->shard_count > 1) {
     int* d_two = d_cnt + 2;   // reuse after the error word has been copied out (stream order)
@@ -846,7 +921,9 @@ int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, alo
   rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  map_register_device(c, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, corner_stack.n + surf_stack.n, c->d_map_pose, false);
+  MapLaneIO io = ctx_map_io(c, nullptr, nullptr);
+  io.counts3 = c->d_stack_counts; io.pose = c->d_map_pose;
+  map_register_device(c, 1, &io, corner_stack.n + surf_stack.n, nullptr);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
@@ -871,9 +948,10 @@ int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_c
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   const int nq = corner_stack.n + surf_stack.n;
   if (nq > 0) {
-    LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, grid_ctas(c)), 256, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner,
-           c->map_surf, c->d_map_pose, c->d_nbr, c->shard_rank, c->shard_count);
-    LAUNCH(c, KID_MAP_FIT, k_map_fit, (nq + 31) / 32, 32, 0, c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->d_nbr, c->d_map_blocks, c->d_fits);
+    Batch<MapAssocArgs> a = {};
+    a.a[0] = MapAssocArgs{c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner, c->map_surf, c->d_map_pose, c->d_nbr, c->d_map_blocks, c->d_fits};
+    LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, grid_ctas(c)), 256, 0, a, c->shard_rank, c->shard_count);
+    LAUNCH(c, KID_MAP_FIT, k_map_fit, (nq + 31) / 32, 32, 0, a);
     CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

@@ -29,7 +29,7 @@ __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i
 // tile histograms -> grid barrier -> every CTA derives the offsets of its own tiles from the histogram table (thread = digit:
 // digit totals over all tiles, block-wide exclusive scan, plus the running sum over the tiles before its own) and scatters ->
 // grid barrier.  Within a digit the keys keep their order (stable); the result is in buffer (passes & 1).
-__global__ void __launch_bounds__(VT) k_radix_sort_all(unsigned* __restrict__ k0, int* __restrict__ v0, unsigned* __restrict__ k1, int* __restrict__ v1,
+__device__ __forceinline__ void radix_sort_all_body(unsigned* __restrict__ k0, int* __restrict__ v0, unsigned* __restrict__ k1, int* __restrict__ v1,
                                                        const int* __restrict__ n_ptr, int bits, int* __restrict__ hist) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
@@ -104,10 +104,17 @@ __global__ void __launch_bounds__(VT) k_radix_sort_all(unsigned* __restrict__ k0
     cur ^= 1;
   }
 }
+// grid (CTAs per lane, 1, lanes), cooperative: every lane sorts its own keys with its own tiles and histograms; the grid barriers
+// span all lanes, which all run the same `bits` passes
+__global__ void __launch_bounds__(VT) k_radix_sort_all(const __grid_constant__ Batch<VoxLane> B, int bits) {
+  const VoxLane& a = B.a[blockIdx.z];
+  radix_sort_all_body(a.keys[0], a.vals[0], a.keys[1], a.vals[1], a.f.total, bits, a.hist);
+}
+
 
 // number of voxel heads (first element of each run of equal keys) per block of VCH sorted elements; the CTAs stride over
 // the blocks, so the grid may be smaller than the live block count
-__global__ void __launch_bounds__(VT) k_vox_heads(const unsigned* __restrict__ keys, const int* __restrict__ n_ptr, int* __restrict__ block_heads) {
+__device__ __forceinline__ void vox_heads_body(const unsigned* __restrict__ keys, const int* __restrict__ n_ptr, int* __restrict__ block_heads) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int n = *n_ptr;
@@ -129,8 +136,13 @@ __global__ void __launch_bounds__(VT) k_vox_heads(const unsigned* __restrict__ k
     __syncthreads();
   }
 }
+__global__ void __launch_bounds__(VT) k_vox_heads(const __grid_constant__ Batch<VoxLane> B, int cur) {
+  const VoxLane& a = B.a[blockIdx.z];
+  vox_heads_body(a.keys[cur], a.f.total, a.block_heads);
+}
 
-__global__ void __launch_bounds__(1024) k_vox_blockscan(int* __restrict__ block_heads, const int* __restrict__ n_ptr, int* __restrict__ total) {
+
+__device__ __forceinline__ void vox_blockscan_body(int* __restrict__ block_heads, const int* __restrict__ n_ptr, int* __restrict__ total) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int nblocks = (*n_ptr + VCH - 1) / VCH;
@@ -155,12 +167,17 @@ __global__ void __launch_bounds__(1024) k_vox_blockscan(int* __restrict__ block_
   int run = s_w[w] + incl - sum;
   for (int k = 0; k < per; ++k) { const int b = t * per + k; if (b < nblocks) { const int c = block_heads[b]; block_heads[b] = run; run += c; } }
 }
+__global__ void __launch_bounds__(1024) k_vox_blockscan(const __grid_constant__ Batch<VoxLane> B) {
+  const VoxLane& a = B.a[blockIdx.z];
+  vox_blockscan_body(a.block_heads, a.f.total, a.heads_total);
+}
+
 
 __device__ __forceinline__ int seg_count(const SegFilter& f) { return min(max(*f.n_seg - f.seg0, 0), f.seg_cap); }
 // segment number of a key; idx_bits may be 32 (one segment), so the shift is done in 64 bits
 __device__ __forceinline__ int seg_of(unsigned key, int idx_bits) { return (int)((unsigned long long)key >> idx_bits); }
 
-__global__ void __launch_bounds__(256) k_seg_prep(SegFilter f) {
+__device__ __forceinline__ void seg_prep_body(SegFilter f) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   __shared__ int s_w[8];
@@ -187,9 +204,11 @@ __global__ void __launch_bounds__(256) k_seg_prep(SegFilter f) {
     f.bbox[6 * t + 3] = INT_MIN; f.bbox[6 * t + 4] = INT_MIN; f.bbox[6 * t + 5] = INT_MIN;
   }
 }
+__global__ void __launch_bounds__(256) k_seg_prep(const __grid_constant__ Batch<VoxLane> B) { seg_prep_body(B.a[blockIdx.z].f); }
+
 
 // grid (chunks, segments)
-__global__ void __launch_bounds__(256) k_seg_bbox(SegFilter f) {
+__device__ __forceinline__ void seg_bbox_body(SegFilter f) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int sgm = blockIdx.y;
@@ -215,9 +234,11 @@ __global__ void __launch_bounds__(256) k_seg_bbox(SegFilter f) {
     if ((threadIdx.x & 31) == 0) { atomicMin(&f.bbox[6 * sgm + a], f2ord(lo[a])); atomicMax(&f.bbox[6 * sgm + 3 + a], f2ord(hi[a])); }
   }
 }
+__global__ void __launch_bounds__(256) k_seg_bbox(const __grid_constant__ Batch<VoxLane> B) { seg_bbox_body(B.a[blockIdx.z].f); }
+
 
 // grid (chunks, segments): keys / vals in the compact order (segment after segment)
-__global__ void __launch_bounds__(256) k_seg_keys(SegFilter f, unsigned* __restrict__ keys, int* __restrict__ vals) {
+__device__ __forceinline__ void seg_keys_body(SegFilter f, unsigned* __restrict__ keys, int* __restrict__ vals) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int sgm = blockIdx.y;
@@ -261,6 +282,11 @@ __global__ void __launch_bounds__(256) k_seg_keys(SegFilter f, unsigned* __restr
     vals[off + i] = off + i;
   }
 }
+__global__ void __launch_bounds__(256) k_seg_keys(const __grid_constant__ Batch<VoxLane> B) {
+  const VoxLane& a = B.a[blockIdx.z];
+  seg_keys_body(a.f, a.keys[0], a.vals[0]);
+}
+
 
 // heads before the first sorted slot of every segment (grid: segments + 1 CTAs of one warp; CTA s ranks slot off[s])
 __device__ __forceinline__ int seg_head_rank(const unsigned* __restrict__ keys, const int* __restrict__ block_offsets, int pos, int total) {
@@ -275,7 +301,7 @@ __device__ __forceinline__ int seg_head_rank(const unsigned* __restrict__ keys, 
   for (int dd = 16; dd > 0; dd >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, dd);
   return block_offsets[b] + cnt;
 }
-__global__ void __launch_bounds__(32) k_seg_rank0(SegFilter f, const unsigned* __restrict__ keys, const int* __restrict__ block_offsets) {
+__device__ __forceinline__ void seg_rank0_body(SegFilter f, const unsigned* __restrict__ keys, const int* __restrict__ block_offsets) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int S = seg_count(f), total = *f.total;
@@ -288,10 +314,15 @@ __global__ void __launch_bounds__(32) k_seg_rank0(SegFilter f, const unsigned* _
     if (threadIdx.x == 0) *f.seg[f.seg0 + sgm].n_out = r1 - r0;
   }
 }
+__global__ void __launch_bounds__(32) k_seg_rank0(const __grid_constant__ Batch<VoxLane> B, int cur) {
+  const VoxLane& a = B.a[blockIdx.z];
+  seg_rank0_body(a.f, a.keys[cur], a.block_heads);
+}
+
 
 // every head sums its run in sorted order (float, like pcl::CentroidPoint); output slot = off[segment] + rank inside the segment.
 // The CTAs stride over the blocks of VCH sorted keys (the grid is sized by a host bound, the live total is on the device).
-__global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __restrict__ keys, const int* __restrict__ vals,
+__device__ __forceinline__ void seg_emit_body(SegFilter f, const unsigned* __restrict__ keys, const int* __restrict__ vals,
                                                  const int* __restrict__ block_offsets, Pt4* __restrict__ tmp) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
@@ -362,10 +393,15 @@ __global__ void __launch_bounds__(VT) k_seg_emit(SegFilter f, const unsigned* __
     __syncthreads();   // s_w, s_pts and s_keys are refilled for the next block
   }
 }
+__global__ void __launch_bounds__(VT) k_seg_emit(const __grid_constant__ Batch<VoxLane> B, int cur) {
+  const VoxLane& a = B.a[blockIdx.z];
+  seg_emit_body(a.f, a.keys[cur], a.vals[cur], a.block_heads, a.tmp);
+}
+
 
 // grid (chunks, segments): filtered points back to their destination (which may be the source slab itself).  A pass-through
 // segment is copied from its source, not from its one-point "centroids": (0.f + x) / 1.f would turn -0.f into +0.f.
-__global__ void __launch_bounds__(256) k_seg_writeback(SegFilter f, const Pt4* __restrict__ tmp) {
+__device__ __forceinline__ void seg_writeback_body(SegFilter f, const Pt4* __restrict__ tmp) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int sgm = blockIdx.y;
@@ -377,44 +413,58 @@ __global__ void __launch_bounds__(256) k_seg_writeback(SegFilter f, const Pt4* _
   const Pt4* __restrict__ from = pass ? d.src : tmp + f.off[sgm];
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) d.dst[i] = from[i];
 }
+__global__ void __launch_bounds__(256) k_seg_writeback(const __grid_constant__ Batch<VoxLane> B) {
+  const VoxLane& a = B.a[blockIdx.z];
+  seg_writeback_body(a.f, a.tmp);
+}
+
 
 }  // namespace aloam
 
 using namespace aloam;
 
-// segmented filter over up to S_upper segments; n_upper / per_seg_upper are host bounds for grid sizing (total points, points of
-// one segment).  The caller guarantees that the live total never exceeds b.cap: nothing here clamps it.  A 32-bit key holds f.idx_bits index bits and the segment number: when S_upper segments do not fit beside the
-// index, the segments are processed in windows of 2^(32 - idx_bits) (idx_bits = 32: one segment, 32 key bits).
-void vox_seg_filter(aloam_ctx* c, const SegFilter& f_in, SegBuffers& b, int S_upper, int n_upper, int per_seg_upper) {
+// segmented filter over up to S_upper segments in each of nb lanes (filter f[l] on buffers *b[l]); every launch covers all lanes,
+// lane l in blockIdx.z.  n_upper / per_seg_upper are host bounds per lane for grid sizing (total points, points of one segment).
+// The caller guarantees that a lane's live total never exceeds its b[l]->cap: nothing here clamps it.  A 32-bit key holds
+// f.idx_bits index bits and the segment number: when S_upper segments do not fit beside the index, the segments are processed
+// in windows of 2^(32 - idx_bits) (idx_bits = 32: one segment, 32 key bits); idx_bits is the same in every lane.
+void vox_seg_filter(aloam_ctx* c, int nb, const SegFilter* f_in, SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper) {
   const int nblk = std::max(1, (n_upper + VCH - 1) / VCH);
-  const int grid_blk = std::min(nblk, 8 * c->sms);   // k_vox_heads / k_seg_emit stride over the blocks: one resident wave at most
+  const int grid_blk = std::min(nblk, std::max(1, 8 * c->sms / nb));   // k_vox_heads / k_seg_emit stride over the blocks: one resident wave at most
   const int chunks = std::max(1, std::min((per_seg_upper + 255) / 256, S_upper > 8 ? 8 : 64));   // grid-stride inside a segment
-  const int win = (int)std::min<long long>(1ll << std::max(0, 32 - f_in.idx_bits), ALOAM_MAX_SEGS);
+  const int idx_bits = f_in[0].idx_bits;
+  const int win = (int)std::min<long long>(1ll << std::max(0, 32 - idx_bits), ALOAM_MAX_SEGS);
   for (int s0 = 0; s0 < S_upper; s0 += win) {
-    SegFilter f = f_in;
-    f.seg0 = s0; f.seg_cap = std::min(win, S_upper - s0);
-    int seg_bits = 0; while ((1 << seg_bits) < f.seg_cap) ++seg_bits;
-    const int bits = f.idx_bits + seg_bits;
-    launch_ex(c, KID_VOXEL, k_seg_prep, dim3(1), dim3(256), 0, 1, true, f);
-    launch_ex(c, KID_VOXEL, k_seg_bbox, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f);
-    launch_ex(c, KID_VOXEL, k_seg_keys, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f, b.keys[0], b.vals[0]);
-    // the radix passes: one cooperative launch (all CTAs co-resident, at most one per SM)
+    const int seg_cap = std::min(win, S_upper - s0);
+    Batch<VoxLane> B = {};
+    for (int l = 0; l < nb; ++l) {
+      SegFilter f = f_in[l];
+      f.seg0 = s0; f.seg_cap = seg_cap;
+      const SegBuffers& bl = *b[l];
+      B.a[l] = VoxLane{f, {bl.keys[0], bl.keys[1]}, {bl.vals[0], bl.vals[1]}, bl.hist, bl.block_heads, bl.heads_total, bl.tmp};
+    }
+    int seg_bits = 0; while ((1 << seg_bits) < seg_cap) ++seg_bits;
+    const int bits = idx_bits + seg_bits;
+    launch_ex(c, KID_VOXEL, k_seg_prep, dim3(1, 1, nb), dim3(256), 0, 1, true, B);
+    launch_ex(c, KID_VOXEL, k_seg_bbox, dim3(chunks, seg_cap, nb), dim3(256), 0, 1, true, B);
+    launch_ex(c, KID_VOXEL, k_seg_keys, dim3(chunks, seg_cap, nb), dim3(256), 0, 1, true, B);
+    // the radix passes: one cooperative launch (all CTAs co-resident, at most one per SM over all lanes)
     {
       prof_begin(c, KID_VOXEL);
       cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(std::min(nblk, b.coop_grid)); cfg.blockDim = dim3(VT); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
+      cfg.gridDim = dim3(std::min(nblk, std::max(1, b[0]->coop_grid / nb)), 1, nb); cfg.blockDim = dim3(VT); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
       cfg.attrs = at; cfg.numAttrs = 1;
-      cudaLaunchKernelEx(&cfg, k_radix_sort_all, b.keys[0], b.vals[0], b.keys[1], b.vals[1], (const int*)f.total, bits, b.hist);
+      cudaLaunchKernelEx(&cfg, k_radix_sort_all, B, bits);
       prof_end(c);
     }
     const int cur = ((bits + 7) / 8) & 1;
-    launch_ex(c, KID_VOXEL, k_vox_heads, dim3(grid_blk), dim3(VT), 0, 1, true, b.keys[cur], f.total, b.block_heads);
-    launch_ex(c, KID_VOXEL, k_vox_blockscan, dim3(1), dim3(1024), 0, 1, true, b.block_heads, f.total, b.heads_total);
-    launch_ex(c, KID_VOXEL, k_seg_rank0, dim3(f.seg_cap + 1), dim3(32), 0, 1, true, f, b.keys[cur], b.block_heads);
-    launch_ex(c, KID_VOXEL, k_seg_emit, dim3(grid_blk), dim3(VT), 0, 1, true, f, b.keys[cur], b.vals[cur], b.block_heads, b.tmp);
-    launch_ex(c, KID_VOXEL, k_seg_writeback, dim3(dim3(chunks, f.seg_cap)), dim3(256), 0, 1, true, f, b.tmp);
+    launch_ex(c, KID_VOXEL, k_vox_heads, dim3(grid_blk, 1, nb), dim3(VT), 0, 1, true, B, cur);
+    launch_ex(c, KID_VOXEL, k_vox_blockscan, dim3(1, 1, nb), dim3(1024), 0, 1, true, B);
+    launch_ex(c, KID_VOXEL, k_seg_rank0, dim3(seg_cap + 1, 1, nb), dim3(32), 0, 1, true, B, cur);
+    launch_ex(c, KID_VOXEL, k_seg_emit, dim3(grid_blk, 1, nb), dim3(VT), 0, 1, true, B, cur);
+    launch_ex(c, KID_VOXEL, k_seg_writeback, dim3(chunks, seg_cap, nb), dim3(256), 0, 1, true, B);
   }
 }
 
@@ -467,7 +517,9 @@ extern "C" int aloam_voxel_filter(aloam_ctx* c, aloam_cloud_view in, float leaf,
   CUDA_CHECK_RET(cudaMemcpyAsync(b.n_seg, &p->vox_nseg, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(io, p->vox_io, sizeof(p->vox_io), cudaMemcpyHostToDevice, c->stream));
   // 32 index bits: the key is PCL's int index itself, so every cloud PCL filters is filtered here and the error word stays 0
-  vox_seg_filter(c, seg_filter(b, 32, io + 2), b, 1, in.n, in.n);
+  const SegFilter f = seg_filter(b, 32, io + 2);
+  SegBuffers* bp = &b;
+  vox_seg_filter(c, 1, &f, &bp, 1, in.n, in.n);
   CUDA_CHECK_RET(cudaMemcpyAsync(&p->vox_out_n, io + 1, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());

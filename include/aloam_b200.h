@@ -158,6 +158,23 @@ int aloam_scan_stream_batch(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_
  * all ranks return the same poses (equal to a single-GPU run to rounding of the summation order). */
 int aloam_scan_stream_mapped(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_scans, int device_resident, double* odom_poses,
                              double* map_poses, aloam_stats* stats_last);
+/* aloam_scan_stream_mapped for `batch` independent trajectories ("lanes") in one context, laid out as aloam_scan_stream_batch:
+ * raws n_scans x batch views, scan-major; odom_poses / map_poses n_scans x batch x 7 doubles each; stats_last `batch` entries
+ * (odometry stats) or NULL.  The odometry of all lanes shares every launch, exactly as aloam_scan_stream_batch (its poses are
+ * bit-identical to that call's), and so does the scan-to-map stage: one frame per scan covers every lane.  For every lane
+ * b, odom_poses[:, b], map_poses[:, b] and the lane's cube store are bit-identical to running trajectory b alone through
+ * aloam_scan_stream_mapped on a fresh context with the same config; batch = 1 IS that call.  State carries over between calls.
+ * Lane 0's cube store is the one aloam_mapper_step uses; the stores of lanes 1 .. batch-1 are created on the first call that
+ * uses them (on allocation failure ALOAM_ERR_CUDA, before any state changes).  Each lane owns its slab pool (1024 x (16 k +
+ * 64 k) points x 16 B = 1.34 GB at the default caps), its re-filter sort buffers (75 x (16 k + 64 k) = 6.1 M keys, about
+ * 200 MB) and registration buffers that scale with cfg.max_points and cfg.max_map_points (about 0.2 GB at 400 000 each):
+ * about 1.75 GB per lane, 28 GB at 16 lanes (arithmetic, not measured).
+ * Errors: ALOAM_ERR_INVALID_ARG when batch > cfg.max_batch, cfg.max_map_points <= 0 or map_poses is NULL; ALOAM_ERR_STATE
+ * after aloam_comm_init with world > 1 (sharded mapping serves one trajectory); ALOAM_ERR_CAPACITY, after filling both pose
+ * arrays, when a frame of any lane met a voxel index range beyond the sort key.  Any other failure drains the streams and
+ * resets the odometry, as aloam_scan_stream does. */
+int aloam_scan_stream_mapped_batch(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident,
+                                   double* odom_poses, double* map_poses, aloam_stats* stats_last);
 int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" clouds (all trajectories) */
 
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
@@ -193,7 +210,8 @@ int aloam_debug_features(aloam_ctx* ctx, float* curvature, int* label, int* scan
 int aloam_mapping_associate(aloam_ctx* ctx, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack,
                             const double x[7], double* fits);
 
-/* ---- map cube store + the mapping loop around it (laserMapping.cpp:74-108,142-163,309-550,736-801; SURVEY.md 8 f-1).
+/* ---- map cube store + the mapping loop around it (lane 0 of the mapper; the other lanes exist only for
+ * aloam_scan_stream_mapped_batch) (laserMapping.cpp:74-108,142-163,309-550,736-801; SURVEY.md 8 f-1).
  * The 21 x 21 x 11 ring buffer of 50 m cubes lives in device memory: a pool of fixed-capacity slabs (1024 per cloud type,
  * 16 k corner / 64 k surf points each, 1.3 GB, created on first use) handed to cubes on their first insertion.
  * aloam_mapper_step is one frame of alaserMapping's process(), entirely on the device with one synchronisation at the end:
@@ -207,7 +225,7 @@ int aloam_mapping_associate(aloam_ctx* ctx, aloam_cloud_view corner_stack, aloam
  * describe that frame only); argument errors are reported before any state changes.  A cube whose voxel index range does
  * not fit the sort key is kept unfiltered and the frame returns ALOAM_ERR_CAPACITY after completing (pose and store are
  * updated); the next frame starts clean.  cfg.max_map_points must be > 0. */
-int aloam_mapper_reset(aloam_ctx* ctx);
+int aloam_mapper_reset(aloam_ctx* ctx);   /* creates lane 0 if needed; resets every lane that exists */
 int aloam_mapper_step(aloam_ctx* ctx, aloam_cloud_view corner_last, aloam_cloud_view surf_last,
                       const double q_wodom_curr[4], const double t_wodom_curr[3], double q_w_curr[4], double t_w_curr[3],
                       aloam_stats* stats);
@@ -217,6 +235,11 @@ int aloam_mapper_step(aloam_ctx* ctx, aloam_cloud_view corner_last, aloam_cloud_
 int aloam_mapper_debug_state(aloam_ctx* ctx, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4],
                              double t_wmap_wodom[3], long long totals[2]);
 int aloam_mapper_debug_cube(aloam_ctx* ctx, int which, int cube_index, aloam_cloud_view* out);
+/* the same for lane `lane` of aloam_scan_stream_mapped_batch (0 <= lane < ALOAM_MAX_BATCH): ALOAM_ERR_STATE while that
+ * lane's cube store does not exist.  aloam_mapper_debug_state / _cube are the lane-0 forms. */
+int aloam_mapper_debug_state_lane(aloam_ctx* ctx, int lane, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4],
+                                  double t_wmap_wodom[3], long long totals[2]);
+int aloam_mapper_debug_cube_lane(aloam_ctx* ctx, int lane, int which, int cube_index, aloam_cloud_view* out);
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
