@@ -24,7 +24,9 @@ EXPORTED_SYMBOLS = [
     "aloam_odometry_associate", "aloam_normal_equations", "aloam_solve", "aloam_debug_features", "aloam_mapping_associate",
     "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_debug_seg_voxel_filter", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
     "aloam_scan_stream_mapped_batch", "aloam_mapper_debug_state_lane", "aloam_mapper_debug_cube_lane",
+    "aloam_scan_stream_lanes",
 ]
+LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 
 
 class Config(C.Structure):
@@ -96,6 +98,7 @@ def lib():
         L.aloam_scan_stream_batch.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, C.c_int, dp, C.POINTER(Stats)]
         L.aloam_scan_stream_mapped.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, dp, dp, C.POINTER(Stats)]
         L.aloam_scan_stream_mapped_batch.argtypes = [C.c_void_p, C.POINTER(cv), C.c_int, C.c_int, C.c_int, dp, dp, C.POINTER(Stats)]
+        L.aloam_scan_stream_lanes.argtypes = [C.c_void_p, C.POINTER(cv), ip, C.c_int, C.c_int, C.c_int, dp, dp, C.POINTER(Stats)]
         L.aloam_transform_to_end.argtypes = [C.c_void_p, cv, dp, dp, C.c_int, C.POINTER(cv)]
         L.aloam_knn.argtypes = [C.c_void_p, C.c_int, cv, C.c_int, ip, fp]
         L.aloam_odometry_associate.argtypes = [C.c_void_p, cv, cv, dp, dp, ip, ip]
@@ -394,6 +397,28 @@ class Aloam:
         _check(lib().aloam_scan_stream_mapped_batch(self._h, views, n, b, int(device_resident), _dp(odom), _dp(mapped), st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return odom, mapped
+
+    def scan_stream_lanes(self, ptrs, counts, ops, device_resident, mapped=True, stride=4):
+        """aloam_scan_stream_lanes: ptrs / counts / ops are (n_scans, batch) arrays, ops[k, b] one of LANE_IDLE, LANE_SCAN,
+        LANE_START (an idle entry's address and count are not read).  Returns (odom poses, map poses), (n_scans, batch, 7)
+        each, NaN rows where idle; map poses is None when mapped=False (odometry only)."""
+        ptrs = np.asarray(ptrs, np.uint64)
+        counts = np.asarray(counts, np.int64)
+        ops = np.ascontiguousarray(ops, np.int32)
+        n, b = ptrs.shape
+        if counts.shape != (n, b) or ops.shape != (n, b):
+            raise ValueError("ptrs, counts and ops are (n_scans, batch) arrays")
+        views = (CloudView * (n * b))()
+        for k in range(n):
+            for j in range(b):
+                views[k * b + j] = CloudView(C.cast(C.c_void_p(int(ptrs[k, j])), C.POINTER(C.c_float)), int(counts[k, j]), stride)
+        odom = np.zeros((n, b, 7))
+        out = np.zeros((n, b, 7)) if mapped else None
+        st = (Stats * b)()
+        _check(lib().aloam_scan_stream_lanes(self._h, views, ops.ctypes.data_as(C.POINTER(C.c_int)), n, b, int(device_resident), _dp(odom),
+                                             _dp(out) if mapped else None, st))
+        self.last_batch_stats = [s.as_dict() for s in st]
+        return odom, out
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

@@ -69,6 +69,8 @@ int aloam_reset_odometry(aloam_ctx* c) {
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   if (c->s_idx) CUDA_CHECK_RET(cudaStreamSynchronize(c->s_idx));   // an index build of the last synchronous call may still be running
   c->frame = 0; c->cur = 0; c->have_last = false;
+  c->lanes_mode = false;
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_running[l] = c->lane_mapped[l] = false;
   return ALOAM_OK;
 }
 
@@ -139,6 +141,10 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
     TRY(dalloc(c, &L.d_pose, 8)); TRY(dalloc(c, &L.d_world, 8)); TRY(dalloc(c, &L.d_summary, 4));
   }
   TRY(dalloc(c, &c->d_out28, 32)); TRY(dalloc(c, &c->d_api_pose, 8));
+  TRY(dalloc(c, &c->d_ident, 7)); TRY(dalloc(c, &c->d_sc_init, 1));
+  { const double ident[7] = {0, 0, 0, 1, 0, 0, 0};
+    TRY(cudaMemcpy(c->d_ident, ident, sizeof(ident), cudaMemcpyHostToDevice));
+    TRY(cudaMemcpy(c->d_sc_init, init, sizeof(ScanScalars), cudaMemcpyHostToDevice)); }
   TRY(dalloc(c, &c->d_packed, (size_t)2 * kMaxQueries * 11));
   TRY(dalloc(c, &c->d_err, 4));
   TRY(dalloc(c, &c->d_query, mp)); TRY(dalloc(c, &c->d_knn_idx, mp)); TRY(dalloc(c, &c->d_knn_d, mp));
@@ -167,21 +173,24 @@ namespace {
 // Feature extraction is issued in two halves so that the pipelined stream call can run them on different streams:
 //   A  ring binning   (k_classify, k_ring_scan, k_scatter)  raw scan -> ring-major cloud `full[buf]`, ring_start[buf]
 //   B  per-ring work  (k_ring_features, k_compact)          full[buf] -> the four feature clouds of feat[slot]
-// Every launch covers lanes 0 .. nb-1.  `sc_slot` (returned by A, consumed by B) is the ScanScalars parity slot of this scan;
-// nfull_out (device, nb ints, may be null) receives the ring-major cloud sizes.
-int run_features_a(aloam_ctx* c, int nb, const float* const* d_raw, const int* n, int stride, int buf, int* sc_slot, int* nfull_out) {
+// Every launch covers nb records; record l is the trajectory of lane pl[l] (pl == null: lane l).  Per-record arrays (d_raw, n)
+// are indexed by record, per-lane ones by lane.  `sc_slot` (returned by A, consumed by B) is the ScanScalars parity slot of
+// this scan; nfull_out (device, one int per lane, may be null) receives the ring-major cloud sizes.
+inline int phys(const int* pl, int l) { return pl ? pl[l] : l; }
+int run_features_a(aloam_ctx* c, int nb, const float* const* d_raw, const int* n, int stride, int buf, int* sc_slot, int* nfull_out,
+                   const int* pl = nullptr) {
   int nmax = 0;
   for (int l = 0; l < nb; ++l) nmax = std::max(nmax, n[l]);
   const int blocks = (nmax + 1023) / 1024;
   const float thres = c->cfg.minimum_range;
   Batch<ClassifyArgs> ca = {}; Batch<RingScanArgs> ra = {}; Batch<ScatterArgs> sa = {};
   for (int l = 0; l < nb; ++l) {
-    Lane& L = c->lanes[l];
+    Lane& L = c->lanes[phys(pl, l)];
     ScanScalars* sc = L.d_sc + c->parity;
     ScanScalars* sc_next = L.d_sc + (c->parity + 1) % 3;
     ca.a[l] = ClassifyArgs{d_raw[l], n[l], stride, L.d_ring, L.d_hist, sc};
     ra.a[l] = RingScanArgs{d_raw[l], stride, (n[l] + 1023) / 1024, L.d_hist, L.d_offsets, L.d_ring_start[buf], L.d_scan_start, L.d_scan_end, sc, sc_next,
-                           nfull_out ? nfull_out + l : nullptr};
+                           nfull_out ? nfull_out + phys(pl, l) : nullptr};
     sa.a[l] = ScatterArgs{d_raw[l], n[l], stride, L.d_ring, L.d_offsets, sc, L.d_full[buf]};
   }
   LAUNCH(c, KID_CLASSIFY, k_classify, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
@@ -193,12 +202,13 @@ int run_features_a(aloam_ctx* c, int nb, const float* const* d_raw, const int* n
   return ALOAM_OK;
 }
 // B1: per-ring kernel -> staging set `buf` ; B2: ring-ordered concatenation of the staging set into feat[slot]
-int run_features_b1(aloam_ctx* c, int nb, int buf, int sc_slot) {
+int run_features_b1(aloam_ctx* c, int nb, int buf, int sc_slot, const int* pl = nullptr) {
   Batch<RingFeatArgs> fa = {};
   for (int l = 0; l < nb; ++l) {
-    Lane& L = c->lanes[l];
+    const int lane = phys(pl, l);
+    Lane& L = c->lanes[lane];
     fa.a[l] = RingFeatArgs{L.d_full[buf], L.d_ring_start[buf], L.st_sharp[buf], L.st_less_sharp[buf], L.st_flat[buf], L.st_less_flat[buf], L.st_counts[buf],
-                           l == 0 ? c->d_curv : nullptr, l == 0 ? c->d_label : nullptr, L.d_sc + sc_slot};
+                           lane == 0 ? c->d_curv : nullptr, lane == 0 ? c->d_label : nullptr, L.d_sc + sc_slot};
   }
   // one trajectory: a cluster of two CTAs per ring (picks | voxel sort, see features.cu) ; a batch: one CTA per ring and trajectory
   if (nb == 1) launch_ex(c, KID_RING_FEATURES, k_ring_features, dim3(2 * c->cfg.n_scans, 1), dim3(512), ring_features_smem_bytes(c->max_ring, true), 2, false, fa, c->cfg.n_scans, 0.2f, c->max_ring);
@@ -206,10 +216,10 @@ int run_features_b1(aloam_ctx* c, int nb, int buf, int sc_slot) {
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
-int run_features_b2(aloam_ctx* c, int nb, int buf, int slot, bool pdl) {
+int run_features_b2(aloam_ctx* c, int nb, int buf, int slot, bool pdl, const int* pl = nullptr) {
   Batch<CompactArgs> ka = {};
   for (int l = 0; l < nb; ++l) {
-    Lane& L = c->lanes[l];
+    Lane& L = c->lanes[phys(pl, l)];
     FeatBuf& out = L.feat[slot];
     ka.a[l] = CompactArgs{L.st_sharp[buf], L.st_less_sharp[buf], L.st_flat[buf], L.st_less_flat[buf], L.st_counts[buf], out.sharp, out.less_sharp, out.flat,
                           out.less_flat, out.counts, out.rs_ls, out.rs_lf};
@@ -228,11 +238,11 @@ int run_features(aloam_ctx* c, int nb, const float* const* d_raw, const int* n, 
 }
 
 // index over the two "last" clouds of feat[slot]: count -> scan -> fill (n_ls / n_lf = host upper bounds on the cloud sizes)
-void run_grid_build(aloam_ctx* c, int nb, int slot, int n_ls, int n_lf) {
+void run_grid_build(aloam_ctx* c, int nb, int slot, int n_ls, int n_lf, const int* pl = nullptr) {
   const int pb = (std::max(std::max(n_ls, n_lf), 1) + 255) / 256;
   Batch<RabArgs> ga = {};
   for (int l = 0; l < nb; ++l) {
-    FeatBuf& f = c->lanes[l].feat[slot];
+    FeatBuf& f = c->lanes[phys(pl, l)].feat[slot];
     ga.a[l] = RabArgs{f.g_ls, f.less_sharp, f.counts + 1, f.g_lf, f.less_flat, f.counts + 3};
   }
   LAUNCH(c, KID_GRID_BUILD, k_rab_count, dim3(pb, 2, nb), 256, 0, ga);
@@ -243,7 +253,7 @@ void run_grid_build(aloam_ctx* c, int nb, int slot, int n_ls, int n_lf) {
 // outer_iters x (association + LM) ; feat[cur] supplies sharp/flat, feat[last] the targets ; pose in lane.d_pose
 // pose_slots (device, lane-major 7 doubles each, may be null): the integrated world pose is also written there by the last solve
 void run_register(aloam_ctx* c, int nb, int cur, int last, int sharp_slots, int flat_slots, bool integrate, bool want_corr, double* pose_slots,
-                  double* pose_override = nullptr /* lane 0: solve for this pose instead of the lane's warm start */) {
+                  double* pose_override = nullptr /* lane 0: solve for this pose instead of the lane's warm start */, const int* pl = nullptr) {
   OdomParams op{c->cfg.dist_sq_thresh, c->cfg.nearby_scan, c->cfg.distortion};
   const LmParams lp = lm_params(c->cfg);
   const int slots = sharp_slots + flat_slots;
@@ -251,12 +261,13 @@ void run_register(aloam_ctx* c, int nb, int cur, int last, int sharp_slots, int 
     const bool last_it = it == c->cfg.outer_iters - 1;
     Batch<AssocArgs> aa = {}; Batch<LmArgs> la = {};
     for (int l = 0; l < nb; ++l) {
-      Lane& L = c->lanes[l];
+      const int lane = phys(pl, l);
+      Lane& L = c->lanes[lane];
       const FeatBuf& fc = L.feat[cur];
       const FeatBuf& fl = L.feat[last];
       double* pose = (l == 0 && pose_override) ? pose_override : L.d_pose;
       aa.a[l] = AssocArgs{fc.sharp, fc.flat, fc.counts, last_corner(fl), last_surf(fl), pose, L.d_blocks, want_corr ? L.d_corr : nullptr};
-      la.a[l] = LmArgs{L.d_blocks, nullptr, slots, pose, L.d_summary + (it & 3), (integrate && last_it && pose_slots) ? pose_slots + (size_t)l * 7 : nullptr, L.d_world};
+      la.a[l] = LmArgs{L.d_blocks, nullptr, slots, pose, L.d_summary + (it & 3), (integrate && last_it && pose_slots) ? pose_slots + (size_t)lane * 7 : nullptr, L.d_world};
     }
     // within one call the chain association -> LM -> association -> LM is launched with programmatic dependencies
     if (slots > 0) launch_ex(c, KID_ODOM_ASSOC, k_odom_assoc, dim3((slots + 7) / 8, nb), dim3(256), 0, 1, it > 0, aa, op, sharp_slots);
@@ -477,6 +488,7 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
 
 int aloam_scan_to_pose(aloam_ctx* c, aloam_cloud_view raw, double q_w[4], double t_w[3], aloam_stats* stats) {
   if (!c || !q_w || !t_w) return ALOAM_ERR_INVALID_ARG;
+  if (c->lanes_mode) return ALOAM_ERR_STATE;   // the frame counter belongs to the lane schedule until aloam_reset_odometry
   int rc = check_view(raw); if (rc) return rc;
   if (raw.n == 0) return ALOAM_ERR_EMPTY_CLOUD;
   if (raw.n > c->max_points) return ALOAM_ERR_CAPACITY;
@@ -488,6 +500,7 @@ int aloam_scan_to_pose(aloam_ctx* c, aloam_cloud_view raw, double q_w[4], double
 
 int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_w[4], double t_w[3], aloam_stats* stats) {
   if (!c || !q_w || !t_w || !d_raw) return ALOAM_ERR_INVALID_ARG;
+  if (c->lanes_mode) return ALOAM_ERR_STATE;
   if (n <= 0) return ALOAM_ERR_EMPTY_CLOUD;
   if (n > c->max_points) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
@@ -500,19 +513,54 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
 // (main stream) and the host->device copies of scan k+2 (s_h2d) -- the overlap the reference gets from its three ROS
 // processes.  Every launch covers all nb trajectories.  Results are identical to calling aloam_scan_to_pose once per scan
 // and trajectory.  raws / poses are scan-major: entry k * nb + b.
+// ops (n_scans x nb, scan-major) is the lane schedule of aloam_scan_stream_lanes, null for the lockstep calls (every lane scans
+// at every step, the context's first step only initialises).  A step runs its non-idle lanes only, packed into records
+// 0 .. na-1 of every launch (record i = lane act[i], which owns the buffers, pose slots and cube store); a step without any
+// issues nothing and leaves the frame counter alone.
 static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int nb, int device_resident, double* poses, aloam_stats* stats_last,
-                            double* map_poses = nullptr) {
+                            double* map_poses = nullptr, const int* ops = nullptr) {
   if (map_poses && (!c || c->cfg.max_map_points <= 0)) return ALOAM_ERR_INVALID_ARG;
   if (!c || !raws || !poses || n_scans < 1 || nb < 1 || nb > c->n_lanes || (long long)n_scans * nb > kMaxStreamScans) return ALOAM_ERR_INVALID_ARG;
-  for (int k = 0; k < n_scans * nb; ++k) {
-    int rc = check_view(raws[k]); if (rc) return rc;
-    if (raws[k].n == 0) return ALOAM_ERR_EMPTY_CLOUD;
-    if (raws[k].n > c->max_points) return ALOAM_ERR_CAPACITY;
-    if (device_resident && raws[k].stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
-    if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call (lane schedule)
+  int run_err = ALOAM_OK;                                   // lane schedule: a scan that cannot run fails the call like a run-time error
+  if (!ops) {
+    if (c->lanes_mode) return ALOAM_ERR_STATE;   // the frame counter belongs to the lane schedule until aloam_reset_odometry
+    for (int k = 0; k < n_scans * nb; ++k) {
+      int rc = check_view(raws[k]); if (rc) return rc;
+      if (raws[k].n == 0) return ALOAM_ERR_EMPTY_CLOUD;
+      if (raws[k].n > c->max_points) return ALOAM_ERR_CAPACITY;
+      if (device_resident && raws[k].stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
+      if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+    }
+  } else {
+    // the whole schedule is checked against the lanes' state before anything changes; lanes >= nb are idle all call
+    for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { running[l] = l < nb && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; }
+    for (size_t i = 0; i < (size_t)n_scans * nb; ++i)
+      if (ops[i] < ALOAM_LANE_IDLE || ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
+    for (int k = 0; k < n_scans; ++k) {
+      int stride = 0;
+      for (int l = 0; l < nb; ++l) {
+        const int op = ops[(size_t)k * nb + l];
+        const aloam_cloud_view& v = raws[(size_t)k * nb + l];
+        if (op == ALOAM_LANE_IDLE) { running[l] = false; continue; }   // its view is not read
+        int rc = check_view(v); if (rc) return rc;
+        if (v.n > 0) {
+          if (device_resident && v.stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
+          if (stride && v.stride_floats != stride) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+          stride = v.stride_floats;
+        }
+        // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
+        if (op == ALOAM_LANE_SCAN && (!running[l] || mapped[l] != (map_poses != nullptr))) return ALOAM_ERR_STATE;
+        if (op == ALOAM_LANE_START) { running[l] = true; mapped[l] = map_poses != nullptr; }
+        if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
+        if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
+      }
+    }
   }
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  if (run_err) { aloam_reset_odometry(c); return run_err; }
   if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
+  if (ops) c->lanes_mode = true;
   StreamGuard guard(c);
   cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
@@ -534,22 +582,37 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   // Waiting on an event that was never recorded, or whose work finished in an earlier call, is a no-op -- so the
   // per-scan waits below need no "first iterations" special cases.
   for (cudaStream_t s : {c->s_h2d, c->s_exa, c->s_ext, c->s_idx, c->s_map}) STREAM_TRY(cudaStreamWaitEvent(s, c->ev0, 0));
-  const float* d_raw[ALOAM_MAX_BATCH];
+  const float* d_raw[ALOAM_MAX_BATCH];      // per record
   int ns[ALOAM_MAX_BATCH];
+  int act[ALOAM_MAX_BATCH], scanning[ALOAM_MAX_BATCH], starting[ALOAM_MAX_BATCH];   // lanes of the step: all, registering, initialising
+  int last_op[ALOAM_MAX_BATCH] = {};        // lane schedule: the last non-idle op of every lane in this call
+  int issued = 0;
   for (int k = 0; k < n_scans; ++k) {
+    const int* op = ops ? ops + (size_t)k * nb : nullptr;
+    int na = 0;
+    for (int l = 0; l < nb; ++l)
+      if (!op || op[l] != ALOAM_LANE_IDLE) { act[na++] = l; if (op) last_op[l] = op[l]; }
+    if (na == 0) continue;                  // an all-idle step: nothing to run, the frame does not advance
     const int f = c->frame;                 // global frame number of this step
-    const int b = k & 1;                    // raw / ring-major double buffer
+    const int b = issued++ & 1;             // raw / ring-major double buffer
     const int cur = f % kFeatSlots, last = (f + kFeatSlots - 1) % kFeatSlots;
     const aloam_cloud_view* rv = raws + (size_t)k * nb;
+    // a lane's first scan only initialises (laserOdometry.cpp:267-271): every lane at the context's first step, or a START
+    int n_scan = 0, n_start = 0;
+    for (int i = 0; i < na; ++i) {
+      const bool start = op ? op[act[i]] == ALOAM_LANE_START : f == 0;
+      if (start) starting[n_start++] = act[i]; else scanning[n_scan++] = act[i];
+    }
     int nmax = 0;
-    for (int l = 0; l < nb; ++l) { ns[l] = rv[l].n; nmax = std::max(nmax, rv[l].n); }
+    for (int i = 0; i < na; ++i) { ns[i] = rv[act[i]].n; nmax = std::max(nmax, ns[i]); }
     if (device_resident) {
-      for (int l = 0; l < nb; ++l) d_raw[l] = rv[l].data;
+      for (int i = 0; i < na; ++i) d_raw[i] = rv[act[i]].data;
     } else {
       STREAM_TRY(cudaStreamWaitEvent(c->s_h2d, c->ev_rawfree[b], 0));   // stage A of scan k-2 has consumed the buffers
-      for (int l = 0; l < nb; ++l) {
+      for (int i = 0; i < na; ++i) {
+        const int l = act[i];
         STREAM_TRY(cudaMemcpyAsync(c->lanes[l].d_raw[b], rv[l].data, (size_t)rv[l].n * rv[l].stride_floats * 4, cudaMemcpyHostToDevice, c->s_h2d));
-        d_raw[l] = c->lanes[l].d_raw[b];
+        d_raw[i] = c->lanes[l].d_raw[b];
       }
       STREAM_TRY(cudaEventRecord(c->ev_h2d[b], c->s_h2d));
       STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_h2d[b], 0));
@@ -557,8 +620,12 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     // ---- stage A (ring binning) on s_exa: needs full[b] free, i.e. stage B of scan k-2 done
     STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_b[b], 0));
     c->stream = c->s_exa;
+    // a START re-arms the lane's ScanScalars slot of this scan: k_ring_scan arms it only for a lane that ran the step before
+    if (op)
+      for (int i = 0; i < n_start; ++i)
+        STREAM_TRY(cudaMemcpyAsync(c->lanes[starting[i]].d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->s_exa));
     int sc_slot = 0;
-    int rc = run_features_a(c, nb, d_raw, ns, device_resident ? 4 : rv[0].stride_floats, b, &sc_slot, c->d_scan_nfull + (size_t)k * nb);
+    int rc = run_features_a(c, na, d_raw, ns, device_resident ? 4 : rv[act[0]].stride_floats, b, &sc_slot, c->d_scan_nfull + (size_t)k * nb, act);
     if (rc) return fail(rc);
     if (!device_resident) STREAM_TRY(cudaEventRecord(c->ev_rawfree[b], c->s_exa));
     STREAM_TRY(cudaEventRecord(c->ev_a[b], c->s_exa));
@@ -567,7 +634,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     c->stream = c->s_ext;
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_a[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_cmp[b], 0));
-    rc = run_features_b1(c, nb, b, sc_slot);
+    rc = run_features_b1(c, na, b, sc_slot, act);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_b[b], c->s_ext));
     // ---- stage C on s_idx: ring-ordered compaction into feat[f % kFeatSlots] -- that slot was last read by the odometry
@@ -577,11 +644,11 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_b[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_odo[(f + 1) % kFeatSlots], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the scan-to-map stage of frame f - kFeatSlots has read this slot
-    rc = run_features_b2(c, nb, b, cur, false);
+    rc = run_features_b2(c, na, b, cur, false, act);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
     STREAM_TRY(cudaEventRecord(c->ev_feat[cur], c->s_idx));
-    run_grid_build(c, nb, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+    run_grid_build(c, na, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points), act);
     STREAM_TRY(cudaEventRecord(c->ev_idx[cur], c->s_idx));
     c->stream = s_main;
     // ---- association + LM on the main stream: this scan's sharp / flat points, the previous scan's clouds + index
@@ -589,8 +656,15 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_idx[last], 0));
     // the last solve of the scan writes the integrated world pose into its slot of d_poses (no copy on the critical chain)
     double* slots = c->d_poses + (size_t)k * nb * 7;
-    if (f > 0) run_register(c, nb, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots);
-    else for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemcpyAsync(slots + (size_t)l * 7, c->lanes[l].d_world, 56, cudaMemcpyDeviceToDevice, s_main));
+    for (int i = 0; i < n_start; ++i) {
+      Lane& L = c->lanes[starting[i]];
+      if (op) {   // a new trajectory of the lane schedule: warm start and world pose back to the identity, in stream order
+        STREAM_TRY(cudaMemcpyAsync(L.d_pose, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
+        STREAM_TRY(cudaMemcpyAsync(L.d_world, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
+      }
+      STREAM_TRY(cudaMemcpyAsync(slots + (size_t)starting[i] * 7, L.d_world, 56, cudaMemcpyDeviceToDevice, s_main));
+    }
+    if (n_scan > 0) run_register(c, n_scan, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots, nullptr, scanning);
     STREAM_TRY(cudaEventRecord(c->ev_odo[cur], s_main));
     if (map_poses) {
       // ---- scan-to-map on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose go
@@ -599,13 +673,16 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
       //      One frame covers every trajectory: each launch of it serves all lanes, each lane with its own cube store.
       STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
       c->stream = c->s_map;
+      //      A START lane's frame begins by resetting its cube store (k_mapper_begin).
       MapperIn in[ALOAM_MAX_BATCH];
-      for (int l = 0; l < nb; ++l) {
+      for (int i = 0; i < na; ++i) {
+        const int l = act[i];
         const FeatBuf& fc = c->lanes[l].feat[cur];
         const size_t slot = ((size_t)k * nb + l) * 7;
-        in[l] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot};
+        in[i] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
+                         op && op[l] == ALOAM_LANE_START};
       }
-      rc = mapper_step_device(c, nb, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+      rc = mapper_step_device(c, na, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
       if (rc) return fail(rc);
       STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
       c->stream = s_main;
@@ -638,14 +715,22 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   for (int l = 0; l < nb; ++l)
     for (int b = 0; b < 3; ++b)
       if (c->h_sc[3 * l + b].error) return fail(c->h_sc[3 * l + b].error);
-  for (size_t i = 0; i < total; ++i)
-    if (c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
+  for (size_t i = 0; i < total; ++i)   // (an idle entry has no scan)
+    if (!(ops && ops[i] == ALOAM_LANE_IDLE) && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
   std::memcpy(poses, c->h_poses, total * 56);
   if (map_poses) std::memcpy(map_poses, c->h_poses + (size_t)kMaxStreamScans * 7, total * 56);
+  if (ops) {
+    for (size_t i = 0; i < total; ++i)
+      if (ops[i] == ALOAM_LANE_IDLE)
+        for (int j = 0; j < 7; ++j) { poses[i * 7 + j] = NAN; if (map_poses) map_poses[i * 7 + j] = NAN; }
+    for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; }
+  }
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (stats_last) {
     for (int l = 0; l < nb; ++l) {
-      if (c->frame <= 1) { std::memset(&stats_last[l], 0, sizeof(aloam_stats)); stats_last[l].flags = ALOAM_FLAG_INITIALISED_ONLY; stats_last[l].ms_total = ms; }
+      const bool init_only = ops ? last_op[l] == ALOAM_LANE_START : c->frame <= 1;
+      if (ops && last_op[l] == ALOAM_LANE_IDLE) std::memset(&stats_last[l], 0, sizeof(aloam_stats));   // idle all call
+      else if (init_only) { std::memset(&stats_last[l], 0, sizeof(aloam_stats)); stats_last[l].flags = ALOAM_FLAG_INITIALISED_ONLY; stats_last[l].ms_total = ms; }
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
@@ -678,6 +763,13 @@ int aloam_scan_stream_mapped_batch(aloam_ctx* c, const aloam_cloud_view* raws, i
   if (!map_poses) return ALOAM_ERR_INVALID_ARG;
   if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   return scan_stream_impl(c, raws, n_scans, batch, device_resident, odom_poses, stats_last, map_poses);
+}
+
+int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch, int device_resident,
+                            double* odom_poses, double* map_poses, aloam_stats* stats_last) {
+  if (!lane_ops) return ALOAM_ERR_INVALID_ARG;
+  if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  return scan_stream_impl(c, raws, n_scans, batch, device_resident, odom_poses, stats_last, map_poses, lane_ops);
 }
 
 // ------------------------------------------------------------------------------------------------ fine-grained

@@ -30,7 +30,8 @@ struct MapLaneIO {
   double* pose;
 };
 // one lane's input to a mapper frame (cubemap.cu): the scan's less-sharp / less-flat clouds and their sizes, its odometry pose
-// and the slot of the refined pose, all device pointers
+// and the slot of the refined pose, all device pointers; the lane whose cube store the frame runs on, and whether that store
+// starts a fresh trajectory with this frame (reset on the device by k_mapper_begin)
 struct MapperIn {
   const Pt4* corner;
   const int* nc;
@@ -38,6 +39,8 @@ struct MapperIn {
   const int* ns;
   const double* odom7;
   double* out7;
+  int lane;
+  int fresh;
 };
 }  // namespace aloam
 
@@ -118,6 +121,8 @@ struct aloam_ctx {
   int* d_scan_nfull = nullptr;     // [kMaxStreamScans] ring-major cloud size of every (scan, lane) of a stream call
   double *d_out28 = nullptr, *d_packed = nullptr;
   double* d_api_pose = nullptr;    // [8] pose of the per-stage entry points (odometry_register, solve, ...): not the warm start of the fused pipeline
+  double* d_ident = nullptr;       // [7] identity pose, the source of a lane's odometry reset inside aloam_scan_stream_lanes
+  ScanScalars* d_sc_init = nullptr;   // [1] an armed ScanScalars slot (what k_ring_scan arms for the next scan), same use
   int* d_err = nullptr;
   Pt4* d_query = nullptr;
   int* d_knn_idx = nullptr;
@@ -179,6 +184,11 @@ struct aloam_ctx {
   int cur = 0;            // fused pipeline: feat[] slot of the most recent scan
   bool have_last = false; // API path: set_last called
   int last_n_full = 0;
+  // aloam_scan_stream_lanes: once used, the lockstep calls are refused until aloam_reset_odometry, which clears all of this.
+  // A lane runs from its START to the step before its next IDLE; `lane_mapped` is the mode of the call that started it.
+  bool lanes_mode = false;
+  bool lane_running[ALOAM_MAX_BATCH] = {};
+  bool lane_mapped[ALOAM_MAX_BATCH] = {};
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
   std::vector<cudaStream_t> streams;

@@ -152,10 +152,37 @@ __device__ void rotate_line(MapperState* S, int axis, bool towards_high, int u, 
   }
 }
 
+// the state of a fresh trajectory (laserMapping.cpp:74-117): identity T_wmap_wodom, centre cube (10, 10, 5), every slab free
+// and no cube holding one.  Run by all threads of one CTA.  It leaves alone the word of the call (err_acc) and every field the
+// stack filter writes while k_mapper_begin runs beside it (stack_counts, err, in_counts): between frames `err` is 0 already
+// (k_mapper_finish), and reset_lane zeroes the whole state before it runs this.
+__device__ void mapper_fresh_state(MapperState* S) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int i = tid; i < NCUBE; i += nt) { S->slab_of[0][i] = -1; S->slab_of[1][i] = -1; }
+  for (int i = tid; i < kPool; i += nt) { S->cnt[0][i] = 0; S->cnt[1][i] = 0; S->free_list[0][i] = i; S->free_list[1][i] = i; }
+  for (int i = tid; i < kMaxValid; i += nt) S->valid[i] = 0;
+  for (int i = tid; i < 2 * (kMaxValid + 1); i += nt) S->sub_off[i / (kMaxValid + 1)][i % (kMaxValid + 1)] = 0;
+  if (tid == 0) {
+    for (int k = 0; k < 4; ++k) { S->q_wmap_wodom[k] = k == 3 ? 1.0 : 0.0; S->q_wodom[k] = 0.0; }
+    for (int k = 0; k < 3; ++k) { S->t_wmap_wodom[k] = 0.0; S->t_wodom[k] = 0.0; S->ctr[k] = 0; }
+    for (int k = 0; k < 7; ++k) S->x[k] = 0.0;
+    S->cen[0] = 10; S->cen[1] = 10; S->cen[2] = 5;
+    S->n_valid = 0; S->n_sub[0] = 0; S->n_sub[1] = 0;
+    S->flags = 0; S->frame_err = 0; S->frames = 0; S->zero = 0; S->sink = 0;
+    S->free_top = 0; S->free_top2 = 0;
+  }
+}
+// grid (1): the host-side reset of one lane (reset_lane)
+__global__ void __launch_bounds__(1024) k_mapper_reset(MapperState* S) { mapper_fresh_state(S); }
+
 // transformAssociateToMap (:142-146), centre cube + shift (:314-509), valid cubes (:511-529), gather offsets
-__device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub) {
+__device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub, bool fresh) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
+  if (fresh) {   // the lane starts a new trajectory with this frame: no extra launch, in order on the mapper stream
+    mapper_fresh_state(S);
+    __syncthreads();
+  }
   __shared__ int s_ctr[3], s_cen[3];
   const int tid = threadIdx.x;
   if (tid == 0) {
@@ -227,10 +254,10 @@ __device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* 
     S->n_sub[ty] = off;
   }
 }
-// grid (1, 1, lanes)
-__global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub) {
+// grid (1, 1, lanes); bit l of `fresh`: record l starts a new trajectory with this frame, its state is reset first
+__global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub, unsigned fresh) {
   const MapperLane& a = B.a[blockIdx.z];
-  mapper_begin_body(a.S, a.odom7, max_sub);
+  mapper_begin_body(a.S, a.odom7, max_sub, (fresh >> blockIdx.z) & 1u);
 }
 
 
@@ -447,17 +474,12 @@ size_t refilter_bound(const Mapper* m, const aloam_ctx* c) {
   return std::max((size_t)75 * (m->cap[0] + m->cap[1]), (size_t)2 * c->max_points);
 }
 
-// the state of a fresh trajectory: identity T_wmap_wodom, centre cube (10, 10, 5), no slabs in use (laserMapping.cpp:74-117)
+// the state of a fresh trajectory (mapper_fresh_state, the routine k_mapper_begin runs for a lane that starts one), with the
+// fields that routine leaves alone zeroed first
 int reset_lane(aloam_ctx* c, Mapper* m) {
-  MapperState* h = m->h_state;
-  std::memset(h, 0, sizeof(*h));
-  h->q_wmap_wodom[3] = 1.0;
-  h->cen[0] = 10; h->cen[1] = 10; h->cen[2] = 5;
-  for (int t = 0; t < 2; ++t) {
-    for (int i = 0; i < NCUBE; ++i) h->slab_of[t][i] = -1;
-    for (int i = 0; i < kPool; ++i) h->free_list[t][i] = i;
-  }
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state, h, sizeof(*h), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
+  LAUNCH(c, KID_CUBES, k_mapper_reset, 1, 1024, 0, m->d_state);
+  CUDA_CHECK_RET(cudaGetLastError());
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   return ALOAM_OK;
 }
@@ -501,12 +523,13 @@ int ensure_mapper(aloam_ctx* c, int lane) {
 // One frame of alaserMapping's process() for nb trajectories ("lanes") on the current stream, entirely on the device: every launch
 // covers all lanes, lane l in blockIdx.z, and each lane has its own cube store, stack filter buffers and registration set, so
 // lane l computes exactly what a frame of lane l alone computes.  in[l]: the lane's less-sharp / less-flat clouds and their
-// sizes, its odometry pose (7 doubles) and its output pose slot, all device pointers; n_upper_* bound the cloud sizes of every
-// lane.  Lane 0 registers with the buffers of mapping.cu that it shares with the host API.  A sharded job maps one lane.
+// sizes, its odometry pose (7 doubles) and its output pose slot, all device pointers, the lane whose cube store record l
+// runs on and whether that store starts a fresh trajectory; n_upper_* bound the cloud sizes of every lane.  Lane 0 registers
+// with the buffers of mapping.cu that it shares with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && c->shard_count > 1)) return ALOAM_ERR_STATE;
-  int rc;
-  for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, l); if (rc) return rc; }
+  int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's auxiliary stream carries the stack filters of every lane
+  for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
   if (!c->map_ready) {
     aloam_cloud_view none{nullptr, 0, 4};
     rc = aloam_map_upload_impl(c, none, none); if (rc) return rc;
@@ -517,18 +540,21 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   SegFilter stack_f[ALOAM_MAX_BATCH], cube_f[ALOAM_MAX_BATCH];
   SegBuffers* bufs[ALOAM_MAX_BATCH];
   Batch<GridArgs> gs = {};
+  unsigned fresh = 0;   // records whose store starts a new trajectory: reset by k_mapper_begin
   // index bits of a 50 m cube at the finer leaf: (50 / leaf + 3)^3 voxels at most (PCL itself gives up beyond 2^31)
   int cube_bits = 1;
   { const double side = std::floor(50.0 / std::min(c->cfg.line_res, c->cfg.plane_res)) + 3.0; const double cells = side * side * side;
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
-  for (int l = 0; l < nb; ++l) {
-    Mapper* m = static_cast<Mapper*>(c->mapper[l]);
+  for (int l = 0; l < nb; ++l) {   // record l runs on the store of lane in[l].lane
+    const int lane = in[l].lane;
+    Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
     MapperState* S = m->d_state;
-    const MapReg reg = l == 0 ? ctx_map_reg(c) : m->reg;
-    Pt4* const stack_corner = l == 0 ? c->d_stack_corner : m->d_stack[0];
-    Pt4* const stack_surf = l == 0 ? c->d_stack_surf : m->d_stack[1];
+    const MapReg reg = lane == 0 ? ctx_map_reg(c) : m->reg;
+    Pt4* const stack_corner = lane == 0 ? c->d_stack_corner : m->d_stack[0];
+    Pt4* const stack_surf = lane == 0 ? c->d_stack_surf : m->d_stack[1];
     B.a[l] = MapperLane{S, in[l].odom7, in[l].out7, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, {m->d_sub[0], m->d_sub[1]}, {in[l].corner, in[l].surf},
                         {in[l].nc, in[l].ns}, {stack_corner, stack_surf}, m->d_world, m->d_cube, m->buf.segs, m->buf.n_seg};
+    if (in[l].fresh) fresh |= 1u << l;
     io[l] = MapLaneIO{reg, {m->d_sub[0], m->d_sub[1]}, {stack_corner, stack_surf}, S->stack_counts, S->x};
     gs.a[l] = GridArgs{reg.corner.grid, m->d_sub[0], &S->n_sub[0], reg.surf.grid, m->d_sub[1], &S->n_sub[1]};
     stack_f[l] = seg_filter(m->buf, 31, &S->err);
@@ -551,7 +577,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     c->stream = main_stream;
     CUDA_CHECK_RET(e);
   }
-  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub);
+  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub, fresh);
   launch_ex(c, KID_CUBES, k_mapper_gather, dim3(kMaxValid, 2, nb), dim3(256), 0, 1, true, B);
   if (c->shard_count > 1) {
     // A rank of a sharded job keeps the WHOLE cube store (the insertions below are replicated: the refined pose is bit-identical
@@ -622,7 +648,7 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   for (int k = 0; k < 4; ++k) c->pin->mapper_pose_in[k] = q_wodom_curr[k];
   for (int k = 0; k < 3; ++k) c->pin->mapper_pose_in[4 + k] = t_wodom_curr[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->pin->mapper_pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  const MapperIn one{m->d_in[0], &m->d_state->in_counts[0], m->d_in[1], &m->d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7};
+  const MapperIn one{m->d_in[0], &m->d_state->in_counts[0], m->d_in[1], &m->d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7, 0, 0};
   rc = mapper_step_device(c, 1, &one, corner_last.n, surf_last.n);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));

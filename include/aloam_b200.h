@@ -66,7 +66,8 @@ typedef struct aloam_config {
   int max_points;        /* capacity of one raw scan (reference: 400000 static arrays, scanRegistration.cpp:66-69) */
   int max_map_points;    /* capacity of the uploaded submap, per cloud type (0 = mapping not used); at most 2^30, larger
                             values are rejected by aloam_create with ALOAM_ERR_INVALID_ARG */
-  int max_batch;         /* trajectories a context can advance in lockstep (aloam_scan_stream_batch); 1..ALOAM_MAX_BATCH, default 1 */
+  int max_batch;         /* trajectories a context can advance in lockstep (aloam_scan_stream_batch), or lanes of
+                            aloam_scan_stream_lanes; 1..ALOAM_MAX_BATCH, default 1 */
   int distortion;        /* 0 (reference build) or 1: #define DISTORTION of laserOdometry.cpp:59 -- per-point interpolation ratio
                             s = (intensity - int(intensity)) / SCAN_PERIOD in TransformToStart (:113-118) and in the
                             residual blocks (:376-379, 470-473; slerp inside the functors, lidarFactor.hpp:27-33) */
@@ -175,7 +176,39 @@ int aloam_scan_stream_mapped(aloam_ctx* ctx, const aloam_cloud_view* raws, int n
  * resets the odometry, as aloam_scan_stream does. */
 int aloam_scan_stream_mapped_batch(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident,
                                    double* odom_poses, double* map_poses, aloam_stats* stats_last);
-int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" clouds (all trajectories) */
+
+/* Lane-scheduled streams: the `batch` lanes of a context run trajectories that start and end independently, so a server
+ * replaying recordings of different lengths refills a lane as soon as its trajectory ends instead of waiting for the longest
+ * one of a group.  lane_ops (n_scans x batch ints, scan-major like raws / odom_poses / map_poses) says per step and lane:
+ *   ALOAM_LANE_START  the first scan of a new trajectory: the lane's odometry (and, mapped, its cube store) is reset first;
+ *   ALOAM_LANE_SCAN   the next scan of the trajectory the lane runs;
+ *   ALOAM_LANE_IDLE   no scan: the lane's trajectory, if any, has ended (its view is not read; its pose rows are NaN).
+ * Lifecycle: START, then SCAN at every step, then IDLE until the next START (a START may also directly follow a SCAN).  An
+ * IDLE step ends the trajectory: a lane cannot pause.  Lanes batch .. cfg.max_batch-1 are IDLE at every step of the call.
+ * A START scan only initialises (laserOdometry.cpp:267-271): its odometry pose is the identity and, mapped, it is the first
+ * mapper frame on a freshly reset cube store.
+ * map_poses == NULL: odometry only, as aloam_scan_stream_batch; otherwise scan-to-map too, as aloam_scan_stream_mapped_batch
+ * (needs cfg.max_map_points > 0).  A trajectory keeps the mode of the call that started it.
+ * Results: for every trajectory, its odometry poses, its map poses and its final cube store are bit-identical to running it
+ * alone through aloam_scan_stream (aloam_scan_stream_mapped) on a fresh context with the same config, whatever its lane,
+ * its start step and the other lanes' schedules.  Each step packs its non-idle lanes into one set of launches; a step where
+ * every lane is IDLE issues nothing.  Lane state carries over between calls, so a trajectory may span several calls.
+ * stats_last[b] (`batch` entries, or NULL): the odometry stats of lane b's last non-idle step of this call,
+ * ALOAM_FLAG_INITIALISED_ONLY when that step was a START, all zero when the lane was idle all call.
+ * Errors before any state changes: ALOAM_ERR_INVALID_ARG for an op outside {0, 1, 2}, batch > cfg.max_batch or map_poses
+ * without cfg.max_map_points; ALOAM_ERR_STATE for a SCAN to a lane that is not running at that step (or that was started in
+ * the other mode), and after aloam_comm_init with world > 1.  Any other failure (an empty or oversized scan included) drains
+ * the streams and resets the odometry, after which no lane is running; ALOAM_ERR_CAPACITY keeps its meaning of
+ * aloam_scan_stream_mapped_batch (pose arrays filled, lanes go on).
+ * Once a context has run this call, aloam_scan_to_pose*, aloam_scan_stream, _batch, _mapped and _mapped_batch (the calls
+ * driven by the context's shared frame counter) return ALOAM_ERR_STATE until aloam_reset_odometry, which also ends every lane. */
+#define ALOAM_LANE_IDLE 0
+#define ALOAM_LANE_SCAN 1
+#define ALOAM_LANE_START 2
+int aloam_scan_stream_lanes(aloam_ctx* ctx, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch,
+                            int device_resident, double* odom_poses, double* map_poses, aloam_stats* stats_last);
+int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" clouds (all trajectories); ends every lane of
+                                             aloam_scan_stream_lanes and allows the lockstep calls again */
 
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
  * interpolation ratio, then carry it to the sweep end with (q_last_curr, t_last_curr); the intensity keeps only the scan id.
