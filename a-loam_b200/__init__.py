@@ -139,6 +139,16 @@ def _dp(a):
     return a.ctypes.data_as(C.POINTER(C.c_double))
 
 
+def _views(ptrs, counts, stride):
+    """CloudView array over raw scans given as addresses and point counts, in the order of the flattened (scan-major) arrays"""
+    ptrs = np.asarray(ptrs, np.uint64).ravel()
+    counts = np.asarray(counts, np.int64).ravel()
+    views = (CloudView * len(ptrs))()
+    for i in range(len(ptrs)):
+        views[i] = CloudView(C.cast(C.c_void_p(int(ptrs[i])), C.POINTER(C.c_float)), int(counts[i]), stride)
+    return views
+
+
 def default_config(n_scans):
     cfg = Config()
     lib().aloam_default_config(C.byref(cfg), n_scans)
@@ -347,38 +357,27 @@ class Aloam:
     def scan_stream(self, ptrs, counts, device_resident, stride=4):
         """pipelined scan_to_pose over a sequence: ptrs = host (or device) addresses of the raw scans; returns (n, 7) poses"""
         n = len(ptrs)
-        views = (CloudView * n)()
-        for i in range(n):
-            views[i] = CloudView(C.cast(C.c_void_p(int(ptrs[i])), C.POINTER(C.c_float)), int(counts[i]), stride)
         poses = np.zeros((n, 7))
         st = Stats()
-        _check(lib().aloam_scan_stream(self._h, views, n, int(device_resident), _dp(poses), C.byref(st)))
+        _check(lib().aloam_scan_stream(self._h, _views(ptrs, counts, stride), n, int(device_resident), _dp(poses), C.byref(st)))
         return poses, st
 
     def scan_stream_mapped(self, ptrs, counts, device_resident, stride=4):
         """aloam_scan_stream_mapped: odometry + scan-to-map of every scan on the device; returns (odom poses, map poses), (n, 7) each"""
         n = len(ptrs)
-        views = (CloudView * n)()
-        for i in range(n):
-            views[i] = CloudView(C.cast(C.c_void_p(int(ptrs[i])), C.POINTER(C.c_float)), int(counts[i]), stride)
         odom = np.zeros((n, 7)); mapped = np.zeros((n, 7))
         st = Stats()
-        _check(lib().aloam_scan_stream_mapped(self._h, views, n, int(device_resident), _dp(odom), _dp(mapped), C.byref(st)))
+        _check(lib().aloam_scan_stream_mapped(self._h, _views(ptrs, counts, stride), n, int(device_resident), _dp(odom), _dp(mapped), C.byref(st)))
         return odom, mapped
 
     def scan_stream_batch(self, ptrs, counts, device_resident, stride=4):
         """aloam_scan_stream_batch: ptrs / counts are (n_scans, batch) arrays of addresses / point counts (scan-major);
         returns poses (n_scans, batch, 7).  Every kernel launch covers all `batch` trajectories of a step."""
         ptrs = np.asarray(ptrs, np.uint64)
-        counts = np.asarray(counts, np.int64)
         n, b = ptrs.shape
-        views = (CloudView * (n * b))()
-        for k in range(n):
-            for j in range(b):
-                views[k * b + j] = CloudView(C.cast(C.c_void_p(int(ptrs[k, j])), C.POINTER(C.c_float)), int(counts[k, j]), stride)
         poses = np.zeros((n, b, 7))
         st = (Stats * b)()
-        _check(lib().aloam_scan_stream_batch(self._h, views, n, b, int(device_resident), _dp(poses), st))
+        _check(lib().aloam_scan_stream_batch(self._h, _views(ptrs, counts, stride), n, b, int(device_resident), _dp(poses), st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return poses
 
@@ -386,15 +385,10 @@ class Aloam:
         """aloam_scan_stream_mapped_batch: ptrs / counts are (n_scans, batch) arrays as for scan_stream_batch; returns
         (odom poses, map poses), (n_scans, batch, 7) each.  Every lane is bit-identical to its solo scan_stream_mapped run."""
         ptrs = np.asarray(ptrs, np.uint64)
-        counts = np.asarray(counts, np.int64)
         n, b = ptrs.shape
-        views = (CloudView * (n * b))()
-        for k in range(n):
-            for j in range(b):
-                views[k * b + j] = CloudView(C.cast(C.c_void_p(int(ptrs[k, j])), C.POINTER(C.c_float)), int(counts[k, j]), stride)
         odom = np.zeros((n, b, 7)); mapped = np.zeros((n, b, 7))
         st = (Stats * b)()
-        _check(lib().aloam_scan_stream_mapped_batch(self._h, views, n, b, int(device_resident), _dp(odom), _dp(mapped), st))
+        _check(lib().aloam_scan_stream_mapped_batch(self._h, _views(ptrs, counts, stride), n, b, int(device_resident), _dp(odom), _dp(mapped), st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return odom, mapped
 
@@ -408,14 +402,10 @@ class Aloam:
         n, b = ptrs.shape
         if counts.shape != (n, b) or ops.shape != (n, b):
             raise ValueError("ptrs, counts and ops are (n_scans, batch) arrays")
-        views = (CloudView * (n * b))()
-        for k in range(n):
-            for j in range(b):
-                views[k * b + j] = CloudView(C.cast(C.c_void_p(int(ptrs[k, j])), C.POINTER(C.c_float)), int(counts[k, j]), stride)
         odom = np.zeros((n, b, 7))
         out = np.zeros((n, b, 7)) if mapped else None
         st = (Stats * b)()
-        _check(lib().aloam_scan_stream_lanes(self._h, views, ops.ctypes.data_as(C.POINTER(C.c_int)), n, b, int(device_resident), _dp(odom),
+        _check(lib().aloam_scan_stream_lanes(self._h, _views(ptrs, counts, stride), ops.ctypes.data_as(C.POINTER(C.c_int)), n, b, int(device_resident), _dp(odom),
                                              _dp(out) if mapped else None, st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return odom, out

@@ -173,24 +173,23 @@ namespace {
 // Feature extraction is issued in two halves so that the pipelined stream call can run them on different streams:
 //   A  ring binning   (k_classify, k_ring_scan, k_scatter)  raw scan -> ring-major cloud `full[buf]`, ring_start[buf]
 //   B  per-ring work  (k_ring_features, k_compact)          full[buf] -> the four feature clouds of feat[slot]
-// Every launch covers nb records; record l is the trajectory of lane pl[l] (pl == null: lane l).  Per-record arrays (d_raw, n)
-// are indexed by record, per-lane ones by lane.  `sc_slot` (returned by A, consumed by B) is the ScanScalars parity slot of
-// this scan; nfull_out (device, one int per lane, may be null) receives the ring-major cloud sizes.
-inline int phys(const int* pl, int l) { return pl ? pl[l] : l; }
-int run_features_a(aloam_ctx* c, int nb, const float* const* d_raw, const int* n, int stride, int buf, int* sc_slot, int* nfull_out,
-                   const int* pl = nullptr) {
+// Every launch covers nb records; record l is the trajectory of lane pl[l] (the single-trajectory paths pass kLane0).
+// Per-record arrays (d_raw, n) are indexed by record, per-lane ones by lane.  `sc_slot` (returned by A, consumed by B) is the
+// ScanScalars parity slot of this scan; nfull_out (device, one int per lane, may be null) receives the ring-major cloud sizes.
+constexpr int kLane0[1] = {0};
+int run_features_a(aloam_ctx* c, int nb, const int* pl, const float* const* d_raw, const int* n, int stride, int buf, int* sc_slot, int* nfull_out) {
   int nmax = 0;
   for (int l = 0; l < nb; ++l) nmax = std::max(nmax, n[l]);
   const int blocks = (nmax + 1023) / 1024;
   const float thres = c->cfg.minimum_range;
   Batch<ClassifyArgs> ca = {}; Batch<RingScanArgs> ra = {}; Batch<ScatterArgs> sa = {};
   for (int l = 0; l < nb; ++l) {
-    Lane& L = c->lanes[phys(pl, l)];
+    Lane& L = c->lanes[pl[l]];
     ScanScalars* sc = L.d_sc + c->parity;
     ScanScalars* sc_next = L.d_sc + (c->parity + 1) % 3;
     ca.a[l] = ClassifyArgs{d_raw[l], n[l], stride, L.d_ring, L.d_hist, sc};
     ra.a[l] = RingScanArgs{d_raw[l], stride, (n[l] + 1023) / 1024, L.d_hist, L.d_offsets, L.d_ring_start[buf], L.d_scan_start, L.d_scan_end, sc, sc_next,
-                           nfull_out ? nfull_out + phys(pl, l) : nullptr};
+                           nfull_out ? nfull_out + pl[l] : nullptr};
     sa.a[l] = ScatterArgs{d_raw[l], n[l], stride, L.d_ring, L.d_offsets, sc, L.d_full[buf]};
   }
   LAUNCH(c, KID_CLASSIFY, k_classify, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
@@ -202,10 +201,10 @@ int run_features_a(aloam_ctx* c, int nb, const float* const* d_raw, const int* n
   return ALOAM_OK;
 }
 // B1: per-ring kernel -> staging set `buf` ; B2: ring-ordered concatenation of the staging set into feat[slot]
-int run_features_b1(aloam_ctx* c, int nb, int buf, int sc_slot, const int* pl = nullptr) {
+int run_features_b1(aloam_ctx* c, int nb, const int* pl, int buf, int sc_slot) {
   Batch<RingFeatArgs> fa = {};
   for (int l = 0; l < nb; ++l) {
-    const int lane = phys(pl, l);
+    const int lane = pl[l];
     Lane& L = c->lanes[lane];
     fa.a[l] = RingFeatArgs{L.d_full[buf], L.d_ring_start[buf], L.st_sharp[buf], L.st_less_sharp[buf], L.st_flat[buf], L.st_less_flat[buf], L.st_counts[buf],
                            lane == 0 ? c->d_curv : nullptr, lane == 0 ? c->d_label : nullptr, L.d_sc + sc_slot};
@@ -216,10 +215,10 @@ int run_features_b1(aloam_ctx* c, int nb, int buf, int sc_slot, const int* pl = 
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
-int run_features_b2(aloam_ctx* c, int nb, int buf, int slot, bool pdl, const int* pl = nullptr) {
+int run_features_b2(aloam_ctx* c, int nb, const int* pl, int buf, int slot, bool pdl) {
   Batch<CompactArgs> ka = {};
   for (int l = 0; l < nb; ++l) {
-    Lane& L = c->lanes[phys(pl, l)];
+    Lane& L = c->lanes[pl[l]];
     FeatBuf& out = L.feat[slot];
     ka.a[l] = CompactArgs{L.st_sharp[buf], L.st_less_sharp[buf], L.st_flat[buf], L.st_less_flat[buf], L.st_counts[buf], out.sharp, out.less_sharp, out.flat,
                           out.less_flat, out.counts, out.rs_ls, out.rs_lf};
@@ -228,21 +227,21 @@ int run_features_b2(aloam_ctx* c, int nb, int buf, int slot, bool pdl, const int
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
-int run_features(aloam_ctx* c, int nb, const float* const* d_raw, const int* n, int stride, int slot) {
+int run_features(aloam_ctx* c, const float* d_raw, int n, int stride, int slot) {
   int sc = 0;
-  int rc = run_features_a(c, nb, d_raw, n, stride, 0, &sc, nullptr);
+  int rc = run_features_a(c, 1, kLane0, &d_raw, &n, stride, 0, &sc, nullptr);
   if (rc) return rc;
-  rc = run_features_b1(c, nb, 0, sc);
+  rc = run_features_b1(c, 1, kLane0, 0, sc);
   if (rc) return rc;
-  return run_features_b2(c, nb, 0, slot, true);
+  return run_features_b2(c, 1, kLane0, 0, slot, true);
 }
 
 // index over the two "last" clouds of feat[slot]: count -> scan -> fill (n_ls / n_lf = host upper bounds on the cloud sizes)
-void run_grid_build(aloam_ctx* c, int nb, int slot, int n_ls, int n_lf, const int* pl = nullptr) {
+void run_grid_build(aloam_ctx* c, int nb, const int* pl, int slot, int n_ls, int n_lf) {
   const int pb = (std::max(std::max(n_ls, n_lf), 1) + 255) / 256;
   Batch<RabArgs> ga = {};
   for (int l = 0; l < nb; ++l) {
-    FeatBuf& f = c->lanes[phys(pl, l)].feat[slot];
+    FeatBuf& f = c->lanes[pl[l]].feat[slot];
     ga.a[l] = RabArgs{f.g_ls, f.less_sharp, f.counts + 1, f.g_lf, f.less_flat, f.counts + 3};
   }
   LAUNCH(c, KID_GRID_BUILD, k_rab_count, dim3(pb, 2, nb), 256, 0, ga);
@@ -252,8 +251,8 @@ void run_grid_build(aloam_ctx* c, int nb, int slot, int n_ls, int n_lf, const in
 
 // outer_iters x (association + LM) ; feat[cur] supplies sharp/flat, feat[last] the targets ; pose in lane.d_pose
 // pose_slots (device, lane-major 7 doubles each, may be null): the integrated world pose is also written there by the last solve
-void run_register(aloam_ctx* c, int nb, int cur, int last, int sharp_slots, int flat_slots, bool integrate, bool want_corr, double* pose_slots,
-                  double* pose_override = nullptr /* lane 0: solve for this pose instead of the lane's warm start */, const int* pl = nullptr) {
+void run_register(aloam_ctx* c, int nb, const int* pl, int cur, int last, int sharp_slots, int flat_slots, bool integrate, bool want_corr,
+                  double* pose_slots, double* pose_override /* may be null; record 0: solve for this pose instead of its lane's warm start */) {
   OdomParams op{c->cfg.dist_sq_thresh, c->cfg.nearby_scan, c->cfg.distortion};
   const LmParams lp = lm_params(c->cfg);
   const int slots = sharp_slots + flat_slots;
@@ -261,7 +260,7 @@ void run_register(aloam_ctx* c, int nb, int cur, int last, int sharp_slots, int 
     const bool last_it = it == c->cfg.outer_iters - 1;
     Batch<AssocArgs> aa = {}; Batch<LmArgs> la = {};
     for (int l = 0; l < nb; ++l) {
-      const int lane = phys(pl, l);
+      const int lane = pl[l];
       Lane& L = c->lanes[lane];
       const FeatBuf& fc = L.feat[cur];
       const FeatBuf& fl = L.feat[last];
@@ -304,8 +303,7 @@ int aloam_extract_features(aloam_ctx* c, aloam_cloud_view raw, aloam_cloud_view*
   CUDA_CHECK_RET(cudaMemcpyAsync(L.d_raw[0], raw.data, (size_t)raw.n * raw.stride_floats * 4, cudaMemcpyHostToDevice, c->stream));
   FeatBuf& f = L.feat[kApiCur];
   const int slot = c->parity;
-  const float* rp = L.d_raw[0];
-  rc = run_features(c, 1, &rp, &raw.n, raw.stride_floats, kApiCur);
+  rc = run_features(c, L.d_raw[0], raw.n, raw.stride_floats, kApiCur);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->feat_counts, f.counts, 16, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_sc, L.d_sc + slot, sizeof(ScanScalars), cudaMemcpyDeviceToHost, c->stream));
@@ -361,7 +359,7 @@ int aloam_odometry_set_last(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cl
   CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
   if (corner_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (corner_last.n + 255) / 256, 256, 0, f.less_sharp, corner_last.n, f.rs_ls, c->d_err);
   if (surf_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (surf_last.n + 255) / 256, 256, 0, f.less_flat, surf_last.n, f.rs_lf, c->d_err);
-  run_grid_build(c, 1, kApiLast, corner_last.n, surf_last.n);
+  run_grid_build(c, 1, kLane0, kApiLast, corner_last.n, surf_last.n);
   CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -392,7 +390,7 @@ int aloam_odometry_register(aloam_ctx* c, aloam_cloud_view sharp, aloam_cloud_vi
   for (int k = 0; k < 3; ++k) c->pin->pose_in[4 + k] = t[k];
   CUDA_CHECK_RET(cudaEventRecord(c->ev0, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  run_register(c, 1, kApiCur, kApiLast, sharp.n, flat.n, false, false, nullptr, c->d_api_pose);
+  run_register(c, 1, kLane0, kApiCur, kApiLast, sharp.n, flat.n, false, false, nullptr, c->d_api_pose);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
@@ -441,7 +439,7 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
   Lane& L = c->lanes[0];
   const int cur = c->frame % kFeatSlots, last = (c->frame + kFeatSlots - 1) % kFeatSlots;
   const int slot = c->parity;
-  int rc = run_features(c, 1, &d_raw, &n, stride, cur);
+  int rc = run_features(c, d_raw, n, stride, cur);
   if (rc) return rc;
   int flags = 0;
   // The search index over this scan's less-sharp / less-flat clouds (what replaces the kd-tree rebuild, laserOdometry.cpp:567-568)
@@ -452,14 +450,14 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
     CUDA_CHECK_RET(cudaEventRecord(c->ev_feat[cur], c->stream));
     CUDA_CHECK_RET(cudaStreamWaitEvent(c->s_idx, c->ev_feat[cur], 0));
     if (!c->prof_on) c->stream = c->s_idx;   // (the per-kernel profiler times everything on one stream)
-    run_grid_build(c, 1, cur, 64 * kMaxLessSharpPerRing, std::min(n, c->max_points));
+    run_grid_build(c, 1, kLane0, cur, 64 * kMaxLessSharpPerRing, std::min(n, c->max_points));
     CUDA_CHECK_RET(cudaEventRecord(c->ev_idx[cur], c->stream));
   }
   if (c->frame == 0) {
     flags |= ALOAM_FLAG_INITIALISED_ONLY;  // laserOdometry.cpp:267-271
   } else {
     CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_idx[last], 0));   // the previous scan's index (built during the previous call)
-    run_register(c, 1, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, nullptr);
+    run_register(c, 1, kLane0, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, nullptr, nullptr);
   }
   CUDA_CHECK_RET(cudaEventRecord(c->ev_odo[cur], c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->world, L.d_world, 56, cudaMemcpyDeviceToHost, c->stream));
@@ -508,59 +506,14 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
   return scan_to_pose_impl(c, d_raw, n, 4, q_w, t_w, stats);
 }
 
-// Pipelined form of aloam_scan_to_pose for a sequence of scans of `nb` trajectories in lockstep: ring binning of scan k+1
-// (s_exa), per-ring extraction (s_ext), compaction + index build (s_idx) run concurrently with association + LM of scan k
-// (main stream) and the host->device copies of scan k+2 (s_h2d) -- the overlap the reference gets from its three ROS
-// processes.  Every launch covers all nb trajectories.  Results are identical to calling aloam_scan_to_pose once per scan
-// and trajectory.  raws / poses are scan-major: entry k * nb + b.
-// ops (n_scans x nb, scan-major) is the lane schedule of aloam_scan_stream_lanes, null for the lockstep calls (every lane scans
-// at every step, the context's first step only initialises).  A step runs its non-idle lanes only, packed into records
-// 0 .. na-1 of every launch (record i = lane act[i], which owns the buffers, pose slots and cube store); a step without any
-// issues nothing and leaves the frame counter alone.
-static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int nb, int device_resident, double* poses, aloam_stats* stats_last,
-                            double* map_poses = nullptr, const int* ops = nullptr) {
-  if (map_poses && (!c || c->cfg.max_map_points <= 0)) return ALOAM_ERR_INVALID_ARG;
-  if (!c || !raws || !poses || n_scans < 1 || nb < 1 || nb > c->n_lanes || (long long)n_scans * nb > kMaxStreamScans) return ALOAM_ERR_INVALID_ARG;
-  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call (lane schedule)
-  int run_err = ALOAM_OK;                                   // lane schedule: a scan that cannot run fails the call like a run-time error
-  if (!ops) {
-    if (c->lanes_mode) return ALOAM_ERR_STATE;   // the frame counter belongs to the lane schedule until aloam_reset_odometry
-    for (int k = 0; k < n_scans * nb; ++k) {
-      int rc = check_view(raws[k]); if (rc) return rc;
-      if (raws[k].n == 0) return ALOAM_ERR_EMPTY_CLOUD;
-      if (raws[k].n > c->max_points) return ALOAM_ERR_CAPACITY;
-      if (device_resident && raws[k].stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
-      if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
-    }
-  } else {
-    // the whole schedule is checked against the lanes' state before anything changes; lanes >= nb are idle all call
-    for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { running[l] = l < nb && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; }
-    for (size_t i = 0; i < (size_t)n_scans * nb; ++i)
-      if (ops[i] < ALOAM_LANE_IDLE || ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
-    for (int k = 0; k < n_scans; ++k) {
-      int stride = 0;
-      for (int l = 0; l < nb; ++l) {
-        const int op = ops[(size_t)k * nb + l];
-        const aloam_cloud_view& v = raws[(size_t)k * nb + l];
-        if (op == ALOAM_LANE_IDLE) { running[l] = false; continue; }   // its view is not read
-        int rc = check_view(v); if (rc) return rc;
-        if (v.n > 0) {
-          if (device_resident && v.stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
-          if (stride && v.stride_floats != stride) return ALOAM_ERR_INVALID_ARG;   // one stride per step
-          stride = v.stride_floats;
-        }
-        // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
-        if (op == ALOAM_LANE_SCAN && (!running[l] || mapped[l] != (map_poses != nullptr))) return ALOAM_ERR_STATE;
-        if (op == ALOAM_LANE_START) { running[l] = true; mapped[l] = map_poses != nullptr; }
-        if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
-        if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
-      }
-    }
-  }
-  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (run_err) { aloam_reset_odometry(c); return run_err; }
-  if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
-  if (ops) c->lanes_mode = true;
+// Pipelined form of aloam_scan_to_pose over `nb` lanes: ring binning of step k+1 (s_exa), per-ring extraction (s_ext), compaction
+// + index build (s_idx) run concurrently with association + LM of step k (main stream) and the host->device copies of step k+2
+// (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on a lane schedule
+// `ops` (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
+// (record i = lane act[i], which owns the buffers, pose slots and cube store); an all-idle step issues nothing.  reset_stores: a
+// START also resets its lane's cube store.  The caller has checked the views and the schedule and created the cube stores.
+static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int* ops, int n_scans, int nb, int device_resident, double* poses,
+                           double* map_poses, aloam_stats* stats_last, bool reset_stores) {
   StreamGuard guard(c);
   cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
@@ -585,24 +538,22 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   const float* d_raw[ALOAM_MAX_BATCH];      // per record
   int ns[ALOAM_MAX_BATCH];
   int act[ALOAM_MAX_BATCH], scanning[ALOAM_MAX_BATCH], starting[ALOAM_MAX_BATCH];   // lanes of the step: all, registering, initialising
-  int last_op[ALOAM_MAX_BATCH] = {};        // lane schedule: the last non-idle op of every lane in this call
+  int last_op[ALOAM_MAX_BATCH] = {};        // the last non-idle op of every lane in this call (IDLE: none)
   int issued = 0;
   for (int k = 0; k < n_scans; ++k) {
-    const int* op = ops ? ops + (size_t)k * nb : nullptr;
-    int na = 0;
-    for (int l = 0; l < nb; ++l)
-      if (!op || op[l] != ALOAM_LANE_IDLE) { act[na++] = l; if (op) last_op[l] = op[l]; }
+    const int* op = ops + (size_t)k * nb;
+    // a lane's first scan, its START, only initialises (laserOdometry.cpp:267-271)
+    int na = 0, n_scan = 0, n_start = 0;
+    for (int l = 0; l < nb; ++l) {
+      if (op[l] == ALOAM_LANE_IDLE) continue;
+      act[na++] = l; last_op[l] = op[l];
+      if (op[l] == ALOAM_LANE_START) starting[n_start++] = l; else scanning[n_scan++] = l;
+    }
     if (na == 0) continue;                  // an all-idle step: nothing to run, the frame does not advance
     const int f = c->frame;                 // global frame number of this step
     const int b = issued++ & 1;             // raw / ring-major double buffer
     const int cur = f % kFeatSlots, last = (f + kFeatSlots - 1) % kFeatSlots;
     const aloam_cloud_view* rv = raws + (size_t)k * nb;
-    // a lane's first scan only initialises (laserOdometry.cpp:267-271): every lane at the context's first step, or a START
-    int n_scan = 0, n_start = 0;
-    for (int i = 0; i < na; ++i) {
-      const bool start = op ? op[act[i]] == ALOAM_LANE_START : f == 0;
-      if (start) starting[n_start++] = act[i]; else scanning[n_scan++] = act[i];
-    }
     int nmax = 0;
     for (int i = 0; i < na; ++i) { ns[i] = rv[act[i]].n; nmax = std::max(nmax, ns[i]); }
     if (device_resident) {
@@ -620,12 +571,13 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     // ---- stage A (ring binning) on s_exa: needs full[b] free, i.e. stage B of scan k-2 done
     STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_b[b], 0));
     c->stream = c->s_exa;
-    // a START re-arms the lane's ScanScalars slot of this scan: k_ring_scan arms it only for a lane that ran the step before
-    if (op)
-      for (int i = 0; i < n_start; ++i)
-        STREAM_TRY(cudaMemcpyAsync(c->lanes[starting[i]].d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->s_exa));
+    // A START re-arms the lane's ScanScalars slot (k_ring_scan arms it only for a lane that ran the step before) and, below, resets its pose.
+    // At a lockstep call's first step these copies change nothing: k_ring_scan armed the slot with d_sc_init's four fields, start_ori /
+    // end_ori are written (k_classify, k_ring_scan) before they are read, and aloam_reset_odometry has put the identity in d_pose / d_world.
+    for (int i = 0; i < n_start; ++i)
+      STREAM_TRY(cudaMemcpyAsync(c->lanes[starting[i]].d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->s_exa));
     int sc_slot = 0;
-    int rc = run_features_a(c, na, d_raw, ns, device_resident ? 4 : rv[act[0]].stride_floats, b, &sc_slot, c->d_scan_nfull + (size_t)k * nb, act);
+    int rc = run_features_a(c, na, act, d_raw, ns, device_resident ? 4 : rv[act[0]].stride_floats, b, &sc_slot, c->d_scan_nfull + (size_t)k * nb);
     if (rc) return fail(rc);
     if (!device_resident) STREAM_TRY(cudaEventRecord(c->ev_rawfree[b], c->s_exa));
     STREAM_TRY(cudaEventRecord(c->ev_a[b], c->s_exa));
@@ -634,7 +586,7 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     c->stream = c->s_ext;
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_a[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_cmp[b], 0));
-    rc = run_features_b1(c, na, b, sc_slot, act);
+    rc = run_features_b1(c, na, act, b, sc_slot);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_b[b], c->s_ext));
     // ---- stage C on s_idx: ring-ordered compaction into feat[f % kFeatSlots] -- that slot was last read by the odometry
@@ -644,11 +596,11 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_b[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_odo[(f + 1) % kFeatSlots], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the scan-to-map stage of frame f - kFeatSlots has read this slot
-    rc = run_features_b2(c, na, b, cur, false, act);
+    rc = run_features_b2(c, na, act, b, cur, false);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
     STREAM_TRY(cudaEventRecord(c->ev_feat[cur], c->s_idx));
-    run_grid_build(c, na, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points), act);
+    run_grid_build(c, na, act, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
     STREAM_TRY(cudaEventRecord(c->ev_idx[cur], c->s_idx));
     c->stream = s_main;
     // ---- association + LM on the main stream: this scan's sharp / flat points, the previous scan's clouds + index
@@ -656,15 +608,13 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_idx[last], 0));
     // the last solve of the scan writes the integrated world pose into its slot of d_poses (no copy on the critical chain)
     double* slots = c->d_poses + (size_t)k * nb * 7;
-    for (int i = 0; i < n_start; ++i) {
+    for (int i = 0; i < n_start; ++i) {   // a new trajectory: warm start and world pose back to the identity, in stream order
       Lane& L = c->lanes[starting[i]];
-      if (op) {   // a new trajectory of the lane schedule: warm start and world pose back to the identity, in stream order
-        STREAM_TRY(cudaMemcpyAsync(L.d_pose, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
-        STREAM_TRY(cudaMemcpyAsync(L.d_world, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
-      }
+      STREAM_TRY(cudaMemcpyAsync(L.d_pose, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
+      STREAM_TRY(cudaMemcpyAsync(L.d_world, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
       STREAM_TRY(cudaMemcpyAsync(slots + (size_t)starting[i] * 7, L.d_world, 56, cudaMemcpyDeviceToDevice, s_main));
     }
-    if (n_scan > 0) run_register(c, n_scan, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots, nullptr, scanning);
+    if (n_scan > 0) run_register(c, n_scan, scanning, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots, nullptr);
     STREAM_TRY(cudaEventRecord(c->ev_odo[cur], s_main));
     if (map_poses) {
       // ---- scan-to-map on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose go
@@ -673,14 +623,13 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
       //      One frame covers every trajectory: each launch of it serves all lanes, each lane with its own cube store.
       STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
       c->stream = c->s_map;
-      //      A START lane's frame begins by resetting its cube store (k_mapper_begin).
       MapperIn in[ALOAM_MAX_BATCH];
       for (int i = 0; i < na; ++i) {
         const int l = act[i];
         const FeatBuf& fc = c->lanes[l].feat[cur];
         const size_t slot = ((size_t)k * nb + l) * 7;
         in[i] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
-                         op && op[l] == ALOAM_LANE_START};
+                         reset_stores && op[l] == ALOAM_LANE_START};
       }
       rc = mapper_step_device(c, na, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
       if (rc) return fail(rc);
@@ -716,21 +665,17 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
     for (int b = 0; b < 3; ++b)
       if (c->h_sc[3 * l + b].error) return fail(c->h_sc[3 * l + b].error);
   for (size_t i = 0; i < total; ++i)   // (an idle entry has no scan)
-    if (!(ops && ops[i] == ALOAM_LANE_IDLE) && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
+    if (ops[i] != ALOAM_LANE_IDLE && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
   std::memcpy(poses, c->h_poses, total * 56);
   if (map_poses) std::memcpy(map_poses, c->h_poses + (size_t)kMaxStreamScans * 7, total * 56);
-  if (ops) {
-    for (size_t i = 0; i < total; ++i)
-      if (ops[i] == ALOAM_LANE_IDLE)
-        for (int j = 0; j < 7; ++j) { poses[i * 7 + j] = NAN; if (map_poses) map_poses[i * 7 + j] = NAN; }
-    for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; }
-  }
+  for (size_t i = 0; i < total; ++i)
+    if (ops[i] == ALOAM_LANE_IDLE)
+      for (int j = 0; j < 7; ++j) { poses[i * 7 + j] = NAN; if (map_poses) map_poses[i * 7 + j] = NAN; }
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (stats_last) {
     for (int l = 0; l < nb; ++l) {
-      const bool init_only = ops ? last_op[l] == ALOAM_LANE_START : c->frame <= 1;
-      if (ops && last_op[l] == ALOAM_LANE_IDLE) std::memset(&stats_last[l], 0, sizeof(aloam_stats));   // idle all call
-      else if (init_only) { std::memset(&stats_last[l], 0, sizeof(aloam_stats)); stats_last[l].flags = ALOAM_FLAG_INITIALISED_ONLY; stats_last[l].ms_total = ms; }
+      if (last_op[l] == ALOAM_LANE_IDLE) std::memset(&stats_last[l], 0, sizeof(aloam_stats));   // idle all call
+      else if (last_op[l] == ALOAM_LANE_START) { std::memset(&stats_last[l], 0, sizeof(aloam_stats)); stats_last[l].flags = ALOAM_FLAG_INITIALISED_ONLY; stats_last[l].ms_total = ms; }
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
@@ -743,33 +688,87 @@ static int scan_stream_impl(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
   return ALOAM_OK;
 }
 
+static bool stream_args_ok(const aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int nb, const double* poses, const double* map_poses) {
+  return c && raws && poses && n_scans >= 1 && nb >= 1 && nb <= c->n_lanes && (long long)n_scans * nb <= kMaxStreamScans && (!map_poses || c->cfg.max_map_points > 0);
+}
+
+// the lockstep calls: every lane STARTs at the context's first step, SCANs after it and keeps its cube store over a START
+static int scan_stream_lockstep(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int nb, int device_resident, double* poses,
+                                double* map_poses, aloam_stats* stats_last) {
+  if (!stream_args_ok(c, raws, n_scans, nb, poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
+  if (c->lanes_mode) return ALOAM_ERR_STATE;   // the frame counter belongs to the lane schedule until aloam_reset_odometry
+  for (int k = 0; k < n_scans * nb; ++k) {
+    int rc = check_view(raws[k]); if (rc) return rc;
+    if (raws[k].n == 0) return ALOAM_ERR_EMPTY_CLOUD;
+    if (raws[k].n > c->max_points) return ALOAM_ERR_CAPACITY;
+    if (device_resident && raws[k].stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
+    if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+  }
+  for (int i = 0; i < n_scans * nb; ++i) c->lockstep_ops[i] =c->frame == 0 && i < nb ? ALOAM_LANE_START : ALOAM_LANE_SCAN;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
+  return scan_stream_run(c, raws, c->lockstep_ops, n_scans, nb, device_resident, poses, map_poses, stats_last, false);
+}
+
 int aloam_scan_stream(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int device_resident, double* poses, aloam_stats* stats_last) {
-  return scan_stream_impl(c, raws, n_scans, 1, device_resident, poses, stats_last);
+  return scan_stream_lockstep(c, raws, n_scans, 1, device_resident, poses, nullptr, stats_last);
 }
 
 int aloam_scan_stream_mapped(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int device_resident, double* odom_poses, double* map_poses,
                              aloam_stats* stats_last) {
   if (!map_poses) return ALOAM_ERR_INVALID_ARG;
-  return scan_stream_impl(c, raws, n_scans, 1, device_resident, odom_poses, stats_last, map_poses);
+  return scan_stream_lockstep(c, raws, n_scans, 1, device_resident, odom_poses, map_poses, stats_last);
 }
 
 int aloam_scan_stream_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* poses,
                             aloam_stats* stats_last) {
-  return scan_stream_impl(c, raws, n_scans, batch, device_resident, poses, stats_last);
+  return scan_stream_lockstep(c, raws, n_scans, batch, device_resident, poses, nullptr, stats_last);
 }
 
 int aloam_scan_stream_mapped_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* odom_poses,
                                    double* map_poses, aloam_stats* stats_last) {
   if (!map_poses) return ALOAM_ERR_INVALID_ARG;
   if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
-  return scan_stream_impl(c, raws, n_scans, batch, device_resident, odom_poses, stats_last, map_poses);
+  return scan_stream_lockstep(c, raws, n_scans, batch, device_resident, odom_poses, map_poses, stats_last);
 }
 
 int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch, int device_resident,
                             double* odom_poses, double* map_poses, aloam_stats* stats_last) {
   if (!lane_ops) return ALOAM_ERR_INVALID_ARG;
   if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
-  return scan_stream_impl(c, raws, n_scans, batch, device_resident, odom_poses, stats_last, map_poses, lane_ops);
+  if (!stream_args_ok(c, raws, n_scans, batch, odom_poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
+  // the whole schedule is checked against the lanes' state before anything changes; lanes >= batch are idle all call
+  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { running[l] = l < batch && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; }
+  for (size_t i = 0; i < (size_t)n_scans * batch; ++i)
+    if (lane_ops[i] < ALOAM_LANE_IDLE || lane_ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
+  int run_err = ALOAM_OK;   // a scan that cannot run fails the call like a run-time error
+  for (int k = 0; k < n_scans; ++k) {
+    int stride = 0;
+    for (int l = 0; l < batch; ++l) {
+      const int op = lane_ops[(size_t)k * batch + l];
+      const aloam_cloud_view& v = raws[(size_t)k * batch + l];
+      if (op == ALOAM_LANE_IDLE) { running[l] = false; continue; }   // its view is not read
+      int rc = check_view(v); if (rc) return rc;
+      if (v.n > 0) {
+        if (device_resident && v.stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
+        if (stride && v.stride_floats != stride) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+        stride = v.stride_floats;
+      }
+      // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
+      if (op == ALOAM_LANE_SCAN && (!running[l] || mapped[l] != (map_poses != nullptr))) return ALOAM_ERR_STATE;
+      if (op == ALOAM_LANE_START) { running[l] = true; mapped[l] = map_poses != nullptr; }
+      if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
+      if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
+    }
+  }
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  if (run_err) { aloam_reset_odometry(c); return run_err; }
+  if (map_poses) { int rc = mapper_ensure_lanes(c, batch); if (rc) return rc; }   // creates the cube stores this call needs
+  // committed before anything is issued: a later failure ends in aloam_reset_odometry, a key overflow leaves the lanes running
+  c->lanes_mode = true;
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; }
+  return scan_stream_run(c, raws, lane_ops, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
 }
 
 // ------------------------------------------------------------------------------------------------ fine-grained

@@ -121,7 +121,7 @@ struct aloam_ctx {
   int* d_scan_nfull = nullptr;     // [kMaxStreamScans] ring-major cloud size of every (scan, lane) of a stream call
   double *d_out28 = nullptr, *d_packed = nullptr;
   double* d_api_pose = nullptr;    // [8] pose of the per-stage entry points (odometry_register, solve, ...): not the warm start of the fused pipeline
-  double* d_ident = nullptr;       // [7] identity pose, the source of a lane's odometry reset inside aloam_scan_stream_lanes
+  double* d_ident = nullptr;       // [7] identity pose, the source of a lane's odometry reset at a START of the stream driver
   ScanScalars* d_sc_init = nullptr;   // [1] an armed ScanScalars slot (what k_ring_scan arms for the next scan), same use
   int* d_err = nullptr;
   Pt4* d_query = nullptr;
@@ -189,6 +189,7 @@ struct aloam_ctx {
   bool lanes_mode = false;
   bool lane_running[ALOAM_MAX_BATCH] = {};
   bool lane_mapped[ALOAM_MAX_BATCH] = {};
+  int lockstep_ops[kMaxStreamScans] = {};   // the lane schedule a lockstep stream call hands to the stream driver
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
   std::vector<cudaStream_t> streams;
