@@ -898,13 +898,4 @@ int aloam_debug_feature_cycles(aloam_ctx* c, long long* out64x8) {
   return ALOAM_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ mapping (mapping.cu)
-int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
-int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats);
-
-int aloam_map_upload(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map) { return aloam_map_upload_impl(c, corner_map, surf_map); }
-int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats) {
-  return aloam_mapping_register_impl(c, corner_stack, surf_stack, x, stats);
-}
-
 }  // extern "C"

@@ -12,20 +12,20 @@
 
 namespace aloam {
 // the buffers of one scan-to-map registration (mapping.cu): the two indexed submaps, the neighbours found by k_map_knn5, the
-// residual blocks and the solve summaries.  The context's set serves the host API and lane 0 of the mapper; every other lane
-// of aloam_scan_stream_mapped_batch owns a set of its own.
+// residual blocks, the solve summaries and the corner / surf stacks being registered.  The context's set serves the host API
+// and lane 0 of the mapper; every other lane of aloam_scan_stream_mapped_batch owns a set of its own.
 struct MapReg {
   MapCloud corner, surf;
   float4* nbr;
   BlockRec* blocks;
   LmSummary* summary;   // [4]
+  Pt4* stack[2];
 };
-// one lane of the mapper's index build (the submap clouds) and registration (the filtered stacks, their sizes
-// {n_corner, n_surf, total} and the pose being refined), all device pointers
+// one lane of the mapper's index build (the submap clouds) and registration (the stacks' sizes {n_corner, n_surf, total} and
+// the pose being refined), all device pointers
 struct MapLaneIO {
   MapReg reg;
   const Pt4* sub[2];
-  const Pt4* stack[2];
   const int* counts3;
   double* pose;
 };
@@ -136,21 +136,17 @@ struct aloam_ctx {
   // map cube store of every lane (cubemap.cu), each created on first use: lane 0 serves the host API and both mapped stream
   // calls, lanes 1 .. max_batch-1 only aloam_scan_stream_mapped_batch
   void* mapper[ALOAM_MAX_BATCH] = {};
-  // scan-to-map: uploaded submap (corner, surf) with hash grids, stack queries, fit debug records
-  MapCloud map_corner = {}, map_surf = {};
+  // scan-to-map: the registration set of the host API and mapper lane 0 (uploaded submap with its hash grids, stacks, ...)
+  MapReg map = {};
   Pt4* d_map_pts[2] = {nullptr, nullptr};   // staging for maps handed in as host views (device views are indexed in place)
   int max_map = 0, map_slots = 0;
   int map_n[2] = {0, 0};          // points indexed on this rank (corner, surf)
   int map_global_n[2] = {0, 0};   // size of the whole submap (== map_n unless the map is sharded over ranks)
   bool have_map = false;
   bool map_ready = false;         // every buffer of this group is allocated (set last by ensure_map_buffers)
-  Pt4 *d_stack_corner = nullptr, *d_stack_surf = nullptr;
-  int* d_stack_counts = nullptr;  // [4] {n_corner, n_surf, total} of the stacks being registered
-  float4* d_nbr = nullptr;        // [queries][5] neighbours found by k_map_knn5 (x, y, z, index bits)
-  double* d_map_pose = nullptr;   // [7] scan-to-map pose being refined (parameters[7], laserMapping.cpp:110)
+  int* d_stack_counts = nullptr;  // [4] {n_corner, n_surf, total} of the host API's stacks
+  double* d_map_pose = nullptr;   // [7] host API: scan-to-map pose being refined (parameters[7], laserMapping.cpp:110)
   double* d_fits = nullptr;       // [queries][14] debug / test records of the line / plane fits
-  BlockRec* d_map_blocks = nullptr;
-  LmSummary* d_map_summary = nullptr;   // [4] summaries of the scan-to-map solves
   // aloam_voxel_filter (voxel.cu): a segmented filter of its own (cap = max_points), created on first use
   SegBuffers vox_seg;
   int* d_seg_io = nullptr;        // [3] the segment's size, its filtered size, the filter's error word
@@ -269,13 +265,11 @@ int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int mapper_ensure_lanes(aloam_ctx* c, int nb);
 int* mapper_err_acc(aloam_ctx* c, int lane);
-MapReg ctx_map_reg(const aloam_ctx* c);
-MapLaneIO ctx_map_io(const aloam_ctx* c, const Pt4* sub_corner, const Pt4* sub_surf);
-Batch<GridArgs> grid_setup_args(const MapLaneIO& io, const int* na, const int* nb);
-int map_reg_alloc(aloam_ctx* c, MapReg* r, Pt4** stack_corner, Pt4** stack_surf);
+int ensure_map_buffers(aloam_ctx* c);
+int map_reg_alloc(aloam_ctx* c, MapReg* r);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
-int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_corner, const Pt4* sub_surf, const int* n_surf, int n_upper, int* err_word);
-void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, double* d_fits);
+int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
+void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper);
 namespace {
 
 LmParams lm_params(const aloam_config& c) {

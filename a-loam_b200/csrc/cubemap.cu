@@ -23,8 +23,6 @@
 #include "common.cuh"
 #include "ctx.h"
 
-extern "C" int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
-
 namespace {
 
 constexpr int CW = 21, CH = 21, CD = 11, NCUBE = CW * CH * CD;   // laserCloudWidth / Height / Depth (:77-82)
@@ -72,8 +70,7 @@ struct Mapper {
   int* d_dbg_counts = nullptr;              //                                their sizes [ALOAM_MAX_SEGS]
   int* d_dbg_err = nullptr;                 //                                private error word
   int max_sub = 0;
-  MapReg reg = {};                          // lanes > 0: a registration set of their own (lane 0 uses the context's, shared with
-  Pt4* d_stack[2] = {nullptr, nullptr};     //            the host API) and the filtered corner / surf stacks
+  MapReg* reg = nullptr;                    // registration set: lane 0 shares the context's with the host API, the others own one
   cudaStream_t s_aux = nullptr;             // the stack filters run here, beside the submap gather + index build
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 };
@@ -507,7 +504,11 @@ int ensure_mapper(aloam_ctx* c, int lane) {
   ok = ok && screate(c, &m->s_aux) == cudaSuccess;
   ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
-  ok = ok && (lane == 0 || map_reg_alloc(c, &m->reg, &m->d_stack[0], &m->d_stack[1]) == ALOAM_OK);
+  // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
+  // created here, after the context's (which fixes the table size)
+  m->reg = lane == 0 ? &c->map : new (std::nothrow) MapReg();
+  if (lane > 0 && m->reg) own(c, [r = m->reg] { delete r; });
+  ok = ok && m->reg && (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK && map_reg_alloc(c, m->reg) == ALOAM_OK));
   if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
     cudaGetLastError();
     return ALOAM_ERR_CUDA;
@@ -525,15 +526,12 @@ int ensure_mapper(aloam_ctx* c, int lane) {
 // lane l computes exactly what a frame of lane l alone computes.  in[l]: the lane's less-sharp / less-flat clouds and their
 // sizes, its odometry pose (7 doubles) and its output pose slot, all device pointers, the lane whose cube store record l
 // runs on and whether that store starts a fresh trajectory; n_upper_* bound the cloud sizes of every lane.  Lane 0 registers
-// with the buffers of mapping.cu that it shares with the host API.  A sharded job maps one lane.
+// with the context's set, shared with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && c->shard_count > 1)) return ALOAM_ERR_STATE;
   int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's auxiliary stream carries the stack filters of every lane
   for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
-  if (!c->map_ready) {
-    aloam_cloud_view none{nullptr, 0, 4};
-    rc = aloam_map_upload_impl(c, none, none); if (rc) return rc;
-  }
+  rc = ensure_map_buffers(c); if (rc) return rc;     // lane 0's set
   Mapper* m0 = static_cast<Mapper*>(c->mapper[0]);
   Batch<MapperLane> B = {};
   MapLaneIO io[ALOAM_MAX_BATCH];
@@ -549,13 +547,11 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     const int lane = in[l].lane;
     Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
     MapperState* S = m->d_state;
-    const MapReg reg = lane == 0 ? ctx_map_reg(c) : m->reg;
-    Pt4* const stack_corner = lane == 0 ? c->d_stack_corner : m->d_stack[0];
-    Pt4* const stack_surf = lane == 0 ? c->d_stack_surf : m->d_stack[1];
+    const MapReg& reg = *m->reg;
     B.a[l] = MapperLane{S, in[l].odom7, in[l].out7, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, {m->d_sub[0], m->d_sub[1]}, {in[l].corner, in[l].surf},
-                        {in[l].nc, in[l].ns}, {stack_corner, stack_surf}, m->d_world, m->d_cube, m->buf.segs, m->buf.n_seg};
+                        {in[l].nc, in[l].ns}, {reg.stack[0], reg.stack[1]}, m->d_world, m->d_cube, m->buf.segs, m->buf.n_seg};
     if (in[l].fresh) fresh |= 1u << l;
-    io[l] = MapLaneIO{reg, {m->d_sub[0], m->d_sub[1]}, {stack_corner, stack_surf}, S->stack_counts, S->x};
+    io[l] = MapLaneIO{reg, {m->d_sub[0], m->d_sub[1]}, S->stack_counts, S->x};
     gs.a[l] = GridArgs{reg.corner.grid, m->d_sub[0], &S->n_sub[0], reg.surf.grid, m->d_sub[1], &S->n_sub[1]};
     stack_f[l] = seg_filter(m->buf, 31, &S->err);
     cube_f[l] = seg_filter(m->buf, cube_bits, &S->err);
@@ -584,7 +580,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     // on every rank) but indexes and searches only its x-slabs (+ halo) of the submap; the ranks meet in the all-reduce of the
     // normal equations inside the solve.  The too-thin test of k_mapper_prep is on the whole submap, the same on every rank.
     MapperState* S = m0->d_state;
-    rc = map_shard_index_device(c, m0->d_sub[0], &S->n_sub[0], m0->d_sub[1], &S->n_sub[1], max_sub, &S->err); if (rc) return rc;
+    rc = map_shard_index_device(c, m0->d_sub, S->n_sub, max_sub, &S->err); if (rc) return rc;
   } else {
     launch_ex(c, KID_MAP_GRID, k_grid_setup, dim3(1, 1, nb), dim3(32), 0, 1, true, gs);
     map_index_build(c, nb, io, max_sub);
@@ -594,7 +590,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- optimisation (:554-733)
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  map_register_device(c, nb, io, nq_upper, nullptr);
+  map_register_device(c, nb, io, nq_upper);
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- insertion (:736-767)
   const int up = std::max(n_upper_c, n_upper_s);
@@ -652,7 +648,7 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   rc = mapper_step_device(c, 1, &one, corner_last.n, surf_last.n);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, m->reg->summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(&m->h_state->flags, &m->d_state->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

@@ -664,41 +664,6 @@ int comm_allreduce_int2(aloam_ctx* c, int* d_two);   // comm.cu
 namespace {
 inline int grid_ctas(const aloam_ctx* c) { return c->sms * 8; }   // grid-stride launches: 8 resident CTAs of 256 threads per SM
 
-// the two grid tables of one registration, sized for cfg.max_map_points (c->map_slots)
-bool alloc_grids(aloam_ctx* c, MapReg* r) {
-  for (int t = 0; t < 2; ++t) {
-    GridTable& g = (t ? r->surf : r->corner).grid;
-    if (dalloc(c, &g.slots, (size_t)c->map_slots) != cudaSuccess || dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, (size_t)c->max_map) != cudaSuccess)
-      return false;
-    if (cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess) return false;
-    g.cap_slots = (unsigned)c->map_slots;
-    g.cs = 1.0f * (1.0f + 1e-5f);   // > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
-    g.inv_cs = 1.0f / g.cs;
-  }
-  return true;
-}
-
-int ensure_map_buffers(aloam_ctx* c) {
-  if (c->map_ready) return ALOAM_OK;
-  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
-  c->max_map = c->cfg.max_map_points;
-  unsigned slots = 1024;
-  while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;   // ends: aloam_create bounds max_map_points by 2^30
-  c->map_slots = (int)slots;
-  const size_t mm = (size_t)c->max_map;
-  MapReg r = {};
-  if (dalloc(c, &c->d_map_pts[0], mm) != cudaSuccess || dalloc(c, &c->d_map_pts[1], mm) != cudaSuccess || !alloc_grids(c, &r)) return ALOAM_ERR_CUDA;
-  c->map_corner = r.corner; c->map_surf = r.surf;
-  const size_t mp = (size_t)c->max_points;
-  if (dalloc(c, &c->d_stack_corner, mp) != cudaSuccess || dalloc(c, &c->d_stack_surf, mp) != cudaSuccess ||
-      dalloc(c, &c->d_fits, 2 * mp * 14) != cudaSuccess || dalloc(c, &c->d_map_blocks, 2 * mp) != cudaSuccess ||
-      dalloc(c, &c->d_nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &c->d_stack_counts, 4) != cudaSuccess ||
-      dalloc(c, &c->d_map_pose, 8) != cudaSuccess || dalloc(c, &c->d_map_summary, 4) != cudaSuccess)
-    return ALOAM_ERR_CUDA;
-  c->map_ready = true;
-  return ALOAM_OK;
-}
-
 // device pointer with 16-byte points: the index can be built straight from the caller's memory (no staging copy)
 bool is_device_ptr(const void* p) {
   cudaPointerAttributes at;
@@ -707,37 +672,49 @@ bool is_device_ptr(const void* p) {
 }
 }  // namespace
 
-// K0 over two clouds already in device memory; their sizes are in the GridDyn records (host path: written by the caller;
-// mapping loop: k_grid_setup).  n_upper bounds the larger cloud (grid sizing only).
-MapReg ctx_map_reg(const aloam_ctx* c) { return MapReg{c->map_corner, c->map_surf, c->d_nbr, c->d_map_blocks, c->d_map_summary}; }
-
-// the host API's lane: the context's registration set, its stacks, and the clouds to index
-MapLaneIO ctx_map_io(const aloam_ctx* c, const Pt4* sub_corner, const Pt4* sub_surf) {
-  return MapLaneIO{ctx_map_reg(c), {sub_corner, sub_surf}, {c->d_stack_corner, c->d_stack_surf}, nullptr, nullptr};
-}
-
-Batch<GridArgs> grid_setup_args(const MapLaneIO& io, const int* na, const int* nb) {
-  Batch<GridArgs> g = {};
-  g.a[0] = GridArgs{io.reg.corner.grid, io.sub[0], na, io.reg.surf.grid, io.sub[1], nb};
-  return g;
-}
-
-// a registration set of its own for a mapper lane other than 0 (the context's map buffers are created first: they fix the
-// table size), with the two stack buffers.  On failure what was acquired belongs to the context until aloam_destroy.
-int map_reg_alloc(aloam_ctx* c, MapReg* r, Pt4** stack_corner, Pt4** stack_surf) {
-  int rc = ensure_map_buffers(c); if (rc) return rc;
+// the buffers of one registration set, its two grid tables sized for cfg.max_map_points (c->map_slots, fixed by
+// ensure_map_buffers, which creates the context's set before any other).  On failure what was acquired belongs to the context
+// until aloam_destroy.
+int map_reg_alloc(aloam_ctx* c, MapReg* r) {
+  for (int t = 0; t < 2; ++t) {
+    GridTable& g = (t ? r->surf : r->corner).grid;
+    if (dalloc(c, &g.slots, (size_t)c->map_slots) != cudaSuccess || dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, (size_t)c->max_map) != cudaSuccess ||
+        cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess)
+      return ALOAM_ERR_CUDA;
+    g.cap_slots = (unsigned)c->map_slots;
+    g.cs = 1.0f * (1.0f + 1e-5f);   // > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
+    g.inv_cs = 1.0f / g.cs;
+  }
   const size_t mp = (size_t)c->max_points;
-  *r = MapReg{};
-  if (!alloc_grids(c, r) || dalloc(c, &r->nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &r->blocks, 2 * mp) != cudaSuccess ||
-      dalloc(c, &r->summary, 4) != cudaSuccess || dalloc(c, stack_corner, mp) != cudaSuccess || dalloc(c, stack_surf, mp) != cudaSuccess)
+  if (dalloc(c, &r->nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &r->blocks, 2 * mp) != cudaSuccess || dalloc(c, &r->summary, 4) != cudaSuccess ||
+      dalloc(c, &r->stack[0], mp) != cudaSuccess || dalloc(c, &r->stack[1], mp) != cudaSuccess)
     return ALOAM_ERR_CUDA;
+  return ALOAM_OK;
+}
+
+// the context's map buffers: the staging of uploaded maps, the registration set of the host API and mapper lane 0, and the
+// host API's stack sizes, pose and fit records
+int ensure_map_buffers(aloam_ctx* c) {
+  if (c->map_ready) return ALOAM_OK;
+  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
+  c->max_map = c->cfg.max_map_points;
+  unsigned slots = 1024;
+  while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;   // ends: aloam_create bounds max_map_points by 2^30
+  c->map_slots = (int)slots;
+  const size_t mm = (size_t)c->max_map, mp = (size_t)c->max_points;
+  if (dalloc(c, &c->d_map_pts[0], mm) != cudaSuccess || dalloc(c, &c->d_map_pts[1], mm) != cudaSuccess || map_reg_alloc(c, &c->map) != ALOAM_OK ||
+      dalloc(c, &c->d_stack_counts, 4) != cudaSuccess || dalloc(c, &c->d_map_pose, 8) != cudaSuccess || dalloc(c, &c->d_fits, 2 * mp * 14) != cudaSuccess)
+    return ALOAM_ERR_CUDA;
+  c->map_ready = true;
   return ALOAM_OK;
 }
 
 // CTAs per lane of a grid-stride launch over nb lanes: one resident wave in all (8 CTAs of 256 threads per SM)
 inline int lane_ctas(const aloam_ctx* c, int nb) { return std::max(1, grid_ctas(c) / nb); }
 
-// K0 of nb lanes in one launch per phase: lane l indexes io[l].sub[0] / [1] into io[l].reg
+// K0 of nb lanes in one launch per phase: lane l indexes io[l].sub[0] / [1], already in device memory, into io[l].reg.  The
+// clouds' sizes are in the GridDyn records (host upload: written by the caller; otherwise: k_grid_setup); n_upper bounds the
+// larger cloud (grid sizing only).
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper) {
   const int pb = std::max(1, std::min((std::max(n_upper, 1) + 255) / 256, lane_ctas(c, nb)));
   const unsigned slots_upper = grid_mask_for(std::max(n_upper, 1), (unsigned)c->map_slots) + 1;
@@ -750,19 +727,28 @@ void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper) {
   launch_ex(c, KID_MAP_GRID, k_grid_fill, dim3(pb, 2, nb), dim3(256), 0, 1, true, g);
 }
 
-// outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers io[l].stack[0] / [1] (sizes
-// io[l].counts3 = {n_corner, n_surf, total}) against io[l].reg at pose io[l].pose, all in device memory.  d_fits: lane 0 only.
-void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, double* d_fits) {
-  const LmParams lp = lm_params(c->cfg);
+namespace {
+// 5-NN + fits of nb lanes, one launch each covering all of them: lane l associates io[l].reg.stack[0] / [1] (sizes io[l].counts3 =
+// {n_corner, n_surf, total}) at pose io[l].pose with io[l].reg's submaps into its residual blocks, all in device memory.  fits:
+// lane 0's debug records, or null.  pdl: the 5-NN may become resident under the previous kernel of the stream.
+void map_associate_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, bool pdl, double* fits) {
   const int kb = std::max(1, std::min((nq_upper + 7) / 8, lane_ctas(c, nb)));
   const int fb = std::max(1, (nq_upper + 31) / 32);   // one warp per CTA: a few thousand serial double-precision fits spread over all SMs
   Batch<MapAssocArgs> a = {};
   for (int l = 0; l < nb; ++l)
-    a.a[l] = MapAssocArgs{io[l].stack[0], io[l].stack[1], io[l].counts3, io[l].reg.corner, io[l].reg.surf, io[l].pose, io[l].reg.nbr, io[l].reg.blocks,
-                          l == 0 ? d_fits : nullptr};
+    a.a[l] = MapAssocArgs{io[l].reg.stack[0], io[l].reg.stack[1], io[l].counts3, io[l].reg.corner, io[l].reg.surf, io[l].pose, io[l].reg.nbr,
+                          io[l].reg.blocks, l == 0 ? fits : nullptr};
+  launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb, 1, nb), dim3(256), 0, 1, pdl, a, c->shard_rank, c->shard_count);
+  launch_ex(c, KID_MAP_FIT, k_map_fit, dim3(fb, 1, nb), dim3(32), 0, 1, true, a);
+}
+}  // namespace
+
+// outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers its stacks against io[l].reg
+// (see map_associate_device) and refines io[l].pose
+void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper) {
+  const LmParams lp = lm_params(c->cfg);
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
-    launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb, 1, nb), dim3(256), 0, 1, it > 0, a, c->shard_rank, c->shard_count);
-    launch_ex(c, KID_MAP_FIT, k_map_fit, dim3(fb, 1, nb), dim3(32), 0, 1, true, a);
+    map_associate_device(c, nb, io, nq_upper, it > 0, nullptr);
     if (c->shard_count <= 1) {
       Batch<LmArgs> lm = {};
       for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
@@ -773,34 +759,71 @@ void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper
   }
 }
 
-// The mapper of a rank of a sharded job (cubemap.cu): the gathered submap (whole, device-resident, sizes on the device) is cut
-// into this rank's x-slabs + halo and indexed, all in stream order -- nothing returns to the host.  An overflow of the shard
-// buffer sets bit 0 of *err_word.
-int map_shard_index_device(aloam_ctx* c, const Pt4* sub_corner, const int* n_corner, const Pt4* sub_surf, const int* n_surf, int n_upper, int* err_word) {
-  const Pt4* subs[2] = {sub_corner, sub_surf};
-  const int* ns[2] = {n_corner, n_surf};
-  int* d_cnt = c->d_stack_counts;    // [0], [1]: points kept per cloud (the mapper keeps its stack counts in its own state)
-  int* d_blocks = reinterpret_cast<int*>(c->d_nbr);
-  const int nb = std::max(1, (n_upper + 255) / 256);
+namespace {
+// One piece of cloud t of a sharded map cut into this rank's x-slabs + halo and appended to d_map_pts[t], behind the d_kept[t]
+// points already there: the n points `stride` floats apart at pts, or only the first *n_dev of them when n_dev is set (a submap
+// gathered on the device; n bounds it).  An overflow of max_map sets bit 0 of *err.
+int shard_cut(aloam_ctx* c, int t, const float* pts, int stride, int n, const int* n_dev, int* d_kept, int* err) {
+  int* d_blocks = reinterpret_cast<int*>(c->map.nbr);   // the per-block counts: scratch outside a registration
+  const int nb = std::max(1, (n + 255) / 256);
   if ((size_t)nb * 4 > (size_t)2 * c->max_points * 5 * sizeof(float4)) return ALOAM_ERR_CAPACITY;
-  CUDA_CHECK_RET(cudaMemsetAsync(d_cnt, 0, 8, c->stream));
-  const float inv_cs = c->map_corner.grid.inv_cs;
-  for (int t = 0; t < 2; ++t) {
-    LAUNCH(c, KID_MAP_GRID, k_shard_count, nb, 256, 0, reinterpret_cast<const float*>(subs[t]), 4, n_upper, ns[t], inv_cs, c->shard_rank, c->shard_count, d_blocks);
-    LAUNCH(c, KID_MAP_GRID, k_shard_scan, 1, 1024, 0, d_blocks, nb, d_cnt + t);
-    LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, reinterpret_cast<const float*>(subs[t]), 4, n_upper, ns[t], inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks,
-           c->d_map_pts[t], c->max_map, err_word);
-  }
-  const MapLaneIO io = ctx_map_io(c, c->d_map_pts[0], c->d_map_pts[1]);
-  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, grid_setup_args(io, d_cnt, d_cnt + 1));
+  const float inv_cs = c->map.corner.grid.inv_cs;
+  LAUNCH(c, KID_MAP_GRID, k_shard_count, nb, 256, 0, pts, stride, n, n_dev, inv_cs, c->shard_rank, c->shard_count, d_blocks);
+  LAUNCH(c, KID_MAP_GRID, k_shard_scan, 1, 1024, 0, d_blocks, nb, d_kept + t);
+  LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, pts, stride, n, n_dev, inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks,
+         c->d_map_pts[t], c->max_map, err);
+  return ALOAM_OK;
+}
+
+// K0 over the cut clouds d_map_pts[0] / [1] into the context's set; their sizes are d_kept[0] / [1] on the device
+void shard_index(aloam_ctx* c, const int* d_kept) {
+  const MapLaneIO io = {c->map, {c->d_map_pts[0], c->d_map_pts[1]}, nullptr, nullptr};
+  Batch<GridArgs> g = {};
+  g.a[0] = GridArgs{c->map.corner.grid, io.sub[0], d_kept, c->map.surf.grid, io.sub[1], d_kept + 1};
+  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, g);
   map_index_build(c, 1, &io, c->max_map);
+}
+
+// The end of both map uploads, once the index build is issued.  A rank of a sharded job sums the points in owned cells over the
+// ranks: the thin-map test of laserMapping.cpp:554 is on the WHOLE submap, so every rank takes the same branch (a rank with a
+// thin shard must still meet the others in the all-reduce).  Then the stream is synchronised and the map published.  kept,
+// read after the synchronise: the points indexed on this rank (corner, surf) and the shard's overflow word.
+int finish_map_upload(aloam_ctx* c, const int* kept) {
+  if (c->shard_count > 1) {
+    int* d_two = c->d_stack_counts;   // scratch: a sharded upload has copied its counts out of it before (stream order)
+    CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map.corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map.surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
+    int rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
+    CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
+  }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  prof_collect(c);
+  if (kept[2]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points
+  for (int t = 0; t < 2; ++t) { c->map_n[t] = kept[t]; c->map_global_n[t] = c->shard_count > 1 ? c->pin->owned[t] : kept[t]; }
+  c->have_map = true;
+  return ALOAM_OK;
+}
+}  // namespace
+
+// The mapper of a rank of a sharded job (cubemap.cu): the gathered submap (whole, device-resident, sizes n_sub[0] / [1] on the
+// device) is cut into this rank's x-slabs + halo and indexed, all in stream order -- nothing returns to the host.  An overflow
+// of the shard buffer sets bit 0 of *err_word.
+int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word) {
+  int* d_kept = c->d_stack_counts;    // [0], [1]: points kept per cloud (the mapper keeps its stack counts in its own state)
+  CUDA_CHECK_RET(cudaMemsetAsync(d_kept, 0, 8, c->stream));
+  for (int t = 0; t < 2; ++t) {
+    const int rc = shard_cut(c, t, reinterpret_cast<const float*>(sub[t]), 4, n_upper, n_sub + t, d_kept, err_word);
+    if (rc) return rc;
+  }
+  shard_index(c, d_kept);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
 
 extern "C" {
 
-int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map) {
+int aloam_map_upload(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view surf_map) {
   if (!c) return ALOAM_ERR_INVALID_ARG;
   int rc = check_view(corner_map); if (rc) return rc;
   rc = check_view(surf_map); if (rc) return rc;
@@ -818,27 +841,12 @@ int aloam_map_upload_impl(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud
   }
   GridDyn* hd = c->pin->grid;
   for (int t = 0; t < 2; ++t) { hd[t].n = views[t].n; hd[t].mask = grid_mask_for(views[t].n, (unsigned)c->map_slots); hd[t].cursor = 0; hd[t].owned = 0; }
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->map_corner.grid.dyn, &hd[0], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->map_surf.grid.dyn, &hd[1], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
-  const MapLaneIO io = ctx_map_io(c, src[0], src[1]);
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->map.corner.grid.dyn, &hd[0], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->map.surf.grid.dyn, &hd[1], sizeof(GridDyn), cudaMemcpyHostToDevice, c->stream));
+  const MapLaneIO io = {c->map, {src[0], src[1]}, nullptr, nullptr};
   map_index_build(c, 1, &io, std::max(corner_map.n, surf_map.n));
-  c->map_n[0] = corner_map.n; c->map_n[1] = surf_map.n;
-  c->map_global_n[0] = corner_map.n; c->map_global_n[1] = surf_map.n;
-  if (c->shard_count > 1) {
-    // the thin-map test of laserMapping.cpp:554 is on the WHOLE submap: sum the points in owned cells over the ranks, so
-    // that every rank takes the same branch (a rank with a thin shard must still meet the others in the all-reduce)
-    int* d_two = c->d_stack_counts ? c->d_stack_counts : nullptr;
-    CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map_corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map_surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
-    rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
-  }
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  CUDA_CHECK_RET(cudaGetLastError());
-  if (c->shard_count > 1) { c->map_global_n[0] = c->pin->owned[0]; c->map_global_n[1] = c->pin->owned[1]; }
-  prof_collect(c);
-  c->have_map = true;
-  return ALOAM_OK;
+  const int kept[3] = {corner_map.n, surf_map.n, 0};
+  return finish_map_upload(c, kept);
 }
 
 // aloam_map_upload for a rank of a sharded job that holds the WHOLE submap: the split into owned slabs + halo happens on the
@@ -851,63 +859,38 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   rc = ensure_map_buffers(c); if (rc) return rc;
   const aloam_cloud_view views[2] = {corner_map, surf_map};
-  // host views go through the stack staging buffer (max_points x 16 bytes), a chunk at a time
-  const float inv_cs = c->map_corner.grid.inv_cs;
-  int* d_cnt = c->d_stack_counts;    // [0], [1]: points kept per cloud ; [2]: error word
-  CUDA_CHECK_RET(cudaMemsetAsync(d_cnt, 0, 16, c->stream));
-  int* d_blocks = reinterpret_cast<int*>(c->d_nbr);   // scratch for the block counts (unused outside a registration)
+  int* d_kept = c->d_stack_counts;    // [0], [1]: points kept per cloud ; [2]: error word
+  CUDA_CHECK_RET(cudaMemsetAsync(d_kept, 0, 16, c->stream));
   for (int t = 0; t < 2; ++t) {
+    // a device view is cut in one piece, a host view goes through the corner stack buffer (max_points x 16 bytes) a chunk at a time
     const aloam_cloud_view v = views[t];
     const bool on_device = v.n > 0 && is_device_ptr(v.data);
-    const int chunk = std::max(1, c->max_points * 4 / std::max(v.stride_floats, 4));
-    for (int off = 0; off < v.n; off += on_device ? v.n : chunk) {
-      const int m = on_device ? v.n : std::min(chunk, v.n - off);
-      const float* src;
-      int stride = v.stride_floats;
-      if (on_device) src = v.data;
-      else {
-        CUDA_CHECK_RET(cudaMemcpyAsync(c->d_stack_corner, v.data + (size_t)off * v.stride_floats, (size_t)m * v.stride_floats * 4, cudaMemcpyHostToDevice, c->stream));
-        src = reinterpret_cast<const float*>(c->d_stack_corner);
+    const int chunk = on_device ? v.n : std::max(1, c->max_points * 4 / std::max(v.stride_floats, 4));
+    for (int off = 0; off < v.n; off += chunk) {
+      const int m = std::min(chunk, v.n - off);
+      const float* src = v.data;
+      if (!on_device) {
+        CUDA_CHECK_RET(cudaMemcpyAsync(c->map.stack[0], v.data + (size_t)off * v.stride_floats, (size_t)m * v.stride_floats * 4, cudaMemcpyHostToDevice, c->stream));
+        src = reinterpret_cast<const float*>(c->map.stack[0]);
       }
-      const int nb = (m + 255) / 256;
-      if ((size_t)nb * 4 > (size_t)2 * c->max_points * 5 * sizeof(float4)) return ALOAM_ERR_CAPACITY;
-      LAUNCH(c, KID_MAP_GRID, k_shard_count, nb, 256, 0, src, stride, m, (const int*)nullptr, inv_cs, c->shard_rank, c->shard_count, d_blocks);
-      LAUNCH(c, KID_MAP_GRID, k_shard_scan, 1, 1024, 0, d_blocks, nb, d_cnt + t);
-      LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, src, stride, m, (const int*)nullptr, inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks, c->d_map_pts[t], c->max_map, d_cnt + 2);
+      rc = shard_cut(c, t, src, v.stride_floats, m, nullptr, d_kept, d_kept + 2); if (rc) return rc;
     }
   }
-  const MapLaneIO io = ctx_map_io(c, c->d_map_pts[0], c->d_map_pts[1]);
-  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, grid_setup_args(io, d_cnt, d_cnt + 1));
-  map_index_build(c, 1, &io, c->max_map);
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->shard, d_cnt, 12, cudaMemcpyDeviceToHost, c->stream));
-  if (c->shard_count > 1) {
-    int* d_two = d_cnt + 2;   // reuse after the error word has been copied out (stream order)
-    CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map_corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map_surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
-    rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
-  }
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  CUDA_CHECK_RET(cudaGetLastError());
-  prof_collect(c);
-  if (c->pin->shard[2]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points
-  c->map_n[0] = c->pin->shard[0]; c->map_n[1] = c->pin->shard[1];
-  c->map_global_n[0] = c->shard_count > 1 ? c->pin->owned[0] : c->map_n[0];
-  c->map_global_n[1] = c->shard_count > 1 ? c->pin->owned[1] : c->map_n[1];
-  c->have_map = true;
-  return ALOAM_OK;
+  shard_index(c, d_kept);
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->shard, d_kept, 12, cudaMemcpyDeviceToHost, c->stream));
+  return finish_map_upload(c, c->pin->shard);
 }
 
 static int upload_stacks(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack) {
-  int rc = upload_cloud(c, corner_stack, c->d_stack_corner, c->max_points); if (rc) return rc;
-  rc = upload_cloud(c, surf_stack, c->d_stack_surf, c->max_points); if (rc) return rc;
+  int rc = upload_cloud(c, corner_stack, c->map.stack[0], c->max_points); if (rc) return rc;
+  rc = upload_cloud(c, surf_stack, c->map.stack[1], c->max_points); if (rc) return rc;
   int* sc = c->pin->stack_counts;
   sc[0] = corner_stack.n; sc[1] = surf_stack.n; sc[2] = corner_stack.n + surf_stack.n;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_stack_counts, sc, 12, cudaMemcpyHostToDevice, c->stream));
   return ALOAM_OK;
 }
 
-int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats) {
+int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, double x[7], aloam_stats* stats) {
   if (!c || !x) return ALOAM_ERR_INVALID_ARG;
   if (!c->have_map) return ALOAM_ERR_STATE;
   int rc = check_view(corner_stack); if (rc) return rc;
@@ -921,11 +904,10 @@ int aloam_mapping_register_impl(aloam_ctx* c, aloam_cloud_view corner_stack, alo
   rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  MapLaneIO io = ctx_map_io(c, nullptr, nullptr);
-  io.counts3 = c->d_stack_counts; io.pose = c->d_map_pose;
-  map_register_device(c, 1, &io, corner_stack.n + surf_stack.n, nullptr);
+  const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
+  map_register_device(c, 1, &io, corner_stack.n + surf_stack.n);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->d_map_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->map.summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -947,11 +929,9 @@ int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_c
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   const int nq = corner_stack.n + surf_stack.n;
-  if (nq > 0) {
-    Batch<MapAssocArgs> a = {};
-    a.a[0] = MapAssocArgs{c->d_stack_corner, c->d_stack_surf, c->d_stack_counts, c->map_corner, c->map_surf, c->d_map_pose, c->d_nbr, c->d_map_blocks, c->d_fits};
-    LAUNCH(c, KID_MAP_KNN5, k_map_knn5, std::min((nq + 7) / 8, grid_ctas(c)), 256, 0, a, c->shard_rank, c->shard_count);
-    LAUNCH(c, KID_MAP_FIT, k_map_fit, (nq + 31) / 32, 32, 0, a);
+  if (nq > 0) {   // the launches of one outer iteration of aloam_mapping_register
+    const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
+    map_associate_device(c, 1, &io, nq, false, c->d_fits);
     CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
@@ -965,7 +945,7 @@ int aloam_map_knn_impl(aloam_ctx* c, int which, aloam_cloud_view queries, int k,
   int rc = upload_cloud(c, queries, c->d_query, c->max_points); if (rc) return rc;
   if (queries.n > 0) {
     if ((size_t)queries.n * k > (size_t)c->max_points) return ALOAM_ERR_CAPACITY;
-    LAUNCH(c, KID_MAP_KNN, k_map_knn, (queries.n + 7) / 8, 256, 0, which == 2 ? c->map_corner : c->map_surf, c->d_query, queries.n, k,
+    LAUNCH(c, KID_MAP_KNN, k_map_knn, (queries.n + 7) / 8, 256, 0, which == 2 ? c->map.corner : c->map.surf, c->d_query, queries.n, k,
            c->d_knn_idx, c->d_knn_d);
     CUDA_CHECK_RET(cudaMemcpyAsync(idx, c->d_knn_idx, (size_t)queries.n * k * 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(sqdist, c->d_knn_d, (size_t)queries.n * k * 4, cudaMemcpyDeviceToHost, c->stream));

@@ -160,7 +160,7 @@ def test_mapper_launches_are_shared_by_all_lanes(aloam, synth):
     for B in (1, 2, 4):
         mapped = _ctx(aloam, 16, maxn, 4096, B)
         odo = aloam.Aloam(n_scans=16, max_points=maxn + 1024, max_batch=B, max_ring_points=4096)
-        # a first call creates the lanes (a first frame of lane 0 also indexes the empty host-API map): count the second
+        # a first call creates the lanes (and, for B = 1, the context's map buffers that lane 0 shares): count the second
         mapped.scan_stream_mapped_batch(ptrs[:, :B], counts[:, :B], True)
         odo.scan_stream_batch(ptrs[:, :B], counts[:, :B], True)
         l0 = mapped.launch_count()

@@ -128,6 +128,52 @@ def test_map_upload_accepts_device_memory(aloam, scene):
     c.close()
 
 
+def _same_bits(a, b):
+    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+    return a.shape == b.shape and a.dtype == b.dtype and np.array_equal(a.view(np.uint8), b.view(np.uint8))
+
+
+def test_sharded_upload_on_one_rank_equals_map_upload(aloam, scene):
+    """without a communicator this rank owns every cell, so aloam_map_upload_sharded cuts nothing away: host views of 4 and
+    8 floats per point, streamed through the stack buffer a chunk at a time, and a device view index what aloam_map_upload
+    indexes -- the same neighbours, fits and registered pose, bit for bit"""
+    import torch
+    cmap, smap, cs, ss, x0, _ = scene
+    mp = 3500   # upload chunks of 3500 (4 floats per point) or 1750 (8 floats) points: both maps span several, the stacks fit
+    assert max(len(cs), len(ss)) <= mp < min(len(cmap), len(smap))
+    R = _rot(x0[:4])
+    queries = []
+    for q in (cs[:mp // 5], ss[:mp // 5]):   # k = 5 neighbours of at most max_points / 5 queries
+        qw = q.copy(); qw[:, :3] = (q[:, :3].astype(np.float64) @ R.T + x0[4:]).astype(np.float32)
+        queries.append(qw)
+
+    def run(upload):
+        c = aloam.Aloam(n_scans=64, max_points=mp, max_map_points=16384)
+        upload(c)
+        out = [*c.knn(2, queries[0], 5), *c.knn(3, queries[1], 5), c.mapping_associate(cs, ss, x0), c.mapping_register(cs, ss, x0)[0]]
+        c.close()
+        return out
+
+    def wide(a):
+        w = np.full((len(a), 8), -7.0, np.float32)
+        w[:, :4] = a
+        return w
+
+    dc, ds = (torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in (cmap, smap))
+    ref = run(lambda c: c.map_upload(cmap, smap))
+    for upload in (lambda c: c.map_upload_sharded(cmap, smap),
+                   lambda c: c.map_upload_sharded(wide(cmap), wide(smap)),
+                   lambda c: c.map_upload_sharded_ptr(dc.data_ptr(), len(cmap), ds.data_ptr(), len(smap))):
+        got = run(upload)
+        for g, r in zip(got[:4], ref[:4]):
+            assert _same_bits(g, r)
+        fits, ref_fits = got[4], ref[4]
+        assert _same_bits(fits[:, 1], ref_fits[:, 1])
+        acc = ref_fits[:, 1] >= 0   # the record of a rejected query is written only in part
+        assert acc.sum() > 1000 and _same_bits(fits[acc], ref_fits[acc])
+        assert _same_bits(got[5], ref[5])
+
+
 # ---- the single-cloud filter at its size limits: > 1024 blocks of 1024 keys (k_vox_blockscan strides), voxel indices of 1 to
 # 4 bytes (the sort always runs 4 passes over the 32-bit key; all-zero high digits leave a stable sort unchanged), runs across
 # blocks, clouds near +-5 km
