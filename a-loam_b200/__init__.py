@@ -24,7 +24,7 @@ EXPORTED_SYMBOLS = [
     "aloam_odometry_associate", "aloam_normal_equations", "aloam_solve", "aloam_debug_features", "aloam_mapping_associate",
     "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_debug_seg_voxel_filter", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
     "aloam_scan_stream_mapped_batch", "aloam_mapper_debug_state_lane", "aloam_mapper_debug_cube_lane",
-    "aloam_scan_stream_lanes",
+    "aloam_scan_stream_lanes", "aloam_debug_shard_emulate", "aloam_debug_map_sizes",
 ]
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 
@@ -112,6 +112,8 @@ def lib():
         L.aloam_mapping_associate.argtypes = [C.c_void_p, cv, cv, dp, dp]
         L.aloam_comm_unique_id.argtypes = [C.c_char_p]
         L.aloam_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p]
+        L.aloam_debug_shard_emulate.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.aloam_debug_map_sizes.argtypes = [C.c_void_p, ip, ip]
         _LIB = L
     return _LIB
 
@@ -318,6 +320,17 @@ class Aloam:
 
     def comm_init(self, rank, world, unique_id):
         _check(lib().aloam_comm_init(self._h, rank, world, C.create_string_buffer(bytes(unique_id), 128)))
+
+    def debug_shard_emulate(self, rank, world, exchange=0, poison_peer_err=False):
+        """test hook: act as rank `rank` of `world` without a communicator, the LM all-reduce a loopback through `exchange`
+        (0 k_lm_solve, 1 per-evaluation kernels, 2 one-rank peer mailbox); world = 0 ends the emulation"""
+        _check(lib().aloam_debug_shard_emulate(self._h, int(rank), int(world), int(exchange), int(bool(poison_peer_err))))
+
+    def debug_map_sizes(self):
+        """(points indexed on this rank, submap size of the thin-map test), each (corner, surf)"""
+        kept = (C.c_int * 2)(); glob = (C.c_int * 2)()
+        _check(lib().aloam_debug_map_sizes(self._h, kept, glob))
+        return (kept[0], kept[1]), (glob[0], glob[1])
 
     def comm_uses_peer_memory(self):
         lib().aloam_comm_uses_peer_memory.argtypes = [C.c_void_p]

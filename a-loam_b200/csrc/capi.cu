@@ -528,8 +528,10 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     return code;
   };
 #define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return fail(ALOAM_ERR_CUDA); } } while (0)
-  if (map_poses)   // the mappers' error bits of this call
+  if (map_poses) {   // the mappers' error bits of this call
     for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
+    const int rc = peer_err_reset(c); if (rc) return fail(rc);
+  }
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
   // everything issued on the main stream before this call (reset, earlier calls) is ordered before the side streams.
   // Waiting on an event that was never recorded, or whose work finished in an earlier call, is a no-op -- so the
@@ -648,6 +650,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapdone[c->cur], 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+    const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return fail(rc);
   }
   for (int l = 0; l < nb; ++l) {
     STREAM_TRY(cudaMemcpyAsync(c->h_summary + 4 * l, c->lanes[l].d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, s_main));
@@ -684,6 +687,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     c->pin->mapper_err = 0;
     for (int l = 0; l < nb; ++l) c->pin->mapper_err |= c->pin->mapper_err_lane[l];
     if (c->pin->mapper_err & 1) return ALOAM_ERR_CAPACITY;
+    if (c->pin->peer_err) return ALOAM_ERR_COMM;   // a peer did not answer: a map pose rests on a partial sum
   }
   return ALOAM_OK;
 }
@@ -728,14 +732,14 @@ int aloam_scan_stream_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
 int aloam_scan_stream_mapped_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* odom_poses,
                                    double* map_poses, aloam_stats* stats_last) {
   if (!map_poses) return ALOAM_ERR_INVALID_ARG;
-  if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  if (c && (c->shard_count > 1 || c->shard_exchange >= 0)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   return scan_stream_lockstep(c, raws, n_scans, batch, device_resident, odom_poses, map_poses, stats_last);
 }
 
 int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch, int device_resident,
                             double* odom_poses, double* map_poses, aloam_stats* stats_last) {
   if (!lane_ops) return ALOAM_ERR_INVALID_ARG;
-  if (c && c->shard_count > 1) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  if (c && (c->shard_count > 1 || c->shard_exchange >= 0)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   if (!stream_args_ok(c, raws, n_scans, batch, odom_poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
   // the whole schedule is checked against the lanes' state before anything changes; lanes >= batch are idle all call
   bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call
@@ -823,8 +827,16 @@ static int run_lm_api(aloam_ctx* c, const double* blocks, int n_blocks, const do
   }
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  launch_lm(c, false, (const BlockRec*)L.d_blocks, (const int*)nullptr, n_blocks, c->d_api_pose, lm_params(c->cfg), L.d_summary, mode,
-            c->d_out28, (double*)nullptr, 0, true /* blocks from the caller may carry any interpolation ratio */);
+  if (mode == 0 && c->shard_exchange > 0) {
+    // a context emulating a rank (aloam_debug_shard_emulate) solves through the sharded solve of the scan-to-map path, which
+    // reads the block count from device memory: a stream call's scan sizes are scratch during this synchronous call
+    c->pin->query_counts[0] = n_blocks;
+    CUDA_CHECK_RET(cudaMemcpyAsync(c->d_scan_nfull, c->pin->query_counts, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    launch_lm_sharded(c, L.d_blocks, c->d_scan_nfull, c->d_api_pose, lm_params(c->cfg), L.d_summary);
+  } else {
+    launch_lm(c, false, (const BlockRec*)L.d_blocks, (const int*)nullptr, n_blocks, c->d_api_pose, lm_params(c->cfg), L.d_summary, mode,
+              c->d_out28, (double*)nullptr, 0, true /* blocks from the caller may carry any interpolation ratio */);
+  }
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->ne, c->d_out28, 28 * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary), cudaMemcpyDeviceToHost, c->stream));

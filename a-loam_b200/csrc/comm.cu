@@ -45,7 +45,22 @@ struct PeerState {
   PeerX px = {};
   void* own = nullptr;                 // this rank's mailbox allocation (boxes, flags, counter, totals, error word)
   void* opened[ALOAM_MAX_RANKS] = {};  // peers' mailboxes mapped into this process (cudaIpcOpenMemHandle)
+  int poison = 0;                      // test hook: the next peer_err_reset writes 1 instead of 0
 };
+
+// a rank's mailbox allocation in a world of `world` ranks: boxes [2 parities][world][32][2] words, flags [2][world], the
+// evaluation counter (64 B), the totals [2][32] and the error word (64 B)
+static size_t mailbox_box_bytes(int world) { return (size_t)2 * world * 32 * 2 * sizeof(unsigned long long); }
+static size_t mailbox_flag_bytes(int world) { return (size_t)2 * world * sizeof(unsigned); }
+static size_t mailbox_bytes(int world) { return mailbox_box_bytes(world) + mailbox_flag_bytes(world) + 64 + 2 * 32 * sizeof(double) + 64; }
+// points the counter, totals and error word of ps->px into this rank's own (zeroed) mailbox
+static void mailbox_locals(PeerState* ps, int rank, int world) {
+  char* mbox = static_cast<char*>(ps->own) + mailbox_box_bytes(world) + mailbox_flag_bytes(world);
+  ps->px.seq = reinterpret_cast<unsigned long long*>(mbox);
+  ps->px.gtot = reinterpret_cast<double*>(mbox + 64);
+  ps->px.err = reinterpret_cast<int*>(mbox + 64 + 2 * 32 * sizeof(double));
+  ps->px.rank = rank; ps->px.world = world;
+}
 
 // unmaps the peers' mailboxes, frees this rank's and forgets the peer state (back to the NCCL path)
 static void peer_drop(aloam_ctx* c) {
@@ -86,8 +101,12 @@ void launch_lm_sharded(aloam_ctx* c, const BlockRec* blocks, const int* d_n, dou
     cfg.attrs = at; cfg.numAttrs = 1;
     cudaLaunchKernelEx(&cfg, k_lm_eval_shard, blocks, d_n, (const double*)pose, c->d_lm_state, first, lp.huber_a, local);
     prof_end(c);
-    ncclResult_t r = g_nccl.AllReduce(local, c->d_lm_tot, 32, ncclDouble, ncclSum, (ncclComm_t)c->comm, c->stream);
-    if (r != ncclSuccess) fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
+    if (c->shard_exchange == 1) {   // an emulated rank: the sum over one rank
+      cudaMemcpyAsync(c->d_lm_tot, local, 32 * sizeof(double), cudaMemcpyDeviceToDevice, c->stream);
+    } else {
+      ncclResult_t r = g_nccl.AllReduce(local, c->d_lm_tot, 32, ncclDouble, ncclSum, (ncclComm_t)c->comm, c->stream);
+      if (r != ncclSuccess) fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
+    }
     LAUNCH(c, KID_LM_SHARD, k_lm_tr_shard, 1, 32, 0, c->d_lm_state, (const double*)c->d_lm_tot, pose, first, last, lp, summary);
   }
 }
@@ -99,8 +118,7 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
   PeerState* ps = new (std::nothrow) PeerState();
   if (!ps) return false;
   c->peer = ps;
-  const size_t box_bytes = (size_t)2 * world * 32 * 2 * sizeof(unsigned long long), flag_bytes = (size_t)2 * world * sizeof(unsigned);
-  const size_t total = box_bytes + flag_bytes + 64 + 2 * 32 * sizeof(double) + 64;
+  const size_t box_bytes = mailbox_box_bytes(world), total = mailbox_bytes(world);
   bool ok = cudaMalloc(&ps->own, total) == cudaSuccess && cudaMemset(ps->own, 0, total) == cudaSuccess;
   cudaIpcMemHandle_t mine;
   ok = ok && cudaIpcGetMemHandle(&mine, ps->own) == cudaSuccess;
@@ -134,24 +152,70 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
     fprintf(stderr, "[aloam_b200] peer-memory exchange unavailable on rank %d: the sharded LM uses ncclAllReduce\n", rank);
     return false;
   }
-  char* mbox = static_cast<char*>(ps->own);
-  ps->px.seq = reinterpret_cast<unsigned long long*>(mbox + box_bytes + flag_bytes);
-  ps->px.gtot = reinterpret_cast<double*>(mbox + box_bytes + flag_bytes + 64);
-  ps->px.err = reinterpret_cast<int*>(mbox + box_bytes + flag_bytes + 64 + 2 * 32 * sizeof(double));
-  ps->px.rank = rank; ps->px.world = world;
+  mailbox_locals(ps, rank, world);
   own(c, [c] { peer_drop(c); });
   return true;
 }
 
 // sum of two ints over the ranks, in place (global submap sizes for the thin-map test, mapping.cu)
 int comm_allreduce_int2(aloam_ctx* c, int* d_two) {
-  if (c->shard_count <= 1) return ALOAM_OK;
+  if (c->shard_count <= 1 || c->shard_exchange >= 0) return ALOAM_OK;   // one rank, or an emulated one: the identity
   ncclResult_t r = g_nccl.AllReduce(d_two, d_two, 2, ncclInt32, ncclSum, (ncclComm_t)c->comm, c->stream);
   if (r != ncclSuccess) { fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?"); return ALOAM_ERR_COMM; }
   return ALOAM_OK;
 }
 
+int peer_err_reset(aloam_ctx* c) {
+  PeerState* ps = static_cast<PeerState*>(c->peer);
+  if (!ps) return ALOAM_OK;
+  static const int kOne = 1;
+  if (ps->poison) CUDA_CHECK_RET(cudaMemcpyAsync(ps->px.err, &kOne, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  else CUDA_CHECK_RET(cudaMemsetAsync(ps->px.err, 0, sizeof(int), c->stream));
+  ps->poison = 0;
+  return ALOAM_OK;
+}
+
+int peer_err_fetch(aloam_ctx* c, int* dst) {
+  *dst = 0;
+  const PeerState* ps = static_cast<const PeerState*>(c->peer);
+  if (ps) CUDA_CHECK_RET(cudaMemcpyAsync(dst, ps->px.err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  return ALOAM_OK;
+}
+
 extern "C" {
+
+int aloam_debug_shard_emulate(aloam_ctx* c, int rank, int world, int exchange, int poison_peer_err) {
+  if (!c) return ALOAM_ERR_INVALID_ARG;
+  if (c->comm) return ALOAM_ERR_STATE;
+  if (world < 0 || (world > 0 && (rank < 0 || rank >= world || exchange < 0 || exchange > 2)) || (poison_peer_err && (world == 0 || exchange != 2)))
+    return ALOAM_ERR_INVALID_ARG;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  if (world > 0) {   // what the sharded LM needs, created on first use (a failure changes no setting)
+    if (!c->d_lm_tot) CUDA_CHECK_RET(dalloc(c, &c->d_lm_tot, 64));
+    if (!c->d_lm_state) CUDA_CHECK_RET(dalloc(c, reinterpret_cast<char**>(&c->d_lm_state), lm_state_bytes()));
+  }
+  if (world == 0 || exchange != 2) {
+    peer_drop(c);
+  } else if (!c->peer) {   // a one-rank mailbox laid out as peer_setup's, without the IPC handles and their gather
+    PeerState* ps = new (std::nothrow) PeerState();
+    if (!ps) return ALOAM_ERR_CUDA;
+    c->peer = ps;
+    own(c, [c] { peer_drop(c); });
+    if (cudaMalloc(&ps->own, mailbox_bytes(1)) != cudaSuccess || cudaMemsetAsync(ps->own, 0, mailbox_bytes(1), c->stream) != cudaSuccess) {
+      cudaGetLastError();
+      peer_drop(c);
+      return ALOAM_ERR_CUDA;
+    }
+    ps->px.box[0] = static_cast<double*>(ps->own);
+    ps->px.flag[0] = reinterpret_cast<unsigned*>(static_cast<char*>(ps->own) + mailbox_box_bytes(1));
+    mailbox_locals(ps, 0, 1);
+  }
+  if (poison_peer_err) static_cast<PeerState*>(c->peer)->poison = 1;
+  const int new_rank = world ? rank : 0, new_count = world ? world : 1;
+  if (new_rank != c->shard_rank || new_count != c->shard_count) c->have_map = false;   // the map was cut for another rank
+  c->shard_rank = new_rank; c->shard_count = new_count; c->shard_exchange = world ? exchange : -1;
+  return ALOAM_OK;
+}
 
 // rank 0 creates the 128-byte NCCL id; the caller ships it to the other ranks (e.g. torch.distributed.broadcast)
 int aloam_comm_unique_id(char out128[128]) {
@@ -169,6 +233,7 @@ int aloam_comm_unique_id(char out128[128]) {
 // (owned slabs + one-cell halo; see a-loam_b200/shard.py for the host-side split).
 int aloam_comm_init(aloam_ctx* c, int rank, int world, const char id128[128]) {
   if (!c || !id128 || world < 1 || rank < 0 || rank >= world) return ALOAM_ERR_INVALID_ARG;
+  if (c->shard_exchange >= 0) return ALOAM_ERR_STATE;   // emulating a rank (aloam_debug_shard_emulate)
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (world == 1) { c->shard_rank = 0; c->shard_count = 1; return ALOAM_OK; }
   if (!load_nccl()) return ALOAM_ERR_COMM;

@@ -97,6 +97,7 @@ struct PinnedScratch {
   int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
   int mapper_err;           // aloam_scan_stream_mapped: the mapper's error bits, OR over the call's frames
   int mapper_err_lane[ALOAM_MAX_BATCH];   // aloam_scan_stream_mapped_batch: the same per lane
+  int peer_err;             // sharded registration / mapper frames: the peer exchange's error word
   SegDesc vox_seg;          // aloam_voxel_filter: the cloud as the one segment of its filter
   int vox_nseg;             //                     1
   int vox_io[3];            //                     cloud size, filtered size, error word: {n, 0, 0}
@@ -129,6 +130,8 @@ struct aloam_ctx {
   float* d_knn_d = nullptr;
   // multi-GPU sharding of the map (spatial slabs + halo, SURVEY.md 8e): this process's rank / world and its communicator
   int shard_rank = 0, shard_count = 1;
+  int shard_exchange = -1;       // >= 0: this context emulates rank shard_rank of shard_count without a communicator (test hook
+                                 // aloam_debug_shard_emulate), its LM all-reduce a loopback: 0 k_lm_solve, 1 per evaluation, 2 peer
   void* comm = nullptr;          // ncclComm_t when shard_count > 1 (comm.cu)
   void* peer = nullptr;          // peer-memory exchange of the sharded LM (comm.cu), when enabled
   double* d_lm_tot = nullptr;    // [64] all-reduced normal equations of one evaluation (sharded LM)
@@ -260,6 +263,10 @@ inline void launch_lm(aloam_ctx* c, bool pdl, const BlockRec* blocks, const int*
 }  // namespace
 // sharded LM (comm.cu): per evaluation one kernel for the local blocks, one exchange of 32 doubles, one step kernel
 void launch_lm_sharded(aloam_ctx* c, const aloam::BlockRec* blocks, const int* d_n, double* pose, const aloam::LmParams& lp, aloam::LmSummary* summary);
+// the error word of the peer exchange (a peer that did not answer in time), on c->stream: cleared at the start of every call
+// that registers against a sharded map, copied to pinned *dst with its pose (*dst = 0 without the peer exchange)
+int peer_err_reset(aloam_ctx* c);
+int peer_err_fetch(aloam_ctx* c, int* dst);
 void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper);
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
@@ -271,6 +278,10 @@ void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
 void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper);
 namespace {
+
+// the scan-to-map LM goes through launch_lm_sharded: on a rank of a sharded job, and on a context that emulates a rank with
+// exchange 1 or 2
+inline bool sharded_lm(const aloam_ctx* c) { return c->shard_exchange < 0 ? c->shard_count > 1 : c->shard_exchange > 0; }
 
 LmParams lm_params(const aloam_config& c) {
   LmParams p;

@@ -528,7 +528,7 @@ int ensure_mapper(aloam_ctx* c, int lane) {
 // runs on and whether that store starts a fresh trajectory; n_upper_* bound the cloud sizes of every lane.  Lane 0 registers
 // with the context's set, shared with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
-  if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && c->shard_count > 1)) return ALOAM_ERR_STATE;
+  if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && (c->shard_count > 1 || c->shard_exchange >= 0))) return ALOAM_ERR_STATE;
   int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's auxiliary stream carries the stack filters of every lane
   for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
   rc = ensure_map_buffers(c); if (rc) return rc;     // lane 0's set
@@ -645,9 +645,11 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   for (int k = 0; k < 3; ++k) c->pin->mapper_pose_in[4 + k] = t_wodom_curr[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->pin->mapper_pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   const MapperIn one{m->d_in[0], &m->d_state->in_counts[0], m->d_in[1], &m->d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7, 0, 0};
+  rc = peer_err_reset(c); if (rc) return rc;
   rc = mapper_step_device(c, 1, &one, corner_last.n, surf_last.n);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
+  rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, m->reg->summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(&m->h_state->flags, &m->d_state->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
@@ -660,6 +662,7 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   if (m->h_state->flags & ALOAM_FLAG_MAP_TOO_THIN) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = m->h_state->flags; stats->ms_total = ms; } }
   else fill_stats(c, stats, c->cfg.outer_iters, m->h_state->flags, ms);
   if (m->h_state->frame_err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
+  if (c->pin->peer_err) return ALOAM_ERR_COMM;                // a peer did not answer: the pose rests on a partial sum
   return ALOAM_OK;
 }
 

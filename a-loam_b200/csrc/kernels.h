@@ -169,7 +169,8 @@ struct LmArgs { const BlockRec* blocks; const int* n_blocks_ptr; int n_blocks_ho
 // Sharded solve over NVLink peer memory (multi-GPU scan-to-map, comm.cu): every rank's LM cluster pushes its 32 partial sums
 // into a mailbox in EVERY rank's memory (peer stores through NVSwitch), raises a flag there, waits for the flags of all ranks
 // in its own mailbox and adds the contributions in rank order -- the all-reduce of the normal equations happens INSIDE the
-// solve kernel, one launch per solve, no kernel boundary around the 256-byte exchange.  world <= 1: no exchange.
+// solve kernel, one launch per solve, no kernel boundary around the 256-byte exchange.  world 0: no exchange; world 1 (never a
+// real job: aloam_comm_init keeps a one-rank world off the sharded path) is the loopback of a context emulating a rank.
 #define ALOAM_MAX_RANKS 16
 struct PeerX {
   double* box[ALOAM_MAX_RANKS];             // mailbox of rank r: [2 parities][world][32][2] 8-byte words {payload half, tag} (peer-mapped device memory)

@@ -654,12 +654,12 @@ __device__ __forceinline__ void lm_solve_body(const Batch<LmArgs>& B, const LmPa
   // one evaluation site (the evaluation body is large; duplicating it costs instruction-cache misses)
   bool first = true;
   long long cyc_eval = 0, cyc_tr = 0, cyc_blocks = 0, cyc_barrier = 0;
-  const unsigned long long seq0 = (GENERAL && px.world > 1) ? *px.seq : 0ull;
+  const unsigned long long seq0 = (GENERAL && px.world >= 1) ? *px.seq : 0ull;
   do {
     const long long c0 = clock64();
     double* tot = s_tot[first ? 0 : 1 - T.acc_buf];
     cluster_evaluate<GENERAL>(cluster, blocks, n, rb0, first ? s_x : T.xc, prm.huber_a, s_red, s_part, s_in, tot, pass, cyc_blocks, cyc_barrier);
-    if (GENERAL && px.world > 1) peer_allreduce(cluster, px, seq0 + (unsigned long long)pass, tot);   // pass was advanced: tags start at seq0 + 1
+    if (GENERAL && px.world >= 1) peer_allreduce(cluster, px, seq0 + (unsigned long long)pass, tot);   // pass was advanced: tags start at seq0 + 1
     const long long c1 = clock64();
     cyc_eval += c1 - c0;
     if (first && mode == 1) {
@@ -686,7 +686,7 @@ __device__ __forceinline__ void lm_solve_body(const Batch<LmArgs>& B, const LmPa
     cyc_tr += clock64() - c1;
   } while (T.go);
   if (writer) {
-    if (GENERAL && px.world > 1) *px.seq = seq0 + (unsigned long long)pass;
+    if (GENERAL && px.world >= 1) *px.seq = seq0 + (unsigned long long)pass;
     tr_finish(T, x7, summary, s_trace);
     summary->cyc_total = clock64() - clk0;
     summary->cyc_eval = cyc_eval;

@@ -40,9 +40,12 @@ __device__ __forceinline__ unsigned hash_key(unsigned long long k) {
   return (unsigned)k;
 }
 __device__ __forceinline__ int cell_of(float v, float inv_cs) { return (int)floorf(v * inv_cs); }
+// floor division and a non-negative remainder, as shard.py's owner_of_cell: a cell left of x = -2^20 m still has an owner
 __device__ __forceinline__ int owner_of(int cx, int count) {
-  int slab = (cx + (1 << 20)) / kSlab;
-  return slab % count;
+  const int v = cx + (1 << 20);
+  const int slab = (v < 0 ? v - (kSlab - 1) : v) / kSlab;
+  const int r = slab % count;
+  return r < 0 ? r + count : r;
 }
 __device__ __forceinline__ unsigned long long slot_key(const uint4& s) { return ((unsigned long long)s.y << 32) | s.x; }
 __device__ __forceinline__ unsigned table_mask_for(int n) {   // next power of two >= 1.25 n (>= 1024), minus one
@@ -213,7 +216,8 @@ __global__ void __launch_bounds__(256) k_shard_count(const float* __restrict__ p
   const int c = __syncthreads_count(keep);
   if (threadIdx.x == 0) block_cnt[blockIdx.x] = c;
 }
-__global__ void __launch_bounds__(1024) k_shard_scan(int* __restrict__ block_cnt, int nblocks, int* __restrict__ base_total) {
+// *base_total ends clamped to cap: the points k_shard_scatter cannot store (it flags them) never reach the index build
+__global__ void __launch_bounds__(1024) k_shard_scan(int* __restrict__ block_cnt, int nblocks, int* __restrict__ base_total, int cap) {
   __shared__ int s_w[32];
   __shared__ int s_carry;
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
@@ -235,7 +239,7 @@ __global__ void __launch_bounds__(1024) k_shard_scan(int* __restrict__ block_cnt
     if (t == 1023) s_carry = carry + wb + incl;
     __syncthreads();
   }
-  if (t == 0) *base_total = s_carry;
+  if (t == 0) *base_total = min(s_carry, cap);
 }
 __global__ void __launch_bounds__(256) k_shard_scatter(const float* __restrict__ pts, int stride, int n, const int* __restrict__ n_ptr, float inv_cs, int rank, int world,
                                                        const int* __restrict__ block_off, Pt4* __restrict__ out, int cap, int* __restrict__ err) {
@@ -749,7 +753,7 @@ void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper
   const LmParams lp = lm_params(c->cfg);
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
     map_associate_device(c, nb, io, nq_upper, it > 0, nullptr);
-    if (c->shard_count <= 1) {
+    if (!sharded_lm(c)) {
       Batch<LmArgs> lm = {};
       for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
       launch_lm_batch(c, true, lm, nb, lp, 0, 0);
@@ -769,7 +773,7 @@ int shard_cut(aloam_ctx* c, int t, const float* pts, int stride, int n, const in
   if ((size_t)nb * 4 > (size_t)2 * c->max_points * 5 * sizeof(float4)) return ALOAM_ERR_CAPACITY;
   const float inv_cs = c->map.corner.grid.inv_cs;
   LAUNCH(c, KID_MAP_GRID, k_shard_count, nb, 256, 0, pts, stride, n, n_dev, inv_cs, c->shard_rank, c->shard_count, d_blocks);
-  LAUNCH(c, KID_MAP_GRID, k_shard_scan, 1, 1024, 0, d_blocks, nb, d_kept + t);
+  LAUNCH(c, KID_MAP_GRID, k_shard_scan, 1, 1024, 0, d_blocks, nb, d_kept + t, c->max_map);
   LAUNCH(c, KID_MAP_GRID, k_shard_scatter, nb, 256, 0, pts, stride, n, n_dev, inv_cs, c->shard_rank, c->shard_count, (const int*)d_blocks,
          c->d_map_pts[t], c->max_map, err);
   return ALOAM_OK;
@@ -799,7 +803,7 @@ int finish_map_upload(aloam_ctx* c, const int* kept) {
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   prof_collect(c);
-  if (kept[2]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points
+  if (kept[2]) return ALOAM_ERR_CAPACITY;   // the shard does not fit cfg.max_map_points: the index holds a part of it, have_map stays false
   for (int t = 0; t < 2; ++t) { c->map_n[t] = kept[t]; c->map_global_n[t] = c->shard_count > 1 ? c->pin->owned[t] : kept[t]; }
   c->have_map = true;
   return ALOAM_OK;
@@ -831,6 +835,7 @@ int aloam_map_upload(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cloud_view
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   rc = ensure_map_buffers(c); if (rc) return rc;
   if (corner_map.n > c->max_map || surf_map.n > c->max_map) return ALOAM_ERR_CAPACITY;
+  c->have_map = false;   // from here on the index is being rebuilt: published again by finish_map_upload
   // a 16-byte-stride cloud that already lives in device memory is indexed in place (the views are only borrowed for
   // the duration of this call: after the build nothing refers to the caller's memory, the cell-sorted copy is complete)
   const aloam_cloud_view views[2] = {corner_map, surf_map};
@@ -858,6 +863,7 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
   rc = ensure_map_buffers(c); if (rc) return rc;
+  c->have_map = false;   // from here on the index is being rebuilt: published again by finish_map_upload
   const aloam_cloud_view views[2] = {corner_map, surf_map};
   int* d_kept = c->d_stack_counts;    // [0], [1]: points kept per cloud ; [2]: error word
   CUDA_CHECK_RET(cudaMemsetAsync(d_kept, 0, 16, c->stream));
@@ -879,6 +885,13 @@ int aloam_map_upload_sharded(aloam_ctx* c, aloam_cloud_view corner_map, aloam_cl
   shard_index(c, d_kept);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->shard, d_kept, 12, cudaMemcpyDeviceToHost, c->stream));
   return finish_map_upload(c, c->pin->shard);
+}
+
+int aloam_debug_map_sizes(aloam_ctx* c, int kept[2], int global[2]) {
+  if (!c || !kept || !global) return ALOAM_ERR_INVALID_ARG;
+  if (!c->have_map) return ALOAM_ERR_STATE;
+  for (int t = 0; t < 2; ++t) { kept[t] = c->map_n[t]; global[t] = c->map_global_n[t]; }
+  return ALOAM_OK;
 }
 
 static int upload_stacks(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack) {
@@ -904,10 +917,12 @@ int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cl
   rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
+  rc = peer_err_reset(c); if (rc) return rc;
   const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
   map_register_device(c, 1, &io, corner_stack.n + surf_stack.n);
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->map.summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
+  rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -915,7 +930,7 @@ int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cl
   for (int k = 0; k < 7; ++k) x[k] = c->pin->pose_out[k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   fill_stats(c, stats, c->cfg.outer_iters, 0, ms);
-  return ALOAM_OK;
+  return c->pin->peer_err ? ALOAM_ERR_COMM : ALOAM_OK;   // a peer did not answer: the pose rests on a partial sum
 }
 
 // association only (tests): fits = (n_corner + n_surf) x 14 doubles [query, type (-1 rejected), p0(3), p1(3), d, nn(5)]

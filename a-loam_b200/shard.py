@@ -16,6 +16,7 @@ def cell_x(x):
 
 
 def owner_of_cell(cx, world):
+    """floor division and a non-negative remainder (Python semantics), as owner_of() on the device for every cell"""
     return ((np.asarray(cx, np.int64) + (1 << 20)) // SLAB) % world
 
 

@@ -286,17 +286,35 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* ctx, const aloam_cloud_view* segs, c
  * after aloam_comm_init each rank uploads only ITS shard of the submap (x-slabs of aloam_shard_slab_cells() cells of
  * 1.00001 m, owner = slab mod world, plus one cell of halo) and aloam_mapping_register fits only the stack points
  * whose cell the rank owns; the ranks meet in one ncclAllReduce of the 6x6 / 6x1 normal equations per evaluation and
- * return the identical pose. */
+ * return the identical pose.  On the peer-memory exchange a peer that does not answer within about 2 s makes
+ * aloam_mapping_register, aloam_mapper_step and aloam_scan_stream_mapped return ALOAM_ERR_COMM (after writing the pose). */
 int aloam_comm_unique_id(char out128[128]);
 int aloam_comm_init(aloam_ctx* ctx, int rank, int world, const char id128[128]);
 int aloam_shard_slab_cells(void);
 /* as aloam_map_upload, for a rank that holds the WHOLE submap (host or device memory): the rank's shard -- its x-slabs plus the
- * one-cell halo -- is cut out on the device (stable compaction), then indexed.  cfg.max_map_points must hold the shard. */
+ * one-cell halo -- is cut out on the device (stable compaction), then indexed.  cfg.max_map_points must hold the shard: a larger
+ * shard returns ALOAM_ERR_CAPACITY and leaves the context without a map (aloam_mapping_register returns ALOAM_ERR_STATE). */
 int aloam_map_upload_sharded(aloam_ctx* ctx, aloam_cloud_view corner_map, aloam_cloud_view surf_map);
 /* 1 when the ranks exchange the normal equations through NVLink peer memory INSIDE the LM kernel (one launch per solve; CUDA IPC
  * mailboxes set up by aloam_comm_init), 0 when they use ncclAllReduce between per-evaluation kernels (no peer access, or the
  * environment variable ALOAM_NO_PEER is set -- kept for A/B measurements). */
 int aloam_comm_uses_peer_memory(aloam_ctx* ctx);
+/* Test hook: one context behaves as rank `rank` of `world` without a communicator, so the sharded path can be checked on one
+ * GPU.  aloam_map_upload_sharded cuts this rank's shard, the index build counts its owned points, the 5-NN rejects queries in
+ * cells it does not own, and aloam_mapping_register / aloam_mapper_step / aloam_scan_stream_mapped run the sharded frame.  The
+ * all-reduces become loopbacks: the global map size is this rank's owned count, and the LM exchange is `exchange`:
+ *   0  k_lm_solve on this rank's blocks (the single-GPU solve);
+ *   1  per evaluation k_lm_eval_shard, a device copy of the 32 sums in place of ncclAllReduce, k_lm_tr_shard;
+ *   2  k_lm_solve_x with a one-rank peer mailbox (aloam_comm_uses_peer_memory returns 1).
+ * With exchange 1 or 2, aloam_solve also goes through that exchange.  world = 0 ends the emulation; a change of rank or world
+ * drops the uploaded map.  poison_peer_err = 1 (exchange 2) makes the next call start with the mailbox's error word set, as
+ * after a peer timeout.  What stays unchecked on one GPU: the NVLink / IPC transport, the tag order across ranks and
+ * ncclAllReduce itself.  ALOAM_ERR_STATE on a context with a communicator (and aloam_comm_init on an emulating context), and
+ * aloam_scan_stream_mapped_batch / aloam_scan_stream_lanes return it while emulating. */
+int aloam_debug_shard_emulate(aloam_ctx* ctx, int rank, int world, int exchange, int poison_peer_err);
+/* points indexed by the last aloam_map_upload(_sharded) (kept: this rank's shard) and the submap size the thin-map test of
+ * aloam_mapping_register sees (global: summed over the ranks); ALOAM_ERR_STATE without a map */
+int aloam_debug_map_sizes(aloam_ctx* ctx, int kept[2], int global[2]);
 
 /* ---- measurement hooks (bench.py): per-kernel CUDA-event timing on the ctx stream, and a launch counter */
 int aloam_profile_enable(aloam_ctx* ctx, int on);
