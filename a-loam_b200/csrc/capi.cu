@@ -270,7 +270,7 @@ void run_register(aloam_ctx* c, int nb, const int* pl, int cur, int last, int sh
     }
     // within one call the chain association -> LM -> association -> LM is launched with programmatic dependencies
     if (slots > 0) launch_ex(c, KID_ODOM_ASSOC, k_odom_assoc, dim3((slots + 7) / 8, nb), dim3(256), 0, 1, it > 0, aa, op, sharp_slots);
-    launch_lm_batch(c, slots > 0, la, nb, lp, 0, (integrate && last_it) ? 1 : 0, c->cfg.distortion != 0);
+    launch_lm_batch(c, slots > 0, la, nb, lp, 0, (integrate && last_it) ? 1 : 0, c->cfg.distortion != 0, false);   // local: cannot fail
   }
 }
 
@@ -732,14 +732,14 @@ int aloam_scan_stream_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_sc
 int aloam_scan_stream_mapped_batch(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int batch, int device_resident, double* odom_poses,
                                    double* map_poses, aloam_stats* stats_last) {
   if (!map_poses) return ALOAM_ERR_INVALID_ARG;
-  if (c && (c->shard_count > 1 || c->shard_exchange >= 0)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  if (c && sharded_job(c)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   return scan_stream_lockstep(c, raws, n_scans, batch, device_resident, odom_poses, map_poses, stats_last);
 }
 
 int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch, int device_resident,
                             double* odom_poses, double* map_poses, aloam_stats* stats_last) {
   if (!lane_ops) return ALOAM_ERR_INVALID_ARG;
-  if (c && (c->shard_count > 1 || c->shard_exchange >= 0)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
+  if (c && sharded_job(c)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   if (!stream_args_ok(c, raws, n_scans, batch, odom_poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
   // the whole schedule is checked against the lanes' state before anything changes; lanes >= batch are idle all call
   bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call
@@ -827,16 +827,12 @@ static int run_lm_api(aloam_ctx* c, const double* blocks, int n_blocks, const do
   }
   for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_api_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  if (mode == 0 && c->shard_exchange > 0) {
-    // a context emulating a rank (aloam_debug_shard_emulate) solves through the sharded solve of the scan-to-map path, which
-    // reads the block count from device memory: a stream call's scan sizes are scratch during this synchronous call
-    c->pin->query_counts[0] = n_blocks;
-    CUDA_CHECK_RET(cudaMemcpyAsync(c->d_scan_nfull, c->pin->query_counts, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    launch_lm_sharded(c, L.d_blocks, c->d_scan_nfull, c->d_api_pose, lm_params(c->cfg), L.d_summary);
-  } else {
-    launch_lm(c, false, (const BlockRec*)L.d_blocks, (const int*)nullptr, n_blocks, c->d_api_pose, lm_params(c->cfg), L.d_summary, mode,
-              c->d_out28, (double*)nullptr, 0, true /* blocks from the caller may carry any interpolation ratio */);
-  }
+  Batch<LmArgs> b = {};
+  b.a[0] = LmArgs{L.d_blocks, nullptr, n_blocks, c->d_api_pose, L.d_summary, c->d_out28, nullptr};
+  // blocks from the caller may carry any interpolation ratio; a context emulating a rank (aloam_debug_shard_emulate) with exchange
+  // 1 or 2 solves through its exchange, a rank of a real sharded job solves alone
+  const int rc = launch_lm_batch(c, false, b, 1, lm_params(c->cfg), mode, 0, true, mode == 0 && c->shard_exchange > 0);
+  if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_api_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->ne, c->d_out28, 28 * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, L.d_summary, sizeof(LmSummary), cudaMemcpyDeviceToHost, c->stream));

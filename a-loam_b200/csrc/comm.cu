@@ -1,7 +1,9 @@
 // Multi-GPU scan-to-map (SURVEY.md 8e): one process per GPU, the submap is split into spatial slabs (+ one-cell halo),
 // every rank fits only the stack points whose cell it owns and the ranks meet in ONE collective per evaluation:
-// ncclAllReduce(sum) of 32 doubles = [J^T J upper 21 | J^T r 6 | cost | #edge | #plane | pad] over NVLink / NVSwitch.
-// Every rank then takes the identical trust-region step (k_lm_tr_shard) -- no broadcast, no host round trip.
+// all-reduce (sum) of 32 doubles = [J^T J upper 21 | J^T r 6 | cost | #edge | #plane | pad] over NVLink / NVSwitch: inside the
+// solve kernel through peer memory when the ranks can map each other's, else ncclAllReduce between per-evaluation kernels.
+// Every rank then takes the identical trust-region step -- no broadcast, no host round trip.  launch_lm_batch (below) issues
+// every LM solve of the library, local or exchanged.
 //
 // NCCL is loaded with dlopen at communicator creation, so libaloam_b200.so itself has no NCCL dependency and loads on a
 // CPU-only box; inside a torch process the already-loaded torch-bundled libnccl.so.2 is picked up by soname.
@@ -43,19 +45,18 @@ bool load_nccl() {
 // peer-memory exchange state of a context (see PeerX, kernels.h)
 struct PeerState {
   PeerX px = {};
-  void* own = nullptr;                 // this rank's mailbox allocation (boxes, flags, counter, totals, error word)
+  void* own = nullptr;                 // this rank's mailbox allocation (boxes, counter, totals, error word)
   void* opened[ALOAM_MAX_RANKS] = {};  // peers' mailboxes mapped into this process (cudaIpcOpenMemHandle)
   int poison = 0;                      // test hook: the next peer_err_reset writes 1 instead of 0
 };
 
-// a rank's mailbox allocation in a world of `world` ranks: boxes [2 parities][world][32][2] words, flags [2][world], the
-// evaluation counter (64 B), the totals [2][32] and the error word (64 B)
+// a rank's mailbox allocation in a world of `world` ranks: boxes [2 parities][world][32][2] words, the evaluation counter (64 B),
+// the totals [2][32] and the error word (64 B)
 static size_t mailbox_box_bytes(int world) { return (size_t)2 * world * 32 * 2 * sizeof(unsigned long long); }
-static size_t mailbox_flag_bytes(int world) { return (size_t)2 * world * sizeof(unsigned); }
-static size_t mailbox_bytes(int world) { return mailbox_box_bytes(world) + mailbox_flag_bytes(world) + 64 + 2 * 32 * sizeof(double) + 64; }
+static size_t mailbox_bytes(int world) { return mailbox_box_bytes(world) + 64 + 2 * 32 * sizeof(double) + 64; }
 // points the counter, totals and error word of ps->px into this rank's own (zeroed) mailbox
 static void mailbox_locals(PeerState* ps, int rank, int world) {
-  char* mbox = static_cast<char*>(ps->own) + mailbox_box_bytes(world) + mailbox_flag_bytes(world);
+  char* mbox = static_cast<char*>(ps->own) + mailbox_box_bytes(world);
   ps->px.seq = reinterpret_cast<unsigned long long*>(mbox);
   ps->px.gtot = reinterpret_cast<double*>(mbox + 64);
   ps->px.err = reinterpret_cast<int*>(mbox + 64 + 2 * 32 * sizeof(double));
@@ -78,37 +79,46 @@ template <typename T> struct DeviceTemp {
   ~DeviceTemp() { if (p) cudaFree(p); }
 };
 
-void launch_lm_sharded(aloam_ctx* c, const BlockRec* blocks, const int* d_n, double* pose, const LmParams& lp, LmSummary* summary) {
-  if (c->peer) {
+// Sum of `count` elements of `type` (ncclDouble or ncclInt32) over the ranks, src -> dst on c->stream (in place when they are
+// equal): ncclAllReduce on a communicator; on a context that emulates a rank the sum over its one rank, a device copy.
+int comm_allreduce(aloam_ctx* c, const void* src, void* dst, size_t count, ncclDataType_t type) {
+  if (!c->comm) {
+    if (src != dst) CUDA_CHECK_RET(cudaMemcpyAsync(dst, src, count * (type == ncclDouble ? sizeof(double) : sizeof(int)), cudaMemcpyDeviceToDevice, c->stream));
+    return ALOAM_OK;
+  }
+  const ncclResult_t r = g_nccl.AllReduce(src, dst, count, type, ncclSum, (ncclComm_t)c->comm, c->stream);
+  if (r != ncclSuccess) { fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?"); return ALOAM_ERR_COMM; }
+  return ALOAM_OK;
+}
+
+int launch_lm_batch(aloam_ctx* c, bool pdl, const Batch<LmArgs>& args, int lanes, const LmParams& lp, int mode, int integrate, bool general,
+                    bool exchange) {
+  const dim3 grid(kLmCluster, lanes), block(ALOAM_LM_THREADS);
+  const size_t smem = lm_dynamic_smem_bytes();
+  if (!exchange) {
+    if (general) launch_ex(c, KID_LM_SOLVE, k_lm_solve_x, grid, block, smem, kLmCluster, pdl, args, lp, mode, integrate, PeerX{});
+    else launch_ex(c, KID_LM_SOLVE, k_lm_solve, grid, block, smem, kLmCluster, pdl, args, lp, mode, integrate);
+    return ALOAM_OK;
+  }
+  if (lanes != 1) return ALOAM_ERR_STATE;   // the ranks solve one trajectory together
+  if (const PeerState* ps = static_cast<const PeerState*>(c->peer)) {
     // ONE launch per solve: the cluster kernel of the single-GPU path with the all-reduce of every evaluation done inside it
     // over NVLink peer memory; early termination ends the solve on every rank at the same evaluation
-    PeerState* ps = static_cast<PeerState*>(c->peer);
-    Batch<LmArgs> b = {};
-    b.a[0] = LmArgs{blocks, d_n, 0, pose, summary, nullptr, nullptr};
-    launch_lm_batch(c, true, b, 1, lp, 0, 0, true, &ps->px);
-    return;
+    launch_ex(c, KID_LM_SOLVE, k_lm_solve_x, grid, block, smem, kLmCluster, pdl, args, lp, mode, integrate, ps->px);
+    return ALOAM_OK;
   }
-  const int evals = 1 + lp.max_iters;
+  // per evaluation: this rank's blocks, the all-reduce, the step (lm.cu, "Sharded solve")
+  const LmArgs& a = args.a[0];
   double* local = c->d_lm_tot + 32;
-  for (int e = 0; e < evals; ++e) {
-    const int first = e == 0, last = e == evals - 1;
-    prof_begin(c, KID_LM_SHARD);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(kLmCluster); cfg.blockDim = dim3(ALOAM_LM_THREADS); cfg.dynamicSmemBytes = lm_dynamic_smem_bytes(); cfg.stream = c->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = kLmCluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, k_lm_eval_shard, blocks, d_n, (const double*)pose, c->d_lm_state, first, lp.huber_a, local);
-    prof_end(c);
-    if (c->shard_exchange == 1) {   // an emulated rank: the sum over one rank
-      cudaMemcpyAsync(c->d_lm_tot, local, 32 * sizeof(double), cudaMemcpyDeviceToDevice, c->stream);
-    } else {
-      ncclResult_t r = g_nccl.AllReduce(local, c->d_lm_tot, 32, ncclDouble, ncclSum, (ncclComm_t)c->comm, c->stream);
-      if (r != ncclSuccess) fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
-    }
-    LAUNCH(c, KID_LM_SHARD, k_lm_tr_shard, 1, 32, 0, c->d_lm_state, (const double*)c->d_lm_tot, pose, first, last, lp, summary);
+  for (int e = 0; e <= lp.max_iters; ++e) {
+    const int first = e == 0;
+    launch_ex(c, KID_LM_SHARD, k_lm_eval_shard, dim3(kLmCluster), block, smem, kLmCluster, false, a.blocks, a.n_blocks_ptr, a.n_blocks_host,
+              a.x7, c->d_lm_state, first, lp.huber_a, local);
+    const int rc = comm_allreduce(c, local, c->d_lm_tot, 32, ncclDouble);
+    if (rc) return rc;
+    LAUNCH(c, KID_LM_SHARD, k_lm_tr_shard, 1, 32, 0, c->d_lm_state, (const double*)c->d_lm_tot, a.x7, first, lp, a.summary);
   }
+  return ALOAM_OK;
 }
 
 // Maps every rank's mailbox into every other rank (CUDA IPC handles exchanged with one ncclAllGather).  Returns false (and leaves
@@ -118,7 +128,7 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
   PeerState* ps = new (std::nothrow) PeerState();
   if (!ps) return false;
   c->peer = ps;
-  const size_t box_bytes = mailbox_box_bytes(world), total = mailbox_bytes(world);
+  const size_t total = mailbox_bytes(world);
   bool ok = cudaMalloc(&ps->own, total) == cudaSuccess && cudaMemset(ps->own, 0, total) == cudaSuccess;
   cudaIpcMemHandle_t mine;
   ok = ok && cudaIpcGetMemHandle(&mine, ps->own) == cudaSuccess;
@@ -144,7 +154,6 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
       base = ps->opened[r];
     }
     ps->px.box[r] = reinterpret_cast<double*>(base);
-    ps->px.flag[r] = reinterpret_cast<unsigned*>(static_cast<char*>(base) + box_bytes);
   }
   if (!ok) {
     cudaGetLastError();
@@ -157,11 +166,10 @@ static bool peer_setup(aloam_ctx* c, int rank, int world) {
   return true;
 }
 
-// sum of two ints over the ranks, in place (global submap sizes for the thin-map test, mapping.cu)
-int comm_allreduce_int2(aloam_ctx* c, int* d_two) {
-  if (c->shard_count <= 1 || c->shard_exchange >= 0) return ALOAM_OK;   // one rank, or an emulated one: the identity
-  ncclResult_t r = g_nccl.AllReduce(d_two, d_two, 2, ncclInt32, ncclSum, (ncclComm_t)c->comm, c->stream);
-  if (r != ncclSuccess) { fprintf(stderr, "[aloam_b200] ncclAllReduce failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?"); return ALOAM_ERR_COMM; }
+// what the per-evaluation solve needs beside the mailbox, created on first use: the all-reduced totals and the trust-region state
+static int lm_exchange_alloc(aloam_ctx* c) {
+  if (!c->d_lm_tot) CUDA_CHECK_RET(dalloc(c, &c->d_lm_tot, 64));
+  if (!c->d_lm_state) CUDA_CHECK_RET(dalloc(c, reinterpret_cast<char**>(&c->d_lm_state), lm_state_bytes()));
   return ALOAM_OK;
 }
 
@@ -190,10 +198,7 @@ int aloam_debug_shard_emulate(aloam_ctx* c, int rank, int world, int exchange, i
   if (world < 0 || (world > 0 && (rank < 0 || rank >= world || exchange < 0 || exchange > 2)) || (poison_peer_err && (world == 0 || exchange != 2)))
     return ALOAM_ERR_INVALID_ARG;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (world > 0) {   // what the sharded LM needs, created on first use (a failure changes no setting)
-    if (!c->d_lm_tot) CUDA_CHECK_RET(dalloc(c, &c->d_lm_tot, 64));
-    if (!c->d_lm_state) CUDA_CHECK_RET(dalloc(c, reinterpret_cast<char**>(&c->d_lm_state), lm_state_bytes()));
-  }
+  if (world > 0) { const int rc = lm_exchange_alloc(c); if (rc) return rc; }   // a failure changes no setting
   if (world == 0 || exchange != 2) {
     peer_drop(c);
   } else if (!c->peer) {   // a one-rank mailbox laid out as peer_setup's, without the IPC handles and their gather
@@ -207,7 +212,6 @@ int aloam_debug_shard_emulate(aloam_ctx* c, int rank, int world, int exchange, i
       return ALOAM_ERR_CUDA;
     }
     ps->px.box[0] = static_cast<double*>(ps->own);
-    ps->px.flag[0] = reinterpret_cast<unsigned*>(static_cast<char*>(ps->own) + mailbox_box_bytes(1));
     mailbox_locals(ps, 0, 1);
   }
   if (poison_peer_err) static_cast<PeerState*>(c->peer)->poison = 1;
@@ -244,8 +248,7 @@ int aloam_comm_init(aloam_ctx* c, int rank, int world, const char id128[128]) {
   if (r != ncclSuccess) { fprintf(stderr, "[aloam_b200] ncclCommInitRank failed: %s\n", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?"); return ALOAM_ERR_COMM; }
   c->comm = comm;
   own(c, [comm] { g_nccl.CommDestroy(comm); });   // an earlier communicator of this context lives on until aloam_destroy
-  if (!c->d_lm_tot) CUDA_CHECK_RET(dalloc(c, &c->d_lm_tot, 64));
-  if (!c->d_lm_state) CUDA_CHECK_RET(dalloc(c, reinterpret_cast<char**>(&c->d_lm_state), lm_state_bytes()));
+  const int rc = lm_exchange_alloc(c); if (rc) return rc;
   c->shard_rank = rank; c->shard_count = world;
   // the 256-byte exchange of every LM evaluation goes through NVLink peer memory inside the solve kernel when the ranks can map
   // each other's memory (all ranks decide alike: the outcome of the handle exchange is the same everywhere ... see below)

@@ -134,8 +134,8 @@ struct aloam_ctx {
                                  // aloam_debug_shard_emulate), its LM all-reduce a loopback: 0 k_lm_solve, 1 per evaluation, 2 peer
   void* comm = nullptr;          // ncclComm_t when shard_count > 1 (comm.cu)
   void* peer = nullptr;          // peer-memory exchange of the sharded LM (comm.cu), when enabled
-  double* d_lm_tot = nullptr;    // [64] all-reduced normal equations of one evaluation (sharded LM)
-  void* d_lm_state = nullptr;    // device-resident trust-region state (sharded LM)
+  double* d_lm_tot = nullptr;    // [64] all-reduced normal equations of one evaluation (per-evaluation sharded LM)
+  void* d_lm_state = nullptr;    // device-resident trust-region state (per-evaluation sharded LM)
   // map cube store of every lane (cubemap.cu), each created on first use: lane 0 serves the host API and both mapped stream
   // calls, lanes 1 .. max_batch-1 only aloam_scan_stream_mapped_batch
   void* mapper[ALOAM_MAX_BATCH] = {};
@@ -241,28 +241,15 @@ void launch_ex(aloam_ctx* c, int kid, K kernel, dim3 grid, dim3 block, size_t sm
 
 // the LM kernel runs as one thread-block cluster per trajectory (distributed-shared-memory reduction, see lm.cu)
 constexpr int kLmCluster = 8;
-// general = false: all blocks have s == 1 and there is no peer exchange (the reference-build odometry, scan-to-map on one GPU)
-inline void launch_lm_batch(aloam_ctx* c, bool pdl, const Batch<LmArgs>& args, int lanes, const LmParams& lp, int mode, int integrate, bool general = false,
-                            const PeerX* px = nullptr) {
-  if (!general && !px) {
-    launch_ex(c, KID_LM_SOLVE, k_lm_solve, dim3(kLmCluster, lanes), dim3(ALOAM_LM_THREADS), lm_dynamic_smem_bytes(), kLmCluster, pdl, args, lp, mode, integrate);
-    return;
-  }
-  PeerX none = {};
-  launch_ex(c, KID_LM_SOLVE, k_lm_solve_x, dim3(kLmCluster, lanes), dim3(ALOAM_LM_THREADS), lm_dynamic_smem_bytes(), kLmCluster, pdl, args, lp, mode, integrate,
-            px ? *px : none);
-}
-// single solve: blocks, n (device pointer or host value), pose in / out
-inline void launch_lm(aloam_ctx* c, bool pdl, const BlockRec* blocks, const int* n_ptr, int n_host, double* x7, const LmParams& lp, LmSummary* summary,
-                      int mode, double* out28, double* world7, int integrate, bool general = false) {
-  Batch<LmArgs> b = {};
-  b.a[0] = LmArgs{blocks, n_ptr, n_host, x7, summary, out28, world7};
-  launch_lm_batch(c, pdl, b, 1, lp, mode, integrate, general);
-}
 
 }  // namespace
-// sharded LM (comm.cu): per evaluation one kernel for the local blocks, one exchange of 32 doubles, one step kernel
-void launch_lm_sharded(aloam_ctx* c, const aloam::BlockRec* blocks, const int* d_n, double* pose, const aloam::LmParams& lp, aloam::LmSummary* summary);
+// Issues one LM solve of trajectories args.a[0 .. lanes-1] on c->stream (comm.cu); every solve of the library goes through here.
+// Without `exchange` it is local: k_lm_solve, or k_lm_solve_x when `general` (blocks may carry any interpolation ratio).  With
+// `exchange` the normal equations of every evaluation are summed over the ranks of a sharded job (a loopback on a context that
+// emulates a rank): one lane in mode 0, through k_lm_solve_x and the peer mailbox when there is one, else per evaluation around
+// an all-reduce.  Returns ALOAM_ERR_STATE for an exchange over several lanes and ALOAM_ERR_COMM when the all-reduce fails.
+int launch_lm_batch(aloam_ctx* c, bool pdl, const aloam::Batch<aloam::LmArgs>& args, int lanes, const aloam::LmParams& lp, int mode, int integrate,
+                    bool general, bool exchange);
 // the error word of the peer exchange (a peer that did not answer in time), on c->stream: cleared at the start of every call
 // that registers against a sharded map, copied to pinned *dst with its pose (*dst = 0 without the peer exchange)
 int peer_err_reset(aloam_ctx* c);
@@ -276,10 +263,12 @@ int ensure_map_buffers(aloam_ctx* c);
 int map_reg_alloc(aloam_ctx* c, MapReg* r);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
-void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper);
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper);
 namespace {
 
-// the scan-to-map LM goes through launch_lm_sharded: on a rank of a sharded job, and on a context that emulates a rank with
+// a rank of a sharded job: joined to a world of several ranks by a communicator, or emulating a rank (aloam_debug_shard_emulate)
+inline bool sharded_job(const aloam_ctx* c) { return c->shard_count > 1 || c->shard_exchange >= 0; }
+// the scan-to-map LM exchanges its normal equations: on a rank of a sharded job, and on a context that emulates a rank with
 // exchange 1 or 2
 inline bool sharded_lm(const aloam_ctx* c) { return c->shard_exchange < 0 ? c->shard_count > 1 : c->shard_exchange > 0; }
 

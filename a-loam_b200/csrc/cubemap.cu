@@ -528,7 +528,7 @@ int ensure_mapper(aloam_ctx* c, int lane) {
 // runs on and whether that store starts a fresh trajectory; n_upper_* bound the cloud sizes of every lane.  Lane 0 registers
 // with the context's set, shared with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
-  if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && (c->shard_count > 1 || c->shard_exchange >= 0))) return ALOAM_ERR_STATE;
+  if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && sharded_job(c))) return ALOAM_ERR_STATE;
   int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's auxiliary stream carries the stack filters of every lane
   for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
   rc = ensure_map_buffers(c); if (rc) return rc;     // lane 0's set
@@ -590,7 +590,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- optimisation (:554-733)
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  map_register_device(c, nb, io, nq_upper);
+  rc = map_register_device(c, nb, io, nq_upper); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- insertion (:736-767)
   const int up = std::max(n_upper_c, n_upper_s);

@@ -166,15 +166,15 @@ struct LmSummary {
 // mode 0: full trust-region solve, x updated in place ; mode 1: one evaluation, out28 = [JtJ upper 21, g 6, cost]
 // integrate != 0 : after the solve compose the world pose (laserOdometry.cpp:504-505): world7 <- world7 (+) x
 struct LmArgs { const BlockRec* blocks; const int* n_blocks_ptr; int n_blocks_host; double* x7; LmSummary* summary; double* out28; double* world7; };
-// Sharded solve over NVLink peer memory (multi-GPU scan-to-map, comm.cu): every rank's LM cluster pushes its 32 partial sums
-// into a mailbox in EVERY rank's memory (peer stores through NVSwitch), raises a flag there, waits for the flags of all ranks
-// in its own mailbox and adds the contributions in rank order -- the all-reduce of the normal equations happens INSIDE the
-// solve kernel, one launch per solve, no kernel boundary around the 256-byte exchange.  world 0: no exchange; world 1 (never a
-// real job: aloam_comm_init keeps a one-rank world off the sharded path) is the loopback of a context emulating a rank.
+// Sharded solve over NVLink peer memory (multi-GPU scan-to-map, comm.cu): every rank's LM cluster stores its 32 partial sums,
+// each 8-byte word tagged with the evaluation's sequence number, into a mailbox in EVERY rank's memory (peer stores through
+// NVSwitch), polls its own mailbox until every rank's words carry the tag and adds the contributions in rank order -- the
+// all-reduce of the normal equations happens INSIDE the solve kernel, one launch per solve, no kernel boundary around the
+// 256-byte exchange.  world 0: no exchange; world 1 (never a real job: aloam_comm_init keeps a one-rank world off the sharded
+// path) is the loopback of a context emulating a rank.
 #define ALOAM_MAX_RANKS 16
 struct PeerX {
   double* box[ALOAM_MAX_RANKS];             // mailbox of rank r: [2 parities][world][32][2] 8-byte words {payload half, tag} (peer-mapped device memory)
-  unsigned* flag[ALOAM_MAX_RANKS];          // (unused by the low-latency protocol)
   unsigned long long* seq;                  // this rank's evaluation counter (device), identical on all ranks by construction
   double* gtot;                             // [2][32] this rank's summed totals (local)
   int* err;                                 // set to 1 when a peer did not answer in time
@@ -185,8 +185,8 @@ __global__ void k_lm_solve_x(const __grid_constant__ Batch<LmArgs> B, LmParams p
 // sharded solve: per-evaluation kernels around an ncclAllReduce (see lm.cu, comm.cu)
 size_t lm_state_bytes();
 size_t lm_dynamic_smem_bytes();   // dynamic shared memory of k_lm_solve / k_lm_eval_shard (opt-in > 48 KB)
-__global__ void k_lm_eval_shard(const BlockRec* blocks, const int* n_ptr, const double* x7, void* state, int first, double huber_a, double* local32);
-__global__ void k_lm_tr_shard(void* state, const double* tot32, double* x7, int first, int last, LmParams prm, LmSummary* summary);
+__global__ void k_lm_eval_shard(const BlockRec* blocks, const int* n_ptr, int n_host, const double* x7, void* state, int first, double huber_a, double* local32);
+__global__ void k_lm_tr_shard(void* state, const double* tot32, double* x7, int first, LmParams prm, LmSummary* summary);
 // packs API-side residual blocks (11 doubles) into BlockRec
 __global__ void k_pack_blocks(const double* packed, int n, BlockRec* out);
 

@@ -669,6 +669,8 @@ __device__ __forceinline__ void lm_solve_body(const Batch<LmArgs>& B, const LmPa
     // thread 0 of EVERY CTA takes the same decision from the same totals (no broadcast needed).  The step works on a LOCAL copy
     // of the state (registers) and of nothing else in shared memory but the two totals vectors: with every field access going to
     // shared memory behind possibly-aliasing stores the step took a large share of the solve.
+    // k_lm_tr_shard takes the same step.  It stays written out in both kernels: as one routine shared with k_lm_tr_shard it
+    // changes k_lm_solve's register allocation and code, and k_lm_solve is on the odometry chain.
     if (tid == 0) {
       TrState t;
       int next = 0;   // 0: nothing to produce, 1: next candidate from the accepted totals, 2: from the totals just evaluated
@@ -733,15 +735,15 @@ __global__ void __launch_bounds__(NT, 1) k_lm_solve_x(const __grid_constant__ Ba
 size_t lm_dynamic_smem_bytes() { return (size_t)NT * RS * sizeof(double); }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Sharded solve (map split over GPUs, SURVEY.md 8e): the same trust-region logic, but every evaluation is
-//   k_lm_eval_shard (this rank's blocks -> local 32-vector)  ->  ncclAllReduce(sum, 32 doubles)  ->  k_lm_tr_shard
+// Sharded solve without the peer mailbox (map split over GPUs, SURVEY.md 8e): the same trust-region logic, but every evaluation is
+//   k_lm_eval_shard (this rank's blocks -> local 32-vector)  ->  all-reduce (sum, 32 doubles; comm.cu)  ->  k_lm_tr_shard
 // all stream-ordered, no host round trip: the schedule is fixed (1 + max_iters evaluations); once the state says
 // "stop" the remaining kernels return immediately.  Every rank runs the identical step on identical totals.
 size_t lm_state_bytes() { return sizeof(TrState); }
 
-__global__ void __launch_bounds__(NT, 1) k_lm_eval_shard(const BlockRec* __restrict__ blocks, const int* __restrict__ n_ptr, const double* __restrict__ x7,
-                                                         void* state, int first, double huber_a, double* __restrict__ local32) {
-  const int n = *n_ptr;
+__global__ void __launch_bounds__(NT, 1) k_lm_eval_shard(const BlockRec* __restrict__ blocks, const int* __restrict__ n_ptr, int n_host,
+                                                         const double* __restrict__ x7, void* state, int first, double huber_a, double* __restrict__ local32) {
+  const int n = n_ptr ? *n_ptr : n_host;
   cg::cluster_group cluster = cg::this_cluster();
   extern __shared__ __align__(16) double s_red[];
   __shared__ double s_part[NW][32];
@@ -765,24 +767,20 @@ __global__ void __launch_bounds__(NT, 1) k_lm_eval_shard(const BlockRec* __restr
   }
 }
 
-__global__ void k_lm_tr_shard(void* state, const double* __restrict__ tot32, double* __restrict__ x7, int first, int last,
-                              LmParams prm, LmSummary* __restrict__ summary) {
+// The step of the cluster kernel (lm_solve_body) on the state in global memory.  It ends the solve by the last evaluation of the
+// schedule at the latest: every candidate costs an iteration and the max_iters-th is the last one produced.
+__global__ void k_lm_tr_shard(void* state, const double* __restrict__ tot32, double* __restrict__ x7, int first, LmParams prm,
+                              LmSummary* __restrict__ summary) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   TrState& T = *reinterpret_cast<TrState*>(state);
-  bool keep = false;
-  if (first) {
-    if (tr_start(T, x7, tot32, prm, summary, true, summary->trace, true)) tr_next_candidate(T, tot32, prm, summary->trace, true);
-    keep = true;
-  } else if (T.go) {
-    const int next = tr_after_eval(T, tot32, prm, summary->trace, true);
-    keep = next == 2;
-    if (next) tr_next_candidate(T, keep ? tot32 : T.acc, prm, summary->trace, true);
-  }
-  if (keep) { for (int k = 0; k < 28; ++k) T.acc[k] = tot32[k]; }
-  if (last || !T.go) {
-    if (last && T.go) { T.go = 0; }   // cannot happen: the schedule covers max_iters evaluations
-    tr_finish(T, x7, summary);
-  }
+  if (!first && !T.go) return;   // the solve has ended at an earlier evaluation
+  int next;   // 0: nothing to produce, 1: next candidate from the accepted totals, 2: from the totals just evaluated
+  if (first) next = tr_start(T, x7, tot32, prm, summary, true, summary->trace, true) ? 2 : 0;
+  else next = tr_after_eval(T, tot32, prm, summary->trace, true);
+  if (next) tr_next_candidate(T, next == 2 ? tot32 : T.acc, prm, summary->trace, true);
+  // the host issues the all-reduce into one fixed buffer, so the accepted point's totals are copied out of it
+  if (first || next == 2) { for (int k = 0; k < 28; ++k) T.acc[k] = tot32[k]; }
+  if (!T.go) tr_finish(T, x7, summary);
 }
 
 }  // namespace aloam

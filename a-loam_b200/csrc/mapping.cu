@@ -23,6 +23,7 @@
 //     shard of the map holds those slabs plus a one-cell halo, so its 27-cell neighbourhoods are complete.
 #include <cfloat>
 #include <climits>
+#include <nccl.h>
 #include "ctx.h"
 
 namespace aloam {
@@ -663,7 +664,7 @@ __global__ void __launch_bounds__(256) k_map_knn(MapCloud map, const Pt4* __rest
 // host side of the mapping entry points
 using namespace aloam;
 
-int comm_allreduce_int2(aloam_ctx* c, int* d_two);   // comm.cu
+int comm_allreduce(aloam_ctx* c, const void* src, void* dst, size_t count, ncclDataType_t type);   // comm.cu
 
 namespace {
 inline int grid_ctas(const aloam_ctx* c) { return c->sms * 8; }   // grid-stride launches: 8 resident CTAs of 256 threads per SM
@@ -748,19 +749,17 @@ void map_associate_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_uppe
 }  // namespace
 
 // outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers its stacks against io[l].reg
-// (see map_associate_device) and refines io[l].pose
-void map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper) {
+// (see map_associate_device) and refines io[l].pose.  A sharded job's solves exchange their normal equations (one lane).
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper) {
   const LmParams lp = lm_params(c->cfg);
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
     map_associate_device(c, nb, io, nq_upper, it > 0, nullptr);
-    if (!sharded_lm(c)) {
-      Batch<LmArgs> lm = {};
-      for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
-      launch_lm_batch(c, true, lm, nb, lp, 0, 0);
-    } else {
-      launch_lm_sharded(c, io[0].reg.blocks, io[0].counts3 + 2, io[0].pose, lp, io[0].reg.summary + (it & 3));
-    }
+    Batch<LmArgs> lm = {};
+    for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
+    const int rc = launch_lm_batch(c, true, lm, nb, lp, 0, 0, false, sharded_lm(c));
+    if (rc) return rc;
   }
+  return ALOAM_OK;
 }
 
 namespace {
@@ -797,7 +796,7 @@ int finish_map_upload(aloam_ctx* c, const int* kept) {
     int* d_two = c->d_stack_counts;   // scratch: a sharded upload has copied its counts out of it before (stream order)
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two, &c->map.corner.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(d_two + 1, &c->map.surf.grid.dyn->owned, 4, cudaMemcpyDeviceToDevice, c->stream));
-    int rc = comm_allreduce_int2(c, d_two); if (rc) return rc;
+    int rc = comm_allreduce(c, d_two, d_two, 2, ncclInt32); if (rc) return rc;
     CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->owned, d_two, 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
@@ -919,7 +918,7 @@ int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cl
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   rc = peer_err_reset(c); if (rc) return rc;
   const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
-  map_register_device(c, 1, &io, corner_stack.n + surf_stack.n);
+  rc = map_register_device(c, 1, &io, corner_stack.n + surf_stack.n); if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->map.summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;

@@ -160,8 +160,10 @@ void KdTree::search(int ni, const float q[3], float mindistsq, float dists[3], i
   const float dst = dists[f];
   const float md = mindistsq + cut - dst;
   dists[f] = cut;
-  // `<=` so that equal-distance candidates with a smaller index are still found (tie rule above)
-  if (count < k || md <= sqd[k - 1]) search(other, q, md, dists, k, count, idx, sqd);
+  // `<=` so that equal-distance candidates with a smaller index are still found (tie rule above).  md is rounded differently
+  // from a point's distance ((dx*dx + dy*dy) + dz*dz): for a point at the bound the two can differ by a few ulps, so the bound
+  // gets a relative slack far above float rounding (a visit more costs time, never exactness)
+  if (count < k || md <= sqd[k - 1] * (1.0f + 1e-4f)) search(other, q, md, dists, k, count, idx, sqd);
   dists[f] = dst;
 }
 
