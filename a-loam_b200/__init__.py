@@ -33,7 +33,7 @@ class Config(C.Structure):
     _fields_ = [("n_scans", C.c_int), ("minimum_range", C.c_float), ("line_res", C.c_float), ("plane_res", C.c_float),
                 ("outer_iters", C.c_int), ("inner_iters", C.c_int), ("huber", C.c_double), ("dist_sq_thresh", C.c_double),
                 ("nearby_scan", C.c_double), ("device", C.c_int), ("max_points", C.c_int), ("max_map_points", C.c_int),
-                ("max_batch", C.c_int), ("distortion", C.c_int), ("max_ring_points", C.c_int)]
+                ("max_batch", C.c_int), ("distortion", C.c_int), ("max_ring_points", C.c_int), ("mapping_skip_frame", C.c_int)]
 
 
 class CloudView(C.Structure):

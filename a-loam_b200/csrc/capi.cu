@@ -28,6 +28,7 @@ void aloam_default_config(aloam_config* cfg, int n_scans) {
   cfg->dist_sq_thresh = 25.0; cfg->nearby_scan = 2.5;
   cfg->device = 0; cfg->max_points = 400000; cfg->max_map_points = 0;
   cfg->max_batch = 1; cfg->distortion = 0; cfg->max_ring_points = ALOAM_MAX_RING_POINTS;
+  cfg->mapping_skip_frame = 1;
 }
 
 const char* aloam_strerror(int code) {
@@ -70,7 +71,7 @@ int aloam_reset_odometry(aloam_ctx* c) {
   if (c->s_idx) CUDA_CHECK_RET(cudaStreamSynchronize(c->s_idx));   // an index build of the last synchronous call may still be running
   c->frame = 0; c->cur = 0; c->have_last = false;
   c->lanes_mode = false;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_running[l] = c->lane_mapped[l] = false;
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = c->lane_mapped[l] = false; c->lane_scan[l] = 0; }
   return ALOAM_OK;
 }
 
@@ -80,6 +81,8 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   aloam_config cfg = *cfg_in;
   if (cfg.max_batch == 0) cfg.max_batch = 1;                                  // zero-initialised tail of an older caller
   if (cfg.max_ring_points == 0) cfg.max_ring_points = ALOAM_MAX_RING_POINTS;
+  if (cfg.mapping_skip_frame == 0) cfg.mapping_skip_frame = 1;
+  if (cfg.mapping_skip_frame < 0) return ALOAM_ERR_INVALID_ARG;
   if (cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64) return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_batch < 1 || cfg.max_batch > ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
@@ -105,7 +108,8 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   for (cudaEvent_t& e : c->prof_ev) TRY(ecreate(c, &e, cudaEventDefault));
   for (cudaStream_t* s : {&c->s_ext, &c->s_h2d, &c->s_exa, &c->s_idx, &c->s_map}) TRY(screate(c, s));
   const std::pair<cudaEvent_t*, int> scan_events[] = {{c->ev_idx, kFeatSlots}, {c->ev_a, 2}, {c->ev_b, 2}, {c->ev_cmp, 2}, {c->ev_feat, kFeatSlots},
-                                                      {c->ev_odo, kFeatSlots}, {c->ev_mapdone, kFeatSlots}, {c->ev_h2d, 2}, {c->ev_rawfree, 2}};
+                                                      {c->ev_odo, kFeatSlots}, {c->ev_mapdone, kFeatSlots}, {c->ev_h2d, 2}, {c->ev_rawfree, 2},
+                                                      {&c->ev_mapend, 1}};
   for (const auto& a : scan_events)
     for (int i = 0; i < a.second; ++i) TRY(ecreate(c, &a.first[i], cudaEventDisableTiming));
   TRY(halloc(c, &c->h_poses, (size_t)kMaxStreamScans * 14)); TRY(dalloc(c, &c->d_poses, (size_t)kMaxStreamScans * 7)); TRY(dalloc(c, &c->d_map_poses, (size_t)kMaxStreamScans * 7));
@@ -546,8 +550,12 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     const int* op = ops + (size_t)k * nb;
     // a lane's first scan, its START, only initialises (laserOdometry.cpp:267-271)
     int na = 0, n_scan = 0, n_start = 0;
+    bool map_scan[ALOAM_MAX_BATCH];         // per record: the scan goes to the mapper (mapped calls)
     for (int l = 0; l < nb; ++l) {
       if (op[l] == ALOAM_LANE_IDLE) continue;
+      const int j = op[l] == ALOAM_LANE_START ? 0 : c->lane_scan[l];   // index of the scan in its trajectory
+      c->lane_scan[l] = j + 1;
+      map_scan[na] = j % c->cfg.mapping_skip_frame == 0;
       act[na++] = l; last_op[l] = op[l];
       if (op[l] == ALOAM_LANE_START) starting[n_start++] = l; else scanning[n_scan++] = l;
     }
@@ -597,7 +605,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     c->stream = c->s_idx;
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_b[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_odo[(f + 1) % kFeatSlots], 0));
-    STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the scan-to-map stage of frame f - kFeatSlots has read this slot
+    STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the last mapper frame that read this slot (of frame f - kFeatSlots at the latest) is done
     rc = run_features_b2(c, na, act, b, cur, false);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
@@ -622,20 +630,32 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
       // ---- scan-to-map on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose go
       //      to the mapping stage on the device -- what the reference ships through /laser_cloud_corner_last, /laser_cloud_surf_last
       //      and /laser_odom_to_init (laserOdometry.cpp:570-591 -> laserMapping.cpp:278-288) never leaves HBM
-      //      One frame covers every trajectory: each launch of it serves all lanes, each lane with its own cube store.
+      //      One frame covers every mapped lane of the step: each launch of it serves all of them, each with its own cube store.
+      //      Scan j of a trajectory is mapped when j % mapping_skip_frame == 0 (laserOdometry.cpp:570); the others get the
+      //      high-frequency pose of laserMapping.cpp:197-229 from one k_mapper_high_freq launch.  A step that maps no lane issues
+      //      no frame and does not record ev_mapdone[cur], so the next writer of this feature slot (stage C, four steps on) waits
+      //      only on a frame that read it.
       STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
       c->stream = c->s_map;
-      MapperIn in[ALOAM_MAX_BATCH];
+      MapperIn in[ALOAM_MAX_BATCH], hf[ALOAM_MAX_BATCH];
+      int n_map = 0, n_hf = 0;
       for (int i = 0; i < na; ++i) {
         const int l = act[i];
         const FeatBuf& fc = c->lanes[l].feat[cur];
         const size_t slot = ((size_t)k * nb + l) * 7;
-        in[i] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
+        const MapperIn r{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
                          reset_stores && op[l] == ALOAM_LANE_START};
+        if (map_scan[i]) in[n_map++] = r; else hf[n_hf++] = r;
       }
-      rc = mapper_step_device(c, na, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
-      if (rc) return fail(rc);
-      STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
+      if (n_map > 0) {
+        rc = mapper_step_device(c, n_map, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+        if (rc) return fail(rc);
+        STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
+      }
+      if (n_hf > 0) {
+        rc = mapper_high_freq_device(c, n_hf, hf);
+        if (rc) return fail(rc);
+      }
       c->stream = s_main;
     }
     c->cur = cur;
@@ -647,7 +667,8 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
   const size_t total = (size_t)n_scans * nb;
   STREAM_TRY(cudaMemcpyAsync(c->h_poses, c->d_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
   if (map_poses) {
-    STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapdone[c->cur], 0));
+    STREAM_TRY(cudaEventRecord(c->ev_mapend, c->s_map));   // the last mapper frame and the last high-frequency poses
+    STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapend, 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
     const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return fail(rc);

@@ -157,8 +157,10 @@ struct aloam_ctx {
   // pipelined scan stream: ring binning on s_exa, per-ring features on s_ext, compaction + index on s_idx, association + LM
   // on `stream`, host->device copies of the raw scans on s_h2d, scan-to-map on s_map; all chained by events
   cudaStream_t s_ext = nullptr, s_exa = nullptr, s_idx = nullptr, s_h2d = nullptr, s_map = nullptr;
+  // ev_mapdone[s]: the last mapper frame that read feature slot s (recorded only by steps that map a lane); ev_mapend: everything
+  // a call issued on s_map, high-frequency poses included
   cudaEvent_t ev_feat[kFeatSlots] = {}, ev_idx[kFeatSlots] = {}, ev_odo[kFeatSlots] = {}, ev_mapdone[kFeatSlots] = {}, ev_h2d[2] = {}, ev_rawfree[2] = {},
-              ev_a[2] = {}, ev_b[2] = {}, ev_cmp[2] = {};
+              ev_a[2] = {}, ev_b[2] = {}, ev_cmp[2] = {}, ev_mapend = nullptr;
   double* h_poses = nullptr;     // pinned [kMaxStreamScans][7]
   double* d_poses = nullptr;     // device [kMaxStreamScans][7]: per-(scan, lane) world poses of a stream call (one D2H at the end)
   double* d_map_poses = nullptr; // device [kMaxStreamScans][7]: map-refined poses (aloam_scan_stream_mapped)
@@ -188,6 +190,9 @@ struct aloam_ctx {
   bool lanes_mode = false;
   bool lane_running[ALOAM_MAX_BATCH] = {};
   bool lane_mapped[ALOAM_MAX_BATCH] = {};
+  // mapped streams: index of every lane's next scan in its trajectory (0 at a START); scan j goes to the mapper when
+  // j % cfg.mapping_skip_frame == 0.  Carries over between calls; aloam_reset_odometry clears it.
+  int lane_scan[ALOAM_MAX_BATCH] = {};
   int lockstep_ops[kMaxStreamScans] = {};   // the lane schedule a lockstep stream call hands to the stream driver
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
@@ -257,6 +262,7 @@ int peer_err_fetch(aloam_ctx* c, int* dst);
 void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper);
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
+int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_ensure_lanes(aloam_ctx* c, int nb);
 int* mapper_err_acc(aloam_ctx* c, int lane);
 int ensure_map_buffers(aloam_ctx* c);

@@ -172,6 +172,17 @@ __device__ void mapper_fresh_state(MapperState* S) {
 // grid (1): the host-side reset of one lane (reset_lane)
 __global__ void __launch_bounds__(1024) k_mapper_reset(MapperState* S) { mapper_fresh_state(S); }
 
+// transformAssociateToMap (:142-146): x = T_wmap_wodom * odometry pose -- also the high-frequency pose of :214-215
+__device__ __forceinline__ void associate_to_map(const MapperState* S, const double* odom7, double* x) {
+  const Qd qm{S->q_wmap_wodom[0], S->q_wmap_wodom[1], S->q_wmap_wodom[2], S->q_wmap_wodom[3]};
+  const Qd qo{odom7[0], odom7[1], odom7[2], odom7[3]};
+  const double to[3] = {odom7[4], odom7[5], odom7[6]};
+  const Qd q0 = qmul(qm, qo);
+  double r[3]; qrot(qm, to, r);
+  x[0] = q0.x; x[1] = q0.y; x[2] = q0.z; x[3] = q0.w;
+  x[4] = r[0] + S->t_wmap_wodom[0]; x[5] = r[1] + S->t_wmap_wodom[1]; x[6] = r[2] + S->t_wmap_wodom[2];
+}
+
 // transformAssociateToMap (:142-146), centre cube + shift (:314-509), valid cubes (:511-529), gather offsets
 __device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub, bool fresh) {
   pdl_launch_dependents();
@@ -183,13 +194,9 @@ __device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* 
   __shared__ int s_ctr[3], s_cen[3];
   const int tid = threadIdx.x;
   if (tid == 0) {
-    const Qd qm{S->q_wmap_wodom[0], S->q_wmap_wodom[1], S->q_wmap_wodom[2], S->q_wmap_wodom[3]};
     const Qd qo{odom7[0], odom7[1], odom7[2], odom7[3]};
     const double to[3] = {odom7[4], odom7[5], odom7[6]};
-    const Qd q0 = qmul(qm, qo);
-    double r[3]; qrot(qm, to, r);
-    S->x[0] = q0.x; S->x[1] = q0.y; S->x[2] = q0.z; S->x[3] = q0.w;
-    S->x[4] = r[0] + S->t_wmap_wodom[0]; S->x[5] = r[1] + S->t_wmap_wodom[1]; S->x[6] = r[2] + S->t_wmap_wodom[2];
+    associate_to_map(S, odom7, S->x);
     S->q_wodom[0] = qo.x; S->q_wodom[1] = qo.y; S->q_wodom[2] = qo.z; S->q_wodom[3] = qo.w;
     S->t_wodom[0] = to[0]; S->t_wodom[1] = to[1]; S->t_wodom[2] = to[2];
     for (int a = 0; a < 3; ++a) { s_cen[a] = S->cen[a]; s_ctr[a] = cube_coord(S->x[4 + a], S->cen[a]); }
@@ -255,6 +262,17 @@ __device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* 
 __global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub, unsigned fresh) {
   const MapperLane& a = B.a[blockIdx.z];
   mapper_begin_body(a.S, a.odom7, max_sub, (fresh >> blockIdx.z) & 1u);
+}
+
+// grid (1, 1, lanes): the scans the mapper skips (mapping_skip_frame > 1) get the high-frequency pose of laserOdometryHandler
+// (:197-229): T_wmap_wodom of the lane's latest mapper frame (queued before this kernel on the mapper stream) times the scan's
+// odometry pose.  The cube store is not touched.
+__global__ void k_mapper_high_freq(const __grid_constant__ Batch<MapperLane> B) {
+  if (threadIdx.x) return;
+  const MapperLane& a = B.a[blockIdx.z];
+  double x[7];
+  associate_to_map(a.S, a.odom7, x);
+  for (int k = 0; k < 7; ++k) a.out7[k] = x[k];
 }
 
 
@@ -600,6 +618,22 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1, 1, nb), dim3(256), 0, 1, true, B, c->cfg.line_res, c->cfg.plane_res);
   vox_seg_filter(c, nb, cube_f, bufs, 2 * 75, refilter_cap, cap1);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
+// The high-frequency pose of nb skipped scans on the current stream, one launch: record l composes the T_wmap_wodom of lane
+// in[l].lane's cube store with in[l].odom7 into in[l].out7 (the clouds and `fresh` of in[l] are not read).  The lanes' stores
+// exist: a trajectory's first scan is always mapped.
+int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
+  if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
+  Batch<MapperLane> B = {};
+  for (int l = 0; l < nb; ++l) {
+    B.a[l].S = static_cast<Mapper*>(c->mapper[in[l].lane])->d_state;
+    B.a[l].odom7 = in[l].odom7;
+    B.a[l].out7 = in[l].out7;
+  }
+  launch_ex(c, KID_CUBES, k_mapper_high_freq, dim3(1, 1, nb), dim3(32), 0, 1, false, B);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }

@@ -73,6 +73,9 @@ typedef struct aloam_config {
                             residual blocks (:376-379, 470-473; slerp inside the functors, lidarFactor.hpp:27-33) */
   int max_ring_points;   /* capacity of one scan ring, multiple of 32, <= ALOAM_MAX_RING_POINTS (default).  Smaller rings take
                             less shared memory per ring CTA, so more of them are resident per SM (batched streams) */
+  int mapping_skip_frame; /* mapping_skip_frame laserOdometry.cpp:191, launch/...:6 -- the mapped stream calls map every k-th scan
+                            of a trajectory and give the others the high-frequency pose (see aloam_scan_stream_mapped).  Default 1
+                            (every scan); 0 counts as 1 (zero-initialised tail of an older caller); < 0 is rejected by aloam_create */
 } aloam_config;
 
 typedef struct aloam_cloud_view {
@@ -156,7 +159,21 @@ int aloam_scan_stream_batch(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_
  * ALOAM_ERR_CAPACITY.  Needs cfg.max_map_points > 0.
  * After aloam_comm_init (every rank fed the same scans) the scan-to-map stage is sharded: each rank keeps the whole cube store,
  * indexes and searches only its x-slabs of the gathered submap, and the ranks meet in the all-reduce of the normal equations;
- * all ranks return the same poses (equal to a single-GPU run to rounding of the summation order). */
+ * all ranks return the same poses (equal to a single-GPU run to rounding of the summation order).
+ * cfg.mapping_skip_frame = k (laserOdometry.cpp:191, 570-597; every launch file sets 1, the default): a trajectory's scans are
+ * numbered from 0 at its START -- for this call and _mapped_batch the context's first scan after creation or
+ * aloam_reset_odometry -- and the number carries over between calls.
+ *   - scan j with j % k == 0 is MAPPED: its mapper frame is the one described above, and its map_poses row is the refined pose
+ *     (/aft_mapped_to_init);
+ *   - every other scan is SKIPPED: no mapper frame runs for it and the cube store does not change; its map_poses row is the
+ *     high-frequency pose of laserMapping.cpp:197-229 (/aft_mapped_to_init_high_frec), q = q_wmap_wodom * q_wodom,
+ *     t = q_wmap_wodom * t_wodom + t_wmap_wodom, with the T_wmap_wodom left by the trajectory's latest mapped scan, in the
+ *     operation order of Eigen (bit-identical to aloam_mapper_debug_state's T composed on the host in that order).
+ * So the map poses equal aloam_mapper_step run on exactly the mapped scans, with the composition for the others.  odom_poses,
+ * stats_last, ALOAM_ERR_CAPACITY and ALOAM_FLAG_CUBE_OVERFLOW keep their meaning; the last two come from mapped scans only.  A
+ * sharded job skips the same scans on every rank.  The reference's real-time drop of queued frames (laserMapping.cpp:299-303)
+ * is not modelled: an offline stream maps every k-th scan, which is what the reference does whenever its mapper keeps up.
+ * aloam_mapper_step does not count scans: a caller skips a frame by not calling it. */
 int aloam_scan_stream_mapped(aloam_ctx* ctx, const aloam_cloud_view* raws, int n_scans, int device_resident, double* odom_poses,
                              double* map_poses, aloam_stats* stats_last);
 /* aloam_scan_stream_mapped for `batch` independent trajectories ("lanes") in one context, laid out as aloam_scan_stream_batch:
@@ -165,6 +182,8 @@ int aloam_scan_stream_mapped(aloam_ctx* ctx, const aloam_cloud_view* raws, int n
  * bit-identical to that call's), and so does the scan-to-map stage: one frame per scan covers every lane.  For every lane
  * b, odom_poses[:, b], map_poses[:, b] and the lane's cube store are bit-identical to running trajectory b alone through
  * aloam_scan_stream_mapped on a fresh context with the same config; batch = 1 IS that call.  State carries over between calls.
+ * With cfg.mapping_skip_frame = k every lane maps its scans j % k == 0 (all lanes together, every k-th step) and gets the
+ * high-frequency pose for the others, as aloam_scan_stream_mapped.
  * Lane 0's cube store is the one aloam_mapper_step uses; the stores of lanes 1 .. batch-1 are created on the first call that
  * uses them (on allocation failure ALOAM_ERR_CUDA, before any state changes).  Each lane owns its slab pool (1024 x (16 k +
  * 64 k) points x 16 B = 1.34 GB at the default caps), its re-filter sort buffers (75 x (16 k + 64 k) = 6.1 M keys, about
@@ -193,6 +212,9 @@ int aloam_scan_stream_mapped_batch(aloam_ctx* ctx, const aloam_cloud_view* raws,
  * alone through aloam_scan_stream (aloam_scan_stream_mapped) on a fresh context with the same config, whatever its lane,
  * its start step and the other lanes' schedules.  Each step packs its non-idle lanes into one set of launches; a step where
  * every lane is IDLE issues nothing.  Lane state carries over between calls, so a trajectory may span several calls.
+ * cfg.mapping_skip_frame = k: a lane's scan index restarts at 0 with every START (a START is always mapped), and scan j of the
+ * trajectory is mapped when j % k == 0, skipped (high-frequency pose, see aloam_scan_stream_mapped) otherwise.  A step packs
+ * only its mapped lanes into the mapper frame; a step without one issues no frame, and one launch serves all its skipped lanes.
  * stats_last[b] (`batch` entries, or NULL): the odometry stats of lane b's last non-idle step of this call,
  * ALOAM_FLAG_INITIALISED_ONLY when that step was a START, all zero when the lane was idle all call.
  * Errors before any state changes: ALOAM_ERR_INVALID_ARG for an op outside {0, 1, 2}, batch > cfg.max_batch or map_poses
@@ -208,7 +230,8 @@ int aloam_scan_stream_mapped_batch(aloam_ctx* ctx, const aloam_cloud_view* raws,
 int aloam_scan_stream_lanes(aloam_ctx* ctx, const aloam_cloud_view* raws, const int* lane_ops, int n_scans, int batch,
                             int device_resident, double* odom_poses, double* map_poses, aloam_stats* stats_last);
 int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" clouds (all trajectories); ends every lane of
-                                             aloam_scan_stream_lanes and allows the lockstep calls again */
+                                             aloam_scan_stream_lanes and allows the lockstep calls again; the next scan of
+                                             every lane is scan 0 for cfg.mapping_skip_frame */
 
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
  * interpolation ratio, then carry it to the sweep end with (q_last_curr, t_last_curr); the intensity keeps only the scan id.
