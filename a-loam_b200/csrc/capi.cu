@@ -41,7 +41,7 @@ const char* aloam_strerror(int code) {
     case ALOAM_ERR_CUDA: return "CUDA error";
     case ALOAM_ERR_NO_DEVICE: return "no CUDA device";
     case ALOAM_ERR_RING_TOO_LARGE: return "a ring holds more than cfg.max_ring_points returns";
-    case ALOAM_ERR_NOT_RING_MAJOR: return "cloud is not in ascending ring order";
+    case ALOAM_ERR_NOT_RING_MAJOR: return "a cloud's int(intensity) is not a ring, or falls two below an earlier one";
     case ALOAM_ERR_STATE: return "call sequence error";
     case ALOAM_ERR_COMM: return "communicator error";
     default: return "unknown error";
@@ -85,6 +85,7 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   if (cfg.mapping_skip_frame < 0) return ALOAM_ERR_INVALID_ARG;
   if (cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64) return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
+  if (!(cfg.nearby_scan >= 1.0)) return ALOAM_ERR_INVALID_ARG;   // the association's break tables need a window of +-1 ring at least
   if (cfg.max_batch < 1 || cfg.max_batch > ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_ring_points < 64 || cfg.max_ring_points > ALOAM_MAX_RING_POINTS || cfg.max_ring_points % 32) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_map_points > (1 << 30)) return ALOAM_ERR_INVALID_ARG;   // the map's hash-grid slot count is a 32-bit power of two
@@ -133,13 +134,17 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
     for (FeatBuf& f : L.feat) {
       TRY(dalloc(c, &f.sharp, kMaxQueries)); TRY(dalloc(c, &f.flat, kMaxQueries));
       TRY(dalloc(c, &f.less_sharp, mp)); TRY(dalloc(c, &f.less_flat, mp));
-      TRY(dalloc(c, &f.counts, 4)); TRY(dalloc(c, &f.rs_ls, 72)); TRY(dalloc(c, &f.rs_lf, 72));
+      TRY(dalloc(c, &f.counts, 4));
       for (RabIndex* g : {&f.g_ls, &f.g_lf}) {
         TRY(dalloc(c, &g->cnt, (size_t)ALOAM_NB * 64)); TRY(dalloc(c, &g->start, (size_t)ALOAM_NB * 64 + 8));
         TRY(dalloc(c, &g->cell_of, mp)); TRY(dalloc(c, &g->rank_of, mp)); TRY(dalloc(c, &g->gpts, mp));
         TRY(cudaMemset(g->cnt, 0, (size_t)ALOAM_NB * 64 * 4)); TRY(cudaMemset(g->start, 0, ((size_t)ALOAM_NB * 64 + 8) * 4));
+        TRY(dalloc(c, &g->first_of, kRabBreakInts));
+        g->last_of = g->first_of + 64; g->fwd_end = g->last_of + 64; g->bwd_begin = g->fwd_end + 65;
+        TRY(cudaMemset(g->first_of, 0x7f, 64 * 4)); TRY(cudaMemset(g->last_of, 0xff, 64 * 4));   // 0x7f7f7f7f (> any index), -1
+        TRY(cudaMemset(g->fwd_end, 0, 130 * 4));
       }
-      TRY(cudaMemset(f.counts, 0, 16)); TRY(cudaMemset(f.rs_ls, 0, 72 * 4)); TRY(cudaMemset(f.rs_lf, 0, 72 * 4));
+      TRY(cudaMemset(f.counts, 0, 16));
     }
     TRY(dalloc(c, &L.d_blocks, (size_t)2 * kMaxQueries)); TRY(dalloc(c, &L.d_corr, (size_t)2 * kMaxQueries * 4));
     TRY(dalloc(c, &L.d_pose, 8)); TRY(dalloc(c, &L.d_world, 8)); TRY(dalloc(c, &L.d_summary, 4));
@@ -225,7 +230,7 @@ int run_features_b2(aloam_ctx* c, int nb, const int* pl, int buf, int slot, bool
     Lane& L = c->lanes[pl[l]];
     FeatBuf& out = L.feat[slot];
     ka.a[l] = CompactArgs{L.st_sharp[buf], L.st_less_sharp[buf], L.st_flat[buf], L.st_less_flat[buf], L.st_counts[buf], out.sharp, out.less_sharp, out.flat,
-                          out.less_flat, out.counts, out.rs_ls, out.rs_lf};
+                          out.less_flat, out.counts};
   }
   launch_ex(c, KID_COMPACT, k_compact, dim3(c->cfg.n_scans, nb), dim3(128), 0, 1, pdl, ka, c->cfg.n_scans, c->max_ring);
   CUDA_CHECK_RET(cudaGetLastError());
@@ -358,12 +363,11 @@ int aloam_odometry_set_last(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cl
   int* lc = c->pin->last_counts;
   lc[0] = 0; lc[1] = corner_last.n; lc[2] = 0; lc[3] = surf_last.n;
   CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, lc, 16, cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemsetAsync(f.rs_ls, 0, 72 * 4, c->stream));
-  CUDA_CHECK_RET(cudaMemsetAsync(f.rs_lf, 0, 72 * 4, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
-  if (corner_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (corner_last.n + 255) / 256, 256, 0, f.less_sharp, corner_last.n, f.rs_ls, c->d_err);
-  if (surf_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (surf_last.n + 255) / 256, 256, 0, f.less_flat, surf_last.n, f.rs_lf, c->d_err);
   run_grid_build(c, 1, kLane0, kApiLast, corner_last.n, surf_last.n);
+  // checked against the break tables of the index just built (k_ring_offsets)
+  if (corner_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (corner_last.n + 255) / 256, 256, 0, f.less_sharp, corner_last.n, f.g_ls.fwd_end, c->d_err);
+  if (surf_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (surf_last.n + 255) / 256, 256, 0, f.less_flat, surf_last.n, f.g_lf.fwd_end, c->d_err);
   CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());

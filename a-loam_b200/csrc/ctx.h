@@ -60,7 +60,6 @@ constexpr int kMaxStreamScans = 4096;                  // scans x lanes per aloa
 struct FeatBuf {
   Pt4 *sharp = nullptr, *less_sharp = nullptr, *flat = nullptr, *less_flat = nullptr;
   int* counts = nullptr;           // [4] n_sharp, n_less_sharp, n_flat, n_less_flat (device)
-  int *rs_ls = nullptr, *rs_lf = nullptr;  // ring_start tables [65+]
   RabIndex g_ls = {}, g_lf = {};           // (azimuth bucket x ring) indices over less_sharp / less_flat
 };
 

@@ -953,7 +953,7 @@ void features_debug_cycles(long long* host64x8) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// ring-ordered concatenation of the staged per-ring outputs ; also ring_start tables of the two "less" clouds
+// ring-ordered concatenation of the staged per-ring outputs
 __global__ void __launch_bounds__(128) k_compact(const __grid_constant__ Batch<CompactArgs> B, int n_scans, int MAXR) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
@@ -968,22 +968,13 @@ __global__ void __launch_bounds__(128) k_compact(const __grid_constant__ Batch<C
   Pt4* __restrict__ flat = A.flat;
   Pt4* __restrict__ less_flat = A.less_flat;
   int* __restrict__ counts = A.counts;
-  int* __restrict__ rs_less_sharp = A.rs_ls;
-  int* __restrict__ rs_less_flat = A.rs_lf;
   __shared__ int s_off[4];
   const int ring = blockIdx.x, tid = threadIdx.x;
   if (tid < 4) {
     int off = 0;
     for (int r = 0; r < ring; ++r) off += st_counts[r * 4 + tid];
     s_off[tid] = off;
-    if (tid == 1) rs_less_sharp[ring] = off;
-    if (tid == 3) rs_less_flat[ring] = off;
-    if (ring == n_scans - 1) {
-      int tot = off + st_counts[ring * 4 + tid];
-      counts[tid] = tot;
-      if (tid == 1) for (int r = n_scans; r <= 64; ++r) rs_less_sharp[r] = tot;
-      if (tid == 3) for (int r = n_scans; r <= 64; ++r) rs_less_flat[r] = tot;
-    }
+    if (ring == n_scans - 1) counts[tid] = off + st_counts[ring * 4 + tid];
   }
   __syncthreads();
   const int c0 = st_counts[ring * 4], c1 = st_counts[ring * 4 + 1], c2 = st_counts[ring * 4 + 2], c3 = st_counts[ring * 4 + 3];

@@ -31,7 +31,7 @@ struct ScatterArgs { const float* raw; int n, stride; const int8_t* ring_in; con
 struct RingFeatArgs { const Pt4* full; const int* ring_start; Pt4 *st_sharp, *st_less_sharp, *st_flat, *st_less_flat; int* st_counts;
                       float* dbg_curv; int8_t* dbg_label; ScanScalars* sc; };
 struct CompactArgs { const Pt4 *st_sharp, *st_less_sharp, *st_flat, *st_less_flat; const int* st_counts; Pt4 *sharp, *less_sharp, *flat, *less_flat;
-                     int* counts; int *rs_ls, *rs_lf; };
+                     int* counts; };
 __global__ void k_classify(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);          // grid (blocks, lanes)
 __global__ void k_ring_scan(const __grid_constant__ Batch<RingScanArgs> B, int n_scans);                       // grid (lanes)
 __global__ void k_scatter(const __grid_constant__ Batch<ScatterArgs> B);                                       // grid (blocks, lanes)
@@ -42,19 +42,26 @@ __global__ void k_compact(const __grid_constant__ Batch<CompactArgs> B, int n_sc
 // ---- odometry.cu
 // (azimuth bucket x ring) index over one cloud = what replaces a kd-tree build (laserOdometry.cpp:567-568)
 #define ALOAM_NB 128   // azimuth buckets (2.8 deg)
+// "ring" below is int(intensity), the closestPointScanID of laserOdometry.cpp:308,398 -- the physical ring or the one below it
+// (relTime in (-2, 6], see DESIGN.md section 3), so it may descend by one between consecutive points of a cloud.
 struct RabIndex {
   int* cnt;         // [NB*64] scratch counters (left zeroed by k_rab_scan)
   int* start;       // [NB*64 + 1] first slot of cell (bucket*64 + ring) in gpts
   int* cell_of;     // [capacity] cell of point i
   int* rank_of;     // [capacity] rank of point i inside its cell
-  float4* gpts;     // [capacity] cell-contiguous copy: x, y, z, bits(ring << 24 | original index)
+  float4* gpts;     // [capacity] cell-contiguous copy: x, y, z, bits(original index << 6 | ring)
+  int* first_of;    // [64] scratch: smallest index of each ring (left above any index by k_rab_scan)
+  int* last_of;     // [64] scratch: largest index of each ring (left -1 by k_rab_scan)
+  int* fwd_end;     // [65] fwd_end[r]   = first index with ring >= r (n if none): the forward loops' break index
+  int* bwd_begin;   // [65] bwd_begin[r] = 1 + last index with ring < r (0 if none): one past the backward loops' break index
 };
+constexpr int kRabBreakInts = 64 + 64 + 65 + 65;   // first_of, last_of, fwd_end, bwd_begin in one allocation
 struct LastCloud {
-  const Pt4* pts;   // the cloud in its original (ring-major) order
+  const Pt4* pts;   // the cloud in its original order
   const int* n;     // device scalar: number of points
   RabIndex index;
 };
-__global__ void k_ring_offsets(const Pt4* pts, int n, int* ring_start, int* err);
+__global__ void k_ring_offsets(const Pt4* pts, int n, const int* fwd_end, int* err);
 struct RabArgs { RabIndex a; const Pt4* pa; const int* na; RabIndex b; const Pt4* pb; const int* nb; };
 __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B);   // grid (blocks, 2 clouds, lanes)
 __global__ void k_rab_scan(const __grid_constant__ Batch<RabArgs> B);    // grid (2 clouds, lanes)

@@ -3,7 +3,7 @@
 //
 // Index = a dense (azimuth bucket x ring) table per "last" cloud instead of a kd-tree (k_rab_* kernels): a counting
 //   sort of the cloud into ALOAM_NB x 64 cells, bucket-major, so that "all rings of an azimuth bucket" and "rings
-//   rc-2..rc+2 of an azimuth bucket" are both contiguous slices of one float4 array (x, y, z, ring<<24 | index).
+//   rc-2..rc+2 of an azimuth bucket" are both contiguous slices of one float4 array (x, y, z, index<<6 | ring).
 //   The order of points inside a cell depends on atomic timing, but every search below compares candidates on
 //   (distance, original index / visiting rank), so results are a pure function of the input.
 // Search = ONE WARP PER QUERY, exact.  The clouds live in the sensor frame of the last scan, so a point whose
@@ -18,6 +18,11 @@
 // The 2nd / 3rd correspondence points of :312-361 / :402-455 use the same sweep restricted to the ring slice
 // rc-2..rc+2, with candidates ranked by the reference's visiting order (forward ascending first, then backward
 // descending, strict '<'), so ties resolve exactly as the sequential loops do.
+// "Ring" is int(intensity) = ring + 0.1 relTime truncated.  scanRegistration.cpp emits relTime in (-2, 6] (DESIGN.md
+// section 3), so a cloud's int(intensity) is the physical ring or the one below and need not ascend: the invariant the search
+// relies on is only  int_i >= max_{j<i} int_j - 1.  Under it (and NEARBY_SCAN >= 1) the loops' break indices do not depend on
+// the closest point -- forward: the first index with int >= rc+3, backward: the last with int <= rc-3 -- every candidate has
+// int in rc-2..rc+2, and the class and visiting rank of a candidate follow from (index vs closest, int vs rc) alone.
 #include <climits>
 #include <cfloat>
 #include "common.cuh"
@@ -25,22 +30,13 @@
 
 namespace aloam {
 
-// validates that a cloud handed in through the C ABI is in ascending ring order (the reference's windowed scans
-// :312-361 assume it) and that every int(intensity) is a legal ring
-__global__ void k_ring_offsets(const Pt4* __restrict__ pts, int n, int* __restrict__ ring_start, int* __restrict__ err) {
+// validates a cloud handed in through the C ABI after its index is built: every int(intensity) is a legal ring and no
+// earlier point has a ring two or more above (fwd_end[r + 2] is the first index with ring >= r + 2)
+__global__ void k_ring_offsets(const Pt4* __restrict__ pts, int n, const int* __restrict__ fwd_end, int* __restrict__ err) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int r = (int)pts[i].i;  // int(intensity) = scan line (laserOdometry.cpp:308,398)
-  if (r < 0 || r > 63) { atomicExch(err, 1); return; }
-  if (i == 0) {
-    for (int k = 0; k <= r; ++k) ring_start[k] = 0;
-  } else {
-    const int rp = (int)pts[i - 1].i;
-    if (r < rp) atomicExch(err, 1);
-    for (int k = max(rp, 0) + 1; k <= r; ++k) ring_start[k] = i;
-  }
-  if (i == n - 1)
-    for (int k = r + 1; k <= 64; ++k) ring_start[k] = n;
+  if (r < 0 || r > 63 || fwd_end[min(r + 2, 64)] < i) atomicExch(err, 1);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -69,9 +65,16 @@ __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B) {
   const int cell = bucket_of(p.x, p.y) * 64 + ring;
   g.cell_of[i] = cell;
   g.rank_of[i] = atomicAdd(&g.cnt[cell], 1);
+  // first / last index of each ring: the lanes of a warp hold consecutive indices, so the lowest / highest lane of a ring's
+  // group carries its smallest / largest index
+  const unsigned grp = __match_any_sync(__activemask(), ring);
+  const unsigned lane = lane_id();
+  if (lane == (unsigned)(__ffs(grp) - 1)) atomicMin(&g.first_of[ring], i);
+  if (lane == 31u - __clz(grp)) atomicMax(&g.last_of[ring], i);
 }
 
-// one CTA per cloud: exclusive scan of the ALOAM_NB*64 cell counts -> start[], and reset the counts for the next build
+// one CTA per cloud: exclusive scan of the ALOAM_NB*64 cell counts -> start[], the break tables, and reset the scratch for
+// the next build
 __global__ void __launch_bounds__(1024) k_rab_scan(const __grid_constant__ Batch<RabArgs> B) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
@@ -79,6 +82,30 @@ __global__ void __launch_bounds__(1024) k_rab_scan(const __grid_constant__ Batch
   constexpr int NC = ALOAM_NB * 64, PER = NC / 1024;
   __shared__ int s_w[32];
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  // break tables, two ring entries per lane: warp 0 takes the suffix minima of first_of, warp 1 the prefix maxima of last_of
+  if (w == 0) {
+    const int n = blockIdx.x == 0 ? *B.a[blockIdx.y].na : *B.a[blockIdx.y].nb;
+    int lo = g.first_of[lane], hi = g.first_of[32 + lane];
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_down_sync(0xffffffffu, hi, d); if (lane + d < 32) hi = min(hi, u); }
+    const int hi_all = __shfl_sync(0xffffffffu, hi, 0);
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_down_sync(0xffffffffu, lo, d); if (lane + d < 32) lo = min(lo, u); }
+    g.fwd_end[lane] = min(min(lo, hi_all), n);
+    g.fwd_end[32 + lane] = min(hi, n);
+    if (lane == 0) g.fwd_end[64] = n;
+  } else if (w == 1) {
+    int lo = g.last_of[lane], hi = g.last_of[32 + lane];
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_up_sync(0xffffffffu, lo, d); if (lane >= d) lo = max(lo, u); }
+    const int lo_all = __shfl_sync(0xffffffffu, lo, 31);
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_up_sync(0xffffffffu, hi, d); if (lane >= d) hi = max(hi, u); }
+    // bwd_begin[r] = 1 + max(last_of[0 .. r-1]): the inclusive maxima shifted by one entry
+    g.bwd_begin[1 + lane] = lo + 1;
+    g.bwd_begin[33 + lane] = max(hi, lo_all) + 1;
+    if (lane == 0) g.bwd_begin[0] = 0;
+  }
   int v[PER], sum = 0;
 #pragma unroll
   for (int k = 0; k < PER; ++k) { v[k] = g.cnt[t * PER + k]; g.cnt[t * PER + k] = 0; sum += v[k]; }
@@ -94,6 +121,7 @@ __global__ void __launch_bounds__(1024) k_rab_scan(const __grid_constant__ Batch
     s_w[lane] = inc - x;
   }
   __syncthreads();
+  if (t < 64) { g.first_of[t] = INT_MAX; g.last_of[t] = -1; }   // every reader of the scratch is past the barriers above
   int run = s_w[w] + incl - sum;
 #pragma unroll
   for (int k = 0; k < PER; ++k) { g.start[t * PER + k] = run; run += v[k]; }
@@ -111,7 +139,8 @@ __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B) {
   if (i >= n) return;
   const Pt4 p = pts[i];
   const int cell = g.cell_of[i];
-  g.gpts[g.start[cell] + g.rank_of[i]] = make_float4(p.x, p.y, p.z, __int_as_float(((cell & 63) << 24) | i));
+  // index-major key: comparing keys compares indices, the reference's tie rule (the ring need not ascend with the index)
+  g.gpts[g.start[cell] + g.rank_of[i]] = make_float4(p.x, p.y, p.z, __int_as_float((i << 6) | (cell & 63)));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -249,9 +278,8 @@ __device__ __forceinline__ void store_none(BlockRec* b, int* corr) {
 
 constexpr int kBig = 1 << 25;       // separates forward ranks [0, 2^24) from backward ranks
 
-// exact nearest neighbour of q with d2 < limit (strict); returns its packed word (ring << 24 | index) or -1, d2 in out_d,
-// the half-width of the bucket interval it had to read in k_out.  Ties -> smaller index (the cloud is ring-major, so
-// packed order == index order).
+// exact nearest neighbour of q with d2 < limit (strict); returns its packed word (index << 6 | ring) or -1, d2 in out_d,
+// the half-width of the bucket interval it had to read in k_out.  Ties -> smaller index (packed order == index order).
 __device__ __forceinline__ int rab_nearest(const RabIndex& g, float qx, float qy, float qz, float limit, float& out_d, int& k_out) {
   const int bq = bucket_of(qx, qy);
   const float rho = sqrtf(qx * qx + qy * qy);
@@ -319,16 +347,18 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   int k_nn;
   const int packed1 = rab_nearest(g, qx, qy, qz, thr, d1, k_nn);
   if (packed1 < 0 || !((double)d1 < prm.dist_sq_thresh)) { if (lane == 0) store_none(out, co); return; }
-  const int closest = packed1 & 0xffffff;
-  const Pt4 pc = L.pts[closest];   // issued now, consumed after the second search
-  const int rc = packed1 >> 24;  // closestPointScanID = int(intensity) of the closest point (k_rab_fill packs it)
+  const int closest = packed1 >> 6;
+  const int rc = packed1 & 63;   // closestPointScanID = int(intensity) of the closest point (k_rab_fill packs it)
   // rings rc-up .. rc+up survive the `> rc + NEARBY_SCAN` / `< rc - NEARBY_SCAN` break tests (:319,345,405,433)
   int up = 0; while ((double)(rc + up + 1) <= (double)rc + prm.nearby_scan) ++up;
+  // the loops' ranges: forward (closest, fwd_end), backward [bwd_begin, closest).  Issued together with the closest point;
+  // aloam_create guarantees up >= 1, which puts both break indices on the right side of `closest`.
+  const int fwd_end = g.fwd_end[min(rc + up + 1, 64)], bwd_begin = g.bwd_begin[max(rc - up, 0)];
+  const Pt4 pc = L.pts[closest];   // issued now, consumed after the second search
 
-  // second search: class 2 / class 3 minima in the reference's visiting order.
-  //   corner: class 2 = other rings within +-up (forward = higher rings first, :312-361)
-  //   surf  : class 2 = same ring (forward = indices after `closest`, :416-420,444-448),
-  //           class 3 = other rings within +-up (:422-426,449-454)
+  // second search: class 2 / class 3 minima in the reference's visiting order (forward ascending, then backward descending).
+  //   corner (:312-361): forward int > rc, backward int < rc; one class
+  //   surf (:402-455):   class 2 = forward int <= rc, backward int >= rc; class 3 = the rest of the two ranges
   float b2 = thr, b3 = thr; int r2 = INT_MAX, r3 = INT_MAX;
   float w2 = FLT_MAX, w3 = FLT_MAX; int k2 = INT_MAX, k3 = INT_MAX;
   {
@@ -336,18 +366,15 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
     const float rho = sqrtf(qx * qx + qy * qy);
     const int r_lo = max(rc - up, 0), r_hi = min(rc + up, 63);
     auto f = [&](float x, float y, float z, int packed) {
-      const int idx = packed & 0xffffff, ring = packed >> 24;
-      const int dr = ring - rc;
+      const int idx = packed >> 6, ring = packed & 63;
+      if (idx == closest || idx >= fwd_end || idx < bwd_begin) return;
+      const bool fwd = idx > closest;
+      const bool same = fwd ? ring <= rc : ring >= rc;   // corner: skipped ; surf: class 2
+      if (is_corner && same) return;
+      const int rank = fwd ? (idx - closest) : (kBig + (closest - idx));
       const float d2 = sqdist3(x, y, z, qx, qy, qz);
-      if (dr == 0) {
-        if (is_corner || idx == closest) return;
-        const int rank = idx > closest ? (idx - closest) : (kBig + (closest - idx));
-        if (d2 < b2 || (d2 == b2 && r2 != INT_MAX && rank < r2)) { b2 = d2; r2 = rank; }
-      } else {
-        const int rank = dr > 0 ? idx : (kBig + (kBig - idx));
-        if (is_corner) { if (d2 < b2 || (d2 == b2 && r2 != INT_MAX && rank < r2)) { b2 = d2; r2 = rank; } }
-        else { if (d2 < b3 || (d2 == b3 && r3 != INT_MAX && rank < r3)) { b3 = d2; r3 = rank; } }
-      }
+      if (is_corner || same) { if (d2 < b2 || (d2 == b2 && r2 != INT_MAX && rank < r2)) { b2 = d2; r2 = rank; } }
+      else { if (d2 < b3 || (d2 == b3 && r3 != INT_MAX && rank < r3)) { b3 = d2; r3 = rank; } }
     };
     int k = min(k_nn, kMaxK0);
     visit_ring_slices(g, bq, k, r_lo, r_hi, f);
@@ -367,11 +394,8 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   }
   // rank -> index
   int j2 = -1, j3 = -1;
-  if (k2 != INT_MAX && w2 != FLT_MAX) {
-    if (is_corner) j2 = k2 < kBig ? k2 : (kBig - (k2 - kBig));
-    else j2 = k2 < kBig ? (closest + k2) : (closest - (k2 - kBig));
-  }
-  if (!is_corner && k3 != INT_MAX && w3 != FLT_MAX) j3 = k3 < kBig ? k3 : (kBig - (k3 - kBig));
+  if (k2 != INT_MAX && w2 != FLT_MAX) j2 = k2 < kBig ? (closest + k2) : (closest - (k2 - kBig));
+  if (!is_corner && k3 != INT_MAX && w3 != FLT_MAX) j3 = k3 < kBig ? (closest + k3) : (closest - (k3 - kBig));
 
   if (is_corner) {
     if (j2 < 0) { if (lane == 0) store_none(out, co); return; }
@@ -441,7 +465,7 @@ __global__ void __launch_bounds__(256) k_knn_last(LastCloud cloud, const Pt4* __
   float d;
   int k_used;
   const int packed = rab_nearest(cloud.index, q.x, q.y, q.z, FLT_MAX, d, k_used);
-  const int j = packed < 0 ? -1 : (packed & 0xffffff);
+  const int j = packed < 0 ? -1 : (packed >> 6);
   if (lane_id() == 0) { idx[wid] = j; sqd[wid] = j < 0 ? __int_as_float(0x7f800000) : d; }
 }
 

@@ -1,5 +1,6 @@
 """Seeded synthetic lidar scans (VLP-16 / HDL-32 / HDL-64 shaped) -- ctypes binding of synth.cc."""
 import ctypes as C
+import math
 import os
 import subprocess
 
@@ -34,6 +35,8 @@ def _lib():
         L.synth_scan.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
                                  C.POINTER(C.c_float), C.c_int]
         L.synth_pose.argtypes = [C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        L.synth_scan_seam.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
+                                      C.POINTER(C.c_double), C.c_int, C.c_int, C.c_double, C.POINTER(C.c_float), C.c_int]
         _LIB = L
     return _LIB
 
@@ -47,6 +50,40 @@ def scan(sensor, index, seed=BASE_SEED, n_az=None, noise=0.02, max_range=120.0):
     n = _lib().synth_scan(seed, n_scans, az, index, noise, max_range, out.ctypes.data_as(C.POINTER(C.c_float)), out.shape[0])
     if n < 0:
         raise RuntimeError("synth_scan failed: %d" % n)
+    return out[:n].copy()
+
+
+class SeamTooClose(ValueError):
+    """a surviving return lies within 1e-5 rad of an azimuth threshold of the reference's sweep walk"""
+
+
+def scan_seam(sensor, index, cut=None, coverage=1.0, ring_offsets_deg=None, laser_major=False, ccw=False, seed=BASE_SEED,
+              n_az=None, noise=0.02, max_range=120.0):
+    """Raw scan `index` of the trajectory, cut and fired differently from scan():
+    cut               atan2(y, x) [rad] of the first firing column (None: the phase of scan(), pi - 2 pi 0.37 / n_az)
+    coverage          revolutions covered, round(coverage * n_az) columns
+    ring_offsets_deg  per-beam azimuth offset [deg] (n_scans values): the beam fires at another azimuth, the world stays put
+    laser_major       all columns of beam 0, then beam 1, ... instead of column by column
+    ccw               atan2(y, x) rises in firing order instead of falling
+    With the neutral arguments the result is bit-identical to scan().  Raises SeamTooClose when a surviving return sits
+    within 1e-5 rad of an azimuth threshold (host and device atan2f may then take different branches)."""
+    n_scans, az, min_range = SENSORS[sensor][:3]
+    if n_az is not None:
+        az = n_az
+    start_col = 0.0 if cut is None else (math.pi - cut) * az / (2 * math.pi) - 0.37
+    n_col = int(round(coverage * az))
+    off = None
+    if ring_offsets_deg is not None:
+        off = np.ascontiguousarray(ring_offsets_deg, np.float64)
+        assert off.shape == (n_scans,)
+    out = np.zeros((n_scans * n_col, 4), np.float32)
+    n = _lib().synth_scan_seam(seed, n_scans, az, index, noise, max_range, start_col, n_col,
+                               None if off is None else off.ctypes.data_as(C.POINTER(C.c_double)), int(laser_major), int(ccw),
+                               min_range, out.ctypes.data_as(C.POINTER(C.c_float)), out.shape[0])
+    if n == -3:
+        raise SeamTooClose("scan_seam(%s, %d, cut=%r, coverage=%r): a return lies on an azimuth threshold" % (sensor, index, cut, coverage))
+    if n < 0:
+        raise RuntimeError("synth_scan_seam failed: %d" % n)
     return out[:n].copy()
 
 

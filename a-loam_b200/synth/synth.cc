@@ -167,6 +167,142 @@ int sensor_elevations(int n_scans, std::vector<double>& elev_deg) {
   return 0;
 }
 
+// Where a sweep is cut and how it is fired.  The neutral value is the layout of synth_scan.
+//   start_col  azimuth of the first firing column, in columns: phi = pi - 2 pi (start_col +- j + 0.37) / n_az
+//   n_col      number of firing columns (n_az = one revolution)
+//   ring_off   per-beam azimuth offset [deg] added to the firing azimuth (nullptr = none); the world is not moved
+//   laser_major  emit beam by beam (all columns of beam 0, then beam 1, ...) instead of column by column
+//   ccw        the firing azimuth rises with j (-atan2(y, x) falls) instead of falling
+struct Layout {
+  double start_col = 0.0;
+  int n_col = 0;
+  const double* ring_off = nullptr;
+  int laser_major = 0, ccw = 0;
+};
+
+// ring id of a return as scanRegistration.cpp:166-205 assigns it, or -1 when it drops the return
+int reference_ring(float x, float y, float z, int n_scans) {
+  const float angle = (float)(std::atan((double)z / std::sqrt((double)(x * x + y * y))) * 180 / M_PI);
+  int id;
+  if (n_scans == 16) {
+    id = int((angle + 15) / 2 + 0.5);
+    return (id > n_scans - 1 || id < 0) ? -1 : id;
+  }
+  if (n_scans == 32) {
+    id = int((angle + 92.0 / 3.0) * 3.0 / 4.0);
+    return (id > n_scans - 1 || id < 0) ? -1 : id;
+  }
+  if (angle >= -8.83) id = int((2 - angle) * 3.0 + 0.5);
+  else id = n_scans / 2 + int((-8.83 - angle) * 2.0 + 0.5);
+  return (angle > 2 || angle < -24.33 || id > 50 || id < 0) ? -1 : id;
+}
+
+// The azimuth fix-ups of scanRegistration.cpp:141-153 and :208-236 compare float -atan2f(y, x) with thresholds.  Host and
+// device atan2f differ in the last ulp, so a return closer than kSeamMargin to a threshold it is tested against could take
+// the other branch on the GPU.  Replays the reference's walk over the surviving returns and returns -3 if one is that close
+// (a return near the half-sweep test is checked against the thresholds of both halves, since the flag may flip there).
+constexpr double kSeamMargin = 1e-5;
+int check_seam_margins(const float* pts, int n, int n_scans, double minimum_range) {
+  const float thres = (float)minimum_range;
+  std::vector<int> keep;
+  for (int i = 0; i < n; ++i) {
+    const float* p = pts + (size_t)i * 4;
+    if (!std::isfinite(p[0]) || !std::isfinite(p[1]) || !std::isfinite(p[2])) continue;
+    if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] < thres * thres) continue;
+    keep.push_back(i);
+  }
+  if (keep.empty()) return 0;
+  auto ori_of = [&](int i) { return -std::atan2(pts[(size_t)i * 4 + 1], pts[(size_t)i * 4]); };
+  const float start = ori_of(keep.front());
+  const float end_raw = ori_of(keep.back()) + 2 * M_PI;
+  auto near = [](double a, double b) { return std::fabs(a - b) < kSeamMargin; };
+  if (near(end_raw - start, 3 * M_PI) || near(end_raw - start, M_PI)) return -3;
+  float end = end_raw;
+  if (end - start > 3 * M_PI) end -= 2 * M_PI;
+  else if (end - start < M_PI) end += 2 * M_PI;
+  bool half = false;
+  for (int i : keep) {
+    const float* p = pts + (size_t)i * 4;
+    if (reference_ring(p[0], p[1], p[2], n_scans) < 0) continue;   // dropped before the azimuth walk (:174-175)
+    float ori = ori_of(i);
+    const bool pre_near = near(ori, start - M_PI / 2) || near(ori, start + M_PI * 3 / 2);
+    const bool post_near = near(ori + 2 * M_PI, end - M_PI * 3 / 2) || near(ori + 2 * M_PI, end + M_PI / 2);
+    if (!half) {
+      if (ori < start - M_PI / 2) ori += 2 * M_PI;
+      else if (ori > start + M_PI * 3 / 2) ori -= 2 * M_PI;
+      const bool at_half = near(ori - start, M_PI);
+      if (pre_near || (at_half && post_near)) return -3;
+      if (ori - start > M_PI) half = true;
+    } else if (post_near) {
+      return -3;
+    }
+  }
+  return 0;
+}
+
+int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma, double max_range, const Layout& lay,
+             float* out, int capacity) {
+  std::vector<double> elev;
+  if (sensor_elevations(n_scans, elev) != 0) return -1;
+  const int n_col = lay.n_col;
+  if (n_az <= 0 || n_col <= 0 || capacity < n_scans * n_col) return -2;
+  World w = make_world(seed);
+  Pose P = trajectory_pose(scan_index);
+  // candidate boxes within range
+  std::vector<int> cand;
+  for (size_t i = 0; i < w.boxes.size(); ++i) {
+    const Box& b = w.boxes[i];
+    double dx = std::max({b.lo[0] - P.t[0], 0.0, P.t[0] - b.hi[0]});
+    double dy = std::max({b.lo[1] - P.t[1], 0.0, P.t[1] - b.hi[1]});
+    if (dx * dx + dy * dy < (max_range + 1) * (max_range + 1)) cand.push_back((int)i);
+  }
+  std::vector<float> tmp((size_t)n_scans * n_col * 4);
+  std::vector<uint8_t> ok((size_t)n_scans * n_col, 0);
+  const int nb = n_scans;
+  unsigned nthreads = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
+  auto work = [&](int j0, int j1) {
+    for (int j = j0; j < j1; ++j) {
+      // per-column rng so the result does not depend on the thread count
+      Rng rng(seed * 1000003ull + (uint64_t)scan_index * 7907ull + (uint64_t)j * 104729ull + 12345ull);
+      const double col = lay.ccw ? lay.start_col - j : j + lay.start_col;
+      double phi = M_PI - 2.0 * M_PI * (col + 0.37) / n_az;  // clockwise unless ccw
+      double cph = std::cos(phi), sph = std::sin(phi);
+      for (int b = 0; b < nb; ++b) {
+        if (lay.ring_off) {
+          const double pb = phi + lay.ring_off[b] * M_PI / 180.0;
+          cph = std::cos(pb); sph = std::sin(pb);
+        }
+        double el = elev[b] * M_PI / 180.0;
+        double ds[3] = {std::cos(el) * cph, std::cos(el) * sph, std::sin(el)};
+        double d[3] = {P.R[0] * ds[0] + P.R[1] * ds[1] + P.R[2] * ds[2],
+                       P.R[3] * ds[0] + P.R[4] * ds[1] + P.R[5] * ds[2],
+                       P.R[6] * ds[0] + P.R[7] * ds[1] + P.R[8] * ds[2]};
+        double t = cast(w, cand, P.t, d, 0.05, max_range);
+        double nz = rng.gauss();  // always drawn, so streams stay aligned
+        size_t o = lay.laser_major ? (size_t)b * n_col + j : (size_t)j * nb + b;
+        if (t >= max_range) continue;
+        double r = t + noise_sigma * nz;
+        tmp[o * 4 + 0] = (float)(r * ds[0]);
+        tmp[o * 4 + 1] = (float)(r * ds[1]);
+        tmp[o * 4 + 2] = (float)(r * ds[2]);
+        tmp[o * 4 + 3] = 0.0f;
+        ok[o] = 1;
+      }
+    }
+  };
+  std::vector<std::thread> th;
+  int per = (n_col + (int)nthreads - 1) / (int)nthreads;
+  for (unsigned i = 0; i < nthreads; ++i) {
+    int j0 = (int)i * per, j1 = std::min(n_col, j0 + per);
+    if (j0 < j1) th.emplace_back(work, j0, j1);
+  }
+  for (auto& t : th) t.join();
+  int n = 0;
+  for (size_t o = 0; o < ok.size(); ++o)
+    if (ok[o]) { std::memcpy(out + (size_t)n * 4, &tmp[o * 4], 16); ++n; }
+  return n;
+}
+
 }  // namespace
 
 extern "C" {
@@ -183,59 +319,23 @@ void synth_pose(int k, double q[4], double t[3]) {
 // Returns the number of points written, or <0 on error.
 int synth_scan(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma,
                double max_range, float* out, int capacity) {
-  std::vector<double> elev;
-  if (sensor_elevations(n_scans, elev) != 0) return -1;
-  if (capacity < n_scans * n_az) return -2;
-  World w = make_world(seed);
-  Pose P = trajectory_pose(scan_index);
-  // candidate boxes within range
-  std::vector<int> cand;
-  for (size_t i = 0; i < w.boxes.size(); ++i) {
-    const Box& b = w.boxes[i];
-    double dx = std::max({b.lo[0] - P.t[0], 0.0, P.t[0] - b.hi[0]});
-    double dy = std::max({b.lo[1] - P.t[1], 0.0, P.t[1] - b.hi[1]});
-    if (dx * dx + dy * dy < (max_range + 1) * (max_range + 1)) cand.push_back((int)i);
-  }
-  std::vector<float> tmp((size_t)n_scans * n_az * 4);
-  std::vector<uint8_t> ok((size_t)n_scans * n_az, 0);
-  const int nb = n_scans;
-  unsigned nthreads = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
-  auto work = [&](int j0, int j1) {
-    for (int j = j0; j < j1; ++j) {
-      // per-azimuth rng so the result does not depend on the thread count
-      Rng rng(seed * 1000003ull + (uint64_t)scan_index * 7907ull + (uint64_t)j * 104729ull + 12345ull);
-      double phi = M_PI - 2.0 * M_PI * (j + 0.37) / n_az;  // clockwise
-      double cph = std::cos(phi), sph = std::sin(phi);
-      for (int b = 0; b < nb; ++b) {
-        double el = elev[b] * M_PI / 180.0;
-        double ds[3] = {std::cos(el) * cph, std::cos(el) * sph, std::sin(el)};
-        double d[3] = {P.R[0] * ds[0] + P.R[1] * ds[1] + P.R[2] * ds[2],
-                       P.R[3] * ds[0] + P.R[4] * ds[1] + P.R[5] * ds[2],
-                       P.R[6] * ds[0] + P.R[7] * ds[1] + P.R[8] * ds[2]};
-        double t = cast(w, cand, P.t, d, 0.05, max_range);
-        double nz = rng.gauss();  // always drawn, so streams stay aligned
-        size_t o = (size_t)j * nb + b;
-        if (t >= max_range) continue;
-        double r = t + noise_sigma * nz;
-        tmp[o * 4 + 0] = (float)(r * ds[0]);
-        tmp[o * 4 + 1] = (float)(r * ds[1]);
-        tmp[o * 4 + 2] = (float)(r * ds[2]);
-        tmp[o * 4 + 3] = 0.0f;
-        ok[o] = 1;
-      }
-    }
-  };
-  std::vector<std::thread> th;
-  int per = (n_az + (int)nthreads - 1) / (int)nthreads;
-  for (unsigned i = 0; i < nthreads; ++i) {
-    int j0 = (int)i * per, j1 = std::min(n_az, j0 + per);
-    if (j0 < j1) th.emplace_back(work, j0, j1);
-  }
-  for (auto& t : th) t.join();
-  int n = 0;
-  for (size_t o = 0; o < ok.size(); ++o)
-    if (ok[o]) { std::memcpy(out + (size_t)n * 4, &tmp[o * 4], 16); ++n; }
-  return n;
+  Layout lay;
+  lay.n_col = n_az;
+  return generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, capacity);
+}
+
+// The same scan cut and fired differently (see Layout): n_col columns from start_col, per-beam azimuth offsets ring_off_deg
+// (n_scans entries, may be null), beam-major order, counter-clockwise rotation.  Returns -3 when a surviving return lies
+// within kSeamMargin of an azimuth threshold of the reference's sweep walk (minimum_range decides what survives).
+int synth_scan_seam(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma, double max_range,
+                    double start_col, int n_col, const double* ring_off_deg, int laser_major, int ccw, double minimum_range,
+                    float* out, int capacity) {
+  Layout lay;
+  lay.start_col = start_col; lay.n_col = n_col; lay.ring_off = ring_off_deg; lay.laser_major = laser_major; lay.ccw = ccw;
+  const int n = generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, capacity);
+  if (n < 0) return n;
+  const int rc = check_seam_margins(out, n, n_scans, minimum_range);
+  return rc ? rc : n;
 }
 
 }  // extern "C"

@@ -36,7 +36,9 @@ extern "C" {
 #define ALOAM_ERR_CUDA (-5)
 #define ALOAM_ERR_NO_DEVICE (-6)
 #define ALOAM_ERR_RING_TOO_LARGE (-7)    /* a single ring holds more than ALOAM_MAX_RING_POINTS returns */
-#define ALOAM_ERR_NOT_RING_MAJOR (-8)    /* "last" cloud not in ascending ring order (laserOdometry.cpp:312-361 relies on it) */
+#define ALOAM_ERR_NOT_RING_MAJOR (-8)    /* "last" cloud with an int(intensity) outside 0..63 or two or more below an earlier
+                                            point's: every scanRegistration output has int_i >= max_{j<i} int_j - 1, and the
+                                            association's break tables rely on it (laserOdometry.cpp:310-361,400-455) */
 #define ALOAM_ERR_STATE (-9)             /* call sequence error, e.g. register before set_last */
 #define ALOAM_ERR_COMM (-10)
 
@@ -249,8 +251,9 @@ int aloam_odometry_associate(aloam_ctx* ctx, aloam_cloud_view sharp, aloam_cloud
                              const double t[3], int* corner_corr, int* plane_corr);
 /* residual blocks are 11 doubles [type(0 edge,1 plane,2 plane-norm), cp(3), a(3), b(3), s]; for type 1 b is the unit
  * normal LidarPlaneFactor precomputes (lidarFactor.hpp:64-65), for type 2 a is the unit normal and s = negative_OA_dot_norm.
- * For types 0 and 1 s is the functor's interpolation ratio (1.0 in the reference build; any value in [0, 1] is evaluated with the
- * slerp of lidarFactor.hpp:27-33 and its analytic Jacobian).  include/lidarFactor.hpp packs these records (PackBlock).
+ * For types 0 and 1 s is the functor's interpolation ratio (1.0 in the reference build; any other value is evaluated with the
+ * slerp of lidarFactor.hpp:27-33 and its analytic Jacobian.  The DISTORTION build makes s = frac(intensity) / 0.1, which lies
+ * in (-2, 10): a return with relTime < 0 has int(intensity) = ring - 1 and s near 10, one on ring 0 has s < 0).  include/lidarFactor.hpp packs these records (PackBlock).
  * JtJ (6x6 row-major), Jtr (6) in the tangent [dtheta(3), dt(3)] with Huber(0.1) applied, cost = sum 0.5 rho. */
 int aloam_normal_equations(aloam_ctx* ctx, const double* blocks, int n_blocks, const double x[7], double JtJ[36],
                            double Jtr[6], double* cost);
