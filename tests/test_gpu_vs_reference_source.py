@@ -42,20 +42,26 @@ def test_features_match_the_reference_source(sensor, index, aloam, orc, synth, s
 
 def test_odometry_poses_match_the_reference_source_chain(aloam, orc, synth, scans):
     """aloam_scan_to_pose per scan vs the reference's scanRegistration -> laserOdometry chain (its own source for feature
-    extraction, TransformToStart, correspondence search, block construction and pose integration): the north_star tolerance is
-    1e-4 m / 1e-4 rad, the bar here is ten times tighter"""
+    extraction, TransformToStart, correspondence search, block construction and pose integration): both correspondence counts
+    equal, the world pose within the bar of tests/test_gpu_vs_reference_chains.py.  The reference's VoxelGrid runs with the
+    device's tie order (index order; std::sort leaves equal voxel indices unordered), so the difference left is the device's"""
     import refsource
+    from test_gpu_vs_reference_chains import ODOM_BAR
     ns, _, mr = synth.SENSORS["VLP-16"][:3]
     reg = _load(refsource.ref_registration, ns, mr)
     odo = refsource.RefOdometry(_load(refsource.private_copy, "libref_odometry.so", "gpu_chain"))
     c = aloam.Aloam(n_scans=ns, max_points=40000)
-    moved = 0.0
+    moved = worst = 0.0
     for k in range(5):
         raw = scans("VLP-16", k, n_az=900)
-        r = reg.run(raw, orc.SORT_LITERAL)
+        r = reg.run(raw, orc.SORT_CANONICAL)
         st = odo.process(types.SimpleNamespace(**{n: r[n] for n in ("sharp", "less_sharp", "flat", "less_flat", "full")}), stamp=0.1 * (k + 1))
-        gq, gt, _ = c.scan_to_pose(raw)
-        assert np.abs(gt - st["tw"]).max() < 1e-5 and rot_angle(gq, st["qw"]) < 1e-5, (k, gt - st["tw"])
+        gq, gt, gst = c.scan_to_pose(raw)
+        worst = max(worst, float(np.abs(gt - st["tw"]).max()), rot_angle(gq, st["qw"]))
+        assert np.abs(gt - st["tw"]).max() <= ODOM_BAR and rot_angle(gq, st["qw"]) <= ODOM_BAR, (k, gt - st["tw"])
+        if k > 0:
+            assert [gst["n_corner_corr"], gst["n_plane_corr"]] == st["counts"].tolist(), (k, gst, st["counts"])
         moved = max(moved, float(np.abs(st["tw"]).max()))
     c.close()
+    print("measured VLP-16 chain vs the reference source: %.3g" % worst)
     assert moved > 0.05

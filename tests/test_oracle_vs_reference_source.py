@@ -178,7 +178,7 @@ def test_laser_mapping_source_ring_buffer_scrolls_like_the_oracle(orc):
     cm = orc.CubeMap()
     ident = np.array([0, 0, 0, 1.0])
     path = [(0, 0, 0), (60, -35, 12), (130, -80, 30), (260, -170, 75), (420, -290, 140), (300, -100, 60), (-90, 40, -30),
-            (-400, 380, -160), (-700, 600, -260), (-640, 610, -250)]
+            (-400, 380, -160), (-700, 600, -260), (-640, 610, -250), (-300, -200, 100), (200, -420, 200)]   # the last two: the shift towards +j
     for k, t in enumerate(path):
         t = np.array(t, float)
         corner = (rng.normal(size=(6, 4)) * [8, 8, 2, 0]).astype(np.float32)
