@@ -25,8 +25,10 @@ EXPORTED_SYMBOLS = [
     "aloam_comm_unique_id", "aloam_comm_init", "aloam_comm_uses_peer_memory", "aloam_map_upload_sharded", "aloam_scan_stream", "aloam_scan_stream_batch", "aloam_scan_stream_mapped", "aloam_transform_to_end", "aloam_mapper_reset", "aloam_mapper_step", "aloam_debug_seg_voxel_filter", "aloam_profile_enable", "aloam_profile_read", "aloam_launch_count",
     "aloam_scan_stream_mapped_batch", "aloam_mapper_debug_state_lane", "aloam_mapper_debug_cube_lane",
     "aloam_scan_stream_lanes", "aloam_debug_shard_emulate", "aloam_debug_map_sizes",
+    "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
 ]
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
+EXPORT_SURROUND, EXPORT_MAP = 0, 1
 
 
 class Config(C.Structure):
@@ -114,6 +116,9 @@ def lib():
         L.aloam_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_char_p]
         L.aloam_debug_shard_emulate.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
         L.aloam_debug_map_sizes.argtypes = [C.c_void_p, ip, ip]
+        L.aloam_mapper_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
+        L.aloam_set_registered_sink.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
+        L.aloam_registered_rows.argtypes = [C.c_void_p, C.POINTER(C.c_longlong), ip, C.c_int]
         _LIB = L
     return _LIB
 
@@ -274,6 +279,46 @@ class Aloam:
         out = CloudView()
         _check(lib().aloam_mapper_debug_cube_lane(self._h, int(lane), which, cube_index, C.byref(out)))
         return _out(out)
+
+    # --- the clouds the reference mapper publishes (laserMapping.cpp:806-848)
+    def mapper_export_size(self, what, lane=0):
+        n = C.c_longlong(0)
+        _check(lib().aloam_mapper_export(self._h, int(lane), int(what), None, 0, C.byref(n)))
+        return n.value
+
+    def mapper_export(self, what, lane=0, out=None):
+        """the cube store of `lane` in the reference's order (EXPORT_SURROUND: /laser_cloud_surround, EXPORT_MAP: /laser_cloud_map).
+        out=None: returns an (n, 4) float32 numpy array.  out = a float32 torch tensor (CUDA or host) of shape (m, 4): filled in
+        place (m >= n points), returns out[:n]."""
+        n = C.c_longlong(0)
+        if out is None:
+            size = self.mapper_export_size(what, lane)
+            arr = np.zeros((max(size, 1), 4), np.float32)
+            _check(lib().aloam_mapper_export(self._h, int(lane), int(what), arr.ctypes.data, arr.shape[0], C.byref(n)))
+            return arr[:n.value]
+        if out.dtype.itemsize != 4 or not out.is_contiguous() or out.dim() != 2 or out.shape[1] != 4:
+            raise ValueError("out is a contiguous (m, 4) float32 tensor")
+        _check(lib().aloam_mapper_export(self._h, int(lane), int(what), C.c_void_p(out.data_ptr()), out.shape[0], C.byref(n)))
+        return out[:n.value]
+
+    def set_registered_sink(self, sink):
+        """sink: a contiguous (m, 4) float32 torch tensor in device or pinned host memory that receives the registered full-
+        resolution cloud of every mapped row of the mapped stream calls (see registered_rows); None turns it off"""
+        if sink is None:
+            _check(lib().aloam_set_registered_sink(self._h, None, 0))
+            self._sink = None
+            return
+        if not sink.is_contiguous() or sink.dim() != 2 or sink.shape[1] != 4:
+            raise ValueError("the sink is a contiguous (m, 4) float32 tensor")
+        _check(lib().aloam_set_registered_sink(self._h, C.c_void_p(sink.data_ptr()), sink.shape[0]))
+        self._sink = sink   # kept alive while it is set
+
+    def registered_rows(self, rows):
+        """(begin, count) of the `rows` = n_scans x batch rows (scan-major) of the last mapped stream call: row r's registered
+        cloud is sink[begin[r] : begin[r] + count[r]]"""
+        begin = np.zeros(max(rows, 1), np.int64); count = np.zeros(max(rows, 1), np.int32)
+        _check(lib().aloam_registered_rows(self._h, begin.ctypes.data_as(C.POINTER(C.c_longlong)), count.ctypes.data_as(C.POINTER(C.c_int)), int(rows)))
+        return begin[:rows], count[:rows]
 
     def seg_voxel_filter(self, segs, leaves, idx_bits=31):
         """the mapper's segmented VoxelGrid over `segs` ((n, 4) float32 clouds, one leaf each) in one pass with `idx_bits`

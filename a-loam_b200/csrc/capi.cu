@@ -514,6 +514,30 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
   return scan_to_pose_impl(c, d_raw, n, 4, q_w, t_w, stats);
 }
 
+// The rows of a mapped stream call over the lane schedule `ops` (as scan_stream_run numbers scans, from the lanes' current
+// state, which it does not change): mapped[r] for the rows that go to the mapper; begin[r] = the sum of raws[r'].n over the mapped
+// rows r' < r, where row r's registered cloud starts in the sink.  Returns the sum over all mapped rows.
+static long long registered_layout(const aloam_ctx* c, const aloam_cloud_view* raws, const int* ops, int n_scans, int nb, std::vector<long long>* begin,
+                                   std::vector<char>* mapped) {
+  int scan[ALOAM_MAX_BATCH];
+  for (int l = 0; l < nb; ++l) scan[l] = c->lane_scan[l];
+  long long total = 0;
+  for (int k = 0; k < n_scans; ++k)
+    for (int l = 0; l < nb; ++l) {
+      const size_t r = (size_t)k * nb + l;
+      bool m = false;
+      if (ops[r] != ALOAM_LANE_IDLE) {
+        const int j = ops[r] == ALOAM_LANE_START ? 0 : scan[l];
+        scan[l] = j + 1;
+        m = j % c->cfg.mapping_skip_frame == 0;
+      }
+      if (begin) (*begin)[r] = total;
+      if (mapped) (*mapped)[r] = m;
+      if (m) total += raws[r].n;
+    }
+  return total;
+}
+
 // Pipelined form of aloam_scan_to_pose over `nb` lanes: ring binning of step k+1 (s_exa), per-ring extraction (s_ext), compaction
 // + index build (s_idx) run concurrently with association + LM of step k (main stream) and the host->device copies of step k+2
 // (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on a lane schedule
@@ -536,6 +560,16 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     return code;
   };
 #define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return fail(ALOAM_ERR_CUDA); } } while (0)
+  // registered clouds (aloam_set_registered_sink): every mapped row's ring-major cloud is stashed with its feature slot by stage C
+  // and moved into the world by k_register_full after the row's mapper frame; without a sink none of this is issued
+  const bool sink = map_poses && c->reg_sink;
+  const size_t rows = (size_t)n_scans * nb;
+  std::vector<char> row_mapped;
+  if (map_poses) {
+    c->reg_rows = -1;
+    c->reg_begin.assign(rows, 0); c->reg_count.assign(rows, 0); row_mapped.assign(rows, 0);
+    registered_layout(c, raws, ops, n_scans, nb, &c->reg_begin, &row_mapped);
+  }
   if (map_poses) {   // the mappers' error bits of this call
     for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
     const int rc = peer_err_reset(c); if (rc) return fail(rc);
@@ -584,6 +618,8 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     }
     // ---- stage A (ring binning) on s_exa: needs full[b] free, i.e. stage B of scan k-2 done
     STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_b[b], 0));
+    // with a sink, full[b] is also read by the stash copy of stage C (which waits on the mapper frame four steps back)
+    if (sink) STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_stash[b], 0));
     c->stream = c->s_exa;
     // A START re-arms the lane's ScanScalars slot (k_ring_scan arms it only for a lane that ran the step before) and, below, resets its pose.
     // At a lockstep call's first step these copies change nothing: k_ring_scan armed the slot with d_sc_init's four fields, start_ori /
@@ -610,6 +646,11 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_b[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_odo[(f + 1) % kFeatSlots], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the last mapper frame that read this slot (of frame f - kFeatSlots at the latest) is done
+    if (sink) {   // the ring-major cloud of every mapped row goes with the slot until its mapper frame has registered it
+      for (int i = 0; i < na; ++i)
+        if (map_scan[i]) { Lane& L = c->lanes[act[i]]; STREAM_TRY(cudaMemcpyAsync(L.feat[cur].full, L.d_full[b], (size_t)ns[i] * sizeof(Pt4), cudaMemcpyDeviceToDevice, c->s_idx)); }
+      STREAM_TRY(cudaEventRecord(c->ev_stash[b], c->s_idx));
+    }
     rc = run_features_b2(c, na, act, b, cur, false);
     if (rc) return fail(rc);
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
@@ -654,6 +695,15 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
       if (n_map > 0) {
         rc = mapper_step_device(c, n_map, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
         if (rc) return fail(rc);
+        if (sink) {   // /velodyne_cloud_registered of the mapped rows, before the lanes' next frame replaces the refined pose
+          const Pt4* src[ALOAM_MAX_BATCH]; const int* nf[ALOAM_MAX_BATCH]; Pt4* dst[ALOAM_MAX_BATCH];
+          for (int j = 0; j < n_map; ++j) {
+            const size_t r = (size_t)k * nb + in[j].lane;
+            src[j] = c->lanes[in[j].lane].feat[cur].full; nf[j] = c->d_scan_nfull + r; dst[j] = c->reg_sink + c->reg_begin[r];
+          }
+          rc = mapper_register_full_device(c, n_map, in, src, nf, dst, nmax);
+          if (rc) return fail(rc);
+        }
         STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
       }
       if (n_hf > 0) {
@@ -707,6 +757,10 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
+  if (map_poses) {   // the registered rows of this call (count 0 without a sink)
+    for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && row_mapped[r] ? c->h_scan_nfull[r] : 0;
+    c->reg_rows = (int)rows;
+  }
   // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
   if (map_poses) {
     c->pin->mapper_err = 0;
@@ -734,6 +788,7 @@ static int scan_stream_lockstep(aloam_ctx* c, const aloam_cloud_view* raws, int 
     if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
   }
   for (int i = 0; i < n_scans * nb; ++i) c->lockstep_ops[i] =c->frame == 0 && i < nb ? ALOAM_LANE_START : ALOAM_LANE_SCAN;
+  if (map_poses && c->reg_sink && registered_layout(c, raws, c->lockstep_ops, n_scans, nb, nullptr, nullptr) > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
   return scan_stream_run(c, raws, c->lockstep_ops, n_scans, nb, device_resident, poses, map_poses, stats_last, false);
@@ -791,6 +846,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
       if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
     }
   }
+  if (map_poses && c->reg_sink && registered_layout(c, raws, lane_ops, n_scans, batch, nullptr, nullptr) > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (run_err) { aloam_reset_odometry(c); return run_err; }
   if (map_poses) { int rc = mapper_ensure_lanes(c, batch); if (rc) return rc; }   // creates the cube stores this call needs
@@ -798,6 +854,33 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   c->lanes_mode = true;
   for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; }
   return scan_stream_run(c, raws, lane_ops, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
+}
+
+int aloam_set_registered_sink(aloam_ctx* c, float* data, long long capacity) {
+  if (!c || capacity < 0) return ALOAM_ERR_INVALID_ARG;
+  if (!data) { c->reg_sink = nullptr; c->reg_cap = 0; return ALOAM_OK; }
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  cudaPointerAttributes at = {};
+  if (cudaPointerGetAttributes(&at, data) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_INVALID_ARG; }
+  const bool device = (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == c->cfg.device;
+  if (!(device || at.type == cudaMemoryTypeHost) || !at.devicePointer) return ALOAM_ERR_INVALID_ARG;   // pageable: no device address
+  if (!c->ev_stash[1]) {   // first use: the stash of every lane, then the events (the last one marks the group as ready)
+    for (Lane& L : c->lanes)
+      for (int s = 0; s < kFeatSlots; ++s)
+        if (!L.feat[s].full) CUDA_CHECK_RET(dalloc(c, &L.feat[s].full, (size_t)c->max_points));
+    for (cudaEvent_t& e : c->ev_stash) if (!e) CUDA_CHECK_RET(ecreate(c, &e, cudaEventDisableTiming));
+  }
+  c->reg_sink = static_cast<Pt4*>(at.devicePointer);
+  c->reg_cap = capacity;
+  return ALOAM_OK;
+}
+
+int aloam_registered_rows(aloam_ctx* c, long long* begin, int* count, int rows) {
+  if (!c || rows < 0 || (rows > 0 && (!begin || !count))) return ALOAM_ERR_INVALID_ARG;
+  if (c->reg_rows < 0) return ALOAM_ERR_STATE;
+  if (rows != c->reg_rows) return ALOAM_ERR_INVALID_ARG;
+  for (int r = 0; r < rows; ++r) { begin[r] = c->reg_begin[r]; count[r] = c->reg_count[r]; }
+  return ALOAM_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ fine-grained

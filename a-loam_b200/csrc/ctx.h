@@ -61,6 +61,7 @@ struct FeatBuf {
   Pt4 *sharp = nullptr, *less_sharp = nullptr, *flat = nullptr, *less_flat = nullptr;
   int* counts = nullptr;           // [4] n_sharp, n_less_sharp, n_flat, n_less_flat (device)
   RabIndex g_ls = {}, g_lf = {};           // (azimuth bucket x ring) indices over less_sharp / less_flat
+  Pt4* full = nullptr;             // ring-major cloud of a mapped scan, kept for its registered cloud (created by aloam_set_registered_sink)
 };
 
 // Everything one trajectory owns on the device.  A context has cfg.max_batch of them; the single-trajectory entry points
@@ -101,6 +102,7 @@ struct PinnedScratch {
   int vox_nseg;             //                     1
   int vox_io[3];            //                     cloud size, filtered size, error word: {n, 0, 0}
   int vox_out_n;            //                     filtered size
+  long long export_total;   // aloam_mapper_export: points of the export
   double pose_in[7], pose_out[7];             // pose of the per-stage entry points
   double world[7];                            // fused pipeline: world pose of the scan
   double ne[28];                              // normal equations: J^T J upper 21, J^T r 6, cost
@@ -160,6 +162,18 @@ struct aloam_ctx {
   // a call issued on s_map, high-frequency poses included
   cudaEvent_t ev_feat[kFeatSlots] = {}, ev_idx[kFeatSlots] = {}, ev_odo[kFeatSlots] = {}, ev_mapdone[kFeatSlots] = {}, ev_h2d[2] = {}, ev_rawfree[2] = {},
               ev_a[2] = {}, ev_b[2] = {}, ev_cmp[2] = {}, ev_mapend = nullptr;
+  // registered full-resolution clouds of the mapped streams (aloam_set_registered_sink): the sink (device or page-locked host memory,
+  // written through its device address) and its capacity in points; ev_stash[b]: the copy of ring-major cloud b into the feature
+  // slot's stash is done (created with the stash).  reg_begin / reg_count: rows of the last mapped stream call, reg_rows of them.
+  Pt4* reg_sink = nullptr;
+  long long reg_cap = 0;
+  cudaEvent_t ev_stash[2] = {};
+  std::vector<long long> reg_begin;
+  std::vector<int> reg_count;
+  int reg_rows = -1;
+  // aloam_mapper_export: segment offsets [2 * 4851 + 2] and the staging buffer of host destinations, created on first use
+  long long* d_export_off = nullptr;
+  Pt4* d_export_stage = nullptr;
   double* h_poses = nullptr;     // pinned [kMaxStreamScans][7]
   double* d_poses = nullptr;     // device [kMaxStreamScans][7]: per-(scan, lane) world poses of a stream call (one D2H at the end)
   double* d_map_poses = nullptr; // device [kMaxStreamScans][7]: map-refined poses (aloam_scan_stream_mapped)
@@ -262,6 +276,7 @@ void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegB
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
+int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);
 int mapper_ensure_lanes(aloam_ctx* c, int nb);
 int* mapper_err_acc(aloam_ctx* c, int lane);
 int ensure_map_buffers(aloam_ctx* c);

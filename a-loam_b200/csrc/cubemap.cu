@@ -16,6 +16,8 @@
 //                      cube and the group leader advances the cube's running end (allocating a slab from the free list
 //                      for a cube that was empty) -- O(n) instead of the O(n^2 / 256) rank search of the first version;
 //   * the per-cube re-filter of the valid cubes as ONE segmented VoxelGrid over up to 150 segments, in place.
+//   * the published clouds (:806-848): k_export_sizes / k_export_gather read a lane's store out in the reference's order
+//                      (aloam_mapper_export), k_register_full moves a mapped scan's full cloud by the frame's refined pose.
 // Slabs are a POOL (1024 per cloud type, 16 k corner / 64 k surf points each: 1.3 GB) handed out on the device on first
 // insertion, not 4851 x 2 slabs (6.4 GB) up front.  A full slab or an exhausted pool drops the overflow and raises
 // ALOAM_FLAG_CUBE_OVERFLOW instead of failing the frame (the reference grows its cubes without bound between re-filters).
@@ -366,7 +368,22 @@ __device__ __forceinline__ void mapper_finish_body(MapperState* S) {
 __global__ void k_mapper_finish(const __grid_constant__ Batch<MapperLane> B) { mapper_finish_body(B.a[blockIdx.z].S); }   // grid (1, 1, lanes)
 
 
-// pointAssociateToMap (:154-163) in double, stored as float, then the cube of the stored point (:741-758)
+// pointAssociateToMap (:154-163): q_w_curr * point + t_w_curr in double in the operation order of Eigen, stored as float,
+// intensity kept.  (ux, uy, uz, w, tx, ty, tz) = parameters[7] of the frame.
+__device__ __forceinline__ Pt4 point_associate_to_map(const Pt4& p, double ux, double uy, double uz, double w, double tx, double ty, double tz) {
+  const double vx = (double)p.x, vy = (double)p.y, vz = (double)p.z;
+  double uvx = uy * vz - uz * vy, uvy = uz * vx - ux * vz, uvz = ux * vy - uy * vx;
+  uvx = uvx + uvx; uvy = uvy + uvy; uvz = uvz + uvz;
+  const double cx = uy * uvz - uz * uvy, cy = uz * uvx - ux * uvz, cz = ux * uvy - uy * uvx;
+  Pt4 s;
+  s.x = (float)(((vx + w * uvx) + cx) + tx);
+  s.y = (float)(((vy + w * uvy) + cy) + ty);
+  s.z = (float)(((vz + w * uvz) + cz) + tz);
+  s.i = p.i;
+  return s;
+}
+
+// pointAssociateToMap (:154-163), then the cube of the stored point (:741-758)
 // blockIdx.y = cloud (0 corner stack, 1 surf stack); the scratch of cloud 1 starts `scratch_stride` elements in
 __device__ __forceinline__ void cube_ids_body(const Pt4* __restrict__ stack0, const Pt4* __restrict__ stack1, const MapperState* __restrict__ S, Pt4* __restrict__ world,
                            int* __restrict__ cube, int scratch_stride) {
@@ -379,16 +396,7 @@ __device__ __forceinline__ void cube_ids_body(const Pt4* __restrict__ stack0, co
   const double ux = S->x[0], uy = S->x[1], uz = S->x[2], w = S->x[3], tx = S->x[4], ty = S->x[5], tz = S->x[6];
   const int c0 = S->cen[0], c1 = S->cen[1], c2 = S->cen[2];
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const Pt4 p = stack[i];
-    const double vx = (double)p.x, vy = (double)p.y, vz = (double)p.z;
-    double uvx = uy * vz - uz * vy, uvy = uz * vx - ux * vz, uvz = ux * vy - uy * vx;
-    uvx = uvx + uvx; uvy = uvy + uvy; uvz = uvz + uvz;
-    const double cx = uy * uvz - uz * uvy, cy = uz * uvx - ux * uvz, cz = ux * uvy - uy * uvx;
-    Pt4 s;
-    s.x = (float)(((vx + w * uvx) + cx) + tx);
-    s.y = (float)(((vy + w * uvy) + cy) + ty);
-    s.z = (float)(((vz + w * uvz) + cz) + tz);
-    s.i = p.i;
+    const Pt4 s = point_associate_to_map(stack[i], ux, uy, uz, w, tx, ty, tz);
     const int ci = cube_coord((double)s.x, c0), cj = cube_coord((double)s.y, c1), ck = cube_coord((double)s.z, c2);
     world[i] = s;
     cube[i] = (ci >= 0 && ci < CW && cj >= 0 && cj < CH && ck >= 0 && ck < CD) ? cube_index(ci, cj, ck) : -1;
@@ -398,6 +406,74 @@ __device__ __forceinline__ void cube_ids_body(const Pt4* __restrict__ stack0, co
 __global__ void k_cube_ids(const __grid_constant__ Batch<MapperLane> B, int scratch_stride) {
   const MapperLane& a = B.a[blockIdx.z];
   cube_ids_body(a.stack[0], a.stack[1], a.S, a.world, a.cube, scratch_stride);
+}
+
+
+// ---- the clouds the reference mapper publishes (:806-848)
+
+// grid (points, 1, lanes): /velodyne_cloud_registered (:838-848) of a mapped scan -- its ring-major full-resolution cloud moved
+// into the world frame by the frame's refined pose (pointAssociateToMap), read from S->x before the lane's next frame overwrites it
+struct RegFullLane {
+  const MapperState* S;
+  const Pt4* src;   // the scan's ring-major cloud
+  const int* n;     // its size (device)
+  Pt4* dst;
+};
+__global__ void k_register_full(const __grid_constant__ Batch<RegFullLane> B) {
+  const RegFullLane a = B.a[blockIdx.z];
+  const MapperState* __restrict__ S = a.S;
+  const double ux = S->x[0], uy = S->x[1], uz = S->x[2], w = S->x[3], tx = S->x[4], ty = S->x[5], tz = S->x[6];
+  const int n = *a.n;
+  const Pt4* __restrict__ src = a.src;
+  Pt4* __restrict__ dst = a.dst;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = point_associate_to_map(src[i], ux, uy, uz, w, tx, ty, tz);
+}
+
+// The segments of a store export in the reference's order, corner cube then surf cube of every cube: ALOAM_EXPORT_SURROUND the
+// valid cubes of the last frame in laserCloudSurroundInd order (:806-821, the same loop as the valid list), ALOAM_EXPORT_MAP
+// i = 0 .. 4850 (:823-836).  Segment s is cloud type s & 1 of cube export_cube(s).
+constexpr int kExportSegs = 2 * NCUBE;
+constexpr long long kExportStage = 4ll << 20;   // points of the staging buffer of a host destination (64 MB)
+__device__ __forceinline__ int export_segments(const MapperState* S, int what) { return what == ALOAM_EXPORT_SURROUND ? 2 * S->n_valid : kExportSegs; }
+__device__ __forceinline__ int export_cube(const MapperState* S, int what, int s) { return what == ALOAM_EXPORT_SURROUND ? S->valid[s >> 1] : s >> 1; }
+__device__ __forceinline__ int export_size(const MapperState* S, int what, int s) {
+  const int ty = s & 1, slab = S->slab_of[ty][export_cube(S, what, s)];
+  return slab < 0 ? 0 : S->cnt[ty][slab];
+}
+
+// one CTA of 1024: off[s] = points of the export before segment s (exclusive scan of the sizes), off[nseg] and off[kExportSegs + 1]
+// = the total (the second at a fixed place for the host to read back)
+__global__ void __launch_bounds__(1024) k_export_sizes(const MapperState* __restrict__ S, int what, long long* __restrict__ off) {
+  __shared__ long long s_part[1024];
+  const int tid = threadIdx.x, nseg = export_segments(S, what);
+  const int per = (nseg + 1023) / 1024, b = tid * per, e = min(b + per, nseg);
+  long long sum = 0;
+  for (int s = b; s < e; ++s) sum += export_size(S, what, s);
+  s_part[tid] = sum;
+  __syncthreads();
+  for (int d = 1; d < 1024; d <<= 1) {   // inclusive scan of the per-thread sums
+    const long long v = tid >= d ? s_part[tid - d] : 0;
+    __syncthreads();
+    s_part[tid] += v;
+    __syncthreads();
+  }
+  long long run = s_part[tid] - sum;
+  for (int s = b; s < e; ++s) { off[s] = run; run += export_size(S, what, s); }
+  if (tid == 1023) { off[nseg] = s_part[1023]; off[kExportSegs + 1] = s_part[1023]; }
+}
+
+// grid-stride over the segments: the points of segment s that fall in the window [lo, hi) of the export, 16-byte copies from the
+// slab to dst[position - lo]
+__global__ void __launch_bounds__(256) k_export_gather(const MapperState* __restrict__ S, int what, const long long* __restrict__ off, const Pt4* __restrict__ p0,
+                                                       const Pt4* __restrict__ p1, int cap0, int cap1, long long lo, long long hi, Pt4* __restrict__ dst) {
+  const int nseg = export_segments(S, what);
+  for (int s = blockIdx.x; s < nseg; s += gridDim.x) {
+    const long long o = off[s], b = max(o, lo), e = min(off[s + 1], hi);
+    if (b >= e) continue;   // (a segment with points has a slab)
+    const int ty = s & 1, slab = S->slab_of[ty][export_cube(S, what, s)];
+    const Pt4* __restrict__ src = (ty ? p1 : p0) + (size_t)slab * (ty ? cap1 : cap0);
+    for (long long i = b + threadIdx.x; i < e; i += blockDim.x) dst[i - lo] = src[i - o];
+  }
 }
 
 
@@ -638,6 +714,19 @@ int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
   return ALOAM_OK;
 }
 
+// The registered full-resolution clouds of the nb lanes of the frame mapper_step_device has just issued, on the current stream
+// (the mapper stream, before any later frame): record l moves the src[l] cloud of *n_full[l] points (device) by the refined pose of
+// lane in[l].lane into dst[l].  n_upper bounds every cloud size.
+int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper) {
+  if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
+  Batch<RegFullLane> B = {};
+  for (int l = 0; l < nb; ++l) B.a[l] = RegFullLane{static_cast<Mapper*>(c->mapper[in[l].lane])->d_state, src[l], n_full[l], dst[l]};
+  const int blocks = std::max(1, std::min((n_upper + 255) / 256, std::max(1, c->sms * 2 / nb)));
+  launch_ex(c, KID_CUBES, k_register_full, dim3(blocks, 1, nb), dim3(256), 0, 1, false, B);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 // the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
 int* mapper_err_acc(aloam_ctx* c, int lane) { return &static_cast<Mapper*>(c->mapper[lane])->d_state->err_acc; }
 
@@ -737,6 +826,43 @@ int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, al
   const int n = s < 0 ? 0 : m->h_state->cnt[which][s];
   out->data = reinterpret_cast<const float*>(c->h_out[4]); out->n = n; out->stride_floats = 4;
   if (n > 0) CUDA_CHECK_RET(cudaMemcpy(c->h_out[4], m->d_pts[which] + (size_t)s * m->cap[which], (size_t)n * sizeof(Pt4), cudaMemcpyDeviceToHost));
+  return ALOAM_OK;
+}
+
+int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long capacity, long long* n_out) {
+  if (!c || !n_out || capacity < 0 || lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
+  if (what != ALOAM_EXPORT_SURROUND && what != ALOAM_EXPORT_MAP) return ALOAM_ERR_INVALID_ARG;
+  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
+  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, c->d_export_off);
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, c->d_export_off + kExportSegs + 1, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  const long long n = c->pin->export_total;
+  *n_out = n;
+  if (!out && capacity == 0) return ALOAM_OK;   // the size only
+  if (!out) return ALOAM_ERR_INVALID_ARG;
+  if (capacity < n) return ALOAM_ERR_CAPACITY;
+  if (n == 0) return ALOAM_OK;
+  cudaPointerAttributes at = {};
+  CUDA_CHECK_RET(cudaPointerGetAttributes(&at, out));
+  const int blocks = std::min(kExportSegs, c->sms * 8);
+  if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) {   // written in place
+    LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], 0ll, n,
+           reinterpret_cast<Pt4*>(out));
+  } else {   // host memory: windows of the export through the bounded staging buffer, one device-to-host copy each
+    if (!c->d_export_stage) CUDA_CHECK_RET(dalloc(c, &c->d_export_stage, (size_t)kExportStage));
+    for (long long lo = 0; lo < n; lo += kExportStage) {
+      const long long hi = std::min(n, lo + kExportStage);
+      LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], lo, hi,
+             c->d_export_stage);
+      CUDA_CHECK_RET(cudaMemcpyAsync(out + 4 * lo, c->d_export_stage, (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyDeviceToHost, c->stream));
+    }
+  }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
 

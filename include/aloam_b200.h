@@ -299,6 +299,41 @@ int aloam_mapper_debug_cube(aloam_ctx* ctx, int which, int cube_index, aloam_clo
 int aloam_mapper_debug_state_lane(aloam_ctx* ctx, int lane, int centre[3], int* n_valid, int valid[125], double q_wmap_wodom[4],
                                   double t_wmap_wodom[3], long long totals[2]);
 int aloam_mapper_debug_cube_lane(aloam_ctx* ctx, int lane, int which, int cube_index, aloam_cloud_view* out);
+/* ---- the clouds the reference mapper publishes (laserMapping.cpp:806-848).
+ * aloam_mapper_export copies the cube store of lane `lane` (0: aloam_mapper_step and the single-trajectory calls) out in the
+ * reference's order, corner cube then surf cube of every cube:
+ *   ALOAM_EXPORT_SURROUND  /laser_cloud_surround (:806-821): the valid cubes of the lane's last frame, in the order of
+ *                          aloam_mapper_debug_state's valid list (laserCloudSurroundInd);
+ *   ALOAM_EXPORT_MAP       /laser_cloud_map (:823-836): all 4851 cubes, i = 0 .. 4850.
+ * out: 4 floats per point, device or host memory (pageable or pinned; the copy kind is inferred from the address).  A host
+ * destination is filled through a device staging buffer of at most 4 M points (created on first use, released by aloam_destroy).
+ * *n_out is always set to the size of the export; out = NULL with capacity = 0 asks for the size only.  capacity < *n_out
+ * returns ALOAM_ERR_CAPACITY and writes nothing.  ALOAM_ERR_INVALID_ARG for a bad `what` or lane, ALOAM_ERR_STATE while the lane's
+ * cube store does not exist.  The call reads the store as it is when it is made: after a stream call, the store of that call's
+ * last frame.  The reference publishes the surround every 5th and the map every 20th frame (ROS control plane, not modelled):
+ * a caller who wants that cadence ends its stream calls at those frames.  On a rank of a sharded job the store is the whole one
+ * (it is replicated), so the export is the same on every rank. */
+#define ALOAM_EXPORT_SURROUND 0
+#define ALOAM_EXPORT_MAP 1
+int aloam_mapper_export(aloam_ctx* ctx, int lane, int what, float* out, long long capacity, long long* n_out);
+/* /velodyne_cloud_registered (:838-848) of the mapped streams.  While a sink is set, every MAPPED row (scan k, lane l) of
+ * aloam_scan_stream_mapped, _mapped_batch and _lanes (with map_poses) -- the rows with j % cfg.mapping_skip_frame == 0 -- writes the
+ * scan's ring-major full-resolution cloud (aloam_extract_features' `full`, intensity = ring + 0.1 relTime) moved into the world
+ * frame by the row's refined pose exactly as pointAssociateToMap (:154-163: in double, stored as float, intensity kept).  With
+ * cfg.distortion = 1 the cloud is not de-skewed first, as in the reference (its TransformToEnd of the full cloud is under if (0)).
+ * data: device memory or page-locked host memory (written by the kernel through its device address), `capacity` points of 4
+ * floats; pageable memory returns ALOAM_ERR_INVALID_ARG.  data = NULL turns the sink off (the default): the stream calls then
+ * issue exactly what they issue without this feature.  The first set call allocates a stash of 4 ring-major clouds per lane
+ * (4 x cfg.max_points x 16 B for each of cfg.max_batch lanes), kept until aloam_destroy.
+ * Layout: every call writes from offset 0; row r = k * batch + l begins at the sum of raws[r'].n over the call's mapped rows
+ * r' < r (a bound known before the call, since the ring-major cloud never holds more points than the raw scan) and holds
+ * count = n_full points; the gaps are left untouched.  If that sum over all of the call's mapped rows exceeds `capacity`, the call
+ * returns ALOAM_ERR_CAPACITY before any state changes.
+ * aloam_registered_rows: begin / count of the `rows` = n_scans x batch rows of the last mapped stream call (skipped and idle rows,
+ * and every row of a call made without a sink, have count 0).  ALOAM_ERR_STATE before any mapped stream call, ALOAM_ERR_INVALID_ARG
+ * when `rows` is not that call's row count. */
+int aloam_set_registered_sink(aloam_ctx* ctx, float* data, long long capacity);
+int aloam_registered_rows(aloam_ctx* ctx, long long* begin, int* count, int rows);
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
