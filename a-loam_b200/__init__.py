@@ -26,7 +26,9 @@ EXPORTED_SYMBOLS = [
     "aloam_scan_stream_mapped_batch", "aloam_mapper_debug_state_lane", "aloam_mapper_debug_cube_lane",
     "aloam_scan_stream_lanes", "aloam_debug_shard_emulate", "aloam_debug_map_sizes",
     "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
+    "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
 ]
+ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 EXPORT_SURROUND, EXPORT_MAP = 0, 1
 
@@ -51,6 +53,11 @@ class Stats(C.Structure):
         return {"n_corner_corr": self.n_corner_corr, "n_plane_corr": self.n_plane_corr, "lm_iters": self.lm_iters,
                 "accepted_steps": self.accepted_steps, "flags": self.flags, "termination": list(self.termination),
                 "init_cost": self.init_cost, "final_cost": self.final_cost, "ms_total": self.ms_total}
+
+
+class SnapshotInfo(C.Structure):
+    _fields_ = [("version", C.c_int), ("mapped", C.c_int), ("n_scans", C.c_int), ("scan_index", C.c_int), ("bytes", C.c_longlong),
+                ("map_points", C.c_longlong), ("world", C.c_double * 7)]
 
 
 class AloamError(RuntimeError):
@@ -119,6 +126,9 @@ def lib():
         L.aloam_mapper_export.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
         L.aloam_set_registered_sink.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
         L.aloam_registered_rows.argtypes = [C.c_void_p, C.POINTER(C.c_longlong), ip, C.c_int]
+        L.aloam_lane_save.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
+        L.aloam_lane_restore.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
+        L.aloam_snapshot_check.argtypes = [C.c_void_p, C.c_longlong, C.POINTER(SnapshotInfo)]
         _LIB = L
     return _LIB
 
@@ -154,6 +164,27 @@ def _views(ptrs, counts, stride):
     for i in range(len(ptrs)):
         views[i] = CloudView(C.cast(C.c_void_p(int(ptrs[i])), C.POINTER(C.c_float)), int(counts[i]), stride)
     return views
+
+
+def _blob(blob):
+    """(address, size in bytes, object to keep alive) of a snapshot: a numpy array, bytes, or a contiguous torch tensor (device
+    or host memory)"""
+    if hasattr(blob, "data_ptr"):
+        if not blob.is_contiguous():
+            raise ValueError("a snapshot tensor is contiguous")
+        return C.c_void_p(blob.data_ptr()), blob.numel() * blob.element_size(), blob
+    a = np.ascontiguousarray(np.frombuffer(blob, np.uint8) if isinstance(blob, (bytes, bytearray)) else blob)
+    return C.c_void_p(a.ctypes.data), a.nbytes, a
+
+
+def snapshot_info(blob):
+    """checks a lane snapshot in host memory without a context or a GPU (aloam_snapshot_check) -> {version, mapped, n_scans,
+    scan_index, bytes, map_points, world}; raises AloamError(ERR_SNAPSHOT) when it is malformed"""
+    ptr, n, keep = _blob(blob)
+    info = SnapshotInfo()
+    _check(lib().aloam_snapshot_check(ptr, n, C.byref(info)))
+    return {"version": info.version, "mapped": bool(info.mapped), "n_scans": info.n_scans, "scan_index": info.scan_index,
+            "bytes": info.bytes, "map_points": info.map_points, "world": np.array(info.world[:])}
 
 
 def default_config(n_scans):
@@ -467,6 +498,26 @@ class Aloam:
                                              _dp(out) if mapped else None, st))
         self.last_batch_stats = [s.as_dict() for s in st]
         return odom, out
+
+    def lane_save(self, lane, out=None):
+        """snapshot of the trajectory `lane` runs (aloam_lane_save).  out=None: returns it as a numpy uint8 array.  out = a
+        contiguous uint8 torch tensor (CUDA, or pinned / pageable host memory) with room for it: written in place, returns
+        out[:n] (a 1-D view)."""
+        n = C.c_longlong(0)
+        if out is None:
+            _check(lib().aloam_lane_save(self._h, int(lane), None, 0, C.byref(n)))
+            arr = np.zeros(max(n.value, 1), np.uint8)
+            _check(lib().aloam_lane_save(self._h, int(lane), arr.ctypes.data, arr.size, C.byref(n)))
+            return arr[:n.value]
+        if out.element_size() != 1 or not out.is_contiguous():
+            raise ValueError("out is a contiguous uint8 tensor")
+        _check(lib().aloam_lane_save(self._h, int(lane), C.c_void_p(out.data_ptr()), out.numel(), C.byref(n)))
+        return out.view(-1)[:n.value]
+
+    def lane_restore(self, lane, blob):
+        """makes `lane` run the trajectory of a snapshot (aloam_lane_restore): a numpy array, bytes, or a torch tensor"""
+        ptr, n, keep = _blob(blob)
+        _check(lib().aloam_lane_restore(self._h, int(lane), ptr, n))
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

@@ -44,6 +44,7 @@ const char* aloam_strerror(int code) {
     case ALOAM_ERR_NOT_RING_MAJOR: return "a cloud's int(intensity) is not a ring, or falls two below an earlier one";
     case ALOAM_ERR_STATE: return "call sequence error";
     case ALOAM_ERR_COMM: return "communicator error";
+    case ALOAM_ERR_SNAPSHOT: return "snapshot malformed, of another format version, or taken under a configuration that changes results";
     default: return "unknown error";
   }
 }
@@ -297,6 +298,21 @@ void sync_all_streams(aloam_ctx* c) {
 
 }  // namespace
 
+// The search index over the "last" clouds of feature set `slot` of lane `lane` (n_ls / n_lf points, their counts already queued on
+// c->stream), then the check of every point's ring against the break tables just built (k_ring_offsets).  Synchronises;
+// ALOAM_ERR_NOT_RING_MAJOR when a cloud is not ring-major.  aloam_odometry_set_last and aloam_lane_restore.
+int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf) {
+  FeatBuf& f = c->lanes[lane].feat[slot];
+  CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
+  run_grid_build(c, 1, &lane, slot, n_ls, n_lf);
+  if (n_ls > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (n_ls + 255) / 256, 256, 0, f.less_sharp, n_ls, f.g_ls.fwd_end, c->d_err);
+  if (n_lf > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (n_lf + 255) / 256, 256, 0, f.less_flat, n_lf, f.g_lf.fwd_end, c->d_err);
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return c->pin->ring_err ? ALOAM_ERR_NOT_RING_MAJOR : ALOAM_OK;
+}
+
 extern "C" {
 
 // ------------------------------------------------------------------------------------------------ feature extraction
@@ -363,15 +379,8 @@ int aloam_odometry_set_last(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cl
   int* lc = c->pin->last_counts;
   lc[0] = 0; lc[1] = corner_last.n; lc[2] = 0; lc[3] = surf_last.n;
   CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, lc, 16, cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
-  run_grid_build(c, 1, kLane0, kApiLast, corner_last.n, surf_last.n);
-  // checked against the break tables of the index just built (k_ring_offsets)
-  if (corner_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (corner_last.n + 255) / 256, 256, 0, f.less_sharp, corner_last.n, f.g_ls.fwd_end, c->d_err);
-  if (surf_last.n > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (surf_last.n + 255) / 256, 256, 0, f.less_flat, surf_last.n, f.g_lf.fwd_end, c->d_err);
-  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  CUDA_CHECK_RET(cudaGetLastError());
-  if (c->pin->ring_err) return ALOAM_ERR_NOT_RING_MAJOR;
+  rc = index_last_clouds(c, 0, kApiLast, corner_last.n, surf_last.n);
+  if (rc) return rc;
   c->have_last = true;
   return ALOAM_OK;
 }

@@ -9,6 +9,7 @@
 #include <vector>
 #include "../../include/aloam_b200.h"
 #include "kernels.h"
+#include "snapshot.h"
 
 namespace aloam {
 // the buffers of one scan-to-map registration (mapping.cu): the two indexed submaps, the neighbours found by k_map_knn5, the
@@ -107,6 +108,8 @@ struct PinnedScratch {
   double world[7];                            // fused pipeline: world pose of the scan
   double ne[28];                              // normal equations: J^T J upper 21, J^T r 6, cost
   double mapper_pose_in[7], mapper_pose_out[7];
+  SnapHeader snap;          // aloam_lane_save / _restore: the snapshot's header
+  int snap_counts[4];       //                             counts of the lane's "last" feature set
 };
 
 }  // namespace
@@ -211,6 +214,9 @@ struct aloam_ctx {
   // runs `release` in reverse order of acquisition
   std::vector<cudaStream_t> streams;
   std::vector<std::function<void()>> release;
+  // aloam_lane_save / _restore of mapped lanes: the store table of a snapshot, pinned and on the device, created on first use
+  SnapStore* h_snap_store = nullptr;
+  SnapStore* d_snap_store = nullptr;
 };
 
 namespace {
@@ -279,6 +285,11 @@ int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);
 int mapper_ensure_lanes(aloam_ctx* c, int nb);
 int* mapper_err_acc(aloam_ctx* c, int lane);
+void mapper_slab_caps(const aloam_ctx* c, int cap[2]);
+int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head);
+int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device);
+int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device);
+int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf);
 int ensure_map_buffers(aloam_ctx* c);
 int map_reg_alloc(aloam_ctx* c, MapReg* r);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);

@@ -30,6 +30,7 @@ namespace {
 constexpr int CW = 21, CH = 21, CD = 11, NCUBE = CW * CH * CD;   // laserCloudWidth / Height / Depth (:77-82)
 constexpr int kMaxValid = 128;
 constexpr int kPool = 1024;                                      // physical slabs per cloud type
+static_assert(NCUBE == kSnapCubes && kMaxValid == kSnapValid && kPool == kSnapPool, "the snapshot format describes this store");
 
 struct MapperState {
   double q_wmap_wodom[4], t_wmap_wodom[3];   // :116-117
@@ -476,6 +477,66 @@ __global__ void __launch_bounds__(256) k_export_gather(const MapperState* __rest
   }
 }
 
+// ---- lane snapshots (aloam_lane_restore): the inverse of the ALOAM_EXPORT_MAP export
+
+// One CTA of 1024: the store a snapshot's table H describes.  State of a fresh trajectory first (the caller has zeroed S), then
+// the cubes with a count >= 0 take slabs 0, 1, 2, ... of their type in cube order (the rest of the pool stays free, ascending),
+// off[s] = exclusive prefix of the segment sizes in export order (segment 2 i + t: cube i, type t; off[kExportSegs] and
+// off[kExportSegs + 1] = the total, as k_export_sizes), and the fields that outlive a frame.
+__global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, long long* __restrict__ off) {
+  __shared__ long long s_pts[1024];
+  __shared__ int s_slabs[2][1024];
+  const int tid = threadIdx.x;
+  mapper_fresh_state(S);
+  const int per = (NCUBE + 1023) / 1024, b = tid * per, e = min(b + per, NCUBE);
+  long long pts = 0;
+  int n0 = 0, n1 = 0;
+  for (int i = b; i < e; ++i) {
+    const int c0 = H->count[0][i], c1 = H->count[1][i];
+    pts += max(c0, 0) + max(c1, 0);
+    n0 += c0 >= 0; n1 += c1 >= 0;
+  }
+  s_pts[tid] = pts; s_slabs[0][tid] = n0; s_slabs[1][tid] = n1;
+  __syncthreads();   // (also orders mapper_fresh_state's writes before the ones below)
+  for (int d = 1; d < 1024; d <<= 1) {   // inclusive scans of the per-thread sums
+    const long long v = tid >= d ? s_pts[tid - d] : 0;
+    const int v0 = tid >= d ? s_slabs[0][tid - d] : 0, v1 = tid >= d ? s_slabs[1][tid - d] : 0;
+    __syncthreads();
+    s_pts[tid] += v; s_slabs[0][tid] += v0; s_slabs[1][tid] += v1;
+    __syncthreads();
+  }
+  long long run = s_pts[tid] - pts;
+  int next[2] = {s_slabs[0][tid] - n0, s_slabs[1][tid] - n1};
+  for (int i = b; i < e; ++i)
+    for (int ty = 0; ty < 2; ++ty) {
+      const int n = H->count[ty][i];
+      off[2 * i + ty] = run;
+      if (n >= 0) { const int s = next[ty]++; S->slab_of[ty][i] = s; S->cnt[ty][s] = n; run += n; }
+    }
+  if (tid == 1023) { off[kExportSegs] = run; off[kExportSegs + 1] = run; S->free_top = s_slabs[0][1023]; S->free_top2 = s_slabs[1][1023]; }
+  if (tid < kMaxValid) S->valid[tid] = tid < H->n_valid ? H->valid[tid] : 0;
+  if (tid == 0) {
+    for (int a = 0; a < 3; ++a) S->cen[a] = H->cen[a];
+    S->n_valid = H->n_valid;
+    S->frames = H->frames;
+    for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = H->q_wmap_wodom[k];
+    for (int k = 0; k < 3; ++k) S->t_wmap_wodom[k] = H->t_wmap_wodom[k];
+  }
+}
+
+// grid-stride over the segments, the inverse of k_export_gather: the points of segment s that fall in the window [lo, hi) of the
+// payload, from src[position - lo] into the cube's slab
+__global__ void __launch_bounds__(256) k_store_import_scatter(const MapperState* __restrict__ S, const long long* __restrict__ off, const Pt4* __restrict__ src,
+                                                              long long lo, long long hi, Pt4* __restrict__ p0, Pt4* __restrict__ p1, int cap0, int cap1) {
+  for (int s = blockIdx.x; s < kExportSegs; s += gridDim.x) {
+    const long long o = off[s], b = max(o, lo), e = min(off[s + 1], hi);
+    if (b >= e) continue;   // (a segment with points has a slab)
+    const int ty = s & 1, slab = S->slab_of[ty][s >> 1];
+    Pt4* __restrict__ dst = (ty ? p1 : p0) + (size_t)slab * (ty ? cap1 : cap0);
+    for (long long i = b + threadIdx.x; i < e; i += blockDim.x) dst[i - o] = src[i - lo];
+  }
+}
+
 
 // stable append of the stack points to their cubes (push_back order = stack order, :759-767).  ONE CTA per cloud (blockIdx.x: the
 // corner and the surf store are independent, the two appends run side by side): the stack is walked in
@@ -581,8 +642,7 @@ int ensure_mapper(aloam_ctx* c, int lane) {
   Mapper* m = new (std::nothrow) Mapper();
   if (!m) return ALOAM_ERR_CUDA;
   own(c, [m] { delete m; });
-  m->cap[0] = std::min(16384, c->max_points);
-  m->cap[1] = std::min(65536, c->max_points);
+  mapper_slab_caps(c, m->cap);
   m->max_sub = c->cfg.max_map_points;
   bool ok = true;
   for (int t = 0; t < 2 && ok; ++t) {
@@ -613,7 +673,116 @@ int ensure_mapper(aloam_ctx* c, int lane) {
   return ALOAM_OK;
 }
 
+// k_export_sizes of `what` over the store of m into c->d_export_off (created on first use); *n = the size of the export.  Synchronises.
+int export_sizes(aloam_ctx* c, const Mapper* m, int what, long long* n) {
+  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
+  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, c->d_export_off);
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, c->d_export_off + kExportSegs + 1, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  *n = c->pin->export_total;
+  return ALOAM_OK;
+}
+
+// the staging buffer of host sources and destinations (kExportStage points), created on first use
+int export_stage(aloam_ctx* c) {
+  if (!c->d_export_stage) CUDA_CHECK_RET(dalloc(c, &c->d_export_stage, (size_t)kExportStage));
+  return ALOAM_OK;
+}
+
+// the n points of the export export_sizes has just sized, into dst on c->stream (not synchronised): device memory is written in
+// place, host memory in windows of the staging buffer, one device-to-host copy each
+int export_gather(aloam_ctx* c, const Mapper* m, int what, long long n, char* dst, bool device) {
+  const int blocks = std::min(kExportSegs, c->sms * 8);
+  if (device) {
+    LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], 0ll, n,
+           reinterpret_cast<Pt4*>(dst));
+  } else {
+    const int rc = export_stage(c); if (rc) return rc;
+    for (long long lo = 0; lo < n; lo += kExportStage) {
+      const long long hi = std::min(n, lo + kExportStage);
+      LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], lo, hi,
+             c->d_export_stage);
+      CUDA_CHECK_RET(cudaMemcpyAsync(dst + lo * sizeof(Pt4), c->d_export_stage, (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyDeviceToHost, c->stream));
+    }
+  }
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 }  // namespace
+
+// points per slab of the two cloud types (16 k corner / 64 k surf, at most cfg.max_points)
+void mapper_slab_caps(const aloam_ctx* c, int cap[2]) {
+  cap[0] = std::min(16384, c->max_points);
+  cap[1] = std::min(65536, c->max_points);
+}
+
+// ---- lane snapshots (snapshot.cu): the cube store of a lane in the slab-free form of SnapStore
+
+// the table of lane `lane`'s store into *head (host memory): the fields that outlive a frame and every cube's point count, -1 for a
+// cube without a slab; head->n_points = the size of the ALOAM_EXPORT_MAP export.  The store exists.  Synchronises.
+int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head) {
+  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  const MapperState* S = m->h_state;
+  std::memset(head, 0, sizeof(*head));
+  for (int a = 0; a < 3; ++a) head->cen[a] = S->cen[a];
+  head->n_valid = S->n_valid;
+  for (int v = 0; v < S->n_valid; ++v) head->valid[v] = S->valid[v];
+  head->frames = S->frames;
+  for (int k = 0; k < 4; ++k) head->q_wmap_wodom[k] = S->q_wmap_wodom[k];
+  for (int k = 0; k < 3; ++k) head->t_wmap_wodom[k] = S->t_wmap_wodom[k];
+  long long n = 0;
+  for (int ty = 0; ty < 2; ++ty)
+    for (int i = 0; i < NCUBE; ++i) {
+      const int s = S->slab_of[ty][i];
+      head->count[ty][i] = s < 0 ? -1 : S->cnt[ty][s];
+      n += s < 0 ? 0 : S->cnt[ty][s];
+    }
+  head->n_points = n;
+  return ALOAM_OK;
+}
+
+// the n points of lane `lane`'s store in ALOAM_EXPORT_MAP order into dst (device memory when `device`, else host memory), on
+// c->stream, not synchronised; n is what mapper_store_tables reported (ALOAM_ERR_STATE when the store disagrees)
+int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device) {
+  const Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  long long total = 0;
+  int rc = export_sizes(c, m, ALOAM_EXPORT_MAP, &total); if (rc) return rc;
+  if (total != n) return ALOAM_ERR_STATE;
+  return n > 0 ? export_gather(c, m, ALOAM_EXPORT_MAP, n, dst, device) : ALOAM_OK;
+}
+
+// Makes lane `lane`'s store (it exists) the one a validated snapshot table describes: *head (pinned host memory) goes to the
+// device, k_store_import_tables rebuilds the tables, k_store_import_scatter moves the head->n_points points of pts into the
+// slabs -- from device memory in place, from host memory through the staging buffer.  Synchronises.
+int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device) {
+  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
+  if (!c->d_snap_store) CUDA_CHECK_RET(dalloc(c, &c->d_snap_store, 1));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_snap_store, head, sizeof(SnapStore), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
+  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, c->d_export_off);
+  const long long n = head->n_points;
+  const int blocks = std::min(kExportSegs, c->sms * 8);
+  if (device && n > 0) {
+    LAUNCH(c, KID_CUBES, k_store_import_scatter, blocks, 256, 0, m->d_state, c->d_export_off, reinterpret_cast<const Pt4*>(pts), 0ll, n, m->d_pts[0], m->d_pts[1],
+           m->cap[0], m->cap[1]);
+  } else if (n > 0) {
+    const int rc = export_stage(c); if (rc) return rc;
+    for (long long lo = 0; lo < n; lo += kExportStage) {
+      const long long hi = std::min(n, lo + kExportStage);
+      CUDA_CHECK_RET(cudaMemcpyAsync(c->d_export_stage, pts + lo * sizeof(Pt4), (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyHostToDevice, c->stream));
+      LAUNCH(c, KID_CUBES, k_store_import_scatter, blocks, 256, 0, m->d_state, c->d_export_off, c->d_export_stage, lo, hi, m->d_pts[0], m->d_pts[1],
+             m->cap[0], m->cap[1]);
+    }
+  }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
 
 // One frame of alaserMapping's process() for nb trajectories ("lanes") on the current stream, entirely on the device: every launch
 // covers all lanes, lane l in blockIdx.z, and each lane has its own cube store, stack filter buffers and registration set, so
@@ -835,12 +1004,8 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
   if (!c->mapper[lane]) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   const Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
-  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
-  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, c->d_export_off);
-  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, c->d_export_off + kExportSegs + 1, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  CUDA_CHECK_RET(cudaGetLastError());
-  const long long n = c->pin->export_total;
+  long long n = 0;
+  int rc = export_sizes(c, m, what, &n); if (rc) return rc;
   *n_out = n;
   if (!out && capacity == 0) return ALOAM_OK;   // the size only
   if (!out) return ALOAM_ERR_INVALID_ARG;
@@ -848,19 +1013,8 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
   if (n == 0) return ALOAM_OK;
   cudaPointerAttributes at = {};
   CUDA_CHECK_RET(cudaPointerGetAttributes(&at, out));
-  const int blocks = std::min(kExportSegs, c->sms * 8);
-  if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) {   // written in place
-    LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], 0ll, n,
-           reinterpret_cast<Pt4*>(out));
-  } else {   // host memory: windows of the export through the bounded staging buffer, one device-to-host copy each
-    if (!c->d_export_stage) CUDA_CHECK_RET(dalloc(c, &c->d_export_stage, (size_t)kExportStage));
-    for (long long lo = 0; lo < n; lo += kExportStage) {
-      const long long hi = std::min(n, lo + kExportStage);
-      LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], lo, hi,
-             c->d_export_stage);
-      CUDA_CHECK_RET(cudaMemcpyAsync(out + 4 * lo, c->d_export_stage, (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyDeviceToHost, c->stream));
-    }
-  }
+  rc = export_gather(c, m, what, n, reinterpret_cast<char*>(out), at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
+  if (rc) return rc;
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;

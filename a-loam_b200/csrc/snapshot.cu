@@ -1,0 +1,229 @@
+// Lane snapshots (include/aloam_b200.h: aloam_lane_save, aloam_lane_restore, aloam_snapshot_check): everything later scans of a
+// lane of aloam_scan_stream_lanes depend on, written out and read back exactly, so a trajectory can be suspended and resumed in
+// any lane of any context with the same result-affecting configuration.  A lane's state between two stream calls:
+//   - its warm start and world pose (Lane::d_pose, d_world);
+//   - its "last" less-sharp / less-flat clouds, in feature slot (frame - 1) mod kFeatSlots -- the slot the next step reads as
+//     "last" -- whose search index is rebuilt from the clouds on restore;
+//   - the index of its next scan (lane_scan) and its mode (lane_mapped);
+//   - mapped: its cube store, in the slab-free form of SnapStore (cubemap.cu saves and restores it).
+// Format: snapshot.h.
+#include <cstring>
+#include "common.cuh"
+#include "ctx.h"
+
+namespace {
+
+constexpr char kMagic[8] = {'A', 'L', 'O', 'A', 'M', 'L', 'S', '1'};
+
+// byte offset of the store section (the end of the unmapped snapshot)
+long long store_offset(const SnapHeader& h) { return (long long)sizeof(SnapHeader) + 16ll * ((long long)h.n_less_sharp + h.n_less_flat); }
+
+// the header on its own: magic, version, sizes of the sections before the store table.  n_bytes must be what the header says
+// the snapshot holds; a mapped snapshot must hold its store table at least.
+int check_header(const SnapHeader& h, long long n_bytes) {
+  if (std::memcmp(h.magic, kMagic, 8) != 0 || h.version != kSnapVersion) return ALOAM_ERR_SNAPSHOT;
+  if ((h.mapped != 0 && h.mapped != 1) || h.scan_index < 1 || h.n_less_sharp < 0 || h.n_less_flat < 0) return ALOAM_ERR_SNAPSHOT;
+  if (h.total_bytes != n_bytes) return ALOAM_ERR_SNAPSHOT;
+  if (!h.mapped) return n_bytes == store_offset(h) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
+  if (h.slab_cap[0] < 1 || h.slab_cap[1] < 1 || h.max_map_points < 1) return ALOAM_ERR_SNAPSHOT;
+  return n_bytes >= store_offset(h) + (long long)sizeof(SnapStore) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
+}
+
+// the store table of a mapped snapshot whose header passed check_header: the valid list, every count within its slab capacity,
+// at most kSnapPool cubes of a type holding a slab, and a payload of exactly the counted points that ends the snapshot
+int check_store(const SnapHeader& h, const SnapStore& s) {
+  if (s.n_valid < 0 || s.n_valid > 125) return ALOAM_ERR_SNAPSHOT;
+  for (int v = 0; v < s.n_valid; ++v)
+    if (s.valid[v] < 0 || s.valid[v] >= kSnapCubes) return ALOAM_ERR_SNAPSHOT;
+  long long points = 0;
+  for (int ty = 0; ty < 2; ++ty) {
+    int slabs = 0;
+    for (int i = 0; i < kSnapCubes; ++i) {
+      const int n = s.count[ty][i];
+      if (n < -1 || n > h.slab_cap[ty]) return ALOAM_ERR_SNAPSHOT;
+      if (n >= 0) { ++slabs; points += n; }
+    }
+    if (slabs > kSnapPool) return ALOAM_ERR_SNAPSHOT;
+  }
+  if (s.n_points != points) return ALOAM_ERR_SNAPSHOT;
+  return h.total_bytes == store_offset(h) + (long long)sizeof(SnapStore) + 16 * points ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
+}
+
+// the configuration fields of the header that can change a result
+void fingerprint(const aloam_ctx* c, SnapHeader* h) {
+  const aloam_config& g = c->cfg;
+  h->n_scans = g.n_scans; h->distortion = g.distortion; h->mapping_skip_frame = g.mapping_skip_frame;
+  h->outer_iters = g.outer_iters; h->inner_iters = g.inner_iters;
+  h->minimum_range = g.minimum_range; h->line_res = g.line_res; h->plane_res = g.plane_res;
+  mapper_slab_caps(c, h->slab_cap);
+  h->max_map_points = g.max_map_points;
+  h->huber = g.huber; h->dist_sq_thresh = g.dist_sq_thresh; h->nearby_scan = g.nearby_scan;
+}
+
+// the snapshot's configuration against the context's, bit patterns for the floating-point fields.  The scan-to-map fields count
+// only for a mapped snapshot: an odometry-only trajectory moves between contexts that map differently (or not at all).
+bool same_config(const SnapHeader& s, const SnapHeader& c) {
+  auto same = [](const void* a, const void* b, size_t n) { return std::memcmp(a, b, n) == 0; };
+  const bool odometry = s.n_scans == c.n_scans && s.distortion == c.distortion && s.outer_iters == c.outer_iters && s.inner_iters == c.inner_iters &&
+                        same(&s.minimum_range, &c.minimum_range, 4) && same(&s.huber, &c.huber, 8) && same(&s.dist_sq_thresh, &c.dist_sq_thresh, 8) &&
+                        same(&s.nearby_scan, &c.nearby_scan, 8);
+  const bool mapping = s.mapping_skip_frame == c.mapping_skip_frame && same(&s.line_res, &c.line_res, 4) && same(&s.plane_res, &c.plane_res, 4) &&
+                       same(s.slab_cap, c.slab_cap, 8) && s.max_map_points == c.max_map_points;
+  return odometry && (!s.mapped || mapping);
+}
+
+// where a lane's "last" clouds are between two stream calls: the feature slot of the context's latest step
+int last_slot(const aloam_ctx* c) { return (c->frame + kFeatSlots - 1) % kFeatSlots; }
+
+// the kind of a caller's snapshot buffer: 1 device memory of this context's device, 0 host memory (pinned or pageable), -1 memory
+// the call cannot use (another device, or device memory not aligned to 16 bytes: the store's points are moved as 16-byte words)
+int buffer_kind(const aloam_ctx* c, const void* p) {
+  cudaPointerAttributes at = {};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+  if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged)
+    return (at.type == cudaMemoryTypeDevice && at.device != c->cfg.device) || reinterpret_cast<uintptr_t>(p) % 16 ? -1 : 1;
+  return 0;
+}
+
+// n bytes between the caller's buffer and host memory, on c->stream (host memory: at once)
+int put(aloam_ctx* c, char* dst, bool device, const void* src, size_t n) {
+  if (device) CUDA_CHECK_RET(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, c->stream));
+  else std::memcpy(dst, src, n);
+  return ALOAM_OK;
+}
+int fetch(aloam_ctx* c, void* dst, const char* src, bool device, size_t n) {
+  if (!device) { std::memcpy(dst, src, n); return ALOAM_OK; }
+  CUDA_CHECK_RET(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  return ALOAM_OK;
+}
+
+int ensure_snap_store(aloam_ctx* c) {
+  if (!c->h_snap_store) CUDA_CHECK_RET(halloc(c, &c->h_snap_store, 1));
+  return ALOAM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int aloam_snapshot_check(const void* blob, long long n_bytes, aloam_snapshot_info* info) {
+  if (!blob || n_bytes < 0) return ALOAM_ERR_INVALID_ARG;
+  if (n_bytes < (long long)sizeof(SnapHeader)) return ALOAM_ERR_SNAPSHOT;
+  const char* b = static_cast<const char*>(blob);
+  SnapHeader h;
+  std::memcpy(&h, b, sizeof(h));
+  int rc = check_header(h, n_bytes); if (rc) return rc;
+  long long map_points = 0;
+  if (h.mapped) {
+    std::vector<char> buf(sizeof(SnapStore));   // (the blob need not be aligned)
+    std::memcpy(buf.data(), b + store_offset(h), sizeof(SnapStore));
+    const SnapStore* s = reinterpret_cast<const SnapStore*>(buf.data());
+    rc = check_store(h, *s); if (rc) return rc;
+    map_points = s->n_points;
+  }
+  if (info) {
+    info->version = h.version; info->mapped = h.mapped; info->n_scans = h.n_scans; info->scan_index = h.scan_index;
+    info->bytes = h.total_bytes; info->map_points = map_points;
+    for (int k = 0; k < 7; ++k) info->world[k] = h.world[k];
+  }
+  return ALOAM_OK;
+}
+
+int aloam_lane_save(aloam_ctx* c, int lane, void* out, long long capacity, long long* n_bytes) {
+  if (!c || !n_bytes || capacity < 0 || lane < 0 || lane >= c->n_lanes) return ALOAM_ERR_INVALID_ARG;
+  if (!c->lanes_mode || !c->lane_running[lane]) return ALOAM_ERR_STATE;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const Lane& L = c->lanes[lane];
+  const FeatBuf& f = L.feat[last_slot(c)];
+  SnapHeader& h = c->pin->snap;
+  std::memset(&h, 0, sizeof(h));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->snap_counts, f.counts, 16, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(h.warm, L.d_pose, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(h.world, L.d_world, 56, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  std::memcpy(h.magic, kMagic, 8);
+  h.version = kSnapVersion;
+  h.mapped = c->lane_mapped[lane];
+  h.scan_index = c->lane_scan[lane];
+  h.n_less_sharp = c->pin->snap_counts[1];
+  h.n_less_flat = c->pin->snap_counts[3];
+  fingerprint(c, &h);
+  const long long store = store_offset(h);
+  h.total_bytes = store;
+  int rc = ALOAM_OK;
+  if (h.mapped) {
+    rc = ensure_snap_store(c); if (rc) return rc;
+    rc = mapper_store_tables(c, lane, c->h_snap_store); if (rc) return rc;
+    h.total_bytes += (long long)sizeof(SnapStore) + 16 * c->h_snap_store->n_points;
+  }
+  *n_bytes = h.total_bytes;
+  if (!out && capacity == 0) return ALOAM_OK;   // the size only
+  if (!out) return ALOAM_ERR_INVALID_ARG;
+  if (capacity < h.total_bytes) return ALOAM_ERR_CAPACITY;
+  const int kind = buffer_kind(c, out);
+  if (kind < 0) return ALOAM_ERR_INVALID_ARG;
+  char* o = static_cast<char*>(out);
+  rc = put(c, o, kind, &h, sizeof(h)); if (rc) return rc;
+  if (h.n_less_sharp > 0) CUDA_CHECK_RET(cudaMemcpyAsync(o + sizeof(h), f.less_sharp, 16 * (size_t)h.n_less_sharp, cudaMemcpyDefault, c->stream));
+  if (h.n_less_flat > 0) CUDA_CHECK_RET(cudaMemcpyAsync(o + sizeof(h) + 16 * (size_t)h.n_less_sharp, f.less_flat, 16 * (size_t)h.n_less_flat, cudaMemcpyDefault, c->stream));
+  if (h.mapped) {
+    rc = put(c, o + store, kind, c->h_snap_store, sizeof(SnapStore)); if (rc) return rc;
+    rc = mapper_store_points(c, lane, c->h_snap_store->n_points, o + store + sizeof(SnapStore), kind); if (rc) return rc;
+  }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
+int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_bytes) {
+  if (!c || !blob || n_bytes < 0 || lane < 0 || lane >= c->n_lanes) return ALOAM_ERR_INVALID_ARG;
+  if (sharded_job(c)) return ALOAM_ERR_STATE;   // as aloam_scan_stream_lanes
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const int kind = buffer_kind(c, blob);
+  if (kind < 0) return ALOAM_ERR_INVALID_ARG;
+  // as at a START: the lane's trajectory, if any, ends here, and the context runs lanes from now on
+  c->lanes_mode = true;
+  c->lane_running[lane] = false;
+  // ---- validation, on the host, before anything is written to the device
+  if (n_bytes < (long long)sizeof(SnapHeader)) return ALOAM_ERR_SNAPSHOT;
+  const char* b = static_cast<const char*>(blob);
+  SnapHeader& h = c->pin->snap;
+  int rc = fetch(c, &h, b, kind, sizeof(h)); if (rc) return rc;
+  rc = check_header(h, n_bytes); if (rc) return rc;
+  SnapHeader mine = {};
+  fingerprint(c, &mine);
+  if (!same_config(h, mine)) return ALOAM_ERR_SNAPSHOT;
+  const long long store = store_offset(h);
+  if (h.mapped) {
+    rc = ensure_snap_store(c); if (rc) return rc;
+    rc = fetch(c, c->h_snap_store, b + store, kind, sizeof(SnapStore)); if (rc) return rc;
+    rc = check_store(h, *c->h_snap_store); if (rc) return rc;
+  }
+  if (h.n_less_sharp > c->max_points || h.n_less_flat > c->max_points) return ALOAM_ERR_CAPACITY;
+  if (h.mapped) { rc = mapper_ensure_lanes(c, lane + 1); if (rc) return rc; }   // creates the lane's cube store if needed
+  // ---- odometry: the "last" clouds into the slot the next step reads, their index and ring check, the poses, the armed scalars
+  Lane& L = c->lanes[lane];
+  const int slot = last_slot(c);
+  FeatBuf& f = L.feat[slot];
+  if (h.n_less_sharp > 0) CUDA_CHECK_RET(cudaMemcpyAsync(f.less_sharp, b + sizeof(h), 16 * (size_t)h.n_less_sharp, cudaMemcpyDefault, c->stream));
+  if (h.n_less_flat > 0) CUDA_CHECK_RET(cudaMemcpyAsync(f.less_flat, b + sizeof(h) + 16 * (size_t)h.n_less_sharp, 16 * (size_t)h.n_less_flat, cudaMemcpyDefault, c->stream));
+  int* lc = c->pin->snap_counts;
+  lc[0] = 0; lc[1] = h.n_less_sharp; lc[2] = 0; lc[3] = h.n_less_flat;
+  CUDA_CHECK_RET(cudaMemcpyAsync(f.counts, lc, 16, cudaMemcpyHostToDevice, c->stream));
+  rc = index_last_clouds(c, lane, slot, h.n_less_sharp, h.n_less_flat); if (rc) return rc;
+  CUDA_CHECK_RET(cudaMemcpyAsync(L.d_pose, h.warm, 56, cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(L.d_world, h.world, 56, cudaMemcpyHostToDevice, c->stream));
+  // k_ring_scan arms a lane's next ScanScalars slot only when the lane ran the step before
+  CUDA_CHECK_RET(cudaMemcpyAsync(L.d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->stream));
+  // ---- the cube store
+  if (h.mapped) { rc = mapper_store_restore(c, lane, c->h_snap_store, b + store + sizeof(SnapStore), kind); if (rc) return rc; }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  c->lane_running[lane] = true;
+  c->lane_mapped[lane] = h.mapped != 0;
+  c->lane_scan[lane] = h.scan_index;
+  return ALOAM_OK;
+}
+
+}  // extern "C"

@@ -41,6 +41,8 @@ extern "C" {
                                             association's break tables rely on it (laserOdometry.cpp:310-361,400-455) */
 #define ALOAM_ERR_STATE (-9)             /* call sequence error, e.g. register before set_last */
 #define ALOAM_ERR_COMM (-10)
+#define ALOAM_ERR_SNAPSHOT (-11)         /* snapshot malformed, of another format version, or taken under a configuration that
+                                            changes results (aloam_lane_restore, aloam_snapshot_check) */
 
 #define ALOAM_MAX_RING_POINTS 4096
 #define ALOAM_MAX_BATCH 16
@@ -205,7 +207,8 @@ int aloam_scan_stream_mapped_batch(aloam_ctx* ctx, const aloam_cloud_view* raws,
  *   ALOAM_LANE_SCAN   the next scan of the trajectory the lane runs;
  *   ALOAM_LANE_IDLE   no scan: the lane's trajectory, if any, has ended (its view is not read; its pose rows are NaN).
  * Lifecycle: START, then SCAN at every step, then IDLE until the next START (a START may also directly follow a SCAN).  An
- * IDLE step ends the trajectory: a lane cannot pause.  Lanes batch .. cfg.max_batch-1 are IDLE at every step of the call.
+ * IDLE step ends the trajectory; to pause one, save it with aloam_lane_save and resume it later with aloam_lane_restore, in
+ * any lane of any context (below).  Lanes batch .. cfg.max_batch-1 are IDLE at every step of the call.
  * A START scan only initialises (laserOdometry.cpp:267-271): its odometry pose is the identity and, mapped, it is the first
  * mapper frame on a freshly reset cube store.
  * map_poses == NULL: odometry only, as aloam_scan_stream_batch; otherwise scan-to-map too, as aloam_scan_stream_mapped_batch
@@ -234,6 +237,63 @@ int aloam_scan_stream_lanes(aloam_ctx* ctx, const aloam_cloud_view* raws, const 
 int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" clouds (all trajectories); ends every lane of
                                              aloam_scan_stream_lanes and allows the lockstep calls again; the next scan of
                                              every lane is scan 0 for cfg.mapping_skip_frame */
+
+/* ---- lane snapshots: suspend a trajectory of aloam_scan_stream_lanes and resume it in any lane of any context, on any GPU, in
+ * this process or a later one -- to time-slice more trajectories than a context has lanes, park a vehicle whose scans stop for a
+ * while, move a trajectory to balance load, or survive a restart in the middle of a long recording.
+ * aloam_lane_save writes the state later scans of `lane` depend on, as it stands after the last stream call (the call changes
+ * nothing): its warm start and world pose, its "last" less-sharp / less-flat clouds, the index of its next scan and its mode,
+ * and, mapped, its cube store.  out: device memory of the context's device (16-byte aligned), or host memory, pinned or pageable
+ * (the copy kind is inferred from the address; the store's points go through the staging buffer of aloam_mapper_export).
+ * *n_bytes is always set to the snapshot's size; out = NULL with capacity = 0 asks for the size only; capacity < *n_bytes
+ * returns ALOAM_ERR_CAPACITY and writes nothing.  ALOAM_ERR_STATE unless the context runs lanes and `lane` is running.  (The
+ * lockstep calls have no snapshots: aloam_scan_stream_lanes with batch 1 is the single-trajectory call.)  Size: 256 B + 16 B per
+ * "last" point, and, mapped, 39 424 B + 16 B per map point.
+ * aloam_lane_restore makes `lane` (0 <= lane < cfg.max_batch) run the saved trajectory: a lanes call that continues it with
+ * ALOAM_LANE_SCAN, in the saved mode (map_poses set or not), gives exactly what the uninterrupted trajectory would have -- odometry
+ * and map poses, stats, cube store, published and registered clouds.  blob: as `out` of aloam_lane_save, n_bytes its size
+ * exactly.  It needs the configuration the snapshot was taken under in every field that can change a result: n_scans,
+ * minimum_range, outer_iters, inner_iters, huber, dist_sq_thresh, nearby_scan and distortion, and for a mapped snapshot also
+ * line_res, plane_res, mapping_skip_frame, max_map_points and the slab capacities min(16384, max_points) / min(65536, max_points)
+ * (floating-point fields compared bit for bit).  max_points beyond the slab capacities, max_batch, max_ring_points and device do
+ * not count.  Errors: ALOAM_ERR_INVALID_ARG (bad lane or buffer: nothing changes), ALOAM_ERR_STATE on a rank of a sharded job or
+ * an emulating context (nothing changes).  Otherwise the call first ends whatever the lane ran and puts the context in lanes
+ * mode, as a START does (the lockstep calls are refused until aloam_reset_odometry); then it checks the whole snapshot on the
+ * host before it writes anything to the device -- ALOAM_ERR_SNAPSHOT for a bad magic or version, a size that does not match the
+ * sections, a count above the slab capacity, more than 1024 cubes of a type holding a slab, a payload that is not the sum of
+ * the counts, a valid list of more than 125 entries or with an index outside 0 .. 4850, or a configuration that differs --
+ * ALOAM_ERR_CAPACITY when a "last" cloud exceeds cfg.max_points, ALOAM_ERR_NOT_RING_MAJOR when it is not ring-major (the check
+ * of aloam_odometry_set_last).  It creates the lane's cube store if needed.  After any failure the lane is not running; no other
+ * lane changes.
+ * aloam_snapshot_check runs the host checks of aloam_lane_restore on a snapshot in host memory without a context or a GPU (no
+ * configuration is compared) and, when info is not NULL, describes it: format version, mode, n_scans, the index of its next scan,
+ * its size, its map points and the world pose of its last scan.
+ *
+ * Snapshot format, version 1: little-endian, sections 16-byte aligned.
+ *   1. header, 256 bytes:
+ *        0 char magic[8] "ALOAMLS1"   8 int32 version (1)   12 int32 mapped (0 / 1)   16 int64 total_bytes
+ *       24 int32 scan_index (the lane's next scan in its trajectory, >= 1)   28 int32 n_less_sharp   32 int32 n_less_flat
+ *       configuration: 36 int32 n_scans   40 int32 distortion   44 int32 mapping_skip_frame   48 int32 outer_iters
+ *       52 int32 inner_iters   56 float minimum_range   60 float line_res   64 float plane_res   68 int32 slab_cap[2]
+ *       76 int32 max_map_points   80 double huber   88 double dist_sq_thresh   96 double nearby_scan
+ *      104 double warm[7] (q_last_curr xyzw, t_last_curr: the next scan's warm start)   160 double world[7]   216 zero to 256
+ *   2. at 256: n_less_sharp, then n_less_flat points of 4 floats (x, y, z, intensity) -- the lane's "last" clouds
+ *   3. mapped snapshots only, at S = 256 + 16 (n_less_sharp + n_less_flat): the cube store
+ *      S+0 int32 cen[3]   S+12 int32 n_valid (<= 125)   S+16 int32 valid[128] (unused entries 0)   S+528 int32 frames
+ *      S+532 zero   S+536 double q_wmap_wodom[4]   S+568 double t_wmap_wodom[3]
+ *      S+592 int32 count[2][4851]: points of corner (0) / surf (1) cube i; -1 = the cube holds no slab (0 = a slab, no points)
+ *      S+39400 zero   S+39408 int64 n_points (the sum of the counts >= 0)   S+39416 zero
+ *      S+39424 n_points points of 4 floats in ALOAM_EXPORT_MAP order: corner cube i, then surf cube i, for i = 0 .. 4850
+ *   total_bytes = S, or S + 39424 + 16 n_points for a mapped snapshot.  Which slab a cube held is not saved: only which cubes hold
+ *   one, and the points, change results. */
+typedef struct aloam_snapshot_info {
+  int version, mapped, n_scans, scan_index;
+  long long bytes, map_points;
+  double world[7];
+} aloam_snapshot_info;
+int aloam_lane_save(aloam_ctx* ctx, int lane, void* out, long long capacity, long long* n_bytes);
+int aloam_lane_restore(aloam_ctx* ctx, int lane, const void* blob, long long n_bytes);
+int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapshot_info* info);
 
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
  * interpolation ratio, then carry it to the sweep end with (q_last_curr, t_last_curr); the intensity keeps only the scan id.
