@@ -27,10 +27,12 @@ EXPORTED_SYMBOLS = [
     "aloam_scan_stream_lanes", "aloam_debug_shard_emulate", "aloam_debug_map_sizes",
     "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
     "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
+    "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 EXPORT_SURROUND, EXPORT_MAP = 0, 1
+PRIOR_MAP = -1   # `lane` of mapper_export: the context's prior map
 
 
 class Config(C.Structure):
@@ -129,6 +131,9 @@ def lib():
         L.aloam_lane_save.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
         L.aloam_lane_restore.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
         L.aloam_snapshot_check.argtypes = [C.c_void_p, C.c_longlong, C.POINTER(SnapshotInfo)]
+        L.aloam_prior_map_load.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
+        L.aloam_prior_map_clear.argtypes = [C.c_void_p]
+        L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
         _LIB = L
     return _LIB
 
@@ -518,6 +523,24 @@ class Aloam:
         """makes `lane` run the trajectory of a snapshot (aloam_lane_restore): a numpy array, bytes, or a torch tensor"""
         ptr, n, keep = _blob(blob)
         _check(lib().aloam_lane_restore(self._h, int(lane), ptr, n))
+
+    # --- localisation against a prior map
+    def prior_map_load(self, blob):
+        """makes the cube store of a mapped lane snapshot the context's prior map (aloam_prior_map_load): a numpy array, bytes,
+        or a torch tensor"""
+        ptr, n, keep = _blob(blob)
+        _check(lib().aloam_prior_map_load(self._h, ptr, n))
+
+    def prior_map_clear(self):
+        _check(lib().aloam_prior_map_clear(self._h))
+
+    def lane_localise(self, lane, q_init, t_init):
+        """arms `lane`: its next LANE_START in a mapped scan_stream_lanes call begins a trajectory that registers against the
+        prior map, its T_wmap_wodom starting at (q_init xyzw, t_init)"""
+        q = np.ascontiguousarray(q_init, np.float64); t = np.ascontiguousarray(t_init, np.float64)
+        if q.shape != (4,) or t.shape != (3,):
+            raise ValueError("q_init is 4 doubles (x, y, z, w), t_init 3")
+        _check(lib().aloam_lane_localise(self._h, int(lane), _dp(q), _dp(t)))
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

@@ -72,7 +72,7 @@ int aloam_reset_odometry(aloam_ctx* c) {
   if (c->s_idx) CUDA_CHECK_RET(cudaStreamSynchronize(c->s_idx));   // an index build of the last synchronous call may still be running
   c->frame = 0; c->cur = 0; c->have_last = false;
   c->lanes_mode = false;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = c->lane_mapped[l] = false; c->lane_scan[l] = 0; }
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = c->lane_mapped[l] = c->lane_localising[l] = c->lane_armed[l] = false; c->lane_scan[l] = 0; }
   return ALOAM_OK;
 }
 
@@ -552,9 +552,11 @@ static long long registered_layout(const aloam_ctx* c, const aloam_cloud_view* r
 // (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on a lane schedule
 // `ops` (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
 // (record i = lane act[i], which owns the buffers, pose slots and cube store); an all-idle step issues nothing.  reset_stores: a
-// START also resets its lane's cube store.  The caller has checked the views and the schedule and created the cube stores.
+// START also resets its lane's cube store.  row_loc (or null: none): the rows that localise -- their lanes register against the
+// prior map in one locate frame per step, beside the mapping frame of the step's other lanes.  The caller has checked the views
+// and the schedule and created the cube stores and locators.
 static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int* ops, int n_scans, int nb, int device_resident, double* poses,
-                           double* map_poses, aloam_stats* stats_last, bool reset_stores) {
+                           double* map_poses, aloam_stats* stats_last, bool reset_stores, const char* row_loc = nullptr) {
   StreamGuard guard(c);
   cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
@@ -580,7 +582,10 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     registered_layout(c, raws, ops, n_scans, nb, &c->reg_begin, &row_mapped);
   }
   if (map_poses) {   // the mappers' error bits of this call
-    for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
+    for (int l = 0; l < nb; ++l) {   // (a lane that only localises has no cube store)
+      if (c->mapper[l]) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
+      if (c->locator[l]) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
+    }
     const int rc = peer_err_reset(c); if (rc) return fail(rc);
   }
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
@@ -691,30 +696,38 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
       //      only on a frame that read it.
       STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
       c->stream = c->s_map;
-      MapperIn in[ALOAM_MAX_BATCH], hf[ALOAM_MAX_BATCH];
-      int n_map = 0, n_hf = 0;
+      //      The step's registered lanes that localise go to one locate frame against the prior map instead (no cube store).
+      MapperIn in[ALOAM_MAX_BATCH], loc[ALOAM_MAX_BATCH], hf[ALOAM_MAX_BATCH];
+      int n_map = 0, n_loc = 0, n_hf = 0;
       for (int i = 0; i < na; ++i) {
         const int l = act[i];
         const FeatBuf& fc = c->lanes[l].feat[cur];
         const size_t slot = ((size_t)k * nb + l) * 7;
+        const bool localise = row_loc && row_loc[(size_t)k * nb + l];
         const MapperIn r{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
-                         reset_stores && op[l] == ALOAM_LANE_START};
-        if (map_scan[i]) in[n_map++] = r; else hf[n_hf++] = r;
+                         reset_stores && op[l] == ALOAM_LANE_START, localise};
+        if (!map_scan[i]) hf[n_hf++] = r; else if (localise) loc[n_loc++] = r; else in[n_map++] = r;
       }
+      // /velodyne_cloud_registered of a frame's rows, before the lanes' next frame replaces the refined pose
+      auto register_rows = [&](const MapperIn* fr, int n) {
+        const Pt4* src[ALOAM_MAX_BATCH]; const int* nf[ALOAM_MAX_BATCH]; Pt4* dst[ALOAM_MAX_BATCH];
+        for (int j = 0; j < n; ++j) {
+          const size_t r = (size_t)k * nb + fr[j].lane;
+          src[j] = c->lanes[fr[j].lane].feat[cur].full; nf[j] = c->d_scan_nfull + r; dst[j] = c->reg_sink + c->reg_begin[r];
+        }
+        return mapper_register_full_device(c, n, fr, src, nf, dst, nmax);
+      };
       if (n_map > 0) {
         rc = mapper_step_device(c, n_map, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
         if (rc) return fail(rc);
-        if (sink) {   // /velodyne_cloud_registered of the mapped rows, before the lanes' next frame replaces the refined pose
-          const Pt4* src[ALOAM_MAX_BATCH]; const int* nf[ALOAM_MAX_BATCH]; Pt4* dst[ALOAM_MAX_BATCH];
-          for (int j = 0; j < n_map; ++j) {
-            const size_t r = (size_t)k * nb + in[j].lane;
-            src[j] = c->lanes[in[j].lane].feat[cur].full; nf[j] = c->d_scan_nfull + r; dst[j] = c->reg_sink + c->reg_begin[r];
-          }
-          rc = mapper_register_full_device(c, n_map, in, src, nf, dst, nmax);
-          if (rc) return fail(rc);
-        }
-        STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
+        if (sink) { rc = register_rows(in, n_map); if (rc) return fail(rc); }
       }
+      if (n_loc > 0) {
+        rc = locate_step_device(c, n_loc, loc, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+        if (rc) return fail(rc);
+        if (sink) { rc = register_rows(loc, n_loc); if (rc) return fail(rc); }
+      }
+      if (n_map + n_loc > 0) STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
       if (n_hf > 0) {
         rc = mapper_high_freq_device(c, n_hf, hf);
         if (rc) return fail(rc);
@@ -733,7 +746,11 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     STREAM_TRY(cudaEventRecord(c->ev_mapend, c->s_map));   // the last mapper frame and the last high-frequency poses
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapend, 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
-    for (int l = 0; l < nb; ++l) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+    for (int l = 0; l < nb; ++l) {
+      c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
+      if (c->mapper[l]) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+      if (c->locator[l]) STREAM_TRY(cudaMemcpyAsync(&c->pin->locate_err_lane[l], locator_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+    }
     const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return fail(rc);
   }
   for (int l = 0; l < nb; ++l) {
@@ -773,7 +790,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
   // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
   if (map_poses) {
     c->pin->mapper_err = 0;
-    for (int l = 0; l < nb; ++l) c->pin->mapper_err |= c->pin->mapper_err_lane[l];
+    for (int l = 0; l < nb; ++l) c->pin->mapper_err |= c->pin->mapper_err_lane[l] | c->pin->locate_err_lane[l];
     if (c->pin->mapper_err & 1) return ALOAM_ERR_CAPACITY;
     if (c->pin->peer_err) return ALOAM_ERR_COMM;   // a peer did not answer: a map pose rests on a partial sum
   }
@@ -831,8 +848,12 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   if (c && sharded_job(c)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   if (!stream_args_ok(c, raws, n_scans, batch, odom_poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
   // the whole schedule is checked against the lanes' state before anything changes; lanes >= batch are idle all call
-  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH];   // lane state after this call
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { running[l] = l < batch && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; }
+  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH], localising[ALOAM_MAX_BATCH], armed[ALOAM_MAX_BATCH];   // lane state after this call
+  bool maps[ALOAM_MAX_BATCH] = {}, localises[ALOAM_MAX_BATCH] = {};   // the lane has a mapping / a localising scan in this call
+  std::vector<char> row_loc((size_t)n_scans * batch, 0);              // the rows that localise
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) {
+    running[l] = l < batch && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; localising[l] = c->lane_localising[l]; armed[l] = c->lane_armed[l];
+  }
   for (size_t i = 0; i < (size_t)n_scans * batch; ++i)
     if (lane_ops[i] < ALOAM_LANE_IDLE || lane_ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
   int run_err = ALOAM_OK;   // a scan that cannot run fails the call like a run-time error
@@ -850,7 +871,12 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
       }
       // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
       if (op == ALOAM_LANE_SCAN && (!running[l] || mapped[l] != (map_poses != nullptr))) return ALOAM_ERR_STATE;
-      if (op == ALOAM_LANE_START) { running[l] = true; mapped[l] = map_poses != nullptr; }
+      if (op == ALOAM_LANE_START) {   // a mapped START consumes the lane's arming (aloam_lane_localise): the trajectory localises
+        running[l] = true; mapped[l] = map_poses != nullptr;
+        localising[l] = mapped[l] && armed[l];
+        if (mapped[l]) armed[l] = false;
+      }
+      if (map_poses) { row_loc[(size_t)k * batch + l] = localising[l]; (localising[l] ? localises : maps)[l] = true; }
       if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
       if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
     }
@@ -858,11 +884,16 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   if (map_poses && c->reg_sink && registered_layout(c, raws, lane_ops, n_scans, batch, nullptr, nullptr) > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (run_err) { aloam_reset_odometry(c); return run_err; }
-  if (map_poses) { int rc = mapper_ensure_lanes(c, batch); if (rc) return rc; }   // creates the cube stores this call needs
+  if (map_poses) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
+    for (int l = 0; l < batch; ++l) {
+      int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
+      rc = maps[l] || !localises[l] ? mapper_ensure_lane(c, l) : ALOAM_OK; if (rc) return rc;
+    }
+  }
   // committed before anything is issued: a later failure ends in aloam_reset_odometry, a key overflow leaves the lanes running
   c->lanes_mode = true;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; }
-  return scan_stream_run(c, raws, lane_ops, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; c->lane_localising[l] = localising[l]; c->lane_armed[l] = armed[l]; }
+  return scan_stream_run(c, raws, lane_ops, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true, row_loc.data());
 }
 
 int aloam_set_registered_sink(aloam_ctx* c, float* data, long long capacity) {

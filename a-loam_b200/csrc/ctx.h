@@ -42,6 +42,14 @@ struct MapperIn {
   double* out7;
   int lane;
   int fresh;
+  int localise;   // the lane registers against the context's prior map: its frame state is its locator's, not a cube store's
+};
+// what the registration of localising lanes searches instead of each lane's indexed submap: the prior map's grids, and per
+// lane the window tables and centre cube k_locate_begin left in its frame state
+struct PriorSearch {
+  PriorGrid grid;
+  const int* win[ALOAM_MAX_BATCH][2];
+  const int* ctr[ALOAM_MAX_BATCH];
 };
 }  // namespace aloam
 
@@ -98,6 +106,7 @@ struct PinnedScratch {
   int mapper_counts[2];     // aloam_mapper_step: input cloud sizes
   int mapper_err;           // aloam_scan_stream_mapped: the mapper's error bits, OR over the call's frames
   int mapper_err_lane[ALOAM_MAX_BATCH];   // aloam_scan_stream_mapped_batch: the same per lane
+  int locate_err_lane[ALOAM_MAX_BATCH];   // aloam_scan_stream_lanes: the same of every lane's localising frames
   int peer_err;             // sharded registration / mapper frames: the peer exchange's error word
   SegDesc vox_seg;          // aloam_voxel_filter: the cloud as the one segment of its filter
   int vox_nseg;             //                     1
@@ -209,6 +218,18 @@ struct aloam_ctx {
   // mapped streams: index of every lane's next scan in its trajectory (0 at a START); scan j goes to the mapper when
   // j % cfg.mapping_skip_frame == 0.  Carries over between calls; aloam_reset_odometry clears it.
   int lane_scan[ALOAM_MAX_BATCH] = {};
+  // localisation (cubemap.cu): the context's prior map, released by prior_map_release; the frame state and registration
+  // buffers of every lane that has localised (created at its first localising START); the auxiliary stream of the locate frame's
+  // stack filters.  lane_localising: the trajectory the lane runs (or ran last) registers against the prior map, fixed at its
+  // START.  lane_armed / lane_init: aloam_lane_localise has armed the lane's next mapped START with this T_wmap_wodom.
+  void* prior = nullptr;
+  bool prior_owned = false;       // prior_map_release is on the release list
+  void* locator[ALOAM_MAX_BATCH] = {};
+  cudaStream_t s_loc_aux = nullptr;
+  cudaEvent_t ev_loc_fork = nullptr, ev_loc_join = nullptr;
+  bool lane_localising[ALOAM_MAX_BATCH] = {};
+  bool lane_armed[ALOAM_MAX_BATCH] = {};
+  double lane_init[ALOAM_MAX_BATCH][7] = {};
   int lockstep_ops[kMaxStreamScans] = {};   // the lane schedule a lockstep stream call hands to the stream driver
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
@@ -222,10 +243,10 @@ struct aloam_ctx {
 namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
-       KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD };
+       KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
-    "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard"};
+    "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -284,17 +305,33 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);
 int mapper_ensure_lanes(aloam_ctx* c, int nb);
+int mapper_ensure_lane(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);
+// localisation against the prior map (cubemap.cu): a lane's locator, created on first use; one frame of nb localising lanes on
+// the current stream (in[l].fresh: the lane starts its trajectory with this frame, from c->lane_init); its per-call error word
+int locator_ensure(aloam_ctx* c, int lane);
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
+int* locator_err_acc(aloam_ctx* c, int lane);
+inline bool any_lane_localising(const aloam_ctx* c) {
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) if (c->lane_running[l] && c->lane_localising[l]) return true;
+  return false;
+}
+// snapshot.cu: the kind of a caller's snapshot buffer (1 device memory of the context's device, 0 host memory, -1 unusable), and
+// the host checks of aloam_lane_restore on the snapshot at b -- header (left in c->pin->snap), configuration against the
+// context's and, mapped, the store table (left in c->h_snap_store); need_mapped: an unmapped snapshot is refused too.
+// *store = byte offset of the store section.
+int snapshot_buffer_kind(const aloam_ctx* c, const void* p);
+int snapshot_validate(aloam_ctx* c, const char* b, long long n_bytes, int kind, bool need_mapped, long long* store);
 void mapper_slab_caps(const aloam_ctx* c, int cap[2]);
 int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head);
 int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device);
 int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device);
 int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf);
 int ensure_map_buffers(aloam_ctx* c);
-int map_reg_alloc(aloam_ctx* c, MapReg* r);
+int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids = true);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
-int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper);
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, const PriorSearch* prior = nullptr);
 namespace {
 
 // a rank of a sharded job: joined to a world of several ranks by a communicator, or emulating a rank (aloam_debug_shard_emulate)

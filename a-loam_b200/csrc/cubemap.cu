@@ -18,6 +18,10 @@
 //   * the per-cube re-filter of the valid cubes as ONE segmented VoxelGrid over up to 150 segments, in place.
 //   * the published clouds (:806-848): k_export_sizes / k_export_gather read a lane's store out in the reference's order
 //                      (aloam_mapper_export), k_register_full moves a mapped scan's full cloud by the frame's refined pose.
+//   * localisation against a prior map (aloam_prior_map_load, aloam_lane_localise): the store of a saved lane, frozen, packed in
+//                      cube order and indexed ONCE with the hash grid of mapping.cu; a localising lane's frame is k_locate_begin
+//                      (hand-off, centre cube, clipped 5 x 5 x 3 window -- no shift), the stack filters, the registration of
+//                      mapping.cu through k_map_knn5_prior, k_mapper_update: no gather, no index build, no insertion, no re-filter.
 // Slabs are a POOL (1024 per cloud type, 16 k corner / 64 k surf points each: 1.3 GB) handed out on the device on first
 // insertion, not 4851 x 2 slabs (6.4 GB) up front.  A full slab or an exhausted pool drops the overflow and raises
 // ALOAM_FLAG_CUBE_OVERFLOW instead of failing the frame (the reference grows its cubes without bound between re-filters).
@@ -276,6 +280,104 @@ __global__ void k_mapper_high_freq(const __grid_constant__ Batch<MapperLane> B) 
   double x[7];
   associate_to_map(a.S, a.odom7, x);
   for (int k = 0; k < 7; ++k) a.out7[k] = x[k];
+}
+
+
+// ---- localisation against a prior map: the frame of a lane that registers its scans against the context's frozen store
+
+// one lane of k_locate_begin: its frame state, the scan's odometry pose, and for a lane that starts its trajectory with this
+// frame (`fresh`) the T_wmap_wodom it starts from (aloam_lane_localise)
+struct LocateLane {
+  MapperState* S;
+  const double* odom7;
+  double init[7];
+  int fresh;
+};
+// grid (1, 1, lanes), 256 threads: the head of a localising frame -- laserMapping.cpp:309-321 and :512-531 with the ring-buffer
+// shift (:323-507) left out.  Pose hand-off as k_mapper_begin; centre cube from the prior map's fixed centre offsets `cen`; the
+// valid list = the window's cubes inside the buffer, in the reference's loop order; and per type the window table
+// S->sub_off[ty][w], w = (di + 2) * 15 + (dj + 2) * 3 + (dk + 1): the offset cube w's points would have in the gathered submap
+// (exclusive scan of the window's counts in loop order), -1 for a cube outside the buffer.  cs = the prior map's cube prefix
+// tables [2][NCUBE + 1].  n_sub feeds the thin-map test of k_mapper_prep.
+__global__ void __launch_bounds__(256) k_locate_begin(const __grid_constant__ Batch<LocateLane> B, const int* __restrict__ cs, int cen0, int cen1, int cen2) {
+  const LocateLane& a = B.a[blockIdx.z];
+  MapperState* S = a.S;
+  pdl_launch_dependents();
+  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
+  const int tid = threadIdx.x;
+  if (a.fresh) {
+    mapper_fresh_state(S);
+    __syncthreads();
+    if (tid < 4) S->q_wmap_wodom[tid] = a.init[tid];
+    else if (tid < 7) S->t_wmap_wodom[tid - 4] = a.init[tid];
+    __syncthreads();
+  }
+  __shared__ int s_ctr[3], s_cnt[2][ALOAM_WINDOW_CUBES];
+  if (tid == 0) {
+    associate_to_map(S, a.odom7, S->x);
+    for (int k = 0; k < 4; ++k) S->q_wodom[k] = a.odom7[k];
+    for (int k = 0; k < 3; ++k) S->t_wodom[k] = a.odom7[4 + k];
+    const int cen[3] = {cen0, cen1, cen2};
+    for (int k = 0; k < 3; ++k) { S->cen[k] = cen[k]; s_ctr[k] = cube_coord(S->x[4 + k], cen[k]); S->ctr[k] = s_ctr[k]; }
+    S->flags = 0;
+  }
+  __syncthreads();
+  if (tid < 2 * ALOAM_WINDOW_CUBES) {   // the counts of the window's cubes, all loads in flight at once
+    const int ty = tid >= ALOAM_WINDOW_CUBES, w = ty ? tid - ALOAM_WINDOW_CUBES : tid;
+    const int i = s_ctr[0] - 2 + w / 15, j = s_ctr[1] - 2 + (w / 3) % 5, k = s_ctr[2] - 1 + w % 3;
+    int n = -1;
+    if (i >= 0 && i < CW && j >= 0 && j < CH && k >= 0 && k < CD) { const int* t = cs + ty * (NCUBE + 1) + cube_index(i, j, k); n = t[1] - t[0]; }
+    s_cnt[ty][w] = n;
+  }
+  __syncthreads();
+  if (tid < 2) {
+    const int ty = tid;
+    int off = 0;
+    for (int w = 0; w < ALOAM_WINDOW_CUBES; ++w) {
+      const int n = s_cnt[ty][w];
+      S->sub_off[ty][w] = n < 0 ? -1 : off;
+      off += max(n, 0);
+    }
+    S->n_sub[ty] = off;
+  } else if (tid == 32) {
+    int nv = 0;
+    for (int w = 0; w < ALOAM_WINDOW_CUBES; ++w)
+      if (s_cnt[0][w] >= 0) S->valid[nv++] = cube_index(s_ctr[0] - 2 + w / 15, s_ctr[1] - 2 + (w / 3) % 5, s_ctr[2] - 1 + w % 3);
+    S->n_valid = nv;
+  }
+}
+
+// grid-stride over the 2 x NCUBE segments of the ALOAM_EXPORT_MAP order (segment 2 i + t: cube i, type t), between that order
+// and the prior map's two packed clouds: segment (i, t) starts at cs[0][i + t] + cs[1][i] of the export and at cs[t][i] of cloud
+// t.  The points of the window [lo, hi) of the export: to_store: io[position - lo] -> cloud, else cloud -> io[position - lo].
+__global__ void __launch_bounds__(256) k_prior_copy(const int* __restrict__ cs, Pt4* __restrict__ p0, Pt4* __restrict__ p1, Pt4* __restrict__ io, long long lo,
+                                                    long long hi, int to_store) {
+  const int* cs0 = cs;
+  const int* cs1 = cs + NCUBE + 1;
+  for (int s = blockIdx.x; s < 2 * NCUBE; s += gridDim.x) {
+    const int i = s >> 1, ty = s & 1;
+    const long long o = (long long)cs0[i + ty] + cs1[i];
+    const int first = ty ? cs1[i] : cs0[i], n = (ty ? cs1[i + 1] : cs0[i + 1]) - first;
+    const long long b = max(o, lo), e = min(o + n, hi);
+    Pt4* __restrict__ cloud = (ty ? p1 : p0) + first;
+    for (long long q = b + threadIdx.x; q < e; q += blockDim.x) {
+      if (to_store) cloud[q - o] = io[q - lo]; else io[q - lo] = cloud[q - o];
+    }
+  }
+}
+
+// grid (CTAs, 2 types): after the index build, every indexed point's packed index g (gpts.w, written by k_grid_fill) becomes
+// prior_tag(cube i, j, k, rank in the cube): the cube is the last one whose prefix is <= g
+__global__ void __launch_bounds__(256) k_prior_tag(const __grid_constant__ GridTable corner, const __grid_constant__ GridTable surf, const int* __restrict__ cs) {
+  const GridTable& g = blockIdx.y == 0 ? corner : surf;
+  const int* __restrict__ t = cs + blockIdx.y * (NCUBE + 1);
+  const int n = g.dyn->n;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) {
+    const int idx = __float_as_int(g.gpts[s].w);
+    int lo = 0, hi = NCUBE;   // t[lo] <= idx < t[hi]
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (t[mid] <= idx) lo = mid; else hi = mid; }
+    g.gpts[s].w = __int_as_float(prior_tag(lo % CW, (lo / CW) % CH, lo / (CW * CH), idx - t[lo]));
+  }
 }
 
 
@@ -710,6 +812,83 @@ int export_gather(aloam_ctx* c, const Mapper* m, int what, long long n, char* ds
   return ALOAM_OK;
 }
 
+
+// ---- localisation: the prior map of a context and the lanes that register against it
+
+// The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
+// exclusive prefix of the snapshot's counts) and a hash grid over ALL of them, built once by prior_index; the centre offsets of
+// the store, which never change (no localising frame shifts the ring buffer).  Plain cudaMalloc, freed by prior_map_release.
+struct PriorMap {
+  Pt4* pts[2] = {nullptr, nullptr};
+  int n[2] = {0, 0};
+  int cen[3] = {0, 0, 0};
+  int* d_cube_start = nullptr;   // [2][NCUBE + 1]
+  int* d_n = nullptr;            // [2]
+  GridTable grid[2] = {};
+};
+// what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
+// k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
+// holds the window tables), a registration set without grid tables, and a segmented filter sized for the two scan stacks
+struct Locator {
+  MapperState* d_state = nullptr;
+  MapperState* h_state = nullptr;
+  MapReg reg = {};
+  SegBuffers buf;
+};
+
+void prior_free(PriorMap* p) {
+  if (!p) return;
+  for (int t = 0; t < 2; ++t) { cudaFree(p->pts[t]); cudaFree(p->grid[t].slots); cudaFree(p->grid[t].dyn); cudaFree(p->grid[t].gpts); }
+  cudaFree(p->d_cube_start); cudaFree(p->d_n);
+  delete p;
+}
+// the one place a context's prior map is released: aloam_prior_map_clear, a load that replaces it, aloam_destroy
+void prior_map_release(aloam_ctx* c) {
+  prior_free(static_cast<PriorMap*>(c->prior));
+  c->prior = nullptr;
+}
+
+// the frame state of the lane a record runs on: its locator's when it localises, else its cube store's
+MapperState* lane_state(const aloam_ctx* c, const MapperIn& in) {
+  return in.localise ? static_cast<Locator*>(c->locator[in.lane])->d_state : static_cast<Mapper*>(c->mapper[in.lane])->d_state;
+}
+
+// the export-order points [0, n) between the prior map's clouds and memory at `mem` (device in place, host through the staging
+// buffer), on c->stream, not synchronised
+int prior_copy(aloam_ctx* c, PriorMap* p, long long n, char* mem, bool device, bool to_store) {
+  const int blocks = std::min(2 * NCUBE, c->sms * 8);
+  if (device) {
+    LAUNCH(c, KID_CUBES, k_prior_copy, blocks, 256, 0, p->d_cube_start, p->pts[0], p->pts[1], reinterpret_cast<Pt4*>(mem), 0ll, n, (int)to_store);
+  } else {
+    const int rc = export_stage(c); if (rc) return rc;
+    for (long long lo = 0; lo < n; lo += kExportStage) {
+      const long long hi = std::min(n, lo + kExportStage);
+      const size_t bytes = (size_t)(hi - lo) * sizeof(Pt4);
+      if (to_store) CUDA_CHECK_RET(cudaMemcpyAsync(c->d_export_stage, mem + lo * sizeof(Pt4), bytes, cudaMemcpyHostToDevice, c->stream));
+      LAUNCH(c, KID_CUBES, k_prior_copy, blocks, 256, 0, p->d_cube_start, p->pts[0], p->pts[1], c->d_export_stage, lo, hi, (int)to_store);
+      if (!to_store) CUDA_CHECK_RET(cudaMemcpyAsync(mem + lo * sizeof(Pt4), c->d_export_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
+    }
+  }
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
+// the persistent index: the k_grid_* chain of mapping.cu once over both packed clouds, then the cube tags
+void prior_index(aloam_ctx* c, PriorMap* p) {
+  Batch<GridArgs> g = {};
+  g.a[0] = GridArgs{p->grid[0], p->pts[0], p->d_n, p->grid[1], p->pts[1], p->d_n + 1};
+  const int n_upper = std::max(1, std::max(p->n[0], p->n[1]));
+  const int wave = c->sms * 8;
+  const int pb = std::min((n_upper + 255) / 256, wave);
+  const int tb = std::min((int)((std::max(p->grid[0].cap_slots, p->grid[1].cap_slots) + 255) / 256), wave);
+  LAUNCH(c, KID_MAP_GRID, k_grid_setup, 1, 32, 0, g);
+  LAUNCH(c, KID_MAP_GRID, k_grid_clear, dim3(tb, 1, 1), 256, 0, g);
+  LAUNCH(c, KID_MAP_GRID, k_grid_insert, dim3(pb, 2, 1), 256, 0, g, 0, 1);
+  LAUNCH(c, KID_MAP_GRID, k_grid_alloc, dim3(tb, 1, 1), 256, 0, g);
+  LAUNCH(c, KID_MAP_GRID, k_grid_fill, dim3(pb, 2, 1), 256, 0, g);
+  LAUNCH(c, KID_MAP_GRID, k_prior_tag, dim3(pb, 2, 1), 256, 0, p->grid[0], p->grid[1], p->d_cube_start);
+}
+
 }  // namespace
 
 // points per slab of the two cloud types (16 k corner / 64 k surf, at most cfg.max_points)
@@ -868,13 +1047,13 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
 }
 
 // The high-frequency pose of nb skipped scans on the current stream, one launch: record l composes the T_wmap_wodom of lane
-// in[l].lane's cube store with in[l].odom7 into in[l].out7 (the clouds and `fresh` of in[l] are not read).  The lanes' stores
-// exist: a trajectory's first scan is always mapped.
+// in[l].lane's cube store (of its locator, when it localises) with in[l].odom7 into in[l].out7 (the clouds and `fresh` of in[l]
+// are not read).  The lanes' stores or locators exist: a trajectory's first scan is always mapped.
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<MapperLane> B = {};
   for (int l = 0; l < nb; ++l) {
-    B.a[l].S = static_cast<Mapper*>(c->mapper[in[l].lane])->d_state;
+    B.a[l].S = lane_state(c, in[l]);
     B.a[l].odom7 = in[l].odom7;
     B.a[l].out7 = in[l].out7;
   }
@@ -889,7 +1068,7 @@ int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<RegFullLane> B = {};
-  for (int l = 0; l < nb; ++l) B.a[l] = RegFullLane{static_cast<Mapper*>(c->mapper[in[l].lane])->d_state, src[l], n_full[l], dst[l]};
+  for (int l = 0; l < nb; ++l) B.a[l] = RegFullLane{lane_state(c, in[l]), src[l], n_full[l], dst[l]};
   const int blocks = std::max(1, std::min((n_upper + 255) / 256, std::max(1, c->sms * 2 / nb)));
   launch_ex(c, KID_CUBES, k_register_full, dim3(blocks, 1, nb), dim3(256), 0, 1, false, B);
   CUDA_CHECK_RET(cudaGetLastError());
@@ -905,6 +1084,150 @@ int mapper_ensure_lanes(aloam_ctx* c, int nb) {
   for (int l = 0; l < nb; ++l) { int rc = ensure_mapper(c, l); if (rc) return rc; }
   return ALOAM_OK;
 }
+
+int mapper_ensure_lane(aloam_ctx* c, int lane) { return ensure_mapper(c, lane); }
+
+// lane `lane`'s locator, created on first use and published only when fully allocated (what was acquired before a failure
+// belongs to the context until aloam_destroy); the auxiliary stream of the locate frame with the first one
+int locator_ensure(aloam_ctx* c, int lane) {
+  if (c->locator[lane]) return ALOAM_OK;
+  if (!c->ev_loc_join) {
+    if (screate(c, &c->s_loc_aux) != cudaSuccess || ecreate(c, &c->ev_loc_fork, cudaEventDisableTiming) != cudaSuccess ||
+        ecreate(c, &c->ev_loc_join, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+  }
+  Locator* m = new (std::nothrow) Locator();
+  if (!m) return ALOAM_ERR_CUDA;
+  own(c, [m] { delete m; });
+  bool ok = dalloc(c, &m->d_state, 1) == cudaSuccess && halloc(c, &m->h_state, 1) == cudaSuccess;
+  ok = ok && map_reg_alloc(c, &m->reg, false) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
+  ok = ok && cudaMemset(m->d_state, 0, sizeof(MapperState)) == cudaSuccess;
+  if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+  c->locator[lane] = m;
+  return ALOAM_OK;
+}
+
+int* locator_err_acc(aloam_ctx* c, int lane) { return &static_cast<Locator*>(c->locator[lane])->d_state->err_acc; }
+
+// One localising frame of nb lanes on the current stream: laserMapping.cpp:309-734 without the ring-buffer shift, against the
+// context's prior map, which it only reads.  Record l as in mapper_step_device; its lane's locator exists.  Every launch covers
+// all lanes: the stack filters (forked, as the mapping frame's), k_locate_begin, the thin-map test, outer_iters x (k_map_knn5_prior,
+// k_map_fit, LM), k_mapper_update, k_mapper_finish (the stack filter's error bit).
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
+  PriorMap* P = static_cast<PriorMap*>(c->prior);
+  if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || sharded_job(c)) return ALOAM_ERR_STATE;
+  Batch<MapperLane> B = {};
+  Batch<LocateLane> L = {};
+  MapLaneIO io[ALOAM_MAX_BATCH];
+  SegFilter stack_f[ALOAM_MAX_BATCH];
+  SegBuffers* bufs[ALOAM_MAX_BATCH];
+  PriorSearch ps = {};
+  ps.grid = PriorGrid{P->grid[0], P->grid[1]};
+  for (int l = 0; l < nb; ++l) {
+    Locator* m = static_cast<Locator*>(c->locator[in[l].lane]);
+    MapperState* S = m->d_state;
+    B.a[l].S = S; B.a[l].odom7 = in[l].odom7; B.a[l].out7 = in[l].out7;
+    B.a[l].in[0] = in[l].corner; B.a[l].in[1] = in[l].surf; B.a[l].n_in[0] = in[l].nc; B.a[l].n_in[1] = in[l].ns;
+    B.a[l].stack[0] = m->reg.stack[0]; B.a[l].stack[1] = m->reg.stack[1];
+    B.a[l].segs = m->buf.segs; B.a[l].n_seg = m->buf.n_seg;
+    L.a[l].S = S; L.a[l].odom7 = in[l].odom7; L.a[l].fresh = in[l].fresh;
+    for (int k = 0; k < 7; ++k) L.a[l].init[k] = c->lane_init[in[l].lane][k];
+    io[l] = MapLaneIO{m->reg, {nullptr, nullptr}, S->stack_counts, S->x};
+    ps.win[l][0] = S->sub_off[0]; ps.win[l][1] = S->sub_off[1]; ps.ctr[l] = S->ctr;
+    stack_f[l] = seg_filter(m->buf, 31, &S->err);
+    bufs[l] = &m->buf;
+  }
+  {
+    cudaStream_t main_stream = c->stream;
+    CUDA_CHECK_RET(cudaEventRecord(c->ev_loc_fork, main_stream));
+    CUDA_CHECK_RET(cudaStreamWaitEvent(c->s_loc_aux, c->ev_loc_fork, 0));
+    c->stream = c->s_loc_aux;
+    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1, 1, nb), dim3(32), 0, 1, false, B, c->cfg.line_res, c->cfg.plane_res);
+    vox_seg_filter(c, nb, stack_f, bufs, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
+    const cudaError_t e = cudaEventRecord(c->ev_loc_join, c->s_loc_aux);
+    c->stream = main_stream;
+    CUDA_CHECK_RET(e);
+  }
+  launch_ex(c, KID_CUBES, k_locate_begin, dim3(1, 1, nb), dim3(256), 0, 1, true, L, (const int*)P->d_cube_start, P->cen[0], P->cen[1], P->cen[2]);
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_loc_join, 0));   // join: the filtered stacks are ready
+  launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
+  const int rc = map_register_device(c, nb, io, nq_upper, &ps); if (rc) return rc;
+  launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
+extern "C" {
+
+int aloam_prior_map_load(aloam_ctx* c, const void* blob, long long n_bytes) {
+  if (!c || !blob || n_bytes < 0) return ALOAM_ERR_INVALID_ARG;
+  if (sharded_job(c) || any_lane_localising(c)) return ALOAM_ERR_STATE;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const int kind = snapshot_buffer_kind(c, blob);
+  if (kind < 0) return ALOAM_ERR_INVALID_ARG;
+  const char* b = static_cast<const char*>(blob);
+  long long store = 0;
+  int rc = snapshot_validate(c, b, n_bytes, kind, true, &store); if (rc) return rc;
+  const SnapStore* H = c->h_snap_store;
+  // ---- the new map is built beside the old one, which is replaced only when the new one is complete
+  std::vector<int> cs((size_t)2 * (NCUBE + 1));
+  PriorMap* p = new (std::nothrow) PriorMap();
+  if (!p) return ALOAM_ERR_CUDA;
+  for (int t = 0; t < 2; ++t) {
+    long long run = 0;
+    for (int i = 0; i < NCUBE; ++i) { cs[(size_t)t * (NCUBE + 1) + i] = (int)run; run += std::max(H->count[t][i], 0); }   // (<= 1024 slabs of <= 65536 points)
+    cs[(size_t)t * (NCUBE + 1) + NCUBE] = (int)run;
+    p->n[t] = (int)run;
+  }
+  for (int a = 0; a < 3; ++a) p->cen[a] = H->cen[a];
+  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess;
+  for (int t = 0; t < 2 && ok; ++t) {
+    GridTable& g = p->grid[t];
+    g.cap_slots = grid_mask_for(p->n[t], 1u << 30) + 1;
+    g.cs = kMapCell; g.inv_cs = 1.0f / g.cs;
+    const size_t n1 = (size_t)std::max(p->n[t], 1);
+    ok = cudaMalloc(&p->pts[t], n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&g.gpts, n1 * sizeof(float4)) == cudaSuccess &&
+         cudaMalloc(&g.slots, (size_t)g.cap_slots * sizeof(uint4)) == cudaSuccess && cudaMalloc(&g.dyn, sizeof(GridDyn)) == cudaSuccess;
+  }
+  auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); prior_free(p); return code; };
+  if (!ok) return fail(ALOAM_ERR_CUDA);
+  if (cudaMemcpyAsync(p->d_cube_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+      cudaMemcpyAsync(p->d_n, p->n, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+    return fail(ALOAM_ERR_CUDA);
+  if (H->n_points > 0) { rc = prior_copy(c, p, H->n_points, const_cast<char*>(b) + store + sizeof(SnapStore), kind, true); if (rc) return fail(rc); }
+  prior_index(c, p);
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ALOAM_ERR_CUDA);
+  if (!c->prior_owned) { own(c, [c] { prior_map_release(c); }); c->prior_owned = true; }
+  prior_map_release(c);
+  c->prior = p;
+  return ALOAM_OK;
+}
+
+int aloam_prior_map_clear(aloam_ctx* c) {
+  if (!c) return ALOAM_ERR_INVALID_ARG;
+  if (any_lane_localising(c)) return ALOAM_ERR_STATE;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  prior_map_release(c);
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_armed[l] = false;   // an arming needs a map
+  return ALOAM_OK;
+}
+
+int aloam_lane_localise(aloam_ctx* c, int lane, const double q_init[4], const double t_init[3]) {
+  if (!c || lane < 0 || lane >= c->n_lanes || !q_init || !t_init) return ALOAM_ERR_INVALID_ARG;
+  double n2 = 0;
+  for (int k = 0; k < 4; ++k) { if (!std::isfinite(q_init[k])) return ALOAM_ERR_INVALID_ARG; n2 += q_init[k] * q_init[k]; }
+  for (int k = 0; k < 3; ++k) if (!std::isfinite(t_init[k])) return ALOAM_ERR_INVALID_ARG;
+  if (!(n2 > 0) || !std::isfinite(n2)) return ALOAM_ERR_INVALID_ARG;
+  if (!c->prior) return ALOAM_ERR_STATE;
+  const double n = std::sqrt(n2);
+  for (int k = 0; k < 4; ++k) c->lane_init[lane][k] = q_init[k] / n;
+  for (int k = 0; k < 3; ++k) c->lane_init[lane][4 + k] = t_init[k];
+  c->lane_armed[lane] = true;
+  return ALOAM_OK;
+}
+
+}  // extern "C"
 
 extern "C" {
 
@@ -962,17 +1285,21 @@ int aloam_mapper_debug_state_lane(aloam_ctx* c, int lane, int centre[3], int* n_
                                   double t_wmap_wodom[3], long long totals[2]) {
   if (!c) return ALOAM_ERR_STATE;
   if (lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
-  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
-  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  // a lane whose trajectory localises answers from its locator, with the totals of the prior map it reads
+  const bool loc = c->lane_localising[lane] && c->locator[lane] && c->prior;
+  if (!loc && !c->mapper[lane]) return ALOAM_ERR_STATE;
+  MapperState* d_state = loc ? static_cast<Locator*>(c->locator[lane])->d_state : static_cast<Mapper*>(c->mapper[lane])->d_state;
+  MapperState* h_state = loc ? static_cast<Locator*>(c->locator[lane])->h_state : static_cast<Mapper*>(c->mapper[lane])->h_state;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
-  const MapperState* h = m->h_state;
+  CUDA_CHECK_RET(cudaMemcpy(h_state, d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
+  const MapperState* h = h_state;
   if (centre) for (int a = 0; a < 3; ++a) centre[a] = h->cen[a];
   if (n_valid) *n_valid = h->n_valid;
   if (valid) for (int i = 0; i < h->n_valid && i < 125; ++i) valid[i] = h->valid[i];
   if (q_wmap_wodom) for (int k = 0; k < 4; ++k) q_wmap_wodom[k] = h->q_wmap_wodom[k];
   if (t_wmap_wodom) for (int k = 0; k < 3; ++k) t_wmap_wodom[k] = h->t_wmap_wodom[k];
-  if (totals)
+  if (totals && loc) { for (int t = 0; t < 2; ++t) totals[t] = static_cast<PriorMap*>(c->prior)->n[t]; }
+  else if (totals)
     for (int t = 0; t < 2; ++t) {
       totals[t] = 0;
       for (int i = 0; i < NCUBE; ++i) { const int s = h->slab_of[t][i]; if (s >= 0) totals[t] += h->cnt[t][s]; }
@@ -999,13 +1326,18 @@ int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, al
 }
 
 int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long capacity, long long* n_out) {
-  if (!c || !n_out || capacity < 0 || lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
+  if (!c || !n_out || capacity < 0 || lane < ALOAM_PRIOR_MAP || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
   if (what != ALOAM_EXPORT_SURROUND && what != ALOAM_EXPORT_MAP) return ALOAM_ERR_INVALID_ARG;
-  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
+  const bool prior = lane == ALOAM_PRIOR_MAP;
+  if (prior && what != ALOAM_EXPORT_MAP) return ALOAM_ERR_INVALID_ARG;   // the prior map has no frame, so no surround
+  if (prior ? !c->prior : !c->mapper[lane]) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  const Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  const Mapper* m = prior ? nullptr : static_cast<Mapper*>(c->mapper[lane]);
+  PriorMap* pm = static_cast<PriorMap*>(c->prior);
   long long n = 0;
-  int rc = export_sizes(c, m, what, &n); if (rc) return rc;
+  int rc = ALOAM_OK;
+  if (prior) n = (long long)pm->n[0] + pm->n[1];
+  else { rc = export_sizes(c, m, what, &n); if (rc) return rc; }
   *n_out = n;
   if (!out && capacity == 0) return ALOAM_OK;   // the size only
   if (!out) return ALOAM_ERR_INVALID_ARG;
@@ -1013,7 +1345,8 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
   if (n == 0) return ALOAM_OK;
   cudaPointerAttributes at = {};
   CUDA_CHECK_RET(cudaPointerGetAttributes(&at, out));
-  rc = export_gather(c, m, what, n, reinterpret_cast<char*>(out), at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
+  const bool device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  rc = prior ? prior_copy(c, pm, n, reinterpret_cast<char*>(out), device, false) : export_gather(c, m, what, n, reinterpret_cast<char*>(out), device);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());

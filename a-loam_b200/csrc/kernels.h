@@ -101,6 +101,7 @@ struct GridTable {
   float cs, inv_cs;  // cell edge [m]
 };
 struct MapCloud { GridTable grid; };
+constexpr float kMapCell = 1.0f * (1.0f + 1e-5f);   // cell edge: > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
 unsigned grid_mask_for(int n, unsigned cap_slots);
 // the mapper's index build and association run over all lanes of aloam_scan_stream_mapped_batch at once: every kernel takes
 // one record per lane and finds its own in blockIdx.z (the host API is the batch of one)
@@ -117,6 +118,20 @@ struct MapAssocArgs { const Pt4* corner_stack; const Pt4* surf_stack; const int*
 __global__ void k_map_knn5(const __grid_constant__ Batch<MapAssocArgs> B, int shard_rank, int shard_count);
 __global__ void k_map_fit(const __grid_constant__ Batch<MapAssocArgs> B);
 __global__ void k_map_knn(MapCloud map, const Pt4* queries, int nq, int k, int* idx, float* sqd);
+// Localisation against a prior map (cubemap.cu): ONE hash grid per cloud type over the whole frozen map, built once at load and
+// shared by every localising lane.  gpts.w of an indexed point is not its index but prior_tag(): the cube it is stored in and its
+// rank inside that cube, so a search can tell without another load whether the point lies in a lane's 5 x 5 x 3 cube window and
+// which index it would have had in the submap the mapping frame gathers (window offset of the cube + rank).  (The alternatives
+// were a uint16 cube id beside gpts, one more 2-byte load per candidate, or a 13-step binary search of the cube prefix table per
+// candidate; the tag costs three shifts and no load.  Ranks fit 16 bits: a cube holds at most 65536 points.)
+#define ALOAM_WINDOW_CUBES 75   // 5 x 5 x 3, entry (di + 2) * 15 + (dj + 2) * 3 + (dk + 1): the loop order of laserMapping.cpp:512-531
+__host__ __device__ inline int prior_tag(int i, int j, int k, int rank) { return (i << 25) | (j << 20) | (k << 16) | rank; }
+struct PriorGrid { GridTable corner, surf; };
+// one lane of the search: its filtered stacks and pose as MapAssocArgs, its window tables (per type ALOAM_WINDOW_CUBES offsets
+// into the submap the window's cubes would gather to) and its centre cube (3 ints)
+struct MapPriorArgs { const Pt4* corner_stack; const Pt4* surf_stack; const int* counts3; const double* pose7; float4* nbr;
+                      const int* win[2]; const int* ctr; };
+__global__ void k_map_knn5_prior(const __grid_constant__ Batch<MapPriorArgs> B, const __grid_constant__ PriorGrid G);
 
 // ---- voxel.cu: segmented, device-resident pcl::VoxelGrid (aloam_voxel_filter, the scan-stack filters and the per-cube re-filter
 // of the mapping loop)

@@ -551,6 +551,72 @@ __global__ void __launch_bounds__(256) k_map_knn5(const __grid_constant__ Batch<
 }
 
 
+// K5 against the prior map (localising lanes): k_map_knn5's search in the ONE grid over the whole frozen map, shared by all lanes.
+// A candidate counts only if its cube lies in the lane's 5 x 5 x 3 window, and candidates are ordered by (distance, window offset
+// of the cube + rank in the cube) -- the index the point would have had in the submap a mapping frame gathers from the same
+// store.  So the five neighbours and their order are those of gather + K0 + k_map_knn5, and nbr (index bits included) is
+// identical.  The window tables of the lane live in shared memory (600 B).
+// grid (CTAs, 1, lanes)
+__global__ void __launch_bounds__(256) k_map_knn5_prior(const __grid_constant__ Batch<MapPriorArgs> B, const __grid_constant__ PriorGrid P) {
+  const MapPriorArgs& a = B.a[blockIdx.z];
+  pdl_launch_dependents();
+  pdl_wait();   // pose7 is produced by the preceding LM solve of the stream, the window by k_locate_begin
+  __shared__ int s_win[2][ALOAM_WINDOW_CUBES];
+  __shared__ int s_ctr[3];
+  if (threadIdx.x < 2 * ALOAM_WINDOW_CUBES) s_win[threadIdx.x / ALOAM_WINDOW_CUBES][threadIdx.x % ALOAM_WINDOW_CUBES] = a.win[threadIdx.x / ALOAM_WINDOW_CUBES][threadIdx.x % ALOAM_WINDOW_CUBES];
+  else if (threadIdx.x < 2 * ALOAM_WINDOW_CUBES + 3) s_ctr[threadIdx.x - 2 * ALOAM_WINDOW_CUBES] = a.ctr[threadIdx.x - 2 * ALOAM_WINDOW_CUBES];
+  __syncthreads();
+  const Pt4* __restrict__ corner_stack = a.corner_stack;
+  const Pt4* __restrict__ surf_stack = a.surf_stack;
+  float4* __restrict__ nbr = a.nbr;
+  const int n_corner = a.counts3[0], nq = a.counts3[2];
+  const unsigned lane = lane_id();
+  const int warps = (gridDim.x * blockDim.x) >> 5;
+  const unsigned mask_c = P.corner.dyn->mask, mask_s = P.surf.dyn->mask;
+  const int c0 = s_ctr[0] - 2, c1 = s_ctr[1] - 2, c2 = s_ctr[2] - 1;   // the window's low corner
+  double pose[7];
+#pragma unroll
+  for (int k = 0; k < 7; ++k) pose[k] = a.pose7[k];
+  for (int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; wid < nq; wid += warps) {
+    const bool is_corner = wid < n_corner;
+    const Pt4 ori = is_corner ? corner_stack[wid] : surf_stack[wid - n_corner];
+    const GridTable& G = is_corner ? P.corner : P.surf;
+    const int* win = s_win[is_corner ? 0 : 1];
+    // pointAssociateToMap (:154-163): q * p + t in double, stored to float
+    float qx, qy, qz;
+    {
+      const D3 u{pose[0], pose[1], pose[2]};
+      const double w = pose[3];
+      const D3 v{(double)ori.x, (double)ori.y, (double)ori.z};
+      D3 uv = cross3(u, v);
+      uv.x = uv.x + uv.x; uv.y = uv.y + uv.y; uv.z = uv.z + uv.z;
+      const D3 c2v = cross3(u, uv);
+      qx = (float)(((v.x + w * uv.x) + c2v.x) + pose[4]);
+      qy = (float)(((v.y + w * uv.y) + c2v.y) + pose[5]);
+      qz = (float)(((v.z + w * uv.z) + c2v.z) + pose[6]);
+    }
+    float nd[5]; int ni[5], np[5];
+    TopK<5> t; t.init();
+    visit_block27(G, is_corner ? mask_c : mask_s, qx, qy, qz, [&](float x, float y, float z, int tag, int slot) {
+      const int di = (tag >> 25) - c0, dj = ((tag >> 20) & 31) - c1, dk = ((tag >> 16) & 15) - c2;
+      if ((unsigned)di < 5u && (unsigned)dj < 5u && (unsigned)dk < 3u)   // a cube of the window (one that holds points is inside the buffer)
+        t.push(sqdist3(x, y, z, qx, qy, qz), win[(di * 5 + dj) * 3 + dk] + (tag & 0xffff), slot);
+    });
+    const int found = warp_merge_topk<5>(t, nd, ni, np);
+    if (!(found == 5 && (double)nd[4] < 1.0)) {   // pointSearchSqDis[4] < 1.0 (:584,652)
+      if (lane == 0) nbr[(size_t)wid * 5] = make_float4(0.f, 0.f, 0.f, __int_as_float(-1));
+    } else if (lane < 5) {
+      int slot = np[0], idx = ni[0];
+#pragma unroll
+      for (int j = 1; j < 5; ++j) if ((int)lane == j) { slot = np[j]; idx = ni[j]; }
+      float4 p = __ldg(G.gpts + slot);
+      p.w = __int_as_float(idx);
+      nbr[(size_t)wid * 5 + lane] = p;
+    }
+  }
+}
+
+
 // K6: one thread per stack point: line fit (:586-621) or plane fit (:650-686) on its five neighbours, residual block out.
 __device__ __forceinline__ void map_fit_body(const Pt4* __restrict__ corner_stack, const Pt4* __restrict__ surf_stack,
                                                  const int* __restrict__ counts3, const float4* __restrict__ nbr,
@@ -677,17 +743,17 @@ bool is_device_ptr(const void* p) {
 }
 }  // namespace
 
-// the buffers of one registration set, its two grid tables sized for cfg.max_map_points (c->map_slots, fixed by
+// the buffers of one registration set, its two grid tables (`grids`: a localising lane searches the prior map's and has none) sized for cfg.max_map_points (c->map_slots, fixed by
 // ensure_map_buffers, which creates the context's set before any other).  On failure what was acquired belongs to the context
 // until aloam_destroy.
-int map_reg_alloc(aloam_ctx* c, MapReg* r) {
-  for (int t = 0; t < 2; ++t) {
+int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids) {
+  for (int t = 0; t < 2 && grids; ++t) {
     GridTable& g = (t ? r->surf : r->corner).grid;
     if (dalloc(c, &g.slots, (size_t)c->map_slots) != cudaSuccess || dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, (size_t)c->max_map) != cudaSuccess ||
         cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess)
       return ALOAM_ERR_CUDA;
     g.cap_slots = (unsigned)c->map_slots;
-    g.cs = 1.0f * (1.0f + 1e-5f);   // > 1 m so that an f32 d^2 < 1.0 neighbour can never sit outside the 27-cell block
+    g.cs = kMapCell;
     g.inv_cs = 1.0f / g.cs;
   }
   const size_t mp = (size_t)c->max_points;
@@ -736,24 +802,32 @@ namespace {
 // 5-NN + fits of nb lanes, one launch each covering all of them: lane l associates io[l].reg.stack[0] / [1] (sizes io[l].counts3 =
 // {n_corner, n_surf, total}) at pose io[l].pose with io[l].reg's submaps into its residual blocks, all in device memory.  fits:
 // lane 0's debug records, or null.  pdl: the 5-NN may become resident under the previous kernel of the stream.
-void map_associate_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, bool pdl, double* fits) {
+// prior: the lanes localise -- the 5-NN searches the prior map's grids through each lane's cube window instead of io[l].reg's.
+void map_associate_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, bool pdl, double* fits, const PriorSearch* prior) {
   const int kb = std::max(1, std::min((nq_upper + 7) / 8, lane_ctas(c, nb)));
   const int fb = std::max(1, (nq_upper + 31) / 32);   // one warp per CTA: a few thousand serial double-precision fits spread over all SMs
   Batch<MapAssocArgs> a = {};
   for (int l = 0; l < nb; ++l)
     a.a[l] = MapAssocArgs{io[l].reg.stack[0], io[l].reg.stack[1], io[l].counts3, io[l].reg.corner, io[l].reg.surf, io[l].pose, io[l].reg.nbr,
                           io[l].reg.blocks, l == 0 ? fits : nullptr};
-  launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb, 1, nb), dim3(256), 0, 1, pdl, a, c->shard_rank, c->shard_count);
+  if (prior) {
+    Batch<MapPriorArgs> p = {};
+    for (int l = 0; l < nb; ++l)
+      p.a[l] = MapPriorArgs{io[l].reg.stack[0], io[l].reg.stack[1], io[l].counts3, io[l].pose, io[l].reg.nbr, {prior->win[l][0], prior->win[l][1]}, prior->ctr[l]};
+    launch_ex(c, KID_MAP_KNN5_PRIOR, k_map_knn5_prior, dim3(kb, 1, nb), dim3(256), 0, 1, pdl, p, prior->grid);
+  } else {
+    launch_ex(c, KID_MAP_KNN5, k_map_knn5, dim3(kb, 1, nb), dim3(256), 0, 1, pdl, a, c->shard_rank, c->shard_count);
+  }
   launch_ex(c, KID_MAP_FIT, k_map_fit, dim3(fb, 1, nb), dim3(32), 0, 1, true, a);
 }
 }  // namespace
 
 // outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers its stacks against io[l].reg
 // (see map_associate_device) and refines io[l].pose.  A sharded job's solves exchange their normal equations (one lane).
-int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper) {
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, const PriorSearch* prior) {
   const LmParams lp = lm_params(c->cfg);
   for (int it = 0; it < c->cfg.outer_iters; ++it) {
-    map_associate_device(c, nb, io, nq_upper, it > 0, nullptr);
+    map_associate_device(c, nb, io, nq_upper, it > 0, nullptr, prior);
     Batch<LmArgs> lm = {};
     for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
     const int rc = launch_lm_batch(c, true, lm, nb, lp, 0, 0, false, sharded_lm(c));
@@ -945,7 +1019,7 @@ int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_c
   const int nq = corner_stack.n + surf_stack.n;
   if (nq > 0) {   // the launches of one outer iteration of aloam_mapping_register
     const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
-    map_associate_device(c, 1, &io, nq, false, c->d_fits);
+    map_associate_device(c, 1, &io, nq, false, c->d_fits, nullptr);
     CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

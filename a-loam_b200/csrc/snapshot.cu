@@ -77,13 +77,19 @@ int last_slot(const aloam_ctx* c) { return (c->frame + kFeatSlots - 1) % kFeatSl
 
 // the kind of a caller's snapshot buffer: 1 device memory of this context's device, 0 host memory (pinned or pageable), -1 memory
 // the call cannot use (another device, or device memory not aligned to 16 bytes: the store's points are moved as 16-byte words)
-int buffer_kind(const aloam_ctx* c, const void* p) {
+int buffer_kind(const aloam_ctx* c, const void* p) { return snapshot_buffer_kind(c, p); }
+
+}  // namespace
+
+int snapshot_buffer_kind(const aloam_ctx* c, const void* p) {
   cudaPointerAttributes at = {};
   if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return -1; }
   if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged)
     return (at.type == cudaMemoryTypeDevice && at.device != c->cfg.device) || reinterpret_cast<uintptr_t>(p) % 16 ? -1 : 1;
   return 0;
 }
+
+namespace {
 
 // n bytes between the caller's buffer and host memory, on c->stream (host memory: at once)
 int put(aloam_ctx* c, char* dst, bool device, const void* src, size_t n) {
@@ -104,6 +110,24 @@ int ensure_snap_store(aloam_ctx* c) {
 }
 
 }  // namespace
+
+int snapshot_validate(aloam_ctx* c, const char* b, long long n_bytes, int kind, bool need_mapped, long long* store) {
+  if (n_bytes < (long long)sizeof(SnapHeader)) return ALOAM_ERR_SNAPSHOT;
+  SnapHeader& h = c->pin->snap;
+  int rc = fetch(c, &h, b, kind, sizeof(h)); if (rc) return rc;
+  rc = check_header(h, n_bytes); if (rc) return rc;
+  if (need_mapped && !h.mapped) return ALOAM_ERR_SNAPSHOT;
+  SnapHeader mine = {};
+  fingerprint(c, &mine);
+  if (!same_config(h, mine)) return ALOAM_ERR_SNAPSHOT;
+  *store = store_offset(h);
+  if (h.mapped) {
+    rc = ensure_snap_store(c); if (rc) return rc;
+    rc = fetch(c, c->h_snap_store, b + *store, kind, sizeof(SnapStore)); if (rc) return rc;
+    rc = check_store(h, *c->h_snap_store); if (rc) return rc;
+  }
+  return ALOAM_OK;
+}
 
 extern "C" {
 
@@ -133,6 +157,7 @@ int aloam_snapshot_check(const void* blob, long long n_bytes, aloam_snapshot_inf
 int aloam_lane_save(aloam_ctx* c, int lane, void* out, long long capacity, long long* n_bytes) {
   if (!c || !n_bytes || capacity < 0 || lane < 0 || lane >= c->n_lanes) return ALOAM_ERR_INVALID_ARG;
   if (!c->lanes_mode || !c->lane_running[lane]) return ALOAM_ERR_STATE;
+  if (c->lane_localising[lane]) return ALOAM_ERR_STATE;   // format v1 has no section for a localising lane's state
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   const Lane& L = c->lanes[lane];
   const FeatBuf& f = L.feat[last_slot(c)];
@@ -185,21 +210,12 @@ int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_byt
   // as at a START: the lane's trajectory, if any, ends here, and the context runs lanes from now on
   c->lanes_mode = true;
   c->lane_running[lane] = false;
+  c->lane_localising[lane] = false;
   // ---- validation, on the host, before anything is written to the device
-  if (n_bytes < (long long)sizeof(SnapHeader)) return ALOAM_ERR_SNAPSHOT;
   const char* b = static_cast<const char*>(blob);
-  SnapHeader& h = c->pin->snap;
-  int rc = fetch(c, &h, b, kind, sizeof(h)); if (rc) return rc;
-  rc = check_header(h, n_bytes); if (rc) return rc;
-  SnapHeader mine = {};
-  fingerprint(c, &mine);
-  if (!same_config(h, mine)) return ALOAM_ERR_SNAPSHOT;
-  const long long store = store_offset(h);
-  if (h.mapped) {
-    rc = ensure_snap_store(c); if (rc) return rc;
-    rc = fetch(c, c->h_snap_store, b + store, kind, sizeof(SnapStore)); if (rc) return rc;
-    rc = check_store(h, *c->h_snap_store); if (rc) return rc;
-  }
+  const SnapHeader& h = c->pin->snap;
+  long long store = 0;
+  int rc = snapshot_validate(c, b, n_bytes, kind, false, &store); if (rc) return rc;
   if (h.n_less_sharp > c->max_points || h.n_less_flat > c->max_points) return ALOAM_ERR_CAPACITY;
   if (h.mapped) { rc = mapper_ensure_lanes(c, lane + 1); if (rc) return rc; }   // creates the lane's cube store if needed
   // ---- odometry: the "last" clouds into the slot the next step reads, their index and ring check, the poses, the armed scalars

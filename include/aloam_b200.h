@@ -295,6 +295,48 @@ int aloam_lane_save(aloam_ctx* ctx, int lane, void* out, long long capacity, lon
 int aloam_lane_restore(aloam_ctx* ctx, int lane, const void* blob, long long n_bytes);
 int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapshot_info* info);
 
+/* ---- localisation against a prior map: vehicles register their scans against ONE saved map that no frame changes.
+ * aloam_prior_map_load makes the cube store of a MAPPED lane snapshot (format v1; blob in device, pinned or pageable memory, as
+ * aloam_lane_restore) the prior map of the context.  Only the store section and the configuration are used: the snapshot's odometry
+ * part and its T_wmap_wodom are ignored.  The snapshot is checked on the host by the routine aloam_lane_restore runs for a mapped
+ * snapshot, with its error codes (ALOAM_ERR_SNAPSHOT also for an unmapped snapshot), and nothing on the device changes on failure.
+ * The map is packed per cloud type and indexed once, with one hash grid over the WHOLE map (1.00001 m cells): it is not bounded by
+ * cfg.max_map_points (no submap is gathered) but by the snapshot format (1024 cubes of a type x the slab capacity) and by memory
+ * (ALOAM_ERR_CUDA before any state changes): 32 B per point plus a table of 16 B x the power of two above 1.25 x the points of the
+ * type.  Loading replaces an earlier prior map.  ALOAM_ERR_STATE while any lane is localising, on a rank of a sharded job and on an
+ * emulating context.  aloam_prior_map_clear releases it (ALOAM_ERR_STATE while any lane is localising) and drops every arming;
+ * aloam_destroy releases it too.
+ * aloam_lane_localise arms `lane` (0 <= lane < cfg.max_batch): its next ALOAM_LANE_START in an aloam_scan_stream_lanes call with
+ * map_poses begins a LOCALISING trajectory whose T_wmap_wodom starts at (q_init, t_init) -- the vehicle's pose in the map frame at
+ * its first scan, i.e. the origin of its odometry frame -- instead of the identity.  That START consumes the arming;
+ * aloam_reset_odometry and aloam_prior_map_clear drop it; a trajectory the lane runs before that START is not disturbed.
+ * ALOAM_ERR_STATE without a prior map; ALOAM_ERR_INVALID_ARG for a bad lane, a NULL or non-finite pose or a zero quaternion (a
+ * finite one is normalised).  There is no new lane op.
+ * So a trajectory is in one of three modes, fixed at its START: odometry only, mapping, localising; one call advances mapping and
+ * localising lanes side by side.  A localising frame is the mapper's frame (laserMapping.cpp:309-734) with two parts left out:
+ *   - no ring-buffer shift (:323-507): the centre offsets are the prior map's and never change.  The centre cube is computed as at
+ *     :312-321 and the 5 x 5 x 3 window of :512-531 is clipped to the buffer by that loop's own bounds test, in its order.  A
+ *     vehicle that leaves the map sees a thin or empty window: ALOAM_FLAG_MAP_TOO_THIN, its pose the hand-off pose;
+ *   - no insertion and no re-filter (:736-801): the map is never written, so every lane sees the same map whoever ran before.
+ * Pose hand-off, the stack filters, the thin-map test on the window's points (corner > 10 and surf > 50), the association, the
+ * two solves and transformUpdate are the mapping frame's.  While a mapping frame would neither shift nor exceed
+ * cfg.max_map_points, a localising frame returns bit for bit the pose a mapping frame returns from the same store and T_wmap_wodom.
+ * cfg.mapping_skip_frame applies as to mapping lanes (scan j registers when j % k == 0, the others get the high-frequency pose
+ * from the lane's T_wmap_wodom); the registered sink serves localising rows like mapped rows; aloam_mapper_debug_state_lane answers
+ * for a localising lane (centre = the prior map's, valid = the clipped window of its last frame, its T_wmap_wodom, totals = the prior
+ * map's); aloam_mapper_export with lane = ALOAM_PRIOR_MAP and ALOAM_EXPORT_MAP exports the prior map (ALOAM_ERR_STATE without one).
+ * Per-frame flags are not returned by the stream calls (as for mapping lanes).
+ * A localising lane owns only what a frame writes, created at its first localising START (ALOAM_ERR_CUDA before any state changes):
+ * its frame state, 5-NN records and residual blocks for 2 x cfg.max_points queries, the two filtered stacks and the stack filter's
+ * sort buffers -- about 450 B per point of cfg.max_points, 0.18 GB at 400 000 and 27 MB at 60 000 (arithmetic from the buffer
+ * sizes, not measured), against about 1.75 GB for a mapping lane -- and no cube store if the lane never maps.
+ * Limits, each ALOAM_ERR_STATE: aloam_lane_save of a localising lane (snapshot format v1 has no section for it); sharded jobs.
+ * The lockstep stream calls and aloam_mapper_step never localise. */
+#define ALOAM_PRIOR_MAP (-1)
+int aloam_prior_map_load(aloam_ctx* ctx, const void* blob, long long n_bytes);
+int aloam_prior_map_clear(aloam_ctx* ctx);
+int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
+
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
  * interpolation ratio, then carry it to the sweep end with (q_last_curr, t_last_curr); the intensity keeps only the scan id.
  * (Dead code in the reference -- its call sites sit under `if (0)`, :533-552 -- provided because the DISTORTION build
