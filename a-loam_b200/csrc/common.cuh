@@ -80,4 +80,19 @@ __device__ __forceinline__ float sqdist3(float ax, float ay, float az, float bx,
   float dx = ax - bx, dy = ay - by, dz = az - bz;
   return dx * dx + dy * dy + dz * dz;
 }
+
+// pointAssociateToMap (laserMapping.cpp:154-163): q_w_curr * point + t_w_curr in double in the operation order of Eigen, stored
+// as float, intensity kept.  (ux, uy, uz, w, tx, ty, tz) = parameters[7] of the frame.
+__device__ __forceinline__ Pt4 point_associate_to_map(const Pt4& p, double ux, double uy, double uz, double w, double tx, double ty, double tz) {
+  const double vx = (double)p.x, vy = (double)p.y, vz = (double)p.z;
+  double uvx = uy * vz - uz * vy, uvy = uz * vx - ux * vz, uvz = ux * vy - uy * vx;
+  uvx = uvx + uvx; uvy = uvy + uvy; uvz = uvz + uvz;
+  const double cx = uy * uvz - uz * uvy, cy = uz * uvx - ux * uvz, cz = ux * uvy - uy * uvx;
+  Pt4 s;
+  s.x = (float)(((vx + w * uvx) + cx) + tx);
+  s.y = (float)(((vy + w * uvy) + cy) + ty);
+  s.z = (float)(((vz + w * uvz) + cz) + tz);
+  s.i = p.i;
+  return s;
+}
 #endif

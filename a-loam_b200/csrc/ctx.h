@@ -51,6 +51,7 @@ struct PriorSearch {
   const int* win[ALOAM_MAX_BATCH][2];
   const int* ctr[ALOAM_MAX_BATCH];
 };
+struct ExportLayout;   // cubemap.cu: where the segments of a store export are in the export and in the store
 }  // namespace aloam
 
 using namespace aloam;
@@ -183,8 +184,9 @@ struct aloam_ctx {
   std::vector<long long> reg_begin;
   std::vector<int> reg_count;
   int reg_rows = -1;
-  // aloam_mapper_export: segment offsets [2 * 4851 + 2] and the staging buffer of host destinations, created on first use
-  long long* d_export_off = nullptr;
+  // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
+  // memory, created on first use
+  ExportLayout* d_export_layout = nullptr;
   Pt4* d_export_stage = nullptr;
   double* h_poses = nullptr;     // pinned [kMaxStreamScans][7]
   double* d_poses = nullptr;     // device [kMaxStreamScans][7]: per-(scan, lane) world poses of a stream call (one D2H at the end)
@@ -218,15 +220,17 @@ struct aloam_ctx {
   // mapped streams: index of every lane's next scan in its trajectory (0 at a START); scan j goes to the mapper when
   // j % cfg.mapping_skip_frame == 0.  Carries over between calls; aloam_reset_odometry clears it.
   int lane_scan[ALOAM_MAX_BATCH] = {};
+  // the stack filters of mapping and localising frames run on s_stack, forked from and joined to the frame's stream by these
+  // events (cubemap.cu; created with the first cube store or locator)
+  cudaStream_t s_stack = nullptr;
+  cudaEvent_t ev_stack_fork = nullptr, ev_stack_join = nullptr;
   // localisation (cubemap.cu): the context's prior map, released by prior_map_release; the frame state and registration
-  // buffers of every lane that has localised (created at its first localising START); the auxiliary stream of the locate frame's
-  // stack filters.  lane_localising: the trajectory the lane runs (or ran last) registers against the prior map, fixed at its
-  // START.  lane_armed / lane_init: aloam_lane_localise has armed the lane's next mapped START with this T_wmap_wodom.
+  // buffers of every lane that has localised (created at its first localising START).  lane_localising: the trajectory the lane
+  // runs (or ran last) registers against the prior map, fixed at its START.  lane_armed / lane_init: aloam_lane_localise has
+  // armed the lane's next mapped START with this T_wmap_wodom.
   void* prior = nullptr;
   bool prior_owned = false;       // prior_map_release is on the release list
   void* locator[ALOAM_MAX_BATCH] = {};
-  cudaStream_t s_loc_aux = nullptr;
-  cudaEvent_t ev_loc_fork = nullptr, ev_loc_join = nullptr;
   bool lane_localising[ALOAM_MAX_BATCH] = {};
   bool lane_armed[ALOAM_MAX_BATCH] = {};
   double lane_init[ALOAM_MAX_BATCH][7] = {};

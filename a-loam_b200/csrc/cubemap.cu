@@ -16,7 +16,7 @@
 //                      cube and the group leader advances the cube's running end (allocating a slab from the free list
 //                      for a cube that was empty) -- O(n) instead of the O(n^2 / 256) rank search of the first version;
 //   * the per-cube re-filter of the valid cubes as ONE segmented VoxelGrid over up to 150 segments, in place.
-//   * the published clouds (:806-848): k_export_sizes / k_export_gather read a lane's store out in the reference's order
+//   * the published clouds (:806-848): k_export_sizes lays a lane's store out in the reference's order and k_store_copy copies it
 //                      (aloam_mapper_export), k_register_full moves a mapped scan's full cloud by the frame's refined pose.
 //   * localisation against a prior map (aloam_prior_map_load, aloam_lane_localise): the store of a saved lane, frozen, packed in
 //                      cube order and indexed ONCE with the hash grid of mapping.cu; a localising lane's frame is k_locate_begin
@@ -26,6 +26,7 @@
 // insertion, not 4851 x 2 slabs (6.4 GB) up front.  A full slab or an exhausted pool drops the overflow and raises
 // ALOAM_FLAG_CUBE_OVERFLOW instead of failing the frame (the reference grows its cubes without bound between re-filters).
 #include <climits>
+#include <memory>
 #include "common.cuh"
 #include "ctx.h"
 
@@ -35,6 +36,20 @@ constexpr int CW = 21, CH = 21, CD = 11, NCUBE = CW * CH * CD;   // laserCloudWi
 constexpr int kMaxValid = 128;
 constexpr int kPool = 1024;                                      // physical slabs per cloud type
 static_assert(NCUBE == kSnapCubes && kMaxValid == kSnapValid && kPool == kSnapPool, "the snapshot format describes this store");
+constexpr int kExportSegs = 2 * NCUBE;                           // segments of an export: segment 2 v + t is type t of its v-th cube
+
+}  // namespace
+
+// Where the points of an export are (device memory): segment s < nseg sits at positions [off[s], off[s + 1]) of the export and
+// at base[s] in the store, which may be a lane's slab or a cube of the prior map; total = off[nseg]
+struct aloam::ExportLayout {
+  int nseg;
+  long long total;
+  long long off[kExportSegs + 1];
+  Pt4* base[kExportSegs];
+};
+
+namespace {
 
 struct MapperState {
   double q_wmap_wodom[4], t_wmap_wodom[3];   // :116-117
@@ -78,8 +93,6 @@ struct Mapper {
   int* d_dbg_err = nullptr;                 //                                private error word
   int max_sub = 0;
   MapReg* reg = nullptr;                    // registration set: lane 0 shares the context's with the host API, the others own one
-  cudaStream_t s_aux = nullptr;             // the stack filters run here, beside the submap gather + index build
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 };
 
 // what every kernel of a frame needs of one lane: the frame runs over all lanes at once, each launch taking one record per lane
@@ -347,25 +360,6 @@ __global__ void __launch_bounds__(256) k_locate_begin(const __grid_constant__ Ba
   }
 }
 
-// grid-stride over the 2 x NCUBE segments of the ALOAM_EXPORT_MAP order (segment 2 i + t: cube i, type t), between that order
-// and the prior map's two packed clouds: segment (i, t) starts at cs[0][i + t] + cs[1][i] of the export and at cs[t][i] of cloud
-// t.  The points of the window [lo, hi) of the export: to_store: io[position - lo] -> cloud, else cloud -> io[position - lo].
-__global__ void __launch_bounds__(256) k_prior_copy(const int* __restrict__ cs, Pt4* __restrict__ p0, Pt4* __restrict__ p1, Pt4* __restrict__ io, long long lo,
-                                                    long long hi, int to_store) {
-  const int* cs0 = cs;
-  const int* cs1 = cs + NCUBE + 1;
-  for (int s = blockIdx.x; s < 2 * NCUBE; s += gridDim.x) {
-    const int i = s >> 1, ty = s & 1;
-    const long long o = (long long)cs0[i + ty] + cs1[i];
-    const int first = ty ? cs1[i] : cs0[i], n = (ty ? cs1[i + 1] : cs0[i + 1]) - first;
-    const long long b = max(o, lo), e = min(o + n, hi);
-    Pt4* __restrict__ cloud = (ty ? p1 : p0) + first;
-    for (long long q = b + threadIdx.x; q < e; q += blockDim.x) {
-      if (to_store) cloud[q - o] = io[q - lo]; else io[q - lo] = cloud[q - o];
-    }
-  }
-}
-
 // grid (CTAs, 2 types): after the index build, every indexed point's packed index g (gpts.w, written by k_grid_fill) becomes
 // prior_tag(cube i, j, k, rank in the cube): the cube is the last one whose prefix is <= g
 __global__ void __launch_bounds__(256) k_prior_tag(const __grid_constant__ GridTable corner, const __grid_constant__ GridTable surf, const int* __restrict__ cs) {
@@ -471,21 +465,6 @@ __device__ __forceinline__ void mapper_finish_body(MapperState* S) {
 __global__ void k_mapper_finish(const __grid_constant__ Batch<MapperLane> B) { mapper_finish_body(B.a[blockIdx.z].S); }   // grid (1, 1, lanes)
 
 
-// pointAssociateToMap (:154-163): q_w_curr * point + t_w_curr in double in the operation order of Eigen, stored as float,
-// intensity kept.  (ux, uy, uz, w, tx, ty, tz) = parameters[7] of the frame.
-__device__ __forceinline__ Pt4 point_associate_to_map(const Pt4& p, double ux, double uy, double uz, double w, double tx, double ty, double tz) {
-  const double vx = (double)p.x, vy = (double)p.y, vz = (double)p.z;
-  double uvx = uy * vz - uz * vy, uvy = uz * vx - ux * vz, uvz = ux * vy - uy * vx;
-  uvx = uvx + uvx; uvy = uvy + uvy; uvz = uvz + uvz;
-  const double cx = uy * uvz - uz * uvy, cy = uz * uvx - ux * uvz, cz = ux * uvy - uy * uvx;
-  Pt4 s;
-  s.x = (float)(((vx + w * uvx) + cx) + tx);
-  s.y = (float)(((vy + w * uvy) + cy) + ty);
-  s.z = (float)(((vz + w * uvz) + cz) + tz);
-  s.i = p.i;
-  return s;
-}
-
 // pointAssociateToMap (:154-163), then the cube of the stored point (:741-758)
 // blockIdx.y = cloud (0 corner stack, 1 surf stack); the scratch of cloud 1 starts `scratch_stride` elements in
 __device__ __forceinline__ void cube_ids_body(const Pt4* __restrict__ stack0, const Pt4* __restrict__ stack1, const MapperState* __restrict__ S, Pt4* __restrict__ world,
@@ -532,50 +511,55 @@ __global__ void k_register_full(const __grid_constant__ Batch<RegFullLane> B) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = point_associate_to_map(src[i], ux, uy, uz, w, tx, ty, tz);
 }
 
-// The segments of a store export in the reference's order, corner cube then surf cube of every cube: ALOAM_EXPORT_SURROUND the
-// valid cubes of the last frame in laserCloudSurroundInd order (:806-821, the same loop as the valid list), ALOAM_EXPORT_MAP
-// i = 0 .. 4850 (:823-836).  Segment s is cloud type s & 1 of cube export_cube(s).
-constexpr int kExportSegs = 2 * NCUBE;
-constexpr long long kExportStage = 4ll << 20;   // points of the staging buffer of a host destination (64 MB)
-__device__ __forceinline__ int export_segments(const MapperState* S, int what) { return what == ALOAM_EXPORT_SURROUND ? 2 * S->n_valid : kExportSegs; }
-__device__ __forceinline__ int export_cube(const MapperState* S, int what, int s) { return what == ALOAM_EXPORT_SURROUND ? S->valid[s >> 1] : s >> 1; }
-__device__ __forceinline__ int export_size(const MapperState* S, int what, int s) {
-  const int ty = s & 1, slab = S->slab_of[ty][export_cube(S, what, s)];
-  return slab < 0 ? 0 : S->cnt[ty][slab];
-}
+// ---- the exports of a store (aloam_mapper_export, lane snapshots, the prior map): the reference's order, corner cube then surf
+// cube of every cube -- ALOAM_EXPORT_SURROUND the valid cubes of the last frame in laserCloudSurroundInd order (:806-821, the same
+// loop as the valid list), ALOAM_EXPORT_MAP i = 0 .. 4850 (:823-836).  An ExportLayout says where each segment is in the export
+// and in the store; k_store_copy moves points between the two.
+constexpr long long kExportStage = 4ll << 20;   // points of the staging buffer of host memory (64 MB)
 
-// one CTA of 1024: off[s] = points of the export before segment s (exclusive scan of the sizes), off[nseg] and off[kExportSegs + 1]
-// = the total (the second at a fixed place for the host to read back)
-__global__ void __launch_bounds__(1024) k_export_sizes(const MapperState* __restrict__ S, int what, long long* __restrict__ off) {
-  __shared__ long long s_part[1024];
-  const int tid = threadIdx.x, nseg = export_segments(S, what);
-  const int per = (nseg + 1023) / 1024, b = tid * per, e = min(b + per, nseg);
-  long long sum = 0;
-  for (int s = b; s < e; ++s) sum += export_size(S, what, s);
-  s_part[tid] = sum;
+// One CTA of 1024 threads: the exclusive prefix of every thread's v over the block; s[1023] holds the total afterwards
+template <typename T> __device__ T block_scan_1024(T v, T* s) {
+  const int tid = threadIdx.x;
+  s[tid] = v;
   __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {   // inclusive scan of the per-thread sums
-    const long long v = tid >= d ? s_part[tid - d] : 0;
+  for (int d = 1; d < 1024; d <<= 1) {
+    const T u = tid >= d ? s[tid - d] : T(0);
     __syncthreads();
-    s_part[tid] += v;
+    s[tid] += u;
     __syncthreads();
   }
-  long long run = s_part[tid] - sum;
-  for (int s = b; s < e; ++s) { off[s] = run; run += export_size(S, what, s); }
-  if (tid == 1023) { off[nseg] = s_part[1023]; off[kExportSegs + 1] = s_part[1023]; }
+  return s[tid] - v;
 }
 
-// grid-stride over the segments: the points of segment s that fall in the window [lo, hi) of the export, 16-byte copies from the
-// slab to dst[position - lo]
-__global__ void __launch_bounds__(256) k_export_gather(const MapperState* __restrict__ S, int what, const long long* __restrict__ off, const Pt4* __restrict__ p0,
-                                                       const Pt4* __restrict__ p1, int cap0, int cap1, long long lo, long long hi, Pt4* __restrict__ dst) {
-  const int nseg = export_segments(S, what);
+// one CTA of 1024: the layout L of export `what` of the store (S, slab pools p0 / p1 of cap0 / cap1 points per slab)
+__global__ void __launch_bounds__(1024) k_export_sizes(const MapperState* __restrict__ S, int what, Pt4* p0, Pt4* p1, int cap0, int cap1, ExportLayout* __restrict__ L) {
+  __shared__ long long s_part[1024];
+  const int tid = threadIdx.x, nseg = what == ALOAM_EXPORT_SURROUND ? 2 * S->n_valid : kExportSegs;
+  const int per = (nseg + 1023) / 1024, b = tid * per, e = min(b + per, nseg);
+  auto slab = [&](int s) { return S->slab_of[s & 1][what == ALOAM_EXPORT_SURROUND ? S->valid[s >> 1] : s >> 1]; };
+  long long sum = 0;
+  for (int s = b; s < e; ++s) { const int k = slab(s); sum += k < 0 ? 0 : S->cnt[s & 1][k]; }
+  long long run = block_scan_1024(sum, s_part);
+  for (int s = b; s < e; ++s) {
+    const int k = slab(s);
+    L->off[s] = run;
+    L->base[s] = k < 0 ? nullptr : (s & 1 ? p1 + (size_t)k * cap1 : p0 + (size_t)k * cap0);
+    run += k < 0 ? 0 : S->cnt[s & 1][k];
+  }
+  if (tid == 1023) { L->off[nseg] = run; L->nseg = nseg; L->total = run; }
+}
+
+// grid-stride over the segments of layout L: the points of the window [lo, hi) of the export between io[position - lo] and the
+// store -- to_store: io -> store, else store -> io
+__global__ void __launch_bounds__(256) k_store_copy(const ExportLayout* __restrict__ L, Pt4* __restrict__ io, long long lo, long long hi, int to_store) {
+  const int nseg = L->nseg;
   for (int s = blockIdx.x; s < nseg; s += gridDim.x) {
-    const long long o = off[s], b = max(o, lo), e = min(off[s + 1], hi);
-    if (b >= e) continue;   // (a segment with points has a slab)
-    const int ty = s & 1, slab = S->slab_of[ty][export_cube(S, what, s)];
-    const Pt4* __restrict__ src = (ty ? p1 : p0) + (size_t)slab * (ty ? cap1 : cap0);
-    for (long long i = b + threadIdx.x; i < e; i += blockDim.x) dst[i - lo] = src[i - o];
+    const long long o = L->off[s], b = max(o, lo), e = min(L->off[s + 1], hi);
+    if (b >= e) continue;   // (a segment with points has a base)
+    Pt4* __restrict__ p = L->base[s];
+    for (long long q = b + threadIdx.x; q < e; q += blockDim.x) {
+      if (to_store) p[q - o] = io[q - lo]; else io[q - lo] = p[q - o];
+    }
   }
 }
 
@@ -583,9 +567,9 @@ __global__ void __launch_bounds__(256) k_export_gather(const MapperState* __rest
 
 // One CTA of 1024: the store a snapshot's table H describes.  State of a fresh trajectory first (the caller has zeroed S), then
 // the cubes with a count >= 0 take slabs 0, 1, 2, ... of their type in cube order (the rest of the pool stays free, ascending),
-// off[s] = exclusive prefix of the segment sizes in export order (segment 2 i + t: cube i, type t; off[kExportSegs] and
-// off[kExportSegs + 1] = the total, as k_export_sizes), and the fields that outlive a frame.
-__global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, long long* __restrict__ off) {
+// L = the layout of the ALOAM_EXPORT_MAP export of the rebuilt store, and the fields that outlive a frame.
+__global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, Pt4* p0, Pt4* p1, int cap0, int cap1,
+                                                              ExportLayout* __restrict__ L) {
   __shared__ long long s_pts[1024];
   __shared__ int s_slabs[2][1024];
   const int tid = threadIdx.x;
@@ -598,24 +582,21 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
     pts += max(c0, 0) + max(c1, 0);
     n0 += c0 >= 0; n1 += c1 >= 0;
   }
-  s_pts[tid] = pts; s_slabs[0][tid] = n0; s_slabs[1][tid] = n1;
-  __syncthreads();   // (also orders mapper_fresh_state's writes before the ones below)
-  for (int d = 1; d < 1024; d <<= 1) {   // inclusive scans of the per-thread sums
-    const long long v = tid >= d ? s_pts[tid - d] : 0;
-    const int v0 = tid >= d ? s_slabs[0][tid - d] : 0, v1 = tid >= d ? s_slabs[1][tid - d] : 0;
-    __syncthreads();
-    s_pts[tid] += v; s_slabs[0][tid] += v0; s_slabs[1][tid] += v1;
-    __syncthreads();
-  }
-  long long run = s_pts[tid] - pts;
-  int next[2] = {s_slabs[0][tid] - n0, s_slabs[1][tid] - n1};
+  // (the first barrier of the scans also orders mapper_fresh_state's writes before the ones below)
+  long long run = block_scan_1024(pts, s_pts);
+  int next[2] = {block_scan_1024(n0, s_slabs[0]), block_scan_1024(n1, s_slabs[1])};
   for (int i = b; i < e; ++i)
     for (int ty = 0; ty < 2; ++ty) {
       const int n = H->count[ty][i];
-      off[2 * i + ty] = run;
-      if (n >= 0) { const int s = next[ty]++; S->slab_of[ty][i] = s; S->cnt[ty][s] = n; run += n; }
+      L->off[2 * i + ty] = run;
+      L->base[2 * i + ty] = nullptr;
+      if (n >= 0) {
+        const int s = next[ty]++;
+        S->slab_of[ty][i] = s; S->cnt[ty][s] = n; run += n;
+        L->base[2 * i + ty] = ty ? p1 + (size_t)s * cap1 : p0 + (size_t)s * cap0;
+      }
     }
-  if (tid == 1023) { off[kExportSegs] = run; off[kExportSegs + 1] = run; S->free_top = s_slabs[0][1023]; S->free_top2 = s_slabs[1][1023]; }
+  if (tid == 1023) { L->off[kExportSegs] = run; L->nseg = kExportSegs; L->total = run; S->free_top = s_slabs[0][1023]; S->free_top2 = s_slabs[1][1023]; }
   if (tid < kMaxValid) S->valid[tid] = tid < H->n_valid ? H->valid[tid] : 0;
   if (tid == 0) {
     for (int a = 0; a < 3; ++a) S->cen[a] = H->cen[a];
@@ -623,19 +604,6 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
     S->frames = H->frames;
     for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = H->q_wmap_wodom[k];
     for (int k = 0; k < 3; ++k) S->t_wmap_wodom[k] = H->t_wmap_wodom[k];
-  }
-}
-
-// grid-stride over the segments, the inverse of k_export_gather: the points of segment s that fall in the window [lo, hi) of the
-// payload, from src[position - lo] into the cube's slab
-__global__ void __launch_bounds__(256) k_store_import_scatter(const MapperState* __restrict__ S, const long long* __restrict__ off, const Pt4* __restrict__ src,
-                                                              long long lo, long long hi, Pt4* __restrict__ p0, Pt4* __restrict__ p1, int cap0, int cap1) {
-  for (int s = blockIdx.x; s < kExportSegs; s += gridDim.x) {
-    const long long o = off[s], b = max(o, lo), e = min(off[s + 1], hi);
-    if (b >= e) continue;   // (a segment with points has a slab)
-    const int ty = s & 1, slab = S->slab_of[ty][s >> 1];
-    Pt4* __restrict__ dst = (ty ? p1 : p0) + (size_t)slab * (ty ? cap1 : cap0);
-    for (long long i = b + threadIdx.x; i < e; i += blockDim.x) dst[i - o] = src[i - lo];
   }
 }
 
@@ -738,6 +706,31 @@ int reset_lane(aloam_ctx* c, Mapper* m) {
   return ALOAM_OK;
 }
 
+// the stream and events of the stack filters' fork (stack_filters_fork), created with the first cube store or locator
+cudaError_t stack_stream_ensure(aloam_ctx* c) {
+  if (c->ev_stack_join) return cudaSuccess;
+  cudaError_t e = screate(c, &c->s_stack);
+  if (e == cudaSuccess) e = ecreate(c, &c->ev_stack_fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = ecreate(c, &c->ev_stack_join, cudaEventDisableTiming);
+  return e;
+}
+
+// the two scan-stack filters of a frame (:541-550) as one segmented pass over both clouds of every lane (records B, filters f on
+// buffers bufs), on s_stack: they read only the scans' clouds, so they run beside what the frame issues next on c->stream until
+// the caller joins on ev_stack_join
+int stack_filters_fork(aloam_ctx* c, int nb, const Batch<MapperLane>& B, const SegFilter* f, SegBuffers* const* bufs, int n_upper_c, int n_upper_s) {
+  cudaStream_t main_stream = c->stream;
+  CUDA_CHECK_RET(cudaEventRecord(c->ev_stack_fork, main_stream));
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->s_stack, c->ev_stack_fork, 0));
+  c->stream = c->s_stack;
+  launch_ex(c, KID_VOXEL, k_seg_two, dim3(1, 1, nb), dim3(32), 0, 1, false, B, c->cfg.line_res, c->cfg.plane_res);
+  vox_seg_filter(c, nb, f, bufs, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
+  const cudaError_t e = cudaEventRecord(c->ev_stack_join, c->s_stack);
+  c->stream = main_stream;
+  CUDA_CHECK_RET(e);
+  return ALOAM_OK;
+}
+
 int ensure_mapper(aloam_ctx* c, int lane) {
   if (c->mapper[lane]) return ALOAM_OK;
   if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
@@ -757,8 +750,7 @@ int ensure_mapper(aloam_ctx* c, int lane) {
   ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
   ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
   ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
-  ok = ok && screate(c, &m->s_aux) == cudaSuccess;
-  ok = ok && ecreate(c, &m->ev_fork, cudaEventDisableTiming) == cudaSuccess && ecreate(c, &m->ev_join, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && stack_stream_ensure(c) == cudaSuccess;
   ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
   // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
   // created here, after the context's (which fixes the table size)
@@ -775,37 +767,33 @@ int ensure_mapper(aloam_ctx* c, int lane) {
   return ALOAM_OK;
 }
 
-// k_export_sizes of `what` over the store of m into c->d_export_off (created on first use); *n = the size of the export.  Synchronises.
+// the layout of export `what` of the store of m into c->d_export_layout (created on first use); *n = the size of the export.
+// Synchronises.
 int export_sizes(aloam_ctx* c, const Mapper* m, int what, long long* n) {
-  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
-  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, c->d_export_off);
-  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, c->d_export_off + kExportSegs + 1, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+  if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
+  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->d_export_layout);
+  CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, &c->d_export_layout->total, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   *n = c->pin->export_total;
   return ALOAM_OK;
 }
 
-// the staging buffer of host sources and destinations (kExportStage points), created on first use
-int export_stage(aloam_ctx* c) {
-  if (!c->d_export_stage) CUDA_CHECK_RET(dalloc(c, &c->d_export_stage, (size_t)kExportStage));
-  return ALOAM_OK;
-}
-
-// the n points of the export export_sizes has just sized, into dst on c->stream (not synchronised): device memory is written in
-// place, host memory in windows of the staging buffer, one device-to-host copy each
-int export_gather(aloam_ctx* c, const Mapper* m, int what, long long n, char* dst, bool device) {
+// the points [0, n) of the export layout L describes, between the store and `mem` (to_store: mem -> store, else store -> mem), on
+// c->stream, not synchronised: device memory in place, host memory through the staging buffer (created on first use) one window
+// at a time, copied in before the window's launch or out after it
+int store_copy(aloam_ctx* c, const ExportLayout* L, long long n, char* mem, bool device, bool to_store) {
   const int blocks = std::min(kExportSegs, c->sms * 8);
   if (device) {
-    LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], 0ll, n,
-           reinterpret_cast<Pt4*>(dst));
+    LAUNCH(c, KID_CUBES, k_store_copy, blocks, 256, 0, L, reinterpret_cast<Pt4*>(mem), 0ll, n, (int)to_store);
   } else {
-    const int rc = export_stage(c); if (rc) return rc;
+    if (!c->d_export_stage) CUDA_CHECK_RET(dalloc(c, &c->d_export_stage, (size_t)kExportStage));
     for (long long lo = 0; lo < n; lo += kExportStage) {
       const long long hi = std::min(n, lo + kExportStage);
-      LAUNCH(c, KID_CUBES, k_export_gather, blocks, 256, 0, m->d_state, what, c->d_export_off, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], lo, hi,
-             c->d_export_stage);
-      CUDA_CHECK_RET(cudaMemcpyAsync(dst + lo * sizeof(Pt4), c->d_export_stage, (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyDeviceToHost, c->stream));
+      const size_t bytes = (size_t)(hi - lo) * sizeof(Pt4);
+      if (to_store) CUDA_CHECK_RET(cudaMemcpyAsync(c->d_export_stage, mem + lo * sizeof(Pt4), bytes, cudaMemcpyHostToDevice, c->stream));
+      LAUNCH(c, KID_CUBES, k_store_copy, blocks, 256, 0, L, c->d_export_stage, lo, hi, (int)to_store);
+      if (!to_store) CUDA_CHECK_RET(cudaMemcpyAsync(mem + lo * sizeof(Pt4), c->d_export_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
     }
   }
   CUDA_CHECK_RET(cudaGetLastError());
@@ -817,7 +805,8 @@ int export_gather(aloam_ctx* c, const Mapper* m, int what, long long n, char* ds
 
 // The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
 // exclusive prefix of the snapshot's counts) and a hash grid over ALL of them, built once by prior_index; the centre offsets of
-// the store, which never change (no localising frame shifts the ring buffer).  Plain cudaMalloc, freed by prior_map_release.
+// the store, which never change (no localising frame shifts the ring buffer); the layout of its ALOAM_EXPORT_MAP export.  Plain
+// cudaMalloc, freed by prior_map_release.
 struct PriorMap {
   Pt4* pts[2] = {nullptr, nullptr};
   int n[2] = {0, 0};
@@ -825,6 +814,7 @@ struct PriorMap {
   int* d_cube_start = nullptr;   // [2][NCUBE + 1]
   int* d_n = nullptr;            // [2]
   GridTable grid[2] = {};
+  ExportLayout* d_layout = nullptr;
 };
 // what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
 // k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
@@ -839,7 +829,7 @@ struct Locator {
 void prior_free(PriorMap* p) {
   if (!p) return;
   for (int t = 0; t < 2; ++t) { cudaFree(p->pts[t]); cudaFree(p->grid[t].slots); cudaFree(p->grid[t].dyn); cudaFree(p->grid[t].gpts); }
-  cudaFree(p->d_cube_start); cudaFree(p->d_n);
+  cudaFree(p->d_cube_start); cudaFree(p->d_n); cudaFree(p->d_layout);
   delete p;
 }
 // the one place a context's prior map is released: aloam_prior_map_clear, a load that replaces it, aloam_destroy
@@ -851,26 +841,6 @@ void prior_map_release(aloam_ctx* c) {
 // the frame state of the lane a record runs on: its locator's when it localises, else its cube store's
 MapperState* lane_state(const aloam_ctx* c, const MapperIn& in) {
   return in.localise ? static_cast<Locator*>(c->locator[in.lane])->d_state : static_cast<Mapper*>(c->mapper[in.lane])->d_state;
-}
-
-// the export-order points [0, n) between the prior map's clouds and memory at `mem` (device in place, host through the staging
-// buffer), on c->stream, not synchronised
-int prior_copy(aloam_ctx* c, PriorMap* p, long long n, char* mem, bool device, bool to_store) {
-  const int blocks = std::min(2 * NCUBE, c->sms * 8);
-  if (device) {
-    LAUNCH(c, KID_CUBES, k_prior_copy, blocks, 256, 0, p->d_cube_start, p->pts[0], p->pts[1], reinterpret_cast<Pt4*>(mem), 0ll, n, (int)to_store);
-  } else {
-    const int rc = export_stage(c); if (rc) return rc;
-    for (long long lo = 0; lo < n; lo += kExportStage) {
-      const long long hi = std::min(n, lo + kExportStage);
-      const size_t bytes = (size_t)(hi - lo) * sizeof(Pt4);
-      if (to_store) CUDA_CHECK_RET(cudaMemcpyAsync(c->d_export_stage, mem + lo * sizeof(Pt4), bytes, cudaMemcpyHostToDevice, c->stream));
-      LAUNCH(c, KID_CUBES, k_prior_copy, blocks, 256, 0, p->d_cube_start, p->pts[0], p->pts[1], c->d_export_stage, lo, hi, (int)to_store);
-      if (!to_store) CUDA_CHECK_RET(cudaMemcpyAsync(mem + lo * sizeof(Pt4), c->d_export_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
-    }
-  }
-  CUDA_CHECK_RET(cudaGetLastError());
-  return ALOAM_OK;
 }
 
 // the persistent index: the k_grid_* chain of mapping.cu once over both packed clouds, then the cube tags
@@ -931,33 +901,20 @@ int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool dev
   long long total = 0;
   int rc = export_sizes(c, m, ALOAM_EXPORT_MAP, &total); if (rc) return rc;
   if (total != n) return ALOAM_ERR_STATE;
-  return n > 0 ? export_gather(c, m, ALOAM_EXPORT_MAP, n, dst, device) : ALOAM_OK;
+  return n > 0 ? store_copy(c, c->d_export_layout, n, dst, device, false) : ALOAM_OK;
 }
 
 // Makes lane `lane`'s store (it exists) the one a validated snapshot table describes: *head (pinned host memory) goes to the
-// device, k_store_import_tables rebuilds the tables, k_store_import_scatter moves the head->n_points points of pts into the
-// slabs -- from device memory in place, from host memory through the staging buffer.  Synchronises.
+// device, k_store_import_tables rebuilds the tables and lays the store out, store_copy moves the head->n_points points of pts into
+// the slabs.  Synchronises.
 int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device) {
   Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
-  if (!c->d_export_off) CUDA_CHECK_RET(dalloc(c, &c->d_export_off, (size_t)kExportSegs + 2));
+  if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
   if (!c->d_snap_store) CUDA_CHECK_RET(dalloc(c, &c->d_snap_store, 1));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_snap_store, head, sizeof(SnapStore), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
-  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, c->d_export_off);
-  const long long n = head->n_points;
-  const int blocks = std::min(kExportSegs, c->sms * 8);
-  if (device && n > 0) {
-    LAUNCH(c, KID_CUBES, k_store_import_scatter, blocks, 256, 0, m->d_state, c->d_export_off, reinterpret_cast<const Pt4*>(pts), 0ll, n, m->d_pts[0], m->d_pts[1],
-           m->cap[0], m->cap[1]);
-  } else if (n > 0) {
-    const int rc = export_stage(c); if (rc) return rc;
-    for (long long lo = 0; lo < n; lo += kExportStage) {
-      const long long hi = std::min(n, lo + kExportStage);
-      CUDA_CHECK_RET(cudaMemcpyAsync(c->d_export_stage, pts + lo * sizeof(Pt4), (size_t)(hi - lo) * sizeof(Pt4), cudaMemcpyHostToDevice, c->stream));
-      LAUNCH(c, KID_CUBES, k_store_import_scatter, blocks, 256, 0, m->d_state, c->d_export_off, c->d_export_stage, lo, hi, m->d_pts[0], m->d_pts[1],
-             m->cap[0], m->cap[1]);
-    }
-  }
+  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->d_export_layout);
+  if (head->n_points > 0) { const int rc = store_copy(c, c->d_export_layout, head->n_points, const_cast<char*>(pts), device, true); if (rc) return rc; }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
@@ -971,7 +928,7 @@ int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const ch
 // with the context's set, shared with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && sharded_job(c))) return ALOAM_ERR_STATE;
-  int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's auxiliary stream carries the stack filters of every lane
+  int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's store gives the sizes every lane shares
   for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
   rc = ensure_map_buffers(c); if (rc) return rc;     // lane 0's set
   Mapper* m0 = static_cast<Mapper*>(c->mapper[0]);
@@ -1001,20 +958,8 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   }
   const int max_sub = m0->max_sub, cap1 = m0->cap[1];
   const int refilter_cap = (int)m0->buf.cap;   // refilter_bound: the same for every lane
-  // ---- stack filters (:541-550): one segmented pass for both clouds of every lane.  They read only the scans' clouds, the
-  // gather + index build below only the cube stores: two independent chains, the filters forked onto an auxiliary stream and
-  // joined before the registration.
-  {
-    cudaStream_t main_stream = c->stream;
-    CUDA_CHECK_RET(cudaEventRecord(m0->ev_fork, main_stream));
-    CUDA_CHECK_RET(cudaStreamWaitEvent(m0->s_aux, m0->ev_fork, 0));
-    c->stream = m0->s_aux;
-    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1, 1, nb), dim3(32), 0, 1, false, B, c->cfg.line_res, c->cfg.plane_res);
-    vox_seg_filter(c, nb, stack_f, bufs, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
-    const cudaError_t e = cudaEventRecord(m0->ev_join, m0->s_aux);
-    c->stream = main_stream;
-    CUDA_CHECK_RET(e);
-  }
+  // ---- stack filters (:541-550), beside the gather + index build below, which read only the cube stores
+  rc = stack_filters_fork(c, nb, B, stack_f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub, fresh);
   launch_ex(c, KID_CUBES, k_mapper_gather, dim3(kMaxValid, 2, nb), dim3(256), 0, 1, true, B);
   if (c->shard_count > 1) {
@@ -1028,7 +973,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     map_index_build(c, nb, io, max_sub);
   }
   c->have_map = true;
-  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, m0->ev_join, 0));   // join: the filtered stacks are ready
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_stack_join, 0));   // join: the filtered stacks are ready
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- optimisation (:554-733)
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
@@ -1088,13 +1033,10 @@ int mapper_ensure_lanes(aloam_ctx* c, int nb) {
 int mapper_ensure_lane(aloam_ctx* c, int lane) { return ensure_mapper(c, lane); }
 
 // lane `lane`'s locator, created on first use and published only when fully allocated (what was acquired before a failure
-// belongs to the context until aloam_destroy); the auxiliary stream of the locate frame with the first one
+// belongs to the context until aloam_destroy)
 int locator_ensure(aloam_ctx* c, int lane) {
   if (c->locator[lane]) return ALOAM_OK;
-  if (!c->ev_loc_join) {
-    if (screate(c, &c->s_loc_aux) != cudaSuccess || ecreate(c, &c->ev_loc_fork, cudaEventDisableTiming) != cudaSuccess ||
-        ecreate(c, &c->ev_loc_join, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
-  }
+  if (stack_stream_ensure(c) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
   Locator* m = new (std::nothrow) Locator();
   if (!m) return ALOAM_ERR_CUDA;
   own(c, [m] { delete m; });
@@ -1136,22 +1078,13 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     stack_f[l] = seg_filter(m->buf, 31, &S->err);
     bufs[l] = &m->buf;
   }
-  {
-    cudaStream_t main_stream = c->stream;
-    CUDA_CHECK_RET(cudaEventRecord(c->ev_loc_fork, main_stream));
-    CUDA_CHECK_RET(cudaStreamWaitEvent(c->s_loc_aux, c->ev_loc_fork, 0));
-    c->stream = c->s_loc_aux;
-    launch_ex(c, KID_VOXEL, k_seg_two, dim3(1, 1, nb), dim3(32), 0, 1, false, B, c->cfg.line_res, c->cfg.plane_res);
-    vox_seg_filter(c, nb, stack_f, bufs, 2, n_upper_c + n_upper_s, std::max(n_upper_c, n_upper_s));
-    const cudaError_t e = cudaEventRecord(c->ev_loc_join, c->s_loc_aux);
-    c->stream = main_stream;
-    CUDA_CHECK_RET(e);
-  }
+  // the stack filters share s_stack with the mapping frame's: this fork is recorded after the whole mapping frame of the step
+  int rc = stack_filters_fork(c, nb, B, stack_f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_locate_begin, dim3(1, 1, nb), dim3(256), 0, 1, true, L, (const int*)P->d_cube_start, P->cen[0], P->cen[1], P->cen[2]);
-  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_loc_join, 0));   // join: the filtered stacks are ready
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_stack_join, 0));   // join: the filtered stacks are ready
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  const int rc = map_register_device(c, nb, io, nq_upper, &ps); if (rc) return rc;
+  rc = map_register_device(c, nb, io, nq_upper, &ps); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1181,7 +1114,8 @@ int aloam_prior_map_load(aloam_ctx* c, const void* blob, long long n_bytes) {
     p->n[t] = (int)run;
   }
   for (int a = 0; a < 3; ++a) p->cen[a] = H->cen[a];
-  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess;
+  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&p->d_layout, sizeof(ExportLayout)) == cudaSuccess;
   for (int t = 0; t < 2 && ok; ++t) {
     GridTable& g = p->grid[t];
     g.cap_slots = grid_mask_for(p->n[t], 1u << 30) + 1;
@@ -1192,10 +1126,21 @@ int aloam_prior_map_load(aloam_ctx* c, const void* blob, long long n_bytes) {
   }
   auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); prior_free(p); return code; };
   if (!ok) return fail(ALOAM_ERR_CUDA);
+  // the ALOAM_EXPORT_MAP layout of the packed clouds: segment 2 i + t is cube i of cloud t
+  std::unique_ptr<ExportLayout> L(new (std::nothrow) ExportLayout());
+  if (!L) return fail(ALOAM_ERR_CUDA);
+  L->nseg = kExportSegs;
+  for (int s = 0; s < kExportSegs; ++s) {
+    const int* t = &cs[(size_t)(s & 1) * (NCUBE + 1) + (s >> 1)];
+    L->base[s] = p->pts[s & 1] + t[0];
+    L->off[s + 1] = L->off[s] + (t[1] - t[0]);
+  }
+  L->total = L->off[kExportSegs];
   if (cudaMemcpyAsync(p->d_cube_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
-      cudaMemcpyAsync(p->d_n, p->n, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+      cudaMemcpyAsync(p->d_n, p->n, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+      cudaMemcpyAsync(p->d_layout, L.get(), sizeof(ExportLayout), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
     return fail(ALOAM_ERR_CUDA);
-  if (H->n_points > 0) { rc = prior_copy(c, p, H->n_points, const_cast<char*>(b) + store + sizeof(SnapStore), kind, true); if (rc) return fail(rc); }
+  if (H->n_points > 0) { rc = store_copy(c, p->d_layout, H->n_points, const_cast<char*>(b) + store + sizeof(SnapStore), kind, true); if (rc) return fail(rc); }
   prior_index(c, p);
   if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ALOAM_ERR_CUDA);
   if (!c->prior_owned) { own(c, [c] { prior_map_release(c); }); c->prior_owned = true; }
@@ -1346,8 +1291,7 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
   cudaPointerAttributes at = {};
   CUDA_CHECK_RET(cudaPointerGetAttributes(&at, out));
   const bool device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
-  rc = prior ? prior_copy(c, pm, n, reinterpret_cast<char*>(out), device, false) : export_gather(c, m, what, n, reinterpret_cast<char*>(out), device);
-  if (rc) return rc;
+  rc = store_copy(c, prior ? pm->d_layout : c->d_export_layout, n, reinterpret_cast<char*>(out), device, false); if (rc) return rc;
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;

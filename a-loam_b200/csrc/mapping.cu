@@ -485,9 +485,6 @@ __device__ __forceinline__ void lsq_5x3(const double (&Ain)[15], const double (&
   for (int c = 0; c < 3; ++c) n[c] = perm[0] == c ? y[0] : (perm[1] == c ? y[1] : y[2]);   // n[perm[k]] = y[k]
 }
 
-struct D3 { double x, y, z; };
-__device__ __forceinline__ D3 cross3(const D3& a, const D3& b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
-
 }  // namespace
 
 // K5: exact 5-NN of every stack point at pose7.  counts3 = {n_corner, n_surf, n_corner + n_surf} in device memory;
@@ -511,19 +508,8 @@ __device__ __forceinline__ void map_knn5_body(const Pt4* __restrict__ corner_sta
     const bool is_corner = wid < n_corner;
     const Pt4 ori = is_corner ? corner_stack[wid] : surf_stack[wid - n_corner];
     const GridTable& G = is_corner ? corner_map.grid : surf_map.grid;
-    // pointAssociateToMap (:154-163): q * p + t in double, stored to float
-    float qx, qy, qz;
-    {
-      const D3 u{pose[0], pose[1], pose[2]};
-      const double w = pose[3];
-      const D3 v{(double)ori.x, (double)ori.y, (double)ori.z};
-      D3 uv = cross3(u, v);
-      uv.x = uv.x + uv.x; uv.y = uv.y + uv.y; uv.z = uv.z + uv.z;
-      const D3 c2 = cross3(u, uv);
-      qx = (float)(((v.x + w * uv.x) + c2.x) + pose[4]);
-      qy = (float)(((v.y + w * uv.y) + c2.y) + pose[5]);
-      qz = (float)(((v.z + w * uv.z) + c2.z) + pose[6]);
-    }
+    const Pt4 q = point_associate_to_map(ori, pose[0], pose[1], pose[2], pose[3], pose[4], pose[5], pose[6]);
+    const float qx = q.x, qy = q.y, qz = q.z;
     bool reject = false;
     if (shard_count > 1 && owner_of(cell_of(qx, G.inv_cs), shard_count) != shard_rank) reject = true;
     float nd[5]; int ni[5], np[5];
@@ -582,19 +568,8 @@ __global__ void __launch_bounds__(256) k_map_knn5_prior(const __grid_constant__ 
     const Pt4 ori = is_corner ? corner_stack[wid] : surf_stack[wid - n_corner];
     const GridTable& G = is_corner ? P.corner : P.surf;
     const int* win = s_win[is_corner ? 0 : 1];
-    // pointAssociateToMap (:154-163): q * p + t in double, stored to float
-    float qx, qy, qz;
-    {
-      const D3 u{pose[0], pose[1], pose[2]};
-      const double w = pose[3];
-      const D3 v{(double)ori.x, (double)ori.y, (double)ori.z};
-      D3 uv = cross3(u, v);
-      uv.x = uv.x + uv.x; uv.y = uv.y + uv.y; uv.z = uv.z + uv.z;
-      const D3 c2v = cross3(u, uv);
-      qx = (float)(((v.x + w * uv.x) + c2v.x) + pose[4]);
-      qy = (float)(((v.y + w * uv.y) + c2v.y) + pose[5]);
-      qz = (float)(((v.z + w * uv.z) + c2v.z) + pose[6]);
-    }
+    const Pt4 q = point_associate_to_map(ori, pose[0], pose[1], pose[2], pose[3], pose[4], pose[5], pose[6]);
+    const float qx = q.x, qy = q.y, qz = q.z;
     float nd[5]; int ni[5], np[5];
     TopK<5> t; t.init();
     visit_block27(G, is_corner ? mask_c : mask_s, qx, qy, qz, [&](float x, float y, float z, int tag, int slot) {
