@@ -27,7 +27,7 @@ EXPORTED_SYMBOLS = [
     "aloam_scan_stream_lanes", "aloam_debug_shard_emulate", "aloam_debug_map_sizes",
     "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
     "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
-    "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise",
+    "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise", "aloam_debug_prior_associate",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -134,6 +134,7 @@ def lib():
         L.aloam_prior_map_load.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
         L.aloam_prior_map_clear.argtypes = [C.c_void_p]
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
+        L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
         _LIB = L
     return _LIB
 
@@ -390,6 +391,15 @@ class Aloam:
         b, kb = _view(surf_stack)
         fits = np.zeros((max(a.n + b.n, 1), 14))
         _check(lib().aloam_mapping_associate(self._h, a, b, _dp(np.ascontiguousarray(x, np.float64)), _dp(fits)))
+        return fits[:a.n + b.n]
+
+    def prior_associate(self, lane, corner_stack, surf_stack, x):
+        """mapping_associate against the prior map through the window of `lane`'s latest localising frame; nn(5) are indices in
+        the submap a mapping frame would gather from the same store"""
+        a, ka = _view(corner_stack)
+        b, kb = _view(surf_stack)
+        fits = np.zeros((max(a.n + b.n, 1), 14))
+        _check(lib().aloam_debug_prior_associate(self._h, int(lane), a, b, _dp(np.ascontiguousarray(x, np.float64)), _dp(fits)))
         return fits[:a.n + b.n]
 
     # --- multi-GPU map sharding: rank 0 makes the id, everybody joins (ship the id with torch.distributed)

@@ -234,6 +234,9 @@ struct aloam_ctx {
   bool lane_localising[ALOAM_MAX_BATCH] = {};
   bool lane_armed[ALOAM_MAX_BATCH] = {};
   double lane_init[ALOAM_MAX_BATCH][7] = {};
+  // the lane's locator holds the window of a localising frame against the current prior map (aloam_debug_prior_associate);
+  // set by the frame, cleared when the prior map is released
+  bool lane_window[ALOAM_MAX_BATCH] = {};
   int lockstep_ops[kMaxStreamScans] = {};   // the lane schedule a lockstep stream call hands to the stream driver
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
@@ -316,6 +319,9 @@ int* mapper_err_acc(aloam_ctx* c, int lane);
 int locator_ensure(aloam_ctx* c, int lane);
 int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int* locator_err_acc(aloam_ctx* c, int lane);
+// the search of lane `lane`'s latest localising frame as record 0 of *ps: the prior map's grids, the window tables and centre cube
+// in the lane's locator.  ALOAM_ERR_STATE without a prior map or when the lane has run no localising frame against it.
+int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps);
 inline bool any_lane_localising(const aloam_ctx* c) {
   for (int l = 0; l < ALOAM_MAX_BATCH; ++l) if (c->lane_running[l] && c->lane_localising[l]) return true;
   return false;

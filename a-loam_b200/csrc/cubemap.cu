@@ -836,6 +836,7 @@ void prior_free(PriorMap* p) {
 void prior_map_release(aloam_ctx* c) {
   prior_free(static_cast<PriorMap*>(c->prior));
   c->prior = nullptr;
+  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_window[l] = false;   // the windows were cut from this map
 }
 
 // the frame state of the lane a record runs on: its locator's when it localises, else its cube store's
@@ -1088,6 +1089,17 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
+  for (int l = 0; l < nb; ++l) c->lane_window[in[l].lane] = true;
+  return ALOAM_OK;
+}
+
+int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps) {
+  const PriorMap* P = static_cast<const PriorMap*>(c->prior);
+  if (!P || !c->lane_window[lane]) return ALOAM_ERR_STATE;
+  MapperState* S = static_cast<Locator*>(c->locator[lane])->d_state;
+  *ps = {};
+  ps->grid = PriorGrid{P->grid[0], P->grid[1]};
+  ps->win[0][0] = S->sub_off[0]; ps->win[0][1] = S->sub_off[1]; ps->ctr[0] = S->ctr;
   return ALOAM_OK;
 }
 

@@ -981,25 +981,48 @@ int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cl
   return c->pin->peer_err ? ALOAM_ERR_COMM : ALOAM_OK;   // a peer did not answer: the pose rests on a partial sum
 }
 
-// association only (tests): fits = (n_corner + n_surf) x 14 doubles [query, type (-1 rejected), p0(3), p1(3), d, nn(5)]
+// association only (tests): the launches of one outer iteration of aloam_mapping_register through the context's registration
+// set -- against its uploaded submaps, or with `prior` against the prior map through one lane's window.  fits = (n_corner +
+// n_surf) x 14 doubles [query, type (-1 rejected), p0(3), p1(3), d, nn(5)].  The records start as NaN, so what a row leaves
+// unwritten is NaN, the same on every call: a query without an accepted neighbourhood has only its type, one whose fit fails
+// its type, query and nn.
+static int associate_fits(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, const double x[7], double* fits,
+                          const PriorSearch* prior) {
+  int rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
+  for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
+  const int nq = corner_stack.n + surf_stack.n;
+  if (nq > 0) {
+    CUDA_CHECK_RET(cudaMemsetAsync(c->d_fits, 0xff, (size_t)nq * 14 * 8, c->stream));
+    const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
+    map_associate_device(c, 1, &io, nq, false, c->d_fits, prior);
+    CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));
+  }
+  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 int aloam_mapping_associate(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, const double x[7], double* fits) {
   if (!c || !x || !fits) return ALOAM_ERR_INVALID_ARG;
   if (!c->have_map) return ALOAM_ERR_STATE;
   int rc = check_view(corner_stack); if (rc) return rc;
   rc = check_view(surf_stack); if (rc) return rc;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  rc = upload_stacks(c, corner_stack, surf_stack); if (rc) return rc;
-  for (int k = 0; k < 7; ++k) c->pin->pose_in[k] = x[k];
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  const int nq = corner_stack.n + surf_stack.n;
-  if (nq > 0) {   // the launches of one outer iteration of aloam_mapping_register
-    const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
-    map_associate_device(c, 1, &io, nq, false, c->d_fits, nullptr);
-    CUDA_CHECK_RET(cudaMemcpyAsync(fits, c->d_fits, (size_t)nq * 14 * 8, cudaMemcpyDeviceToHost, c->stream));
-  }
-  CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  CUDA_CHECK_RET(cudaGetLastError());
-  return ALOAM_OK;
+  return associate_fits(c, corner_stack, surf_stack, x, fits, nullptr);
+}
+
+// aloam_mapping_associate against the prior map through the window of lane `lane`'s latest localising frame (tests)
+int aloam_debug_prior_associate(aloam_ctx* c, int lane, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack, const double x[7],
+                                double* fits) {
+  if (!c || !x || !fits || lane < 0 || lane >= c->n_lanes) return ALOAM_ERR_INVALID_ARG;
+  int rc = check_view(corner_stack); if (rc) return rc;
+  rc = check_view(surf_stack); if (rc) return rc;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  PriorSearch ps;
+  rc = locator_prior_search(c, lane, &ps); if (rc) return rc;
+  rc = ensure_map_buffers(c); if (rc) return rc;   // the stacks, 5-NN records, residual blocks and fit records of the context's set
+  return associate_fits(c, corner_stack, surf_stack, x, fits, &ps);
 }
 
 int aloam_map_knn_impl(aloam_ctx* c, int which, aloam_cloud_view queries, int k, int* idx, float* sqdist) {

@@ -367,9 +367,16 @@ int aloam_solve(aloam_ctx* ctx, const double* blocks, int n_blocks, double x[7],
 int aloam_debug_features(aloam_ctx* ctx, float* curvature, int* label, int* scan_start, int* scan_end);
 
 /* association + fits of laserMapping.cpp:577-687 at pose x (tests): fits = (n_corner + n_surf) x 14 doubles
- * [query, type (-1 rejected, 0 edge, 2 plane-norm), p0(3), p1(3), d, nn(5)], corner rows first */
+ * [query, type (-1 rejected, 0 edge, 2 plane-norm), p0(3), p1(3), d, nn(5)], corner rows first.  A field a row does not reach
+ * is NaN: a query without an accepted neighbourhood has only its type, one whose fit fails its type, query and nn. */
 int aloam_mapping_associate(aloam_ctx* ctx, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack,
                             const double x[7], double* fits);
+/* association + fits against the prior map through the window that lane `lane`'s latest localising frame left (tests):
+ * k_map_knn5_prior + k_map_fit at pose x; fits as aloam_mapping_associate, nn(5) = window offset + rank in the cube,
+ * i.e. the index in the submap a mapping frame would gather from the same store.  ALOAM_ERR_STATE without a prior map or
+ * when the lane has not run a localising frame against the current one. */
+int aloam_debug_prior_associate(aloam_ctx* ctx, int lane, aloam_cloud_view corner_stack, aloam_cloud_view surf_stack,
+                                const double x[7], double* fits);
 
 /* ---- map cube store + the mapping loop around it (lane 0 of the mapper; the other lanes exist only for
  * aloam_scan_stream_mapped_batch) (laserMapping.cpp:74-108,142-163,309-550,736-801; SURVEY.md 8 f-1).
