@@ -87,6 +87,8 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   if (cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64) return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
   if (!(cfg.nearby_scan >= 1.0)) return ALOAM_ERR_INVALID_ARG;   // the association's break tables need a window of +-1 ring at least
+  // HuberLoss(a) needs a > 0, and a VoxelGrid leaf <= 0 or NaN has no voxels
+  if (!(cfg.huber > 0) || !(cfg.line_res > 0) || !(cfg.plane_res > 0)) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_batch < 1 || cfg.max_batch > ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_ring_points < 64 || cfg.max_ring_points > ALOAM_MAX_RING_POINTS || cfg.max_ring_points % 32) return ALOAM_ERR_INVALID_ARG;
   if (cfg.max_map_points > (1 << 30)) return ALOAM_ERR_INVALID_ARG;   // the map's hash-grid slot count is a 32-bit power of two

@@ -13,16 +13,18 @@
 //   once -- it is one contiguous slice of the bucket-major array: one round for its two delimiters, then 12 coalesced
 //   float4 loads in flight per lane -- with k0 = 1 (3 for rho < 6.5 m, where a bucket is narrower than the point
 //   spacing); 98 % of the queries end there.  The rest grow the interval bucket by bucket.  The sweep stops at the
-//   latest when the bound exceeds the reference's own threshold (DISTANCE_SQ_THRESHOLD = 25 m^2), beyond which the
-//   reference discards the match anyway, or when the whole circle has been read.
+//   latest when the bound exceeds the reference's own threshold (DISTANCE_SQ_THRESHOLD, 25 m^2 by default), beyond which
+//   the reference discards the match anyway, or when the whole circle has been read.
 // The 2nd / 3rd correspondence points of :312-361 / :402-455 use the same sweep restricted to the ring slice
-// rc-2..rc+2, with candidates ranked by the reference's visiting order (forward ascending first, then backward
-// descending, strict '<'), so ties resolve exactly as the sequential loops do.
+// rc-dn..rc+up (rc-2..rc+2 at the default NEARBY_SCAN 2.5), with candidates ranked by the reference's visiting order
+// (forward ascending first, then backward descending, strict '<'), so ties resolve exactly as the sequential loops do.
 // "Ring" is int(intensity) = ring + 0.1 relTime truncated.  scanRegistration.cpp emits relTime in (-2, 6] (DESIGN.md
 // section 3), so a cloud's int(intensity) is the physical ring or the one below and need not ascend: the invariant the search
 // relies on is only  int_i >= max_{j<i} int_j - 1.  Under it (and NEARBY_SCAN >= 1) the loops' break indices do not depend on
-// the closest point -- forward: the first index with int >= rc+3, backward: the last with int <= rc-3 -- every candidate has
-// int in rc-2..rc+2, and the class and visiting rank of a candidate follow from (index vs closest, int vs rc) alone.
+// the closest point.  With up = the largest u with rc + u <= rc + NEARBY_SCAN and dn = the largest u with rc - u >=
+// rc - NEARBY_SCAN (both in double, as the reference's int-vs-double tests; at most 64) the forward break is the first index
+// with int >= rc+up+1 and the backward break the last with int <= rc-dn-1, every candidate has int in rc-dn..rc+up, and the
+// class and visiting rank of a candidate follow from (index vs closest, int vs rc) alone.
 #include <climits>
 #include <cfloat>
 #include "common.cuh"
@@ -340,7 +342,11 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   float qx, qy, qz;
   const double s_ratio = ratio_of(cur.i, prm.distortion);
   transform_to_start(pose, s_ratio, cur.x, cur.y, cur.z, qx, qy, qz);
-  const float thr = (float)prm.dist_sq_thresh;
+  // The reference compares a float distance with the DOUBLE threshold (:305,310,393,399).  thr is the smallest float whose
+  // double value is >= it, so that d2 < thr holds for a float d2 exactly when (double)d2 < dist_sq_thresh: (float)25.3 rounds
+  // below 25.3 and would reject a d2 of that float, which the reference accepts.  NaN stays NaN (no match), above FLT_MAX inf.
+  float thr = (float)prm.dist_sq_thresh;
+  if ((double)thr < prm.dist_sq_thresh) thr = nextafterf(thr, INFINITY);
 
   // nearest neighbour (kdtree*Last->nearestKSearch(pointSel, 1, ...), :302,390) then `< DISTANCE_SQ_THRESHOLD`
   float d1;
@@ -349,11 +355,15 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   if (packed1 < 0 || !((double)d1 < prm.dist_sq_thresh)) { if (lane == 0) store_none(out, co); return; }
   const int closest = packed1 >> 6;
   const int rc = packed1 & 63;   // closestPointScanID = int(intensity) of the closest point (k_rab_fill packs it)
-  // rings rc-up .. rc+up survive the `> rc + NEARBY_SCAN` / `< rc - NEARBY_SCAN` break tests (:319,345,405,433)
-  int up = 0; while ((double)(rc + up + 1) <= (double)rc + prm.nearby_scan) ++up;
+  // rings rc-dn .. rc+up survive the break tests `int > rc + NEARBY_SCAN` / `int < rc - NEARBY_SCAN` (:319,345,405,433),
+  // evaluated in double as the reference does.  The two sides are counted separately: rc + N and rc - N need not round
+  // symmetrically (N = 3 - 2^-48 at rc = 32 keeps ring 35 but not ring 29).  64 rings cover 0..63 from any rc, so the
+  // bound makes a huge or infinite NEARBY_SCAN mean "never break", as in the reference.
+  int up = 0; while (up < 64 && (double)(rc + up + 1) <= (double)rc + prm.nearby_scan) ++up;
+  int dn = 0; while (dn < 64 && (double)(rc - dn - 1) >= (double)rc - prm.nearby_scan) ++dn;
   // the loops' ranges: forward (closest, fwd_end), backward [bwd_begin, closest).  Issued together with the closest point;
-  // aloam_create guarantees up >= 1, which puts both break indices on the right side of `closest`.
-  const int fwd_end = g.fwd_end[min(rc + up + 1, 64)], bwd_begin = g.bwd_begin[max(rc - up, 0)];
+  // aloam_create guarantees NEARBY_SCAN >= 1, hence up, dn >= 1, which puts both break indices on the right side of `closest`.
+  const int fwd_end = g.fwd_end[min(rc + up + 1, 64)], bwd_begin = g.bwd_begin[max(rc - dn, 0)];
   const Pt4 pc = L.pts[closest];   // issued now, consumed after the second search
 
   // second search: class 2 / class 3 minima in the reference's visiting order (forward ascending, then backward descending).
@@ -364,7 +374,7 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   {
     const int bq = bucket_of(qx, qy);
     const float rho = sqrtf(qx * qx + qy * qy);
-    const int r_lo = max(rc - up, 0), r_hi = min(rc + up, 63);
+    const int r_lo = max(rc - dn, 0), r_hi = min(rc + up, 63);
     auto f = [&](float x, float y, float z, int packed) {
       const int idx = packed >> 6, ring = packed & 63;
       if (idx == closest || idx >= fwd_end || idx < bwd_begin) return;

@@ -61,11 +61,14 @@ typedef struct aloam_config {
   float minimum_range;   /* minimum_range                   scanRegistration.cpp:468 */
   float line_res;        /* mapping_line_resolution         laserMapping.cpp:902-906 */
   float plane_res;       /* mapping_plane_resolution */
-  int outer_iters;       /* 2   laserOdometry.cpp:278, laserMapping.cpp:562 */
-  int inner_iters;       /* 4   options.max_num_iterations, laserOdometry.cpp:496 */
-  double huber;          /* 0.1 HuberLoss, laserOdometry.cpp:284 */
-  double dist_sq_thresh; /* 25  DISTANCE_SQ_THRESHOLD, laserOdometry.cpp:65 */
-  double nearby_scan;    /* 2.5 NEARBY_SCAN, laserOdometry.cpp:66 */
+  int outer_iters;       /* 2   laserOdometry.cpp:278, laserMapping.cpp:562; 1..4 */
+  int inner_iters;       /* 4   options.max_num_iterations, laserOdometry.cpp:496, laserMapping.cpp:715; >= 0 */
+  double huber;          /* 0.1 HuberLoss, laserOdometry.cpp:284, laserMapping.cpp:565; > 0.  huber, outer_iters and inner_iters
+                            apply to both solves, scan-to-scan and scan-to-map (the reference hard-codes the same values in both
+                            nodes); line_res and plane_res must be > 0 too */
+  double dist_sq_thresh; /* 25  DISTANCE_SQ_THRESHOLD, laserOdometry.cpp:65; compared as the reference does, a float squared
+                            distance against this double */
+  double nearby_scan;    /* 2.5 NEARBY_SCAN, laserOdometry.cpp:66; >= 1, may be +inf (the ring-window walks never break) */
   int device;            /* CUDA device ordinal */
   int max_points;        /* capacity of one raw scan (reference: 400000 static arrays, scanRegistration.cpp:66-69) */
   int max_map_points;    /* capacity of the uploaded submap, per cloud type (0 = mapping not used); at most 2^30, larger

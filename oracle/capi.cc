@@ -156,6 +156,10 @@ void orc_quat_plus(const double x[4], const double d[3], double out[4]) { quat_p
 void* orc_odom_create() { return new Odometry(); }
 void orc_odom_free(void* h) { delete (Odometry*)h; }
 void orc_odom_set_distortion(void* h, int on) { ((Odometry*)h)->distortion = on != 0; }
+// DISTANCE_SQ_THRESHOLD and NEARBY_SCAN of the association (laserOdometry.cpp:65-66)
+void orc_odom_set_params(void* h, double dist_sq_thresh, double nearby_scan) {
+  Odometry* o = (Odometry*)h; o->dist_sq_thresh = dist_sq_thresh; o->nearby_scan = nearby_scan;
+}
 void orc_transform_to_end(const float* in, int n, const double q[4], const double t[3], int distortion, float* out) {
   Cloud o; transform_to_end(to_cloud(in, n), q, t, distortion != 0, &o);
   for (int i = 0; i < n; ++i) { out[4 * i] = o[i].x; out[4 * i + 1] = o[i].y; out[4 * i + 2] = o[i].z; out[4 * i + 3] = o[i].intensity; }
@@ -232,9 +236,9 @@ void* orc_cubemap_create() { return new orc::CubeMap(); }
 void orc_cubemap_free(void* h) { delete (orc::CubeMap*)h; }
 // one mapping frame ; pose7 out ; info[0..5] = optimised, n valid cubes, corner_from_map, surf_from_map, corner_stack, surf_stack sizes
 int orc_cubemap_step(void* h, const float* corner, int nc, const float* surf, int ns, const double q_odom[4], const double t_odom[3],
-                     float line_res, float plane_res, int outer, int max_iters, int sort_mode, double pose7[7], int info[6]) {
+                     float line_res, float plane_res, int outer, int max_iters, double huber, int sort_mode, double pose7[7], int info[6]) {
   orc::CubeMap* m = (orc::CubeMap*)h;
-  orc::SolveOptions opt; opt.max_num_iterations = max_iters;
+  orc::SolveOptions opt; opt.max_num_iterations = max_iters; opt.huber_a = huber;
   orc::Cloud c(nc), s(ns);
   for (int i = 0; i < nc; ++i) c[i] = orc::PointXYZI{corner[4 * i], corner[4 * i + 1], corner[4 * i + 2], corner[4 * i + 3]};
   for (int i = 0; i < ns; ++i) s[i] = orc::PointXYZI{surf[4 * i], surf[4 * i + 1], surf[4 * i + 2], surf[4 * i + 3]};

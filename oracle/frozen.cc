@@ -56,10 +56,10 @@ int orc_frozen_get_cube(void* h, int which, int index, float* out, int cap) {
 // pose7 = parameters[7] afterwards; valid = the clipped window in loop order; info = {optimised, n valid, corner / surf points of
 // the window, corner / surf stack sizes}.  Returns 1 when the optimisation ran.
 int orc_frozen_step(void* h, const float* corner, int nc, const float* surf, int ns, const double q_odom[4], const double t_odom[3],
-                    double q_wmap_wodom[4], double t_wmap_wodom[3], float line_res, float plane_res, int outer, int max_iters, int sort_mode,
-                    double pose7[7], int valid[75], int info[6]) {
+                    double q_wmap_wodom[4], double t_wmap_wodom[3], float line_res, float plane_res, int outer, int max_iters, double huber,
+                    int sort_mode, double pose7[7], int valid[75], int info[6]) {
   const FrozenMap* m = (const FrozenMap*)h;
-  orc::SolveOptions opt; opt.max_num_iterations = max_iters;
+  orc::SolveOptions opt; opt.max_num_iterations = max_iters; opt.huber_a = huber;
   orc::Cloud c(nc), s(ns);
   for (int i = 0; i < nc; ++i) c[i] = orc::PointXYZI{corner[4 * i], corner[4 * i + 1], corner[4 * i + 2], corner[4 * i + 3]};
   for (int i = 0; i < ns; ++i) s[i] = orc::PointXYZI{surf[4 * i], surf[4 * i + 1], surf[4 * i + 2], surf[4 * i + 3]};

@@ -3,16 +3,13 @@
 //   :278-501  2 x { corner association (:299-384), plane association (:387-483), ceres::Solve (:494-499) }
 //   :504-505  pose integration            :554-568  swap "last" clouds, rebuild both kd-trees
 // All squared distances in the ring-window scans are float expressions (operands are float members; only the
-// result is widened to double, :322-327) and the break tests compare int ring ids with a double (+-2.5).
+// result is widened to double, :322-327) and the break tests compare int ring ids with a double (+-NEARBY_SCAN).
 #include <cmath>
 #include "oracle.h"
 
 namespace orc {
 
 namespace {
-const double DISTANCE_SQ_THRESHOLD = 25;  // laserOdometry.cpp:65
-const double NEARBY_SCAN = 2.5;           // :66
-
 const double SCAN_PERIOD = 0.1;           // :64
 
 // interpolation ratio (:113-118,376-379): float intensity minus its integer part (float arithmetic), divided by the double
@@ -51,6 +48,8 @@ void Odometry::set_last(const Cloud& c, const Cloud& s) {
 void Odometry::associate(const Cloud& sharp, const Cloud& flat, const double qv[4], const double tv[3],
                          std::vector<Correspondence>* ccorr, std::vector<Correspondence>* pcorr,
                          std::vector<ResidualBlock>* blocks) const {
+  const double DISTANCE_SQ_THRESHOLD = dist_sq_thresh;   // laserOdometry.cpp:65 (25 there)
+  const double NEARBY_SCAN = nearby_scan;                // :66 (2.5 there)
   const Quat q{qv[0], qv[1], qv[2], qv[3]};
   const Vec3 t{tv[0], tv[1], tv[2]};
   const int n_corner_last = (int)corner_last.size(), n_surf_last = (int)surf_last.size();

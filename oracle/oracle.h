@@ -124,6 +124,8 @@ class Odometry {
   // #define DISTORTION (laserOdometry.cpp:59): 0 in the reference build; 1 = per-point interpolation ratio
   // s = (intensity - int(intensity)) / SCAN_PERIOD in TransformToStart (:115-116) and in the residual blocks (:376-379,470-473)
   bool distortion = false;
+  // DISTANCE_SQ_THRESHOLD and NEARBY_SCAN (laserOdometry.cpp:65-66, constants there; aloam_config.dist_sq_thresh / nearby_scan)
+  double dist_sq_thresh = 25, nearby_scan = 2.5;
   Cloud corner_last, surf_last;
   KdTree tree_corner, tree_surf;
   OdomTimes times;

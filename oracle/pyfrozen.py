@@ -27,7 +27,7 @@ def lib():
         L.orc_frozen_set_cube.argtypes = [C.c_void_p, C.c_int, C.c_int, _f32p, C.c_int]
         L.orc_frozen_get_cube.argtypes = [C.c_void_p, C.c_int, C.c_int, _f32p, C.c_int]
         L.orc_frozen_step.argtypes = [C.c_void_p, _f32p, C.c_int, _f32p, C.c_int, _f64p, _f64p, _f64p, _f64p, C.c_float, C.c_float, C.c_int, C.c_int,
-                                      C.c_int, _f64p, _i32p, _i32p]
+                                      C.c_double, C.c_int, _f64p, _i32p, _i32p]
         L.orc_frozen_high_freq.argtypes = [_f64p] * 5
         L.orc_frozen_high_freq.restype = None
         _LIB = L
@@ -104,7 +104,8 @@ class Localiser:
         self.skip, self.scan = int(skip), 0
         self.valid, self.info = [], {}
 
-    def step(self, corner_last, surf_last, q_wodom_curr, t_wodom_curr, line_res=0.4, plane_res=0.8, outer=2, max_iters=4, sort_mode=1):
+    def step(self, corner_last, surf_last, q_wodom_curr, t_wodom_curr, line_res=0.4, plane_res=0.8, outer=2, max_iters=4, sort_mode=1,
+             huber=0.1):
         qo, to = np.ascontiguousarray(q_wodom_curr, np.float64), np.ascontiguousarray(t_wodom_curr, np.float64)
         pose = np.zeros(7)
         j, self.scan = self.scan, self.scan + 1
@@ -114,7 +115,7 @@ class Localiser:
         c, s = _cloud(corner_last), _cloud(surf_last)
         valid = np.zeros(75, np.int32); info = np.zeros(6, np.int32)
         lib().orc_frozen_step(self.map.h, c.ctypes.data_as(_f32p), c.shape[0], s.ctypes.data_as(_f32p), s.shape[0], _dp(qo), _dp(to), _dp(self.q),
-                              _dp(self.t), line_res, plane_res, outer, max_iters, sort_mode, _dp(pose), valid.ctypes.data_as(_i32p),
+                              _dp(self.t), line_res, plane_res, outer, max_iters, huber, sort_mode, _dp(pose), valid.ctypes.data_as(_i32p),
                               info.ctypes.data_as(_i32p))
         keys = ["optimised", "n_valid", "corner_from_map", "surf_from_map", "corner_stack", "surf_stack"]
         self.info = dict(zip(keys, (int(v) for v in info)))

@@ -82,7 +82,8 @@ def lib():
         L.orc_cubemap_create.restype = C.c_void_p
         L.orc_cubemap_free.argtypes = [C.c_void_p]
         L.orc_cubemap_step.argtypes = [C.c_void_p, _f32p, C.c_int, _f32p, C.c_int, _f64p, _f64p, C.c_float, C.c_float, C.c_int,
-                                       C.c_int, C.c_int, _f64p, _i32p]
+                                       C.c_int, C.c_double, C.c_int, _f64p, _i32p]
+        L.orc_odom_set_params.argtypes = [C.c_void_p, C.c_double, C.c_double]
         L.orc_cubemap_get.argtypes = [C.c_void_p, C.c_int, _f32p, C.c_int]
         L.orc_cubemap_state.argtypes = [C.c_void_p, _i32p, _i32p, _i32p, C.POINTER(C.c_longlong), _f64p, _f64p]
         L.orc_cubemap_cube.argtypes = [C.c_void_p, C.c_int, C.c_int, _f32p, C.c_int]
@@ -240,10 +241,11 @@ def quat_plus(q, d):
 
 
 class Odometry:
-    def __init__(self, distortion=False):
+    def __init__(self, distortion=False, dist_sq_thresh=25.0, nearby_scan=2.5):
         self.h = lib().orc_odom_create()
         if distortion:
             lib().orc_odom_set_distortion(self.h, 1)     # laserOdometry.cpp:59 #define DISTORTION 1
+        lib().orc_odom_set_params(self.h, float(dist_sq_thresh), float(nearby_scan))   # :65-66
 
     def set_last(self, corner, surf):
         corner, surf = _cloud(corner), _cloud(surf)
@@ -354,12 +356,12 @@ class CubeMap:
         self.h = lib().orc_cubemap_create()
 
     def step(self, corner_last, surf_last, q_wodom_curr, t_wodom_curr, line_res=0.4, plane_res=0.8, outer=2, max_iters=4,
-             sort_mode=SORT_CANONICAL):
+             sort_mode=SORT_CANONICAL, huber=0.1):
         c, s = _cloud(corner_last), _cloud(surf_last)
         pose = np.zeros(7)
         info = np.zeros(6, np.int32)
         lib().orc_cubemap_step(self.h, _fp(c), c.shape[0], _fp(s), s.shape[0], _dp(np.ascontiguousarray(q_wodom_curr, np.float64)),
-                               _dp(np.ascontiguousarray(t_wodom_curr, np.float64)), line_res, plane_res, outer, max_iters, sort_mode,
+                               _dp(np.ascontiguousarray(t_wodom_curr, np.float64)), line_res, plane_res, outer, max_iters, huber, sort_mode,
                                _dp(pose), info.ctypes.data_as(_i32p))
         keys = ["optimised", "n_valid", "corner_from_map", "surf_from_map", "corner_stack", "surf_stack"]
         return pose, dict(zip(keys, (int(v) for v in info)))
