@@ -72,7 +72,7 @@ int aloam_reset_odometry(aloam_ctx* c) {
   if (c->s_idx) CUDA_CHECK_RET(cudaStreamSynchronize(c->s_idx));   // an index build of the last synchronous call may still be running
   c->frame = 0; c->cur = 0; c->have_last = false;
   c->lanes_mode = false;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = c->lane_mapped[l] = c->lane_localising[l] = c->lane_armed[l] = false; c->lane_scan[l] = 0; }
+  for (Lane& L : c->lanes) L.sched = LaneSched();
   return ALOAM_OK;
 }
 
@@ -525,40 +525,49 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
   return scan_to_pose_impl(c, d_raw, n, 4, q_w, t_w, stats);
 }
 
-// The rows of a mapped stream call over the lane schedule `ops` (as scan_stream_run numbers scans, from the lanes' current
-// state, which it does not change): mapped[r] for the rows that go to the mapper; begin[r] = the sum of raws[r'].n over the mapped
-// rows r' < r, where row r's registered cloud starts in the sink.  Returns the sum over all mapped rows.
-static long long registered_layout(const aloam_ctx* c, const aloam_cloud_view* raws, const int* ops, int n_scans, int nb, std::vector<long long>* begin,
-                                   std::vector<char>* mapped) {
-  int scan[ALOAM_MAX_BATCH];
-  for (int l = 0; l < nb; ++l) scan[l] = c->lane_scan[l];
-  long long total = 0;
-  for (int k = 0; k < n_scans; ++k)
-    for (int l = 0; l < nb; ++l) {
-      const size_t r = (size_t)k * nb + l;
-      bool m = false;
-      if (ops[r] != ALOAM_LANE_IDLE) {
-        const int j = ops[r] == ALOAM_LANE_START ? 0 : scan[l];
-        scan[l] = j + 1;
-        m = j % c->cfg.mapping_skip_frame == 0;
-      }
-      if (begin) (*begin)[r] = total;
-      if (mapped) (*mapped)[r] = m;
-      if (m) total += raws[r].n;
+// Row k * nb + l of a stream call: scan k of lane l, as the call will run it
+struct StreamRow {
+  int op;               // ALOAM_LANE_*
+  int scan;             // index of the scan in its trajectory (-1: an IDLE row)
+  bool mapped;          // a mapped call's scan that goes to the mapper (or its lane's locator); the others get a high-frequency pose
+  bool localise;        // a mapped call's scan that registers against the prior map
+  long long reg_begin;  // where the row's registered cloud begins in the sink: the sum of raws[r'].n over the mapped rows r' before it
+};
+// the rows of a stream call, built before anything is issued (room for all n in one allocation); reg_total: the points of every
+// mapped row's registered cloud
+struct StreamTable { std::vector<StreamRow> rows; long long reg_total = 0; explicit StreamTable(size_t n) { rows.reserve(n); } };
+
+// Appends the next row to *t, `op` on the lane whose schedule state is *s (its raw scan v), and applies the op to *s: a START
+// begins a trajectory at scan 0 -- in a mapped call (map) a mapped one that consumes the lane's arming, so that it localises --,
+// a SCAN continues it, an IDLE ends it.  The one place a lane's scan index advances.
+static void add_row(const aloam_ctx* c, StreamTable* t, LaneSched* s, int op, const aloam_cloud_view& v, bool map) {
+  StreamRow r{op, -1, false, false, t->reg_total};
+  if (op == ALOAM_LANE_IDLE) {
+    s->running = false;
+  } else {
+    if (op == ALOAM_LANE_START) {
+      s->running = true; s->mapped = map; s->scan = 0;
+      s->localising = map && s->armed;
+      if (map) s->armed = false;
     }
-  return total;
+    r.scan = s->scan++;
+    r.mapped = map && r.scan % c->cfg.mapping_skip_frame == 0;   // laserOdometry.cpp:570
+    r.localise = map && s->localising;
+    if (r.mapped) t->reg_total += v.n;
+  }
+  t->rows.push_back(r);
 }
 
 // Pipelined form of aloam_scan_to_pose over `nb` lanes: ring binning of step k+1 (s_exa), per-ring extraction (s_ext), compaction
 // + index build (s_idx) run concurrently with association + LM of step k (main stream) and the host->device copies of step k+2
-// (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on a lane schedule
-// `ops` (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
+// (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on the rows t of its
+// lane schedule (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
 // (record i = lane act[i], which owns the buffers, pose slots and cube store); an all-idle step issues nothing.  reset_stores: a
-// START also resets its lane's cube store.  row_loc (or null: none): the rows that localise -- their lanes register against the
-// prior map in one locate frame per step, beside the mapping frame of the step's other lanes.  The caller has checked the views
-// and the schedule and created the cube stores and locators.
-static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int* ops, int n_scans, int nb, int device_resident, double* poses,
-                           double* map_poses, aloam_stats* stats_last, bool reset_stores, const char* row_loc = nullptr) {
+// START also resets its lane's cube store.  The rows that localise register against the prior map in one locate frame per step,
+// beside the mapping frame of the step's other lanes.  The caller has checked the views and the schedule, built its rows t and
+// created the cube stores and locators.
+static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const StreamTable& t, int n_scans, int nb, int device_resident, double* poses,
+                           double* map_poses, aloam_stats* stats_last, bool reset_stores) {
   StreamGuard guard(c);
   cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
@@ -577,16 +586,13 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
   // and moved into the world by k_register_full after the row's mapper frame; without a sink none of this is issued
   const bool sink = map_poses && c->reg_sink;
   const size_t rows = (size_t)n_scans * nb;
-  std::vector<char> row_mapped;
   if (map_poses) {
     c->reg_rows = -1;
-    c->reg_begin.assign(rows, 0); c->reg_count.assign(rows, 0); row_mapped.assign(rows, 0);
-    registered_layout(c, raws, ops, n_scans, nb, &c->reg_begin, &row_mapped);
-  }
-  if (map_poses) {   // the mappers' error bits of this call
-    for (int l = 0; l < nb; ++l) {   // (a lane that only localises has no cube store)
-      if (c->mapper[l]) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
-      if (c->locator[l]) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
+    c->reg_begin.resize(rows); c->reg_count.assign(rows, 0);
+    for (size_t r = 0; r < rows; ++r) c->reg_begin[r] = t.rows[r].reg_begin;
+    for (int l = 0; l < nb; ++l) {   // the mappers' error bits of this call (a lane that only localises has no cube store)
+      if (c->lanes[l].mapper) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
+      if (c->lanes[l].locator) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
     }
     const int rc = peer_err_reset(c); if (rc) return fail(rc);
   }
@@ -601,17 +607,13 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
   int last_op[ALOAM_MAX_BATCH] = {};        // the last non-idle op of every lane in this call (IDLE: none)
   int issued = 0;
   for (int k = 0; k < n_scans; ++k) {
-    const int* op = ops + (size_t)k * nb;
+    const StreamRow* row = t.rows.data() + (size_t)k * nb;   // the step's rows, one per lane
     // a lane's first scan, its START, only initialises (laserOdometry.cpp:267-271)
     int na = 0, n_scan = 0, n_start = 0;
-    bool map_scan[ALOAM_MAX_BATCH];         // per record: the scan goes to the mapper (mapped calls)
     for (int l = 0; l < nb; ++l) {
-      if (op[l] == ALOAM_LANE_IDLE) continue;
-      const int j = op[l] == ALOAM_LANE_START ? 0 : c->lane_scan[l];   // index of the scan in its trajectory
-      c->lane_scan[l] = j + 1;
-      map_scan[na] = j % c->cfg.mapping_skip_frame == 0;
-      act[na++] = l; last_op[l] = op[l];
-      if (op[l] == ALOAM_LANE_START) starting[n_start++] = l; else scanning[n_scan++] = l;
+      if (row[l].op == ALOAM_LANE_IDLE) continue;
+      act[na++] = l; last_op[l] = row[l].op;
+      if (row[l].op == ALOAM_LANE_START) starting[n_start++] = l; else scanning[n_scan++] = l;
     }
     if (na == 0) continue;                  // an all-idle step: nothing to run, the frame does not advance
     const int f = c->frame;                 // global frame number of this step
@@ -664,7 +666,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the last mapper frame that read this slot (of frame f - kFeatSlots at the latest) is done
     if (sink) {   // the ring-major cloud of every mapped row goes with the slot until its mapper frame has registered it
       for (int i = 0; i < na; ++i)
-        if (map_scan[i]) { Lane& L = c->lanes[act[i]]; STREAM_TRY(cudaMemcpyAsync(L.feat[cur].full, L.d_full[b], (size_t)ns[i] * sizeof(Pt4), cudaMemcpyDeviceToDevice, c->s_idx)); }
+        if (row[act[i]].mapped) { Lane& L = c->lanes[act[i]]; STREAM_TRY(cudaMemcpyAsync(L.feat[cur].full, L.d_full[b], (size_t)ns[i] * sizeof(Pt4), cudaMemcpyDeviceToDevice, c->s_idx)); }
       STREAM_TRY(cudaEventRecord(c->ev_stash[b], c->s_idx));
     }
     rc = run_features_b2(c, na, act, b, cur, false);
@@ -705,17 +707,16 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
         const int l = act[i];
         const FeatBuf& fc = c->lanes[l].feat[cur];
         const size_t slot = ((size_t)k * nb + l) * 7;
-        const bool localise = row_loc && row_loc[(size_t)k * nb + l];
         const MapperIn r{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
-                         reset_stores && op[l] == ALOAM_LANE_START, localise};
-        if (!map_scan[i]) hf[n_hf++] = r; else if (localise) loc[n_loc++] = r; else in[n_map++] = r;
+                         reset_stores && row[l].op == ALOAM_LANE_START, row[l].localise};
+        if (!row[l].mapped) hf[n_hf++] = r; else if (row[l].localise) loc[n_loc++] = r; else in[n_map++] = r;
       }
       // /velodyne_cloud_registered of a frame's rows, before the lanes' next frame replaces the refined pose
       auto register_rows = [&](const MapperIn* fr, int n) {
         const Pt4* src[ALOAM_MAX_BATCH]; const int* nf[ALOAM_MAX_BATCH]; Pt4* dst[ALOAM_MAX_BATCH];
         for (int j = 0; j < n; ++j) {
-          const size_t r = (size_t)k * nb + fr[j].lane;
-          src[j] = c->lanes[fr[j].lane].feat[cur].full; nf[j] = c->d_scan_nfull + r; dst[j] = c->reg_sink + c->reg_begin[r];
+          const int l = fr[j].lane;
+          src[j] = c->lanes[l].feat[cur].full; nf[j] = c->d_scan_nfull + (size_t)k * nb + l; dst[j] = c->reg_sink + row[l].reg_begin;
         }
         return mapper_register_full_device(c, n, fr, src, nf, dst, nmax);
       };
@@ -750,8 +751,8 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) {
       c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
-      if (c->mapper[l]) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
-      if (c->locator[l]) STREAM_TRY(cudaMemcpyAsync(&c->pin->locate_err_lane[l], locator_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+      if (c->lanes[l].mapper) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+      if (c->lanes[l].locator) STREAM_TRY(cudaMemcpyAsync(&c->pin->locate_err_lane[l], locator_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
     }
     const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return fail(rc);
   }
@@ -771,11 +772,11 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     for (int b = 0; b < 3; ++b)
       if (c->h_sc[3 * l + b].error) return fail(c->h_sc[3 * l + b].error);
   for (size_t i = 0; i < total; ++i)   // (an idle entry has no scan)
-    if (ops[i] != ALOAM_LANE_IDLE && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
+    if (t.rows[i].op != ALOAM_LANE_IDLE && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
   std::memcpy(poses, c->h_poses, total * 56);
   if (map_poses) std::memcpy(map_poses, c->h_poses + (size_t)kMaxStreamScans * 7, total * 56);
   for (size_t i = 0; i < total; ++i)
-    if (ops[i] == ALOAM_LANE_IDLE)
+    if (t.rows[i].op == ALOAM_LANE_IDLE)
       for (int j = 0; j < 7; ++j) { poses[i * 7 + j] = NAN; if (map_poses) map_poses[i * 7 + j] = NAN; }
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (stats_last) {
@@ -786,7 +787,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const int
     }
   }
   if (map_poses) {   // the registered rows of this call (count 0 without a sink)
-    for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && row_mapped[r] ? c->h_scan_nfull[r] : 0;
+    for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
     c->reg_rows = (int)rows;
   }
   // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
@@ -815,11 +816,16 @@ static int scan_stream_lockstep(aloam_ctx* c, const aloam_cloud_view* raws, int 
     if (device_resident && raws[k].stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
     if (raws[k].stride_floats != raws[k - k % nb].stride_floats) return ALOAM_ERR_INVALID_ARG;   // one stride per step
   }
-  for (int i = 0; i < n_scans * nb; ++i) c->lockstep_ops[i] =c->frame == 0 && i < nb ? ALOAM_LANE_START : ALOAM_LANE_SCAN;
-  if (map_poses && c->reg_sink && registered_layout(c, raws, c->lockstep_ops, n_scans, nb, nullptr, nullptr) > c->reg_cap) return ALOAM_ERR_CAPACITY;
+  // the rows from the lanes' scan indices alone: a lockstep call neither localises nor changes a lane's mode or arming
+  StreamTable t((size_t)n_scans * nb);
+  LaneSched s[ALOAM_MAX_BATCH];
+  for (int l = 0; l < nb; ++l) s[l].scan = c->lanes[l].sched.scan;
+  for (int i = 0; i < n_scans * nb; ++i) add_row(c, &t, &s[i % nb], c->frame == 0 && i < nb ? ALOAM_LANE_START : ALOAM_LANE_SCAN, raws[i], map_poses);
+  if (map_poses && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (map_poses) { int rc = mapper_ensure_lanes(c, nb); if (rc) return rc; }   // creates the cube stores this call needs
-  return scan_stream_run(c, raws, c->lockstep_ops, n_scans, nb, device_resident, poses, map_poses, stats_last, false);
+  for (int l = 0; map_poses && l < nb; ++l) { int rc = mapper_ensure(c, l); if (rc) return rc; }   // creates the cube stores this call needs
+  for (int l = 0; l < nb; ++l) c->lanes[l].sched.scan = s[l].scan;
+  return scan_stream_run(c, raws, t, n_scans, nb, device_resident, poses, map_poses, stats_last, false);
 }
 
 int aloam_scan_stream(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int device_resident, double* poses, aloam_stats* stats_last) {
@@ -849,53 +855,47 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   if (!lane_ops) return ALOAM_ERR_INVALID_ARG;
   if (c && sharded_job(c)) return ALOAM_ERR_STATE;   // a sharded job maps one trajectory (aloam_scan_stream_mapped)
   if (!stream_args_ok(c, raws, n_scans, batch, odom_poses, map_poses)) return ALOAM_ERR_INVALID_ARG;
-  // the whole schedule is checked against the lanes' state before anything changes; lanes >= batch are idle all call
-  bool running[ALOAM_MAX_BATCH], mapped[ALOAM_MAX_BATCH], localising[ALOAM_MAX_BATCH], armed[ALOAM_MAX_BATCH];   // lane state after this call
+  // the whole schedule is checked on a copy of the lanes' schedule state before anything changes; lanes >= batch are idle all call
+  const bool map = map_poses != nullptr;
+  LaneSched s[ALOAM_MAX_BATCH];
+  for (int l = 0; l < c->n_lanes; ++l) { s[l] = c->lanes[l].sched; s[l].running = s[l].running && l < batch; }
   bool maps[ALOAM_MAX_BATCH] = {}, localises[ALOAM_MAX_BATCH] = {};   // the lane has a mapping / a localising scan in this call
-  std::vector<char> row_loc((size_t)n_scans * batch, 0);              // the rows that localise
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) {
-    running[l] = l < batch && c->lane_running[l]; mapped[l] = c->lane_mapped[l]; localising[l] = c->lane_localising[l]; armed[l] = c->lane_armed[l];
-  }
   for (size_t i = 0; i < (size_t)n_scans * batch; ++i)
     if (lane_ops[i] < ALOAM_LANE_IDLE || lane_ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
+  StreamTable t((size_t)n_scans * batch);
   int run_err = ALOAM_OK;   // a scan that cannot run fails the call like a run-time error
   for (int k = 0; k < n_scans; ++k) {
     int stride = 0;
     for (int l = 0; l < batch; ++l) {
       const int op = lane_ops[(size_t)k * batch + l];
       const aloam_cloud_view& v = raws[(size_t)k * batch + l];
-      if (op == ALOAM_LANE_IDLE) { running[l] = false; continue; }   // its view is not read
-      int rc = check_view(v); if (rc) return rc;
-      if (v.n > 0) {
-        if (device_resident && v.stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
-        if (stride && v.stride_floats != stride) return ALOAM_ERR_INVALID_ARG;   // one stride per step
-        stride = v.stride_floats;
+      if (op != ALOAM_LANE_IDLE) {   // an idle row's view is not read
+        int rc = check_view(v); if (rc) return rc;
+        if (v.n > 0) {
+          if (device_resident && v.stride_floats != 4) return ALOAM_ERR_INVALID_ARG;
+          if (stride && v.stride_floats != stride) return ALOAM_ERR_INVALID_ARG;   // one stride per step
+          stride = v.stride_floats;
+        }
+        // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
+        if (op == ALOAM_LANE_SCAN && (!s[l].running || s[l].mapped != map)) return ALOAM_ERR_STATE;
+        if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
+        if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
       }
-      // a SCAN continues the trajectory its lane runs, in the mode (mapped or not) it was started in
-      if (op == ALOAM_LANE_SCAN && (!running[l] || mapped[l] != (map_poses != nullptr))) return ALOAM_ERR_STATE;
-      if (op == ALOAM_LANE_START) {   // a mapped START consumes the lane's arming (aloam_lane_localise): the trajectory localises
-        running[l] = true; mapped[l] = map_poses != nullptr;
-        localising[l] = mapped[l] && armed[l];
-        if (mapped[l]) armed[l] = false;
-      }
-      if (map_poses) { row_loc[(size_t)k * batch + l] = localising[l]; (localising[l] ? localises : maps)[l] = true; }
-      if (!run_err && v.n == 0) run_err = ALOAM_ERR_EMPTY_CLOUD;
-      if (!run_err && v.n > c->max_points) run_err = ALOAM_ERR_CAPACITY;
+      add_row(c, &t, &s[l], op, v, map);
+      if (map && op != ALOAM_LANE_IDLE) (t.rows.back().localise ? localises : maps)[l] = true;
     }
   }
-  if (map_poses && c->reg_sink && registered_layout(c, raws, lane_ops, n_scans, batch, nullptr, nullptr) > c->reg_cap) return ALOAM_ERR_CAPACITY;
+  if (map && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (run_err) { aloam_reset_odometry(c); return run_err; }
-  if (map_poses) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
-    for (int l = 0; l < batch; ++l) {
-      int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
-      rc = maps[l] || !localises[l] ? mapper_ensure_lane(c, l) : ALOAM_OK; if (rc) return rc;
-    }
+  for (int l = 0; map && l < batch; ++l) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
+    int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
+    rc = maps[l] || !localises[l] ? mapper_ensure(c, l) : ALOAM_OK; if (rc) return rc;
   }
   // committed before anything is issued: a later failure ends in aloam_reset_odometry, a key overflow leaves the lanes running
   c->lanes_mode = true;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) { c->lane_running[l] = running[l]; c->lane_mapped[l] = mapped[l]; c->lane_localising[l] = localising[l]; c->lane_armed[l] = armed[l]; }
-  return scan_stream_run(c, raws, lane_ops, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true, row_loc.data());
+  for (int l = 0; l < c->n_lanes; ++l) c->lanes[l].sched = s[l];
+  return scan_stream_run(c, raws, t, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
 }
 
 int aloam_set_registered_sink(aloam_ctx* c, float* data, long long capacity) {

@@ -52,6 +52,9 @@ struct PriorSearch {
   const int* ctr[ALOAM_MAX_BATCH];
 };
 struct ExportLayout;   // cubemap.cu: where the segments of a store export are in the export and in the store
+struct Mapper;         // cubemap.cu: a lane's cube store
+struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
+struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexed
 }  // namespace aloam
 
 using namespace aloam;
@@ -74,9 +77,28 @@ struct FeatBuf {
   Pt4* full = nullptr;             // ring-major cloud of a mapped scan, kept for its registered cloud (created by aloam_set_registered_sink)
 };
 
-// Everything one trajectory owns on the device.  A context has cfg.max_batch of them; the single-trajectory entry points
-// use lane 0, aloam_scan_stream_batch drives lanes 0 .. batch-1 in lockstep with shared launches.
+// Where a lane is in the schedule of the stream calls.  A lane of aloam_scan_stream_lanes runs from its START to the step before
+// its next IDLE; `mapped` is the mode of the call that started it; `localising`: the trajectory it runs (or ran last) registers
+// against the prior map, fixed at its START; `armed`: aloam_lane_localise has armed its next mapped START with Lane::init.
+// `scan`: index of its next scan in its trajectory (0 at a START), which every stream call advances; scan j goes to the mapper
+// when j % cfg.mapping_skip_frame == 0.  aloam_reset_odometry puts back the default.
+struct LaneSched {
+  bool running = false, mapped = false, localising = false, armed = false;
+  int scan = 0;
+};
+
+// Everything one trajectory owns.  A context has cfg.max_batch of them; the single-trajectory entry points use lane 0,
+// aloam_scan_stream_batch drives lanes 0 .. batch-1 in lockstep with shared launches.
 struct Lane {
+  LaneSched sched;
+  // its cube store and its locator (cubemap.cu), each created on first use: lane 0's store serves the host API and both mapped
+  // stream calls; a lane that only localises has no store
+  Mapper* mapper = nullptr;
+  Locator* locator = nullptr;
+  double init[7] = {};   // the T_wmap_wodom an armed START localises from (aloam_lane_localise)
+  // the locator holds the window of a localising frame against the current prior map (aloam_debug_prior_associate); set by the
+  // frame, cleared when the prior map is released
+  bool window = false;
   float* d_raw[2] = {nullptr, nullptr};          // raw-scan staging, double-buffered by scan parity
   int8_t* d_ring = nullptr;
   int *d_hist = nullptr, *d_offsets = nullptr, *d_scan_start = nullptr, *d_scan_end = nullptr;
@@ -150,9 +172,6 @@ struct aloam_ctx {
   void* peer = nullptr;          // peer-memory exchange of the sharded LM (comm.cu), when enabled
   double* d_lm_tot = nullptr;    // [64] all-reduced normal equations of one evaluation (per-evaluation sharded LM)
   void* d_lm_state = nullptr;    // device-resident trust-region state (per-evaluation sharded LM)
-  // map cube store of every lane (cubemap.cu), each created on first use: lane 0 serves the host API and both mapped stream
-  // calls, lanes 1 .. max_batch-1 only aloam_scan_stream_mapped_batch
-  void* mapper[ALOAM_MAX_BATCH] = {};
   // scan-to-map: the registration set of the host API and mapper lane 0 (uploaded submap with its hash grids, stacks, ...)
   MapReg map = {};
   Pt4* d_map_pts[2] = {nullptr, nullptr};   // staging for maps handed in as host views (device views are indexed in place)
@@ -212,32 +231,16 @@ struct aloam_ctx {
   int cur = 0;            // fused pipeline: feat[] slot of the most recent scan
   bool have_last = false; // API path: set_last called
   int last_n_full = 0;
-  // aloam_scan_stream_lanes: once used, the lockstep calls are refused until aloam_reset_odometry, which clears all of this.
-  // A lane runs from its START to the step before its next IDLE; `lane_mapped` is the mode of the call that started it.
+  // aloam_scan_stream_lanes: once used, the lockstep calls are refused until aloam_reset_odometry, which clears it and every
+  // lane's schedule state
   bool lanes_mode = false;
-  bool lane_running[ALOAM_MAX_BATCH] = {};
-  bool lane_mapped[ALOAM_MAX_BATCH] = {};
-  // mapped streams: index of every lane's next scan in its trajectory (0 at a START); scan j goes to the mapper when
-  // j % cfg.mapping_skip_frame == 0.  Carries over between calls; aloam_reset_odometry clears it.
-  int lane_scan[ALOAM_MAX_BATCH] = {};
   // the stack filters of mapping and localising frames run on s_stack, forked from and joined to the frame's stream by these
   // events (cubemap.cu; created with the first cube store or locator)
   cudaStream_t s_stack = nullptr;
   cudaEvent_t ev_stack_fork = nullptr, ev_stack_join = nullptr;
-  // localisation (cubemap.cu): the context's prior map, released by prior_map_release; the frame state and registration
-  // buffers of every lane that has localised (created at its first localising START).  lane_localising: the trajectory the lane
-  // runs (or ran last) registers against the prior map, fixed at its START.  lane_armed / lane_init: aloam_lane_localise has
-  // armed the lane's next mapped START with this T_wmap_wodom.
-  void* prior = nullptr;
+  // localisation (cubemap.cu): the context's prior map, released by prior_map_release
+  PriorMap* prior = nullptr;
   bool prior_owned = false;       // prior_map_release is on the release list
-  void* locator[ALOAM_MAX_BATCH] = {};
-  bool lane_localising[ALOAM_MAX_BATCH] = {};
-  bool lane_armed[ALOAM_MAX_BATCH] = {};
-  double lane_init[ALOAM_MAX_BATCH][7] = {};
-  // the lane's locator holds the window of a localising frame against the current prior map (aloam_debug_prior_associate);
-  // set by the frame, cleared when the prior map is released
-  bool lane_window[ALOAM_MAX_BATCH] = {};
-  int lockstep_ops[kMaxStreamScans] = {};   // the lane schedule a lockstep stream call hands to the stream driver
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
   std::vector<cudaStream_t> streams;
@@ -311,11 +314,11 @@ int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);
-int mapper_ensure_lanes(aloam_ctx* c, int nb);
-int mapper_ensure_lane(aloam_ctx* c, int lane);
+// the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
+int mapper_ensure(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);
 // localisation against the prior map (cubemap.cu): a lane's locator, created on first use; one frame of nb localising lanes on
-// the current stream (in[l].fresh: the lane starts its trajectory with this frame, from c->lane_init); its per-call error word
+// the current stream (in[l].fresh: the lane starts its trajectory with this frame, from its Lane::init); its per-call error word
 int locator_ensure(aloam_ctx* c, int lane);
 int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int* locator_err_acc(aloam_ctx* c, int lane);
@@ -323,7 +326,7 @@ int* locator_err_acc(aloam_ctx* c, int lane);
 // in the lane's locator.  ALOAM_ERR_STATE without a prior map or when the lane has run no localising frame against it.
 int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps);
 inline bool any_lane_localising(const aloam_ctx* c) {
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) if (c->lane_running[l] && c->lane_localising[l]) return true;
+  for (const Lane& L : c->lanes) if (L.sched.running && L.sched.localising) return true;
   return false;
 }
 // snapshot.cu: the kind of a caller's snapshot buffer (1 device memory of the context's device, 0 host memory, -1 unusable), and

@@ -77,7 +77,9 @@ struct MapperState {
   int free_list[2][kPool];
 };
 
-struct Mapper {
+}  // namespace
+
+struct aloam::Mapper {
   int cap[2] = {0, 0};
   Pt4* d_pts[2] = {nullptr, nullptr};       // [kPool * cap] slabs
   Pt4* d_sub[2] = {nullptr, nullptr};       // gathered submap
@@ -94,6 +96,31 @@ struct Mapper {
   int max_sub = 0;
   MapReg* reg = nullptr;                    // registration set: lane 0 shares the context's with the host API, the others own one
 };
+
+// The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
+// exclusive prefix of the snapshot's counts) and a hash grid over ALL of them, built once by prior_index; the centre offsets of
+// the store, which never change (no localising frame shifts the ring buffer); the layout of its ALOAM_EXPORT_MAP export.  Plain
+// cudaMalloc, freed by prior_map_release.
+struct aloam::PriorMap {
+  Pt4* pts[2] = {nullptr, nullptr};
+  int n[2] = {0, 0};
+  int cen[3] = {0, 0, 0};
+  int* d_cube_start = nullptr;   // [2][NCUBE + 1]
+  int* d_n = nullptr;            // [2]
+  GridTable grid[2] = {};
+  ExportLayout* d_layout = nullptr;
+};
+// what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
+// k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
+// holds the window tables), a registration set without grid tables, and a segmented filter sized for the two scan stacks
+struct aloam::Locator {
+  MapperState* d_state = nullptr;
+  MapperState* h_state = nullptr;
+  MapReg reg = {};
+  SegBuffers buf;
+};
+
+namespace {
 
 // what every kernel of a frame needs of one lane: the frame runs over all lanes at once, each launch taking one record per lane
 // (lane = blockIdx.z)
@@ -731,42 +758,6 @@ int stack_filters_fork(aloam_ctx* c, int nb, const Batch<MapperLane>& B, const S
   return ALOAM_OK;
 }
 
-int ensure_mapper(aloam_ctx* c, int lane) {
-  if (c->mapper[lane]) return ALOAM_OK;
-  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
-  Mapper* m = new (std::nothrow) Mapper();
-  if (!m) return ALOAM_ERR_CUDA;
-  own(c, [m] { delete m; });
-  mapper_slab_caps(c, m->cap);
-  m->max_sub = c->cfg.max_map_points;
-  bool ok = true;
-  for (int t = 0; t < 2 && ok; ++t) {
-    ok = ok && dalloc(c, &m->d_pts[t], (size_t)kPool * m->cap[t]) == cudaSuccess;
-    ok = ok && dalloc(c, &m->d_sub[t], (size_t)m->max_sub) == cudaSuccess;
-    ok = ok && dalloc(c, &m->d_in[t], (size_t)c->max_points) == cudaSuccess;
-  }
-  ok = ok && dalloc(c, &m->d_world, (size_t)2 * c->max_points) == cudaSuccess;   // both stacks side by side
-  ok = ok && dalloc(c, &m->d_cube, (size_t)2 * c->max_points) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
-  ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
-  ok = ok && stack_stream_ensure(c) == cudaSuccess;
-  ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
-  // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
-  // created here, after the context's (which fixes the table size)
-  m->reg = lane == 0 ? &c->map : new (std::nothrow) MapReg();
-  if (lane > 0 && m->reg) own(c, [r = m->reg] { delete r; });
-  ok = ok && m->reg && (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK && map_reg_alloc(c, m->reg) == ALOAM_OK));
-  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
-    cudaGetLastError();
-    return ALOAM_ERR_CUDA;
-  }
-  const int rc = reset_lane(c, m);   // a lane is published with the state of a fresh trajectory, never uninitialised
-  if (rc) return rc;
-  c->mapper[lane] = m;
-  return ALOAM_OK;
-}
-
 // the layout of export `what` of the store of m into c->d_export_layout (created on first use); *n = the size of the export.
 // Synchronises.
 int export_sizes(aloam_ctx* c, const Mapper* m, int what, long long* n) {
@@ -803,29 +794,6 @@ int store_copy(aloam_ctx* c, const ExportLayout* L, long long n, char* mem, bool
 
 // ---- localisation: the prior map of a context and the lanes that register against it
 
-// The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
-// exclusive prefix of the snapshot's counts) and a hash grid over ALL of them, built once by prior_index; the centre offsets of
-// the store, which never change (no localising frame shifts the ring buffer); the layout of its ALOAM_EXPORT_MAP export.  Plain
-// cudaMalloc, freed by prior_map_release.
-struct PriorMap {
-  Pt4* pts[2] = {nullptr, nullptr};
-  int n[2] = {0, 0};
-  int cen[3] = {0, 0, 0};
-  int* d_cube_start = nullptr;   // [2][NCUBE + 1]
-  int* d_n = nullptr;            // [2]
-  GridTable grid[2] = {};
-  ExportLayout* d_layout = nullptr;
-};
-// what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
-// k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
-// holds the window tables), a registration set without grid tables, and a segmented filter sized for the two scan stacks
-struct Locator {
-  MapperState* d_state = nullptr;
-  MapperState* h_state = nullptr;
-  MapReg reg = {};
-  SegBuffers buf;
-};
-
 void prior_free(PriorMap* p) {
   if (!p) return;
   for (int t = 0; t < 2; ++t) { cudaFree(p->pts[t]); cudaFree(p->grid[t].slots); cudaFree(p->grid[t].dyn); cudaFree(p->grid[t].gpts); }
@@ -834,14 +802,15 @@ void prior_free(PriorMap* p) {
 }
 // the one place a context's prior map is released: aloam_prior_map_clear, a load that replaces it, aloam_destroy
 void prior_map_release(aloam_ctx* c) {
-  prior_free(static_cast<PriorMap*>(c->prior));
+  prior_free(c->prior);
   c->prior = nullptr;
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_window[l] = false;   // the windows were cut from this map
+  for (Lane& L : c->lanes) L.window = false;   // the windows were cut from this map
 }
 
 // the frame state of the lane a record runs on: its locator's when it localises, else its cube store's
 MapperState* lane_state(const aloam_ctx* c, const MapperIn& in) {
-  return in.localise ? static_cast<Locator*>(c->locator[in.lane])->d_state : static_cast<Mapper*>(c->mapper[in.lane])->d_state;
+  const Lane& L = c->lanes[in.lane];
+  return in.localise ? L.locator->d_state : L.mapper->d_state;
 }
 
 // the persistent index: the k_grid_* chain of mapping.cu once over both packed clouds, then the cube tags
@@ -873,7 +842,7 @@ void mapper_slab_caps(const aloam_ctx* c, int cap[2]) {
 // the table of lane `lane`'s store into *head (host memory): the fields that outlive a frame and every cube's point count, -1 for a
 // cube without a slab; head->n_points = the size of the ALOAM_EXPORT_MAP export.  The store exists.  Synchronises.
 int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head) {
-  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  Mapper* m = c->lanes[lane].mapper;
   CUDA_CHECK_RET(cudaMemcpyAsync(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   const MapperState* S = m->h_state;
@@ -898,7 +867,7 @@ int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head) {
 // the n points of lane `lane`'s store in ALOAM_EXPORT_MAP order into dst (device memory when `device`, else host memory), on
 // c->stream, not synchronised; n is what mapper_store_tables reported (ALOAM_ERR_STATE when the store disagrees)
 int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device) {
-  const Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  const Mapper* m = c->lanes[lane].mapper;
   long long total = 0;
   int rc = export_sizes(c, m, ALOAM_EXPORT_MAP, &total); if (rc) return rc;
   if (total != n) return ALOAM_ERR_STATE;
@@ -909,7 +878,7 @@ int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool dev
 // device, k_store_import_tables rebuilds the tables and lays the store out, store_copy moves the head->n_points points of pts into
 // the slabs.  Synchronises.
 int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device) {
-  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  Mapper* m = c->lanes[lane].mapper;
   if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
   if (!c->d_snap_store) CUDA_CHECK_RET(dalloc(c, &c->d_snap_store, 1));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_snap_store, head, sizeof(SnapStore), cudaMemcpyHostToDevice, c->stream));
@@ -929,10 +898,10 @@ int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const ch
 // with the context's set, shared with the host API.  A sharded job maps one lane.
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH || (nb > 1 && sharded_job(c))) return ALOAM_ERR_STATE;
-  int rc = ensure_mapper(c, 0); if (rc) return rc;   // lane 0's store gives the sizes every lane shares
-  for (int l = 0; l < nb; ++l) { rc = ensure_mapper(c, in[l].lane); if (rc) return rc; }
+  int rc = mapper_ensure(c, 0); if (rc) return rc;   // lane 0's store gives the sizes every lane shares
+  for (int l = 0; l < nb; ++l) { rc = mapper_ensure(c, in[l].lane); if (rc) return rc; }
   rc = ensure_map_buffers(c); if (rc) return rc;     // lane 0's set
-  Mapper* m0 = static_cast<Mapper*>(c->mapper[0]);
+  const Mapper* m0 = c->lanes[0].mapper;
   Batch<MapperLane> B = {};
   MapLaneIO io[ALOAM_MAX_BATCH];
   SegFilter stack_f[ALOAM_MAX_BATCH], cube_f[ALOAM_MAX_BATCH];
@@ -944,8 +913,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   { const double side = std::floor(50.0 / std::min(c->cfg.line_res, c->cfg.plane_res)) + 3.0; const double cells = side * side * side;
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
   for (int l = 0; l < nb; ++l) {   // record l runs on the store of lane in[l].lane
-    const int lane = in[l].lane;
-    Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+    Mapper* m = c->lanes[in[l].lane].mapper;
     MapperState* S = m->d_state;
     const MapReg& reg = *m->reg;
     B.a[l] = MapperLane{S, in[l].odom7, in[l].out7, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, {m->d_sub[0], m->d_sub[1]}, {in[l].corner, in[l].surf},
@@ -1022,21 +990,48 @@ int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const 
 }
 
 // the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
-int* mapper_err_acc(aloam_ctx* c, int lane) { return &static_cast<Mapper*>(c->mapper[lane])->d_state->err_acc; }
+int* mapper_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].mapper->d_state->err_acc; }
 
-// the cube stores of lanes 0 .. nb-1, each created on first use with the state of a fresh trajectory.  A failure leaves the
-// lanes that existed untouched.
-int mapper_ensure_lanes(aloam_ctx* c, int nb) {
-  for (int l = 0; l < nb; ++l) { int rc = ensure_mapper(c, l); if (rc) return rc; }
+int mapper_ensure(aloam_ctx* c, int lane) {
+  if (c->lanes[lane].mapper) return ALOAM_OK;
+  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
+  Mapper* m = new (std::nothrow) Mapper();
+  if (!m) return ALOAM_ERR_CUDA;
+  own(c, [m] { delete m; });
+  mapper_slab_caps(c, m->cap);
+  m->max_sub = c->cfg.max_map_points;
+  bool ok = true;
+  for (int t = 0; t < 2 && ok; ++t) {
+    ok = ok && dalloc(c, &m->d_pts[t], (size_t)kPool * m->cap[t]) == cudaSuccess;
+    ok = ok && dalloc(c, &m->d_sub[t], (size_t)m->max_sub) == cudaSuccess;
+    ok = ok && dalloc(c, &m->d_in[t], (size_t)c->max_points) == cudaSuccess;
+  }
+  ok = ok && dalloc(c, &m->d_world, (size_t)2 * c->max_points) == cudaSuccess;   // both stacks side by side
+  ok = ok && dalloc(c, &m->d_cube, (size_t)2 * c->max_points) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
+  ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
+  ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
+  ok = ok && stack_stream_ensure(c) == cudaSuccess;
+  ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
+  // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
+  // created here, after the context's (which fixes the table size)
+  m->reg = lane == 0 ? &c->map : new (std::nothrow) MapReg();
+  if (lane > 0 && m->reg) own(c, [r = m->reg] { delete r; });
+  ok = ok && m->reg && (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK && map_reg_alloc(c, m->reg) == ALOAM_OK));
+  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
+    cudaGetLastError();
+    return ALOAM_ERR_CUDA;
+  }
+  const int rc = reset_lane(c, m);   // a lane is published with the state of a fresh trajectory, never uninitialised
+  if (rc) return rc;
+  c->lanes[lane].mapper = m;
   return ALOAM_OK;
 }
-
-int mapper_ensure_lane(aloam_ctx* c, int lane) { return ensure_mapper(c, lane); }
 
 // lane `lane`'s locator, created on first use and published only when fully allocated (what was acquired before a failure
 // belongs to the context until aloam_destroy)
 int locator_ensure(aloam_ctx* c, int lane) {
-  if (c->locator[lane]) return ALOAM_OK;
+  if (c->lanes[lane].locator) return ALOAM_OK;
   if (stack_stream_ensure(c) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
   Locator* m = new (std::nothrow) Locator();
   if (!m) return ALOAM_ERR_CUDA;
@@ -1045,18 +1040,18 @@ int locator_ensure(aloam_ctx* c, int lane) {
   ok = ok && map_reg_alloc(c, &m->reg, false) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
   ok = ok && cudaMemset(m->d_state, 0, sizeof(MapperState)) == cudaSuccess;
   if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
-  c->locator[lane] = m;
+  c->lanes[lane].locator = m;
   return ALOAM_OK;
 }
 
-int* locator_err_acc(aloam_ctx* c, int lane) { return &static_cast<Locator*>(c->locator[lane])->d_state->err_acc; }
+int* locator_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].locator->d_state->err_acc; }
 
 // One localising frame of nb lanes on the current stream: laserMapping.cpp:309-734 without the ring-buffer shift, against the
 // context's prior map, which it only reads.  Record l as in mapper_step_device; its lane's locator exists.  Every launch covers
 // all lanes: the stack filters (forked, as the mapping frame's), k_locate_begin, the thin-map test, outer_iters x (k_map_knn5_prior,
 // k_map_fit, LM), k_mapper_update, k_mapper_finish (the stack filter's error bit).
 int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
-  PriorMap* P = static_cast<PriorMap*>(c->prior);
+  const PriorMap* P = c->prior;
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || sharded_job(c)) return ALOAM_ERR_STATE;
   Batch<MapperLane> B = {};
   Batch<LocateLane> L = {};
@@ -1066,14 +1061,15 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   PriorSearch ps = {};
   ps.grid = PriorGrid{P->grid[0], P->grid[1]};
   for (int l = 0; l < nb; ++l) {
-    Locator* m = static_cast<Locator*>(c->locator[in[l].lane]);
+    const Lane& lane = c->lanes[in[l].lane];
+    Locator* m = lane.locator;
     MapperState* S = m->d_state;
     B.a[l].S = S; B.a[l].odom7 = in[l].odom7; B.a[l].out7 = in[l].out7;
     B.a[l].in[0] = in[l].corner; B.a[l].in[1] = in[l].surf; B.a[l].n_in[0] = in[l].nc; B.a[l].n_in[1] = in[l].ns;
     B.a[l].stack[0] = m->reg.stack[0]; B.a[l].stack[1] = m->reg.stack[1];
     B.a[l].segs = m->buf.segs; B.a[l].n_seg = m->buf.n_seg;
     L.a[l].S = S; L.a[l].odom7 = in[l].odom7; L.a[l].fresh = in[l].fresh;
-    for (int k = 0; k < 7; ++k) L.a[l].init[k] = c->lane_init[in[l].lane][k];
+    for (int k = 0; k < 7; ++k) L.a[l].init[k] = lane.init[k];
     io[l] = MapLaneIO{m->reg, {nullptr, nullptr}, S->stack_counts, S->x};
     ps.win[l][0] = S->sub_off[0]; ps.win[l][1] = S->sub_off[1]; ps.ctr[l] = S->ctr;
     stack_f[l] = seg_filter(m->buf, 31, &S->err);
@@ -1089,14 +1085,15 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
-  for (int l = 0; l < nb; ++l) c->lane_window[in[l].lane] = true;
+  for (int l = 0; l < nb; ++l) c->lanes[in[l].lane].window = true;
   return ALOAM_OK;
 }
 
 int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps) {
-  const PriorMap* P = static_cast<const PriorMap*>(c->prior);
-  if (!P || !c->lane_window[lane]) return ALOAM_ERR_STATE;
-  MapperState* S = static_cast<Locator*>(c->locator[lane])->d_state;
+  const PriorMap* P = c->prior;
+  const Lane& L = c->lanes[lane];
+  if (!P || !L.window) return ALOAM_ERR_STATE;
+  MapperState* S = L.locator->d_state;
   *ps = {};
   ps->grid = PriorGrid{P->grid[0], P->grid[1]};
   ps->win[0][0] = S->sub_off[0]; ps->win[0][1] = S->sub_off[1]; ps->ctr[0] = S->ctr;
@@ -1166,7 +1163,7 @@ int aloam_prior_map_clear(aloam_ctx* c) {
   if (any_lane_localising(c)) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   prior_map_release(c);
-  for (int l = 0; l < ALOAM_MAX_BATCH; ++l) c->lane_armed[l] = false;   // an arming needs a map
+  for (Lane& L : c->lanes) L.sched.armed = false;   // an arming needs a map
   return ALOAM_OK;
 }
 
@@ -1178,9 +1175,10 @@ int aloam_lane_localise(aloam_ctx* c, int lane, const double q_init[4], const do
   if (!(n2 > 0) || !std::isfinite(n2)) return ALOAM_ERR_INVALID_ARG;
   if (!c->prior) return ALOAM_ERR_STATE;
   const double n = std::sqrt(n2);
-  for (int k = 0; k < 4; ++k) c->lane_init[lane][k] = q_init[k] / n;
-  for (int k = 0; k < 3; ++k) c->lane_init[lane][4 + k] = t_init[k];
-  c->lane_armed[lane] = true;
+  Lane& L = c->lanes[lane];
+  for (int k = 0; k < 4; ++k) L.init[k] = q_init[k] / n;
+  for (int k = 0; k < 3; ++k) L.init[4 + k] = t_init[k];
+  L.sched.armed = true;
   return ALOAM_OK;
 }
 
@@ -1191,10 +1189,10 @@ extern "C" {
 int aloam_mapper_reset(aloam_ctx* c) {
   if (!c) return ALOAM_ERR_INVALID_ARG;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  const bool fresh = c->mapper[0] == nullptr;
-  int rc = ensure_mapper(c, 0); if (rc) return rc;   // a new lane 0 is reset already
-  for (int l = fresh ? 1 : 0; l < ALOAM_MAX_BATCH; ++l)   // every lane that exists
-    if (c->mapper[l]) { rc = reset_lane(c, static_cast<Mapper*>(c->mapper[l])); if (rc) return rc; }
+  const bool fresh = !c->lanes[0].mapper;
+  int rc = mapper_ensure(c, 0); if (rc) return rc;   // a new lane 0 is reset already
+  for (size_t l = fresh ? 1 : 0; l < c->lanes.size(); ++l)   // every lane that exists
+    if (c->lanes[l].mapper) { rc = reset_lane(c, c->lanes[l].mapper); if (rc) return rc; }
   return ALOAM_OK;
 }
 
@@ -1205,8 +1203,8 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   rc = check_view(surf_last); if (rc) return rc;
   if (corner_last.n > c->max_points || surf_last.n > c->max_points) return ALOAM_ERR_CAPACITY;   // before any state is touched
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  rc = mapper_ensure_lanes(c, 1); if (rc) return rc;
-  Mapper* m = static_cast<Mapper*>(c->mapper[0]);
+  rc = mapper_ensure(c, 0); if (rc) return rc;
+  Mapper* m = c->lanes[0].mapper;
   CUDA_CHECK_RET(cudaEventRecord(c->ev0, c->stream));
   // the inputs are uploaded to mapper-owned device buffers first: the views may alias any ctx-owned pinned buffer
   rc = upload_cloud(c, corner_last, m->d_in[0], c->max_points); if (rc) return rc;
@@ -1242,11 +1240,13 @@ int aloam_mapper_debug_state_lane(aloam_ctx* c, int lane, int centre[3], int* n_
                                   double t_wmap_wodom[3], long long totals[2]) {
   if (!c) return ALOAM_ERR_STATE;
   if (lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
+  if (lane >= c->n_lanes) return ALOAM_ERR_STATE;   // no such lane, so no store
   // a lane whose trajectory localises answers from its locator, with the totals of the prior map it reads
-  const bool loc = c->lane_localising[lane] && c->locator[lane] && c->prior;
-  if (!loc && !c->mapper[lane]) return ALOAM_ERR_STATE;
-  MapperState* d_state = loc ? static_cast<Locator*>(c->locator[lane])->d_state : static_cast<Mapper*>(c->mapper[lane])->d_state;
-  MapperState* h_state = loc ? static_cast<Locator*>(c->locator[lane])->h_state : static_cast<Mapper*>(c->mapper[lane])->h_state;
+  const Lane& L = c->lanes[lane];
+  const bool loc = L.sched.localising && L.locator && c->prior;
+  if (!loc && !L.mapper) return ALOAM_ERR_STATE;
+  MapperState* d_state = loc ? L.locator->d_state : L.mapper->d_state;
+  MapperState* h_state = loc ? L.locator->h_state : L.mapper->h_state;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   CUDA_CHECK_RET(cudaMemcpy(h_state, d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
   const MapperState* h = h_state;
@@ -1255,7 +1255,7 @@ int aloam_mapper_debug_state_lane(aloam_ctx* c, int lane, int centre[3], int* n_
   if (valid) for (int i = 0; i < h->n_valid && i < 125; ++i) valid[i] = h->valid[i];
   if (q_wmap_wodom) for (int k = 0; k < 4; ++k) q_wmap_wodom[k] = h->q_wmap_wodom[k];
   if (t_wmap_wodom) for (int k = 0; k < 3; ++k) t_wmap_wodom[k] = h->t_wmap_wodom[k];
-  if (totals && loc) { for (int t = 0; t < 2; ++t) totals[t] = static_cast<PriorMap*>(c->prior)->n[t]; }
+  if (totals && loc) { for (int t = 0; t < 2; ++t) totals[t] = c->prior->n[t]; }
   else if (totals)
     for (int t = 0; t < 2; ++t) {
       totals[t] = 0;
@@ -1271,8 +1271,8 @@ int aloam_mapper_debug_state(aloam_ctx* c, int centre[3], int* n_valid, int vali
 
 int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, aloam_cloud_view* out) {
   if (!c || !out || which < 0 || which > 1 || cube < 0 || cube >= NCUBE || lane < 0 || lane >= ALOAM_MAX_BATCH) return ALOAM_ERR_INVALID_ARG;
-  if (!c->mapper[lane]) return ALOAM_ERR_STATE;
-  Mapper* m = static_cast<Mapper*>(c->mapper[lane]);
+  if (lane >= c->n_lanes || !c->lanes[lane].mapper) return ALOAM_ERR_STATE;
+  Mapper* m = c->lanes[lane].mapper;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
   const int s = m->h_state->slab_of[which][cube];
@@ -1287,10 +1287,10 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
   if (what != ALOAM_EXPORT_SURROUND && what != ALOAM_EXPORT_MAP) return ALOAM_ERR_INVALID_ARG;
   const bool prior = lane == ALOAM_PRIOR_MAP;
   if (prior && what != ALOAM_EXPORT_MAP) return ALOAM_ERR_INVALID_ARG;   // the prior map has no frame, so no surround
-  if (prior ? !c->prior : !c->mapper[lane]) return ALOAM_ERR_STATE;
+  const Mapper* m = prior || lane >= c->n_lanes ? nullptr : c->lanes[lane].mapper;
+  const PriorMap* pm = c->prior;
+  if (prior ? !pm : !m) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  const Mapper* m = prior ? nullptr : static_cast<Mapper*>(c->mapper[lane]);
-  PriorMap* pm = static_cast<PriorMap*>(c->prior);
   long long n = 0;
   int rc = ALOAM_OK;
   if (prior) n = (long long)pm->n[0] + pm->n[1];
@@ -1310,7 +1310,7 @@ int aloam_mapper_export(aloam_ctx* c, int lane, int what, float* out, long long 
 }
 
 int aloam_mapper_debug_cube(aloam_ctx* c, int which, int cube, aloam_cloud_view* out) {
-  if (!c || !c->mapper[0]) return ALOAM_ERR_INVALID_ARG;
+  if (!c || !c->lanes[0].mapper) return ALOAM_ERR_INVALID_ARG;
   return aloam_mapper_debug_cube_lane(c, 0, which, cube, out);
 }
 
@@ -1328,8 +1328,8 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
   }
   if (total > 0 && !out) return ALOAM_ERR_INVALID_ARG;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  int rc = mapper_ensure_lanes(c, 1); if (rc) return rc;
-  Mapper* m = static_cast<Mapper*>(c->mapper[0]);
+  int rc = mapper_ensure(c, 0); if (rc) return rc;
+  Mapper* m = c->lanes[0].mapper;
   if (total > m->buf.cap) return ALOAM_ERR_CAPACITY;
   if (!m->d_dbg_err) {   // first use; the pointer that marks the group as ready is allocated last
     CUDA_CHECK_RET(dalloc(c, &m->d_dbg_pts, m->buf.cap));

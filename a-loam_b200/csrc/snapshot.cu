@@ -4,7 +4,7 @@
 //   - its warm start and world pose (Lane::d_pose, d_world);
 //   - its "last" less-sharp / less-flat clouds, in feature slot (frame - 1) mod kFeatSlots -- the slot the next step reads as
 //     "last" -- whose search index is rebuilt from the clouds on restore;
-//   - the index of its next scan (lane_scan) and its mode (lane_mapped);
+//   - the index of its next scan and its mode (LaneSched::scan, mapped);
 //   - mapped: its cube store, in the slab-free form of SnapStore (cubemap.cu saves and restores it).
 // Format: snapshot.h.
 #include <cstring>
@@ -156,10 +156,10 @@ int aloam_snapshot_check(const void* blob, long long n_bytes, aloam_snapshot_inf
 
 int aloam_lane_save(aloam_ctx* c, int lane, void* out, long long capacity, long long* n_bytes) {
   if (!c || !n_bytes || capacity < 0 || lane < 0 || lane >= c->n_lanes) return ALOAM_ERR_INVALID_ARG;
-  if (!c->lanes_mode || !c->lane_running[lane]) return ALOAM_ERR_STATE;
-  if (c->lane_localising[lane]) return ALOAM_ERR_STATE;   // format v1 has no section for a localising lane's state
-  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   const Lane& L = c->lanes[lane];
+  if (!c->lanes_mode || !L.sched.running) return ALOAM_ERR_STATE;
+  if (L.sched.localising) return ALOAM_ERR_STATE;   // format v1 has no section for a localising lane's state
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   const FeatBuf& f = L.feat[last_slot(c)];
   SnapHeader& h = c->pin->snap;
   std::memset(&h, 0, sizeof(h));
@@ -169,8 +169,8 @@ int aloam_lane_save(aloam_ctx* c, int lane, void* out, long long capacity, long 
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   std::memcpy(h.magic, kMagic, 8);
   h.version = kSnapVersion;
-  h.mapped = c->lane_mapped[lane];
-  h.scan_index = c->lane_scan[lane];
+  h.mapped = L.sched.mapped;
+  h.scan_index = L.sched.scan;
   h.n_less_sharp = c->pin->snap_counts[1];
   h.n_less_flat = c->pin->snap_counts[3];
   fingerprint(c, &h);
@@ -208,18 +208,17 @@ int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_byt
   const int kind = buffer_kind(c, blob);
   if (kind < 0) return ALOAM_ERR_INVALID_ARG;
   // as at a START: the lane's trajectory, if any, ends here, and the context runs lanes from now on
+  Lane& L = c->lanes[lane];
   c->lanes_mode = true;
-  c->lane_running[lane] = false;
-  c->lane_localising[lane] = false;
+  L.sched.running = L.sched.localising = false;
   // ---- validation, on the host, before anything is written to the device
   const char* b = static_cast<const char*>(blob);
   const SnapHeader& h = c->pin->snap;
   long long store = 0;
   int rc = snapshot_validate(c, b, n_bytes, kind, false, &store); if (rc) return rc;
   if (h.n_less_sharp > c->max_points || h.n_less_flat > c->max_points) return ALOAM_ERR_CAPACITY;
-  if (h.mapped) { rc = mapper_ensure_lanes(c, lane + 1); if (rc) return rc; }   // creates the lane's cube store if needed
+  for (int l = 0; h.mapped && l <= lane; ++l) { rc = mapper_ensure(c, l); if (rc) return rc; }   // the stores of lanes 0 .. lane, if needed
   // ---- odometry: the "last" clouds into the slot the next step reads, their index and ring check, the poses, the armed scalars
-  Lane& L = c->lanes[lane];
   const int slot = last_slot(c);
   FeatBuf& f = L.feat[slot];
   if (h.n_less_sharp > 0) CUDA_CHECK_RET(cudaMemcpyAsync(f.less_sharp, b + sizeof(h), 16 * (size_t)h.n_less_sharp, cudaMemcpyDefault, c->stream));
@@ -236,9 +235,9 @@ int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_byt
   if (h.mapped) { rc = mapper_store_restore(c, lane, c->h_snap_store, b + store + sizeof(SnapStore), kind); if (rc) return rc; }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
-  c->lane_running[lane] = true;
-  c->lane_mapped[lane] = h.mapped != 0;
-  c->lane_scan[lane] = h.scan_index;
+  L.sched.running = true;
+  L.sched.mapped = h.mapped != 0;
+  L.sched.scan = h.scan_index;
   return ALOAM_OK;
 }
 

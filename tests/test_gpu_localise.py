@@ -324,6 +324,22 @@ def test_refusals_leave_the_state_untouched(aloam, synth):
     c.close()
 
 
+def test_a_refused_call_keeps_the_arming(aloam, synth):
+    """a call that STARTs the armed lane 0 at step 0 and is refused at step 1 (a SCAN on lane 1, which runs nothing) consumes
+    nothing: lane 0's next accepted START localises, as its solo run"""
+    W = _world(aloam, synth)
+    n = 6
+    init = _perturbed(_rebased(W, 2), 0.1, 1.0)
+    c = _localiser(aloam, W, 2)
+    c.lane_localise(0, *init)
+    stray = (W["dev"][2].data_ptr(), W["dev"][2].shape[0], SCAN)
+    _expect(aloam, ERR_STATE, lambda: _call(c, 2, {0: _entries(W["dev"], 2, 2 + n), 1: [stray]}, first_step={1: 1}))
+    r = _call(c, 2, {0: _entries(W["dev"], 2, 2 + n)})[0]
+    ref = _solo(aloam, W, 2, n, init)
+    assert np.array_equal(r[0], ref[0]) and np.array_equal(r[1], ref[1])
+    c.close()
+
+
 def test_create_load_destroy_returns_the_memory(aloam, synth):
     W = _world(aloam, synth)
     _localiser(aloam, W).close()   # first use: the process's one-time allocations

@@ -14,7 +14,7 @@ import skip_refs as S
 
 pytestmark = pytest.mark.gpu
 
-ERR_INVALID_ARG = -1
+ERR_INVALID_ARG, ERR_CAPACITY, ERR_STATE = -1, -4, -9
 N = 24
 KEY = ("VLP-16", 0, 900)
 _RUNS = {}
@@ -134,36 +134,47 @@ def test_sixteen_lane_batch_with_skip_3(aloam, synth):
     ctx.close()
 
 
-def test_lane_schedule_with_staggered_starts_restarts_and_idle_lanes(aloam, synth):
-    """4 lanes, 12 steps in two calls, skip 3.  Step 0 maps every lane, steps 1, 2 none, others a subset; lane 3 restarts at
-    step 4 (its scan index starts again at 0), lanes 1 and 2 are idle for two steps between trajectories"""
-    skip, n = 3, 12
-    I, Sc, St = 0, 1, 2   # LANE_IDLE, LANE_SCAN, LANE_START
-    # lane -> list of (start step, trajectory id, length)
-    plan = {0: [(0, 10, 12)], 1: [(0, 11, 5), (7, 12, 5)], 2: [(0, 13, 3), (5, 14, 7)], 3: [(0, 15, 4), (4, 16, 8)]}
-    B = len(plan)
+I, Sc, St = 0, 1, 2   # LANE_IDLE, LANE_SCAN, LANE_START
+# the staggered schedule: lane -> list of (start step, trajectory id, length) over 12 steps
+PLAN = {0: [(0, 10, 12)], 1: [(0, 11, 5), (7, 12, 5)], 2: [(0, 13, 3), (5, 14, 7)], 3: [(0, 15, 4), (4, 16, 8)]}
+
+
+def _staggered(synth, n=12):
+    """PLAN as (n, lanes) arrays of ops, device addresses and counts, with the trajectories' scans by id"""
+    B = len(PLAN)
     ops = np.full((n, B), I, np.int32)
-    scans = {tid: R.traj(synth, tid, ln) for runs in plan.values() for (_, tid, ln) in runs}
+    scans = {tid: R.traj(synth, tid, ln) for runs in PLAN.values() for (_, tid, ln) in runs}
     dev = {tid: R.to_device(sc) for tid, sc in scans.items()}
     ptrs = np.zeros((n, B), np.uint64)
     counts = np.zeros((n, B), np.int64)
-    for lane, runs in plan.items():
+    for lane, runs in PLAN.items():
         for s0, tid, ln in runs:
             for j in range(ln):
                 ops[s0 + j, lane] = St if j == 0 else Sc
                 ptrs[s0 + j, lane] = dev[tid][j].data_ptr()
                 counts[s0 + j, lane] = scans[tid][j].shape[0]
+    return ops, ptrs, counts, scans, dev
+
+
+def _mapped_rows(ops, skip):
+    """(n, lanes) booleans: the row's scan goes to the mapper, its lane's scan index counted from its START"""
+    idx, m = {}, np.zeros(ops.shape, bool)
+    for k in range(ops.shape[0]):
+        for lane in range(ops.shape[1]):
+            if ops[k, lane] != I:
+                idx[lane] = 0 if ops[k, lane] == St else idx[lane] + 1
+                m[k, lane] = S.mapped(idx[lane], skip)
+    return m
+
+
+def test_lane_schedule_with_staggered_starts_restarts_and_idle_lanes(aloam, synth):
+    """4 lanes, 12 steps in two calls, skip 3.  Step 0 maps every lane, steps 1, 2 none, others a subset; lane 3 restarts at
+    step 4 (its scan index starts again at 0), lanes 1 and 2 are idle for two steps between trajectories"""
+    skip, n = 3, 12
+    B = len(PLAN)
+    ops, ptrs, counts, scans, dev = _staggered(synth, n)
     # the schedule covers the cases it is meant to
-    idx = {}
-    maps = []
-    for k in range(n):
-        m = []
-        for lane in range(B):
-            if ops[k, lane] == I:
-                continue
-            idx[lane] = 0 if ops[k, lane] == St else idx[lane] + 1
-            m.append(S.mapped(idx[lane], skip))
-        maps.append(m)
+    maps = [[bool(m) for m, op in zip(row, ops[k]) if op != I] for k, row in enumerate(_mapped_rows(ops, skip))]
     assert all(maps[0]) and len(maps[0]) == B and not any(maps[1]) and not any(maps[2])
     assert any(any(m) and not all(m) for m in maps)
     assert ops[4, 3] == St and ops[3, 3] == Sc
@@ -172,13 +183,74 @@ def test_lane_schedule_with_staggered_starts_restarts_and_idle_lanes(aloam, synt
     o2, m2 = ctx.scan_stream_lanes(ptrs[6:], counts[6:], ops[6:], True)
     odom, mapped = np.concatenate([o1, o2]), np.concatenate([m1, m2])
     assert np.isnan(odom[ops == I]).all() and np.isnan(mapped[ops == I]).all()
-    for lane, runs in plan.items():
+    for lane, runs in PLAN.items():
         for s0, tid, ln in runs:
             so, sm, sst = _solo_skip(aloam, scans[tid], ("VLP-16", tid, 900), skip)
             rows = slice(s0, s0 + ln)
             assert np.array_equal(odom[rows, lane], so) and np.array_equal(mapped[rows, lane], sm), (lane, tid)
         R.same_store(R.snapshot(ctx, lane), sst, "lane %d, last trajectory" % lane)
     ctx.close()
+
+
+def test_refused_lanes_calls_leave_the_skip_phase_alone(aloam, synth):
+    """the staggered schedule in two calls with a registered sink, skip 3, refused calls between them: an op of 3, a SCAN on an
+    idle lane after a step that advances the other lanes, an unmapped call on mapped lanes, and a call whose registered rows
+    exceed the sink by one point.  The second call equals the uninterrupted run and the solo runs bit for bit."""
+    import torch
+    skip, n, cut = 3, 12, 6
+    ops, ptrs, counts, scans, dev = _staggered(synth, n)
+    B = ops.shape[1]
+    second = int(counts[cut:][_mapped_rows(ops, skip)[cut:]].sum())   # points the second call registers
+    assert second > 0
+
+    def run(refusals):
+        ctx = aloam.Aloam(**_kw(list(scans.values()), max_batch=B, mapping_skip_frame=skip))
+        sink = torch.zeros((int(counts.sum()), 4), dtype=torch.float32, device="cuda")
+        torch.cuda.synchronize()
+        ctx.set_registered_sink(sink)
+        ctx.scan_stream_lanes(ptrs[:cut], counts[:cut], ops[:cut], True)
+        if refusals:
+            p2, c2 = ptrs[cut:], counts[cut:]
+            bad = ops[cut:].copy(); bad[2, 1] = 3
+            with pytest.raises(aloam.AloamError) as e:
+                ctx.scan_stream_lanes(p2, c2, bad, True)
+            assert e.value.code == ERR_INVALID_ARG
+            bad = ops[cut:].copy()
+            assert bad[0, 1] == I and bad[1, 1] == St
+            bad[1, 1] = Sc   # lane 1 has been idle since step 5
+            with pytest.raises(aloam.AloamError) as e:
+                ctx.scan_stream_lanes(p2, c2, bad, True)
+            assert e.value.code == ERR_STATE
+            with pytest.raises(aloam.AloamError) as e:
+                ctx.scan_stream_lanes(p2, c2, ops[cut:], True, mapped=False)
+            assert e.value.code == ERR_STATE
+            ctx.set_registered_sink(sink[:second - 1])
+            with pytest.raises(aloam.AloamError) as e:
+                ctx.scan_stream_lanes(p2, c2, ops[cut:], True)
+            assert e.value.code == ERR_CAPACITY
+            ctx.set_registered_sink(sink[:second])
+        o, m = ctx.scan_stream_lanes(ptrs[cut:], counts[cut:], ops[cut:], True)
+        begin, count = ctx.registered_rows((n - cut) * B)
+        assert count.sum() == second
+        torch.cuda.synchronize()
+        out = (o, m, begin, count, sink[:second].cpu().numpy().copy(), [R.snapshot(ctx, l) for l in range(B)])
+        ctx.close()
+        return out
+
+    got, ref = run(True), run(False)
+    for a, b, what in zip(got[:5], ref[:5], ("odometry", "map poses", "row begins", "row counts", "registered clouds")):
+        assert np.array_equal(a, b, equal_nan=a.dtype.kind == "f"), what
+    for lane in range(B):
+        R.same_store(got[5][lane], ref[5][lane], "lane %d against the uninterrupted run" % lane)
+    for lane, runs in PLAN.items():
+        for s0, tid, ln in runs:
+            if s0 + ln <= cut:
+                continue
+            so, sm, sst = _solo_skip(aloam, scans[tid], ("VLP-16", tid, 900), skip)
+            k0 = max(s0, cut)
+            rows = slice(k0 - cut, s0 + ln - cut)
+            assert np.array_equal(got[0][rows, lane], so[k0 - s0:]) and np.array_equal(got[1][rows, lane], sm[k0 - s0:]), (lane, tid)
+        R.same_store(got[5][lane], sst, "lane %d, last trajectory" % lane)
 
 
 @pytest.mark.parametrize("world", [2, 4])
