@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = [
     "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
     "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
     "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise", "aloam_debug_prior_associate",
+    "aloam_prior_map_build",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -133,6 +134,7 @@ def lib():
         L.aloam_snapshot_check.argtypes = [C.c_void_p, C.c_longlong, C.POINTER(SnapshotInfo)]
         L.aloam_prior_map_load.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
         L.aloam_prior_map_clear.argtypes = [C.c_void_p]
+        L.aloam_prior_map_build.argtypes = [C.c_void_p, cv, cv, ip, C.POINTER(C.c_longlong)]
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
         L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
         _LIB = L
@@ -191,6 +193,37 @@ def snapshot_info(blob):
     _check(lib().aloam_snapshot_check(ptr, n, C.byref(info)))
     return {"version": info.version, "mapped": bool(info.mapped), "n_scans": info.n_scans, "scan_index": info.scan_index,
             "bytes": info.bytes, "map_points": info.map_points, "world": np.array(info.world[:])}
+
+
+def _cloud_view(a):
+    """a cloud argument that may live on the device: a float32 torch tensor (n, 4 | 8), contiguous, in device or host memory,
+    or anything numpy takes -> (CloudView, object to keep alive)"""
+    if hasattr(a, "data_ptr"):
+        if a.dim() != 2 or a.shape[1] not in (4, 8) or a.element_size() != 4 or not a.is_floating_point() or not a.is_contiguous():
+            raise ValueError("a cloud tensor is a contiguous (n, 4) or (n, 8) float32 tensor")
+        return CloudView(C.cast(C.c_void_p(a.data_ptr()), C.POINTER(C.c_float)), a.shape[0], a.shape[1]), a
+    return _view(a)
+
+
+def snapshot_store_clouds(blob):
+    """the cube store of a MAPPED lane snapshot in host memory, split into its two clouds (no context, no GPU): {"corner", "surf":
+    (n, 4) float32, each type's cubes in cube order; "centre": the store's centre offsets; "counts": (2, 4851) int32, points per
+    corner / surf cube, -1 for a cube without a slab}.  prior_map_build(corner, surf, centre) of a single snapshot's clouds
+    rebuilds that store's map; the clouds of several snapshots, moved into one frame and concatenated, make a joined map."""
+    import struct
+    info = snapshot_info(blob)
+    if not info["mapped"]:
+        raise ValueError("the snapshot holds no cube store")
+    b = np.ascontiguousarray(np.frombuffer(bytes(blob), np.uint8) if isinstance(blob, (bytes, bytearray)) else np.asarray(blob, np.uint8)).ravel()
+    nls, nlf = struct.unpack_from("<ii", b, 28)
+    s = 256 + 16 * (nls + nlf)   # the store section
+    centre = struct.unpack_from("<3i", b, s)
+    counts = np.frombuffer(b, np.int32, 2 * 4851, s + 592).reshape(2, 4851).copy()
+    n = int(struct.unpack_from("<q", b, s + 39408)[0])
+    pts = np.frombuffer(b, np.float32, 4 * n, s + 39424).reshape(n, 4)
+    # export order: corner cube i, then surf cube i -- the type of every point, then a stable split
+    kind = np.repeat(np.tile(np.array([0, 1], np.int8), 4851), np.maximum(counts, 0).T.ravel())
+    return {"corner": pts[kind == 0].copy(), "surf": pts[kind == 1].copy(), "centre": tuple(int(v) for v in centre), "counts": counts}
 
 
 def default_config(n_scans):
@@ -540,6 +573,18 @@ class Aloam:
         or a torch tensor"""
         ptr, n, keep = _blob(blob)
         _check(lib().aloam_prior_map_load(self._h, ptr, n))
+
+    def prior_map_build(self, corner, surf, centre=None):
+        """makes the prior map from two clouds in the map frame (aloam_prior_map_build): each point binned into its 50 m cube of the
+        21 x 21 x 11 buffer around `centre` (the ring buffer's centre offsets, default (10, 10, 5)), every cube voxel-filtered as the
+        mapper's re-filter.  Clouds: numpy arrays or float32 torch tensors (device or host), (n, 4) or (n, 8).
+        Returns (dropped corner, dropped surf): the points outside the buffer or with a non-finite coordinate."""
+        a, ka = _cloud_view(corner)
+        b, kb = _cloud_view(surf)
+        cen = None if centre is None else (C.c_int * 3)(*(int(v) for v in centre))
+        dropped = (C.c_longlong * 2)()
+        _check(lib().aloam_prior_map_build(self._h, a, b, cen, dropped))
+        return int(dropped[0]), int(dropped[1])
 
     def prior_map_clear(self):
         _check(lib().aloam_prior_map_clear(self._h))

@@ -253,10 +253,12 @@ struct aloam_ctx {
 namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
-       KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR };
+       KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
+       KID_PRIOR_BUILD };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
-    "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior"};
+    "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
+    "k_prior_build"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -311,6 +313,10 @@ int peer_err_reset(aloam_ctx* c);
 int peer_err_fetch(aloam_ctx* c, int* dst);
 void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper);
 int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
+// voxel.cu: the segmented filter's stable radix sort over one key array of up to n_upper keys (the prior-map build), and the ints
+// of histogram it needs for n keys
+int vox_radix_sort(aloam_ctx* c, int kid, unsigned* k0, int* v0, unsigned* k1, int* v1, const int* n_dev, int n_upper, int bits, int* hist);
+size_t vox_radix_hist_ints(int n);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);

@@ -829,6 +829,278 @@ void prior_index(aloam_ctx* c, PriorMap* p) {
   LAUNCH(c, KID_MAP_GRID, k_prior_tag, dim3(pb, 2, 1), 256, 0, p->grid[0], p->grid[1], p->d_cube_start);
 }
 
+// Makes a new map the context's prior map: centre offsets cen, cloud t of cs[t][NCUBE] points with cube i at [cs[t][i], cs[t][i + 1])
+// (cs in host memory, 2 x (NCUBE + 1) ints).  Allocates the map, uploads the cube table and the ALOAM_EXPORT_MAP layout, lets
+// fill(p) write the points of p->pts[0 / 1] on c->stream (returns an ALOAM_* code), builds the index, synchronises and swaps the
+// map in.  The old map is replaced only on success; on failure the new one is freed.  aloam_prior_map_load and
+// aloam_prior_map_build end here.
+template <typename Fill> int prior_install(aloam_ctx* c, const int cen[3], const std::vector<int>& cs, Fill fill) {
+  PriorMap* p = new (std::nothrow) PriorMap();
+  if (!p) return ALOAM_ERR_CUDA;
+  for (int t = 0; t < 2; ++t) p->n[t] = cs[(size_t)t * (NCUBE + 1) + NCUBE];
+  for (int a = 0; a < 3; ++a) p->cen[a] = cen[a];
+  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&p->d_layout, sizeof(ExportLayout)) == cudaSuccess;
+  for (int t = 0; t < 2 && ok; ++t) {
+    GridTable& g = p->grid[t];
+    g.cap_slots = grid_mask_for(p->n[t], 1u << 30) + 1;
+    g.cs = kMapCell; g.inv_cs = 1.0f / g.cs;
+    const size_t n1 = (size_t)std::max(p->n[t], 1);
+    ok = cudaMalloc(&p->pts[t], n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&g.gpts, n1 * sizeof(float4)) == cudaSuccess &&
+         cudaMalloc(&g.slots, (size_t)g.cap_slots * sizeof(uint4)) == cudaSuccess && cudaMalloc(&g.dyn, sizeof(GridDyn)) == cudaSuccess;
+  }
+  auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); prior_free(p); return code; };
+  if (!ok) return fail(ALOAM_ERR_CUDA);
+  // the ALOAM_EXPORT_MAP layout of the packed clouds: segment 2 i + t is cube i of cloud t
+  std::unique_ptr<ExportLayout> L(new (std::nothrow) ExportLayout());
+  if (!L) return fail(ALOAM_ERR_CUDA);
+  L->nseg = kExportSegs;
+  for (int s = 0; s < kExportSegs; ++s) {
+    const int* t = &cs[(size_t)(s & 1) * (NCUBE + 1) + (s >> 1)];
+    L->base[s] = p->pts[s & 1] + t[0];
+    L->off[s + 1] = L->off[s] + (t[1] - t[0]);
+  }
+  L->total = L->off[kExportSegs];
+  if (cudaMemcpyAsync(p->d_cube_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+      cudaMemcpyAsync(p->d_n, p->n, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+      cudaMemcpyAsync(p->d_layout, L.get(), sizeof(ExportLayout), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+    return fail(ALOAM_ERR_CUDA);
+  const int rc = fill(p); if (rc) return fail(rc);
+  prior_index(c, p);
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ALOAM_ERR_CUDA);
+  if (!c->prior_owned) { own(c, [c] { prior_map_release(c); }); c->prior_owned = true; }
+  prior_map_release(c);
+  c->prior = p;
+  return ALOAM_OK;
+}
+
+// ---- building a prior map from two map-frame clouds (aloam_prior_map_build): the insertion of laserMapping.cpp:741-767 for every
+// point at once, then the per-cube VoxelGrid of :787-801 over every cube.  Segment s = t NCUBE + i holds the points of type t in
+// cube i; kBuildSegs marks a dropped point.  Order of launches: k_build_init, k_build_classify (cube, finite check, per-segment
+// counts and boxes), k_build_params (min_b / div_b / PCL's overflow test per segment, segment offsets), k_build_keys (voxel index
+// of every point), two stable sorts (voxel index, then segment: lexicographic), k_build_heads / k_build_scan (run starts and their
+// ranks), k_build_ranks (voxels before every segment) -- one synchronisation to learn the map's sizes -- then k_build_emit writes
+// every voxel's centroid straight into the map at its rank.
+constexpr int kBuildSegs = 2 * NCUBE;
+constexpr int kBuildTile = 256;
+
+struct BuildSeg {
+  int min_b[3], div_b[3];
+  float inv;
+  int pass;   // PCL's "leaf size is too small": the cube's points are kept as they are, in input order
+};
+
+// one coordinate's cube index (laserMapping.cpp:741-750), decided in double before any conversion: false when (v + 25) / 50 is
+// not finite or lies beyond int, which the reference leaves undefined (the conversion is undefined on the CPU, saturates on the GPU)
+__device__ __forceinline__ bool build_cube_coord(float v, int centre, long long* out) {
+  const double s = (double)v + 25.0;
+  const double q = s / 50.0;
+  if (!(q > -2147483649.0 && q < 2147483648.0)) return false;
+  *out = (long long)(int)q + centre - (s < 0 ? 1 : 0);
+  return true;
+}
+
+__device__ __forceinline__ int build_f2ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : (i ^ 0x7fffffff); }
+__device__ __forceinline__ float build_ord2f(int i) { return __int_as_float(i >= 0 ? i : (i ^ 0x7fffffff)); }
+
+__global__ void __launch_bounds__(256) k_build_init(int* __restrict__ cnt, int* __restrict__ bbox, int* __restrict__ dropped) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < kBuildSegs) {
+    cnt[s] = 0;
+    for (int a = 0; a < 3; ++a) { bbox[6 * s + a] = INT_MAX; bbox[6 * s + 3 + a] = INT_MIN; }
+  }
+  if (s < 2) dropped[s] = 0;
+}
+
+// grid-stride over the n points (corner [0, n_c), surf after): seg[i], and per segment the count and the bounding box (atomics on
+// the order-preserving int of the float, once per group of a warp's lanes that share a segment); dropped[t] per type
+__global__ void __launch_bounds__(256) k_build_classify(const Pt4* __restrict__ pts, int n_c, int n, int c0, int c1, int c2, int* __restrict__ seg,
+                                                        int* __restrict__ cnt, int* __restrict__ bbox, int* __restrict__ dropped) {
+  const int lane = threadIdx.x & 31;
+  for (int base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
+    const int i = base + threadIdx.x;
+    int s = -1;   // -1: no point; kBuildSegs + t: a dropped point of type t
+    Pt4 p = {0.f, 0.f, 0.f, 0.f};
+    if (i < n) {
+      p = pts[i];
+      long long a = -1, b = -1, d = -1;
+      const bool ok = build_cube_coord(p.x, c0, &a) && build_cube_coord(p.y, c1, &b) && build_cube_coord(p.z, c2, &d) &&
+                      a >= 0 && a < CW && b >= 0 && b < CH && d >= 0 && d < CD;   // :751-756
+      const int t = i >= n_c ? 1 : 0;
+      s = ok ? t * NCUBE + (int)(a + CW * b + CW * CH * d) : kBuildSegs + t;
+      seg[i] = ok ? s : kBuildSegs;
+    }
+    const unsigned grp = __match_any_sync(0xffffffffu, s);
+    const bool leader = lane == __ffs(grp) - 1;
+    if (s >= kBuildSegs) {
+      if (leader) atomicAdd(&dropped[s - kBuildSegs], __popc(grp));
+    } else if (s >= 0) {
+      const int lo[3] = {__reduce_min_sync(grp, build_f2ord(p.x)), __reduce_min_sync(grp, build_f2ord(p.y)), __reduce_min_sync(grp, build_f2ord(p.z))};
+      const int hi[3] = {__reduce_max_sync(grp, build_f2ord(p.x)), __reduce_max_sync(grp, build_f2ord(p.y)), __reduce_max_sync(grp, build_f2ord(p.z))};
+      if (leader) {
+        atomicAdd(&cnt[s], __popc(grp));
+        for (int k = 0; k < 3; ++k) { atomicMin(&bbox[6 * s + k], lo[k]); atomicMax(&bbox[6 * s + 3 + k], hi[k]); }
+      }
+    }
+  }
+}
+
+// one CTA of 1024: every segment's voxel parameters, as seg_keys_body (voxel.cu) derives them from the segment's box; off = the
+// exclusive prefix of the counts (off[kBuildSegs] = the points kept)
+__global__ void __launch_bounds__(1024) k_build_params(const int* __restrict__ cnt, const int* __restrict__ bbox, float leaf0, float leaf1,
+                                                       BuildSeg* __restrict__ par, int* __restrict__ off) {
+  __shared__ int s_part[1024];
+  const int per = (kBuildSegs + 1023) / 1024, b = threadIdx.x * per, e = min(b + per, kBuildSegs);
+  int sum = 0;
+  for (int s = b; s < e; ++s) sum += cnt[s];
+  int run = block_scan_1024(sum, s_part);
+  for (int s = b; s < e; ++s) {
+    off[s] = run;
+    run += cnt[s];
+    BuildSeg g = {};
+    if (cnt[s] > 0) {
+      const float inv = 1.0f / (s < NCUBE ? leaf0 : leaf1);
+      long long dxyz[3];
+      for (int a = 0; a < 3; ++a) {
+        const float mn = build_ord2f(bbox[6 * s + a]), mx = build_ord2f(bbox[6 * s + 3 + a]);
+        dxyz[a] = (long long)((mx - mn) * inv) + 1;
+        g.min_b[a] = (int)floorf(mn * inv);
+        g.div_b[a] = (int)floorf(mx * inv) - g.min_b[a] + 1;
+      }
+      g.inv = inv;
+      // PCL's test in int64 (dx dy dz > INT_MAX); in double here so that no product overflows -- exact while it matters
+      g.pass = (double)dxyz[0] * (double)dxyz[1] * (double)dxyz[2] > (double)INT_MAX;
+    }
+    par[s] = g;
+  }
+  if (threadIdx.x == 1023) off[kBuildSegs] = run;
+}
+
+// grid-stride: vox[i] = PCL's voxel index of point i in its segment's box (0 in a pass-through segment and for a dropped point,
+// whose order the stable sorts keep); keys / values of the first sort
+__global__ void __launch_bounds__(256) k_build_keys(const Pt4* __restrict__ pts, int n, const int* __restrict__ seg, const BuildSeg* __restrict__ par,
+                                                    unsigned* __restrict__ vox, unsigned* __restrict__ keys, int* __restrict__ vals) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int s = seg[i];
+    unsigned idx = 0;
+    if (s < kBuildSegs && !par[s].pass) {
+      const BuildSeg& g = par[s];
+      const Pt4 p = pts[i];
+      const int i0 = (int)(floorf(p.x * g.inv) - (float)g.min_b[0]);
+      const int i1 = (int)(floorf(p.y * g.inv) - (float)g.min_b[1]);
+      const int i2 = (int)(floorf(p.z * g.inv) - (float)g.min_b[2]);
+      idx = (unsigned)i0 + (unsigned)i1 * (unsigned)g.div_b[0] + (unsigned)i2 * ((unsigned)g.div_b[0] * (unsigned)g.div_b[1]);   // PCL's int, wrapped
+    }
+    vox[i] = idx;
+    keys[i] = idx;
+    vals[i] = i;
+  }
+}
+
+// grid-stride: the keys of the second sort, the segment of the point at every slot of the first
+__global__ void __launch_bounds__(256) k_build_gather(const int* __restrict__ seg, int n, unsigned* __restrict__ keys, const int* __restrict__ vals) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) keys[j] = (unsigned)seg[vals[j]];
+}
+
+// one thread per sorted slot, a tile of kBuildTile per CTA: head[j] = slot j starts a voxel (every slot of a pass-through segment
+// does; a dropped point never does); tile_heads = heads per tile
+__global__ void __launch_bounds__(kBuildTile) k_build_heads(const unsigned* __restrict__ sseg, const int* __restrict__ sval, int n, const unsigned* __restrict__ vox,
+                                                            const BuildSeg* __restrict__ par, unsigned char* __restrict__ head, int* __restrict__ tile_heads) {
+  const int j = blockIdx.x * kBuildTile + threadIdx.x;
+  bool h = false;
+  if (j < n) {
+    const unsigned s = sseg[j];
+    h = s < (unsigned)kBuildSegs && (j == 0 || s != sseg[j - 1] || par[s].pass || vox[sval[j]] != vox[sval[j - 1]]);
+    head[j] = h ? 1 : 0;
+  }
+  const int cnt = __syncthreads_count(h);
+  if (threadIdx.x == 0) tile_heads[blockIdx.x] = cnt;
+}
+
+// one CTA of 1024: exclusive scan of the tiles' head counts in place; *total = all heads
+__global__ void __launch_bounds__(1024) k_build_scan(int* __restrict__ tile_heads, int tiles, int* __restrict__ total) {
+  __shared__ int s_part[1024];
+  const int per = (tiles + 1023) / 1024, b = threadIdx.x * per, e = min(b + per, tiles);
+  int sum = 0;
+  for (int k = b; k < e; ++k) sum += tile_heads[k];
+  int run = block_scan_1024(sum, s_part);
+  for (int k = b; k < e; ++k) { const int v = tile_heads[k]; tile_heads[k] = run; run += v; }
+  if (threadIdx.x == 1023) *total = run;
+}
+
+// one warp per segment s <= kBuildSegs: rank[s] = voxels before the segment's first sorted slot off[s]
+__global__ void __launch_bounds__(32) k_build_ranks(const int* __restrict__ off, const unsigned char* __restrict__ head, const int* __restrict__ tile_off,
+                                                    const int* __restrict__ total, int n, int* __restrict__ rank) {
+  const int s = blockIdx.x, pos = off[s];
+  if (pos >= n) { if (threadIdx.x == 0) rank[s] = *total; return; }
+  const int t = pos / kBuildTile;
+  int c = 0;
+  for (int j = t * kBuildTile + threadIdx.x; j < pos; j += 32) c += head[j];
+  for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
+  if (threadIdx.x == 0) rank[s] = tile_off[t] + c;
+}
+
+// one thread per sorted slot: a head sums its voxel's run in sorted order (float, pcl::CentroidPoint) and writes the centroid to
+// its rank in the map (cloud 0 below n0 voxels, cloud 1 after); a pass-through head copies its point (keeps -0.f)
+__global__ void __launch_bounds__(kBuildTile) k_build_emit(const Pt4* __restrict__ pts, const unsigned* __restrict__ sseg, const int* __restrict__ sval, int n,
+                                                           const BuildSeg* __restrict__ par, const unsigned char* __restrict__ head,
+                                                           const int* __restrict__ tile_off, int n0, Pt4* __restrict__ out0, Pt4* __restrict__ out1) {
+  __shared__ int s_w[kBuildTile / 32];
+  const int j = blockIdx.x * kBuildTile + threadIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const bool h = j < n && head[j];
+  const unsigned bal = __ballot_sync(0xffffffffu, h);
+  if (lane == 0) s_w[w] = __popc(bal);
+  __syncthreads();
+  if (!h) return;
+  int r = tile_off[blockIdx.x] + __popc(bal & ((1u << lane) - 1u));
+  for (int v = 0; v < w; ++v) r += s_w[v];
+  const unsigned s = sseg[j];
+  Pt4* dst = s < NCUBE ? out0 + r : out1 + (r - n0);
+  if (par[s].pass) { *dst = pts[sval[j]]; return; }
+  float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
+  int cnt = 0;
+  for (int k = j; k < n && (k == j || (!head[k] && sseg[k] == s)); ++k) {
+    const Pt4 p = pts[sval[k]];
+    sx += p.x; sy += p.y; sz += p.z; si += p.i;
+    ++cnt;
+  }
+  const float nf = (float)cnt;
+  Pt4 o; o.x = sx / nf; o.y = sy / nf; o.z = sz / nf; o.i = si / nf;
+  *dst = o;
+}
+
+// the build's scratch, plain cudaMalloc: freed (after the stream has drained) when the call returns
+struct BuildScratch {
+  cudaStream_t stream;
+  Pt4* pts = nullptr;
+  int *seg = nullptr, *cnt = nullptr, *bbox = nullptr, *dropped = nullptr, *off = nullptr, *vals[2] = {nullptr, nullptr}, *hist = nullptr;
+  int *tile_heads = nullptr, *total = nullptr, *rank = nullptr, *n_dev = nullptr;
+  unsigned *vox = nullptr, *keys[2] = {nullptr, nullptr};
+  unsigned char* head = nullptr;
+  BuildSeg* par = nullptr;
+  explicit BuildScratch(cudaStream_t s) : stream(s) {}
+  ~BuildScratch() {
+    cudaStreamSynchronize(stream);
+    cudaGetLastError();
+    for (void* q : {(void*)pts, (void*)seg, (void*)cnt, (void*)bbox, (void*)dropped, (void*)off, (void*)vals[0], (void*)vals[1], (void*)hist,
+                    (void*)tile_heads, (void*)total, (void*)rank, (void*)n_dev, (void*)vox, (void*)keys[0], (void*)keys[1], (void*)head, (void*)par})
+      cudaFree(q);
+  }
+  bool alloc(size_t n, int tiles) {
+    const size_t n1 = std::max<size_t>(n, 1);
+    return cudaMalloc(&pts, n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&seg, n1 * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&cnt, kBuildSegs * sizeof(int)) == cudaSuccess && cudaMalloc(&bbox, 6 * kBuildSegs * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&dropped, 2 * sizeof(int)) == cudaSuccess && cudaMalloc(&off, (kBuildSegs + 1) * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&vals[0], n1 * sizeof(int)) == cudaSuccess && cudaMalloc(&vals[1], n1 * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&hist, vox_radix_hist_ints((int)n1) * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&tile_heads, (size_t)std::max(tiles, 1) * sizeof(int)) == cudaSuccess && cudaMalloc(&total, sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&rank, (kBuildSegs + 1) * sizeof(int)) == cudaSuccess && cudaMalloc(&n_dev, sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&vox, n1 * sizeof(unsigned)) == cudaSuccess && cudaMalloc(&keys[0], n1 * sizeof(unsigned)) == cudaSuccess &&
+           cudaMalloc(&keys[1], n1 * sizeof(unsigned)) == cudaSuccess && cudaMalloc(&head, n1) == cudaSuccess &&
+           cudaMalloc(&par, kBuildSegs * sizeof(BuildSeg)) == cudaSuccess;
+  }
+};
+
 }  // namespace
 
 // points per slab of the two cloud types (16 k corner / 64 k surf, at most cfg.max_points)
@@ -1114,47 +1386,68 @@ int aloam_prior_map_load(aloam_ctx* c, const void* blob, long long n_bytes) {
   const SnapStore* H = c->h_snap_store;
   // ---- the new map is built beside the old one, which is replaced only when the new one is complete
   std::vector<int> cs((size_t)2 * (NCUBE + 1));
-  PriorMap* p = new (std::nothrow) PriorMap();
-  if (!p) return ALOAM_ERR_CUDA;
   for (int t = 0; t < 2; ++t) {
     long long run = 0;
     for (int i = 0; i < NCUBE; ++i) { cs[(size_t)t * (NCUBE + 1) + i] = (int)run; run += std::max(H->count[t][i], 0); }   // (<= 1024 slabs of <= 65536 points)
     cs[(size_t)t * (NCUBE + 1) + NCUBE] = (int)run;
-    p->n[t] = (int)run;
   }
-  for (int a = 0; a < 3; ++a) p->cen[a] = H->cen[a];
-  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&p->d_layout, sizeof(ExportLayout)) == cudaSuccess;
-  for (int t = 0; t < 2 && ok; ++t) {
-    GridTable& g = p->grid[t];
-    g.cap_slots = grid_mask_for(p->n[t], 1u << 30) + 1;
-    g.cs = kMapCell; g.inv_cs = 1.0f / g.cs;
-    const size_t n1 = (size_t)std::max(p->n[t], 1);
-    ok = cudaMalloc(&p->pts[t], n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&g.gpts, n1 * sizeof(float4)) == cudaSuccess &&
-         cudaMalloc(&g.slots, (size_t)g.cap_slots * sizeof(uint4)) == cudaSuccess && cudaMalloc(&g.dyn, sizeof(GridDyn)) == cudaSuccess;
+  return prior_install(c, H->cen, cs, [&](PriorMap* p) {
+    return H->n_points > 0 ? store_copy(c, p->d_layout, H->n_points, const_cast<char*>(b) + store + sizeof(SnapStore), kind, true) : ALOAM_OK;
+  });
+}
+
+int aloam_prior_map_build(aloam_ctx* c, aloam_cloud_view corner, aloam_cloud_view surf, const int centre[3], long long dropped[2]) {
+  if (!c) return ALOAM_ERR_INVALID_ARG;
+  int rc = check_view(corner); if (rc) return rc;
+  rc = check_view(surf); if (rc) return rc;
+  const int cen[3] = {centre ? centre[0] : 10, centre ? centre[1] : 10, centre ? centre[2] : 5};
+  for (int a = 0; a < 3; ++a) if (cen[a] < -(1 << 20) || cen[a] > (1 << 20)) return ALOAM_ERR_INVALID_ARG;
+  if (sharded_job(c) || any_lane_localising(c)) return ALOAM_ERR_STATE;
+  // a cloud of more than 2^30 points, or two that together leave no room for a tile of the sort in int, cannot be indexed
+  if (corner.n > (1 << 30) || surf.n > (1 << 30) || (long long)corner.n + surf.n > (long long)INT_MAX - 4096) return ALOAM_ERR_CAPACITY;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  const int n = corner.n + surf.n, tiles = (n + kBuildTile - 1) / kBuildTile;
+  const int blocks = std::max(1, std::min(tiles, c->sms * 8));
+  std::vector<int> rank(kBuildSegs + 1, 0);
+  int drop[2] = {0, 0};
+  BuildScratch B(c->stream);
+  if (!B.alloc((size_t)n, tiles)) return ALOAM_ERR_CUDA;
+  if (n > 0) {
+    rc = upload_cloud(c, corner, B.pts, n); if (rc) return rc;
+    rc = upload_cloud(c, surf, B.pts + corner.n, surf.n); if (rc) return rc;
+    CUDA_CHECK_RET(cudaMemcpyAsync(B.n_dev, &n, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_init, (kBuildSegs + 255) / 256, 256, 0, B.cnt, B.bbox, B.dropped);
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_classify, blocks, 256, 0, B.pts, corner.n, n, cen[0], cen[1], cen[2], B.seg, B.cnt, B.bbox, B.dropped);
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_params, 1, 1024, 0, B.cnt, B.bbox, c->cfg.line_res, c->cfg.plane_res, B.par, B.off);
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_keys, blocks, 256, 0, B.pts, n, B.seg, B.par, B.vox, B.keys[0], B.vals[0]);
+    // stable: by voxel index (4 passes), then by segment (2 passes); both results end in buffer 0
+    rc = vox_radix_sort(c, KID_PRIOR_BUILD, B.keys[0], B.vals[0], B.keys[1], B.vals[1], B.n_dev, n, 32, B.hist); if (rc) return rc;
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_gather, blocks, 256, 0, B.seg, n, B.keys[0], B.vals[0]);
+    rc = vox_radix_sort(c, KID_PRIOR_BUILD, B.keys[0], B.vals[0], B.keys[1], B.vals[1], B.n_dev, n, 16, B.hist); if (rc) return rc;
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_heads, tiles, kBuildTile, 0, B.keys[0], B.vals[0], n, B.vox, B.par, B.head, B.tile_heads);
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_scan, 1, 1024, 0, B.tile_heads, tiles, B.total);
+    LAUNCH(c, KID_PRIOR_BUILD, k_build_ranks, kBuildSegs + 1, 32, 0, B.off, B.head, B.tile_heads, B.total, n, B.rank);
+    // the one synchronisation before the map exists: its sizes, every cube's, and the drops
+    CUDA_CHECK_RET(cudaMemcpyAsync(rank.data(), B.rank, rank.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(drop, B.dropped, sizeof(drop), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+    CUDA_CHECK_RET(cudaGetLastError());
   }
-  auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); prior_free(p); return code; };
-  if (!ok) return fail(ALOAM_ERR_CUDA);
-  // the ALOAM_EXPORT_MAP layout of the packed clouds: segment 2 i + t is cube i of cloud t
-  std::unique_ptr<ExportLayout> L(new (std::nothrow) ExportLayout());
-  if (!L) return fail(ALOAM_ERR_CUDA);
-  L->nseg = kExportSegs;
-  for (int s = 0; s < kExportSegs; ++s) {
-    const int* t = &cs[(size_t)(s & 1) * (NCUBE + 1) + (s >> 1)];
-    L->base[s] = p->pts[s & 1] + t[0];
-    L->off[s + 1] = L->off[s] + (t[1] - t[0]);
-  }
-  L->total = L->off[kExportSegs];
-  if (cudaMemcpyAsync(p->d_cube_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
-      cudaMemcpyAsync(p->d_n, p->n, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
-      cudaMemcpyAsync(p->d_layout, L.get(), sizeof(ExportLayout), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
-    return fail(ALOAM_ERR_CUDA);
-  if (H->n_points > 0) { rc = store_copy(c, p->d_layout, H->n_points, const_cast<char*>(b) + store + sizeof(SnapStore), kind, true); if (rc) return fail(rc); }
-  prior_index(c, p);
-  if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ALOAM_ERR_CUDA);
-  if (!c->prior_owned) { own(c, [c] { prior_map_release(c); }); c->prior_owned = true; }
-  prior_map_release(c);
-  c->prior = p;
+  const int n0 = rank[NCUBE];
+  std::vector<int> cs((size_t)2 * (NCUBE + 1));
+  for (int t = 0; t < 2; ++t)
+    for (int i = 0; i <= NCUBE; ++i) {
+      const int r = rank[(size_t)t * NCUBE + i] - (t ? n0 : 0);
+      cs[(size_t)t * (NCUBE + 1) + i] = r;
+      if (i > 0 && r - cs[(size_t)t * (NCUBE + 1) + i - 1] > 65536) return ALOAM_ERR_CAPACITY;   // the 16-bit rank of prior_tag
+    }
+  rc = prior_install(c, cen, cs, [&](PriorMap* p) {
+    if (n > 0) LAUNCH(c, KID_PRIOR_BUILD, k_build_emit, tiles, kBuildTile, 0, B.pts, B.keys[0], B.vals[0], n, B.par, B.head, B.tile_heads, n0, p->pts[0], p->pts[1]);
+    return cudaGetLastError() == cudaSuccess ? ALOAM_OK : ALOAM_ERR_CUDA;
+  });
+  prof_collect(c);
+  if (rc) return rc;
+  if (dropped) { dropped[0] = drop[0]; dropped[1] = drop[1]; }
   return ALOAM_OK;
 }
 

@@ -110,6 +110,10 @@ __global__ void __launch_bounds__(VT) k_radix_sort_all(const __grid_constant__ B
   const VoxLane& a = B.a[blockIdx.z];
   radix_sort_all_body(a.keys[0], a.vals[0], a.keys[1], a.vals[1], a.f.total, bits, a.hist);
 }
+// one key array of any size (the prior-map build, cubemap.cu): the same passes over *n keys
+__global__ void __launch_bounds__(VT) k_radix_sort_flat(unsigned* k0, int* v0, unsigned* k1, int* v1, const int* n, int bits, int* hist) {
+  radix_sort_all_body(k0, v0, k1, v1, n, bits, hist);
+}
 
 
 // number of voxel heads (first element of each run of equal keys) per block of VCH sorted elements; the CTAs stride over
@@ -467,6 +471,25 @@ void vox_seg_filter(aloam_ctx* c, int nb, const SegFilter* f_in, SegBuffers* con
     launch_ex(c, KID_VOXEL, k_seg_writeback, dim3(chunks, seg_cap, nb), dim3(256), 0, 1, true, B);
   }
 }
+
+// a stable LSD sort of the *n_dev (<= n_upper) keys k0 / values v0 by their low `bits` bits, one cooperative launch; the result is
+// in (k0, v0) when bits / 8 is even, else in (k1, v1).  hist holds 256 ints per tile of VCH keys.  Kernel id kid.
+int vox_radix_sort(aloam_ctx* c, int kid, unsigned* k0, int* v0, unsigned* k1, int* v1, const int* n_dev, int n_upper, int bits, int* hist) {
+  int per_sm = 0;
+  CUDA_CHECK_RET(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort_flat, VT, 0));
+  const int tiles = std::max(1, (n_upper + VCH - 1) / VCH);
+  prof_begin(c, kid);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(tiles, std::max(1, per_sm * c->sms))); cfg.blockDim = dim3(VT); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, k_radix_sort_flat, k0, v0, k1, v1, n_dev, bits, hist);
+  prof_end(c);
+  CUDA_CHECK_RET(e);
+  return ALOAM_OK;
+}
+size_t vox_radix_hist_ints(int n) { return (size_t)std::max(1, (n + VCH - 1) / VCH) * 256; }
 
 int vox_seg_alloc(aloam_ctx* c, SegBuffers& b, size_t cap) {
   const size_t nb = (cap + VCH - 1) / VCH + 1;

@@ -334,9 +334,33 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  * sort buffers -- about 450 B per point of cfg.max_points, 0.18 GB at 400 000 and 27 MB at 60 000 (arithmetic from the buffer
  * sizes, not measured), against about 1.75 GB for a mapping lane -- and no cube store if the lane never maps.
  * Limits, each ALOAM_ERR_STATE: aloam_lane_save of a localising lane (snapshot format v1 has no section for it); sharded jobs.
- * The lockstep stream calls and aloam_mapper_step never localise. */
+ * The lockstep stream calls and aloam_mapper_step never localise.
+ *
+ * aloam_prior_map_build makes the prior map from two clouds in the MAP frame (the frame of aloam_lane_localise's q_init / t_init):
+ * the points a cube store holds, e.g. the reference's laserCloudCornerArray / laserCloudSurfArray, the store clouds of one or more
+ * snapshots moved into one frame, or a map built offline.  The clouds are aloam_cloud_views (stride 4 or 8, host memory pageable or
+ * pinned, or device memory; the copy kind follows from the address).  centre = the ring buffer's centre offsets
+ * (laserCloudCenWidth / Height / Depth), NULL for {10, 10, 5} (a fresh store's); it chooses which 1050 x 1050 x 550 m window of the
+ * map frame the 21 x 21 x 11 cubes cover; |centre[a]| <= 2^20, else ALOAM_ERR_INVALID_ARG.
+ *   - cube of a point, as the reference's insertion (laserMapping.cpp:741-757): int((x + 25.0) / 50.0) + centre, in double from the
+ *     float coordinate, minus 1 when x + 25.0 < 0.  A point whose cube lies outside the buffer is dropped (:751-756), and so is one
+ *     with a non-finite coordinate or with a (x + 25.0) / 50.0 beyond the range of int (undefined in the reference).  dropped[t]
+ *     (may be NULL) = the points of type t (0 corner, 1 surf) dropped.
+ *   - every cube of every type is voxel-filtered on its own (the re-filter of :787-801: cfg.line_res for corner cubes, cfg.plane_res
+ *     for surf cubes) over its points in input order, with aloam_voxel_filter's semantics: the box is the cube's points, ties go by
+ *     input index, centroids are float sums in sorted order, and a cube whose voxel index range overflows int is kept unfiltered in
+ *     input order (PCL).  There is no key-width limit: every other cube is filtered.
+ *   - the result is what aloam_prior_map_load makes of a store: per type the filtered cubes packed in cube order, points in voxel
+ *     order, the same index, cube tags and ALOAM_EXPORT_MAP export, centre offsets = centre.  Nothing downstream tells the two apart.
+ *   - limits: ALOAM_ERR_CAPACITY when a filtered cube holds more than 65536 points, or a cloud more than 2^30 points (or the two
+ *     together more than 2^31 - 4097); nothing changes.  No bound on cubes per type or points per cube otherwise.  Memory: the map as
+ *     for a load, plus about 42 B per input point of scratch that is freed before the call returns; ALOAM_ERR_CUDA when it fails.
+ *   - state rules are aloam_prior_map_load's: ALOAM_ERR_STATE while any lane is localising, on a rank of a sharded job and on an
+ *     emulating context; the new map is built beside the old one, which is replaced only on success; armings survive;
+ *     aloam_prior_map_clear and aloam_destroy release it.  Two host synchronisations: one to learn the map's sizes, one at the end. */
 #define ALOAM_PRIOR_MAP (-1)
 int aloam_prior_map_load(aloam_ctx* ctx, const void* blob, long long n_bytes);
+int aloam_prior_map_build(aloam_ctx* ctx, aloam_cloud_view corner_map, aloam_cloud_view surf_map, const int centre[3], long long dropped[2]);
 int aloam_prior_map_clear(aloam_ctx* ctx);
 int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
 
