@@ -28,7 +28,7 @@ EXPORTED_SYMBOLS = [
     "aloam_mapper_export", "aloam_set_registered_sink", "aloam_registered_rows",
     "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
     "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise", "aloam_debug_prior_associate",
-    "aloam_prior_map_build",
+    "aloam_prior_map_build", "aloam_prior_relocalise",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -61,6 +61,14 @@ class Stats(C.Structure):
 class SnapshotInfo(C.Structure):
     _fields_ = [("version", C.c_int), ("mapped", C.c_int), ("n_scans", C.c_int), ("scan_index", C.c_int), ("bytes", C.c_longlong),
                 ("map_points", C.c_longlong), ("world", C.c_double * 7)]
+
+
+class RelocOpts(C.Structure):
+    _fields_ = [("inlier_sq", C.c_float), ("max_score_points", C.c_int), ("refine", C.c_int)]
+
+
+class RelocResult(C.Structure):
+    _fields_ = [("hyp", C.c_int), ("score", C.c_int), ("refined_score", C.c_int), ("flags", C.c_int), ("pose", C.c_double * 7)]
 
 
 class AloamError(RuntimeError):
@@ -137,6 +145,7 @@ def lib():
         L.aloam_prior_map_build.argtypes = [C.c_void_p, cv, cv, ip, C.POINTER(C.c_longlong)]
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
         L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
+        L.aloam_prior_relocalise.argtypes = [C.c_void_p, cv, cv, dp, C.c_int, C.POINTER(RelocOpts), ip, C.POINTER(RelocResult)]
         _LIB = L
     return _LIB
 
@@ -224,6 +233,30 @@ def snapshot_store_clouds(blob):
     # export order: corner cube i, then surf cube i -- the type of every point, then a stable split
     kind = np.repeat(np.tile(np.array([0, 1], np.int8), 4851), np.maximum(counts, 0).T.ravel())
     return {"corner": pts[kind == 0].copy(), "surf": pts[kind == 1].copy(), "centre": tuple(int(v) for v in centre), "counts": counts}
+
+
+def pose_grid(q_base, t_centre, half_extent_xy, step_xy, yaws):
+    """relocalisation hypotheses, (n, 7) float64 rows (q xyzw, t): every heading yaw of `yaws` (radians; a turn about the map z
+    axis applied after q_base) at every point t_centre + (i step_xy, j step_xy, 0) of the square lattice with |i step_xy| and
+    |j step_xy| <= half_extent_xy.  Rows run over yaw fastest, then y, then x."""
+    q0 = np.asarray(q_base, np.float64)
+    t0 = np.asarray(t_centre, np.float64)
+    if q0.shape != (4,) or t0.shape != (3,) or not step_xy > 0 or half_extent_xy < 0:
+        raise ValueError("q_base is 4 doubles (x, y, z, w), t_centre 3, step_xy > 0, half_extent_xy >= 0")
+    k = int(np.floor(half_extent_xy / step_xy + 1e-9))
+    offs = np.arange(-k, k + 1) * float(step_xy)
+    yaws = np.atleast_1d(np.asarray(yaws, np.float64))
+    s, c = np.sin(yaws / 2), np.cos(yaws / 2)   # dq = (0, 0, s, c) times q0
+    x, y, z, w = q0
+    q = np.stack([c * x - s * y, c * y + s * x, c * z + s * w, c * w - s * z], axis=1)
+    n = len(offs) * len(offs) * len(yaws)
+    out = np.empty((n, 7))
+    out[:, :4] = np.tile(q, (len(offs) * len(offs), 1))
+    gx, gy = np.meshgrid(offs, offs, indexing="ij")
+    out[:, 4] = np.repeat(t0[0] + gx.ravel(), len(yaws))
+    out[:, 5] = np.repeat(t0[1] + gy.ravel(), len(yaws))
+    out[:, 6] = t0[2]
+    return out
 
 
 def default_config(n_scans):
@@ -596,6 +629,29 @@ class Aloam:
         if q.shape != (4,) or t.shape != (3,):
             raise ValueError("q_init is 4 doubles (x, y, z, w), t_init 3")
         _check(lib().aloam_lane_localise(self._h, int(lane), _dp(q), _dp(t)))
+
+    def prior_relocalise(self, hyps, less_sharp=None, less_flat=None, raw=None, inlier_sq=1.0, max_score_points=1024, refine=1,
+                         scores=True):
+        """scores the hypotheses hyps ((n, 7): candidate T_wmap_wodom, q xyzw, t) of one scan against the prior map and refines
+        the `refine` best with a localising frame each (aloam_prior_relocalise).  The scan is its less_sharp / less_flat clouds, or
+        a raw scan (`raw`) whose features are extracted first.  Returns (results, scores): results = `refine` dicts {hyp, score,
+        refined_score, flags, pose (7,)} best first, scores = the (n,) int32 coarse scores (None when scores=False)."""
+        if raw is not None:
+            f = self.extract_features(raw)
+            less_sharp, less_flat = f["less_sharp"], f["less_flat"]
+        a, ka = _view(less_sharp)
+        b, kb = _view(less_flat)
+        h = np.ascontiguousarray(hyps, np.float64)
+        if h.ndim != 2 or h.shape[1] != 7:
+            raise ValueError("hyps is an (n, 7) array of poses (q xyzw, t)")
+        opts = RelocOpts(float(inlier_sq), int(max_score_points), int(refine))
+        out = (RelocResult * max(int(refine), 1))()
+        sc = np.zeros(max(h.shape[0], 1), np.int32) if scores else None
+        _check(lib().aloam_prior_relocalise(self._h, a, b, _dp(h), h.shape[0], C.byref(opts),
+                                            sc.ctypes.data_as(C.POINTER(C.c_int)) if scores else None, out))
+        res = [{"hyp": r.hyp, "score": r.score, "refined_score": r.refined_score, "flags": r.flags, "pose": np.array(r.pose[:])}
+               for r in out[:int(refine)]]
+        return res, (sc[:h.shape[0]] if scores else None)
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

@@ -726,8 +726,12 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
         if (sink) { rc = register_rows(in, n_map); if (rc) return fail(rc); }
       }
       if (n_loc > 0) {
-        rc = locate_step_device(c, n_loc, loc, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+        Locator* lp[ALOAM_MAX_BATCH];
+        const double* init[ALOAM_MAX_BATCH];
+        for (int j = 0; j < n_loc; ++j) { Lane& L = c->lanes[loc[j].lane]; lp[j] = L.locator; init[j] = L.init; }
+        rc = locate_step_device(c, n_loc, loc, lp, init, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
         if (rc) return fail(rc);
+        for (int j = 0; j < n_loc; ++j) c->lanes[loc[j].lane].window = true;
         if (sink) { rc = register_rows(loc, n_loc); if (rc) return fail(rc); }
       }
       if (n_map + n_loc > 0) STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));

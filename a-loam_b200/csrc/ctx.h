@@ -55,6 +55,7 @@ struct ExportLayout;   // cubemap.cu: where the segments of a store export are i
 struct Mapper;         // cubemap.cu: a lane's cube store
 struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
 struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexed
+struct Relocaliser;    // reloc.cu: the scratch of aloam_prior_relocalise
 }  // namespace aloam
 
 using namespace aloam;
@@ -241,6 +242,7 @@ struct aloam_ctx {
   // localisation (cubemap.cu): the context's prior map, released by prior_map_release
   PriorMap* prior = nullptr;
   bool prior_owned = false;       // prior_map_release is on the release list
+  Relocaliser* reloc = nullptr;   // aloam_prior_relocalise (reloc.cu), created on first use, released through `release`
   // every resource the context acquires (dalloc, halloc, screate, ecreate, own): aloam_destroy synchronises `streams`, then
   // runs `release` in reverse order of acquisition
   std::vector<cudaStream_t> streams;
@@ -254,11 +256,11 @@ namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
-       KID_PRIOR_BUILD };
+       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
-    "k_prior_build"};
+    "k_prior_build", "k_reloc_score", "k_reloc_topk"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -323,11 +325,34 @@ int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const 
 // the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
 int mapper_ensure(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);
-// localisation against the prior map (cubemap.cu): a lane's locator, created on first use; one frame of nb localising lanes on
-// the current stream (in[l].fresh: the lane starts its trajectory with this frame, from its Lane::init); its per-call error word
+// localisation against the prior map (cubemap.cu): a new locator; a lane's locator, created on first use; one frame of nb
+// localising records on the current stream, record l on locator loc[l] (in[l].fresh: it starts a trajectory with this frame,
+// from T_wmap_wodom init[l]); a lane's per-call error word
+int locator_create(aloam_ctx* c, Locator** out);
 int locator_ensure(aloam_ctx* c, int lane);
-int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const* loc, const double* const* init, int n_upper_c, int n_upper_s);
 int* locator_err_acc(aloam_ctx* c, int lane);
+// what a locator's latest frame left on the device: its filtered corner / surf stacks, their sizes (counts[0], counts[1]) and
+// its flags followed by its error word (2 ints)
+struct LocatorFrame { const Pt4* stack[2]; const int* counts; const int* flags; };
+LocatorFrame locator_frame(const Locator* m);
+// the stack filters of a localising frame alone, for locator m on the clouds of `in`, joined to the current stream: the
+// filtered stacks and their sizes as locator_frame reports them (a stack filter's error bit joins the locator's next frame)
+int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_upper_c, int n_upper_s);
+// the hash grids of the context's prior map (it exists)
+PriorGrid prior_grid(const aloam_ctx* c);
+// the checks and normalisation of an initial T_wmap_wodom (aloam_lane_localise, aloam_prior_relocalise): false for a non-finite
+// value or a zero quaternion, else out = (q / |q|, t), |q|^2 summed in index order
+inline bool map_pose_normalise(const double q[4], const double t[3], double out[7]) {
+  double n2 = 0;
+  for (int k = 0; k < 4; ++k) { if (!std::isfinite(q[k])) return false; n2 += q[k] * q[k]; }
+  for (int k = 0; k < 3; ++k) if (!std::isfinite(t[k])) return false;
+  if (!(n2 > 0) || !std::isfinite(n2)) return false;
+  const double n = std::sqrt(n2);
+  for (int k = 0; k < 4; ++k) out[k] = q[k] / n;
+  for (int k = 0; k < 3; ++k) out[4 + k] = t[k];
+  return true;
+}
 // the search of lane `lane`'s latest localising frame as record 0 of *ps: the prior map's grids, the window tables and centre cube
 // in the lane's locator.  ALOAM_ERR_STATE without a prior map or when the lane has run no localising frame against it.
 int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps);

@@ -1300,10 +1300,9 @@ int mapper_ensure(aloam_ctx* c, int lane) {
   return ALOAM_OK;
 }
 
-// lane `lane`'s locator, created on first use and published only when fully allocated (what was acquired before a failure
-// belongs to the context until aloam_destroy)
-int locator_ensure(aloam_ctx* c, int lane) {
-  if (c->lanes[lane].locator) return ALOAM_OK;
+// a new locator in *out, published only when fully allocated (what was acquired before a failure belongs to the context until
+// aloam_destroy)
+int locator_create(aloam_ctx* c, Locator** out) {
   if (stack_stream_ensure(c) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
   Locator* m = new (std::nothrow) Locator();
   if (!m) return ALOAM_ERR_CUDA;
@@ -1312,17 +1311,45 @@ int locator_ensure(aloam_ctx* c, int lane) {
   ok = ok && map_reg_alloc(c, &m->reg, false) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
   ok = ok && cudaMemset(m->d_state, 0, sizeof(MapperState)) == cudaSuccess;
   if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
-  c->lanes[lane].locator = m;
+  *out = m;
   return ALOAM_OK;
+}
+
+// lane `lane`'s locator, created on first use
+int locator_ensure(aloam_ctx* c, int lane) {
+  return c->lanes[lane].locator ? ALOAM_OK : locator_create(c, &c->lanes[lane].locator);
 }
 
 int* locator_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].locator->d_state->err_acc; }
 
-// One localising frame of nb lanes on the current stream: laserMapping.cpp:309-734 without the ring-buffer shift, against the
-// context's prior map, which it only reads.  Record l as in mapper_step_device; its lane's locator exists.  Every launch covers
-// all lanes: the stack filters (forked, as the mapping frame's), k_locate_begin, the thin-map test, outer_iters x (k_map_knn5_prior,
-// k_map_fit, LM), k_mapper_update, k_mapper_finish (the stack filter's error bit).
-int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s) {
+LocatorFrame locator_frame(const Locator* m) {
+  const MapperState* S = m->d_state;
+  return LocatorFrame{{m->reg.stack[0], m->reg.stack[1]}, S->stack_counts, &S->flags};
+}
+
+PriorGrid prior_grid(const aloam_ctx* c) { return PriorGrid{c->prior->grid[0], c->prior->grid[1]}; }
+
+int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_upper_c, int n_upper_s) {
+  Batch<MapperLane> B = {};
+  MapperState* S = m->d_state;
+  B.a[0].S = S;
+  B.a[0].in[0] = in.corner; B.a[0].in[1] = in.surf; B.a[0].n_in[0] = in.nc; B.a[0].n_in[1] = in.ns;
+  B.a[0].stack[0] = m->reg.stack[0]; B.a[0].stack[1] = m->reg.stack[1];
+  B.a[0].segs = m->buf.segs; B.a[0].n_seg = m->buf.n_seg;
+  const SegFilter f = seg_filter(m->buf, 31, &S->err);
+  SegBuffers* bufs[1] = {&m->buf};
+  const int rc = stack_filters_fork(c, 1, B, &f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
+  CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_stack_join, 0));
+  return ALOAM_OK;
+}
+
+// One localising frame of nb records on the current stream: laserMapping.cpp:309-734 without the ring-buffer shift, against the
+// context's prior map, which it only reads.  Record l as in mapper_step_device (in[l].lane is not read), run on the frame state
+// and registration set of locator loc[l]; a record that starts a trajectory (in[l].fresh) begins from T_wmap_wodom init[l] (7
+// doubles, host memory).  Every launch covers all records: the stack filters (forked, as the mapping frame's), k_locate_begin,
+// the thin-map test, outer_iters x (k_map_knn5_prior, k_map_fit, LM), k_mapper_update, k_mapper_finish (the stack filter's error
+// bit).
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const* loc, const double* const* init, int n_upper_c, int n_upper_s) {
   const PriorMap* P = c->prior;
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || sharded_job(c)) return ALOAM_ERR_STATE;
   Batch<MapperLane> B = {};
@@ -1333,15 +1360,14 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   PriorSearch ps = {};
   ps.grid = PriorGrid{P->grid[0], P->grid[1]};
   for (int l = 0; l < nb; ++l) {
-    const Lane& lane = c->lanes[in[l].lane];
-    Locator* m = lane.locator;
+    Locator* m = loc[l];
     MapperState* S = m->d_state;
     B.a[l].S = S; B.a[l].odom7 = in[l].odom7; B.a[l].out7 = in[l].out7;
     B.a[l].in[0] = in[l].corner; B.a[l].in[1] = in[l].surf; B.a[l].n_in[0] = in[l].nc; B.a[l].n_in[1] = in[l].ns;
     B.a[l].stack[0] = m->reg.stack[0]; B.a[l].stack[1] = m->reg.stack[1];
     B.a[l].segs = m->buf.segs; B.a[l].n_seg = m->buf.n_seg;
     L.a[l].S = S; L.a[l].odom7 = in[l].odom7; L.a[l].fresh = in[l].fresh;
-    for (int k = 0; k < 7; ++k) L.a[l].init[k] = lane.init[k];
+    for (int k = 0; k < 7; ++k) L.a[l].init[k] = init[l][k];
     io[l] = MapLaneIO{m->reg, {nullptr, nullptr}, S->stack_counts, S->x};
     ps.win[l][0] = S->sub_off[0]; ps.win[l][1] = S->sub_off[1]; ps.ctr[l] = S->ctr;
     stack_f[l] = seg_filter(m->buf, 31, &S->err);
@@ -1357,7 +1383,6 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
-  for (int l = 0; l < nb; ++l) c->lanes[in[l].lane].window = true;
   return ALOAM_OK;
 }
 
@@ -1462,15 +1487,11 @@ int aloam_prior_map_clear(aloam_ctx* c) {
 
 int aloam_lane_localise(aloam_ctx* c, int lane, const double q_init[4], const double t_init[3]) {
   if (!c || lane < 0 || lane >= c->n_lanes || !q_init || !t_init) return ALOAM_ERR_INVALID_ARG;
-  double n2 = 0;
-  for (int k = 0; k < 4; ++k) { if (!std::isfinite(q_init[k])) return ALOAM_ERR_INVALID_ARG; n2 += q_init[k] * q_init[k]; }
-  for (int k = 0; k < 3; ++k) if (!std::isfinite(t_init[k])) return ALOAM_ERR_INVALID_ARG;
-  if (!(n2 > 0) || !std::isfinite(n2)) return ALOAM_ERR_INVALID_ARG;
+  double init[7];
+  if (!map_pose_normalise(q_init, t_init, init)) return ALOAM_ERR_INVALID_ARG;
   if (!c->prior) return ALOAM_ERR_STATE;
-  const double n = std::sqrt(n2);
   Lane& L = c->lanes[lane];
-  for (int k = 0; k < 4; ++k) L.init[k] = q_init[k] / n;
-  for (int k = 0; k < 3; ++k) L.init[4 + k] = t_init[k];
+  for (int k = 0; k < 7; ++k) L.init[k] = init[k];
   L.sched.armed = true;
   return ALOAM_OK;
 }

@@ -25,22 +25,13 @@
 #include <climits>
 #include <nccl.h>
 #include "ctx.h"
+#include "grid.cuh"
 
 namespace aloam {
 
 namespace {
-constexpr unsigned long long kEmpty = ~0ull;
 constexpr int kSlab = 8;  // cells per ownership slab (x direction)
 
-__device__ __forceinline__ unsigned long long cell_key(int cx, int cy, int cz) {
-  return ((unsigned long long)(unsigned)(cx + (1 << 20)) << 42) | ((unsigned long long)(unsigned)(cy + (1 << 20)) << 21) |
-         (unsigned long long)(unsigned)(cz + (1 << 20));
-}
-__device__ __forceinline__ unsigned hash_key(unsigned long long k) {
-  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-  return (unsigned)k;
-}
-__device__ __forceinline__ int cell_of(float v, float inv_cs) { return (int)floorf(v * inv_cs); }
 // floor division and a non-negative remainder, as shard.py's owner_of_cell: a cell left of x = -2^20 m still has an owner
 __device__ __forceinline__ int owner_of(int cx, int count) {
   const int v = cx + (1 << 20);
@@ -48,7 +39,6 @@ __device__ __forceinline__ int owner_of(int cx, int count) {
   const int r = slab % count;
   return r < 0 ? r + count : r;
 }
-__device__ __forceinline__ unsigned long long slot_key(const uint4& s) { return ((unsigned long long)s.y << 32) | s.x; }
 __device__ __forceinline__ unsigned table_mask_for(int n) {   // next power of two >= 1.25 n (>= 1024), minus one
   unsigned want = (unsigned)n + ((unsigned)n >> 2);
   unsigned m = 1024;
@@ -266,16 +256,6 @@ __global__ void __launch_bounds__(256) k_shard_scatter(const float* __restrict__
 }
 
 namespace {
-
-__device__ __forceinline__ int warp_incl_scan(int v) {
-  const unsigned lane = lane_id();
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= (unsigned)d) v += t;
-  }
-  return v;
-}
 
 // per-lane sorted list of the K best (distance, original index) with the point's slot in gpts as payload
 template <int K>

@@ -364,6 +364,53 @@ int aloam_prior_map_build(aloam_ctx* ctx, aloam_cloud_view corner_map, aloam_clo
 int aloam_prior_map_clear(aloam_ctx* ctx);
 int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
 
+/* ---- relocalisation: finding the map pose aloam_lane_localise needs, for a vehicle that boots on the map, a lane that lost
+ * track or a recording that starts somewhere unknown.  aloam_prior_relocalise scores n_hyp pose hypotheses of ONE scan against
+ * the context's prior map on the device and refines the `refine` best of them with a localising frame each.
+ *   - inputs: less_sharp / less_flat = the scan's clouds in the sensor frame, as aloam_mapper_step and a localising frame take
+ *     them.  hyps (host memory, n_hyp x 7 doubles q xyzw, t; 1 <= n_hyp <= 1 << 24): candidate T_wmap_wodom of a vehicle whose
+ *     odometry frame starts at this scan, each checked and normalised as aloam_lane_localise does (a non-finite value or a zero
+ *     quaternion: ALOAM_ERR_INVALID_ARG, and nothing runs).
+ *   - scoring points: the frame's stack filters (cfg.line_res / cfg.plane_res) over the two clouds; per type, with n_t stack
+ *     points and m = min(n_t, max_score_points), scoring point i < m is stack point floor(i * n_t / m) (64-bit integers).
+ *   - score of a hypothesis: every scoring point is moved by pointAssociateToMap at the normalised hypothesis (the association's
+ *     own float coordinates) and is an inlier when SOME map point of its type anywhere in the prior map (no cube window) lies at
+ *     float ((dx*dx + dy*dy) + dz*dz) < inlier_sq.  The 27 grid cells around the point hold every such point (1.00001 m cells,
+ *     inlier_sq <= 1).  score = inliers of both types, an integer independent of evaluation order.
+ *   - selection: hypotheses ranked by (score descending, index ascending); the first `refine` = K go on.
+ *   - refinement: each of the K runs one localising frame from T_wmap_wodom = its hypothesis and the identity odometry pose, all
+ *     K in one batched frame.  out[r].pose is bit for bit the map pose of the START row of a lane armed with
+ *     aloam_lane_localise(lane, hyps[out[r].hyp]) whose aloam_scan_stream_lanes START scan is this scan.  A thin window
+ *     (ALOAM_FLAG_MAP_TOO_THIN in out[r].flags) leaves the pose at the hypothesis.  The refined pose is scored again
+ *     (refined_score), and out is sorted by (refined_score descending, coarse rank ascending): out[0] is the answer.  Arm a lane
+ *     with out[0].pose and START it on this scan or the next.
+ *   - scores (may be NULL): the n_hyp coarse scores in hypothesis order.
+ *   - errors, each before anything changes: ALOAM_ERR_STATE without a prior map, on a rank of a sharded job or on an emulating
+ *     context; ALOAM_ERR_INVALID_ARG for NULL arguments, a bad cloud view, n_hyp out of range, or options outside
+ *     0 < inlier_sq <= 1, max_score_points >= 1, 1 <= refine <= min(ALOAM_MAX_BATCH, n_hyp); ALOAM_ERR_CAPACITY for a cloud of
+ *     more than cfg.max_points.  After a frame whose stack filter overflowed its key (as aloam_mapper_step) the outputs are
+ *     written and the call returns ALOAM_ERR_CAPACITY.
+ *   - synchronous; every lane, the prior map and the stream state are left as they were, so the call may run between any two
+ *     stream calls.
+ *   - memory, created on first use and kept until aloam_destroy: the K registration sets (a localising lane's, about 450 B per
+ *     point of cfg.max_points each, created as calls need them), the two uploaded clouds (32 B per point of cfg.max_points), and
+ *     60 B per hypothesis (the normalised hypotheses and their scores), grown to the largest call (arithmetic from the buffer
+ *     sizes, not measured). */
+typedef struct aloam_reloc_opts {
+  float inlier_sq;        /* 0 < inlier_sq <= 1 (m^2) */
+  int max_score_points;   /* per type, >= 1: how many stack points score each hypothesis */
+  int refine;             /* K: the K best hypotheses are refined, 1 <= K <= min(ALOAM_MAX_BATCH, n_hyp) */
+} aloam_reloc_opts;
+typedef struct aloam_reloc_result {
+  int hyp;                /* index into hyps */
+  int score;              /* inliers at the hypothesis */
+  int refined_score;      /* inliers at the refined pose */
+  int flags;              /* ALOAM_FLAG_MAP_TOO_THIN when the refining frame saw a thin window (pose = the hypothesis) */
+  double pose[7];         /* the refined map pose of this scan (q xyzw, t) */
+} aloam_reloc_result;
+int aloam_prior_relocalise(aloam_ctx* ctx, aloam_cloud_view less_sharp, aloam_cloud_view less_flat, const double* hyps, int n_hyp,
+                           const aloam_reloc_opts* opts, int* scores, aloam_reloc_result* out);
+
 /* TransformToEnd of laserOdometry.cpp:133-148 on a whole cloud: undistort every point to the sweep start with its own
  * interpolation ratio, then carry it to the sweep end with (q_last_curr, t_last_curr); the intensity keeps only the scan id.
  * (Dead code in the reference -- its call sites sit under `if (0)`, :533-552 -- provided because the DISTORTION build
