@@ -29,11 +29,13 @@ EXPORTED_SYMBOLS = [
     "aloam_lane_save", "aloam_lane_restore", "aloam_snapshot_check",
     "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise", "aloam_debug_prior_associate",
     "aloam_prior_map_build", "aloam_prior_relocalise",
+    "aloam_set_map_rows", "aloam_map_rows",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 EXPORT_SURROUND, EXPORT_MAP = 0, 1
 PRIOR_MAP = -1   # `lane` of mapper_export: the context's prior map
+ROW_IDLE, ROW_MAPPED, ROW_LOCALISED, ROW_SKIPPED = 0, 1, 2, 3   # aloam_map_row.kind
 
 
 class Config(C.Structure):
@@ -69,6 +71,11 @@ class RelocOpts(C.Structure):
 
 class RelocResult(C.Structure):
     _fields_ = [("hyp", C.c_int), ("score", C.c_int), ("refined_score", C.c_int), ("flags", C.c_int), ("pose", C.c_double * 7)]
+
+
+class MapRow(C.Structure):
+    _fields_ = [("kind", C.c_int), ("err", C.c_int), ("n_valid", C.c_int), ("n_sub", C.c_int * 2), ("n_stack", C.c_int * 2),
+                ("score", C.c_int), ("n_score", C.c_int), ("stats", Stats)]
 
 
 class AloamError(RuntimeError):
@@ -146,6 +153,8 @@ def lib():
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
         L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
         L.aloam_prior_relocalise.argtypes = [C.c_void_p, cv, cv, dp, C.c_int, C.POINTER(RelocOpts), ip, C.POINTER(RelocResult)]
+        L.aloam_set_map_rows.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int]
+        L.aloam_map_rows.argtypes = [C.c_void_p, C.POINTER(MapRow), C.c_int]
         _LIB = L
     return _LIB
 
@@ -422,6 +431,29 @@ class Aloam:
         begin = np.zeros(max(rows, 1), np.int64); count = np.zeros(max(rows, 1), np.int32)
         _check(lib().aloam_registered_rows(self._h, begin.ctypes.data_as(C.POINTER(C.c_longlong)), count.ctypes.data_as(C.POINTER(C.c_int)), int(rows)))
         return begin[:rows], count[:rows]
+
+    def set_map_rows(self, on=True, inlier_sq=1.0, max_score_points=0):
+        """turns per-row records of the mapped stream calls on or off (aloam_set_map_rows): from the next mapped stream call every row
+        records its frame's flags, stats and sizes, and with max_score_points > 0 every localising row its prior-map inlier score
+        (at most max_score_points stack points per type, inliers at float d2 < inlier_sq) -- see map_rows"""
+        _check(lib().aloam_set_map_rows(self._h, int(on), float(inlier_sq), int(max_score_points)))
+
+    def map_rows(self, rows):
+        """the `rows` = n_scans x batch rows (scan-major) of the last mapped stream call (aloam_map_rows), as a dict of numpy arrays:
+        kind (ROW_*), err, n_valid, score (-1: not scored), n_score, flags, n_corner_corr, n_plane_corr, lm_iters, accepted_steps,
+        init_cost, final_cost, each (rows,); n_sub and n_stack (rows, 2); termination (rows, 4)"""
+        out = (MapRow * max(int(rows), 1))()
+        _check(lib().aloam_map_rows(self._h, out, int(rows)))
+        out = out[:int(rows)]
+        d = {k: np.array([getattr(r, k) for r in out], np.int32) for k in ("kind", "err", "n_valid", "score", "n_score")}
+        for k in ("n_sub", "n_stack"):
+            d[k] = np.array([list(getattr(r, k)) for r in out], np.int32).reshape(-1, 2)
+        for k in ("flags", "n_corner_corr", "n_plane_corr", "lm_iters", "accepted_steps"):
+            d[k] = np.array([getattr(r.stats, k) for r in out], np.int32)
+        d["termination"] = np.array([list(r.stats.termination) for r in out], np.int32).reshape(-1, 4)
+        for k in ("init_cost", "final_cost"):
+            d[k] = np.array([getattr(r.stats, k) for r in out], np.float64)
+        return d
 
     def seg_voxel_filter(self, segs, leaves, idx_bits=31):
         """the mapper's segmented VoxelGrid over `segs` ((n, 4) float32 clouds, one leaf each) in one pass with `idx_bits`

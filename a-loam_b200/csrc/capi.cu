@@ -585,11 +585,23 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
   // registered clouds (aloam_set_registered_sink): every mapped row's ring-major cloud is stashed with its feature slot by stage C
   // and moved into the world by k_register_full after the row's mapper frame; without a sink none of this is issued
   const bool sink = map_poses && c->reg_sink;
+  // per-row records (aloam_set_map_rows): k_map_rows after every frame, k_track_score after every localising frame when scoring is
+  // on; without recording none of this is issued
+  const bool rec = map_poses && c->rows_on;
+  const bool score = rec && c->rows_max_score > 0;
   const size_t rows = (size_t)n_scans * nb;
   if (map_poses) {
     c->reg_rows = -1;
     c->reg_begin.resize(rows); c->reg_count.assign(rows, 0);
     for (size_t r = 0; r < rows; ++r) c->reg_begin[r] = t.rows[r].reg_begin;
+    c->rows_n = -1;
+    if (rec) {
+      c->rows_kind.resize(rows);
+      for (size_t r = 0; r < rows; ++r) {
+        const StreamRow& w = t.rows[r];
+        c->rows_kind[r] = w.op == ALOAM_LANE_IDLE ? ALOAM_ROW_IDLE : !w.mapped ? ALOAM_ROW_SKIPPED : w.localise ? ALOAM_ROW_LOCALISED : ALOAM_ROW_MAPPED;
+      }
+    }
     for (int l = 0; l < nb; ++l) {   // the mappers' error bits of this call (a lane that only localises has no cube store)
       if (c->lanes[l].mapper) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
       if (c->lanes[l].locator) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
@@ -720,9 +732,13 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
         }
         return mapper_register_full_device(c, n, fr, src, nf, dst, nmax);
       };
+      // the row slots of a frame's records
+      auto row_slots = [&](const MapperIn* fr, int n, MapRowRec** out) { for (int j = 0; j < n; ++j) out[j] = c->d_rows + (size_t)k * nb + fr[j].lane; };
+      MapRowRec* slots_rec[ALOAM_MAX_BATCH];
       if (n_map > 0) {
         rc = mapper_step_device(c, n_map, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
         if (rc) return fail(rc);
+        if (rec) { row_slots(in, n_map, slots_rec); rc = map_rows_device(c, n_map, in, slots_rec, 0); if (rc) return fail(rc); }
         if (sink) { rc = register_rows(in, n_map); if (rc) return fail(rc); }
       }
       if (n_loc > 0) {
@@ -731,6 +747,11 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
         for (int j = 0; j < n_loc; ++j) { Lane& L = c->lanes[loc[j].lane]; lp[j] = L.locator; init[j] = L.init; }
         rc = locate_step_device(c, n_loc, loc, lp, init, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
         if (rc) return fail(rc);
+        if (rec) {
+          row_slots(loc, n_loc, slots_rec);
+          rc = map_rows_device(c, n_loc, loc, slots_rec, c->rows_max_score); if (rc) return fail(rc);
+          if (score) { rc = track_score_device(c, n_loc, loc, slots_rec, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points)); if (rc) return fail(rc); }
+        }
         for (int j = 0; j < n_loc; ++j) c->lanes[loc[j].lane].window = true;
         if (sink) { rc = register_rows(loc, n_loc); if (rc) return fail(rc); }
       }
@@ -753,6 +774,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     STREAM_TRY(cudaEventRecord(c->ev_mapend, c->s_map));   // the last mapper frame and the last high-frequency poses
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapend, 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
+    if (rec) STREAM_TRY(cudaMemcpyAsync(c->h_rows, c->d_rows, total * sizeof(MapRowRec), cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) {
       c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
       if (c->lanes[l].mapper) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
@@ -793,6 +815,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
   if (map_poses) {   // the registered rows of this call (count 0 without a sink)
     for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
     c->reg_rows = (int)rows;
+    if (rec) c->rows_n = (int)rows;   // readable after ALOAM_ERR_CAPACITY and ALOAM_ERR_COMM below: they name the row that was hit
   }
   // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
   if (map_poses) {
@@ -891,7 +914,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   }
   if (map && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (run_err) { aloam_reset_odometry(c); return run_err; }
+  if (run_err) { if (map) c->rows_n = -1; aloam_reset_odometry(c); return run_err; }
   for (int l = 0; map && l < batch; ++l) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
     int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
     rc = maps[l] || !localises[l] ? mapper_ensure(c, l) : ALOAM_OK; if (rc) return rc;

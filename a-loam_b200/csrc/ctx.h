@@ -51,6 +51,26 @@ struct PriorSearch {
   const int* win[ALOAM_MAX_BATCH][2];
   const int* ctr[ALOAM_MAX_BATCH];
 };
+// the head of an LmSummary, termination through final_cost: what a frame's stats are made of
+struct LmHead {
+  int termination, num_iterations, num_successful, num_jac_evals;
+  int n_edge, n_plane;
+  double initial_cost, final_cost;
+};
+// one row of a mapped stream call as k_map_rows (cubemap.cu) and k_track_score (rows.cu) leave it on the device: the frame's
+// flags and error word, its window and stack sizes, the summaries of its outer iterations and its prior-map inlier score (-1: not
+// scored; k_track_score adds to 0)
+struct MapRowRec {
+  int flags, err, n_valid, n_sub[2], n_stack[2], score, n_score, pad;
+  LmHead lm[4];
+};
+// one record of k_track_score: the localising frame's filtered stacks and their sizes, the row's map pose and its row slot
+struct TrackArgs {
+  const Pt4* stack[2];
+  const int* counts;
+  const double* pose;
+  MapRowRec* row;
+};
 struct ExportLayout;   // cubemap.cu: where the segments of a store export are in the export and in the store
 struct Mapper;         // cubemap.cu: a lane's cube store
 struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
@@ -204,6 +224,16 @@ struct aloam_ctx {
   std::vector<long long> reg_begin;
   std::vector<int> reg_count;
   int reg_rows = -1;
+  // per-row records of the mapped stream calls (aloam_set_map_rows, rows.cu): the setting, the device row table and its pinned
+  // copy ([kMaxStreamScans] each, created by the first call that turns recording on), and the kinds (ALOAM_ROW_*) of the last
+  // mapped stream call's rows -- rows_n of them, -1 when that call's rows cannot be read
+  bool rows_on = false;
+  float rows_inlier_sq = 1.f;
+  int rows_max_score = 0;
+  MapRowRec* d_rows = nullptr;
+  MapRowRec* h_rows = nullptr;
+  std::vector<signed char> rows_kind;
+  int rows_n = -1;
   // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
   // memory, created on first use
   ExportLayout* d_export_layout = nullptr;
@@ -256,11 +286,11 @@ namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
-       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK };
+       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
-    "k_prior_build", "k_reloc_score", "k_reloc_topk"};
+    "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -322,6 +352,10 @@ size_t vox_radix_hist_ints(int n);
 int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, int n_upper_s);
 int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in);
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper);
+// per-row records (aloam_set_map_rows): the rows of the nb records of the frame just issued (cubemap.cu), and the prior-map inlier
+// score of its localising records at their map poses (rows.cu; n_upper_c / n_upper_s bound the stacks as for the frame)
+int map_rows_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int max_score);
+int track_score_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int n_upper_c, int n_upper_s);
 // the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
 int mapper_ensure(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);
@@ -432,13 +466,15 @@ int upload_cloud(aloam_ctx* c, aloam_cloud_view v, Pt4* dst, int capacity) {
 LastCloud last_corner(const FeatBuf& f) { return LastCloud{f.less_sharp, f.counts + 1, f.g_ls}; }
 LastCloud last_surf(const FeatBuf& f) { return LastCloud{f.less_flat, f.counts + 3, f.g_lf}; }
 
-void fill_stats_from(const LmSummary* h_summary, aloam_stats* st, int outer, int flags, float ms) {
+// S: LmSummary, or the LmHead of a recorded row (the same fields)
+template <typename S>
+void fill_stats_from(const S* h_summary, aloam_stats* st, int outer, int flags, float ms) {
   if (!st) return;
   std::memset(st, 0, sizeof(*st));
   st->flags = flags;
   st->ms_total = ms;
   for (int it = 0; it < outer && it < 4; ++it) {
-    const LmSummary& s = h_summary[it];
+    const S& s = h_summary[it];
     st->lm_iters += s.num_iterations;
     st->accepted_steps += s.num_successful;
     st->termination[it] = s.termination;
@@ -450,6 +486,16 @@ void fill_stats_from(const LmSummary* h_summary, aloam_stats* st, int outer, int
   }
 }
 inline void fill_stats(aloam_ctx* c, aloam_stats* st, int outer, int flags, float ms) { fill_stats_from(c->h_summary, st, outer, flags, ms); }
+// the stats of one scan-to-map frame (aloam_mapper_step, and the rows of the mapped stream calls): a frame that skipped its
+// optimisation on a thin map has zeroed stats and only its flags; any other, its outer iterations' summaries
+template <typename S>
+void frame_stats_from(const S* summary, aloam_stats* st, int outer, int flags, float ms) {
+  if (!(flags & ALOAM_FLAG_MAP_TOO_THIN)) { fill_stats_from(summary, st, outer, flags, ms); return; }
+  if (!st) return;
+  std::memset(st, 0, sizeof(*st));
+  st->flags = flags;
+  st->ms_total = ms;
+}
 
 int check_view(const aloam_cloud_view& v) {
   if (v.n < 0) return ALOAM_ERR_INVALID_ARG;

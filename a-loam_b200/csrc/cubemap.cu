@@ -1261,6 +1261,52 @@ int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const 
   return ALOAM_OK;
 }
 
+namespace {
+// one record of k_map_rows: the frame state and the solve summaries of the frame a row's lane has just run, the row's slot, and
+// the scoring points per type behind its score (0: the row is not scored)
+struct MapRowLane {
+  const MapperState* S;
+  const LmSummary* summary;
+  MapRowRec* row;
+  int max_score;
+};
+
+// the rows of a frame's records, grid (1, 1, records) x 32 threads, after the frame's last kernel: thread t < outer copies the head
+// of outer iteration t's summary, thread 0 the frame's flags, error word and sizes.  A scored row starts its count at 0 for
+// k_track_score and records the scoring points it covers.
+__global__ void __launch_bounds__(32) k_map_rows(const __grid_constant__ Batch<MapRowLane> B, int outer) {
+  const MapRowLane& a = B.a[blockIdx.z];
+  const MapperState* S = a.S;
+  MapRowRec* r = a.row;
+  const int t = threadIdx.x;
+  if (t < outer) {
+    const LmSummary& s = a.summary[t];
+    r->lm[t] = LmHead{s.termination, s.num_iterations, s.num_successful, s.num_jac_evals, s.n_edge, s.n_plane, s.initial_cost, s.final_cost};
+  }
+  if (t == 0) {
+    r->flags = S->flags; r->err = S->frame_err; r->n_valid = S->n_valid;
+    for (int k = 0; k < 2; ++k) { r->n_sub[k] = S->n_sub[k]; r->n_stack[k] = S->stack_counts[k]; }
+    const int m = a.max_score > 0 ? min(S->stack_counts[0], a.max_score) + min(S->stack_counts[1], a.max_score) : 0;
+    r->score = a.max_score > 0 ? 0 : -1;
+    r->n_score = m;
+  }
+}
+}  // namespace
+
+// k_map_rows over the nb records of the frame just issued on the current stream (the mapper stream, before the lanes' next
+// frame): record l into rows[l]; its localising records are scored at max_score points per type (0: none is)
+int map_rows_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int max_score) {
+  if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
+  Batch<MapRowLane> B = {};
+  for (int l = 0; l < nb; ++l) {
+    const Lane& L = c->lanes[in[l].lane];
+    B.a[l] = MapRowLane{lane_state(c, in[l]), in[l].localise ? L.locator->reg.summary : L.mapper->reg->summary, rows[l], in[l].localise ? max_score : 0};
+  }
+  LAUNCH(c, KID_MAP_ROWS, k_map_rows, dim3(1, 1, nb), 32, 0, B, std::min(c->cfg.outer_iters, 4));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 // the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
 int* mapper_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].mapper->d_state->err_acc; }
 
@@ -1543,8 +1589,7 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   for (int k = 0; k < 4; ++k) q_w_curr[k] = c->pin->mapper_pose_out[k];
   for (int k = 0; k < 3; ++k) t_w_curr[k] = c->pin->mapper_pose_out[4 + k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-  if (m->h_state->flags & ALOAM_FLAG_MAP_TOO_THIN) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = m->h_state->flags; stats->ms_total = ms; } }
-  else fill_stats(c, stats, c->cfg.outer_iters, m->h_state->flags, ms);
+  frame_stats_from(c->h_summary, stats, c->cfg.outer_iters, m->h_state->flags, ms);
   if (m->h_state->frame_err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
   if (c->pin->peer_err) return ALOAM_ERR_COMM;                // a peer did not answer: the pose rests on a partial sum
   return ALOAM_OK;

@@ -328,7 +328,8 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  * from the lane's T_wmap_wodom); the registered sink serves localising rows like mapped rows; aloam_mapper_debug_state_lane answers
  * for a localising lane (centre = the prior map's, valid = the clipped window of its last frame, its T_wmap_wodom, totals = the prior
  * map's); aloam_mapper_export with lane = ALOAM_PRIOR_MAP and ALOAM_EXPORT_MAP exports the prior map (ALOAM_ERR_STATE without one).
- * Per-frame flags are not returned by the stream calls (as for mapping lanes).
+ * Per-frame flags, stats and sizes of mapping and localising rows, and a prior-map inlier score of localising rows, come from
+ * aloam_map_rows (per-row records, below) while recording is on.
  * A localising lane owns only what a frame writes, created at its first localising START (ALOAM_ERR_CUDA before any state changes):
  * its frame state, 5-NN records and residual blocks for 2 x cfg.max_points queries, the two filtered stacks and the stack filter's
  * sort buffers -- about 450 B per point of cfg.max_points, 0.18 GB at 400 000 and 27 MB at 60 000 (arithmetic from the buffer
@@ -517,6 +518,53 @@ int aloam_mapper_export(aloam_ctx* ctx, int lane, int what, float* out, long lon
  * when `rows` is not that call's row count. */
 int aloam_set_registered_sink(aloam_ctx* ctx, float* data, long long capacity);
 int aloam_registered_rows(aloam_ctx* ctx, long long* begin, int* count, int rows);
+/* ---- per-row records of the mapped stream calls: what every scan-to-map row of aloam_scan_stream_mapped, _mapped_batch and _lanes
+ * (with map_poses) did -- its flags, stats and sizes, which the stream calls do not return, and for a localising row how many of
+ * its scan's points still land on the prior map at the row's map pose.  A lane that drives off the map, locks onto a wrong pose
+ * or overflows a cube slab shows in its own rows, so a caller can tell which lane to relocalise (aloam_prior_relocalise) and
+ * which row made a call return ALOAM_ERR_CAPACITY.
+ * aloam_set_map_rows(ctx, 1, inlier_sq, max_score_points) turns recording on from the next mapped stream call; on = 0 turns it
+ * off (the default): the stream calls then issue exactly what they issue without this feature, same launches and copies.  The
+ * first call that turns it on allocates a device row table of 4096 rows (kMaxStreamScans) and its pinned host copy, 200 B per
+ * row each, kept until aloam_destroy; ALOAM_ERR_CUDA, with nothing changed, when that fails.  ALOAM_ERR_INVALID_ARG for on
+ * outside {0, 1}, max_score_points < 0, or max_score_points > 0 with inlier_sq outside (0, 1] (the 27 cells of the 1.00001 m
+ * grid hold every point that close, as for aloam_prior_relocalise); max_score_points = 0 records rows without scoring.
+ * ALOAM_ERR_STATE on a rank of a sharded job and on an emulating context; aloam_comm_init and aloam_debug_shard_emulate with
+ * world > 0 turn recording off.  Cost with recording on: one launch (k_map_rows) per frame, one more (k_track_score) per
+ * localising frame when scoring, one device-to-host copy of the call's rows.
+ * aloam_map_rows copies the `rows` = n_scans x batch rows of the last mapped stream call, scan-major like map_poses (it mirrors
+ * aloam_registered_rows).  ALOAM_ERR_INVALID_ARG when out is NULL or `rows` is not that call's row count; ALOAM_ERR_STATE before
+ * any mapped stream call, when that call ran with recording off, or when it failed with anything but ALOAM_ERR_CAPACITY or
+ * ALOAM_ERR_COMM (after those two the rows are readable: they say which row was hit).
+ * Rows:
+ *   - ALOAM_ROW_MAPPED / ALOAM_ROW_LOCALISED: `stats` is exactly what aloam_mapper_step returns for that frame, ms_total = 0 -- a
+ *     frame on a thin map (ALOAM_FLAG_MAP_TOO_THIN) has zeroed stats and only its flags, any other the stats of its outer_iters
+ *     solves with ALOAM_FLAG_FEW_CORRESPONDENCES from the last; ALOAM_FLAG_CUBE_OVERFLOW from the frame's error word.
+ *   - ALOAM_ROW_SKIPPED (cfg.mapping_skip_frame): zero stats, score = -1.  ALOAM_ROW_IDLE: kind only, every other field 0.
+ *   - score (ALOAM_ROW_LOCALISED rows while max_score_points > 0, thin frames included): aloam_prior_relocalise's score at the row's
+ *     map pose.  The scoring points are the frame's own filtered stacks: per type, with n_t stack points and m_t = min(n_t,
+ *     max_score_points), scoring point i is stack point floor(i n_t / m_t); each is moved by pointAssociateToMap at the row's map
+ *     pose and is an inlier when some prior-map point of its type, anywhere in the map, lies at float ((dx*dx + dy*dy) + dz*dz) <
+ *     inlier_sq.  So for a lane armed with hyps[out[r].hyp] of an aloam_prior_relocalise call and STARTed on that call's scan, the
+ *     START row's score equals out[r].refined_score when both run with the same inlier_sq and max_score_points.  A lane that keeps
+ *     track scores near n_score; one that lost track scores far below it. */
+#define ALOAM_ROW_IDLE 0        /* no scan at this step */
+#define ALOAM_ROW_MAPPED 1      /* a mapping frame ran for the row */
+#define ALOAM_ROW_LOCALISED 2   /* a localising frame against the prior map ran for the row */
+#define ALOAM_ROW_SKIPPED 3     /* cfg.mapping_skip_frame: high-frequency pose, no frame */
+typedef struct aloam_map_row {
+  int kind;          /* ALOAM_ROW_* */
+  int err;           /* the frame's error word: bit 0 voxel index range beyond the sort key (why the call returned ALOAM_ERR_CAPACITY),
+                        bits 1-3 slab overflow / pool exhausted / submap truncated */
+  int n_valid;       /* cubes in the frame's window */
+  int n_sub[2];      /* corner / surf map points the frame registered against (the gathered submap, or a localising lane's window) */
+  int n_stack[2];    /* the filtered corner / surf stacks */
+  int score;         /* ALOAM_ROW_LOCALISED rows with scoring on: inliers at the row's map pose; otherwise -1 */
+  int n_score;       /* scoring points behind `score` (m_corner + m_surf); 0 when not scored */
+  aloam_stats stats; /* exactly what aloam_mapper_step returns for this frame, ms_total = 0 */
+} aloam_map_row;
+int aloam_set_map_rows(aloam_ctx* ctx, int on, float inlier_sq, int max_score_points);
+int aloam_map_rows(aloam_ctx* ctx, aloam_map_row* out, int rows);
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
