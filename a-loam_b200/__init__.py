@@ -30,6 +30,7 @@ EXPORTED_SYMBOLS = [
     "aloam_prior_map_load", "aloam_prior_map_clear", "aloam_lane_localise", "aloam_debug_prior_associate",
     "aloam_prior_map_build", "aloam_prior_relocalise",
     "aloam_set_map_rows", "aloam_map_rows",
+    "aloam_set_recovery", "aloam_recovery_rows", "aloam_debug_recovery_scores",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -76,6 +77,14 @@ class RelocResult(C.Structure):
 class MapRow(C.Structure):
     _fields_ = [("kind", C.c_int), ("err", C.c_int), ("n_valid", C.c_int), ("n_sub", C.c_int * 2), ("n_stack", C.c_int * 2),
                 ("score", C.c_int), ("n_score", C.c_int), ("stats", Stats)]
+
+
+class RecoveryOpts(C.Structure):
+    _fields_ = [("trigger_frac", C.c_float), ("accept_frac", C.c_float)]
+
+
+class RecoveryRow(C.Structure):
+    _fields_ = [("triggered", C.c_int), ("best", C.c_int), ("best_score", C.c_int), ("adopted", C.c_int), ("pose", C.c_double * 7)]
 
 
 class AloamError(RuntimeError):
@@ -155,6 +164,9 @@ def lib():
         L.aloam_prior_relocalise.argtypes = [C.c_void_p, cv, cv, dp, C.c_int, C.POINTER(RelocOpts), ip, C.POINTER(RelocResult)]
         L.aloam_set_map_rows.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int]
         L.aloam_map_rows.argtypes = [C.c_void_p, C.POINTER(MapRow), C.c_int]
+        L.aloam_set_recovery.argtypes = [C.c_void_p, C.c_int, C.POINTER(RecoveryOpts), dp, C.c_int]
+        L.aloam_recovery_rows.argtypes = [C.c_void_p, C.POINTER(RecoveryRow), C.c_int]
+        L.aloam_debug_recovery_scores.argtypes = [C.c_void_p, C.c_int, ip, C.c_int]
         _LIB = L
     return _LIB
 
@@ -454,6 +466,41 @@ class Aloam:
         for k in ("init_cost", "final_cost"):
             d[k] = np.array([getattr(r.stats, k) for r in out], np.float64)
         return d
+
+    def set_recovery(self, on=True, trigger_frac=0.5, accept_frac=0.75, deltas=None):
+        """turns recovery of localising lanes on or off (aloam_set_recovery): from the next mapped stream call a localising row whose
+        score is below trigger_frac of its scoring points scores the candidates (q_d * q_P normalised, t_P + t_d) around its map pose
+        P for every delta d of `deltas` ((n, 7) float64, q xyzw, t: pose_grid(identity, 0, half, step, yaws) lays out a search), and
+        the lane's T_wmap_wodom is re-seated at the best one when it beats the row's score and holds accept_frac of its scoring
+        points.  Needs set_map_rows with max_score_points > 0.  on=False turns it off and reads nothing else."""
+        if not on:
+            _check(lib().aloam_set_recovery(self._h, 0, None, None, 0))
+            return
+        d = np.ascontiguousarray(deltas, np.float64)
+        if d.ndim != 2 or d.shape[1] != 7:
+            raise ValueError("deltas are (n, 7) float64 rows (q xyzw, t)")
+        o = RecoveryOpts(float(trigger_frac), float(accept_frac))
+        _check(lib().aloam_set_recovery(self._h, 1, C.byref(o), _dp(d), d.shape[0]))
+        self._n_delta = d.shape[0]
+
+    def recovery_rows(self, rows):
+        """what recovery did on the `rows` = n_scans x batch rows (scan-major) of the last mapped stream call (aloam_recovery_rows), as
+        a dict of numpy arrays: triggered, best (-1: not triggered), best_score (-1), adopted, each (rows,); pose (rows, 7), the best
+        candidate's map pose (zeros when not triggered)"""
+        out = (RecoveryRow * max(int(rows), 1))()
+        _check(lib().aloam_recovery_rows(self._h, out, int(rows)))
+        out = out[:int(rows)]
+        d = {k: np.array([getattr(r, k) for r in out], np.int32) for k in ("triggered", "best", "best_score", "adopted")}
+        d["pose"] = np.array([list(r.pose) for r in out], np.float64).reshape(-1, 7)
+        return d
+
+    def debug_recovery_scores(self, lane):
+        """the candidate scores, one per delta of the last set_recovery, of lane `lane`'s latest triggered row of the last mapped
+        stream call"""
+        n_delta = getattr(self, "_n_delta", 0)
+        out = np.zeros(max(int(n_delta), 1), np.int32)
+        _check(lib().aloam_debug_recovery_scores(self._h, int(lane), out.ctypes.data_as(C.POINTER(C.c_int)), int(n_delta)))
+        return out[:int(n_delta)]
 
     def seg_voxel_filter(self, segs, leaves, idx_bits=31):
         """the mapper's segmented VoxelGrid over `segs` ((n, 4) float32 clouds, one leaf each) in one pass with `idx_bits`

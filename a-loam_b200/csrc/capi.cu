@@ -589,8 +589,12 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
   // on; without recording none of this is issued
   const bool rec = map_poses && c->rows_on;
   const bool score = rec && c->rows_max_score > 0;
+  // recovery of localising lanes (aloam_set_recovery, recover.cu): four more launches after every scored localising frame
+  const bool recov = score && c->rec_on;
   const size_t rows = (size_t)n_scans * nb;
   if (map_poses) {
+    c->rec_call = recov;
+    recover_call_done(c, 0, nb);   // no lane's candidate scores belong to this call yet
     c->reg_rows = -1;
     c->reg_begin.resize(rows); c->reg_count.assign(rows, 0);
     for (size_t r = 0; r < rows; ++r) c->reg_begin[r] = t.rows[r].reg_begin;
@@ -751,6 +755,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
           row_slots(loc, n_loc, slots_rec);
           rc = map_rows_device(c, n_loc, loc, slots_rec, c->rows_max_score); if (rc) return fail(rc);
           if (score) { rc = track_score_device(c, n_loc, loc, slots_rec, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points)); if (rc) return fail(rc); }
+          if (recov) { rc = recover_device(c, n_loc, loc, slots_rec); if (rc) return fail(rc); }
         }
         for (int j = 0; j < n_loc; ++j) c->lanes[loc[j].lane].window = true;
         if (sink) { rc = register_rows(loc, n_loc); if (rc) return fail(rc); }
@@ -816,6 +821,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
     c->reg_rows = (int)rows;
     if (rec) c->rows_n = (int)rows;   // readable after ALOAM_ERR_CAPACITY and ALOAM_ERR_COMM below: they name the row that was hit
+    if (rec) recover_call_done(c, n_scans, nb);
   }
   // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
   if (map_poses) {

@@ -59,10 +59,26 @@ struct LmHead {
 };
 // one row of a mapped stream call as k_map_rows (cubemap.cu) and k_track_score (rows.cu) leave it on the device: the frame's
 // flags and error word, its window and stack sizes, the summaries of its outer iterations and its prior-map inlier score (-1: not
-// scored; k_track_score adds to 0)
+// scored; k_track_score adds to 0).  With recovery on (aloam_set_recovery), a localising row also holds what its recovery did:
+// k_recover_cand (recover.cu) sets rec_triggered, k_recover_adopt (cubemap.cu) the rest of a triggered row.
 struct MapRowRec {
   int flags, err, n_valid, n_sub[2], n_stack[2], score, n_score, pad;
   LmHead lm[4];
+  int rec_triggered, rec_best, rec_best_score, rec_adopted;
+  double rec_pose[7];
+};
+// one hypothesis set of k_reloc_score / k_reloc_topk (reloc.cu): n_hyp normalised poses (7 doubles each) scored against the
+// stacks (sizes counts[0], counts[1]) into score[h]; part (may be null): the CTAs' best keys, kRelocTop per CTA; best: the best
+// keys of the set; gate (may be null): the set is ranked only when *gate != 0 -- its CTAs leave at once otherwise
+struct RelocRec {
+  const double* hyp;
+  int n_hyp;
+  const Pt4* stack[2];
+  const int* counts;
+  int* score;
+  unsigned long long* part;
+  unsigned long long* best;
+  const int* gate;
 };
 // one record of k_track_score: the localising frame's filtered stacks and their sizes, the row's map pose and its row slot
 struct TrackArgs {
@@ -76,6 +92,7 @@ struct Mapper;         // cubemap.cu: a lane's cube store
 struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
 struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexed
 struct Relocaliser;    // reloc.cu: the scratch of aloam_prior_relocalise
+struct Recovery;       // recover.cu: the setting and buffers of aloam_set_recovery
 }  // namespace aloam
 
 using namespace aloam;
@@ -90,6 +107,7 @@ constexpr int kProfSlots = 192;                        // kernel launches timed 
 constexpr int kFeatSlots = 4;                          // feature-set ring of the fused / stream paths
 constexpr int kApiLast = kFeatSlots, kApiCur = kFeatSlots + 1;   // feature sets of the per-stage entry points (set_last / extract, register): never the ring's
 constexpr int kMaxStreamScans = 4096;                  // scans x lanes per aloam_scan_stream(_batch) call
+constexpr int kRelocTop = ALOAM_MAX_BATCH;             // best keys k_reloc_score keeps per CTA and k_reloc_topk returns
 
 struct FeatBuf {
   Pt4 *sharp = nullptr, *less_sharp = nullptr, *flat = nullptr, *less_flat = nullptr;
@@ -234,6 +252,11 @@ struct aloam_ctx {
   MapRowRec* h_rows = nullptr;
   std::vector<signed char> rows_kind;
   int rows_n = -1;
+  // recovery of localising lanes (aloam_set_recovery, recover.cu): on only while rows are scored; its buffers, created by the first
+  // call that turns it on; whether the last mapped stream call ran it
+  bool rec_on = false;
+  Recovery* recover = nullptr;
+  bool rec_call = false;
   // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
   // memory, created on first use
   ExportLayout* d_export_layout = nullptr;
@@ -286,11 +309,11 @@ namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
-       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE };
+       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE, KID_RECOVER_CAND, KID_RECOVER_ADOPT };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
-    "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score"};
+    "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score", "k_recover_cand", "k_recover_adopt"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -356,6 +379,20 @@ int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const 
 // score of its localising records at their map poses (rows.cu; n_upper_c / n_upper_s bound the stacks as for the frame)
 int map_rows_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int max_score);
 int track_score_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int n_upper_c, int n_upper_s);
+// relocalisation scoring (reloc.cu), one hypothesis set per record in blockIdx.z: k_reloc_score over nrec sets with `ctas` CTAs
+// each (max_pts scoring points per type, inliers at float d2 < inlier_sq); k_reloc_topk: the `rounds` best keys of each set's
+// ctas x kRelocTop CTA keys.  reloc_score_ctas: the CTAs a set of n_hyp hypotheses is scored with (at most one resident wave).
+void reloc_score_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int max_pts, float inlier_sq);
+void reloc_topk_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int rounds);
+int reloc_score_ctas(aloam_ctx* c, int n_hyp);
+// recovery of localising lanes (recover.cu): after track_score_device, the recovery of the frame's nb localising records, whose
+// scored rows are rows[l]; and its last kernel (cubemap.cu), which adopts record l's best candidate (of cand[l], best key *best[l])
+int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows);
+int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, const double* const* cand,
+                         const unsigned long long* const* best, float accept_frac);
+// which lanes' candidate scores belong to a triggered row of the mapped stream call whose n_scans x nb rows are in c->h_rows
+// (recover.cu; n_scans = 0 at the start of a call: none)
+void recover_call_done(aloam_ctx* c, int n_scans, int nb);
 // the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
 int mapper_ensure(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);

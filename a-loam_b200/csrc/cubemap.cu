@@ -29,6 +29,7 @@
 #include <memory>
 #include "common.cuh"
 #include "ctx.h"
+#include "quat.cuh"
 
 namespace {
 
@@ -139,27 +140,6 @@ struct MapperLane {
   SegDesc* segs;         // the lane's segmented filter
   int* n_seg;
 };
-
-// ---- Eigen-order quaternion helpers (operation order of Eigen::Quaternion: the pose hand-off is compared bit for bit)
-struct Qd { double x, y, z, w; };
-__host__ __device__ inline Qd qmul(const Qd& a, const Qd& b) {
-  Qd r;
-  r.w = a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z;
-  r.x = a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y;
-  r.y = a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z;
-  r.z = a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x;
-  return r;
-}
-__host__ __device__ inline Qd qinv(const Qd& a) {
-  const double n2 = a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
-  return Qd{-a.x / n2, -a.y / n2, -a.z / n2, a.w / n2};
-}
-__host__ __device__ inline void qrot(const Qd& q, const double v[3], double o[3]) {
-  double uv[3] = {q.y * v[2] - q.z * v[1], q.z * v[0] - q.x * v[2], q.x * v[1] - q.y * v[0]};
-  uv[0] = uv[0] + uv[0]; uv[1] = uv[1] + uv[1]; uv[2] = uv[2] + uv[2];
-  const double c2[3] = {q.y * uv[2] - q.z * uv[1], q.z * uv[0] - q.x * uv[2], q.x * uv[1] - q.y * uv[0]};
-  o[0] = v[0] + q.w * uv[0] + c2[0]; o[1] = v[1] + q.w * uv[1] + c2[1]; o[2] = v[2] + q.w * uv[2] + c2[2];
-}
 
 // int((v + 25.0) / 50.0) + centre, minus one when v + 25.0 < 0   (:314-325, :741-750)
 __host__ __device__ inline int cube_coord(double v, int centre) {
@@ -455,17 +435,22 @@ __device__ __forceinline__ void mapper_prep_body(MapperState* S) {
 __global__ void k_mapper_prep(const __grid_constant__ Batch<MapperLane> B) { mapper_prep_body(B.a[blockIdx.z].S); }   // grid (1, 1, lanes)
 
 
-// transformUpdate (:148-152) ; refined pose out
-__device__ __forceinline__ void mapper_update_body(MapperState* S, double* __restrict__ out7) {
-  pdl_launch_dependents();
-  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
-  if (threadIdx.x || blockIdx.x) return;
-  const Qd qw{S->x[0], S->x[1], S->x[2], S->x[3]};
+// transformUpdate (:148-152): T_wmap_wodom from the map pose x (7 doubles: the frame's S->x, or an adopted recovery candidate)
+// and the frame's odometry pose
+__device__ __forceinline__ void transform_update(MapperState* S, const double* x) {
+  const Qd qw{x[0], x[1], x[2], x[3]};
   const Qd qo{S->q_wodom[0], S->q_wodom[1], S->q_wodom[2], S->q_wodom[3]};
   const Qd qn = qmul(qw, qinv(qo));
   double r[3]; qrot(qn, S->t_wodom, r);
   S->q_wmap_wodom[0] = qn.x; S->q_wmap_wodom[1] = qn.y; S->q_wmap_wodom[2] = qn.z; S->q_wmap_wodom[3] = qn.w;
-  S->t_wmap_wodom[0] = S->x[4] - r[0]; S->t_wmap_wodom[1] = S->x[5] - r[1]; S->t_wmap_wodom[2] = S->x[6] - r[2];
+  S->t_wmap_wodom[0] = x[4] - r[0]; S->t_wmap_wodom[1] = x[5] - r[1]; S->t_wmap_wodom[2] = x[6] - r[2];
+}
+// transformUpdate ; refined pose out
+__device__ __forceinline__ void mapper_update_body(MapperState* S, double* __restrict__ out7) {
+  pdl_launch_dependents();
+  pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
+  if (threadIdx.x || blockIdx.x) return;
+  transform_update(S, S->x);
   if (out7) for (int k = 0; k < 7; ++k) out7[k] = S->x[k];
   S->frames++;
 }
@@ -1303,6 +1288,50 @@ int map_rows_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* 
     B.a[l] = MapRowLane{lane_state(c, in[l]), in[l].localise ? L.locator->reg.summary : L.mapper->reg->summary, rows[l], in[l].localise ? max_score : 0};
   }
   LAUNCH(c, KID_MAP_ROWS, k_map_rows, dim3(1, 1, nb), 32, 0, B, std::min(c->cfg.outer_iters, 4));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
+namespace {
+// one record of k_recover_adopt: the localising lane's frame state, the row, the row's candidates and the best key k_reloc_topk
+// left for them
+struct RecoverAdopt {
+  MapperState* S;
+  MapRowRec* row;
+  const double* cand;
+  const unsigned long long* best;
+};
+
+// the last kernel of a recovery (recover.cu), one thread per record after k_reloc_topk: a triggered row records its best candidate
+// (key = score << 32 | ~h) and adopts it when it beats the row's score and holds accept_frac of its scoring points -- transformUpdate
+// at the candidate with the frame's odometry pose replaces the lane's T_wmap_wodom, which the lane's next frame hands off from.
+// The row's map pose and frame state are left as the frame wrote them.
+__global__ void __launch_bounds__(32) k_recover_adopt(const __grid_constant__ Batch<RecoverAdopt> B, int nb, float accept_frac) {
+  const int l = threadIdx.x;
+  if (l >= nb) return;
+  const RecoverAdopt& a = B.a[l];
+  MapRowRec* r = a.row;
+  if (!r->rec_triggered) return;
+  const unsigned long long key = a.best[0];
+  const int h = (int)~(unsigned)(key & 0xffffffffull), s = (int)(key >> 32);
+  const double* x = a.cand + (size_t)h * 7;
+  const bool adopt = s > r->score && (float)s >= accept_frac * (float)r->n_score;
+  r->rec_best = h;
+  r->rec_best_score = s;
+  r->rec_adopted = adopt;
+  for (int k = 0; k < 7; ++k) r->rec_pose[k] = x[k];
+  if (adopt) transform_update(a.S, x);
+}
+}  // namespace
+
+// k_recover_adopt over the nb localising records of the frame just issued (recover.cu, after the candidates' scores and best keys):
+// record l on its lane's locator, its row rows[l], candidates cand[l] and best key best[l]
+int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, const double* const* cand,
+                         const unsigned long long* const* best, float accept_frac) {
+  if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
+  Batch<RecoverAdopt> B = {};
+  for (int l = 0; l < nb; ++l) B.a[l] = RecoverAdopt{lane_state(c, in[l]), rows[l], cand[l], best[l]};
+  LAUNCH(c, KID_RECOVER_ADOPT, k_recover_adopt, 1, 32, 0, B, nb, accept_frac);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }

@@ -9,6 +9,9 @@
 //     map point, not the nearest one.  The count stays in a register; lane 0 writes it, and the warp keeps its 16 best keys
 //     (score << 32 | ~index) in lanes 0-15, merged per CTA at the end.
 //   * k_reloc_topk: one CTA merges the per-CTA lists into the 16 best keys: ranking by (score descending, index ascending).
+//   * both take one hypothesis set per record (RelocRec, blockIdx.z), with an optional device gate word: aloam_prior_relocalise is
+//     the one-record, ungated case; the recovery of localising lanes (recover.cu) scores every localising record of a stream step
+//     in one launch, gated on whether the record's row triggered.
 //   * refinement: locate_step_device (cubemap.cu) over K records, each on a locator of the relocaliser's own, from T_wmap_wodom =
 //     the hypothesis and the identity odometry pose: the first frame of a localising lane armed with that hypothesis.
 #include <climits>
@@ -17,9 +20,10 @@
 #include "grid.cuh"
 
 namespace {
-constexpr int kRelocWarps = 8;                 // warps (hypotheses in flight) per CTA of k_reloc_score
+constexpr int kRelocWarps = 8;                 // warps (hypotheses in flight) per CTA of k_reloc_score, 4 CTAs per SM (55 registers:
+                                               // without the bound ptxas aims for 5 and spills the key list)
 constexpr int kRelocStage = 2048;              // scoring points staged in shared memory at once (32 KB)
-constexpr int kTop = ALOAM_MAX_BATCH;          // best keys kept per CTA and returned: the largest K
+constexpr int kTop = kRelocTop;                // best keys kept per CTA and returned: the largest K
 constexpr int kMaxHyp = 1 << 24;
 }  // namespace
 
@@ -45,13 +49,19 @@ struct aloam::Relocaliser {
 
 namespace {
 
-// Scores of the n_hyp poses hyp[h] (7 doubles, q xyzw, t): score[h] = the scoring points of the stacks (sizes counts[0],
-// counts[1]; at most max_pts of each type) that have a map point of their type at float d2 < inlier_sq.  best (may be null): the
-// CTA's kTop best keys (score << 32 | ~h), descending, 0 where there are fewer, at best[kTop * blockIdx.x].
-__global__ void __launch_bounds__(kRelocWarps * 32) k_reloc_score(const double* __restrict__ hyp, int n_hyp, const Pt4* __restrict__ corner,
-                                                                  const Pt4* __restrict__ surf, const int* __restrict__ counts, int max_pts, float inlier_sq,
-                                                                  const __grid_constant__ PriorGrid G, int* __restrict__ score,
-                                                                  unsigned long long* __restrict__ best) {
+// Scores of record blockIdx.z's set (RelocRec): score[h] of its n_hyp poses hyp[h] (7 doubles, q xyzw, t) = the scoring points of
+// its stacks (sizes counts[0], counts[1]; at most max_pts of each type) that have a map point of their type at float d2 < inlier_sq.
+// part (may be null): the CTA's kTop best keys (score << 32 | ~h), descending, 0 where there are fewer, at part[kTop * blockIdx.x].
+// A gated set whose gate word is 0 leaves at once.
+__global__ void __launch_bounds__(kRelocWarps * 32, 4) k_reloc_score(const __grid_constant__ Batch<RelocRec> B, int max_pts, float inlier_sq,
+                                                                  const __grid_constant__ PriorGrid G) {
+  const RelocRec& a = B.a[blockIdx.z];
+  if (a.gate && !*a.gate) return;   // CTA-uniform
+  const double* __restrict__ hyp = a.hyp;
+  const Pt4* __restrict__ corner = a.stack[0];
+  const Pt4* __restrict__ surf = a.stack[1];
+  const int n_hyp = a.n_hyp;
+  const int* counts = a.counts;
   __shared__ float4 s_pts[kRelocStage];
   __shared__ unsigned long long s_top[kRelocWarps * kTop], s_out[kTop];
   const int n_c = counts[0], n_s = counts[1];
@@ -98,13 +108,14 @@ __global__ void __launch_bounds__(kRelocWarps * 32) k_reloc_score(const double* 
       }
     }
     if (!live) continue;
-    if (lane == 0) score[h] = cnt;
+    if (lane == 0) a.score[h] = cnt;
     // insert the key into the warp's descending list: the lanes that beat it stay, the others move one lane down
     const unsigned long long key = ((unsigned long long)(unsigned)cnt << 32) | (unsigned)~(unsigned)h;
     const int pos = __popc(__ballot_sync(0xffffffffu, top > key));
     const unsigned long long up = __shfl_up_sync(0xffffffffu, top, 1);
     if ((int)lane < kTop && (int)lane >= pos) top = (int)lane == pos ? key : up;
   }
+  unsigned long long* best = a.part;
   if (!best) return;
   // the CTA's kTop best of its warps' lists: a key's rank is the number of keys above it (keys are unique, 0 is no key)
   if ((int)lane < kTop) s_top[warp * kTop + lane] = top;
@@ -126,12 +137,17 @@ __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v)
   return v;
 }
 
-// one CTA of 1024: out[r] = the r-th largest of the n keys of part (0 where there are fewer), r < kTop -- kTop rounds of a block
-// maximum over the keys below the previous round's
-__global__ void __launch_bounds__(1024) k_reloc_topk(const unsigned long long* __restrict__ part, int n, unsigned long long* __restrict__ out) {
+// one CTA of 1024 per record (blockIdx.z): best[r] = the r-th largest of the n keys of its part (0 where there are fewer),
+// r < rounds <= kTop -- `rounds` rounds of a block maximum over the keys below the previous round's.  A gated record whose gate
+// word is 0 leaves at once.
+__global__ void __launch_bounds__(1024) k_reloc_topk(const __grid_constant__ Batch<RelocRec> B, int n, int rounds) {
+  const RelocRec& a = B.a[blockIdx.z];
+  if (a.gate && !*a.gate) return;   // CTA-uniform
+  const unsigned long long* __restrict__ part = a.part;
+  unsigned long long* __restrict__ out = a.best;
   __shared__ unsigned long long s_w[32];
   unsigned long long prev = ~0ull;
-  for (int r = 0; r < kTop; ++r) {
+  for (int r = 0; r < rounds; ++r) {
     unsigned long long m = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) { const unsigned long long k = part[i]; if (k < prev && k > m) m = k; }
     m = warp_max_u64(m);
@@ -146,6 +162,25 @@ __global__ void __launch_bounds__(1024) k_reloc_topk(const unsigned long long* _
     if (threadIdx.x == 0) out[r] = prev;
   }
 }
+
+}  // namespace
+
+void reloc_score_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int max_pts, float inlier_sq) {
+  LAUNCH(c, KID_RELOC, k_reloc_score, dim3(ctas, 1, nrec), kRelocWarps * 32, 0, B, max_pts, inlier_sq, prior_grid(c));
+}
+
+void reloc_topk_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int rounds) {
+  LAUNCH(c, KID_RELOC_TOPK, k_reloc_topk, dim3(1, 1, nrec), 1024, 0, B, ctas * kTop, rounds);
+}
+
+// one resident wave of k_reloc_score, at most one warp per hypothesis
+int reloc_score_ctas(aloam_ctx* c, int n_hyp) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reloc_score, kRelocWarps * 32, 0) != cudaSuccess) { cudaGetLastError(); per_sm = 1; }
+  return std::max(1, std::min(c->sms * std::max(per_sm, 1), (n_hyp + kRelocWarps - 1) / kRelocWarps));
+}
+
+namespace {
 
 void reloc_free(Relocaliser* R) {
   cudaFree(R->d_hyp);
@@ -187,11 +222,10 @@ int reloc_ensure(aloam_ctx* c, int k, int n_hyp) {
   return ALOAM_OK;
 }
 
-// k_reloc_score over n poses at d_pose on c->stream, best keys per CTA into part when it is set
-void reloc_score(aloam_ctx* c, const Relocaliser* R, const LocatorFrame& F, const double* d_pose, int n, const aloam_reloc_opts& o, int* d_score,
-                 unsigned long long* part, int ctas) {
-  LAUNCH(c, KID_RELOC, k_reloc_score, ctas, kRelocWarps * 32, 0, d_pose, n, F.stack[0], F.stack[1], F.counts, o.max_score_points, o.inlier_sq,
-         prior_grid(c), d_score, part);
+// the one-record, ungated set of aloam_prior_relocalise: n poses at d_pose scored on its stacks into d_score, best keys per CTA into
+// part when it is set
+RelocRec reloc_set(const Relocaliser* R, const LocatorFrame& F, const double* d_pose, int n, int* d_score, unsigned long long* part) {
+  return RelocRec{d_pose, n, {F.stack[0], F.stack[1]}, F.counts, d_score, part, R->d_best, nullptr};
 }
 
 }  // namespace
@@ -227,8 +261,10 @@ extern "C" int aloam_prior_relocalise(aloam_ctx* c, aloam_cloud_view less_sharp,
   const LocatorFrame F = locator_frame(R->loc[0]);
   // ---- coarse scores and the K best
   const int ctas = std::max(1, std::min(R->ctas, (n_hyp + kRelocWarps - 1) / kRelocWarps));
-  reloc_score(c, R, F, R->d_hyp, n_hyp, o, R->d_score, R->d_part, ctas);
-  LAUNCH(c, KID_RELOC_TOPK, k_reloc_topk, 1, 1024, 0, R->d_part, ctas * kTop, R->d_best);
+  Batch<RelocRec> B = {};
+  B.a[0] = reloc_set(R, F, R->d_hyp, n_hyp, R->d_score, R->d_part);
+  reloc_score_device(c, 1, B, ctas, o.max_score_points, o.inlier_sq);
+  reloc_topk_device(c, 1, B, ctas, kTop);
   CUDA_CHECK_RET(cudaMemcpyAsync(H->best, R->d_best, sizeof(H->best), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -243,7 +279,8 @@ extern "C" int aloam_prior_relocalise(aloam_ctx* c, aloam_cloud_view less_sharp,
   }
   // ---- refinement: one localising frame per winner, all in one batch, then the refined poses scored by the same kernel
   rc = locate_step_device(c, K, rec, lp, init, n_up_c, n_up_s); if (rc) return rc;
-  reloc_score(c, R, F, R->d_pose, K, o, R->d_rscore, nullptr, (K + kRelocWarps - 1) / kRelocWarps);
+  B.a[0] = reloc_set(R, F, R->d_pose, K, R->d_rscore, nullptr);
+  reloc_score_device(c, 1, B, (K + kRelocWarps - 1) / kRelocWarps, o.max_score_points, o.inlier_sq);
   CUDA_CHECK_RET(cudaMemcpyAsync(H->pose, R->d_pose, sizeof(double) * 7 * K, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(H->rscore, R->d_rscore, sizeof(int) * K, cudaMemcpyDeviceToHost, c->stream));
   for (int r = 0; r < K; ++r) CUDA_CHECK_RET(cudaMemcpyAsync(H->flags[r], locator_frame(R->loc[r]).flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));

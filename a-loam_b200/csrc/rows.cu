@@ -84,6 +84,7 @@ int aloam_set_map_rows(aloam_ctx* c, int on, float inlier_sq, int max_score_poin
   c->rows_on = on == 1;
   c->rows_inlier_sq = inlier_sq;
   c->rows_max_score = on ? max_score_points : 0;
+  if (c->rows_max_score == 0) c->rec_on = false;   // recovery reads the rows' scores (aloam_set_recovery)
   return ALOAM_OK;
 }
 

@@ -565,6 +565,56 @@ typedef struct aloam_map_row {
 } aloam_map_row;
 int aloam_set_map_rows(aloam_ctx* ctx, int on, float inlier_sq, int max_score_points);
 int aloam_map_rows(aloam_ctx* ctx, aloam_map_row* out, int rows);
+/* ---- recovery of localising lanes inside the mapped stream calls: when a localising row's score (above) falls below a threshold,
+ * the same stream scores pose candidates around the row's map pose on the device and, when one is clearly better, re-seats the
+ * lane's T_wmap_wodom.  The lane's next registered frame refines from there and its odometry goes on: no host round trip, no
+ * relocalise call, no re-arming and no START.
+ * aloam_set_recovery(ctx, 1, opts, deltas, n_delta) turns it on from the next mapped stream call; on = 0 turns it off (the default;
+ * nothing else is read): the stream calls then issue exactly what they issue without this feature.  Recovery needs scoring rows
+ * (aloam_set_map_rows with max_score_points > 0) and uses their inlier_sq and max_score_points; an aloam_set_map_rows call that
+ * turns recording or scoring off turns recovery off too.
+ *   - scope: ALOAM_ROW_LOCALISED rows (START rows included) of aloam_scan_stream_lanes with map_poses.  Mapping rows, skipped rows
+ *     and odometry-only lanes are never touched.
+ *   - trigger, per row: n_score > 0 and (float)score < opts->trigger_frac * (float)n_score (a float product).
+ *   - candidates: the n_delta relative poses deltas[h] = (q_d, t_d), 7 doubles each, normalised at set time as aloam_lane_localise
+ *     normalises.  With P = (q_P, t_P) the row's map pose, candidate h is q_h = normalise(q_d * q_P) (Eigen's product order,
+ *     normalised as aloam_lane_localise does, all double) and t_h = t_P + t_d: headings turn about the sensor's position and offsets
+ *     are in the map frame, as pose_grid(identity, 0, half, step, yaws) of the Python package lays them out.
+ *   - scores: candidate h's score is aloam_prior_relocalise's coarse score of (q_d * q_P, t_P + t_d) for the row's scan, on the same
+ *     scoring points as the row's score.  Candidates rank by (score descending, h ascending); `best` is the first.
+ *   - adoption: when best_score > score and (float)best_score >= opts->accept_frac * (float)n_score, the lane's T_wmap_wodom becomes
+ *     transformUpdate (laserMapping.cpp:148-152) at the best candidate with the row's odometry pose.  The row's map pose, its
+ *     aloam_map_row and its registered cloud stay as the frame made them; the lane's next registered frame hands off from the
+ *     adopted T, and skipped rows before it (cfg.mapping_skip_frame) compose with it.  The lane's odometry is untouched.
+ *   - cost while on: four launches per localising frame, whether or not a row triggers (k_recover_cand, k_reloc_score,
+ *     k_reloc_topk, k_recover_adopt), decided on the device without a host synchronisation; an untriggered row's CTAs leave at
+ *     once.  A triggered row scores its n_delta candidates at max_score_points points per type.
+ *   - buffers, created at set time and kept until aloam_destroy (a larger n_delta grows them): 16 lanes x n_delta candidates (56 B)
+ *     and scores (4 B), and per lane the CTA key lists of one resident wave of k_reloc_score.
+ *   - errors, each before anything changes: ALOAM_ERR_INVALID_ARG for on outside {0, 1}, n_delta outside 1 ... 65536, a NULL opts
+ *     or deltas, a non-finite delta or a zero quaternion, fractions that are not finite or lie outside [0, 1]; ALOAM_ERR_STATE
+ *     without scoring rows, on a rank of a sharded job and on an emulating context (aloam_comm_init and aloam_debug_shard_emulate
+ *     with world > 0 turn recovery off); ALOAM_ERR_CUDA when the buffers cannot be allocated.
+ * aloam_recovery_rows mirrors aloam_map_rows (same row count, scan-major order and state rules, readable after ALOAM_ERR_CAPACITY
+ * and ALOAM_ERR_COMM): one aloam_recovery_row per row of the last mapped stream call.  Rows that are not localised, that did not
+ * trigger, or of a call made with recovery off have triggered = adopted = 0, best = best_score = -1 and a zero pose.
+ * aloam_debug_recovery_scores copies the n = n_delta candidate scores of lane `lane`'s latest triggered row of the last mapped
+ * stream call: ALOAM_ERR_STATE when that call triggered no row of the lane (or recovery was set since), ALOAM_ERR_INVALID_ARG for
+ * a bad lane, NULL scores or n != n_delta. */
+typedef struct aloam_recovery_opts {
+  float trigger_frac;  /* 0 <= . <= 1: a localising row triggers when n_score > 0 and (float)score < trigger_frac * (float)n_score */
+  float accept_frac;   /* 0 <= . <= 1: the best candidate is adopted when best_score > score and (float)best_score >= accept_frac * (float)n_score */
+} aloam_recovery_opts;
+int aloam_set_recovery(aloam_ctx* ctx, int on, const aloam_recovery_opts* opts, const double* deltas, int n_delta);
+typedef struct aloam_recovery_row {
+  int triggered;     /* the row's score met the trigger and its candidates were scored */
+  int best;          /* index into deltas of the best candidate, -1 when not triggered */
+  int best_score;    /* its score, -1 when not triggered */
+  int adopted;       /* the lane's T_wmap_wodom was re-seated after this row */
+  double pose[7];    /* the best candidate's map pose (q xyzw, t); zeros when not triggered */
+} aloam_recovery_row;
+int aloam_recovery_rows(aloam_ctx* ctx, aloam_recovery_row* out, int rows);
+int aloam_debug_recovery_scores(aloam_ctx* ctx, int lane, int* scores, int n);
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
