@@ -37,6 +37,9 @@ def _lib():
         L.synth_pose.argtypes = [C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.synth_scan_seam.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
                                       C.POINTER(C.c_double), C.c_int, C.c_int, C.c_double, C.POINTER(C.c_float), C.c_int]
+        L.synth_scan_beams.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
+                                       C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int,
+                                       C.c_int, C.c_double, C.POINTER(C.c_float), C.POINTER(C.c_int), C.c_int]
         _LIB = L
     return _LIB
 
@@ -85,6 +88,48 @@ def scan_seam(sensor, index, cut=None, coverage=1.0, ring_offsets_deg=None, lase
     if n < 0:
         raise RuntimeError("synth_scan_seam failed: %d" % n)
     return out[:n].copy()
+
+
+def nominal_elevations(sensor):
+    """the beam elevations [deg] scan() fires: the centres of the reference's ring bins (HDL-64: shifted by -0.04 deg)"""
+    n_scans = SENSORS[sensor][0]
+    if n_scans == 16:
+        return np.array([-15.0 + 2.0 * k for k in range(16)])
+    if n_scans == 32:
+        return np.array([-92.0 / 3.0 + (k + 0.5) * 4.0 / 3.0 for k in range(32)])
+    return np.array([1.96 - k / 3.0 for k in range(32)] + [-8.87 - 0.5 * m for m in range(32)])
+
+
+def scan_beams(sensor, index, elevations_deg, z_offsets_m=None, cut=None, coverage=1.0, ring_offsets_deg=None,
+               laser_major=False, ccw=False, seed=BASE_SEED, n_az=None, noise=0.02, max_range=120.0, return_beams=False):
+    """scan_seam() fired by a beam table of its own: laser b at elevation elevations_deg[b] [deg], firing from (0, 0,
+    z_offsets_m[b]) [m] in the sensor frame (None: all at the origin).  The number of lasers may differ from the sensor's
+    scan-line count; the reference still bins every return by the sensor's ring formula, so lasers off the bin centres or off
+    the origin put returns on and across ring edges.  ring_offsets_deg has one value per laser.  With the nominal table
+    (nominal_elevations) and zero offsets the result is bit-identical to scan_seam().  return_beams: also the laser of
+    every return, (n,) int32.  Raises SeamTooClose like scan_seam()."""
+    n_scans, az, min_range = SENSORS[sensor][:3]
+    if n_az is not None:
+        az = n_az
+    el = np.ascontiguousarray(elevations_deg, np.float64)
+    nb = el.shape[0]
+    dz = None if z_offsets_m is None else np.ascontiguousarray(z_offsets_m, np.float64)
+    off = None if ring_offsets_deg is None else np.ascontiguousarray(ring_offsets_deg, np.float64)
+    assert el.ndim == 1 and nb > 0 and (dz is None or dz.shape == (nb,)) and (off is None or off.shape == (nb,))
+    start_col = 0.0 if cut is None else (math.pi - cut) * az / (2 * math.pi) - 0.37
+    n_col = int(round(coverage * az))
+    out = np.zeros((nb * n_col, 4), np.float32)
+    beams = np.zeros(nb * n_col, np.int32)
+    dp = C.POINTER(C.c_double)
+    n = _lib().synth_scan_beams(seed, n_scans, az, index, noise, max_range, start_col, n_col, nb, el.ctypes.data_as(dp),
+                                None if dz is None else dz.ctypes.data_as(dp), None if off is None else off.ctypes.data_as(dp),
+                                int(laser_major), int(ccw), min_range, out.ctypes.data_as(C.POINTER(C.c_float)),
+                                beams.ctypes.data_as(C.POINTER(C.c_int)), out.shape[0])
+    if n == -3:
+        raise SeamTooClose("scan_beams(%s, %d): a return lies on an azimuth threshold" % (sensor, index))
+    if n < 0:
+        raise RuntimeError("synth_scan_beams failed: %d" % n)
+    return (out[:n].copy(), beams[:n].copy()) if return_beams else out[:n].copy()
 
 
 def pose(index):

@@ -9,7 +9,9 @@
 //   HDL-64  scanRegistration.cpp:189-199  two blocks, keep id 0..50, -24.33 <= angle <= 2
 // Points are emitted in firing order (azimuth-major, clockwise so that -atan2(y,x) increases,
 // scanRegistration.cpp:141-153,208), no-return rays are dropped, range noise is Gaussian along
-// the ray (so the elevation angle -- hence the ring -- is unaffected by the noise).
+// the ray (so the elevation angle -- hence the ring -- is unaffected by the noise).  synth_scan_beams replaces the nominal
+// beams with a table of its own (calibration offsets, lasers off the sensor origin) whose returns do land on and across
+// the ring edges.
 //
 // World: an "urban canyon" made only of a ground plane and axis-aligned boxes, so every ray is
 // intersected in closed form.
@@ -173,11 +175,18 @@ int sensor_elevations(int n_scans, std::vector<double>& elev_deg) {
 //   ring_off   per-beam azimuth offset [deg] added to the firing azimuth (nullptr = none); the world is not moved
 //   laser_major  emit beam by beam (all columns of beam 0, then beam 1, ...) instead of column by column
 //   ccw        the firing azimuth rises with j (-atan2(y, x) falls) instead of falling
+//   n_beams, elev, z_off  a beam table instead of the sensor's nominal one (elev == nullptr): n_beams lasers (any count, not
+//              tied to n_scans) at elevations elev[b] [deg], each firing from (0, 0, z_off[b]) [m] in the sensor frame
+//              (z_off may be null).  A laser origin off the sensor origin makes the elevation seen from the origin -- the one
+//              the reference bins -- change with range, so one laser's returns can fall on either side of a ring edge.
 struct Layout {
   double start_col = 0.0;
   int n_col = 0;
   const double* ring_off = nullptr;
   int laser_major = 0, ccw = 0;
+  int n_beams = 0;
+  const double* elev = nullptr;
+  const double* z_off = nullptr;
 };
 
 // ring id of a return as scanRegistration.cpp:166-205 assigns it, or -1 when it drops the return
@@ -240,12 +249,18 @@ int check_seam_margins(const float* pts, int n, int n_scans, double minimum_rang
   return 0;
 }
 
+// beam_out (may be null): the beam index of every return written
 int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma, double max_range, const Layout& lay,
-             float* out, int capacity) {
+             float* out, int* beam_out, int capacity) {
   std::vector<double> elev;
   if (sensor_elevations(n_scans, elev) != 0) return -1;
+  if (lay.elev) {
+    if (lay.n_beams <= 0) return -2;
+    elev.assign(lay.elev, lay.elev + lay.n_beams);
+  }
+  const int nb = (int)elev.size();
   const int n_col = lay.n_col;
-  if (n_az <= 0 || n_col <= 0 || capacity < n_scans * n_col) return -2;
+  if (n_az <= 0 || n_col <= 0 || capacity < nb * n_col) return -2;
   World w = make_world(seed);
   Pose P = trajectory_pose(scan_index);
   // candidate boxes within range
@@ -256,9 +271,8 @@ int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_
     double dy = std::max({b.lo[1] - P.t[1], 0.0, P.t[1] - b.hi[1]});
     if (dx * dx + dy * dy < (max_range + 1) * (max_range + 1)) cand.push_back((int)i);
   }
-  std::vector<float> tmp((size_t)n_scans * n_col * 4);
-  std::vector<uint8_t> ok((size_t)n_scans * n_col, 0);
-  const int nb = n_scans;
+  std::vector<float> tmp((size_t)nb * n_col * 4);
+  std::vector<uint8_t> ok((size_t)nb * n_col, 0);
   unsigned nthreads = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
   auto work = [&](int j0, int j1) {
     for (int j = j0; j < j1; ++j) {
@@ -277,14 +291,25 @@ int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_
         double d[3] = {P.R[0] * ds[0] + P.R[1] * ds[1] + P.R[2] * ds[2],
                        P.R[3] * ds[0] + P.R[4] * ds[1] + P.R[5] * ds[2],
                        P.R[6] * ds[0] + P.R[7] * ds[1] + P.R[8] * ds[2]};
-        double t = cast(w, cand, P.t, d, 0.05, max_range);
-        double nz = rng.gauss();  // always drawn, so streams stay aligned
+        double t, r;
         size_t o = lay.laser_major ? (size_t)b * n_col + j : (size_t)j * nb + b;
-        if (t >= max_range) continue;
-        double r = t + noise_sigma * nz;
+        if (lay.elev) {  // the laser fires from (0, 0, dz) of the sensor frame
+          const double dz = lay.z_off ? lay.z_off[b] : 0.0;
+          const double org[3] = {P.t[0] + P.R[2] * dz, P.t[1] + P.R[5] * dz, P.t[2] + P.R[8] * dz};
+          t = cast(w, cand, org, d, 0.05, max_range);
+          const double nz = rng.gauss();
+          if (t >= max_range) continue;
+          r = t + noise_sigma * nz;
+          tmp[o * 4 + 2] = (float)(dz + r * ds[2]);
+        } else {
+          t = cast(w, cand, P.t, d, 0.05, max_range);
+          const double nz = rng.gauss();  // always drawn, so streams stay aligned
+          if (t >= max_range) continue;
+          r = t + noise_sigma * nz;
+          tmp[o * 4 + 2] = (float)(r * ds[2]);
+        }
         tmp[o * 4 + 0] = (float)(r * ds[0]);
         tmp[o * 4 + 1] = (float)(r * ds[1]);
-        tmp[o * 4 + 2] = (float)(r * ds[2]);
         tmp[o * 4 + 3] = 0.0f;
         ok[o] = 1;
       }
@@ -299,7 +324,11 @@ int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_
   for (auto& t : th) t.join();
   int n = 0;
   for (size_t o = 0; o < ok.size(); ++o)
-    if (ok[o]) { std::memcpy(out + (size_t)n * 4, &tmp[o * 4], 16); ++n; }
+    if (ok[o]) {
+      std::memcpy(out + (size_t)n * 4, &tmp[o * 4], 16);
+      if (beam_out) beam_out[n] = lay.laser_major ? (int)(o / n_col) : (int)(o % nb);
+      ++n;
+    }
   return n;
 }
 
@@ -321,7 +350,7 @@ int synth_scan(uint64_t seed, int n_scans, int n_az, int scan_index, double nois
                double max_range, float* out, int capacity) {
   Layout lay;
   lay.n_col = n_az;
-  return generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, capacity);
+  return generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, nullptr, capacity);
 }
 
 // The same scan cut and fired differently (see Layout): n_col columns from start_col, per-beam azimuth offsets ring_off_deg
@@ -332,7 +361,25 @@ int synth_scan_seam(uint64_t seed, int n_scans, int n_az, int scan_index, double
                     float* out, int capacity) {
   Layout lay;
   lay.start_col = start_col; lay.n_col = n_col; lay.ring_off = ring_off_deg; lay.laser_major = laser_major; lay.ccw = ccw;
-  const int n = generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, capacity);
+  const int n = generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, nullptr, capacity);
+  if (n < 0) return n;
+  const int rc = check_seam_margins(out, n, n_scans, minimum_range);
+  return rc ? rc : n;
+}
+
+// synth_scan_seam with a beam table of its own (see Layout): n_beams lasers at elev_deg[b] firing from (0, 0, z_off_m[b])
+// (z_off_m may be null), per-beam azimuth offsets ring_off_deg (n_beams entries, may be null).  The rings are still binned
+// by the reference's n_scans formula.  beam_out (may be null) receives the laser of every return.  Returns -3 like
+// synth_scan_seam.  Capacity: n_beams * n_col returns.
+int synth_scan_beams(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma, double max_range,
+                     double start_col, int n_col, int n_beams, const double* elev_deg, const double* z_off_m,
+                     const double* ring_off_deg, int laser_major, int ccw, double minimum_range, float* out, int* beam_out,
+                     int capacity) {
+  if (!elev_deg) return -2;
+  Layout lay;
+  lay.start_col = start_col; lay.n_col = n_col; lay.ring_off = ring_off_deg; lay.laser_major = laser_major; lay.ccw = ccw;
+  lay.n_beams = n_beams; lay.elev = elev_deg; lay.z_off = z_off_m;
+  const int n = generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, beam_out, capacity);
   if (n < 0) return n;
   const int rc = check_seam_margins(out, n, n_scans, minimum_range);
   return rc ? rc : n;
