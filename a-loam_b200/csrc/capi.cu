@@ -7,6 +7,7 @@
 #include <chrono>
 #include <cstring>
 #include <new>
+#include <utility>
 #include <vector>
 #include "../../include/aloam_b200.h"
 #include "kernels.h"
@@ -70,7 +71,7 @@ int aloam_reset_odometry(aloam_ctx* c) {
   }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   if (c->s_idx) CUDA_CHECK_RET(cudaStreamSynchronize(c->s_idx));   // an index build of the last synchronous call may still be running
-  c->frame = 0; c->cur = 0; c->have_last = false;
+  c->frame = 0; c->have_last = false;
   c->lanes_mode = false;
   for (Lane& L : c->lanes) L.sched = LaneSched();
   return ALOAM_OK;
@@ -498,7 +499,6 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
   if (c->frame == 0) { if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->flags = flags; stats->ms_total = ms; } }
   else fill_stats(c, stats, c->cfg.outer_iters, flags, ms);
-  c->cur = cur;
   c->frame++;
   return ALOAM_OK;
 }
@@ -525,18 +525,6 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
   return scan_to_pose_impl(c, d_raw, n, 4, q_w, t_w, stats);
 }
 
-// Row k * nb + l of a stream call: scan k of lane l, as the call will run it
-struct StreamRow {
-  int op;               // ALOAM_LANE_*
-  int scan;             // index of the scan in its trajectory (-1: an IDLE row)
-  bool mapped;          // a mapped call's scan that goes to the mapper (or its lane's locator); the others get a high-frequency pose
-  bool localise;        // a mapped call's scan that registers against the prior map
-  long long reg_begin;  // where the row's registered cloud begins in the sink: the sum of raws[r'].n over the mapped rows r' before it
-};
-// the rows of a stream call, built before anything is issued (room for all n in one allocation); reg_total: the points of every
-// mapped row's registered cloud
-struct StreamTable { std::vector<StreamRow> rows; long long reg_total = 0; explicit StreamTable(size_t n) { rows.reserve(n); } };
-
 // Appends the next row to *t, `op` on the lane whose schedule state is *s (its raw scan v), and applies the op to *s: a START
 // begins a trajectory at scan 0 -- in a mapped call (map) a mapped one that consumes the lane's arming, so that it localises --,
 // a SCAN continues it, an IDLE ends it.  The one place a lane's scan index advances.
@@ -558,59 +546,82 @@ static void add_row(const aloam_ctx* c, StreamTable* t, LaneSched* s, int op, co
   t->rows.push_back(r);
 }
 
-// Pipelined form of aloam_scan_to_pose over `nb` lanes: ring binning of step k+1 (s_exa), per-ring extraction (s_ext), compaction
-// + index build (s_idx) run concurrently with association + LM of step k (main stream) and the host->device copies of step k+2
-// (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on the rows t of its
-// lane schedule (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
-// (record i = lane act[i], which owns the buffers, pose slots and cube store); an all-idle step issues nothing.  reset_stores: a
-// START also resets its lane's cube store.  The rows that localise register against the prior map in one locate frame per step,
-// beside the mapping frame of the step's other lanes.  The caller has checked the views and the schedule, built its rows t and
-// created the cube stores and locators.
-static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const StreamTable& t, int n_scans, int nb, int device_resident, double* poses,
-                           double* map_poses, aloam_stats* stats_last, bool reset_stores) {
-  StreamGuard guard(c);
-  cudaStream_t s_main = c->stream;
-  const auto host_t0 = std::chrono::steady_clock::now();
-  // on any failure: drain everything, clear the sticky device errors and forget the odometry state (a partially issued
-  // pipeline cannot be rolled back scan by scan)
-  auto fail = [&](int code) {
-    sync_all_streams(c);
-    cudaGetLastError();
-    for (Lane& L : c->lanes) for (int b = 0; b < 3; ++b) cudaMemset(&(L.d_sc + b)->error, 0, 4);
-    c->stream = s_main;
-    aloam_reset_odometry(c);
-    return code;
-  };
-#define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return fail(ALOAM_ERR_CUDA); } } while (0)
+// What a stream call issues beside its odometry, fixed for the whole call from the context's settings
+struct StreamSwitches {
+  bool map;            // a mapped call: scan-to-map on s_map
   // registered clouds (aloam_set_registered_sink): every mapped row's ring-major cloud is stashed with its feature slot by stage C
   // and moved into the world by k_register_full after the row's mapper frame; without a sink none of this is issued
-  const bool sink = map_poses && c->reg_sink;
+  bool sink;
   // per-row records (aloam_set_map_rows): k_map_rows after every frame, k_track_score after every localising frame when scoring is
   // on; without recording none of this is issued
-  const bool rec = map_poses && c->rows_on;
-  const bool score = rec && c->rows_max_score > 0;
-  // recovery of localising lanes (aloam_set_recovery, recover.cu): four more launches after every scored localising frame
-  const bool recov = score && c->rec_on;
-  const size_t rows = (size_t)n_scans * nb;
-  if (map_poses) {
-    c->rec_call = recov;
-    recover_call_done(c, 0, nb);   // no lane's candidate scores belong to this call yet
-    c->reg_rows = -1;
-    c->reg_begin.resize(rows); c->reg_count.assign(rows, 0);
-    for (size_t r = 0; r < rows; ++r) c->reg_begin[r] = t.rows[r].reg_begin;
-    c->rows_n = -1;
-    if (rec) {
-      c->rows_kind.resize(rows);
-      for (size_t r = 0; r < rows; ++r) {
-        const StreamRow& w = t.rows[r];
-        c->rows_kind[r] = w.op == ALOAM_LANE_IDLE ? ALOAM_ROW_IDLE : !w.mapped ? ALOAM_ROW_SKIPPED : w.localise ? ALOAM_ROW_LOCALISED : ALOAM_ROW_MAPPED;
-      }
+  bool rec, score;
+  bool recov;          // recovery of localising lanes (aloam_set_recovery, recover.cu): four more launches after every scored localising frame
+  bool reset_stores;   // a START also resets its lane's cube store
+  StreamSwitches(const aloam_ctx* c, bool mapped, bool reset)
+      : map(mapped), sink(map && c->reg_sink), rec(map && c->rows_on), score(rec && c->rows_max_score > 0), recov(score && c->rec_on), reset_stores(reset) {}
+};
+#define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return ALOAM_ERR_CUDA; } } while (0)
+
+// ---- scan-to-map of one step on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose
+//      go to the mapping stage on the device -- what the reference ships through /laser_cloud_corner_last, /laser_cloud_surf_last
+//      and /laser_odom_to_init (laserOdometry.cpp:570-591 -> laserMapping.cpp:278-288) never leaves HBM.
+//      One frame covers every mapped lane of the step: each launch of it serves all of them, each with its own cube store; the
+//      step's mapped lanes that localise go to one locate frame against the prior map instead (no cube store).  Scan j of a
+//      trajectory is mapped when j % mapping_skip_frame == 0 (laserOdometry.cpp:570); the others get the high-frequency pose of
+//      laserMapping.cpp:197-229 from one k_mapper_high_freq launch.  A step that maps no lane issues no frame and does not record
+//      ev_mapdone[cur], so the next writer of this feature slot (stage C, four steps on) waits only on a frame that read it.
+// The step's rows are row[0 .. nb-1], rows r0 .. r0+nb-1 of the call; act[0 .. na-1] its non-idle lanes, cur its feature slot and
+// nmax its largest scan.  Leaves c->stream on s_map; returns the error the call fails with.
+static int map_stage(aloam_ctx* c, const StreamSwitches& w, const StreamRow* row, size_t r0, const int* act, int na, int cur, int nmax) {
+  STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
+  c->stream = c->s_map;
+  MapperIn fr[3][ALOAM_MAX_BATCH];   // the records of the mapping frame, of the locate frame and of the high-frequency poses
+  int n_fr[3] = {0, 0, 0};
+  for (int i = 0; i < na; ++i) {
+    const int l = act[i];
+    const FeatBuf& fc = c->lanes[l].feat[cur]; const size_t slot = (r0 + l) * 7;
+    const int g = !row[l].mapped ? 2 : row[l].localise;
+    fr[g][n_fr[g]++] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
+                                w.reset_stores && row[l].op == ALOAM_LANE_START, row[l].localise};
+  }
+  const int n_upper_c = 64 * kMaxLessSharpPerRing, n_upper_s = std::min(nmax, c->max_points);
+  for (int loc = 0; loc < 2; ++loc) {   // the mapping frame, then the locate frame, each followed by its rows and registered clouds
+    const MapperIn* in = fr[loc]; const int n = n_fr[loc];
+    if (n == 0) continue;
+    MapRowRec* rows[ALOAM_MAX_BATCH] = {};                    // the row slots of the frame's records
+    const Pt4* src[ALOAM_MAX_BATCH] = {}; const int* nf[ALOAM_MAX_BATCH] = {}; Pt4* dst[ALOAM_MAX_BATCH] = {};   // their registered clouds
+    Locator* lp[ALOAM_MAX_BATCH] = {}; const double* init[ALOAM_MAX_BATCH] = {};                                    // their locators
+    for (int j = 0; j < n; ++j) {
+      Lane& L = c->lanes[in[j].lane];
+      if (w.rec) rows[j] = c->d_rows + r0 + in[j].lane;
+      if (w.sink) { src[j] = L.feat[cur].full; nf[j] = c->d_scan_nfull + r0 + in[j].lane; dst[j] = c->reg_sink + row[in[j].lane].reg_begin; }
+      lp[j] = L.locator; init[j] = L.init;
     }
+    int rc = loc ? locate_step_device(c, n, in, lp, init, n_upper_c, n_upper_s) : mapper_step_device(c, n, in, n_upper_c, n_upper_s);
+    if (rc) return rc;
+    if (w.rec) { rc = map_rows_device(c, n, in, rows, loc ? c->rows_max_score : 0); if (rc) return rc; }
+    if (loc && w.score) { rc = track_score_device(c, n, in, rows, n_upper_c, n_upper_s); if (rc) return rc; }
+    if (loc && w.recov) { rc = recover_device(c, n, in, rows); if (rc) return rc; }
+    for (int j = 0; loc && j < n; ++j) c->lanes[in[j].lane].window = true;
+    // /velodyne_cloud_registered of the frame's rows, before the lanes' next frame replaces the refined pose
+    if (w.sink) { rc = mapper_register_full_device(c, n, in, src, nf, dst, nmax); if (rc) return rc; }
+  }
+  if (n_fr[0] + n_fr[1] > 0) STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
+  return n_fr[2] > 0 ? mapper_high_freq_device(c, n_fr[2], fr[2]) : ALOAM_OK;
+}
+
+// Issues every step of a stream call on the rows t, drains it and checks what its scans left on the device (scan_stream_run);
+// last_op: the last non-idle op of every lane in this call (IDLE: none).  Returns the error the call fails with.
+static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const StreamTable& t, int n_scans, int nb, int device_resident,
+                        const StreamSwitches& w, int* last_op) {
+  const cudaStream_t s_main = c->stream;
+  const auto host_t0 = std::chrono::steady_clock::now();
+  if (w.map) {
     for (int l = 0; l < nb; ++l) {   // the mappers' error bits of this call (a lane that only localises has no cube store)
       if (c->lanes[l].mapper) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
       if (c->lanes[l].locator) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
     }
-    const int rc = peer_err_reset(c); if (rc) return fail(rc);
+    const int rc = peer_err_reset(c); if (rc) return rc;
   }
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
   // everything issued on the main stream before this call (reset, earlier calls) is ordered before the side streams.
@@ -620,7 +631,6 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
   const float* d_raw[ALOAM_MAX_BATCH];      // per record
   int ns[ALOAM_MAX_BATCH];
   int act[ALOAM_MAX_BATCH], scanning[ALOAM_MAX_BATCH], starting[ALOAM_MAX_BATCH];   // lanes of the step: all, registering, initialising
-  int last_op[ALOAM_MAX_BATCH] = {};        // the last non-idle op of every lane in this call (IDLE: none)
   int issued = 0;
   for (int k = 0; k < n_scans; ++k) {
     const StreamRow* row = t.rows.data() + (size_t)k * nb;   // the step's rows, one per lane
@@ -653,7 +663,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     // ---- stage A (ring binning) on s_exa: needs full[b] free, i.e. stage B of scan k-2 done
     STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_b[b], 0));
     // with a sink, full[b] is also read by the stash copy of stage C (which waits on the mapper frame four steps back)
-    if (sink) STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_stash[b], 0));
+    if (w.sink) STREAM_TRY(cudaStreamWaitEvent(c->s_exa, c->ev_stash[b], 0));
     c->stream = c->s_exa;
     // A START re-arms the lane's ScanScalars slot (k_ring_scan arms it only for a lane that ran the step before) and, below, resets its pose.
     // At a lockstep call's first step these copies change nothing: k_ring_scan armed the slot with d_sc_init's four fields, start_ori /
@@ -662,7 +672,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
       STREAM_TRY(cudaMemcpyAsync(c->lanes[starting[i]].d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->s_exa));
     int sc_slot = 0;
     int rc = run_features_a(c, na, act, d_raw, ns, device_resident ? 4 : rv[act[0]].stride_floats, b, &sc_slot, c->d_scan_nfull + (size_t)k * nb);
-    if (rc) return fail(rc);
+    if (rc) return rc;
     if (!device_resident) STREAM_TRY(cudaEventRecord(c->ev_rawfree[b], c->s_exa));
     STREAM_TRY(cudaEventRecord(c->ev_a[b], c->s_exa));
     // ---- stage B (k_ring_features, the longest kernel) on s_ext: needs stage A of this scan and the staging set b free
@@ -671,7 +681,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_a[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_ext, c->ev_cmp[b], 0));
     rc = run_features_b1(c, na, act, b, sc_slot);
-    if (rc) return fail(rc);
+    if (rc) return rc;
     STREAM_TRY(cudaEventRecord(c->ev_b[b], c->s_ext));
     // ---- stage C on s_idx: ring-ordered compaction into feat[f % kFeatSlots] -- that slot was last read by the odometry
     //      of frame f - (kFeatSlots - 1) as its "last" clouds -- then the search index over its less-sharp / less-flat
@@ -680,13 +690,13 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_b[b], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_odo[(f + 1) % kFeatSlots], 0));
     STREAM_TRY(cudaStreamWaitEvent(c->s_idx, c->ev_mapdone[cur], 0));   // the last mapper frame that read this slot (of frame f - kFeatSlots at the latest) is done
-    if (sink) {   // the ring-major cloud of every mapped row goes with the slot until its mapper frame has registered it
+    if (w.sink) {   // the ring-major cloud of every mapped row goes with the slot until its mapper frame has registered it
       for (int i = 0; i < na; ++i)
         if (row[act[i]].mapped) { Lane& L = c->lanes[act[i]]; STREAM_TRY(cudaMemcpyAsync(L.feat[cur].full, L.d_full[b], (size_t)ns[i] * sizeof(Pt4), cudaMemcpyDeviceToDevice, c->s_idx)); }
       STREAM_TRY(cudaEventRecord(c->ev_stash[b], c->s_idx));
     }
     rc = run_features_b2(c, na, act, b, cur, false);
-    if (rc) return fail(rc);
+    if (rc) return rc;
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
     STREAM_TRY(cudaEventRecord(c->ev_feat[cur], c->s_idx));
     run_grid_build(c, na, act, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
@@ -705,69 +715,11 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
     }
     if (n_scan > 0) run_register(c, n_scan, scanning, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots, nullptr);
     STREAM_TRY(cudaEventRecord(c->ev_odo[cur], s_main));
-    if (map_poses) {
-      // ---- scan-to-map on s_map (laserMapping.cpp process()): the scan's less-sharp / less-flat clouds and its odometry pose go
-      //      to the mapping stage on the device -- what the reference ships through /laser_cloud_corner_last, /laser_cloud_surf_last
-      //      and /laser_odom_to_init (laserOdometry.cpp:570-591 -> laserMapping.cpp:278-288) never leaves HBM
-      //      One frame covers every mapped lane of the step: each launch of it serves all of them, each with its own cube store.
-      //      Scan j of a trajectory is mapped when j % mapping_skip_frame == 0 (laserOdometry.cpp:570); the others get the
-      //      high-frequency pose of laserMapping.cpp:197-229 from one k_mapper_high_freq launch.  A step that maps no lane issues
-      //      no frame and does not record ev_mapdone[cur], so the next writer of this feature slot (stage C, four steps on) waits
-      //      only on a frame that read it.
-      STREAM_TRY(cudaStreamWaitEvent(c->s_map, c->ev_odo[cur], 0));
-      c->stream = c->s_map;
-      //      The step's registered lanes that localise go to one locate frame against the prior map instead (no cube store).
-      MapperIn in[ALOAM_MAX_BATCH], loc[ALOAM_MAX_BATCH], hf[ALOAM_MAX_BATCH];
-      int n_map = 0, n_loc = 0, n_hf = 0;
-      for (int i = 0; i < na; ++i) {
-        const int l = act[i];
-        const FeatBuf& fc = c->lanes[l].feat[cur];
-        const size_t slot = ((size_t)k * nb + l) * 7;
-        const MapperIn r{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
-                         reset_stores && row[l].op == ALOAM_LANE_START, row[l].localise};
-        if (!row[l].mapped) hf[n_hf++] = r; else if (row[l].localise) loc[n_loc++] = r; else in[n_map++] = r;
-      }
-      // /velodyne_cloud_registered of a frame's rows, before the lanes' next frame replaces the refined pose
-      auto register_rows = [&](const MapperIn* fr, int n) {
-        const Pt4* src[ALOAM_MAX_BATCH]; const int* nf[ALOAM_MAX_BATCH]; Pt4* dst[ALOAM_MAX_BATCH];
-        for (int j = 0; j < n; ++j) {
-          const int l = fr[j].lane;
-          src[j] = c->lanes[l].feat[cur].full; nf[j] = c->d_scan_nfull + (size_t)k * nb + l; dst[j] = c->reg_sink + row[l].reg_begin;
-        }
-        return mapper_register_full_device(c, n, fr, src, nf, dst, nmax);
-      };
-      // the row slots of a frame's records
-      auto row_slots = [&](const MapperIn* fr, int n, MapRowRec** out) { for (int j = 0; j < n; ++j) out[j] = c->d_rows + (size_t)k * nb + fr[j].lane; };
-      MapRowRec* slots_rec[ALOAM_MAX_BATCH];
-      if (n_map > 0) {
-        rc = mapper_step_device(c, n_map, in, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
-        if (rc) return fail(rc);
-        if (rec) { row_slots(in, n_map, slots_rec); rc = map_rows_device(c, n_map, in, slots_rec, 0); if (rc) return fail(rc); }
-        if (sink) { rc = register_rows(in, n_map); if (rc) return fail(rc); }
-      }
-      if (n_loc > 0) {
-        Locator* lp[ALOAM_MAX_BATCH];
-        const double* init[ALOAM_MAX_BATCH];
-        for (int j = 0; j < n_loc; ++j) { Lane& L = c->lanes[loc[j].lane]; lp[j] = L.locator; init[j] = L.init; }
-        rc = locate_step_device(c, n_loc, loc, lp, init, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
-        if (rc) return fail(rc);
-        if (rec) {
-          row_slots(loc, n_loc, slots_rec);
-          rc = map_rows_device(c, n_loc, loc, slots_rec, c->rows_max_score); if (rc) return fail(rc);
-          if (score) { rc = track_score_device(c, n_loc, loc, slots_rec, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points)); if (rc) return fail(rc); }
-          if (recov) { rc = recover_device(c, n_loc, loc, slots_rec); if (rc) return fail(rc); }
-        }
-        for (int j = 0; j < n_loc; ++j) c->lanes[loc[j].lane].window = true;
-        if (sink) { rc = register_rows(loc, n_loc); if (rc) return fail(rc); }
-      }
-      if (n_map + n_loc > 0) STREAM_TRY(cudaEventRecord(c->ev_mapdone[cur], c->s_map));
-      if (n_hf > 0) {
-        rc = mapper_high_freq_device(c, n_hf, hf);
-        if (rc) return fail(rc);
-      }
+    if (w.map) {
+      rc = map_stage(c, w, row, (size_t)k * nb, act, na, cur, nmax);
+      if (rc) return rc;
       c->stream = s_main;
     }
-    c->cur = cur;
     c->frame++;
   }
   if (getenv("ALOAM_DEBUG_TIMING")) fprintf(stderr, "[aloam_b200] scan_stream: host issued %d x %d scans in %.1f us (%.1f us / step)\n", n_scans, nb,
@@ -775,17 +727,17 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
       std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - host_t0).count() / n_scans);
   const size_t total = (size_t)n_scans * nb;
   STREAM_TRY(cudaMemcpyAsync(c->h_poses, c->d_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
-  if (map_poses) {
+  if (w.map) {
     STREAM_TRY(cudaEventRecord(c->ev_mapend, c->s_map));   // the last mapper frame and the last high-frequency poses
     STREAM_TRY(cudaStreamWaitEvent(s_main, c->ev_mapend, 0));
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
-    if (rec) STREAM_TRY(cudaMemcpyAsync(c->h_rows, c->d_rows, total * sizeof(MapRowRec), cudaMemcpyDeviceToHost, s_main));
+    if (w.rec) STREAM_TRY(cudaMemcpyAsync(c->h_rows, c->d_rows, total * sizeof(MapRowRec), cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) {
       c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
       if (c->lanes[l].mapper) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
       if (c->lanes[l].locator) STREAM_TRY(cudaMemcpyAsync(&c->pin->locate_err_lane[l], locator_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
     }
-    const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return fail(rc);
+    const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;
   }
   for (int l = 0; l < nb; ++l) {
     STREAM_TRY(cudaMemcpyAsync(c->h_summary + 4 * l, c->lanes[l].d_summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, s_main));
@@ -797,13 +749,46 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
   STREAM_TRY(cudaMemcpyAsync(c->h_scan_nfull, c->d_scan_nfull, total * 4, cudaMemcpyDeviceToHost, s_main));
   sync_all_streams(c);
   STREAM_TRY(cudaGetLastError());
-#undef STREAM_TRY
   prof_collect(c);
   for (int l = 0; l < nb; ++l)
     for (int b = 0; b < 3; ++b)
-      if (c->h_sc[3 * l + b].error) return fail(c->h_sc[3 * l + b].error);
+      if (c->h_sc[3 * l + b].error) return c->h_sc[3 * l + b].error;
   for (size_t i = 0; i < total; ++i)   // (an idle entry has no scan)
-    if (t.rows[i].op != ALOAM_LANE_IDLE && c->h_scan_nfull[i] <= 0) return fail(ALOAM_ERR_EMPTY_CLOUD);   // scanRegistration.cpp:136-137 left nothing of this scan
+    if (t.rows[i].op != ALOAM_LANE_IDLE && c->h_scan_nfull[i] <= 0) return ALOAM_ERR_EMPTY_CLOUD;   // scanRegistration.cpp:136-137 left nothing of this scan
+  return ALOAM_OK;
+}
+#undef STREAM_TRY
+
+// Pipelined form of aloam_scan_to_pose over `nb` lanes: ring binning of step k+1 (s_exa), per-ring extraction (s_ext), compaction
+// + index build (s_idx) run concurrently with association + LM of step k (main stream) and the host->device copies of step k+2
+// (s_h2d) -- the overlap the reference gets from its three ROS processes.  Every stream call runs this driver on the rows t of its
+// lane schedule (scan-major as raws and poses: entry k * nb + b).  A step packs its non-idle lanes into records 0 .. na-1 of every launch
+// (record i = lane act[i], which owns the buffers, pose slots and cube store); an all-idle step issues nothing.  reset_stores: a
+// START also resets its lane's cube store.  The rows that localise register against the prior map in one locate frame per step,
+// beside the mapping frame of the step's other lanes.  The caller has checked the views and the schedule, built its rows t and
+// created the cube stores and locators.
+static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, StreamTable table, int n_scans, int nb, int device_resident, double* poses,
+                           double* map_poses, aloam_stats* stats_last, bool reset_stores) {
+  StreamGuard guard(c);
+  const StreamSwitches w(c, map_poses != nullptr, reset_stores);
+  MappedCall& M = c->last_mapped;
+  if (w.map) {   // this call's rows replace the last mapped call's, unreadable until the call has drained
+    M.table = std::move(table); M.n_scans = n_scans; M.nb = nb;
+    M.registered = M.records = false; M.recovered = w.recov;
+    recover_call_done(c);   // no lane's candidate scores belong to this call yet
+  }
+  const StreamTable& t = w.map ? M.table : table;
+  int last_op[ALOAM_MAX_BATCH] = {};
+  if (const int rc = stream_issue(c, raws, t, n_scans, nb, device_resident, w, last_op)) {
+    // drain everything, clear the sticky device errors and forget the odometry state: a partial pipeline cannot be rolled back
+    sync_all_streams(c);
+    cudaGetLastError();
+    for (Lane& L : c->lanes) for (int b = 0; b < 3; ++b) cudaMemset(&(L.d_sc + b)->error, 0, 4);
+    c->stream = guard.main;
+    aloam_reset_odometry(c);
+    return rc;
+  }
+  const size_t total = (size_t)n_scans * nb;
   std::memcpy(poses, c->h_poses, total * 56);
   if (map_poses) std::memcpy(map_poses, c->h_poses + (size_t)kMaxStreamScans * 7, total * 56);
   for (size_t i = 0; i < total; ++i)
@@ -817,14 +802,12 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, const Str
       else fill_stats_from(c->h_summary + 4 * l, &stats_last[l], c->cfg.outer_iters, 0, ms);
     }
   }
-  if (map_poses) {   // the registered rows of this call (count 0 without a sink)
-    for (size_t r = 0; r < rows; ++r) c->reg_count[r] = sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
-    c->reg_rows = (int)rows;
-    if (rec) c->rows_n = (int)rows;   // readable after ALOAM_ERR_CAPACITY and ALOAM_ERR_COMM below: they name the row that was hit
-    if (rec) recover_call_done(c, n_scans, nb);
-  }
-  // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
-  if (map_poses) {
+  if (w.map) {   // the call's rows are readable (after ALOAM_ERR_CAPACITY and ALOAM_ERR_COMM below too: they name the row that was hit)
+    M.reg_count.resize(total);
+    for (size_t r = 0; r < total; ++r) M.reg_count[r] = w.sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
+    M.registered = true; M.records = w.rec;
+    recover_call_done(c);
+    // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
     c->pin->mapper_err = 0;
     for (int l = 0; l < nb; ++l) c->pin->mapper_err |= c->pin->mapper_err_lane[l] | c->pin->locate_err_lane[l];
     if (c->pin->mapper_err & 1) return ALOAM_ERR_CAPACITY;
@@ -858,7 +841,7 @@ static int scan_stream_lockstep(aloam_ctx* c, const aloam_cloud_view* raws, int 
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   for (int l = 0; map_poses && l < nb; ++l) { int rc = mapper_ensure(c, l); if (rc) return rc; }   // creates the cube stores this call needs
   for (int l = 0; l < nb; ++l) c->lanes[l].sched.scan = s[l].scan;
-  return scan_stream_run(c, raws, t, n_scans, nb, device_resident, poses, map_poses, stats_last, false);
+  return scan_stream_run(c, raws, std::move(t), n_scans, nb, device_resident, poses, map_poses, stats_last, false);
 }
 
 int aloam_scan_stream(aloam_ctx* c, const aloam_cloud_view* raws, int n_scans, int device_resident, double* poses, aloam_stats* stats_last) {
@@ -920,7 +903,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   }
   if (map && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (run_err) { if (map) c->rows_n = -1; aloam_reset_odometry(c); return run_err; }
+  if (run_err) { if (map) c->last_mapped.records = false; aloam_reset_odometry(c); return run_err; }
   for (int l = 0; map && l < batch; ++l) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
     int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
     rc = maps[l] || !localises[l] ? mapper_ensure(c, l) : ALOAM_OK; if (rc) return rc;
@@ -928,7 +911,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   // committed before anything is issued: a later failure ends in aloam_reset_odometry, a key overflow leaves the lanes running
   c->lanes_mode = true;
   for (int l = 0; l < c->n_lanes; ++l) c->lanes[l].sched = s[l];
-  return scan_stream_run(c, raws, t, n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
+  return scan_stream_run(c, raws, std::move(t), n_scans, batch, device_resident, odom_poses, map_poses, stats_last, true);
 }
 
 int aloam_set_registered_sink(aloam_ctx* c, float* data, long long capacity) {
@@ -952,9 +935,9 @@ int aloam_set_registered_sink(aloam_ctx* c, float* data, long long capacity) {
 
 int aloam_registered_rows(aloam_ctx* c, long long* begin, int* count, int rows) {
   if (!c || rows < 0 || (rows > 0 && (!begin || !count))) return ALOAM_ERR_INVALID_ARG;
-  if (c->reg_rows < 0) return ALOAM_ERR_STATE;
-  if (rows != c->reg_rows) return ALOAM_ERR_INVALID_ARG;
-  for (int r = 0; r < rows; ++r) { begin[r] = c->reg_begin[r]; count[r] = c->reg_count[r]; }
+  const MappedCall& M = c->last_mapped;
+  if (const int rc = M.check(M.registered, rows)) return rc;
+  for (int r = 0; r < rows; ++r) { begin[r] = M.table.rows[r].reg_begin; count[r] = M.reg_count[r]; }
   return ALOAM_OK;
 }
 

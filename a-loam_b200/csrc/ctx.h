@@ -116,6 +116,31 @@ struct FeatBuf {
   Pt4* full = nullptr;             // ring-major cloud of a mapped scan, kept for its registered cloud (created by aloam_set_registered_sink)
 };
 
+// Row k * nb + l of a stream call: scan k of lane l, as the call will run it
+struct StreamRow {
+  int op;               // ALOAM_LANE_*
+  int scan;             // index of the scan in its trajectory (-1: an IDLE row)
+  bool mapped;          // a mapped call's scan that goes to the mapper (or its lane's locator); the others get a high-frequency pose
+  bool localise;        // a mapped call's scan that registers against the prior map
+  long long reg_begin;  // where the row's registered cloud begins in the sink: the sum of raws[r'].n over the mapped rows r' before it
+};
+// the rows of a stream call, built before anything is issued (room for all n in one allocation); reg_total: the points of every
+// mapped row's registered cloud
+struct StreamTable { std::vector<StreamRow> rows; long long reg_total = 0; explicit StreamTable(size_t n = 0) { rows.reserve(n); } };
+// the ALOAM_ROW_* of a row (aloam_map_row::kind)
+inline int row_kind(const StreamRow& r) { return r.op == ALOAM_LANE_IDLE ? ALOAM_ROW_IDLE : !r.mapped ? ALOAM_ROW_SKIPPED : r.localise ? ALOAM_ROW_LOCALISED : ALOAM_ROW_MAPPED; }
+// The last mapped stream call, all its readers read: scan_stream_run takes over its rows and clears the flags before it issues
+// anything, sets them once the call has drained; a mapped lanes call refused with a scan that cannot run clears `records`.
+struct MappedCall {
+  StreamTable table; int n_scans = 0, nb = 0;   // n_scans x nb rows
+  std::vector<int> reg_count;    // per row: points of its registered cloud in the sink (0 without a sink or for a row not mapped)
+  bool registered = false;       // aloam_registered_rows may read the table and reg_count
+  bool records = false;          // aloam_map_rows and aloam_recovery_rows may read the table and the pinned row table h_rows
+  bool recovered = false;        // the call ran recovery (aloam_set_recovery)
+  // a reader's check: ALOAM_ERR_STATE while its flag is off, ALOAM_ERR_INVALID_ARG for a row count other than the call's
+  int check(bool readable, int rows) const { return !readable ? ALOAM_ERR_STATE : rows != n_scans * nb ? ALOAM_ERR_INVALID_ARG : ALOAM_OK; }
+};
+
 // Where a lane is in the schedule of the stream calls.  A lane of aloam_scan_stream_lanes runs from its START to the step before
 // its next IDLE; `mapped` is the mode of the call that started it; `localising`: the trajectory it runs (or ran last) registers
 // against the prior map, fixed at its START; `armed`: aloam_lane_localise has armed its next mapped START with Lane::init.
@@ -235,28 +260,21 @@ struct aloam_ctx {
               ev_a[2] = {}, ev_b[2] = {}, ev_cmp[2] = {}, ev_mapend = nullptr;
   // registered full-resolution clouds of the mapped streams (aloam_set_registered_sink): the sink (device or page-locked host memory,
   // written through its device address) and its capacity in points; ev_stash[b]: the copy of ring-major cloud b into the feature
-  // slot's stash is done (created with the stash).  reg_begin / reg_count: rows of the last mapped stream call, reg_rows of them.
+  // slot's stash is done (created with the stash).  The rows' places in the sink are in last_mapped.
   Pt4* reg_sink = nullptr;
   long long reg_cap = 0;
   cudaEvent_t ev_stash[2] = {};
-  std::vector<long long> reg_begin;
-  std::vector<int> reg_count;
-  int reg_rows = -1;
-  // per-row records of the mapped stream calls (aloam_set_map_rows, rows.cu): the setting, the device row table and its pinned
-  // copy ([kMaxStreamScans] each, created by the first call that turns recording on), and the kinds (ALOAM_ROW_*) of the last
-  // mapped stream call's rows -- rows_n of them, -1 when that call's rows cannot be read
+  // per-row records of the mapped stream calls (aloam_set_map_rows, rows.cu): the setting, and the device row table and its pinned
+  // copy ([kMaxStreamScans] each, created by the first call that turns recording on)
   bool rows_on = false;
   float rows_inlier_sq = 1.f;
   int rows_max_score = 0;
   MapRowRec* d_rows = nullptr;
   MapRowRec* h_rows = nullptr;
-  std::vector<signed char> rows_kind;
-  int rows_n = -1;
-  // recovery of localising lanes (aloam_set_recovery, recover.cu): on only while rows are scored; its buffers, created by the first
-  // call that turns it on; whether the last mapped stream call ran it
+  // recovery of localising lanes (aloam_set_recovery, recover.cu): on only while rows are scored; its buffers, created on first use
   bool rec_on = false;
   Recovery* recover = nullptr;
-  bool rec_call = false;
+  MappedCall last_mapped;   // the rows of the last mapped stream call and which of its readers may read them
   // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
   // memory, created on first use
   ExportLayout* d_export_layout = nullptr;
@@ -282,7 +300,6 @@ struct aloam_ctx {
   // state (all lanes advance in lockstep)
   int parity = 0;         // ScanScalars slot of the next scan
   int frame = 0;          // fused pipeline: scans seen
-  int cur = 0;            // fused pipeline: feat[] slot of the most recent scan
   bool have_last = false; // API path: set_last called
   int last_n_full = 0;
   // aloam_scan_stream_lanes: once used, the lockstep calls are refused until aloam_reset_odometry, which clears it and every
@@ -349,8 +366,6 @@ void launch_ex(aloam_ctx* c, int kid, K kernel, dim3 grid, dim3 block, size_t sm
   prof_end(c);
 }
 
-#define LAUNCH_PDL(c, kid, kernel, grid, block, smem, ...) launch_ex(c, kid, kernel, dim3(grid), dim3(block), smem, 1, true, __VA_ARGS__)
-
 // the LM kernel runs as one thread-block cluster per trajectory (distributed-shared-memory reduction, see lm.cu)
 constexpr int kLmCluster = 8;
 
@@ -390,9 +405,9 @@ int reloc_score_ctas(aloam_ctx* c, int n_hyp);
 int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows);
 int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, const double* const* cand,
                          const unsigned long long* const* best, float accept_frac);
-// which lanes' candidate scores belong to a triggered row of the mapped stream call whose n_scans x nb rows are in c->h_rows
-// (recover.cu; n_scans = 0 at the start of a call: none)
-void recover_call_done(aloam_ctx* c, int n_scans, int nb);
+// which lanes' candidate scores belong to a triggered row of the last mapped stream call (recover.cu; none while its records
+// cannot be read or it ran no recovery)
+void recover_call_done(aloam_ctx* c);
 // the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
 int mapper_ensure(aloam_ctx* c, int lane);
 int* mapper_err_acc(aloam_ctx* c, int lane);

@@ -124,14 +124,15 @@ int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* r
   return recover_adopt_device(c, nb, in, rows, cand, best, R->accept_frac);
 }
 
-// which lanes' slices hold a triggered row of the call that just ended (its rows are in c->h_rows)
-void recover_call_done(aloam_ctx* c, int n_scans, int nb) {
+// which lanes' slices hold a triggered row of the last mapped stream call (its rows are in c->h_rows)
+void recover_call_done(aloam_ctx* c) {
   Recovery* R = c->recover;
   if (!R) return;
   for (bool& s : R->scored) s = false;
-  if (!c->rec_call) return;
-  for (int r = 0; r < n_scans * nb; ++r)
-    if (c->rows_kind[r] == ALOAM_ROW_LOCALISED && c->h_rows[r].rec_triggered) R->scored[r % nb] = true;
+  const MappedCall& M = c->last_mapped;
+  if (!M.records || !M.recovered) return;
+  for (int r = 0; r < M.n_scans * M.nb; ++r)
+    if (row_kind(M.table.rows[r]) == ALOAM_ROW_LOCALISED && c->h_rows[r].rec_triggered) R->scored[r % M.nb] = true;
 }
 
 extern "C" {
@@ -166,13 +167,13 @@ int aloam_set_recovery(aloam_ctx* c, int on, const aloam_recovery_opts* opts, co
 
 int aloam_recovery_rows(aloam_ctx* c, aloam_recovery_row* out, int rows) {
   if (!c || !out) return ALOAM_ERR_INVALID_ARG;
-  if (c->rows_n < 0) return ALOAM_ERR_STATE;
-  if (rows != c->rows_n) return ALOAM_ERR_INVALID_ARG;
+  const MappedCall& M = c->last_mapped;
+  if (const int rc = M.check(M.records, rows)) return rc;
   for (int r = 0; r < rows; ++r) {
     aloam_recovery_row& o = out[r];
     std::memset(&o, 0, sizeof(o));
     o.best = o.best_score = -1;
-    if (!c->rec_call || c->rows_kind[r] != ALOAM_ROW_LOCALISED) continue;
+    if (!M.recovered || row_kind(M.table.rows[r]) != ALOAM_ROW_LOCALISED) continue;
     const MapRowRec& h = c->h_rows[r];
     if (!h.rec_triggered) continue;
     o.triggered = 1;

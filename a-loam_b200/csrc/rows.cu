@@ -90,12 +90,12 @@ int aloam_set_map_rows(aloam_ctx* c, int on, float inlier_sq, int max_score_poin
 
 int aloam_map_rows(aloam_ctx* c, aloam_map_row* out, int rows) {
   if (!c || !out) return ALOAM_ERR_INVALID_ARG;
-  if (c->rows_n < 0) return ALOAM_ERR_STATE;
-  if (rows != c->rows_n) return ALOAM_ERR_INVALID_ARG;
+  const MappedCall& M = c->last_mapped;
+  if (const int rc = M.check(M.records, rows)) return rc;
   for (int r = 0; r < rows; ++r) {
     aloam_map_row& o = out[r];
     std::memset(&o, 0, sizeof(o));
-    o.kind = c->rows_kind[r];
+    o.kind = row_kind(M.table.rows[r]);
     if (o.kind == ALOAM_ROW_IDLE) continue;
     o.score = -1;
     if (o.kind == ALOAM_ROW_SKIPPED) continue;
