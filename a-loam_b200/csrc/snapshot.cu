@@ -7,13 +7,32 @@
 //   - the index of its next scan and its mode (LaneSched::scan, mapped);
 //   - mapped: its cube store, in the slab-free form of SnapStore (cubemap.cu saves and restores it).
 // Format: snapshot.h.
+#include <cmath>
 #include <cstring>
 #include "common.cuh"
 #include "ctx.h"
+#include "quat.cuh"
 
 namespace {
 
 constexpr char kMagic[8] = {'A', 'L', 'O', 'A', 'M', 'L', 'S', '1'};
+constexpr int kMaxCentre = 1 << 20;    // |cen[a]|: the range aloam_prior_map_build accepts
+constexpr int kCubeSlack = 16;         // cubes the map position may lie outside the buffer on an axis (the shift loop's steps)
+
+bool all_finite(const double* v, int n) {
+  for (int k = 0; k < n; ++k) if (!std::isfinite(v[k])) return false;
+  return true;
+}
+
+// the cube coordinate of map coordinate v under centre offset `centre` (laserMapping.cpp:314-325), with the range check of
+// build_cube_coord (cubemap.cu): false when (v + 25) / 50 is not finite or lies beyond int
+bool centre_cube(double v, int centre, long long* out) {
+  const double s = v + 25.0;
+  const double q = s / 50.0;
+  if (!(q > -2147483649.0 && q < 2147483648.0)) return false;
+  *out = (long long)(int)q + centre - (s < 0 ? 1 : 0);
+  return true;
+}
 
 // byte offset of the store section (the end of the unmapped snapshot)
 long long store_offset(const SnapHeader& h) { return (long long)sizeof(SnapHeader) + 16ll * ((long long)h.n_less_sharp + h.n_less_flat); }
@@ -24,14 +43,30 @@ int check_header(const SnapHeader& h, long long n_bytes) {
   if (std::memcmp(h.magic, kMagic, 8) != 0 || h.version != kSnapVersion) return ALOAM_ERR_SNAPSHOT;
   if ((h.mapped != 0 && h.mapped != 1) || h.scan_index < 1 || h.n_less_sharp < 0 || h.n_less_flat < 0) return ALOAM_ERR_SNAPSHOT;
   if (h.total_bytes != n_bytes) return ALOAM_ERR_SNAPSHOT;
+  if (!all_finite(h.warm, 7) || !all_finite(h.world, 7)) return ALOAM_ERR_SNAPSHOT;
   if (!h.mapped) return n_bytes == store_offset(h) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
   if (h.slab_cap[0] < 1 || h.slab_cap[1] < 1 || h.max_map_points < 1) return ALOAM_ERR_SNAPSHOT;
   return n_bytes >= store_offset(h) + (long long)sizeof(SnapStore) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
 }
 
-// the store table of a mapped snapshot whose header passed check_header: the valid list, every count within its slab capacity,
-// at most kSnapPool cubes of a type holding a slab, and a payload of exactly the counted points that ends the snapshot
+// the store table of a mapped snapshot whose header passed check_header: centre offsets within +-2^20, a finite T_wmap_wodom, a
+// map position T_wmap_wodom * world whose centre cube lies at most kCubeSlack cubes outside the buffer on every axis (the next
+// frame's shift loop runs one pass per cube beyond the edge: an unbounded position would never end it), the valid list, every
+// count within its slab capacity, at most kSnapPool cubes of a type holding a slab, and a payload of exactly the counted points
+// that ends the snapshot
 int check_store(const SnapHeader& h, const SnapStore& s) {
+  for (int a = 0; a < 3; ++a) if (s.cen[a] < -kMaxCentre || s.cen[a] > kMaxCentre) return ALOAM_ERR_SNAPSHOT;
+  if (!all_finite(s.q_wmap_wodom, 4) || !all_finite(s.t_wmap_wodom, 3)) return ALOAM_ERR_SNAPSHOT;
+  {
+    const Qd qm{s.q_wmap_wodom[0], s.q_wmap_wodom[1], s.q_wmap_wodom[2], s.q_wmap_wodom[3]};
+    double p[3];
+    qrot(qm, h.world + 4, p);
+    const int dims[3] = {21, 21, 11};
+    for (int a = 0; a < 3; ++a) {
+      long long c = 0;
+      if (!centre_cube(p[a] + s.t_wmap_wodom[a], s.cen[a], &c) || c < -kCubeSlack || c >= dims[a] + kCubeSlack) return ALOAM_ERR_SNAPSHOT;
+    }
+  }
   if (s.n_valid < 0 || s.n_valid > 125) return ALOAM_ERR_SNAPSHOT;
   for (int v = 0; v < s.n_valid; ++v)
     if (s.valid[v] < 0 || s.valid[v] >= kSnapCubes) return ALOAM_ERR_SNAPSHOT;

@@ -264,7 +264,14 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  * mode, as a START does (the lockstep calls are refused until aloam_reset_odometry); then it checks the whole snapshot on the
  * host before it writes anything to the device -- ALOAM_ERR_SNAPSHOT for a bad magic or version, a size that does not match the
  * sections, a count above the slab capacity, more than 1024 cubes of a type holding a slab, a payload that is not the sum of
- * the counts, a valid list of more than 125 entries or with an index outside 0 .. 4850, or a configuration that differs --
+ * the counts, a valid list of more than 125 entries or with an index outside 0 .. 4850, a non-finite warm start or world pose,
+ * and for a mapped snapshot a non-finite T_wmap_wodom, a centre offset cen[a] outside -2^20 .. 2^20 (the range of
+ * aloam_prior_map_build) or a map position T_wmap_wodom * world (translation) whose centre cube -- int((x + 25.0) / 50.0) + cen[a],
+ * minus 1 when x + 25.0 < 0, refused when (x + 25.0) / 50.0 is not finite or lies beyond int -- is more than 16 cubes outside the
+ * 21 x 21 x 11 buffer on an axis (below -16 or above 36 in i and j, above 26 in k: the next frame's ring-buffer shift runs one
+ * step per cube beyond its edges, so a far or infinite position would never end it; after a mapped frame the centre cube is
+ * 3 .. 17 (3 .. 7 in k), so a lane's own snapshot is refused only when the scans it skipped since then moved it more than
+ * 950 m), or a configuration that differs --
  * ALOAM_ERR_CAPACITY when a "last" cloud exceeds cfg.max_points, ALOAM_ERR_NOT_RING_MAJOR when it is not ring-major (the check
  * of aloam_odometry_set_last).  It creates the lane's cube store if needed.  After any failure the lane is not running; no other
  * lane changes.
@@ -301,8 +308,9 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
 /* ---- localisation against a prior map: vehicles register their scans against ONE saved map that no frame changes.
  * aloam_prior_map_load makes the cube store of a MAPPED lane snapshot (format v1; blob in device, pinned or pageable memory, as
  * aloam_lane_restore) the prior map of the context.  Only the store section and the configuration are used: the snapshot's odometry
- * part and its T_wmap_wodom are ignored.  The snapshot is checked on the host by the routine aloam_lane_restore runs for a mapped
- * snapshot, with its error codes (ALOAM_ERR_SNAPSHOT also for an unmapped snapshot), and nothing on the device changes on failure.
+ * part and its T_wmap_wodom are ignored beyond the range checks on them.  The snapshot is checked on the host by the routine
+ * aloam_lane_restore runs for a mapped snapshot, with its error codes (ALOAM_ERR_SNAPSHOT also for an unmapped snapshot), and nothing
+ * on the device changes on failure.
  * The map is packed per cloud type and indexed once, with one hash grid over the WHOLE map (1.00001 m cells): it is not bounded by
  * cfg.max_map_points (no submap is gathered) but by the snapshot format (1024 cubes of a type x the slab capacity) and by memory
  * (ALOAM_ERR_CUDA before any state changes): 32 B per point plus a table of 16 B x the power of two above 1.25 x the points of the
