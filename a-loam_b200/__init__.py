@@ -31,6 +31,7 @@ EXPORTED_SYMBOLS = [
     "aloam_prior_map_build", "aloam_prior_relocalise",
     "aloam_set_map_rows", "aloam_map_rows",
     "aloam_set_recovery", "aloam_recovery_rows", "aloam_debug_recovery_scores",
+    "aloam_lane_map_on_prior",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -160,6 +161,7 @@ def lib():
         L.aloam_prior_map_clear.argtypes = [C.c_void_p]
         L.aloam_prior_map_build.argtypes = [C.c_void_p, cv, cv, ip, C.POINTER(C.c_longlong)]
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
+        L.aloam_lane_map_on_prior.argtypes = [C.c_void_p, C.c_int, dp, dp]
         L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
         L.aloam_prior_relocalise.argtypes = [C.c_void_p, cv, cv, dp, C.c_int, C.POINTER(RelocOpts), ip, C.POINTER(RelocResult)]
         L.aloam_set_map_rows.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int]
@@ -708,6 +710,14 @@ class Aloam:
         if q.shape != (4,) or t.shape != (3,):
             raise ValueError("q_init is 4 doubles (x, y, z, w), t_init 3")
         _check(lib().aloam_lane_localise(self._h, int(lane), _dp(q), _dp(t)))
+
+    def lane_map_on_prior(self, lane, q_init, t_init):
+        """arms `lane`: its next LANE_START in a mapped scan_stream_lanes call begins a mapping trajectory on a copy of the prior
+        map, its T_wmap_wodom starting at (q_init xyzw, t_init); the prior map itself is never written"""
+        q = np.ascontiguousarray(q_init, np.float64); t = np.ascontiguousarray(t_init, np.float64)
+        if q.shape != (4,) or t.shape != (3,):
+            raise ValueError("q_init is 4 doubles (x, y, z, w), t_init 3")
+        _check(lib().aloam_lane_map_on_prior(self._h, int(lane), _dp(q), _dp(t)))
 
     def prior_relocalise(self, hyps, less_sharp=None, less_flat=None, raw=None, inlier_sq=1.0, max_score_points=1024, refine=1,
                          scores=True):

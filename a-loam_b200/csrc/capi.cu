@@ -526,17 +526,18 @@ int aloam_scan_to_pose_device(aloam_ctx* c, const float* d_raw, int n, double q_
 }
 
 // Appends the next row to *t, `op` on the lane whose schedule state is *s (its raw scan v), and applies the op to *s: a START
-// begins a trajectory at scan 0 -- in a mapped call (map) a mapped one that consumes the lane's arming, so that it localises --,
-// a SCAN continues it, an IDLE ends it.  The one place a lane's scan index advances.
+// begins a trajectory at scan 0 -- in a mapped call (map) a mapped one that consumes the lane's arming, so that it localises or
+// maps on a copy of the prior map --, a SCAN continues it, an IDLE ends it.  The one place a lane's scan index advances.
 static void add_row(const aloam_ctx* c, StreamTable* t, LaneSched* s, int op, const aloam_cloud_view& v, bool map) {
-  StreamRow r{op, -1, false, false, t->reg_total};
+  StreamRow r{op, -1, false, false, false, t->reg_total};
   if (op == ALOAM_LANE_IDLE) {
     s->running = false;
   } else {
     if (op == ALOAM_LANE_START) {
       s->running = true; s->mapped = map; s->scan = 0;
-      s->localising = map && s->armed;
-      if (map) s->armed = false;
+      s->localising = map && s->arm == ARM_LOCALISE;
+      r.seed = map && s->arm == ARM_MAP_ON_PRIOR;
+      if (map) s->arm = ARM_NONE;
     }
     r.scan = s->scan++;
     r.mapped = map && r.scan % c->cfg.mapping_skip_frame == 0;   // laserOdometry.cpp:570
@@ -582,7 +583,7 @@ static int map_stage(aloam_ctx* c, const StreamSwitches& w, const StreamRow* row
     const FeatBuf& fc = c->lanes[l].feat[cur]; const size_t slot = (r0 + l) * 7;
     const int g = !row[l].mapped ? 2 : row[l].localise;
     fr[g][n_fr[g]++] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
-                                w.reset_stores && row[l].op == ALOAM_LANE_START, row[l].localise};
+                                w.reset_stores && row[l].op == ALOAM_LANE_START && !row[l].seed, row[l].localise, row[l].seed};
   }
   const int n_upper_c = 64 * kMaxLessSharpPerRing, n_upper_s = std::min(nmax, c->max_points);
   for (int loc = 0; loc < 2; ++loc) {   // the mapping frame, then the locate frame, each followed by its rows and registered clouds
@@ -876,6 +877,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   LaneSched s[ALOAM_MAX_BATCH];
   for (int l = 0; l < c->n_lanes; ++l) { s[l] = c->lanes[l].sched; s[l].running = s[l].running && l < batch; }
   bool maps[ALOAM_MAX_BATCH] = {}, localises[ALOAM_MAX_BATCH] = {};   // the lane has a mapping / a localising scan in this call
+  bool seeds = false;                                                 // a START maps on a copy of the prior map
   for (size_t i = 0; i < (size_t)n_scans * batch; ++i)
     if (lane_ops[i] < ALOAM_LANE_IDLE || lane_ops[i] > ALOAM_LANE_START) return ALOAM_ERR_INVALID_ARG;
   StreamTable t((size_t)n_scans * batch);
@@ -899,6 +901,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
       }
       add_row(c, &t, &s[l], op, v, map);
       if (map && op != ALOAM_LANE_IDLE) (t.rows.back().localise ? localises : maps)[l] = true;
+      seeds = seeds || t.rows.back().seed;
     }
   }
   if (map && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
@@ -908,6 +911,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
     int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
     rc = maps[l] || !localises[l] ? mapper_ensure(c, l) : ALOAM_OK; if (rc) return rc;
   }
+  if (seeds) { const int rc = mapper_seed_ensure(c); if (rc) return rc; }
   // committed before anything is issued: a later failure ends in aloam_reset_odometry, a key overflow leaves the lanes running
   c->lanes_mode = true;
   for (int l = 0; l < c->n_lanes; ++l) c->lanes[l].sched = s[l];

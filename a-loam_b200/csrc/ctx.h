@@ -43,6 +43,8 @@ struct MapperIn {
   int lane;
   int fresh;
   int localise;   // the lane registers against the context's prior map: its frame state is its locator's, not a cube store's
+  int seed;       // the lane starts a mapping trajectory with this frame on a copy of the prior map, from T_wmap_wodom Lane::init
+                  // (aloam_lane_map_on_prior): its store is seeded before the frame, `fresh` is off
 };
 // what the registration of localising lanes searches instead of each lane's indexed submap: the prior map's grids, and per
 // lane the window tables and centre cube k_locate_begin left in its frame state
@@ -122,6 +124,7 @@ struct StreamRow {
   int scan;             // index of the scan in its trajectory (-1: an IDLE row)
   bool mapped;          // a mapped call's scan that goes to the mapper (or its lane's locator); the others get a high-frequency pose
   bool localise;        // a mapped call's scan that registers against the prior map
+  bool seed;            // a mapped call's START that maps on a copy of the prior map (consumes an aloam_lane_map_on_prior arming)
   long long reg_begin;  // where the row's registered cloud begins in the sink: the sum of raws[r'].n over the mapped rows r' before it
 };
 // the rows of a stream call, built before anything is issued (room for all n in one allocation); reg_total: the points of every
@@ -143,11 +146,14 @@ struct MappedCall {
 
 // Where a lane is in the schedule of the stream calls.  A lane of aloam_scan_stream_lanes runs from its START to the step before
 // its next IDLE; `mapped` is the mode of the call that started it; `localising`: the trajectory it runs (or ran last) registers
-// against the prior map, fixed at its START; `armed`: aloam_lane_localise has armed its next mapped START with Lane::init.
+// against the prior map, fixed at its START; `arm`: what its next mapped START does with Lane::init -- localise from it
+// (aloam_lane_localise) or map on a copy of the prior map from it (aloam_lane_map_on_prior); the later arming replaces the other.
 // `scan`: index of its next scan in its trajectory (0 at a START), which every stream call advances; scan j goes to the mapper
 // when j % cfg.mapping_skip_frame == 0.  aloam_reset_odometry puts back the default.
+enum LaneArm { ARM_NONE = 0, ARM_LOCALISE, ARM_MAP_ON_PRIOR };
 struct LaneSched {
-  bool running = false, mapped = false, localising = false, armed = false;
+  bool running = false, mapped = false, localising = false;
+  int arm = ARM_NONE;
   int scan = 0;
 };
 
@@ -159,7 +165,7 @@ struct Lane {
   // stream calls; a lane that only localises has no store
   Mapper* mapper = nullptr;
   Locator* locator = nullptr;
-  double init[7] = {};   // the T_wmap_wodom an armed START localises from (aloam_lane_localise)
+  double init[7] = {};   // the T_wmap_wodom an armed START starts from (aloam_lane_localise, aloam_lane_map_on_prior)
   // the locator holds the window of a localising frame against the current prior map (aloam_debug_prior_associate); set by the
   // frame, cleared when the prior map is released
   bool window = false;
@@ -320,6 +326,9 @@ struct aloam_ctx {
   // aloam_lane_save / _restore of mapped lanes: the store table of a snapshot, pinned and on the device, created on first use
   SnapStore* h_snap_store = nullptr;
   SnapStore* d_snap_store = nullptr;
+  // the seeded STARTs of a step (aloam_lane_map_on_prior): the ALOAM_EXPORT_MAP layout of record l's new store, [n_lanes], created
+  // by the first stream call that seeds a store
+  ExportLayout* d_seed_layout = nullptr;
 };
 
 namespace {
@@ -410,6 +419,8 @@ int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* co
 void recover_call_done(aloam_ctx* c);
 // the cube store of lane `lane`, created on first use with the state of a fresh trajectory (a failure publishes nothing)
 int mapper_ensure(aloam_ctx* c, int lane);
+// the layouts of seeded STARTs (aloam_ctx::d_seed_layout), created on first use
+int mapper_seed_ensure(aloam_ctx* c);
 int* mapper_err_acc(aloam_ctx* c, int lane);
 // localisation against the prior map (cubemap.cu): a new locator; a lane's locator, created on first use; one frame of nb
 // localising records on the current stream, record l on locator loc[l] (in[l].fresh: it starts a trajectory with this frame,
@@ -452,6 +463,9 @@ inline bool any_lane_localising(const aloam_ctx* c) {
 // *store = byte offset of the store section.
 int snapshot_buffer_kind(const aloam_ctx* c, const void* p);
 int snapshot_validate(aloam_ctx* c, const char* b, long long n_bytes, int kind, bool need_mapped, long long* store);
+// snapshot.cu: the map position p (T_wmap_wodom times a world pose) may start a mapping frame of a store with centre offsets cen --
+// its centre cube lies at most kCubeSlack cubes outside the buffer on every axis, so the frame's shift loop ends
+bool map_position_fits(const double p[3], const int cen[3]);
 void mapper_slab_caps(const aloam_ctx* c, int cap[2]);
 int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head);
 int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device);

@@ -110,6 +110,9 @@ struct aloam::PriorMap {
   int* d_n = nullptr;            // [2]
   GridTable grid[2] = {};
   ExportLayout* d_layout = nullptr;
+  // per type, from the cube table: the largest cube and the cubes that hold points -- whether a lane store can hold a copy of
+  // the map (aloam_lane_map_on_prior)
+  int max_cube[2] = {0, 0}, n_cubes[2] = {0, 0};
 };
 // what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
 // k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
@@ -575,13 +578,13 @@ __global__ void __launch_bounds__(256) k_store_copy(const ExportLayout* __restri
   }
 }
 
-// ---- lane snapshots (aloam_lane_restore): the inverse of the ALOAM_EXPORT_MAP export
+// ---- lane snapshots (aloam_lane_restore): the inverse of the ALOAM_EXPORT_MAP export; seeded STARTs (aloam_lane_map_on_prior)
 
-// One CTA of 1024: the store a snapshot's table H describes.  State of a fresh trajectory first (the caller has zeroed S), then
-// the cubes with a count >= 0 take slabs 0, 1, 2, ... of their type in cube order (the rest of the pool stays free, ascending),
-// L = the layout of the ALOAM_EXPORT_MAP export of the rebuilt store, and the fields that outlive a frame.
-__global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, Pt4* p0, Pt4* p1, int cap0, int cap1,
-                                                              ExportLayout* __restrict__ L) {
+// One CTA of 1024: the store whose cube i holds count(ty, i) points of type ty (-1: no slab).  State of a fresh trajectory first,
+// then the cubes with a count >= 0 take slabs 0, 1, 2, ... of their type in cube order (the rest of the pool stays free,
+// ascending), L = the layout of the ALOAM_EXPORT_MAP export of the new store.  The caller sets the fields that outlive a frame.
+template <typename Count>
+__device__ __forceinline__ void store_import_body(MapperState* __restrict__ S, Count count, Pt4* p0, Pt4* p1, int cap0, int cap1, ExportLayout* __restrict__ L) {
   __shared__ long long s_pts[1024];
   __shared__ int s_slabs[2][1024];
   const int tid = threadIdx.x;
@@ -590,7 +593,7 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
   long long pts = 0;
   int n0 = 0, n1 = 0;
   for (int i = b; i < e; ++i) {
-    const int c0 = H->count[0][i], c1 = H->count[1][i];
+    const int c0 = count(0, i), c1 = count(1, i);
     pts += max(c0, 0) + max(c1, 0);
     n0 += c0 >= 0; n1 += c1 >= 0;
   }
@@ -599,7 +602,7 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
   int next[2] = {block_scan_1024(n0, s_slabs[0]), block_scan_1024(n1, s_slabs[1])};
   for (int i = b; i < e; ++i)
     for (int ty = 0; ty < 2; ++ty) {
-      const int n = H->count[ty][i];
+      const int n = count(ty, i);
       L->off[2 * i + ty] = run;
       L->base[2 * i + ty] = nullptr;
       if (n >= 0) {
@@ -609,6 +612,13 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
       }
     }
   if (tid == 1023) { L->off[kExportSegs] = run; L->nseg = kExportSegs; L->total = run; S->free_top = s_slabs[0][1023]; S->free_top2 = s_slabs[1][1023]; }
+}
+
+// the store a snapshot's table H describes (the caller has zeroed S), and the fields of H that outlive a frame
+__global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, Pt4* p0, Pt4* p1, int cap0, int cap1,
+                                                              ExportLayout* __restrict__ L) {
+  store_import_body(S, [H](int ty, int i) { return H->count[ty][i]; }, p0, p1, cap0, cap1, L);
+  const int tid = threadIdx.x;
   if (tid < kMaxValid) S->valid[tid] = tid < H->n_valid ? H->valid[tid] : 0;
   if (tid == 0) {
     for (int a = 0; a < 3; ++a) S->cen[a] = H->cen[a];
@@ -616,6 +626,43 @@ __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __res
     S->frames = H->frames;
     for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = H->q_wmap_wodom[k];
     for (int k = 0; k < 3; ++k) S->t_wmap_wodom[k] = H->t_wmap_wodom[k];
+  }
+}
+
+// one seeded START: the lane's store, its slab pools and the layout its copy of the prior map gets, and the T_wmap_wodom it
+// starts from (normalised by aloam_lane_map_on_prior)
+struct SeedLane {
+  MapperState* S;
+  Pt4* pts[2];
+  int cap[2];
+  ExportLayout* L;
+  double init[7];
+};
+// grid (1, 1, records), 1024 threads: record z's store becomes the prior map's (cube table cs [2][NCUBE + 1], centre offsets cen):
+// every cube that holds points gets a slab of its type, in cube order, the others none; frames = 0, an empty valid list and
+// T_wmap_wodom = init.  Fields the stack filter writes (stack_counts, err, in_counts) stay as mapper_fresh_state leaves them.
+__global__ void __launch_bounds__(1024) k_store_seed_tables(const __grid_constant__ Batch<SeedLane> B, const int* __restrict__ cs, int cen0, int cen1, int cen2) {
+  const SeedLane& a = B.a[blockIdx.z];
+  MapperState* S = a.S;
+  store_import_body(S, [cs](int ty, int i) { const int* t = cs + ty * (NCUBE + 1) + i; const int n = t[1] - t[0]; return n > 0 ? n : -1; },
+                    a.pts[0], a.pts[1], a.cap[0], a.cap[1], a.L);
+  if (threadIdx.x == 0) {
+    S->cen[0] = cen0; S->cen[1] = cen1; S->cen[2] = cen2;
+    for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = a.init[k];
+    for (int k = 0; k < 3; ++k) S->t_wmap_wodom[k] = a.init[4 + k];
+  }
+}
+
+// grid-stride over the segments, grid (CTAs, 1, records): the points of record z's store (layout D[z]) from the prior map's (layout
+// P).  Segment s of both layouts is the same cube and type with the same number of points.
+__global__ void __launch_bounds__(256) k_store_seed_copy(const ExportLayout* __restrict__ P, const ExportLayout* __restrict__ D) {
+  const ExportLayout* __restrict__ L = D + blockIdx.z;
+  for (int s = blockIdx.x; s < kExportSegs; s += gridDim.x) {
+    const int n = (int)(L->off[s + 1] - L->off[s]);
+    if (n <= 0) continue;
+    const Pt4* __restrict__ src = P->base[s];
+    Pt4* __restrict__ dst = L->base[s];
+    for (int q = threadIdx.x; q < n; q += blockDim.x) dst[q] = src[q];
   }
 }
 
@@ -822,7 +869,14 @@ void prior_index(aloam_ctx* c, PriorMap* p) {
 template <typename Fill> int prior_install(aloam_ctx* c, const int cen[3], const std::vector<int>& cs, Fill fill) {
   PriorMap* p = new (std::nothrow) PriorMap();
   if (!p) return ALOAM_ERR_CUDA;
-  for (int t = 0; t < 2; ++t) p->n[t] = cs[(size_t)t * (NCUBE + 1) + NCUBE];
+  for (int t = 0; t < 2; ++t) {
+    p->n[t] = cs[(size_t)t * (NCUBE + 1) + NCUBE];
+    for (int i = 0; i < NCUBE; ++i) {
+      const int n = cs[(size_t)t * (NCUBE + 1) + i + 1] - cs[(size_t)t * (NCUBE + 1) + i];
+      p->max_cube[t] = std::max(p->max_cube[t], n);
+      p->n_cubes[t] += n > 0;
+    }
+  }
   for (int a = 0; a < 3; ++a) p->cen[a] = cen[a];
   bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess &&
             cudaMalloc(&p->d_layout, sizeof(ExportLayout)) == cudaSuccess;
@@ -856,6 +910,7 @@ template <typename Fill> int prior_install(aloam_ctx* c, const int cen[3], const
   if (!c->prior_owned) { own(c, [c] { prior_map_release(c); }); c->prior_owned = true; }
   prior_map_release(c);
   c->prior = p;
+  for (Lane& L : c->lanes) if (L.sched.arm == ARM_MAP_ON_PRIOR) L.sched.arm = ARM_NONE;   // its fit was checked against the old map
   return ALOAM_OK;
 }
 
@@ -1147,6 +1202,29 @@ int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const ch
   return ALOAM_OK;
 }
 
+// The seeded records of a mapping frame (in[l].seed) on the current stream, two launches for all of them: k_store_seed_tables
+// lays out record l's store as a copy of the prior map in c->d_seed_layout[l], k_store_seed_copy copies the map's points into it.
+// Nothing is issued when no record seeds.
+static int seed_stores(aloam_ctx* c, int nb, const MapperIn* in) {
+  Batch<SeedLane> B = {};
+  int n = 0;
+  for (int l = 0; l < nb; ++l) {
+    if (!in[l].seed) continue;
+    const Lane& L = c->lanes[in[l].lane];
+    const Mapper* m = L.mapper;
+    B.a[n] = SeedLane{m->d_state, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, c->d_seed_layout + n, {}};
+    for (int k = 0; k < 7; ++k) B.a[n].init[k] = L.init[k];
+    ++n;
+  }
+  if (n == 0) return ALOAM_OK;
+  const PriorMap* P = c->prior;
+  if (!P || !c->d_seed_layout) return ALOAM_ERR_STATE;   // an arming is dropped with the map it was checked against
+  LAUNCH(c, KID_CUBES, k_store_seed_tables, dim3(1, 1, n), 1024, 0, B, (const int*)P->d_cube_start, P->cen[0], P->cen[1], P->cen[2]);
+  LAUNCH(c, KID_CUBES, k_store_seed_copy, dim3(std::min(kExportSegs, c->sms * 8), 1, n), 256, 0, (const ExportLayout*)P->d_layout, (const ExportLayout*)c->d_seed_layout);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 // One frame of alaserMapping's process() for nb trajectories ("lanes") on the current stream, entirely on the device: every launch
 // covers all lanes, lane l in blockIdx.z, and each lane has its own cube store, stack filter buffers and registration set, so
 // lane l computes exactly what a frame of lane l alone computes.  in[l]: the lane's less-sharp / less-flat clouds and their
@@ -1184,6 +1262,9 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   }
   const int max_sub = m0->max_sub, cap1 = m0->cap[1];
   const int refilter_cap = (int)m0->buf.cap;   // refilter_bound: the same for every lane
+  // ---- seeded STARTs: their stores become copies of the prior map, in order on this stream after the lanes' previous frames and
+  //      before this frame's stack filters are forked, so nothing of the frame runs beside the seed
+  rc = seed_stores(c, nb, in); if (rc) return rc;
   // ---- stack filters (:541-550), beside the gather + index build below, which read only the cube stores
   rc = stack_filters_fork(c, nb, B, stack_f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub, fresh);
@@ -1338,6 +1419,11 @@ int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* co
 
 // the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
 int* mapper_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].mapper->d_state->err_acc; }
+
+int mapper_seed_ensure(aloam_ctx* c) {
+  if (!c->d_seed_layout) CUDA_CHECK_RET(dalloc(c, &c->d_seed_layout, (size_t)c->n_lanes));
+  return ALOAM_OK;
+}
 
 int mapper_ensure(aloam_ctx* c, int lane) {
   if (c->lanes[lane].mapper) return ALOAM_OK;
@@ -1556,7 +1642,7 @@ int aloam_prior_map_clear(aloam_ctx* c) {
   if (any_lane_localising(c)) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   prior_map_release(c);
-  for (Lane& L : c->lanes) L.sched.armed = false;   // an arming needs a map
+  for (Lane& L : c->lanes) L.sched.arm = ARM_NONE;   // an arming needs a map
   return ALOAM_OK;
 }
 
@@ -1567,7 +1653,24 @@ int aloam_lane_localise(aloam_ctx* c, int lane, const double q_init[4], const do
   if (!c->prior) return ALOAM_ERR_STATE;
   Lane& L = c->lanes[lane];
   for (int k = 0; k < 7; ++k) L.init[k] = init[k];
-  L.sched.armed = true;
+  L.sched.arm = ARM_LOCALISE;
+  return ALOAM_OK;
+}
+
+int aloam_lane_map_on_prior(aloam_ctx* c, int lane, const double q_init[4], const double t_init[3]) {
+  if (!c || lane < 0 || lane >= c->n_lanes || !q_init || !t_init) return ALOAM_ERR_INVALID_ARG;
+  double init[7];
+  if (!map_pose_normalise(q_init, t_init, init)) return ALOAM_ERR_INVALID_ARG;
+  const PriorMap* P = c->prior;
+  if (!P || sharded_job(c)) return ALOAM_ERR_STATE;
+  // the START's map position is init's translation (identity odometry pose): its first frame's shift loop must end
+  if (!map_position_fits(init + 4, P->cen)) return ALOAM_ERR_INVALID_ARG;
+  int cap[2];
+  mapper_slab_caps(c, cap);
+  for (int t = 0; t < 2; ++t) if (P->max_cube[t] > cap[t] || P->n_cubes[t] > kPool) return ALOAM_ERR_CAPACITY;
+  Lane& L = c->lanes[lane];
+  for (int k = 0; k < 7; ++k) L.init[k] = init[k];
+  L.sched.arm = ARM_MAP_ON_PRIOR;
   return ALOAM_OK;
 }
 

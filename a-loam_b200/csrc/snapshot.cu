@@ -61,11 +61,8 @@ int check_store(const SnapHeader& h, const SnapStore& s) {
     const Qd qm{s.q_wmap_wodom[0], s.q_wmap_wodom[1], s.q_wmap_wodom[2], s.q_wmap_wodom[3]};
     double p[3];
     qrot(qm, h.world + 4, p);
-    const int dims[3] = {21, 21, 11};
-    for (int a = 0; a < 3; ++a) {
-      long long c = 0;
-      if (!centre_cube(p[a] + s.t_wmap_wodom[a], s.cen[a], &c) || c < -kCubeSlack || c >= dims[a] + kCubeSlack) return ALOAM_ERR_SNAPSHOT;
-    }
+    for (int a = 0; a < 3; ++a) p[a] += s.t_wmap_wodom[a];
+    if (!map_position_fits(p, s.cen)) return ALOAM_ERR_SNAPSHOT;
   }
   if (s.n_valid < 0 || s.n_valid > 125) return ALOAM_ERR_SNAPSHOT;
   for (int v = 0; v < s.n_valid; ++v)
@@ -115,6 +112,15 @@ int last_slot(const aloam_ctx* c) { return (c->frame + kFeatSlots - 1) % kFeatSl
 int buffer_kind(const aloam_ctx* c, const void* p) { return snapshot_buffer_kind(c, p); }
 
 }  // namespace
+
+bool map_position_fits(const double p[3], const int cen[3]) {
+  const int dims[3] = {21, 21, 11};
+  for (int a = 0; a < 3; ++a) {
+    long long c = 0;
+    if (!centre_cube(p[a], cen[a], &c) || c < -kCubeSlack || c >= dims[a] + kCubeSlack) return false;
+  }
+  return true;
+}
 
 int snapshot_buffer_kind(const aloam_ctx* c, const void* p) {
   cudaPointerAttributes at = {};

@@ -373,6 +373,39 @@ int aloam_prior_map_build(aloam_ctx* ctx, aloam_cloud_view corner_map, aloam_clo
 int aloam_prior_map_clear(aloam_ctx* ctx);
 int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
 
+/* ---- extending a saved map in a later session: a MAPPING trajectory that starts on a copy of the prior map.
+ * aloam_lane_map_on_prior arms `lane` (0 <= lane < cfg.max_batch): its next ALOAM_LANE_START in an aloam_scan_stream_lanes call with
+ * map_poses begins a mapping trajectory (its rows are ALOAM_ROW_MAPPED; there is no new mode) whose cube store is, at that START, a
+ * copy of the context's prior map and whose T_wmap_wodom is (q_init, t_init), normalised as aloam_lane_localise normalises it.  From
+ * then on the lane is an ordinary mapping lane: it shifts the ring buffer, inserts and re-filters; aloam_lane_save,
+ * aloam_mapper_export, the registered sink, aloam_map_rows and cfg.mapping_skip_frame work as for any mapping lane.  The prior map is
+ * never written: to publish the extended map, save the lane and aloam_prior_map_load the snapshot, or export it and build from it.
+ *   - the seeded store: the centre offsets are the prior map's; every cube the prior map holds points in gets a slab of its type,
+ *     slabs 0, 1, 2, ... in cube order (the layout aloam_lane_restore gives a snapshot's store), the points in the prior map's
+ *     per-cube order; cubes without points get no slab; frames = 0 and the valid list is empty (the START frame computes it).
+ *   - equivalence: every row of the trajectory -- map pose, stats and flags -- and the final store are bit for bit those of
+ *     aloam_mapper_step on a lane 0 restored (aloam_lane_restore) from a mapped snapshot that holds the prior map's store with
+ *     T_wmap_wodom = the normalised init and frames = 0, driven with the same clouds and odometry poses (the START's odometry pose is
+ *     the identity).  It is also the reference node (laserMapping.cpp) started with its cube arrays, centre offsets and
+ *     q_wmap_wodom / t_wmap_wodom set that way.
+ *   - errors, each with nothing armed: ALOAM_ERR_STATE without a prior map, on a rank of a sharded job and on an emulating context;
+ *     ALOAM_ERR_INVALID_ARG for a bad lane, a NULL or non-finite pose, a zero quaternion, or an init position t_init whose centre
+ *     cube (int((t + 25.0) / 50.0) + the prior map's centre offset, minus 1 below -25) lies more than 16 cubes outside the
+ *     21 x 21 x 11 buffer on an axis -- the rule aloam_lane_restore applies to a snapshot's map position (the first frame's shift
+ *     loop must end); ALOAM_ERR_CAPACITY when the prior map does not fit a lane's store: a cube with more points than the slab
+ *     capacity of its type (min(16384, cfg.max_points) corner, min(65536, cfg.max_points) surf; a built map may hold up to 65536
+ *     corner points in a cube), or more than 1024 cubes of one type that hold points.
+ *   - arming: a lane has one arming; aloam_lane_localise and aloam_lane_map_on_prior replace each other (the later call wins).  An
+ *     odometry-only START does not consume it; aloam_reset_odometry drops it, and so do aloam_prior_map_load, aloam_prior_map_build
+ *     and aloam_prior_map_clear when they succeed, since the fit was checked against the map of the time (aloam_lane_localise
+ *     armings keep their rules).  After its START a seeded lane no longer depends on the prior map: loading, building or clearing a
+ *     map between calls does not change it.
+ *   - cost: arming allocates nothing and a stream call in which no seeded START runs issues exactly what it issued before.  A step
+ *     with seeded STARTs issues 2 more launches on the mapper stream, for all of them together, before its mapping frame
+ *     (k_store_seed_tables, k_store_seed_copy).  The lane's store is created as for any mapped START; the first call that seeds a
+ *     store also creates cfg.max_batch export layouts of about 155 kB each on the device, kept until aloam_destroy. */
+int aloam_lane_map_on_prior(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
+
 /* ---- relocalisation: finding the map pose aloam_lane_localise needs, for a vehicle that boots on the map, a lane that lost
  * track or a recording that starts somewhere unknown.  aloam_prior_relocalise scores n_hyp pose hypotheses of ONE scan against
  * the context's prior map on the device and refines the `refine` best of them with a localising frame each.
