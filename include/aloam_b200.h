@@ -386,8 +386,12 @@ int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const 
  *   - equivalence: every row of the trajectory -- map pose, stats and flags -- and the final store are bit for bit those of
  *     aloam_mapper_step on a lane 0 restored (aloam_lane_restore) from a mapped snapshot that holds the prior map's store with
  *     T_wmap_wodom = the normalised init and frames = 0, driven with the same clouds and odometry poses (the START's odometry pose is
- *     the identity).  It is also the reference node (laserMapping.cpp) started with its cube arrays, centre offsets and
- *     q_wmap_wodom / t_wmap_wodom set that way.
+ *     the identity).  One exception: a cube the snapshot counts with 0 points (a slab, no points) has no slab in the seeded store,
+ *     since the prior map keeps only counts.  Until a frame inserts into it, aloam_lane_save writes -1 for it where the restored
+ *     lane writes 0, and the seeded lane's slab pool holds one more free slab of that type.  While the restored lane's pool is not
+ *     exhausted nothing else differs; once it is, a new cube the restored lane must drop (ALOAM_FLAG_CUBE_OVERFLOW) can still take
+ *     a slab on the seeded lane, and from that frame on its rows, points and poses may differ.  It is also the reference node
+ *     (laserMapping.cpp) started with its cube arrays, centre offsets and q_wmap_wodom / t_wmap_wodom set that way.
  *   - errors, each with nothing armed: ALOAM_ERR_STATE without a prior map, on a rank of a sharded job and on an emulating context;
  *     ALOAM_ERR_INVALID_ARG for a bad lane, a NULL or non-finite pose, a zero quaternion, or an init position t_init whose centre
  *     cube (int((t + 25.0) / 50.0) + the prior map's centre offset, minus 1 below -25) lies more than 16 cubes outside the

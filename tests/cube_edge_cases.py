@@ -352,10 +352,26 @@ def relabel(blob, d):
     return np.frombuffer(bytes(out), np.uint8)
 
 
-def with_store_fields(blob, cen=None, t_wmap=None, q_wmap=None, world=None, warm=None):
-    """a copy of `blob` with header / store fields replaced (for the snapshot checks)"""
+def with_store_fields(blob, cen=None, t_wmap=None, q_wmap=None, world=None, warm=None, valid=None, frames=None, counts=None,
+                      points=None):
+    """a copy of `blob` with header / store fields replaced (for the snapshot checks and crafted stores).  counts ((2, NCUBE), -1:
+    no slab) and points (the ALOAM_EXPORT_MAP payload) go together: the point total and the snapshot's size follow them"""
     b, s = store_section(blob)
     out = bytearray(b)
+    if counts is not None:
+        counts = np.ascontiguousarray(counts, np.int32).reshape(2, NCUBE)
+        pts = np.ascontiguousarray(points, F32).reshape(-1, 4)
+        assert len(pts) == int(np.maximum(counts, 0).sum()), "points must hold the counted points"
+        out = out[:s + TABLE] + bytearray(pts.tobytes())
+        out[s + 592:s + 592 + counts.nbytes] = counts.tobytes()
+        struct.pack_into("<q", out, s + 39408, len(pts))
+        struct.pack_into("<q", out, 16, len(out))
+    if valid is not None:
+        out[s + 16:s + 528] = bytes(512)
+        struct.pack_into("<i", out, s + 12, len(valid))
+        struct.pack_into("<%di" % len(valid), out, s + 16, *valid)
+    if frames is not None:
+        struct.pack_into("<i", out, s + 528, frames)
     if cen is not None:
         struct.pack_into("<3i", out, s, *cen)
     if q_wmap is not None:
