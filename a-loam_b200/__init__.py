@@ -32,12 +32,14 @@ EXPORTED_SYMBOLS = [
     "aloam_set_map_rows", "aloam_map_rows",
     "aloam_set_recovery", "aloam_recovery_rows", "aloam_debug_recovery_scores",
     "aloam_lane_map_on_prior",
+    "aloam_io_unpack_points_ring",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
 EXPORT_SURROUND, EXPORT_MAP = 0, 1
 PRIOR_MAP = -1   # `lane` of mapper_export: the context's prior map
 ROW_IDLE, ROW_MAPPED, ROW_LOCALISED, ROW_SKIPPED = 0, 1, 2, 3   # aloam_map_row.kind
+RING_ELEVATION, RING_FIELD = 0, 1   # aloam_config.ring_source: the elevation formula, or the driver's ring in float 3 of a raw point
 
 
 class Config(C.Structure):
@@ -45,6 +47,20 @@ class Config(C.Structure):
                 ("outer_iters", C.c_int), ("inner_iters", C.c_int), ("huber", C.c_double), ("dist_sq_thresh", C.c_double),
                 ("nearby_scan", C.c_double), ("device", C.c_int), ("max_points", C.c_int), ("max_map_points", C.c_int),
                 ("max_batch", C.c_int), ("distortion", C.c_int), ("max_ring_points", C.c_int), ("mapping_skip_frame", C.c_int)]
+
+    # aloam_config.ring_source, appended after mapping_skip_frame, is the int in the 8-byte tail padding of the fields above:
+    # the structure keeps the size and layout of aloam_config (80 bytes) with the older field list
+    @property
+    def ring_source(self):
+        return C.c_int.from_buffer(self, _RING_SOURCE_AT).value
+
+    @ring_source.setter
+    def ring_source(self, v):
+        C.c_int.from_buffer(self, _RING_SOURCE_AT).value = v
+
+
+_RING_SOURCE_AT = Config.mapping_skip_frame.offset + 4
+assert C.sizeof(Config) == _RING_SOURCE_AT + 4, "aloam_config layout"
 
 
 class CloudView(C.Structure):

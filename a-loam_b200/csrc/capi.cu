@@ -36,7 +36,7 @@ const char* aloam_strerror(int code) {
   switch (code) {
     case ALOAM_OK: return "ok";
     case ALOAM_ERR_INVALID_ARG: return "invalid argument";
-    case ALOAM_ERR_UNSUPPORTED_SCANS: return "only 16, 32 or 64 scan lines are supported";
+    case ALOAM_ERR_UNSUPPORTED_SCANS: return "n_scans must be 16, 32 or 64 for elevation rings, 1..64 for driver rings";
     case ALOAM_ERR_EMPTY_CLOUD: return "no point survives the NaN / minimum-range filter";
     case ALOAM_ERR_CAPACITY: return "cloud larger than the context capacity";
     case ALOAM_ERR_CUDA: return "CUDA error";
@@ -85,7 +85,9 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   if (cfg.max_ring_points == 0) cfg.max_ring_points = ALOAM_MAX_RING_POINTS;
   if (cfg.mapping_skip_frame == 0) cfg.mapping_skip_frame = 1;
   if (cfg.mapping_skip_frame < 0) return ALOAM_ERR_INVALID_ARG;
-  if (cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64) return ALOAM_ERR_UNSUPPORTED_SCANS;
+  if (cfg.ring_source != ALOAM_RING_ELEVATION && cfg.ring_source != ALOAM_RING_FIELD) return ALOAM_ERR_INVALID_ARG;
+  if (cfg.ring_source == ALOAM_RING_FIELD ? cfg.n_scans < 1 || cfg.n_scans > 64 : cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64)
+    return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
   if (!(cfg.nearby_scan >= 1.0)) return ALOAM_ERR_INVALID_ARG;   // the association's break tables need a window of +-1 ring at least
   // HuberLoss(a) needs a > 0, and a VoxelGrid leaf <= 0 or NaN has no voxels
@@ -205,7 +207,8 @@ int run_features_a(aloam_ctx* c, int nb, const int* pl, const float* const* d_ra
                            nfull_out ? nfull_out + pl[l] : nullptr};
     sa.a[l] = ScatterArgs{d_raw[l], n[l], stride, L.d_ring, L.d_offsets, sc, L.d_full[buf]};
   }
-  LAUNCH(c, KID_CLASSIFY, k_classify, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
+  if (c->cfg.ring_source == ALOAM_RING_FIELD) LAUNCH(c, KID_CLASSIFY, k_classify<ALOAM_RING_FIELD>, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
+  else LAUNCH(c, KID_CLASSIFY, k_classify<ALOAM_RING_ELEVATION>, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
   launch_ex(c, KID_RING_SCAN, k_ring_scan, dim3(nb), dim3(1024), 0, 1, true, ra, c->cfg.n_scans);
   launch_ex(c, KID_SCATTER, k_scatter, dim3(blocks, nb), dim3(256), 0, 1, true, sa);
   *sc_slot = c->parity;

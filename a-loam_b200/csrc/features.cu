@@ -1,6 +1,7 @@
 // Feature extraction on the GPU -- replaces scanRegistration.cpp:85-112,129-408.
 //
-//   k_classify   (thread / return)   NaN + minimum-range removal (:85-112,136-137), elevation -> ring id (:166-205),
+//   k_classify   (thread / return)   NaN + minimum-range removal (:85-112,136-137), elevation -> ring id (:166-205) or, with
+//                                    cfg.ring_source = ALOAM_RING_FIELD, the driver's ring in float 3 of the raw point,
 //                                    sweep-start azimuth (:141), the return that flips `halfPassed` (:209-224, found
 //                                    with a parallel min instead of the sequential state machine), per-block ring
 //                                    histograms for the stable counting sort that replaces laserCloudScans[] (:240)
@@ -67,6 +68,22 @@ __device__ __forceinline__ void load_xyz(const float* __restrict__ raw, int i, i
   }
 }
 
+// the driver's ring id w (float 3 of a raw point, ALOAM_RING_FIELD): w when it is an integer in 0 .. n_scans - 1, else -1, the
+// id of a dropped return.  NaN fails every comparison, +-inf and 1e9 fail the range, 2.5 the integer test; -0.0 is ring 0
+__device__ __forceinline__ int ring_field(float w, int n_scans) {
+  return w >= 0.f && w < (float)n_scans && w == truncf(w) ? (int)w : -1;
+}
+
+__device__ __forceinline__ void load_xyzw(const float* __restrict__ raw, int i, int stride, float& x, float& y, float& z, float& w) {
+  if (stride == 4) {
+    float4 v = __ldg(reinterpret_cast<const float4*>(raw) + i);
+    x = v.x; y = v.y; z = v.z; w = v.w;
+  } else {
+    const float* p = raw + (size_t)i * stride;
+    x = __ldg(p); y = __ldg(p + 1); z = __ldg(p + 2); w = __ldg(p + 3);
+  }
+}
+
 // azimuth of a return before the halfPassed flip (:208-218)
 __device__ __forceinline__ float ori_first_half(float x, float y, float start_ori) {
   float ori = -atan2f(y, x);
@@ -78,6 +95,7 @@ __device__ __forceinline__ float ori_first_half(float x, float y, float start_or
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
+template <int RingSource>
 __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2) {
   pdl_launch_dependents();   // the next kernel of the stream may become resident (it blocks in pdl_wait())
   // blockIdx.y = trajectory (lane) of the batch; a lane with fewer returns than the largest one has idle trailing CTAs
@@ -117,11 +135,13 @@ __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<C
   for (int it = 0; it < ITERS; ++it) {
     int i = blockIdx.x * CHUNK + it * CT + tid;
     if (i >= n) continue;
-    float x, y, z; load_xyz(raw, i, stride, x, y, z);
+    float x, y, z, w = 0.f;
+    if (RingSource == ALOAM_RING_FIELD_DEV) load_xyzw(raw, i, stride, x, y, z, w);
+    else load_xyz(raw, i, stride, x, y, z);
     int ring = -2;
     if (point_ok(x, y, z, thres2)) {
       my_last = max(my_last, i);
-      ring = ring_of(x, y, z, n_scans);
+      ring = RingSource == ALOAM_RING_FIELD_DEV ? ring_field(w, n_scans) : ring_of(x, y, z, n_scans);
       if (ring >= 0) {
         atomicAdd(&s_hist[ring], 1);
         float ori = ori_first_half(x, y, start_ori);
@@ -140,6 +160,8 @@ __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<C
     if (blockIdx.x == 0) { sc->first_valid = first; sc->start_ori = start_ori; }
   }
 }
+template __global__ void k_classify<ALOAM_RING_ELEVATION_DEV>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
+template __global__ void k_classify<ALOAM_RING_FIELD_DEV>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
 
 // ---------------------------------------------------------------------------------------------------------------
 // one CTA of 1024 threads: thread (r = t>>4, s = t&15) owns slice s of ring r's per-block histogram column

@@ -2,6 +2,7 @@
 // pcl::PointXYZI.  No device code; the file has a .cu suffix only because the library is built from one source list.
 // Follows kittiHelper.cpp:25-35 (file read), :78-80 and :97-113 (pose parsing through float, camera -> lidar frame).
 #include <cmath>
+#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -144,6 +145,23 @@ int aloam_io_unpack_points(const unsigned char* data, long n, int point_step, in
     std::memcpy(xyzi + 4 * i + 2, p + off_z, 4);
     if (off_intensity >= 0) std::memcpy(xyzi + 4 * i + 3, p + off_intensity, 4);
     else xyzi[4 * i + 3] = 0.f;
+  }
+  return 0;
+}
+
+int aloam_io_unpack_points_ring(const unsigned char* data, long n, int point_step, int off_x, int off_y, int off_z, int off_ring,
+                                int ring_type, float* xyzr) {
+  const int ring_bytes = ring_type == 2 ? 1 : ring_type == 4 ? 2 : 0;   // sensor_msgs/PointField UINT8, UINT16
+  if (!data || !xyzr || n < 0 || ring_bytes == 0 || point_step < 12 || off_x < 0 || off_y < 0 || off_z < 0 || off_ring < 0) return -1;
+  if (off_x + 4 > point_step || off_y + 4 > point_step || off_z + 4 > point_step || off_ring + ring_bytes > point_step) return -1;
+  for (long i = 0; i < n; ++i) {
+    const unsigned char* p = data + (size_t)point_step * i;
+    std::memcpy(xyzr + 4 * i, p + off_x, 4);
+    std::memcpy(xyzr + 4 * i + 1, p + off_y, 4);
+    std::memcpy(xyzr + 4 * i + 2, p + off_z, 4);
+    uint16_t r = p[off_ring];
+    if (ring_bytes == 2) std::memcpy(&r, p + off_ring, 2);   // little-endian payload (is_bigendian = false)
+    xyzr[4 * i + 3] = (float)r;
   }
   return 0;
 }

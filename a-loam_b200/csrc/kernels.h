@@ -6,6 +6,8 @@
 
 #define ALOAM_MAX_RING 4096                  // == ALOAM_MAX_RING_POINTS of the public header
 #define ALOAM_ERR_RING_TOO_LARGE_DEV (-7)    // == ALOAM_ERR_RING_TOO_LARGE
+#define ALOAM_RING_ELEVATION_DEV 0           // == ALOAM_RING_ELEVATION
+#define ALOAM_RING_FIELD_DEV 1               // == ALOAM_RING_FIELD
 #define ALOAM_LM_THREADS 288
 #define ALOAM_LM_MAX_TRACE 8
 #define ALOAM_N_KERNEL_IDS 32
@@ -32,6 +34,8 @@ struct RingFeatArgs { const Pt4* full; const int* ring_start; Pt4 *st_sharp, *st
                       float* dbg_curv; int8_t* dbg_label; ScanScalars* sc; };
 struct CompactArgs { const Pt4 *st_sharp, *st_less_sharp, *st_flat, *st_less_flat; const int* st_counts; Pt4 *sharp, *less_sharp, *flat, *less_flat;
                      int* counts; };
+// RingSource: where a return's ring comes from, ALOAM_RING_ELEVATION_DEV or ALOAM_RING_FIELD_DEV (both instances in features.cu)
+template <int RingSource>
 __global__ void k_classify(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);          // grid (blocks, lanes)
 __global__ void k_ring_scan(const __grid_constant__ Batch<RingScanArgs> B, int n_scans);                       // grid (lanes)
 __global__ void k_scatter(const __grid_constant__ Batch<ScatterArgs> B);                                       // grid (blocks, lanes)

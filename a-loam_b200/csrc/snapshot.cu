@@ -42,6 +42,7 @@ long long store_offset(const SnapHeader& h) { return (long long)sizeof(SnapHeade
 int check_header(const SnapHeader& h, long long n_bytes) {
   if (std::memcmp(h.magic, kMagic, 8) != 0 || h.version != kSnapVersion) return ALOAM_ERR_SNAPSHOT;
   if ((h.mapped != 0 && h.mapped != 1) || h.scan_index < 1 || h.n_less_sharp < 0 || h.n_less_flat < 0) return ALOAM_ERR_SNAPSHOT;
+  if (h.ring_source != ALOAM_RING_ELEVATION && h.ring_source != ALOAM_RING_FIELD) return ALOAM_ERR_SNAPSHOT;
   if (h.total_bytes != n_bytes) return ALOAM_ERR_SNAPSHOT;
   if (!all_finite(h.warm, 7) || !all_finite(h.world, 7)) return ALOAM_ERR_SNAPSHOT;
   if (!h.mapped) return n_bytes == store_offset(h) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
@@ -84,7 +85,7 @@ int check_store(const SnapHeader& h, const SnapStore& s) {
 // the configuration fields of the header that can change a result
 void fingerprint(const aloam_ctx* c, SnapHeader* h) {
   const aloam_config& g = c->cfg;
-  h->n_scans = g.n_scans; h->distortion = g.distortion; h->mapping_skip_frame = g.mapping_skip_frame;
+  h->n_scans = g.n_scans; h->ring_source = g.ring_source; h->distortion = g.distortion; h->mapping_skip_frame = g.mapping_skip_frame;
   h->outer_iters = g.outer_iters; h->inner_iters = g.inner_iters;
   h->minimum_range = g.minimum_range; h->line_res = g.line_res; h->plane_res = g.plane_res;
   mapper_slab_caps(c, h->slab_cap);
@@ -96,7 +97,7 @@ void fingerprint(const aloam_ctx* c, SnapHeader* h) {
 // only for a mapped snapshot: an odometry-only trajectory moves between contexts that map differently (or not at all).
 bool same_config(const SnapHeader& s, const SnapHeader& c) {
   auto same = [](const void* a, const void* b, size_t n) { return std::memcmp(a, b, n) == 0; };
-  const bool odometry = s.n_scans == c.n_scans && s.distortion == c.distortion && s.outer_iters == c.outer_iters && s.inner_iters == c.inner_iters &&
+  const bool odometry = s.n_scans == c.n_scans && s.ring_source == c.ring_source && s.distortion == c.distortion && s.outer_iters == c.outer_iters && s.inner_iters == c.inner_iters &&
                         same(&s.minimum_range, &c.minimum_range, 4) && same(&s.huber, &c.huber, 8) && same(&s.dist_sq_thresh, &c.dist_sq_thresh, 8) &&
                         same(&s.nearby_scan, &c.nearby_scan, 8);
   const bool mapping = s.mapping_skip_frame == c.mapping_skip_frame && same(&s.line_res, &c.line_res, 4) && same(&s.plane_res, &c.plane_res, 4) &&

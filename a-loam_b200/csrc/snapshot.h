@@ -26,12 +26,13 @@ struct SnapHeader {
   double huber, dist_sq_thresh, nearby_scan;
   double warm[7];                      // para_q / para_t of the next scan's solve
   double world[7];                     // world pose of the lane's last scan
-  char zero[40];
+  int32_t ring_source;                 // 0 elevation (what a snapshot written before the field held), 1 driver ring
+  char zero[36];
 };
 static_assert(sizeof(SnapHeader) == 256, "snapshot header");
 static_assert(offsetof(SnapHeader, scan_index) == 24 && offsetof(SnapHeader, n_scans) == 36 && offsetof(SnapHeader, minimum_range) == 56 &&
               offsetof(SnapHeader, slab_cap) == 68 && offsetof(SnapHeader, huber) == 80 && offsetof(SnapHeader, warm) == 104 &&
-              offsetof(SnapHeader, world) == 160, "snapshot header layout");
+              offsetof(SnapHeader, world) == 160 && offsetof(SnapHeader, ring_source) == 216, "snapshot header layout");
 
 // section 2 at offset 256: n_less_sharp, then n_less_flat points of 4 floats.  Section 3 (mapped snapshots only) follows: this
 // table, then n_points points of 4 floats in ALOAM_EXPORT_MAP order

@@ -25,6 +25,8 @@ def _lib():
         L.aloam_io_pack_pointxyzi.argtypes = [C.POINTER(C.c_float), C.c_long, C.POINTER(C.c_ubyte)]
         L.aloam_io_pack_pointxyzi.restype = None
         L.aloam_io_unpack_points.argtypes = [C.POINTER(C.c_ubyte), C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]
+        L.aloam_io_unpack_points_ring.argtypes = [C.POINTER(C.c_ubyte), C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                  C.POINTER(C.c_float)]
         _LIB = L
     return _LIB
 
@@ -89,4 +91,21 @@ def unpack_points(data, n, point_step=32, off_x=0, off_y=4, off_z=8, off_intensi
                                        out.ctypes.data_as(C.POINTER(C.c_float)))
     if rc != 0:
         raise ValueError("bad PointCloud2 layout")
+    return out
+
+
+RING_UINT8, RING_UINT16 = 2, 4   # sensor_msgs/PointField datatypes of a driver's ring field
+
+
+def unpack_points_ring(data, n, point_step, off_x, off_y, off_z, off_ring, ring_type):
+    """(n, 4) float32 x, y, z, ring from a PointCloud2 payload with a ring field (ring_type RING_UINT8 or RING_UINT16): the raw
+    scan of a context with ring_source = RING_FIELD"""
+    d = np.ascontiguousarray(data, np.uint8)
+    if len(d) < n * point_step:
+        raise ValueError("payload shorter than n * point_step")
+    out = np.zeros((n, 4), np.float32)
+    rc = _lib().aloam_io_unpack_points_ring(d.ctypes.data_as(C.POINTER(C.c_ubyte)), n, point_step, off_x, off_y, off_z, off_ring,
+                                            ring_type, out.ctypes.data_as(C.POINTER(C.c_float)))
+    if rc != 0:
+        raise ValueError("bad PointCloud2 layout or ring type")
     return out

@@ -1,4 +1,5 @@
-"""Seeded synthetic lidar scans (VLP-16 / HDL-32 / HDL-64 shaped) -- ctypes binding of synth.cc."""
+"""Seeded synthetic lidar scans (VLP-16 / HDL-32 / HDL-64 shaped, and sensors that report each return's ring) -- ctypes binding
+of synth.cc."""
 import ctypes as C
 import math
 import os
@@ -15,6 +16,23 @@ SENSORS = {  # name -> (n_scans, azimuth steps, minimum_range [launch/*.launch],
     "HDL-64": (64, 2000, 5.0, 0.4, 0.8),
 }
 BASE_SEED = 20240901
+
+# Sensors whose driver reports each return's ring (aloam_config.ring_source = ALOAM_RING_FIELD): name -> (beam elevations [deg]
+# in ring order, ring 0 first; azimuth steps).  Apart from the edge tables R1 / R2, none of them is binned right by a Velodyne
+# formula of the reference.  Shaped like:
+#   OS64  an Ouster OS1-64: uniform +16.6 .. -16.6 deg, ring 0 the highest beam
+#   V32C  a Velodyne VLP-32C: the non-uniform table, ring 0 the lowest beam
+#   L40   40 uniform beams -25 .. +15 deg (a ring count that is not a power of two), ring 0 the lowest
+#   R1, R2  one and two beams, the edges of the ring count
+RING_SENSORS = {
+    "OS64": (tuple(16.6 - k * 33.2 / 63 for k in range(64)), 1024),
+    "V32C": ((-25.0, -15.639, -11.31, -8.843, -7.254, -6.148, -5.333, -4.667, -4.0) + tuple(-4.0 + k / 3.0 for k in range(1, 18)) +
+             (2.333, 3.333, 4.667, 7.0, 10.333, 15.0), 1800),
+    "L40": (tuple(-25.0 + k * 40.0 / 39 for k in range(40)), 1200),
+    "R1": ((-4.0,), 1800),
+    "R2": ((-8.0, 2.0), 1800),
+}
+RING_RANGES = (0.3, 0.2, 0.4)   # minimum_range, line_res, plane_res of every RING_SENSORS sensor
 
 
 def build(force=False):
@@ -40,6 +58,9 @@ def _lib():
         L.synth_scan_beams.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
                                        C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int,
                                        C.c_int, C.c_double, C.POINTER(C.c_float), C.POINTER(C.c_int), C.c_int]
+        L.synth_scan_rings.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int,
+                                       C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_int, C.c_int, C.c_double,
+                                       C.POINTER(C.c_float), C.c_int]
         _LIB = L
     return _LIB
 
@@ -130,6 +151,33 @@ def scan_beams(sensor, index, elevations_deg, z_offsets_m=None, cut=None, covera
     if n < 0:
         raise RuntimeError("synth_scan_beams failed: %d" % n)
     return (out[:n].copy(), beams[:n].copy()) if return_beams else out[:n].copy()
+
+
+def scan_rings(sensor, index, reverse=False, cut=None, coverage=1.0, laser_major=False, ccw=False, seed=BASE_SEED, n_az=None,
+               noise=0.02, max_range=120.0):
+    """Raw scan `index` of the trajectory from RING_SENSORS[sensor], with its driver ring: (n, 4) float32 x, y, z, ring.  The
+    ring of laser b is b, or n_beams - 1 - b with reverse (the other elevation order).  cut, coverage, laser_major and ccw as
+    for scan_seam().  Raises SeamTooClose when a return that survives minimum_range (RING_RANGES) sits within 1e-5 rad of an
+    azimuth threshold of the sweep walk: every such return takes part in it."""
+    elev, az = RING_SENSORS[sensor]
+    if n_az is not None:
+        az = n_az
+    el = np.ascontiguousarray(elev, np.float64)
+    nb = el.shape[0]
+    rings = np.arange(nb, dtype=np.int32)
+    if reverse:
+        rings = np.ascontiguousarray(rings[::-1])
+    start_col = 0.0 if cut is None else (math.pi - cut) * az / (2 * math.pi) - 0.37
+    n_col = int(round(coverage * az))
+    out = np.zeros((nb * n_col, 4), np.float32)
+    n = _lib().synth_scan_rings(seed, az, index, noise, max_range, start_col, n_col, nb, el.ctypes.data_as(C.POINTER(C.c_double)),
+                                rings.ctypes.data_as(C.POINTER(C.c_int)), None, int(laser_major), int(ccw), RING_RANGES[0],
+                                out.ctypes.data_as(C.POINTER(C.c_float)), out.shape[0])
+    if n == -3:
+        raise SeamTooClose("scan_rings(%s, %d): a return lies on an azimuth threshold" % (sensor, index))
+    if n < 0:
+        raise RuntimeError("synth_scan_rings failed: %d" % n)
+    return out[:n].copy()
 
 
 def pose(index):

@@ -210,6 +210,7 @@ int reference_ring(float x, float y, float z, int n_scans) {
 // device atan2f differ in the last ulp, so a return closer than kSeamMargin to a threshold it is tested against could take
 // the other branch on the GPU.  Replays the reference's walk over the surviving returns and returns -3 if one is that close
 // (a return near the half-sweep test is checked against the thresholds of both halves, since the flag may flip there).
+// n_scans = 0: every surviving return takes part in the walk (rings from the driver, not from a formula).
 constexpr double kSeamMargin = 1e-5;
 int check_seam_margins(const float* pts, int n, int n_scans, double minimum_range) {
   const float thres = (float)minimum_range;
@@ -232,7 +233,7 @@ int check_seam_margins(const float* pts, int n, int n_scans, double minimum_rang
   bool half = false;
   for (int i : keep) {
     const float* p = pts + (size_t)i * 4;
-    if (reference_ring(p[0], p[1], p[2], n_scans) < 0) continue;   // dropped before the azimuth walk (:174-175)
+    if (n_scans > 0 && reference_ring(p[0], p[1], p[2], n_scans) < 0) continue;   // dropped before the azimuth walk (:174-175)
     float ori = ori_of(i);
     const bool pre_near = near(ori, start - M_PI / 2) || near(ori, start + M_PI * 3 / 2);
     const bool post_near = near(ori + 2 * M_PI, end - M_PI * 3 / 2) || near(ori + 2 * M_PI, end + M_PI / 2);
@@ -253,10 +254,11 @@ int check_seam_margins(const float* pts, int n, int n_scans, double minimum_rang
 int generate(uint64_t seed, int n_scans, int n_az, int scan_index, double noise_sigma, double max_range, const Layout& lay,
              float* out, int* beam_out, int capacity) {
   std::vector<double> elev;
-  if (sensor_elevations(n_scans, elev) != 0) return -1;
   if (lay.elev) {
     if (lay.n_beams <= 0) return -2;
     elev.assign(lay.elev, lay.elev + lay.n_beams);
+  } else if (sensor_elevations(n_scans, elev) != 0) {
+    return -1;
   }
   const int nb = (int)elev.size();
   const int n_col = lay.n_col;
@@ -382,6 +384,24 @@ int synth_scan_beams(uint64_t seed, int n_scans, int n_az, int scan_index, doubl
   const int n = generate(seed, n_scans, n_az, scan_index, noise_sigma, max_range, lay, out, beam_out, capacity);
   if (n < 0) return n;
   const int rc = check_seam_margins(out, n, n_scans, minimum_range);
+  return rc ? rc : n;
+}
+
+// A sensor that reports each return's ring (a driver's `ring` field): n_beams lasers at elev_deg[b], laser b's returns carry
+// ring_of_beam[b] in float 3.  Cut and fired like synth_scan_seam (ring_off_deg: n_beams entries, may be null).  No formula
+// drops a return, so the seam margins are checked on every return that survives minimum_range (-3 like synth_scan_seam).
+int synth_scan_rings(uint64_t seed, int n_az, int scan_index, double noise_sigma, double max_range, double start_col, int n_col,
+                     int n_beams, const double* elev_deg, const int* ring_of_beam, const double* ring_off_deg, int laser_major, int ccw,
+                     double minimum_range, float* out, int capacity) {
+  if (!elev_deg || !ring_of_beam || n_beams <= 0) return -2;
+  Layout lay;
+  lay.start_col = start_col; lay.n_col = n_col; lay.ring_off = ring_off_deg; lay.laser_major = laser_major; lay.ccw = ccw;
+  lay.n_beams = n_beams; lay.elev = elev_deg;
+  std::vector<int> beam((size_t)std::max(capacity, 0));
+  const int n = generate(seed, 0, n_az, scan_index, noise_sigma, max_range, lay, out, beam.data(), capacity);
+  if (n < 0) return n;
+  for (int i = 0; i < n; ++i) out[(size_t)i * 4 + 3] = (float)ring_of_beam[beam[i]];
+  const int rc = check_seam_margins(out, n, 0, minimum_range);
   return rc ? rc : n;
 }
 

@@ -30,7 +30,8 @@ extern "C" {
 
 #define ALOAM_OK 0
 #define ALOAM_ERR_INVALID_ARG (-1)
-#define ALOAM_ERR_UNSUPPORTED_SCANS (-2) /* scanRegistration.cpp:472-476: only 16, 32 or 64 scan lines */
+#define ALOAM_ERR_UNSUPPORTED_SCANS (-2) /* scanRegistration.cpp:472-476: only 16, 32 or 64 scan lines under
+                                            ALOAM_RING_ELEVATION; 1..64 under ALOAM_RING_FIELD */
 #define ALOAM_ERR_EMPTY_CLOUD (-3)       /* no point survives the NaN / minimum-range filter */
 #define ALOAM_ERR_CAPACITY (-4)          /* more points than the ctx was created for */
 #define ALOAM_ERR_CUDA (-5)
@@ -83,7 +84,28 @@ typedef struct aloam_config {
   int mapping_skip_frame; /* mapping_skip_frame laserOdometry.cpp:191, launch/...:6 -- the mapped stream calls map every k-th scan
                             of a trajectory and give the others the high-frequency pose (see aloam_scan_stream_mapped).  Default 1
                             (every scan); 0 counts as 1 (zero-initialised tail of an older caller); < 0 is rejected by aloam_create */
+  int ring_source;       /* where a raw return's ring id comes from (see below); 0 = ALOAM_RING_ELEVATION, the default and what a
+                            zero-initialised tail of an older caller gets; any other value than 0 or 1 is ALOAM_ERR_INVALID_ARG */
 } aloam_config;
+
+/* Ring sources (aloam_config.ring_source).  Every entry point that takes a raw scan uses it: aloam_extract_features,
+ * aloam_scan_to_pose(_device) and every stream call, device-resident raws included.
+ *   ALOAM_RING_ELEVATION  the reference's elevation formula of the configured Velodyne (scanRegistration.cpp:166-205);
+ *                         n_scans must be 16, 32 or 64.
+ *   ALOAM_RING_FIELD      the sensor driver's ring: float 3 of every raw point (the 4th float, at stride 4 and 8 alike; the
+ *                         reference never reads that slot of a raw scan).  n_scans may be 1..64.  After the NaN and
+ *                         minimum-range filters a return's ring is w = float 3 when w is finite, integral and 0 <= w < n_scans;
+ *                         any other w drops the return as an out-of-range formula id does (it does not count in the sweep walk
+ *                         either, scanRegistration.cpp:174-175).  Everything after the ring binning is unchanged: the azimuth
+ *                         walk, relTime, intensity = ring + 0.1 relTime, the per-ring features and voxel filter.
+ *                         The ids must number the beams in elevation order, in either direction (Velodyne drivers put ring 0
+ *                         at the lowest beam, Ouster drivers at the highest): the scan-to-scan association's NEARBY_SCAN
+ *                         window assumes that neighbouring ids are neighbouring beams.  This is not checked.  A ring still
+ *                         holds at most cfg.max_ring_points returns (ALOAM_ERR_RING_TOO_LARGE).
+ * aloam_default_config(cfg, n) fills the VLP-16 / HDL-32 launch values for every n other than 64, and ring_source = 0: a caller
+ * with another sensor sets n_scans, ring_source and, where its sensor needs them, minimum_range, line_res and plane_res. */
+#define ALOAM_RING_ELEVATION 0
+#define ALOAM_RING_FIELD 1
 
 typedef struct aloam_cloud_view {
   const float* data;
@@ -256,7 +278,7 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  * ALOAM_LANE_SCAN, in the saved mode (map_poses set or not), gives exactly what the uninterrupted trajectory would have -- odometry
  * and map poses, stats, cube store, published and registered clouds.  blob: as `out` of aloam_lane_save, n_bytes its size
  * exactly.  It needs the configuration the snapshot was taken under in every field that can change a result: n_scans,
- * minimum_range, outer_iters, inner_iters, huber, dist_sq_thresh, nearby_scan and distortion, and for a mapped snapshot also
+ * ring_source, minimum_range, outer_iters, inner_iters, huber, dist_sq_thresh, nearby_scan and distortion, and for a mapped snapshot also
  * line_res, plane_res, mapping_skip_frame, max_map_points and the slab capacities min(16384, max_points) / min(65536, max_points)
  * (floating-point fields compared bit for bit).  max_points beyond the slab capacities, max_batch, max_ring_points and device do
  * not count.  Errors: ALOAM_ERR_INVALID_ARG (bad lane or buffer: nothing changes), ALOAM_ERR_STATE on a rank of a sharded job or
@@ -286,7 +308,8 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  *       configuration: 36 int32 n_scans   40 int32 distortion   44 int32 mapping_skip_frame   48 int32 outer_iters
  *       52 int32 inner_iters   56 float minimum_range   60 float line_res   64 float plane_res   68 int32 slab_cap[2]
  *       76 int32 max_map_points   80 double huber   88 double dist_sq_thresh   96 double nearby_scan
- *      104 double warm[7] (q_last_curr xyzw, t_last_curr: the next scan's warm start)   160 double world[7]   216 zero to 256
+ *      104 double warm[7] (q_last_curr xyzw, t_last_curr: the next scan's warm start)   160 double world[7]
+ *      216 int32 ring_source (0 or 1; snapshots written before the field existed hold 0 there, the elevation source)   220 zero to 256
  *   2. at 256: n_less_sharp, then n_less_flat points of 4 floats (x, y, z, intensity) -- the lane's "last" clouds
  *   3. mapped snapshots only, at S = 256 + 16 (n_less_sharp + n_less_flat): the cube store
  *      S+0 int32 cen[3]   S+12 int32 n_valid (<= 125)   S+16 int32 valid[128] (unused entries 0)   S+528 int32 frames

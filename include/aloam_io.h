@@ -34,6 +34,12 @@ void aloam_io_lidar_pose_to_kitti(const double q[4], const double t[3], double T
 void aloam_io_pack_pointxyzi(const float* xyzi, long n, unsigned char* data32);
 int aloam_io_unpack_points(const unsigned char* data, long n, int point_step, int off_x, int off_y, int off_z,
                            int off_intensity /* < 0: none, intensity = 0 */, float* xyzi);
+/* PointCloud2 `data` of a driver cloud with a per-return ring field -> packed x,y,z,ring: the raw scan of
+ * cfg.ring_source = ALOAM_RING_FIELD (float 3 = the ring id).  ring_type is the sensor_msgs/PointField datatype of the ring
+ * field: 2 (UINT8) or 4 (UINT16), the types Velodyne (PointXYZIR: uint16 at byte 20 of 32) and Ouster drivers publish;
+ * little-endian payloads.  Returns 0, or -1 for another ring_type or an offset whose field does not fit in point_step. */
+int aloam_io_unpack_points_ring(const unsigned char* data, long n, int point_step, int off_x, int off_y, int off_z, int off_ring,
+                                int ring_type, float* xyzr);
 
 #ifdef __cplusplus
 }
