@@ -31,7 +31,7 @@ EXPORTED_SYMBOLS = [
     "aloam_prior_map_build", "aloam_prior_relocalise",
     "aloam_set_map_rows", "aloam_map_rows",
     "aloam_set_recovery", "aloam_recovery_rows", "aloam_debug_recovery_scores",
-    "aloam_lane_map_on_prior",
+    "aloam_lane_map_on_prior", "aloam_set_cube_growth",
     "aloam_io_unpack_points_ring",
 ]
 ERR_SNAPSHOT = -11
@@ -40,6 +40,7 @@ EXPORT_SURROUND, EXPORT_MAP = 0, 1
 PRIOR_MAP = -1   # `lane` of mapper_export: the context's prior map
 ROW_IDLE, ROW_MAPPED, ROW_LOCALISED, ROW_SKIPPED = 0, 1, 2, 3   # aloam_map_row.kind
 RING_ELEVATION, RING_FIELD = 0, 1   # aloam_config.ring_source: the elevation formula, or the driver's ring in float 3 of a raw point
+MAX_CUBE_POINTS = 262144   # ALOAM_MAX_CUBE_POINTS: the most points one map cube holds with cube growth on (set_cube_growth)
 
 
 class Config(C.Structure):
@@ -178,6 +179,7 @@ def lib():
         L.aloam_prior_map_build.argtypes = [C.c_void_p, cv, cv, ip, C.POINTER(C.c_longlong)]
         L.aloam_lane_localise.argtypes = [C.c_void_p, C.c_int, dp, dp]
         L.aloam_lane_map_on_prior.argtypes = [C.c_void_p, C.c_int, dp, dp]
+        L.aloam_set_cube_growth.argtypes = [C.c_void_p, C.c_int]
         L.aloam_debug_prior_associate.argtypes = [C.c_void_p, C.c_int, cv, cv, dp, dp]
         L.aloam_prior_relocalise.argtypes = [C.c_void_p, cv, cv, dp, C.c_int, C.POINTER(RelocOpts), ip, C.POINTER(RelocResult)]
         L.aloam_set_map_rows.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int]
@@ -734,6 +736,13 @@ class Aloam:
         if q.shape != (4,) or t.shape != (3,):
             raise ValueError("q_init is 4 doubles (x, y, z, w), t_init 3")
         _check(lib().aloam_lane_map_on_prior(self._h, int(lane), _dp(q), _dp(t)))
+
+    def set_cube_growth(self, on):
+        """turns cube growth on (1) or off (0, the default) for the lanes that start a mapped trajectory from now on (aloam_set_cube_growth):
+        a cube whose slab fills moves to a larger run of slabs of the same pool, up to MAX_CUBE_POINTS points, instead of dropping
+        points; lane 0 of mapper_step takes the setting at mapper_reset, a restored lane its snapshot's.  Drops every
+        lane_map_on_prior arming."""
+        _check(lib().aloam_set_cube_growth(self._h, int(on)))
 
     def prior_relocalise(self, hyps, less_sharp=None, less_flat=None, raw=None, inlier_sq=1.0, max_score_points=1024, refine=1,
                          scores=True):

@@ -292,6 +292,7 @@ struct aloam_ctx {
   // pinned host mirrors
   Pt4* h_out[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   Pt4* h_vox_out = nullptr;     // result of aloam_voxel_filter (never aliases the feature views)
+  Pt4* h_cube = nullptr;        // aloam_mapper_debug_cube of a cube beyond max_points (cube growth), created on first use
   PinnedScratch* pin = nullptr;
   LmSummary* h_summary = nullptr;   // [n_lanes][4]
   ScanScalars* h_sc = nullptr;      // [n_lanes][3]
@@ -329,6 +330,8 @@ struct aloam_ctx {
   // the seeded STARTs of a step (aloam_lane_map_on_prior): the ALOAM_EXPORT_MAP layout of record l's new store, [n_lanes], created
   // by the first stream call that seeds a store
   ExportLayout* d_seed_layout = nullptr;
+  // aloam_set_cube_growth: what a lane's store takes at its next mapped START (lane 0 of the host API at aloam_mapper_reset)
+  bool cube_growth = false;
 };
 
 namespace {
@@ -467,9 +470,11 @@ int snapshot_validate(aloam_ctx* c, const char* b, long long n_bytes, int kind, 
 // its centre cube lies at most kCubeSlack cubes outside the buffer on every axis, so the frame's shift loop ends
 bool map_position_fits(const double p[3], const int cen[3]);
 void mapper_slab_caps(const aloam_ctx* c, int cap[2]);
-int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head);
+// cubemap.cu: the largest run of a lane store per type (2^ord[t] slabs) under cube growth `growth`
+void mapper_run_orders(const aloam_ctx* c, bool growth, int ord[2]);
+int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head, int* growth);
 int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device);
-int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device);
+int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device, bool growth);
 int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf);
 int ensure_map_buffers(aloam_ctx* c);
 int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids = true);

@@ -4,17 +4,18 @@
 //
 // Second version: the WHOLE frame runs on the device without a host synchronisation, so it can sit at the end of the scan
 // stream (aloam_scan_stream_mapped) or behind the host API (aloam_mapper_step, one sync at the end to return the pose):
-//   * state (T_wmap_wodom, centre offsets, cube -> slab table, per-slab counts, slab free list) lives in device memory;
+//   * state (T_wmap_wodom, centre offsets, cube -> run table, per-run counts and orders, slab occupancy bitmaps) lives in device memory;
 //   * k_mapper_begin : transformAssociateToMap, centre cube, ring-buffer shift (the reference rotates 4851 smart pointers;
-//                      here one CTA permutes the cube -> slab table, one thread per line of cubes, and returns the slabs
-//                      of the cubes that scroll out to the free list), valid-cube list in the reference's i, j, k order;
+//                      here one CTA permutes the cube -> run table, one thread per line of cubes, and frees the runs of
+//                      the cubes that scroll out), valid-cube list in the reference's i, j, k order;
 //   * k_mapper_gather: the <= 75 valid cubes device-to-device into the submap, then the hash-grid build of mapping.cu;
 //   * the two scan-stack filters as ONE segmented VoxelGrid (voxel.cu), the registration of mapping.cu on device views;
 //   * k_mapper_update: transformUpdate, refined pose out;
-//   * k_cube_ids / k_cube_insert: pointAssociateToMap + cube of the stored point, then a STABLE append (push_back order =
-//                      stack order): one CTA walks the stack in chunks, warps take turns, __match_any groups the lanes of a
-//                      cube and the group leader advances the cube's running end (allocating a slab from the free list
-//                      for a cube that was empty) -- O(n) instead of the O(n^2 / 256) rank search of the first version;
+//   * k_cube_ids / k_cube_insert: pointAssociateToMap + cube of the stored point, then a count pass, the runs every cube
+//                      needs (a new cube's first run, a grown cube's larger one, in the order of their first stack point),
+//                      the move of grown cubes, and a STABLE append (push_back order = stack order): one CTA walks the
+//                      stack in chunks, warps take turns, __match_any groups the lanes of a cube and the group leader
+//                      advances the cube's running end -- O(n) instead of the O(n^2 / 256) rank search of the first version;
 //   * the per-cube re-filter of the valid cubes as ONE segmented VoxelGrid over up to 150 segments, in place.
 //   * the published clouds (:806-848): k_export_sizes lays a lane's store out in the reference's order and k_store_copy copies it
 //                      (aloam_mapper_export), k_register_full moves a mapped scan's full cloud by the frame's refined pose.
@@ -23,7 +24,9 @@
 //                      (hand-off, centre cube, clipped 5 x 5 x 3 window -- no shift), the stack filters, the registration of
 //                      mapping.cu through k_map_knn5_prior, k_mapper_update: no gather, no index build, no insertion, no re-filter.
 // Slabs are a POOL (1024 per cloud type, 16 k corner / 64 k surf points each: 1.3 GB) handed out on the device on first
-// insertion, not 4851 x 2 slabs (6.4 GB) up front.  A full slab or an exhausted pool drops the overflow and raises
+// insertion, not 4851 x 2 slabs (6.4 GB) up front.  A cube holds an aligned RUN of 2^k slabs (k = 0 while its lane's cube
+// growth is off, aloam_set_cube_growth); with growth on a cube whose run fills moves to the smallest run that holds its new
+// count, up to ALOAM_MAX_CUBE_POINTS.  A cube at its ceiling or a run that cannot be found drops the overflow and raises
 // ALOAM_FLAG_CUBE_OVERFLOW instead of failing the frame (the reference grows its cubes without bound between re-filters).
 #include <climits>
 #include <memory>
@@ -36,6 +39,8 @@ namespace {
 constexpr int CW = 21, CH = 21, CD = 11, NCUBE = CW * CH * CD;   // laserCloudWidth / Height / Depth (:77-82)
 constexpr int kMaxValid = 128;
 constexpr int kPool = 1024;                                      // physical slabs per cloud type
+constexpr int kPoolWords = kPool / 32;                           // words of a type's occupancy bitmap
+constexpr int kMaxOrder = 10;                                    // a run of 2^10 slabs is the whole pool
 static_assert(NCUBE == kSnapCubes && kMaxValid == kSnapValid && kPool == kSnapPool, "the snapshot format describes this store");
 constexpr int kExportSegs = 2 * NCUBE;                           // segments of an export: segment 2 v + t is type t of its v-th cube
 
@@ -66,16 +71,18 @@ struct MapperState {
   int in_counts[2];                          // sizes of the incoming less-sharp / less-flat clouds (host API path)
   int flags;                                 // ALOAM_FLAG_* of this frame
   int frame_err;                             // `err` of the last completed frame (read back with `flags`)
-  int err;                                   // of the running frame -- bit 0: voxel index range, bit 1: slab overflow, bit 2: pool
-                                             // exhausted, bit 3: submap capacity; cleared when the frame ends
+  int err;                                   // of the running frame -- bit 0: voxel index range, bit 1: a cube at its capacity
+                                             // dropped points, bit 2: no free run, bit 3: submap capacity, bit 4: cubes left out
+                                             // of the re-filter (its buffer); cleared when the frame ends
   int err_acc;                               // OR of the frames' words over one aloam_scan_stream_mapped call
   int frames;
   int zero, sink;                            // always 0 (count of a cube without a slab) ; write-only dummy
-  int free_top;                              // slabs [free_top, kPool) of free_list are free ... per type
-  int free_top2;
-  int slab_of[2][NCUBE];                     // cube -> slab of that type, -1 = none
-  int cnt[2][kPool];                         // points per slab
-  int free_list[2][kPool];
+  int max_ord[2];                            // the largest run of the lane's store per type is 2^max_ord slabs: 0 with cube
+                                             // growth off, fixed at the trajectory's start
+  unsigned used[2][kPoolWords];              // slab occupancy per type: bit s of word s / 32 is set while slab s is in a run
+  int slab_of[2][NCUBE];                     // cube -> first slab of its run of that type, -1 = none
+  int cnt[2][kPool];                         // points of the run that starts at a slab
+  unsigned char ord[2][kPool];               // the run that starts at a slab holds 2^ord slabs
 };
 
 }  // namespace
@@ -110,9 +117,9 @@ struct aloam::PriorMap {
   int* d_n = nullptr;            // [2]
   GridTable grid[2] = {};
   ExportLayout* d_layout = nullptr;
-  // per type, from the cube table: the largest cube and the cubes that hold points -- whether a lane store can hold a copy of
-  // the map (aloam_lane_map_on_prior)
-  int max_cube[2] = {0, 0}, n_cubes[2] = {0, 0};
+  // per type, from the cube table: the largest cube, the cubes that hold points and the slabs their runs take with cube growth
+  // on -- whether a lane store can hold a copy of the map (aloam_lane_map_on_prior)
+  int max_cube[2] = {0, 0}, n_cubes[2] = {0, 0}, run_slabs[2] = {0, 0};
 };
 // what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
 // k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
@@ -152,8 +159,15 @@ __host__ __device__ inline int cube_coord(double v, int centre) {
 }
 __host__ __device__ inline int cube_index(int i, int j, int k) { return i + CW * j + CW * CH * k; }
 
+// the slabs of the run of 2^o slabs that starts at slab s: the bits of the occupancy bitmap `used` they cover.  Word w's mask.
+__host__ __device__ inline unsigned run_mask(int s, int o, int w) {
+  const int n = 1 << o;
+  if (n >= 32) return w >= (s >> 5) && w < ((s + n) >> 5) ? ~0u : 0u;
+  return w == (s >> 5) ? ((1u << n) - 1u) << (s & 31) : 0u;
+}
+
 // :327-509 -- one step of the ring buffer along `axis` for the line (u, v) of this thread; towards_high: every cube moves one
-// index up, the top cube wraps to index 0 and is emptied (its slabs go back to the free lists)
+// index up, the top cube wraps to index 0 and is emptied (its run goes back to the pool)
 __device__ void rotate_line(MapperState* S, int axis, bool towards_high, int u, int v) {
   const int n[3] = {CW, CH, CD};
   const int a = axis, b = (axis + 1) % 3, cc = (axis + 2) % 3;
@@ -173,20 +187,25 @@ __device__ void rotate_line(MapperState* S, int axis, bool towards_high, int u, 
     }
     if (wrapped >= 0) {
       S->cnt[ty][wrapped] = 0;
-      const int slot = atomicSub(ty == 0 ? &S->free_top : &S->free_top2, 1) - 1;   // push
-      S->free_list[ty][slot] = wrapped;
+      const int o = S->ord[ty][wrapped];
+      for (int w = wrapped >> 5; w < kPoolWords; ++w) {   // other lines free other runs of the same words
+        const unsigned m = run_mask(wrapped, o, w);
+        if (!m) break;
+        atomicAnd(&S->used[ty][w], ~m);
+      }
     }
   }
 }
 
 // the state of a fresh trajectory (laserMapping.cpp:74-117): identity T_wmap_wodom, centre cube (10, 10, 5), every slab free
-// and no cube holding one.  Run by all threads of one CTA.  It leaves alone the word of the call (err_acc) and every field the
+// and no cube holding one, runs of up to 2^ord0 corner / 2^ord1 surf slabs.  Run by all threads of one CTA.  It leaves alone the word of the call (err_acc) and every field the
 // stack filter writes while k_mapper_begin runs beside it (stack_counts, err, in_counts): between frames `err` is 0 already
 // (k_mapper_finish), and reset_lane zeroes the whole state before it runs this.
-__device__ void mapper_fresh_state(MapperState* S) {
+__device__ void mapper_fresh_state(MapperState* S, int ord0, int ord1) {
   const int tid = threadIdx.x, nt = blockDim.x;
   for (int i = tid; i < NCUBE; i += nt) { S->slab_of[0][i] = -1; S->slab_of[1][i] = -1; }
-  for (int i = tid; i < kPool; i += nt) { S->cnt[0][i] = 0; S->cnt[1][i] = 0; S->free_list[0][i] = i; S->free_list[1][i] = i; }
+  for (int i = tid; i < kPool; i += nt) { S->cnt[0][i] = 0; S->cnt[1][i] = 0; S->ord[0][i] = 0; S->ord[1][i] = 0; }
+  for (int i = tid; i < 2 * kPoolWords; i += nt) S->used[i / kPoolWords][i % kPoolWords] = 0u;
   for (int i = tid; i < kMaxValid; i += nt) S->valid[i] = 0;
   for (int i = tid; i < 2 * (kMaxValid + 1); i += nt) S->sub_off[i / (kMaxValid + 1)][i % (kMaxValid + 1)] = 0;
   if (tid == 0) {
@@ -196,11 +215,11 @@ __device__ void mapper_fresh_state(MapperState* S) {
     S->cen[0] = 10; S->cen[1] = 10; S->cen[2] = 5;
     S->n_valid = 0; S->n_sub[0] = 0; S->n_sub[1] = 0;
     S->flags = 0; S->frame_err = 0; S->frames = 0; S->zero = 0; S->sink = 0;
-    S->free_top = 0; S->free_top2 = 0;
+    S->max_ord[0] = ord0; S->max_ord[1] = ord1;
   }
 }
 // grid (1): the host-side reset of one lane (reset_lane)
-__global__ void __launch_bounds__(1024) k_mapper_reset(MapperState* S) { mapper_fresh_state(S); }
+__global__ void __launch_bounds__(1024) k_mapper_reset(MapperState* S, int ord0, int ord1) { mapper_fresh_state(S, ord0, ord1); }
 
 // transformAssociateToMap (:142-146): x = T_wmap_wodom * odometry pose -- also the high-frequency pose of :214-215
 __device__ __forceinline__ void associate_to_map(const MapperState* S, const double* odom7, double* x) {
@@ -214,11 +233,11 @@ __device__ __forceinline__ void associate_to_map(const MapperState* S, const dou
 }
 
 // transformAssociateToMap (:142-146), centre cube + shift (:314-509), valid cubes (:511-529), gather offsets
-__device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub, bool fresh) {
+__device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* __restrict__ odom7, int max_sub, bool fresh, int ord0, int ord1) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (fresh) {   // the lane starts a new trajectory with this frame: no extra launch, in order on the mapper stream
-    mapper_fresh_state(S);
+    mapper_fresh_state(S, ord0, ord1);
     __syncthreads();
   }
   __shared__ int s_ctr[3], s_cen[3];
@@ -288,10 +307,11 @@ __device__ __forceinline__ void mapper_begin_body(MapperState* S, const double* 
     S->n_sub[ty] = off;
   }
 }
-// grid (1, 1, lanes); bit l of `fresh`: record l starts a new trajectory with this frame, its state is reset first
-__global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub, unsigned fresh) {
+// grid (1, 1, lanes); bit l of `fresh`: record l starts a new trajectory with this frame, its state is reset first, with runs of
+// up to 2^ord0 / 2^ord1 slabs (the context's cube growth)
+__global__ void __launch_bounds__(1024) k_mapper_begin(const __grid_constant__ Batch<MapperLane> B, int max_sub, unsigned fresh, int ord0, int ord1) {
   const MapperLane& a = B.a[blockIdx.z];
-  mapper_begin_body(a.S, a.odom7, max_sub, (fresh >> blockIdx.z) & 1u);
+  mapper_begin_body(a.S, a.odom7, max_sub, (fresh >> blockIdx.z) & 1u, ord0, ord1);
 }
 
 // grid (1, 1, lanes): the scans the mapper skips (mapping_skip_frame > 1) get the high-frequency pose of laserOdometryHandler
@@ -329,7 +349,7 @@ __global__ void __launch_bounds__(256) k_locate_begin(const __grid_constant__ Ba
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   const int tid = threadIdx.x;
   if (a.fresh) {
-    mapper_fresh_state(S);
+    mapper_fresh_state(S, 0, 0);   // (a locator's store tables stay unused)
     __syncthreads();
     if (tid < 4) S->q_wmap_wodom[tid] = a.init[tid];
     else if (tid < 7) S->t_wmap_wodom[tid - 4] = a.init[tid];
@@ -380,7 +400,7 @@ __global__ void __launch_bounds__(256) k_prior_tag(const __grid_constant__ GridT
     const int idx = __float_as_int(g.gpts[s].w);
     int lo = 0, hi = NCUBE;   // t[lo] <= idx < t[hi]
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (t[mid] <= idx) lo = mid; else hi = mid; }
-    g.gpts[s].w = __int_as_float(prior_tag(lo % CW, (lo / CW) % CH, lo / (CW * CH), idx - t[lo]));
+    g.gpts[s].w = __uint_as_float(prior_tag(lo % CW, (lo / CW) % CH, lo / (CW * CH), idx - t[lo]));
   }
 }
 
@@ -463,8 +483,8 @@ __global__ void k_mapper_update(const __grid_constant__ Batch<MapperLane> B) {  
 }
 
 
-// end of the frame, after insertion and re-filter have set their error bits: slab overflow, pool exhaustion and submap
-// truncation become this frame's ALOAM_FLAG_CUBE_OVERFLOW, the frame's word joins the per-call accumulation, and `err` starts
+// end of the frame, after insertion and re-filter have set their error bits: a full cube, no free run, submap truncation and
+// cubes left out of the re-filter become this frame's ALOAM_FLAG_CUBE_OVERFLOW, the frame's word joins the per-call accumulation, and `err` starts
 // the next frame clear (everything of the next frame -- the stack filter forked onto the auxiliary stream included -- is
 // ordered after this kernel)
 __device__ __forceinline__ void mapper_finish_body(MapperState* S) {
@@ -472,7 +492,7 @@ __device__ __forceinline__ void mapper_finish_body(MapperState* S) {
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
   if (threadIdx.x || blockIdx.x) return;
   const int e = S->err;
-  if (e & 14) S->flags |= ALOAM_FLAG_CUBE_OVERFLOW;
+  if (e & 30) S->flags |= ALOAM_FLAG_CUBE_OVERFLOW;
   S->frame_err = e;
   S->err_acc |= e;
   S->err = 0;
@@ -580,44 +600,74 @@ __global__ void __launch_bounds__(256) k_store_copy(const ExportLayout* __restri
 
 // ---- lane snapshots (aloam_lane_restore): the inverse of the ALOAM_EXPORT_MAP export; seeded STARTs (aloam_lane_map_on_prior)
 
-// One CTA of 1024: the store whose cube i holds count(ty, i) points of type ty (-1: no slab).  State of a fresh trajectory first,
-// then the cubes with a count >= 0 take slabs 0, 1, 2, ... of their type in cube order (the rest of the pool stays free,
-// ascending), L = the layout of the ALOAM_EXPORT_MAP export of the new store.  The caller sets the fields that outlive a frame.
+// the order of the run a cube of n points needs at cap points per slab: 0 for n <= cap, else the k with 2^k the next power of two
+// of ceil(n / cap)
+__host__ __device__ inline int run_order(int n, int cap) {
+  int o = 0;
+  while (((long long)cap << o) < n) ++o;
+  return o;
+}
+
+// One CTA of 1024: the store whose cube i holds count(ty, i) points of type ty (-1: no slab), with runs of up to 2^ord0 corner /
+// 2^ord1 surf slabs (every count fits its type's largest run: the caller has checked).  State of a fresh trajectory first, then
+// every cube with a count >= 0 takes the run its count needs (run_order), packed from slab 0 up: the runs by decreasing size,
+// cubes of one size in cube order, so every run is aligned (a size class starts at the sum of the larger ones).  When every run
+// is one slab this is slabs 0, 1, 2, ... in cube order.  The rest of the pool stays free.  L = the layout of the ALOAM_EXPORT_MAP
+// export of the new store.  The caller sets the fields that outlive a frame.
 template <typename Count>
-__device__ __forceinline__ void store_import_body(MapperState* __restrict__ S, Count count, Pt4* p0, Pt4* p1, int cap0, int cap1, ExportLayout* __restrict__ L) {
+__device__ __forceinline__ void store_import_body(MapperState* __restrict__ S, Count count, Pt4* p0, Pt4* p1, int cap0, int cap1, int ord0, int ord1,
+                                                  ExportLayout* __restrict__ L) {
   __shared__ long long s_pts[1024];
-  __shared__ int s_slabs[2][1024];
+  __shared__ int s_scan[1024];
+  __shared__ int s_top[2];
   const int tid = threadIdx.x;
-  mapper_fresh_state(S);
+  const int cap[2] = {cap0, cap1};
+  mapper_fresh_state(S, ord0, ord1);
+  if (tid < 2) s_top[tid] = 0;
   const int per = (NCUBE + 1023) / 1024, b = tid * per, e = min(b + per, NCUBE);
   long long pts = 0;
-  int n0 = 0, n1 = 0;
-  for (int i = b; i < e; ++i) {
-    const int c0 = count(0, i), c1 = count(1, i);
-    pts += max(c0, 0) + max(c1, 0);
-    n0 += c0 >= 0; n1 += c1 >= 0;
-  }
-  // (the first barrier of the scans also orders mapper_fresh_state's writes before the ones below)
-  long long run = block_scan_1024(pts, s_pts);
-  int next[2] = {block_scan_1024(n0, s_slabs[0]), block_scan_1024(n1, s_slabs[1])};
+  int top[2] = {0, 0};
   for (int i = b; i < e; ++i)
     for (int ty = 0; ty < 2; ++ty) {
       const int n = count(ty, i);
-      L->off[2 * i + ty] = run;
-      L->base[2 * i + ty] = nullptr;
-      if (n >= 0) {
-        const int s = next[ty]++;
-        S->slab_of[ty][i] = s; S->cnt[ty][s] = n; run += n;
-        L->base[2 * i + ty] = ty ? p1 + (size_t)s * cap1 : p0 + (size_t)s * cap0;
+      pts += max(n, 0);
+      if (n >= 0) top[ty] = max(top[ty], run_order(n, cap[ty]));
+    }
+  __syncthreads();
+  atomicMax(&s_top[0], top[0]); atomicMax(&s_top[1], top[1]);
+  // (the first barrier of the scan also orders mapper_fresh_state's writes and the atomics before the ones below)
+  long long run = block_scan_1024(pts, s_pts);
+  for (int ty = 0; ty < 2; ++ty) {
+    int base = 0;   // slabs the larger size classes take
+    for (int o = s_top[ty]; o >= 0; --o) {
+      int k = 0;
+      for (int i = b; i < e; ++i) { const int n = count(ty, i); k += n >= 0 && run_order(n, cap[ty]) == o; }
+      int slab = base + (block_scan_1024(k, s_scan) << o);
+      base += s_scan[1023] << o;
+      __syncthreads();   // s_scan is read before the next class overwrites it
+      for (int i = b; i < e; ++i) {
+        const int n = count(ty, i);
+        if (n < 0 || run_order(n, cap[ty]) != o) continue;
+        S->slab_of[ty][i] = slab; S->cnt[ty][slab] = n; S->ord[ty][slab] = (unsigned char)o;
+        slab += 1 << o;
       }
     }
-  if (tid == 1023) { L->off[kExportSegs] = run; L->nseg = kExportSegs; L->total = run; S->free_top = s_slabs[0][1023]; S->free_top2 = s_slabs[1][1023]; }
+    if (tid < kPoolWords) S->used[ty][tid] = base >= 32 * (tid + 1) ? ~0u : base <= 32 * tid ? 0u : (1u << (base - 32 * tid)) - 1u;
+  }
+  for (int i = b; i < e; ++i)
+    for (int ty = 0; ty < 2; ++ty) {
+      const int s = count(ty, i) >= 0 ? S->slab_of[ty][i] : -1;   // (this thread wrote it)
+      L->off[2 * i + ty] = run;
+      L->base[2 * i + ty] = s < 0 ? nullptr : ty ? p1 + (size_t)s * cap1 : p0 + (size_t)s * cap0;
+      if (s >= 0) run += S->cnt[ty][s];
+    }
+  if (tid == 1023) { L->off[kExportSegs] = run; L->nseg = kExportSegs; L->total = run; }
 }
 
 // the store a snapshot's table H describes (the caller has zeroed S), and the fields of H that outlive a frame
 __global__ void __launch_bounds__(1024) k_store_import_tables(MapperState* __restrict__ S, const SnapStore* __restrict__ H, Pt4* p0, Pt4* p1, int cap0, int cap1,
-                                                              ExportLayout* __restrict__ L) {
-  store_import_body(S, [H](int ty, int i) { return H->count[ty][i]; }, p0, p1, cap0, cap1, L);
+                                                              int ord0, int ord1, ExportLayout* __restrict__ L) {
+  store_import_body(S, [H](int ty, int i) { return H->count[ty][i]; }, p0, p1, cap0, cap1, ord0, ord1, L);
   const int tid = threadIdx.x;
   if (tid < kMaxValid) S->valid[tid] = tid < H->n_valid ? H->valid[tid] : 0;
   if (tid == 0) {
@@ -639,13 +689,15 @@ struct SeedLane {
   double init[7];
 };
 // grid (1, 1, records), 1024 threads: record z's store becomes the prior map's (cube table cs [2][NCUBE + 1], centre offsets cen):
-// every cube that holds points gets a slab of its type, in cube order, the others none; frames = 0, an empty valid list and
+// every cube that holds points gets a run of its type as store_import_body packs them (one slab each with growth off: slabs 0,
+// 1, 2, ... in cube order), the others none; runs of up to 2^ord0 / 2^ord1 slabs; frames = 0, an empty valid list and
 // T_wmap_wodom = init.  Fields the stack filter writes (stack_counts, err, in_counts) stay as mapper_fresh_state leaves them.
-__global__ void __launch_bounds__(1024) k_store_seed_tables(const __grid_constant__ Batch<SeedLane> B, const int* __restrict__ cs, int cen0, int cen1, int cen2) {
+__global__ void __launch_bounds__(1024) k_store_seed_tables(const __grid_constant__ Batch<SeedLane> B, const int* __restrict__ cs, int cen0, int cen1, int cen2,
+                                                            int ord0, int ord1) {
   const SeedLane& a = B.a[blockIdx.z];
   MapperState* S = a.S;
   store_import_body(S, [cs](int ty, int i) { const int* t = cs + ty * (NCUBE + 1) + i; const int n = t[1] - t[0]; return n > 0 ? n : -1; },
-                    a.pts[0], a.pts[1], a.cap[0], a.cap[1], a.L);
+                    a.pts[0], a.pts[1], a.cap[0], a.cap[1], ord0, ord1, a.L);
   if (threadIdx.x == 0) {
     S->cen[0] = cen0; S->cen[1] = cen1; S->cen[2] = cen2;
     for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = a.init[k];
@@ -667,10 +719,41 @@ __global__ void __launch_bounds__(256) k_store_seed_copy(const ExportLayout* __r
 }
 
 
+// The run of 2^o slabs at the lowest aligned free position of the occupancy bitmap whose word `lane` this warp lane holds in w
+// (all 32 lanes call it with the same o): its first slab, marked used in w, or -1 when no aligned free run of that size exists.
+__device__ __forceinline__ int take_run(unsigned& w, int o, int lane) {
+  if (o <= 5) {   // the run lies inside one word
+    const int n = 1 << o;
+    unsigned g = ~w;
+    for (int k = 1; k < n; k <<= 1) g &= g >> k;   // bit p: slabs p .. p + n - 1 of the word are free
+    g &= (unsigned)(0xffffffffull / ((1ull << n) - 1ull));   // the aligned positions: every n-th bit from bit 0
+    const unsigned hit = __ballot_sync(0xffffffffu, g != 0u);
+    if (!hit) return -1;
+    const int L = __ffs(hit) - 1, bit = __ffs(__shfl_sync(0xffffffffu, g, L)) - 1;
+    if (lane == L) w |= run_mask(32 * L + bit, o, L);
+    return 32 * L + bit;
+  }
+  const int q = 1 << (o - 5);   // whole words
+  const unsigned m = q == 32 ? 0xffffffffu : (1u << q) - 1u;
+  const unsigned empty = __ballot_sync(0xffffffffu, w == 0u);
+  const unsigned hit = __ballot_sync(0xffffffffu, lane % q == 0 && ((empty >> lane) & m) == m);
+  if (!hit) return -1;
+  const int L = __ffs(hit) - 1;
+  if (lane >= L && lane < L + q) w = 0xffffffffu;
+  return 32 * L;
+}
+
 // stable append of the stack points to their cubes (push_back order = stack order, :759-767).  ONE CTA per cloud (blockIdx.x: the
-// corner and the surf store are independent, the two appends run side by side): the stack is walked in
-// chunks of 1024; inside a chunk the warps take turns, the lanes of one cube form a group (__match_any) whose leader
-// advances the cube's running end in shared memory -- and takes a slab from the free list when the cube had none.
+// corner and the surf store are independent, the two appends run side by side), in four phases:
+//   1. count: the points every cube gets and its first stack point;
+//   2. runs: a cube that gets points and has no run, or whose run cannot hold its new count while a larger one is allowed, needs
+//      the smallest run that holds min(new count, its ceiling) -- served by warp 0 in the order of the cubes' first stack points,
+//      each from the lowest aligned free block of the bitmap; a cube whose run cannot be found keeps what it had (flagged);
+//   3. move: a grown cube's points go to the start of its new run, in order; the old runs are freed once all are served;
+//   4. append: the stack is walked in chunks of 1024; inside a chunk the warps take turns, the lanes of one cube form a group
+//      (__match_any) whose leader advances the cube's running end in shared memory; a point beyond its cube's run is dropped.
+// With growth off (max_ord 0) every run is one slab and no cube ever grows.  Dynamic shared memory: kInsertSmem bytes.
+constexpr int kInsertSmem = 5 * NCUBE * (int)sizeof(int);
 __device__ __forceinline__ void cube_insert_body(const Pt4* __restrict__ world, const int* __restrict__ cube, int scratch_stride, MapperState* S,
                                                       Pt4* __restrict__ pts0, int cap0, Pt4* __restrict__ pts1, int cap1) {
   pdl_launch_dependents();
@@ -679,14 +762,92 @@ __device__ __forceinline__ void cube_insert_body(const Pt4* __restrict__ world, 
   world += (size_t)ty * scratch_stride; cube += (size_t)ty * scratch_stride;
   Pt4* __restrict__ pts = ty ? pts1 : pts0;
   const int cap = ty ? cap1 : cap0;
-  __shared__ int s_end[NCUBE];    // running end of every cube
-  __shared__ int s_slab[NCUBE];   // cube -> slab (the warps' turns must not wait on global memory)
+  extern __shared__ int s_dyn[];
+  int* s_end = s_dyn;               // running end of every cube: its count before the insert, then the append's cursor
+  int* s_slab = s_dyn + NCUBE;      // cube -> first slab of its run (the warps' turns must not wait on global memory)
+  int* s_lim = s_dyn + 2 * NCUBE;   // points the stack brings, then the capacity of the cube's run (INT_MAX: no point comes)
+  int* s_first = s_dyn + 3 * NCUBE; // its first stack point while it needs a run (INT_MAX otherwise), then its old run (-1: none)
+  int* s_list = s_dyn + 4 * NCUBE;  // the cubes that need a run, in the order of their first stack point
+  __shared__ int s_wsum[32], s_nlist;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = S->stack_counts[ty];
+  const int n = S->stack_counts[ty], max_ord = S->max_ord[ty];
+  const int ceiling = cap << max_ord;
   int* slab_of = S->slab_of[ty];
   int* cnt = S->cnt[ty];
-  for (int c = tid; c < NCUBE; c += blockDim.x) { const int s = slab_of[c]; s_slab[c] = s; s_end[c] = s < 0 ? 0 : cnt[s]; }
+  unsigned char* ord = S->ord[ty];
+  for (int c = tid; c < NCUBE; c += blockDim.x) {
+    const int s = slab_of[c];
+    s_slab[c] = s; s_end[c] = s < 0 ? 0 : cnt[s]; s_lim[c] = 0; s_first[c] = INT_MAX;
+  }
   __syncthreads();
+  // ---- 1. count
+  for (int i = tid; i < n; i += blockDim.x) {
+    const int c = cube[i];
+    if (c >= 0) { atomicAdd(&s_lim[c], 1); atomicMin(&s_first[c], i); }
+  }
+  __syncthreads();
+  // ---- 2. runs
+  int need = 0;
+  for (int c = tid; c < NCUBE; c += blockDim.x) {
+    if (s_lim[c] == 0) continue;
+    const int s = s_slab[c], o = run_order(min(s_end[c] + s_lim[c], ceiling), cap);
+    if (s >= 0 && o <= ord[s]) s_first[c] = INT_MAX;
+    else need = 1;
+  }
+  if (__syncthreads_or(need)) {
+    if (tid == 0) s_nlist = 0;
+    __syncthreads();
+    for (int base = 0; base < n; base += blockDim.x) {   // the cubes that need a run, compacted in stack order
+      const int i = base + tid;
+      const int c = i < n ? cube[i] : -1;
+      const bool f = c >= 0 && s_first[c] == i;
+      const unsigned bal = __ballot_sync(0xffffffffu, f);
+      if (lane == 0) s_wsum[warp] = __popc(bal);
+      __syncthreads();
+      int off = s_nlist;
+      for (int v = 0; v < warp; ++v) off += s_wsum[v];
+      if (f) s_list[off + __popc(bal & ((1u << lane) - 1u))] = c;
+      __syncthreads();
+      if (tid == 0) { int t = 0; for (int v = 0; v < 32; ++v) t += s_wsum[v]; s_nlist += t; }
+      __syncthreads();
+    }
+    const int nl = s_nlist;
+    if (warp == 0) {
+      unsigned w = S->used[ty][lane];
+      for (int k = 0; k < nl; ++k) {
+        const int c = s_list[k], old = s_slab[c];
+        const int o = run_order(min(s_end[c] + s_lim[c], ceiling), cap);
+        const int s = take_run(w, o, lane);
+        if (lane == 0) {
+          s_first[c] = -1;
+          if (s < 0) atomicOr(&S->err, 4);   // no free run of that size: the cube keeps what it had
+          else { s_slab[c] = s; ord[s] = (unsigned char)o; s_first[c] = old; }
+        }
+      }
+      __syncwarp();
+      for (int k = 0; k < nl; ++k) {   // the old runs of grown cubes go back to the pool once every run is served
+        const int old = s_first[s_list[k]];
+        if (old >= 0) { const unsigned m = run_mask(old, ord[old], lane); w &= ~m; }
+      }
+      S->used[ty][lane] = w;
+    }
+    __syncthreads();
+    // ---- 3. move
+    for (int k = 0; k < nl; ++k) {
+      const int c = s_list[k], old = s_first[c];
+      if (old < 0) continue;
+      const Pt4* __restrict__ src = pts + (size_t)old * cap;
+      Pt4* __restrict__ dst = pts + (size_t)s_slab[c] * cap;
+      for (int q = tid; q < s_end[c]; q += blockDim.x) dst[q] = src[q];
+      if (tid == 0) cnt[old] = 0;
+    }
+  }
+  for (int c = tid; c < NCUBE; c += blockDim.x) {
+    const int s = s_slab[c];
+    s_lim[c] = s_lim[c] == 0 ? INT_MAX : s < 0 ? 0 : cap << ord[s];
+  }
+  __syncthreads();
+  // ---- 4. append
   for (int base = 0; base < n; base += 1024) {
     const int i = base + tid;
     const int mine = i < n ? cube[i] : -1;
@@ -696,56 +857,74 @@ __device__ __forceinline__ void cube_insert_body(const Pt4* __restrict__ world, 
       if (warp == w) {
         const unsigned grp = __match_any_sync(0xffffffffu, mine);
         const int leader = __ffs(grp) - 1;
-        int start = 0, slab = -1;
+        int start = 0, slab = -1, lim = 0;
         if (mine >= 0 && lane == leader) {
           slab = s_slab[mine];
-          if (slab < 0) {   // first point of an empty cube: take a slab from the pool (several group leaders of one warp may do so at once)
-            int* top = ty == 0 ? &S->free_top : &S->free_top2;
-            const int idx = atomicAdd(top, 1);
-            if (idx < kPool) { slab = S->free_list[ty][idx]; s_slab[mine] = slab; }
-            else { atomicSub(top, 1); atomicOr(&S->err, 4); }
-          }
+          lim = s_lim[mine];
           start = s_end[mine];
           s_end[mine] = start + __popc(grp);
         }
         start = __shfl_sync(0xffffffffu, start, leader);
         slab = __shfl_sync(0xffffffffu, slab, leader);
+        lim = __shfl_sync(0xffffffffu, lim, leader);
         if (mine >= 0 && slab >= 0) {
           const int pos = start + __popc(grp & ((1u << lane) - 1u));
-          if (pos < cap) pts[(size_t)slab * cap + pos] = p;
-          else atomicOr(&S->err, 2);   // slab full: the overflow is dropped (flagged), the frame goes on
+          if (pos < lim) pts[(size_t)slab * cap + pos] = p;
+          else atomicOr(&S->err, 2);   // the cube's run is full: the overflow is dropped (flagged), the frame goes on
         }
       }
       __syncthreads();
     }
   }
-  for (int c = tid; c < NCUBE; c += blockDim.x) { const int s = s_slab[c]; if (s >= 0) { slab_of[c] = s; cnt[s] = min(s_end[c], cap); } }
+  for (int c = tid; c < NCUBE; c += blockDim.x) { const int s = s_slab[c]; if (s >= 0) { slab_of[c] = s; cnt[s] = min(s_end[c], s_lim[c]); } }
 }
-// grid (2 clouds, 1, lanes): every CTA has its own shared cube tables and takes slabs from its lane's free list
+// grid (2 clouds, 1, lanes), kInsertSmem bytes of dynamic shared memory: every CTA has its own shared cube tables and takes runs
+// from its lane's pool
 __global__ void __launch_bounds__(1024) k_cube_insert(const __grid_constant__ Batch<MapperLane> B, int scratch_stride) {
   const MapperLane& a = B.a[blockIdx.z];
   cube_insert_body(a.world, a.cube, scratch_stride, a.S, a.pts[0], a.cap[0], a.pts[1], a.cap[1]);
 }
 
 
-// segment descriptors of the per-cube re-filter (:770-801): every valid cube that has a slab, corner cubes then surf cubes, in place
-__device__ __forceinline__ void seg_cubes_body(MapperState* S, SegDesc* segs, int* n_seg, Pt4* p0, Pt4* p1, int cap0, int cap1, float leaf0, float leaf1) {
+// segment descriptors of the per-cube re-filter (:770-801): the valid cubes, corner cubes then surf cubes, in place -- as long as
+// their running total fits the filter's buffer of `budget` points.  The cubes from the first one that does not fit on are left
+// unfiltered for this frame (flagged: err bit 4).  With growth off a cube holds at most one slab and every valid cube fits.
+__device__ __forceinline__ void seg_cubes_body(MapperState* S, SegDesc* segs, int* n_seg, Pt4* p0, Pt4* p1, int cap0, int cap1, float leaf0, float leaf1,
+                                               int budget) {
   pdl_launch_dependents();
   pdl_wait();   // may have been launched with a programmatic dependency on the previous kernel of the stream
-  const int t = threadIdx.x, nv = S->n_valid;
+  __shared__ int s_w[8];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5, nv = S->n_valid;
+  int s = -1, n = 0;
   if (t < 2 * nv) {
     const int ty = t >= nv, v = ty ? t - nv : t;
-    const int s = S->slab_of[ty][S->valid[v]];
+    s = S->slab_of[ty][S->valid[v]];
+    n = s < 0 ? 0 : S->cnt[ty][s];
+  }
+  // the running total through this cube (block scan; <= 150 x 2^18 points fits int): the counts are >= 0, so the cubes that fit
+  // are a prefix of the list
+  int incl = n;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += u; }
+  if (lane == 31) s_w[w] = incl;
+  __syncthreads();
+  for (int v = 0; v < w; ++v) incl += s_w[v];
+  const int keep = __syncthreads_count(t < 2 * nv && incl <= budget);
+  if (t == 0) {
+    if (keep < 2 * nv) atomicOr(&S->err, 16);
+    *n_seg = keep; S->zero = 0;
+  }
+  if (t < keep) {
+    const int ty = t >= nv;
     Pt4* base = s < 0 ? (ty ? p1 : p0) : (ty ? p1 : p0) + (size_t)s * (ty ? cap1 : cap0);
     int* np = s < 0 ? &S->zero : &S->cnt[ty][s];
     segs[t] = SegDesc{base, np, ty ? leaf1 : leaf0, base, s < 0 ? &S->sink : np};
   }
-  if (t == 0) { *n_seg = 2 * nv; S->zero = 0; }
 }
 // grid (1, 1, lanes)
-__global__ void __launch_bounds__(256) k_seg_cubes(const __grid_constant__ Batch<MapperLane> B, float leaf0, float leaf1) {
+__global__ void __launch_bounds__(256) k_seg_cubes(const __grid_constant__ Batch<MapperLane> B, float leaf0, float leaf1, int budget) {
   const MapperLane& a = B.a[blockIdx.z];
-  seg_cubes_body(a.S, a.segs, a.n_seg, a.pts[0], a.pts[1], a.cap[0], a.cap[1], leaf0, leaf1);
+  seg_cubes_body(a.S, a.segs, a.n_seg, a.pts[0], a.pts[1], a.cap[0], a.cap[1], leaf0, leaf1, budget);
 }
 
 
@@ -756,10 +935,12 @@ size_t refilter_bound(const Mapper* m, const aloam_ctx* c) {
 }
 
 // the state of a fresh trajectory (mapper_fresh_state, the routine k_mapper_begin runs for a lane that starts one), with the
-// fields that routine leaves alone zeroed first
+// fields that routine leaves alone zeroed first, under the context's cube growth
 int reset_lane(aloam_ctx* c, Mapper* m) {
+  int ord[2];
+  mapper_run_orders(c, c->cube_growth, ord);
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
-  LAUNCH(c, KID_CUBES, k_mapper_reset, 1, 1024, 0, m->d_state);
+  LAUNCH(c, KID_CUBES, k_mapper_reset, 1, 1024, 0, m->d_state, ord[0], ord[1]);
   CUDA_CHECK_RET(cudaGetLastError());
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   return ALOAM_OK;
@@ -869,12 +1050,15 @@ void prior_index(aloam_ctx* c, PriorMap* p) {
 template <typename Fill> int prior_install(aloam_ctx* c, const int cen[3], const std::vector<int>& cs, Fill fill) {
   PriorMap* p = new (std::nothrow) PriorMap();
   if (!p) return ALOAM_ERR_CUDA;
+  int cap[2];
+  mapper_slab_caps(c, cap);
   for (int t = 0; t < 2; ++t) {
     p->n[t] = cs[(size_t)t * (NCUBE + 1) + NCUBE];
     for (int i = 0; i < NCUBE; ++i) {
       const int n = cs[(size_t)t * (NCUBE + 1) + i + 1] - cs[(size_t)t * (NCUBE + 1) + i];
       p->max_cube[t] = std::max(p->max_cube[t], n);
       p->n_cubes[t] += n > 0;
+      if (n > 0) p->run_slabs[t] = (int)std::min<long long>((long long)p->run_slabs[t] + (1ll << std::min(run_order(n, cap[t]), 30)), INT_MAX);
     }
   }
   for (int a = 0; a < 3; ++a) p->cen[a] = cen[a];
@@ -1149,11 +1333,23 @@ void mapper_slab_caps(const aloam_ctx* c, int cap[2]) {
   cap[1] = std::min(65536, c->max_points);
 }
 
+// the largest run of a lane store per type, 2^ord[t] slabs: with growth on the largest power of two r with r x cap <=
+// ALOAM_MAX_CUBE_POINTS (and r <= the pool), else one slab
+void mapper_run_orders(const aloam_ctx* c, bool growth, int ord[2]) {
+  int cap[2];
+  mapper_slab_caps(c, cap);
+  for (int t = 0; t < 2; ++t) {
+    ord[t] = 0;
+    while (growth && ord[t] < kMaxOrder && ((long long)cap[t] << (ord[t] + 1)) <= ALOAM_MAX_CUBE_POINTS) ++ord[t];
+  }
+}
+
 // ---- lane snapshots (snapshot.cu): the cube store of a lane in the slab-free form of SnapStore
 
 // the table of lane `lane`'s store into *head (host memory): the fields that outlive a frame and every cube's point count, -1 for a
-// cube without a slab; head->n_points = the size of the ALOAM_EXPORT_MAP export.  The store exists.  Synchronises.
-int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head) {
+// cube without a run; head->n_points = the size of the ALOAM_EXPORT_MAP export; *growth = the store's cube growth.  The store
+// exists.  Synchronises.
+int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head, int* growth) {
   Mapper* m = c->lanes[lane].mapper;
   CUDA_CHECK_RET(cudaMemcpyAsync(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
@@ -1173,6 +1369,7 @@ int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head) {
       n += s < 0 ? 0 : S->cnt[ty][s];
     }
   head->n_points = n;
+  *growth = S->max_ord[0] > 0;
   return ALOAM_OK;
 }
 
@@ -1186,16 +1383,19 @@ int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool dev
   return n > 0 ? store_copy(c, c->d_export_layout, n, dst, device, false) : ALOAM_OK;
 }
 
-// Makes lane `lane`'s store (it exists) the one a validated snapshot table describes: *head (pinned host memory) goes to the
-// device, k_store_import_tables rebuilds the tables and lays the store out, store_copy moves the head->n_points points of pts into
-// the slabs.  Synchronises.
-int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device) {
+// Makes lane `lane`'s store (it exists) the one a validated snapshot table describes, with the snapshot's cube growth: *head
+// (pinned host memory) goes to the device, k_store_import_tables rebuilds the tables and lays the store out, store_copy moves the
+// head->n_points points of pts into the runs.  Synchronises.
+int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device, bool growth) {
   Mapper* m = c->lanes[lane].mapper;
+  int ord[2];
+  mapper_run_orders(c, growth, ord);
   if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
   if (!c->d_snap_store) CUDA_CHECK_RET(dalloc(c, &c->d_snap_store, 1));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_snap_store, head, sizeof(SnapStore), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
-  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->d_export_layout);
+  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], ord[0], ord[1],
+         c->d_export_layout);
   if (head->n_points > 0) { const int rc = store_copy(c, c->d_export_layout, head->n_points, const_cast<char*>(pts), device, true); if (rc) return rc; }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1219,7 +1419,9 @@ static int seed_stores(aloam_ctx* c, int nb, const MapperIn* in) {
   if (n == 0) return ALOAM_OK;
   const PriorMap* P = c->prior;
   if (!P || !c->d_seed_layout) return ALOAM_ERR_STATE;   // an arming is dropped with the map it was checked against
-  LAUNCH(c, KID_CUBES, k_store_seed_tables, dim3(1, 1, n), 1024, 0, B, (const int*)P->d_cube_start, P->cen[0], P->cen[1], P->cen[2]);
+  int ord[2];
+  mapper_run_orders(c, c->cube_growth, ord);   // a seeded START is a mapped START: the context's cube growth
+  LAUNCH(c, KID_CUBES, k_store_seed_tables, dim3(1, 1, n), 1024, 0, B, (const int*)P->d_cube_start, P->cen[0], P->cen[1], P->cen[2], ord[0], ord[1]);
   LAUNCH(c, KID_CUBES, k_store_seed_copy, dim3(std::min(kExportSegs, c->sms * 8), 1, n), 256, 0, (const ExportLayout*)P->d_layout, (const ExportLayout*)c->d_seed_layout);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
@@ -1262,12 +1464,14 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   }
   const int max_sub = m0->max_sub, cap1 = m0->cap[1];
   const int refilter_cap = (int)m0->buf.cap;   // refilter_bound: the same for every lane
+  int ord[2];                                  // the runs of the lanes that start a trajectory with this frame
+  mapper_run_orders(c, c->cube_growth, ord);
   // ---- seeded STARTs: their stores become copies of the prior map, in order on this stream after the lanes' previous frames and
   //      before this frame's stack filters are forked, so nothing of the frame runs beside the seed
   rc = seed_stores(c, nb, in); if (rc) return rc;
   // ---- stack filters (:541-550), beside the gather + index build below, which read only the cube stores
   rc = stack_filters_fork(c, nb, B, stack_f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
-  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub, fresh);
+  launch_ex(c, KID_CUBES, k_mapper_begin, dim3(1, 1, nb), dim3(1024), 0, 1, true, B, max_sub, fresh, ord[0], ord[1]);
   launch_ex(c, KID_CUBES, k_mapper_gather, dim3(kMaxValid, 2, nb), dim3(256), 0, 1, true, B);
   if (c->shard_count > 1) {
     // A rank of a sharded job keeps the WHOLE cube store (the insertions below are replicated: the refined pose is bit-identical
@@ -1289,9 +1493,9 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   // ---- insertion (:736-767)
   const int up = std::max(n_upper_c, n_upper_s);
   launch_ex(c, KID_CUBES, k_cube_ids, dim3(std::max(1, std::min((up + 255) / 256, std::max(1, c->sms * 2 / nb))), 2, nb), dim3(256), 0, 1, true, B, c->max_points);
-  launch_ex(c, KID_CUBES, k_cube_insert, dim3(2, 1, nb), dim3(1024), 0, 1, true, B, c->max_points);
+  launch_ex(c, KID_CUBES, k_cube_insert, dim3(2, 1, nb), dim3(1024), (size_t)kInsertSmem, 1, true, B, c->max_points);
   // ---- per-cube re-filter of the valid cubes (:770-801): one segmented pass over <= 150 cubes of every lane, in place
-  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1, 1, nb), dim3(256), 0, 1, true, B, c->cfg.line_res, c->cfg.plane_res);
+  launch_ex(c, KID_CUBES, k_seg_cubes, dim3(1, 1, nb), dim3(256), 0, 1, true, B, c->cfg.line_res, c->cfg.plane_res, refilter_cap);
   vox_seg_filter(c, nb, cube_f, bufs, 2 * 75, refilter_cap, cap1);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1445,6 +1649,7 @@ int mapper_ensure(aloam_ctx* c, int lane) {
   ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
   ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
   ok = ok && stack_stream_ensure(c) == cudaSuccess;
+  ok = ok && cudaFuncSetAttribute(k_cube_insert, cudaFuncAttributeMaxDynamicSharedMemorySize, kInsertSmem) == cudaSuccess;
   ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
   // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
   // created here, after the context's (which fixes the table size)
@@ -1620,12 +1825,14 @@ int aloam_prior_map_build(aloam_ctx* c, aloam_cloud_view corner, aloam_cloud_vie
     CUDA_CHECK_RET(cudaGetLastError());
   }
   const int n0 = rank[NCUBE];
+  // a filtered cube: at most 65536 points while cube growth is off, ALOAM_MAX_CUBE_POINTS (the 18-bit rank of prior_tag) while on
+  const int limit = c->cube_growth ? ALOAM_MAX_CUBE_POINTS : 65536;
   std::vector<int> cs((size_t)2 * (NCUBE + 1));
   for (int t = 0; t < 2; ++t)
     for (int i = 0; i <= NCUBE; ++i) {
       const int r = rank[(size_t)t * NCUBE + i] - (t ? n0 : 0);
       cs[(size_t)t * (NCUBE + 1) + i] = r;
-      if (i > 0 && r - cs[(size_t)t * (NCUBE + 1) + i - 1] > 65536) return ALOAM_ERR_CAPACITY;   // the 16-bit rank of prior_tag
+      if (i > 0 && r - cs[(size_t)t * (NCUBE + 1) + i - 1] > limit) return ALOAM_ERR_CAPACITY;
     }
   rc = prior_install(c, cen, cs, [&](PriorMap* p) {
     if (n > 0) LAUNCH(c, KID_PRIOR_BUILD, k_build_emit, tiles, kBuildTile, 0, B.pts, B.keys[0], B.vals[0], n, B.par, B.head, B.tile_heads, n0, p->pts[0], p->pts[1]);
@@ -1665,12 +1872,23 @@ int aloam_lane_map_on_prior(aloam_ctx* c, int lane, const double q_init[4], cons
   if (!P || sharded_job(c)) return ALOAM_ERR_STATE;
   // the START's map position is init's translation (identity odometry pose): its first frame's shift loop must end
   if (!map_position_fits(init + 4, P->cen)) return ALOAM_ERR_INVALID_ARG;
-  int cap[2];
+  // every cube within its ceiling and every run in the pool, under the context's cube growth now: one slab per cube while it is
+  // off, the runs store_import_body packs while it is on
+  int cap[2], ord[2];
   mapper_slab_caps(c, cap);
-  for (int t = 0; t < 2; ++t) if (P->max_cube[t] > cap[t] || P->n_cubes[t] > kPool) return ALOAM_ERR_CAPACITY;
+  mapper_run_orders(c, c->cube_growth, ord);
+  for (int t = 0; t < 2; ++t)
+    if (P->max_cube[t] > (cap[t] << ord[t]) || (c->cube_growth ? P->run_slabs[t] : P->n_cubes[t]) > kPool) return ALOAM_ERR_CAPACITY;
   Lane& L = c->lanes[lane];
   for (int k = 0; k < 7; ++k) L.init[k] = init[k];
   L.sched.arm = ARM_MAP_ON_PRIOR;
+  return ALOAM_OK;
+}
+
+int aloam_set_cube_growth(aloam_ctx* c, int on) {
+  if (!c || (on != 0 && on != 1)) return ALOAM_ERR_INVALID_ARG;
+  c->cube_growth = on != 0;
+  for (Lane& L : c->lanes) if (L.sched.arm == ARM_MAP_ON_PRIOR) L.sched.arm = ARM_NONE;   // its fit was checked under the old setting
   return ALOAM_OK;
 }
 
@@ -1768,8 +1986,11 @@ int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, al
   CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
   const int s = m->h_state->slab_of[which][cube];
   const int n = s < 0 ? 0 : m->h_state->cnt[which][s];
-  out->data = reinterpret_cast<const float*>(c->h_out[4]); out->n = n; out->stride_floats = 4;
-  if (n > 0) CUDA_CHECK_RET(cudaMemcpy(c->h_out[4], m->d_pts[which] + (size_t)s * m->cap[which], (size_t)n * sizeof(Pt4), cudaMemcpyDeviceToHost));
+  // a cube beyond max_points (cube growth) is read into a pinned buffer of ALOAM_MAX_CUBE_POINTS points, created on first use
+  if (n > c->max_points && !c->h_cube) CUDA_CHECK_RET(halloc(c, &c->h_cube, (size_t)ALOAM_MAX_CUBE_POINTS));
+  Pt4* h = n > c->max_points ? c->h_cube : c->h_out[4];
+  out->data = reinterpret_cast<const float*>(h); out->n = n; out->stride_floats = 4;
+  if (n > 0) CUDA_CHECK_RET(cudaMemcpy(h, m->d_pts[which] + (size_t)s * m->cap[which], (size_t)n * sizeof(Pt4), cudaMemcpyDeviceToHost));
   return ALOAM_OK;
 }
 

@@ -127,9 +127,13 @@ __global__ void k_map_knn(MapCloud map, const Pt4* queries, int nq, int k, int* 
 // rank inside that cube, so a search can tell without another load whether the point lies in a lane's 5 x 5 x 3 cube window and
 // which index it would have had in the submap the mapping frame gathers (window offset of the cube + rank).  (The alternatives
 // were a uint16 cube id beside gpts, one more 2-byte load per candidate, or a 13-step binary search of the cube prefix table per
-// candidate; the tag costs three shifts and no load.  Ranks fit 16 bits: a cube holds at most 65536 points.)
+// candidate; the tag costs three shifts and no load.  i, j, k take 5 + 5 + 4 bits and the rank 18: a cube of the prior map
+// holds at most ALOAM_MAX_CUBE_POINTS = 2^18 points.  The tag is unsigned: i >= 16 sets bit 31.  It is only moved and
+// reinterpreted, never used in float arithmetic.)
 #define ALOAM_WINDOW_CUBES 75   // 5 x 5 x 3, entry (di + 2) * 15 + (dj + 2) * 3 + (dk + 1): the loop order of laserMapping.cpp:512-531
-__host__ __device__ inline int prior_tag(int i, int j, int k, int rank) { return (i << 25) | (j << 20) | (k << 16) | rank; }
+__host__ __device__ inline unsigned prior_tag(int i, int j, int k, int rank) {
+  return ((unsigned)i << 27) | ((unsigned)j << 22) | ((unsigned)k << 18) | (unsigned)rank;
+}
 struct PriorGrid { GridTable corner, surf; };
 // one lane of the search: its filtered stacks and pose as MapAssocArgs, its window tables (per type ALOAM_WINDOW_CUBES offsets
 // into the submap the window's cubes would gather to) and its centre cube (3 ints)

@@ -553,9 +553,10 @@ __global__ void __launch_bounds__(256) k_map_knn5_prior(const __grid_constant__ 
     float nd[5]; int ni[5], np[5];
     TopK<5> t; t.init();
     visit_block27(G, is_corner ? mask_c : mask_s, qx, qy, qz, [&](float x, float y, float z, int tag, int slot) {
-      const int di = (tag >> 25) - c0, dj = ((tag >> 20) & 31) - c1, dk = ((tag >> 16) & 15) - c2;
+      const unsigned u = (unsigned)tag;   // i sets bit 31 from i = 16 on: decoded unsigned
+      const int di = (int)(u >> 27) - c0, dj = (int)((u >> 22) & 31u) - c1, dk = (int)((u >> 18) & 15u) - c2;
       if ((unsigned)di < 5u && (unsigned)dj < 5u && (unsigned)dk < 3u)   // a cube of the window (one that holds points is inside the buffer)
-        t.push(sqdist3(x, y, z, qx, qy, qz), win[(di * 5 + dj) * 3 + dk] + (tag & 0xffff), slot);
+        t.push(sqdist3(x, y, z, qx, qy, qz), win[(di * 5 + dj) * 3 + dk] + (int)(u & 0x3ffffu), slot);
     });
     const int found = warp_merge_topk<5>(t, nd, ni, np);
     if (!(found == 5 && (double)nd[4] < 1.0)) {   // pointSearchSqDis[4] < 1.0 (:584,652)

@@ -43,6 +43,7 @@ int check_header(const SnapHeader& h, long long n_bytes) {
   if (std::memcmp(h.magic, kMagic, 8) != 0 || h.version != kSnapVersion) return ALOAM_ERR_SNAPSHOT;
   if ((h.mapped != 0 && h.mapped != 1) || h.scan_index < 1 || h.n_less_sharp < 0 || h.n_less_flat < 0) return ALOAM_ERR_SNAPSHOT;
   if (h.ring_source != ALOAM_RING_ELEVATION && h.ring_source != ALOAM_RING_FIELD) return ALOAM_ERR_SNAPSHOT;
+  if (h.cube_growth != 0 && h.cube_growth != 1) return ALOAM_ERR_SNAPSHOT;
   if (h.total_bytes != n_bytes) return ALOAM_ERR_SNAPSHOT;
   if (!all_finite(h.warm, 7) || !all_finite(h.world, 7)) return ALOAM_ERR_SNAPSHOT;
   if (!h.mapped) return n_bytes == store_offset(h) ? ALOAM_OK : ALOAM_ERR_SNAPSHOT;
@@ -53,8 +54,10 @@ int check_header(const SnapHeader& h, long long n_bytes) {
 // the store table of a mapped snapshot whose header passed check_header: centre offsets within +-2^20, a finite T_wmap_wodom, a
 // map position T_wmap_wodom * world whose centre cube lies at most kCubeSlack cubes outside the buffer on every axis (the next
 // frame's shift loop runs one pass per cube beyond the edge: an unbounded position would never end it), the valid list, every
-// count within its slab capacity, at most kSnapPool cubes of a type holding a slab, and a payload of exactly the counted points
-// that ends the snapshot
+// count within its ceiling under the snapshot's cube growth (the slab capacity while off, the largest run's while on), the runs
+// the counts need (store_import_body: one slab up to the slab capacity, else the next power of two of ceil(n / cap)) at most
+// kSnapPool slabs per type -- with every run one slab: at most kSnapPool cubes of a type hold a slab --, and a payload of exactly
+// the counted points that ends the snapshot
 int check_store(const SnapHeader& h, const SnapStore& s) {
   for (int a = 0; a < 3; ++a) if (s.cen[a] < -kMaxCentre || s.cen[a] > kMaxCentre) return ALOAM_ERR_SNAPSHOT;
   if (!all_finite(s.q_wmap_wodom, 4) || !all_finite(s.t_wmap_wodom, 3)) return ALOAM_ERR_SNAPSHOT;
@@ -70,11 +73,17 @@ int check_store(const SnapHeader& h, const SnapStore& s) {
     if (s.valid[v] < 0 || s.valid[v] >= kSnapCubes) return ALOAM_ERR_SNAPSHOT;
   long long points = 0;
   for (int ty = 0; ty < 2; ++ty) {
-    int slabs = 0;
+    const long long cap = h.slab_cap[ty];
+    long long top = cap;   // the largest run's capacity: the largest power of two r <= kSnapPool with r cap <= ALOAM_MAX_CUBE_POINTS
+    for (int r = 2; h.cube_growth && r <= kSnapPool && r * cap <= ALOAM_MAX_CUBE_POINTS; r *= 2) top = r * cap;
+    long long slabs = 0;
     for (int i = 0; i < kSnapCubes; ++i) {
       const int n = s.count[ty][i];
-      if (n < -1 || n > h.slab_cap[ty]) return ALOAM_ERR_SNAPSHOT;
-      if (n >= 0) { ++slabs; points += n; }
+      if (n < -1 || n > top) return ALOAM_ERR_SNAPSHOT;
+      if (n < 0) continue;
+      long long run = 1;
+      while (run * cap < n) run *= 2;
+      slabs += run; points += n;
     }
     if (slabs > kSnapPool) return ALOAM_ERR_SNAPSHOT;
   }
@@ -221,7 +230,7 @@ int aloam_lane_save(aloam_ctx* c, int lane, void* out, long long capacity, long 
   int rc = ALOAM_OK;
   if (h.mapped) {
     rc = ensure_snap_store(c); if (rc) return rc;
-    rc = mapper_store_tables(c, lane, c->h_snap_store); if (rc) return rc;
+    rc = mapper_store_tables(c, lane, c->h_snap_store, &h.cube_growth); if (rc) return rc;   // the lane's own, not the context's
     h.total_bytes += (long long)sizeof(SnapStore) + 16 * c->h_snap_store->n_points;
   }
   *n_bytes = h.total_bytes;
@@ -274,7 +283,7 @@ int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_byt
   // k_ring_scan arms a lane's next ScanScalars slot only when the lane ran the step before
   CUDA_CHECK_RET(cudaMemcpyAsync(L.d_sc + c->parity, c->d_sc_init, sizeof(ScanScalars), cudaMemcpyDeviceToDevice, c->stream));
   // ---- the cube store
-  if (h.mapped) { rc = mapper_store_restore(c, lane, c->h_snap_store, b + store + sizeof(SnapStore), kind); if (rc) return rc; }
+  if (h.mapped) { rc = mapper_store_restore(c, lane, c->h_snap_store, b + store + sizeof(SnapStore), kind, h.cube_growth != 0); if (rc) return rc; }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   L.sched.running = true;

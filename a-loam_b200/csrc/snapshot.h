@@ -9,7 +9,7 @@ namespace aloam {
 constexpr int kSnapVersion = 1;
 constexpr int kSnapCubes = 4851;   // 21 x 21 x 11 cubes of the mapper's ring buffer
 constexpr int kSnapValid = 128;
-constexpr int kSnapPool = 1024;    // slabs per cloud type: at most this many cubes of a type hold points
+constexpr int kSnapPool = 1024;    // slabs per cloud type: the runs of a type's cubes take at most this many
 
 // section 1, at offset 0
 struct SnapHeader {
@@ -27,12 +27,14 @@ struct SnapHeader {
   double warm[7];                      // para_q / para_t of the next scan's solve
   double world[7];                     // world pose of the lane's last scan
   int32_t ring_source;                 // 0 elevation (what a snapshot written before the field held), 1 driver ring
-  char zero[36];
+  int32_t cube_growth;                 // the store's cube growth: 0 off (what a snapshot written before the field held), 1 on
+  char zero[32];
 };
 static_assert(sizeof(SnapHeader) == 256, "snapshot header");
 static_assert(offsetof(SnapHeader, scan_index) == 24 && offsetof(SnapHeader, n_scans) == 36 && offsetof(SnapHeader, minimum_range) == 56 &&
               offsetof(SnapHeader, slab_cap) == 68 && offsetof(SnapHeader, huber) == 80 && offsetof(SnapHeader, warm) == 104 &&
-              offsetof(SnapHeader, world) == 160 && offsetof(SnapHeader, ring_source) == 216, "snapshot header layout");
+              offsetof(SnapHeader, world) == 160 && offsetof(SnapHeader, ring_source) == 216 &&
+              offsetof(SnapHeader, cube_growth) == 220, "snapshot header layout");
 
 // section 2 at offset 256: n_less_sharp, then n_less_flat points of 4 floats.  Section 3 (mapped snapshots only) follows: this
 // table, then n_points points of 4 floats in ALOAM_EXPORT_MAP order
@@ -41,7 +43,7 @@ struct SnapStore {
   int32_t valid[kSnapValid];          // entries n_valid .. 127 are 0
   int32_t frames, zero0;
   double q_wmap_wodom[4], t_wmap_wodom[3];
-  int32_t count[2][kSnapCubes];       // points of cube i of type t (0 corner, 1 surf); -1: the cube holds no slab
+  int32_t count[2][kSnapCubes];       // points of cube i of type t (0 corner, 1 surf); -1: the cube holds no run
   int32_t zero1[2];
   int64_t n_points;
   int64_t zero2;

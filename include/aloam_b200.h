@@ -47,11 +47,14 @@ extern "C" {
 
 #define ALOAM_MAX_RING_POINTS 4096
 #define ALOAM_MAX_BATCH 16
+#define ALOAM_MAX_CUBE_POINTS 262144   /* 2^18: the most points one map cube holds with cube growth on (aloam_set_cube_growth) */
 
 #define ALOAM_FLAG_FEW_CORRESPONDENCES 1
 #define ALOAM_FLAG_MAP_TOO_THIN 2
 #define ALOAM_FLAG_INITIALISED_ONLY 4 /* first frame: laserOdometry.cpp:267-271 */
-#define ALOAM_FLAG_CUBE_OVERFLOW 8    /* map cube store: a cube slab (16 k corner / 64 k surf points) or the slab pool was full; the overflow was dropped */
+#define ALOAM_FLAG_CUBE_OVERFLOW 8    /* map cube store: a cube was at its capacity (one slab of 16 k corner / 64 k surf points with
+                                         cube growth off, its ceiling with growth on), no free run of slabs was left, the submap was
+                                         truncated, or cubes were left out of the re-filter; see aloam_set_cube_growth */
 
 typedef struct aloam_ctx aloam_ctx;
 
@@ -285,7 +288,10 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  * an emulating context (nothing changes).  Otherwise the call first ends whatever the lane ran and puts the context in lanes
  * mode, as a START does (the lockstep calls are refused until aloam_reset_odometry); then it checks the whole snapshot on the
  * host before it writes anything to the device -- ALOAM_ERR_SNAPSHOT for a bad magic or version, a size that does not match the
- * sections, a count above the slab capacity, more than 1024 cubes of a type holding a slab, a payload that is not the sum of
+ * sections, a cube_growth other than 0 or 1, a count above the cube's ceiling (the slab capacity when the snapshot's cube_growth
+ * is 0, the largest run's capacity when it is 1), runs that need more than 1024 slabs of a type (one slab for a count up to the
+ * slab capacity, else the next power of two of ceil(count / capacity); with growth off: more than 1024 cubes of a type holding a
+ * slab), a payload that is not the sum of
  * the counts, a valid list of more than 125 entries or with an index outside 0 .. 4850, a non-finite warm start or world pose,
  * and for a mapped snapshot a non-finite T_wmap_wodom, a centre offset cen[a] outside -2^20 .. 2^20 (the range of
  * aloam_prior_map_build) or a map position T_wmap_wodom * world (translation) whose centre cube -- int((x + 25.0) / 50.0) + cen[a],
@@ -296,7 +302,10 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  * 950 m), or a configuration that differs --
  * ALOAM_ERR_CAPACITY when a "last" cloud exceeds cfg.max_points, ALOAM_ERR_NOT_RING_MAJOR when it is not ring-major (the check
  * of aloam_odometry_set_last).  It creates the lane's cube store if needed.  After any failure the lane is not running; no other
- * lane changes.
+ * lane changes.  The restored lane takes the cube growth the snapshot records, not the context's (it is not a configuration field
+ * that is compared).  Its runs are packed afresh (decreasing size, cube order within a size), so they can be smaller than those
+ * of the uninterrupted lane, whose runs never shrink: the restored lane is bit-identical to the uninterrupted run while no run
+ * allocation fails on either side.
  * aloam_snapshot_check runs the host checks of aloam_lane_restore on a snapshot in host memory without a context or a GPU (no
  * configuration is compared) and, when info is not NULL, describes it: format version, mode, n_scans, the index of its next scan,
  * its size, its map points and the world pose of its last scan.
@@ -309,16 +318,17 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  *       52 int32 inner_iters   56 float minimum_range   60 float line_res   64 float plane_res   68 int32 slab_cap[2]
  *       76 int32 max_map_points   80 double huber   88 double dist_sq_thresh   96 double nearby_scan
  *      104 double warm[7] (q_last_curr xyzw, t_last_curr: the next scan's warm start)   160 double world[7]
- *      216 int32 ring_source (0 or 1; snapshots written before the field existed hold 0 there, the elevation source)   220 zero to 256
+ *      216 int32 ring_source (0 or 1; snapshots written before the field existed hold 0 there, the elevation source)
+ *      220 int32 cube_growth (0 or 1: the store's aloam_set_cube_growth setting; snapshots written before the field hold 0)   224 zero to 256
  *   2. at 256: n_less_sharp, then n_less_flat points of 4 floats (x, y, z, intensity) -- the lane's "last" clouds
  *   3. mapped snapshots only, at S = 256 + 16 (n_less_sharp + n_less_flat): the cube store
  *      S+0 int32 cen[3]   S+12 int32 n_valid (<= 125)   S+16 int32 valid[128] (unused entries 0)   S+528 int32 frames
  *      S+532 zero   S+536 double q_wmap_wodom[4]   S+568 double t_wmap_wodom[3]
- *      S+592 int32 count[2][4851]: points of corner (0) / surf (1) cube i; -1 = the cube holds no slab (0 = a slab, no points)
+ *      S+592 int32 count[2][4851]: points of corner (0) / surf (1) cube i; -1 = the cube holds no run (0 = a run, no points)
  *      S+39400 zero   S+39408 int64 n_points (the sum of the counts >= 0)   S+39416 zero
  *      S+39424 n_points points of 4 floats in ALOAM_EXPORT_MAP order: corner cube i, then surf cube i, for i = 0 .. 4850
- *   total_bytes = S, or S + 39424 + 16 n_points for a mapped snapshot.  Which slab a cube held is not saved: only which cubes hold
- *   one, and the points, change results. */
+ *   total_bytes = S, or S + 39424 + 16 n_points for a mapped snapshot.  Which slabs a cube held is not saved: only which cubes hold
+ *   a run, and the points, change results. */
 typedef struct aloam_snapshot_info {
   int version, mapped, n_scans, scan_index;
   long long bytes, map_points;
@@ -335,7 +345,8 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  * aloam_lane_restore runs for a mapped snapshot, with its error codes (ALOAM_ERR_SNAPSHOT also for an unmapped snapshot), and nothing
  * on the device changes on failure.
  * The map is packed per cloud type and indexed once, with one hash grid over the WHOLE map (1.00001 m cells): it is not bounded by
- * cfg.max_map_points (no submap is gathered) but by the snapshot format (1024 cubes of a type x the slab capacity) and by memory
+ * cfg.max_map_points (no submap is gathered) but by the snapshot format (1024 slabs of a type, cubes up to the snapshot's ceiling:
+ * a growth-on snapshot's cube may hold up to ALOAM_MAX_CUBE_POINTS) and by memory
  * (ALOAM_ERR_CUDA before any state changes): 32 B per point plus a table of 16 B x the power of two above 1.25 x the points of the
  * type.  Loading replaces an earlier prior map.  ALOAM_ERR_STATE while any lane is localising, on a rank of a sharded job and on an
  * emulating context.  aloam_prior_map_clear releases it (ALOAM_ERR_STATE while any lane is localising) and drops every arming;
@@ -384,7 +395,8 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  *     input order (PCL).  There is no key-width limit: every other cube is filtered.
  *   - the result is what aloam_prior_map_load makes of a store: per type the filtered cubes packed in cube order, points in voxel
  *     order, the same index, cube tags and ALOAM_EXPORT_MAP export, centre offsets = centre.  Nothing downstream tells the two apart.
- *   - limits: ALOAM_ERR_CAPACITY when a filtered cube holds more than 65536 points, or a cloud more than 2^30 points (or the two
+ *   - limits: ALOAM_ERR_CAPACITY when a filtered cube holds more than 65536 points while the context's cube growth is off, more than
+ *     ALOAM_MAX_CUBE_POINTS while it is on, or a cloud more than 2^30 points (or the two
  *     together more than 2^31 - 4097); nothing changes.  No bound on cubes per type or points per cube otherwise.  Memory: the map as
  *     for a load, plus about 42 B per input point of scratch that is freed before the call returns; ALOAM_ERR_CUDA when it fails.
  *   - state rules are aloam_prior_map_load's: ALOAM_ERR_STATE while any lane is localising, on a rank of a sharded job and on an
@@ -403,9 +415,10 @@ int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const 
  * then on the lane is an ordinary mapping lane: it shifts the ring buffer, inserts and re-filters; aloam_lane_save,
  * aloam_mapper_export, the registered sink, aloam_map_rows and cfg.mapping_skip_frame work as for any mapping lane.  The prior map is
  * never written: to publish the extended map, save the lane and aloam_prior_map_load the snapshot, or export it and build from it.
- *   - the seeded store: the centre offsets are the prior map's; every cube the prior map holds points in gets a slab of its type,
- *     slabs 0, 1, 2, ... in cube order (the layout aloam_lane_restore gives a snapshot's store), the points in the prior map's
- *     per-cube order; cubes without points get no slab; frames = 0 and the valid list is empty (the START frame computes it).
+ *   - the seeded store: the centre offsets are the prior map's; every cube the prior map holds points in gets a run of its type,
+ *     packed as aloam_lane_restore packs a snapshot's store (with cube growth off one slab each: slabs 0, 1, 2, ... in cube order),
+ *     the points in the prior map's per-cube order; cubes without points get no run; frames = 0 and the valid list is empty (the
+ *     START frame computes it).  The lane takes the context's cube growth at that START.
  *   - equivalence: every row of the trajectory -- map pose, stats and flags -- and the final store are bit for bit those of
  *     aloam_mapper_step on a lane 0 restored (aloam_lane_restore) from a mapped snapshot that holds the prior map's store with
  *     T_wmap_wodom = the normalised init and frames = 0, driven with the same clouds and odometry poses (the START's odometry pose is
@@ -419,12 +432,15 @@ int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const 
  *     ALOAM_ERR_INVALID_ARG for a bad lane, a NULL or non-finite pose, a zero quaternion, or an init position t_init whose centre
  *     cube (int((t + 25.0) / 50.0) + the prior map's centre offset, minus 1 below -25) lies more than 16 cubes outside the
  *     21 x 21 x 11 buffer on an axis -- the rule aloam_lane_restore applies to a snapshot's map position (the first frame's shift
- *     loop must end); ALOAM_ERR_CAPACITY when the prior map does not fit a lane's store: a cube with more points than the slab
- *     capacity of its type (min(16384, cfg.max_points) corner, min(65536, cfg.max_points) surf; a built map may hold up to 65536
- *     corner points in a cube), or more than 1024 cubes of one type that hold points.
+ *     loop must end); ALOAM_ERR_CAPACITY when the prior map does not fit a lane's store under the context's cube growth at the time
+ *     of the call.  Growth off: a cube with more points than the slab capacity of its type (min(16384, cfg.max_points) corner,
+ *     min(65536, cfg.max_points) surf; a built map may hold up to 65536 corner points in a cube), or more than 1024 cubes of one
+ *     type that hold points.  Growth on: a cube above its type's ceiling (the largest run's capacity), or runs that need more than
+ *     1024 slabs of one type.
  *   - arming: a lane has one arming; aloam_lane_localise and aloam_lane_map_on_prior replace each other (the later call wins).  An
  *     odometry-only START does not consume it; aloam_reset_odometry drops it, and so do aloam_prior_map_load, aloam_prior_map_build
- *     and aloam_prior_map_clear when they succeed, since the fit was checked against the map of the time (aloam_lane_localise
+ *     and aloam_prior_map_clear when they succeed and every aloam_set_cube_growth call, since the fit was checked against the map
+ *     and the setting of the time (aloam_lane_localise
  *     armings keep their rules).  After its START a seeded lane no longer depends on the prior map: loading, building or clearing a
  *     map between calls does not change it.
  *   - cost: arming allocates nothing and a stream call in which no seeded START runs issues exactly what it issued before.  A step
@@ -432,6 +448,37 @@ int aloam_lane_localise(aloam_ctx* ctx, int lane, const double q_init[4], const 
  *     (k_store_seed_tables, k_store_seed_copy).  The lane's store is created as for any mapped START; the first call that seeds a
  *     store also creates cfg.max_batch export layouts of about 155 kB each on the device, kept until aloam_destroy. */
 int aloam_lane_map_on_prior(aloam_ctx* ctx, int lane, const double q_init[4], const double t_init[3]);
+
+/* ---- cube growth: map cubes that outgrow one slab, for dense lidars (OS1-64, HDL-64, VLP-32C, a VLP-16 at the default leaves).
+ * The reference's cubes grow without bound; each cube of a lane store here holds a RUN of 2^k consecutive slabs of its type from
+ * the lane's pool (1024 slabs per type, as before: store memory and re-filter buffers do not change).  With growth off (the
+ * default) every run is one slab and the store is what it always was: a cube holds at most min(16384, max_points) corner /
+ * min(65536, max_points) surf points and the rest is dropped (ALOAM_FLAG_CUBE_OVERFLOW).
+ * aloam_set_cube_growth(ctx, on): on = 1 turns growth on, 0 off; anything else is ALOAM_ERR_INVALID_ARG.  It may be called at any
+ * time between calls.  A lane takes the context's setting at each mapped START (a seeded START of aloam_lane_map_on_prior too);
+ * lane 0 of the host API and the lockstep stream calls take it at aloam_mapper_reset and when a store is created; a running lane
+ * keeps the setting it started with; a restored lane takes its snapshot's (header byte 220).  The call drops every
+ * aloam_lane_map_on_prior arming (its fit was checked under the old setting).
+ * With growth on:
+ *   - runs: a run of 2^k slabs starts at a slab index that is a multiple of 2^k, so a cube's points lie contiguously.  The largest
+ *     run is the largest power of two r with r x slab capacity <= ALOAM_MAX_CUBE_POINTS: 16 corner / 4 surf slabs at the default
+ *     capacities.  A cube's first point takes one slab; when an insert would pass its run's capacity the cube moves to the smallest
+ *     run that holds its new count (at most its ceiling), its points copied in order to the start of the new run, the old run freed
+ *     once the insert has served every cube.  Points are appended in stack order: a cube's points are the reference's push_back
+ *     order.  Which run a cube holds never changes a result, only whether a later allocation succeeds.  Runs never shrink while
+ *     the cube stays in the buffer; a cube that scrolls out of the ring buffer frees its whole run.
+ *   - allocation is deterministic: the lowest-address aligned free block, cubes served in the order of their first point in the
+ *     frame's stack (so when the pool runs out, the new cubes that come first in the stack get runs).
+ *   - drops: a point is dropped, with ALOAM_FLAG_CUBE_OVERFLOW, only when its cube already holds its ceiling or when no aligned free
+ *     block of the needed size exists; the points dropped are those beyond the cube's current capacity, in stack order.
+ *   - re-filter: the per-cube voxel filter of a frame sorts at most max(75 x (corner + surf slab capacity), 2 x max_points) points,
+ *     as before.  The valid cubes go in, corner then surf, while their running total fits; the cubes from the first one that does
+ *     not fit on stay unfiltered for that frame, and the frame raises ALOAM_FLAG_CUBE_OVERFLOW (error word bit 4).  This is the one
+ *     way the store can differ from the reference without a drop.  With growth off every valid cube fits.
+ * So with growth on a dense trajectory matches the reference until a cube passes ALOAM_MAX_CUBE_POINTS or the pool fragments.
+ * Prior maps: a growth-on snapshot's cubes load (aloam_prior_map_load); aloam_prior_map_build accepts filtered cubes of up to
+ * ALOAM_MAX_CUBE_POINTS while growth is on; aloam_lane_map_on_prior checks its fit under the setting at the time of the call. */
+int aloam_set_cube_growth(aloam_ctx* ctx, int on);
 
 /* ---- relocalisation: finding the map pose aloam_lane_localise needs, for a vehicle that boots on the map, a lane that lost
  * track or a recording that starts somewhere unknown.  aloam_prior_relocalise scores n_hyp pose hypotheses of ONE scan against
@@ -524,14 +571,16 @@ int aloam_debug_prior_associate(aloam_ctx* ctx, int lane, aloam_cloud_view corne
 /* ---- map cube store + the mapping loop around it (lane 0 of the mapper; the other lanes exist only for
  * aloam_scan_stream_mapped_batch) (laserMapping.cpp:74-108,142-163,309-550,736-801; SURVEY.md 8 f-1).
  * The 21 x 21 x 11 ring buffer of 50 m cubes lives in device memory: a pool of fixed-capacity slabs (1024 per cloud type,
- * 16 k corner / 64 k surf points each, 1.3 GB, created on first use) handed to cubes on their first insertion.
+ * 16 k corner / 64 k surf points each, 1.3 GB, created on first use) handed to cubes on their first insertion, one slab per cube
+ * with cube growth off, a run of up to ALOAM_MAX_CUBE_POINTS points with growth on (aloam_set_cube_growth).
  * aloam_mapper_step is one frame of alaserMapping's process(), entirely on the device with one synchronisation at the end:
  * pose hand-off from the odometry (transformAssociateToMap), ring-buffer shift, gather of the <= 75 valid cubes (device
  * to device), stack filters at line_res / plane_res, optimisation against the gathered submap (skipped while it is thinner
  * than 10 corner / 50 surf points), transformUpdate, insertion of the registered stacks and per-cube VoxelGrid of the valid
  * cubes.  corner_last / surf_last are the less-sharp / less-flat clouds of the scan (what /laser_cloud_corner_last and
  * /laser_cloud_surf_last carry); the odometry pose is q_wodom_curr / t_wodom_curr; the refined pose is returned.
- * The call never fails half-way: a full cube slab, an exhausted pool or a submap beyond cfg.max_map_points drop the
+ * The call never fails half-way: a full cube, an exhausted pool, cubes beyond the re-filter's buffer (growth on) or a submap
+ * beyond cfg.max_map_points drop (or leave unfiltered) the
  * overflow and set ALOAM_FLAG_CUBE_OVERFLOW in stats->flags of the frame where it happened (the flags of every frame
  * describe that frame only); argument errors are reported before any state changes.  A cube whose voxel index range does
  * not fit the sort key is kept unfiltered and the frame returns ALOAM_ERR_CAPACITY after completing (pose and store are
@@ -623,7 +672,8 @@ int aloam_registered_rows(aloam_ctx* ctx, long long* begin, int* count, int rows
 typedef struct aloam_map_row {
   int kind;          /* ALOAM_ROW_* */
   int err;           /* the frame's error word: bit 0 voxel index range beyond the sort key (why the call returned ALOAM_ERR_CAPACITY),
-                        bits 1-3 slab overflow / pool exhausted / submap truncated */
+                        bit 1 a cube at its capacity dropped points, bit 2 no free run of slabs, bit 3 submap truncated, bit 4
+                        cubes left out of the re-filter (aloam_set_cube_growth) */
   int n_valid;       /* cubes in the frame's window */
   int n_sub[2];      /* corner / surf map points the frame registered against (the gathered submap, or a localising lane's window) */
   int n_stack[2];    /* the filtered corner / surf stacks */
