@@ -467,6 +467,10 @@ int aloam_lane_map_on_prior(aloam_ctx* ctx, int lane, const double q_init[4], co
  *     once the insert has served every cube.  Points are appended in stack order: a cube's points are the reference's push_back
  *     order.  Which run a cube holds never changes a result, only whether a later allocation succeeds.  Runs never shrink while
  *     the cube stays in the buffer; a cube that scrolls out of the ring buffer frees its whole run.
+ *   - the whole pool: when a type's largest run is all 1024 slabs (slab capacity <= 256 points, max_points <= 256), an insert
+ *     grows a cube to at most 512 slabs, 512 x capacity points (131072 at 256): the new run is taken while the old one is still
+ *     held, so the whole pool is never free for it.  The points beyond are dropped with ALOAM_FLAG_CUBE_OVERFLOW.  A restore or a
+ *     seeded START can still give one cube the whole pool (up to ALOAM_MAX_CUBE_POINTS points).
  *   - allocation is deterministic: the lowest-address aligned free block, cubes served in the order of their first point in the
  *     frame's stack (so when the pool runs out, the new cubes that come first in the stack get runs).
  *   - drops: a point is dropped, with ALOAM_FLAG_CUBE_OVERFLOW, only when its cube already holds its ceiling or when no aligned free
@@ -475,7 +479,8 @@ int aloam_lane_map_on_prior(aloam_ctx* ctx, int lane, const double q_init[4], co
  *     as before.  The valid cubes go in, corner then surf, while their running total fits; the cubes from the first one that does
  *     not fit on stay unfiltered for that frame, and the frame raises ALOAM_FLAG_CUBE_OVERFLOW (error word bit 4).  This is the one
  *     way the store can differ from the reference without a drop.  With growth off every valid cube fits.
- * So with growth on a dense trajectory matches the reference until a cube passes ALOAM_MAX_CUBE_POINTS or the pool fragments.
+ * So with growth on a dense trajectory matches the reference until a cube passes the largest run's capacity (half of it where that
+ * run is the whole pool) or the pool fragments.
  * Prior maps: a growth-on snapshot's cubes load (aloam_prior_map_load); aloam_prior_map_build accepts filtered cubes of up to
  * ALOAM_MAX_CUBE_POINTS while growth is on; aloam_lane_map_on_prior checks its fit under the setting at the time of the call. */
 int aloam_set_cube_growth(aloam_ctx* ctx, int on);

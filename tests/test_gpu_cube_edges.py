@@ -111,16 +111,19 @@ def _grid_cloud(rng, cen, t, kk):
     return out[rng.permutation(n)]
 
 
+@pytest.mark.parametrize("growth", [0, 1])
 @pytest.mark.parametrize("jump,fill_k", [(40, (4, 5, 6)), (12, (5,)), (-40, (4, 5, 6)), (-12, (5,))])
-def test_slab_pool_after_wraps(aloam, orc, jump, fill_k):
+def test_slab_pool_after_wraps(aloam, orc, jump, fill_k, growth):
     """frame 0 puts a point in every cube of layers fill_k (1323 or 441 cubes); frame 1 jumps `jump` cubes along i, wrapping every
     cube (+-40) or five i-planes (+-12: the lowest ones on the shifts towards low indices, the highest ones on the shifts towards
     high indices); frame 2 puts a point in all 1323 cubes of layers 4-6 around the new centre.  The
     wrapped cubes' slabs are back in the pool: the store holds exactly the model's cubes -- those kept plus as many new ones as
-    the 1024 slabs allow -- and every cube it holds equals the oracle's"""
+    the 1024 slabs allow -- and every cube it holds equals the oracle's.  With growth on (one point per cube, so every run is one
+    slab) the result is the same"""
     rng = np.random.default_rng(abs(jump) + (jump < 0))
     c = aloam.Aloam(n_scans=16, max_points=3000, max_map_points=20000)
     try:
+        c.set_cube_growth(growth)
         c.mapper_reset()
         m, cm = E.Model(), orc.CubeMap()
         ident = np.array(E.IDENT_Q)
