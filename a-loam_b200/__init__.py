@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = [
     "aloam_set_recovery", "aloam_recovery_rows", "aloam_debug_recovery_scores",
     "aloam_lane_map_on_prior", "aloam_set_cube_growth",
     "aloam_io_unpack_points_ring",
+    "aloam_create_wide",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -40,6 +41,7 @@ EXPORT_SURROUND, EXPORT_MAP = 0, 1
 PRIOR_MAP = -1   # `lane` of mapper_export: the context's prior map
 ROW_IDLE, ROW_MAPPED, ROW_LOCALISED, ROW_SKIPPED = 0, 1, 2, 3   # aloam_map_row.kind
 RING_ELEVATION, RING_FIELD = 0, 1   # aloam_config.ring_source: the elevation formula, or the driver's ring in float 3 of a raw point
+MAX_RINGS = 128   # ALOAM_MAX_RINGS: the most rings a context takes (Aloam(..., wide=True), driver rings only)
 MAX_CUBE_POINTS = 262144   # ALOAM_MAX_CUBE_POINTS: the most points one map cube holds with cube growth on (set_cube_growth)
 
 
@@ -127,6 +129,7 @@ def lib():
         L.aloam_default_config.argtypes = [C.POINTER(Config), C.c_int]
         L.aloam_default_config.restype = None
         L.aloam_create.argtypes = [C.POINTER(Config), C.POINTER(C.c_void_p)]
+        L.aloam_create_wide.argtypes = [C.POINTER(Config), C.POINTER(C.c_void_p)]
         L.aloam_destroy.argtypes = [C.c_void_p]
         L.aloam_strerror.argtypes = [C.c_int]
         L.aloam_strerror.restype = C.c_char_p
@@ -309,7 +312,8 @@ def default_config(n_scans):
 class Aloam:
     """One context = one caller thread = one CUDA stream on one GPU (mirrors `aloam_ctx`)."""
 
-    def __init__(self, n_scans=64, device=0, max_points=None, **overrides):
+    def __init__(self, n_scans=64, device=0, max_points=None, wide=False, **overrides):
+        """wide=True creates the context with aloam_create_wide: driver rings (ring_source=RING_FIELD) up to MAX_RINGS"""
         cfg = default_config(n_scans)
         cfg.device = device
         if max_points is not None:
@@ -318,7 +322,8 @@ class Aloam:
             setattr(cfg, k, v)
         self.cfg = cfg
         self._h = C.c_void_p()
-        _check(lib().aloam_create(C.byref(cfg), C.byref(self._h)))
+        create = lib().aloam_create_wide if wide else lib().aloam_create
+        _check(create(C.byref(cfg), C.byref(self._h)))
 
     def close(self):
         if getattr(self, "_h", None) and self._h:
@@ -342,8 +347,8 @@ class Aloam:
     def debug_features(self, n_full):
         curv = np.zeros(n_full, np.float32)
         label = np.zeros(n_full, np.int32)
-        s = np.zeros(64, np.int32)
-        e = np.zeros(64, np.int32)
+        s = np.zeros(MAX_RINGS, np.int32)
+        e = np.zeros(MAX_RINGS, np.int32)
         ip = C.POINTER(C.c_int)
         _check(lib().aloam_debug_features(self._h, curv.ctypes.data_as(C.POINTER(C.c_float)), label.ctypes.data_as(ip),
                                           s.ctypes.data_as(ip), e.ctypes.data_as(ip)))

@@ -36,7 +36,7 @@ const char* aloam_strerror(int code) {
   switch (code) {
     case ALOAM_OK: return "ok";
     case ALOAM_ERR_INVALID_ARG: return "invalid argument";
-    case ALOAM_ERR_UNSUPPORTED_SCANS: return "n_scans must be 16, 32 or 64 for elevation rings, 1..64 for driver rings";
+    case ALOAM_ERR_UNSUPPORTED_SCANS: return "n_scans must be 16, 32 or 64 for elevation rings, 1..64 for driver rings (1..128 through aloam_create_wide)";
     case ALOAM_ERR_EMPTY_CLOUD: return "no point survives the NaN / minimum-range filter";
     case ALOAM_ERR_CAPACITY: return "cloud larger than the context capacity";
     case ALOAM_ERR_CUDA: return "CUDA error";
@@ -77,7 +77,8 @@ int aloam_reset_odometry(aloam_ctx* c) {
   return ALOAM_OK;
 }
 
-int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
+// aloam_create (max_field_rings 64) and aloam_create_wide (ALOAM_MAX_RINGS): the same context, only the range of driver rings differs
+static int create_ctx(const aloam_config* cfg_in, aloam_ctx** out, int max_field_rings) {
   if (!cfg_in || !out) return ALOAM_ERR_INVALID_ARG;
   *out = nullptr;
   aloam_config cfg = *cfg_in;
@@ -86,9 +87,13 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   if (cfg.mapping_skip_frame == 0) cfg.mapping_skip_frame = 1;
   if (cfg.mapping_skip_frame < 0) return ALOAM_ERR_INVALID_ARG;
   if (cfg.ring_source != ALOAM_RING_ELEVATION && cfg.ring_source != ALOAM_RING_FIELD) return ALOAM_ERR_INVALID_ARG;
-  if (cfg.ring_source == ALOAM_RING_FIELD ? cfg.n_scans < 1 || cfg.n_scans > 64 : cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64)
+  if (cfg.ring_source == ALOAM_RING_FIELD ? cfg.n_scans < 1 || cfg.n_scans > max_field_rings : cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64)
     return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
+  // a 128-wide association index packs a point's index into 24 bits (index << 7 | ring), and aloam_odometry_set_last takes
+  // clouds of up to max_points
+  const int ring_w = ring_width(cfg.n_scans);
+  if (ring_w > 64 && cfg.max_points > (1 << 24)) return ALOAM_ERR_INVALID_ARG;
   if (!(cfg.nearby_scan >= 1.0)) return ALOAM_ERR_INVALID_ARG;   // the association's break tables need a window of +-1 ring at least
   // HuberLoss(a) needs a > 0, and a VoxelGrid leaf <= 0 or NaN has no voxels
   if (!(cfg.huber > 0) || !(cfg.line_res > 0) || !(cfg.plane_res > 0)) return ALOAM_ERR_INVALID_ARG;
@@ -104,10 +109,12 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   c->cfg = cfg;
   c->max_points = cfg.max_points;
   c->max_ring = cfg.max_ring_points;
+  c->ring_w = ring_w;
   c->n_lanes = cfg.max_batch;
   c->nblocks_max = (c->max_points + 1023) / 1024;
   const size_t mp = (size_t)c->max_points;
   const size_t mr = (size_t)c->max_ring;
+  const size_t rw = (size_t)ring_w;   // the per-ring tables below hold rw rings: a 64-wide context allocates what it always did
 #define TRY(e) do { if ((e) != cudaSuccess) { fprintf(stderr, "[aloam_b200] %s failed: %s\n", #e, cudaGetErrorString(cudaGetLastError())); aloam_destroy(c); return ALOAM_ERR_CUDA; } } while (0)
   TRY(cudaDeviceGetAttribute(&c->sms, cudaDevAttrMultiProcessorCount, cfg.device));
   TRY(screate(c, &c->stream));
@@ -127,14 +134,14 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   for (ScanScalars& s : init) { s.first_valid = INT32_MAX; s.last_valid = -1; s.half_idx = INT32_MAX; s.n_full = 0; s.start_ori = 0; s.end_ori = 0; s.error = 0; s.pad = 0; }
   for (Lane& L : c->lanes) {
     for (int b = 0; b < 2; ++b) {
-      TRY(dalloc(c, &L.d_raw[b], mp * 8)); TRY(dalloc(c, &L.d_full[b], mp)); TRY(dalloc(c, &L.d_ring_start[b], 72));
-      TRY(dalloc(c, &L.st_sharp[b], 64 * kMaxSharpPerRing)); TRY(dalloc(c, &L.st_less_sharp[b], 64 * kMaxLessSharpPerRing));
-      TRY(dalloc(c, &L.st_flat[b], 64 * kMaxFlatPerRing)); TRY(dalloc(c, &L.st_less_flat[b], (size_t)64 * mr));
-      TRY(dalloc(c, &L.st_counts[b], 64 * 4));
+      TRY(dalloc(c, &L.d_raw[b], mp * 8)); TRY(dalloc(c, &L.d_full[b], mp)); TRY(dalloc(c, &L.d_ring_start[b], rw + 8));
+      TRY(dalloc(c, &L.st_sharp[b], rw * kMaxSharpPerRing)); TRY(dalloc(c, &L.st_less_sharp[b], rw * kMaxLessSharpPerRing));
+      TRY(dalloc(c, &L.st_flat[b], rw * kMaxFlatPerRing)); TRY(dalloc(c, &L.st_less_flat[b], rw * mr));
+      TRY(dalloc(c, &L.st_counts[b], rw * 4));
     }
     TRY(dalloc(c, &L.d_ring, mp));
-    TRY(dalloc(c, &L.d_hist, (size_t)c->nblocks_max * 64)); TRY(dalloc(c, &L.d_offsets, (size_t)c->nblocks_max * 64));
-    TRY(dalloc(c, &L.d_scan_start, 64)); TRY(dalloc(c, &L.d_scan_end, 64));
+    TRY(dalloc(c, &L.d_hist, (size_t)c->nblocks_max * rw)); TRY(dalloc(c, &L.d_offsets, (size_t)c->nblocks_max * rw));
+    TRY(dalloc(c, &L.d_scan_start, rw)); TRY(dalloc(c, &L.d_scan_end, rw));
     TRY(dalloc(c, &L.d_sc, 3));
     TRY(cudaMemcpy(L.d_sc, init, sizeof(init), cudaMemcpyHostToDevice));
     for (FeatBuf& f : L.feat) {
@@ -142,13 +149,13 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
       TRY(dalloc(c, &f.less_sharp, mp)); TRY(dalloc(c, &f.less_flat, mp));
       TRY(dalloc(c, &f.counts, 4));
       for (RabIndex* g : {&f.g_ls, &f.g_lf}) {
-        TRY(dalloc(c, &g->cnt, (size_t)ALOAM_NB * 64)); TRY(dalloc(c, &g->start, (size_t)ALOAM_NB * 64 + 8));
+        TRY(dalloc(c, &g->cnt, (size_t)ALOAM_NB * rw)); TRY(dalloc(c, &g->start, (size_t)ALOAM_NB * rw + 8));
         TRY(dalloc(c, &g->cell_of, mp)); TRY(dalloc(c, &g->rank_of, mp)); TRY(dalloc(c, &g->gpts, mp));
-        TRY(cudaMemset(g->cnt, 0, (size_t)ALOAM_NB * 64 * 4)); TRY(cudaMemset(g->start, 0, ((size_t)ALOAM_NB * 64 + 8) * 4));
-        TRY(dalloc(c, &g->first_of, kRabBreakInts));
-        g->last_of = g->first_of + 64; g->fwd_end = g->last_of + 64; g->bwd_begin = g->fwd_end + 65;
-        TRY(cudaMemset(g->first_of, 0x7f, 64 * 4)); TRY(cudaMemset(g->last_of, 0xff, 64 * 4));   // 0x7f7f7f7f (> any index), -1
-        TRY(cudaMemset(g->fwd_end, 0, 130 * 4));
+        TRY(cudaMemset(g->cnt, 0, (size_t)ALOAM_NB * rw * 4)); TRY(cudaMemset(g->start, 0, ((size_t)ALOAM_NB * rw + 8) * 4));
+        TRY(dalloc(c, &g->first_of, rab_break_ints(ring_w)));
+        g->last_of = g->first_of + rw; g->fwd_end = g->last_of + rw; g->bwd_begin = g->fwd_end + rw + 1;
+        TRY(cudaMemset(g->first_of, 0x7f, rw * 4)); TRY(cudaMemset(g->last_of, 0xff, rw * 4));   // 0x7f7f7f7f (> any index), -1
+        TRY(cudaMemset(g->fwd_end, 0, (2 * rw + 2) * 4));
       }
       TRY(cudaMemset(f.counts, 0, 16));
     }
@@ -180,6 +187,9 @@ int aloam_create(const aloam_config* cfg_in, aloam_ctx** out) {
   return ALOAM_OK;
 }
 
+int aloam_create(const aloam_config* cfg, aloam_ctx** out) { return create_ctx(cfg, out, 64); }
+int aloam_create_wide(const aloam_config* cfg, aloam_ctx** out) { return create_ctx(cfg, out, ALOAM_MAX_RINGS); }
+
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------ kernel sequencing
@@ -207,10 +217,12 @@ int run_features_a(aloam_ctx* c, int nb, const int* pl, const float* const* d_ra
                            nfull_out ? nfull_out + pl[l] : nullptr};
     sa.a[l] = ScatterArgs{d_raw[l], n[l], stride, L.d_ring, L.d_offsets, sc, L.d_full[buf]};
   }
-  if (c->cfg.ring_source == ALOAM_RING_FIELD) LAUNCH(c, KID_CLASSIFY, k_classify<ALOAM_RING_FIELD>, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
-  else LAUNCH(c, KID_CLASSIFY, k_classify<ALOAM_RING_ELEVATION>, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
-  launch_ex(c, KID_RING_SCAN, k_ring_scan, dim3(nb), dim3(1024), 0, 1, true, ra, c->cfg.n_scans);
-  launch_ex(c, KID_SCATTER, k_scatter, dim3(blocks, nb), dim3(256), 0, 1, true, sa);
+  // one instance per (ring source, ring width); elevation rings stop at 64
+  const auto classify = c->ring_w == 128 ? k_classify<ALOAM_RING_FIELD, 128>
+                      : c->cfg.ring_source == ALOAM_RING_FIELD ? k_classify<ALOAM_RING_FIELD, 64> : k_classify<ALOAM_RING_ELEVATION, 64>;
+  LAUNCH(c, KID_CLASSIFY, classify, dim3(blocks, nb), 256, 0, ca, c->cfg.n_scans, thres * thres);
+  launch_ex(c, KID_RING_SCAN, c->ring_w == 128 ? k_ring_scan<128> : k_ring_scan<64>, dim3(nb), dim3(1024), 0, 1, true, ra, c->cfg.n_scans);
+  launch_ex(c, KID_SCATTER, c->ring_w == 128 ? k_scatter<128> : k_scatter<64>, dim3(blocks, nb), dim3(256), 0, 1, true, sa);
   *sc_slot = c->parity;
   c->parity = (c->parity + 1) % 3;
   CUDA_CHECK_RET(cudaGetLastError());
@@ -260,9 +272,10 @@ void run_grid_build(aloam_ctx* c, int nb, const int* pl, int slot, int n_ls, int
     FeatBuf& f = c->lanes[pl[l]].feat[slot];
     ga.a[l] = RabArgs{f.g_ls, f.less_sharp, f.counts + 1, f.g_lf, f.less_flat, f.counts + 3};
   }
-  LAUNCH(c, KID_GRID_BUILD, k_rab_count, dim3(pb, 2, nb), 256, 0, ga);
-  launch_ex(c, KID_GRID_BUILD, k_rab_scan, dim3(2, nb), dim3(1024), 0, 1, true, ga);
-  launch_ex(c, KID_GRID_BUILD, k_rab_fill, dim3(pb, 2, nb), dim3(256), 0, 1, true, ga);
+  const bool wide = c->ring_w == 128;
+  LAUNCH(c, KID_GRID_BUILD, (wide ? k_rab_count<128> : k_rab_count<64>), dim3(pb, 2, nb), 256, 0, ga);
+  launch_ex(c, KID_GRID_BUILD, wide ? k_rab_scan<128> : k_rab_scan<64>, dim3(2, nb), dim3(1024), 0, 1, true, ga);
+  launch_ex(c, KID_GRID_BUILD, wide ? k_rab_fill<128> : k_rab_fill<64>, dim3(pb, 2, nb), dim3(256), 0, 1, true, ga);
 }
 
 // outer_iters x (association + LM) ; feat[cur] supplies sharp/flat, feat[last] the targets ; pose in lane.d_pose
@@ -285,7 +298,7 @@ void run_register(aloam_ctx* c, int nb, const int* pl, int cur, int last, int sh
       la.a[l] = LmArgs{L.d_blocks, nullptr, slots, pose, L.d_summary + (it & 3), (integrate && last_it && pose_slots) ? pose_slots + (size_t)lane * 7 : nullptr, L.d_world};
     }
     // within one call the chain association -> LM -> association -> LM is launched with programmatic dependencies
-    if (slots > 0) launch_ex(c, KID_ODOM_ASSOC, k_odom_assoc, dim3((slots + 7) / 8, nb), dim3(256), 0, 1, it > 0, aa, op, sharp_slots);
+    if (slots > 0) launch_ex(c, KID_ODOM_ASSOC, c->ring_w == 128 ? k_odom_assoc<128> : k_odom_assoc<64>, dim3((slots + 7) / 8, nb), dim3(256), 0, 1, it > 0, aa, op, sharp_slots);
     launch_lm_batch(c, slots > 0, la, nb, lp, 0, (integrate && last_it) ? 1 : 0, c->cfg.distortion != 0, false);   // local: cannot fail
   }
 }
@@ -311,8 +324,9 @@ int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf) {
   FeatBuf& f = c->lanes[lane].feat[slot];
   CUDA_CHECK_RET(cudaMemsetAsync(c->d_err, 0, 4, c->stream));
   run_grid_build(c, 1, &lane, slot, n_ls, n_lf);
-  if (n_ls > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (n_ls + 255) / 256, 256, 0, f.less_sharp, n_ls, f.g_ls.fwd_end, c->d_err);
-  if (n_lf > 0) LAUNCH(c, KID_RING_OFFSETS, k_ring_offsets, (n_lf + 255) / 256, 256, 0, f.less_flat, n_lf, f.g_lf.fwd_end, c->d_err);
+  const auto ring_offsets = c->ring_w == 128 ? k_ring_offsets<128> : k_ring_offsets<64>;   // int(intensity) in 0 .. ring_w - 1
+  if (n_ls > 0) LAUNCH(c, KID_RING_OFFSETS, ring_offsets, (n_ls + 255) / 256, 256, 0, f.less_sharp, n_ls, f.g_ls.fwd_end, c->d_err);
+  if (n_lf > 0) LAUNCH(c, KID_RING_OFFSETS, ring_offsets, (n_lf + 255) / 256, 256, 0, f.less_flat, n_lf, f.g_lf.fwd_end, c->d_err);
   CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->ring_err, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -443,7 +457,7 @@ int aloam_odometry_associate(aloam_ctx* c, aloam_cloud_view sharp, aloam_cloud_v
   if (slots > 0) {
     Batch<AssocArgs> aa = {};
     aa.a[0] = AssocArgs{cur.sharp, cur.flat, cur.counts, last_corner(L.feat[kApiLast]), last_surf(L.feat[kApiLast]), c->d_api_pose, L.d_blocks, L.d_corr};
-    LAUNCH(c, KID_ODOM_ASSOC, k_odom_assoc, dim3((slots + 7) / 8, 1), 256, 0, aa, op, sharp.n);
+    LAUNCH(c, KID_ODOM_ASSOC, (c->ring_w == 128 ? k_odom_assoc<128> : k_odom_assoc<64>), dim3((slots + 7) / 8, 1), 256, 0, aa, op, sharp.n);
   }
   std::vector<int> h((size_t)slots * 4 + 4);
   if (slots > 0) CUDA_CHECK_RET(cudaMemcpyAsync(h.data(), L.d_corr, (size_t)slots * 16, cudaMemcpyDeviceToHost, c->stream));
@@ -473,14 +487,14 @@ static int scan_to_pose_impl(aloam_ctx* c, const float* d_raw, int n, int stride
     CUDA_CHECK_RET(cudaEventRecord(c->ev_feat[cur], c->stream));
     CUDA_CHECK_RET(cudaStreamWaitEvent(c->s_idx, c->ev_feat[cur], 0));
     if (!c->prof_on) c->stream = c->s_idx;   // (the per-kernel profiler times everything on one stream)
-    run_grid_build(c, 1, kLane0, cur, 64 * kMaxLessSharpPerRing, std::min(n, c->max_points));
+    run_grid_build(c, 1, kLane0, cur, c->less_sharp_upper(), std::min(n, c->max_points));
     CUDA_CHECK_RET(cudaEventRecord(c->ev_idx[cur], c->stream));
   }
   if (c->frame == 0) {
     flags |= ALOAM_FLAG_INITIALISED_ONLY;  // laserOdometry.cpp:267-271
   } else {
     CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_idx[last], 0));   // the previous scan's index (built during the previous call)
-    run_register(c, 1, kLane0, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, nullptr, nullptr);
+    run_register(c, 1, kLane0, cur, last, c->fused_sharp_slots(), c->fused_flat_slots(), true, false, nullptr, nullptr);
   }
   CUDA_CHECK_RET(cudaEventRecord(c->ev_odo[cur], c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->world, L.d_world, 56, cudaMemcpyDeviceToHost, c->stream));
@@ -588,7 +602,7 @@ static int map_stage(aloam_ctx* c, const StreamSwitches& w, const StreamRow* row
     fr[g][n_fr[g]++] = MapperIn{fc.less_sharp, fc.counts + 1, fc.less_flat, fc.counts + 3, c->d_poses + slot, c->d_map_poses + slot, l,
                                 w.reset_stores && row[l].op == ALOAM_LANE_START && !row[l].seed, row[l].localise, row[l].seed};
   }
-  const int n_upper_c = 64 * kMaxLessSharpPerRing, n_upper_s = std::min(nmax, c->max_points);
+  const int n_upper_c = c->less_sharp_upper(), n_upper_s = std::min(nmax, c->max_points);
   for (int loc = 0; loc < 2; ++loc) {   // the mapping frame, then the locate frame, each followed by its rows and registered clouds
     const MapperIn* in = fr[loc]; const int n = n_fr[loc];
     if (n == 0) continue;
@@ -703,7 +717,7 @@ static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const Stream
     if (rc) return rc;
     STREAM_TRY(cudaEventRecord(c->ev_cmp[b], c->s_idx));
     STREAM_TRY(cudaEventRecord(c->ev_feat[cur], c->s_idx));
-    run_grid_build(c, na, act, cur, 64 * kMaxLessSharpPerRing, std::min(nmax, c->max_points));
+    run_grid_build(c, na, act, cur, c->less_sharp_upper(), std::min(nmax, c->max_points));
     STREAM_TRY(cudaEventRecord(c->ev_idx[cur], c->s_idx));
     c->stream = s_main;
     // ---- association + LM on the main stream: this scan's sharp / flat points, the previous scan's clouds + index
@@ -717,7 +731,7 @@ static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const Stream
       STREAM_TRY(cudaMemcpyAsync(L.d_world, c->d_ident, 56, cudaMemcpyDeviceToDevice, s_main));
       STREAM_TRY(cudaMemcpyAsync(slots + (size_t)starting[i] * 7, L.d_world, 56, cudaMemcpyDeviceToDevice, s_main));
     }
-    if (n_scan > 0) run_register(c, n_scan, scanning, cur, last, kFusedSharpSlots, kFusedFlatSlots, true, false, slots, nullptr);
+    if (n_scan > 0) run_register(c, n_scan, scanning, cur, last, c->fused_sharp_slots(), c->fused_flat_slots(), true, false, slots, nullptr);
     STREAM_TRY(cudaEventRecord(c->ev_odo[cur], s_main));
     if (w.map) {
       rc = map_stage(c, w, row, (size_t)k * nb, act, na, cur, nmax);
@@ -960,7 +974,7 @@ int aloam_knn(aloam_ctx* c, int which, aloam_cloud_view queries, int k, int* idx
     if (queries.n > 0) {
       const FeatBuf& f0 = c->lanes[0].feat[kApiLast];
       LastCloud L = which == 0 ? last_corner(f0) : last_surf(f0);
-      LAUNCH(c, KID_KNN_LAST, k_knn_last, (queries.n + 7) / 8, 256, 0, L, c->d_query, queries.n, c->d_knn_idx, c->d_knn_d);
+      LAUNCH(c, KID_KNN_LAST, (c->ring_w == 128 ? k_knn_last<128> : k_knn_last<64>), (queries.n + 7) / 8, 256, 0, L, c->d_query, queries.n, c->d_knn_idx, c->d_knn_d);
       CUDA_CHECK_RET(cudaMemcpyAsync(idx, c->d_knn_idx, (size_t)queries.n * 4, cudaMemcpyDeviceToHost, c->stream));
       CUDA_CHECK_RET(cudaMemcpyAsync(sqdist, c->d_knn_d, (size_t)queries.n * 4, cudaMemcpyDeviceToHost, c->stream));
     }

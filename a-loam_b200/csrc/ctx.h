@@ -101,9 +101,8 @@ using namespace aloam;
 
 namespace {
 
+// per-ring caps of the feature clouds; a context's query slots and staging sets are ring_w (64 or 128) times these
 constexpr int kMaxSharpPerRing = 12, kMaxLessSharpPerRing = 120, kMaxFlatPerRing = 24;
-constexpr int kFusedSharpSlots = 64 * kMaxSharpPerRing;  // 768
-constexpr int kFusedFlatSlots = 64 * kMaxFlatPerRing;    // 1536
 constexpr int kMaxQueries = ALOAM_MAX_QUERIES;         // API-path capacity for sharp / flat query clouds
 constexpr int kProfSlots = 192;                        // kernel launches timed per profile window (one API call)
 constexpr int kFeatSlots = 4;                          // feature-set ring of the fused / stream paths
@@ -221,6 +220,12 @@ struct aloam_ctx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int max_points = 0, nblocks_max = 0, max_ring = ALOAM_MAX_RING, n_lanes = 1;
+  // ring width (kernels.h ring_width): 64, or 128 for a context of aloam_create_wide with more than 64 rings.  The fused paths'
+  // query slots (sharp 12 / flat 24 per ring: 768 / 1536 at 64) and the less-sharp bound (120 per ring) follow from it.
+  int ring_w = 64;
+  int fused_sharp_slots() const { return ring_w * kMaxSharpPerRing; }
+  int fused_flat_slots() const { return ring_w * kMaxFlatPerRing; }
+  int less_sharp_upper() const { return ring_w * kMaxLessSharpPerRing; }
   int sms = 1;                     // SMs of cfg.device (grid-stride launch sizes)
   std::vector<Lane> lanes;
   float* d_curv = nullptr;         // debug outputs of the last extraction (lane 0 only)

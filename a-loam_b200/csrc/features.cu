@@ -95,7 +95,8 @@ __device__ __forceinline__ float ori_first_half(float x, float y, float start_or
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
-template <int RingSource>
+// W: ring width of the context (64 or 128, ring_width()): the histogram has W entries per CTA
+template <int RingSource, int W>
 __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2) {
   pdl_launch_dependents();   // the next kernel of the stream may become resident (it blocks in pdl_wait())
   // blockIdx.y = trajectory (lane) of the batch; a lane with fewer returns than the largest one has idle trailing CTAs
@@ -106,10 +107,10 @@ __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<C
   int* __restrict__ hist = A.hist;
   ScanScalars* __restrict__ sc = A.sc;
   if (blockIdx.x * CHUNK >= n && blockIdx.x > 0) return;
-  __shared__ int s_hist[64];
+  __shared__ int s_hist[W];
   __shared__ int s_first, s_last, s_half;
   const int tid = threadIdx.x;
-  if (tid < 64) s_hist[tid] = 0;
+  if (tid < W) s_hist[tid] = 0;
   if (tid == 0) { s_first = INT_MAX; s_last = -1; s_half = INT_MAX; }
   __syncthreads();
   // every CTA finds the first surviving return itself (normally raw[0]) so start_ori needs no grid-wide step
@@ -153,18 +154,21 @@ __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<C
   if (my_last >= 0) atomicMax(&s_last, my_last);
   if (my_half != INT_MAX) atomicMin(&s_half, my_half);
   __syncthreads();
-  if (tid < 64) hist[blockIdx.x * 64 + tid] = s_hist[tid];
+  if (tid < W) hist[blockIdx.x * W + tid] = s_hist[tid];
   if (tid == 0) {
     if (s_last >= 0) atomicMax(&sc->last_valid, s_last);
     if (s_half != INT_MAX) atomicMin(&sc->half_idx, s_half);
     if (blockIdx.x == 0) { sc->first_valid = first; sc->start_ori = start_ori; }
   }
 }
-template __global__ void k_classify<ALOAM_RING_ELEVATION_DEV>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
-template __global__ void k_classify<ALOAM_RING_FIELD_DEV>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
+template __global__ void k_classify<ALOAM_RING_ELEVATION_DEV, 64>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
+template __global__ void k_classify<ALOAM_RING_FIELD_DEV, 64>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
+template __global__ void k_classify<ALOAM_RING_FIELD_DEV, 128>(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);
 
 // ---------------------------------------------------------------------------------------------------------------
-// one CTA of 1024 threads: thread (r = t>>4, s = t&15) owns slice s of ring r's per-block histogram column
+// one CTA of 1024 threads: thread (r = t / SL, s = t % SL) owns slice s of ring r's per-block histogram column, SL = 1024 / W
+// slices per ring (16 at W = 64, 8 at W = 128)
+template <int W>
 __global__ void __launch_bounds__(1024) k_ring_scan(const __grid_constant__ Batch<RingScanArgs> B, int n_scans) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
@@ -178,23 +182,25 @@ __global__ void __launch_bounds__(1024) k_ring_scan(const __grid_constant__ Batc
   int* __restrict__ scan_end = A.scan_end;
   ScanScalars* __restrict__ sc = A.sc;
   ScanScalars* __restrict__ sc_next = A.sc_next;
-  __shared__ int s_tot[64];
-  __shared__ int s_start[65];
-  const int t = threadIdx.x, r = t >> 4, s = t & 15;
-  const int bps = (nblocks + 15) / 16;
+  constexpr int SL = 1024 / W, LSL = W == 64 ? 4 : 3;
+  static_assert(W == 64 || W == 128, "ring width");
+  __shared__ int s_tot[W];
+  __shared__ int s_start[W + 1];
+  const int t = threadIdx.x, r = t >> LSL, s = t & (SL - 1);
+  const int bps = (nblocks + SL - 1) / SL;
   const int b0 = min(nblocks, s * bps), b1 = min(nblocks, b0 + bps);
   int local = 0;
-  for (int b = b0; b < b1; ++b) local += hist[b * 64 + r];
-  // inclusive scan across the 16 slices (half-warp)
+  for (int b = b0; b < b1; ++b) local += hist[b * W + r];
+  // inclusive scan across the SL slices (a segment of the warp)
   int incl = local;
 #pragma unroll
-  for (int d = 1; d < 16; d <<= 1) {
-    int v = __shfl_up_sync(0xffffffffu, incl, d, 16);
+  for (int d = 1; d < SL; d <<= 1) {
+    int v = __shfl_up_sync(0xffffffffu, incl, d, SL);
     if (s >= d) incl += v;
   }
-  if (s == 15) s_tot[r] = incl;
+  if (s == SL - 1) s_tot[r] = incl;
   __syncthreads();
-  if (t < 32) {  // exclusive scan of 64 ring totals, two per lane
+  if (W == 64 && t < 32) {  // exclusive scan of 64 ring totals, two per lane
     int a = s_tot[2 * t], b = s_tot[2 * t + 1];
     int pair = a + b, inc = pair;
 #pragma unroll
@@ -206,20 +212,35 @@ __global__ void __launch_bounds__(1024) k_ring_scan(const __grid_constant__ Batc
     s_start[2 * t] = ex;
     s_start[2 * t + 1] = ex + a;
     if (t == 31) s_start[64] = inc;
+  } else if (W == 128 && t < 32) {  // exclusive scan of 128 ring totals, four per lane
+    const int a0 = s_tot[4 * t], a1 = s_tot[4 * t + 1], a2 = s_tot[4 * t + 2], a3 = s_tot[4 * t + 3];
+    const int quad = a0 + a1 + a2 + a3;
+    int inc = quad;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      int v = __shfl_up_sync(0xffffffffu, inc, d);
+      if (t >= d) inc += v;
+    }
+    const int ex = inc - quad;
+    s_start[4 * t] = ex;
+    s_start[4 * t + 1] = ex + a0;
+    s_start[4 * t + 2] = ex + a0 + a1;
+    s_start[4 * t + 3] = ex + a0 + a1 + a2;
+    if (t == 31) s_start[W] = inc;
   }
   __syncthreads();
   int running = s_start[r] + (incl - local);
   for (int b = b0; b < b1; ++b) {
-    offsets[b * 64 + r] = running;
-    running += hist[b * 64 + r];
+    offsets[b * W + r] = running;
+    running += hist[b * W + r];
   }
-  if (t <= 64) ring_start[t] = s_start[t];
-  if (t < 64) {  // :249-251
+  if (t <= W) ring_start[t] = s_start[t];
+  if (t < W) {  // :249-251
     scan_start[t] = s_start[t] + 5;
     scan_end[t] = s_start[t + 1] - 6;
   }
   if (t == 0) {
-    sc->n_full = s_start[64];
+    sc->n_full = s_start[W];
     float end_ori = 0.f;
     if (sc->last_valid >= 0) {
       float x, y, z; load_xyz(raw, sc->last_valid, stride, x, y, z);
@@ -229,13 +250,16 @@ __global__ void __launch_bounds__(1024) k_ring_scan(const __grid_constant__ Batc
       else if ((double)(end_ori - start_ori) < kPi) end_ori = (float)((double)end_ori + 2 * kPi);
     }
     sc->end_ori = end_ori;
-    if (A.n_full_out) *A.n_full_out = s_start[64];   // per-scan record of a stream call (0 = nothing survived the filters)
+    if (A.n_full_out) *A.n_full_out = s_start[W];   // per-scan record of a stream call (0 = nothing survived the filters)
     // arm the other parity slot for the next scan
     sc_next->first_valid = INT_MAX; sc_next->last_valid = -1; sc_next->half_idx = INT_MAX; sc_next->n_full = 0;
   }
 }
+template __global__ void k_ring_scan<64>(const __grid_constant__ Batch<RingScanArgs> B, int n_scans);
+template __global__ void k_ring_scan<128>(const __grid_constant__ Batch<RingScanArgs> B, int n_scans);
 
 // ---------------------------------------------------------------------------------------------------------------
+template <int W>
 __global__ void __launch_bounds__(CT) k_scatter(const __grid_constant__ Batch<ScatterArgs> B) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
@@ -247,9 +271,9 @@ __global__ void __launch_bounds__(CT) k_scatter(const __grid_constant__ Batch<Sc
   const ScanScalars* __restrict__ sc = A.sc;
   Pt4* __restrict__ full = A.full;
   if (blockIdx.x * CHUNK >= n) return;
-  __shared__ int s_cnt[ITERS * (CT / 32)][64];  // [slot = it*8 + warp][ring], then exclusive prefix over slots
+  __shared__ int s_cnt[ITERS * (CT / 32)][W];  // [slot = it*8 + warp][ring], then exclusive prefix over slots (16 KB at W = 128)
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
-  for (int k = tid; k < ITERS * (CT / 32) * 64; k += CT) (&s_cnt[0][0])[k] = 0;
+  for (int k = tid; k < ITERS * (CT / 32) * W; k += CT) (&s_cnt[0][0])[k] = 0;
   __syncthreads();
   int ring[ITERS], rank[ITERS];
 #pragma unroll
@@ -262,8 +286,8 @@ __global__ void __launch_bounds__(CT) k_scatter(const __grid_constant__ Batch<Sc
     if (r >= 0 && rank[it] == 0) s_cnt[it * (CT / 32) + w][r] = __popc(grp);
   }
   __syncthreads();
-  if (tid < 64) {
-    int run = offsets[blockIdx.x * 64 + tid];
+  if (tid < W) {
+    int run = offsets[blockIdx.x * W + tid];
 #pragma unroll
     for (int k = 0; k < ITERS * (CT / 32); ++k) { int c = s_cnt[k][tid]; s_cnt[k][tid] = run; run += c; }
   }
@@ -290,6 +314,8 @@ __global__ void __launch_bounds__(CT) k_scatter(const __grid_constant__ Batch<Sc
     full[s_cnt[it * (CT / 32) + w][r] + rank[it]] = p;
   }
 }
+template __global__ void k_scatter<64>(const __grid_constant__ Batch<ScatterArgs> B);
+template __global__ void k_scatter<128>(const __grid_constant__ Batch<ScatterArgs> B);
 
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
@@ -550,7 +576,10 @@ __device__ __forceinline__ void pick_segment(const float* curv, const unsigned c
   __syncwarp();
 }
 
-__device__ long long g_dbg_cycles[65 * 8];   // per-ring phase time stamps (clock64) of the last k_ring_features launch
+// per-ring phase time stamps (clock64) of the last k_ring_features launch: row = ring of lane 0, row 64 = the dummy row of the
+// other lanes.  128 + 1 rows so that lane 0's rings 64..127 of a 128-wide context stay inside the buffer; ring 64 shares the
+// dummy row and features_debug_cycles reads rows 0..63 only.
+__device__ long long g_dbg_cycles[129 * 8];
 
 // dynamic shared memory layout (bytes), maxr = ring capacity of the context (multiple of 32, <= ALOAM_MAX_RING), P = sort width
 // (next power of two >= maxr, >= 1024):  pts 16*maxr | keys 8*P | curv 4*maxr | label maxr | gap 4*(maxr/32+2) | picked same | fb maxr

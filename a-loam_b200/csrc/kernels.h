@@ -8,6 +8,7 @@
 #define ALOAM_ERR_RING_TOO_LARGE_DEV (-7)    // == ALOAM_ERR_RING_TOO_LARGE
 #define ALOAM_RING_ELEVATION_DEV 0           // == ALOAM_RING_ELEVATION
 #define ALOAM_RING_FIELD_DEV 1               // == ALOAM_RING_FIELD
+#define ALOAM_MAX_RINGS_DEV 128              // == ALOAM_MAX_RINGS
 #define ALOAM_LM_THREADS 288
 #define ALOAM_LM_MAX_TRACE 8
 #define ALOAM_N_KERNEL_IDS 32
@@ -22,6 +23,12 @@ namespace aloam {
 #endif
 template <typename T> struct Batch { T a[ALOAM_MAX_BATCH]; };
 
+// ---- ring width W: the ring-indexed kernels (binning, the association index and its search) are templates on W, the number of
+// ring slots their tables hold.  A context picks W once from cfg.n_scans: 64 up to 64 rings, else 128 (aloam_create_wide).  The
+// W = 64 instances are the kernels of a context of aloam_create, unchanged; W = 128 doubles the tables only where it is used.
+inline int ring_width(int n_scans) { return n_scans <= 64 ? 64 : ALOAM_MAX_RINGS_DEV; }
+inline int ring_width_log2(int w) { return w == 64 ? 6 : 7; }
+
 // ---- features.cu
 size_t ring_features_smem_bytes(int max_ring, bool merge);   // merge: the 512-thread kernel (second key buffer)
 void features_debug_cycles(long long* host64x8);   // 65 rows of 8 + 12: per-ring phase stamps, pick-walk stamps of ring 8
@@ -34,10 +41,13 @@ struct RingFeatArgs { const Pt4* full; const int* ring_start; Pt4 *st_sharp, *st
                       float* dbg_curv; int8_t* dbg_label; ScanScalars* sc; };
 struct CompactArgs { const Pt4 *st_sharp, *st_less_sharp, *st_flat, *st_less_flat; const int* st_counts; Pt4 *sharp, *less_sharp, *flat, *less_flat;
                      int* counts; };
-// RingSource: where a return's ring comes from, ALOAM_RING_ELEVATION_DEV or ALOAM_RING_FIELD_DEV (both instances in features.cu)
-template <int RingSource>
+// RingSource: where a return's ring comes from, ALOAM_RING_ELEVATION_DEV or ALOAM_RING_FIELD_DEV; W: the ring width.  Instances
+// in features.cu: <ELEVATION, 64>, <FIELD, 64>, <FIELD, 128> (elevation rings stop at 64)
+template <int RingSource, int W>
 __global__ void k_classify(const __grid_constant__ Batch<ClassifyArgs> B, int n_scans, float thres2);          // grid (blocks, lanes)
+template <int W>
 __global__ void k_ring_scan(const __grid_constant__ Batch<RingScanArgs> B, int n_scans);                       // grid (lanes)
+template <int W>
 __global__ void k_scatter(const __grid_constant__ Batch<ScatterArgs> B);                                       // grid (blocks, lanes)
 __global__ void k_ring_features(const __grid_constant__ Batch<RingFeatArgs> B, int n_scans, float leaf, int max_ring);        // grid (2 * rings, 1), clusters of 2 CTAs x 512 threads
 __global__ void k_ring_features_batch(const __grid_constant__ Batch<RingFeatArgs> B, int n_scans, float leaf, int max_ring);  // same, 256 threads (batches)
@@ -48,28 +58,30 @@ __global__ void k_compact(const __grid_constant__ Batch<CompactArgs> B, int n_sc
 #define ALOAM_NB 128   // azimuth buckets (2.8 deg)
 // "ring" below is int(intensity), the closestPointScanID of laserOdometry.cpp:308,398 -- the physical ring or the one below it
 // (relTime in (-2, 6], see DESIGN.md section 3), so it may descend by one between consecutive points of a cloud.
+// W = the context's ring width (64 or 128), log2 W = 6 or 7 bits of ring in the packed word
 struct RabIndex {
-  int* cnt;         // [NB*64] scratch counters (left zeroed by k_rab_scan)
-  int* start;       // [NB*64 + 1] first slot of cell (bucket*64 + ring) in gpts
+  int* cnt;         // [NB*W] scratch counters (left zeroed by k_rab_scan)
+  int* start;       // [NB*W + 1] first slot of cell (bucket*W + ring) in gpts
   int* cell_of;     // [capacity] cell of point i
   int* rank_of;     // [capacity] rank of point i inside its cell
-  float4* gpts;     // [capacity] cell-contiguous copy: x, y, z, bits(original index << 6 | ring)
-  int* first_of;    // [64] scratch: smallest index of each ring (left above any index by k_rab_scan)
-  int* last_of;     // [64] scratch: largest index of each ring (left -1 by k_rab_scan)
-  int* fwd_end;     // [65] fwd_end[r]   = first index with ring >= r (n if none): the forward loops' break index
-  int* bwd_begin;   // [65] bwd_begin[r] = 1 + last index with ring < r (0 if none): one past the backward loops' break index
+  float4* gpts;     // [capacity] cell-contiguous copy: x, y, z, bits(original index << log2 W | ring)
+  int* first_of;    // [W] scratch: smallest index of each ring (left above any index by k_rab_scan)
+  int* last_of;     // [W] scratch: largest index of each ring (left -1 by k_rab_scan)
+  int* fwd_end;     // [W + 1] fwd_end[r]   = first index with ring >= r (n if none): the forward loops' break index
+  int* bwd_begin;   // [W + 1] bwd_begin[r] = 1 + last index with ring < r (0 if none): one past the backward loops' break index
 };
-constexpr int kRabBreakInts = 64 + 64 + 65 + 65;   // first_of, last_of, fwd_end, bwd_begin in one allocation
+constexpr int rab_break_ints(int w) { return w + w + (w + 1) + (w + 1); }   // first_of, last_of, fwd_end, bwd_begin in one allocation
 struct LastCloud {
   const Pt4* pts;   // the cloud in its original order
   const int* n;     // device scalar: number of points
   RabIndex index;
 };
-__global__ void k_ring_offsets(const Pt4* pts, int n, const int* fwd_end, int* err);
+// every kernel that reads or writes the index is a template on W, with instances for 64 and 128 in odometry.cu
+template <int W> __global__ void k_ring_offsets(const Pt4* __restrict__ pts, int n, const int* __restrict__ fwd_end, int* __restrict__ err);
 struct RabArgs { RabIndex a; const Pt4* pa; const int* na; RabIndex b; const Pt4* pb; const int* nb; };
-__global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B);   // grid (blocks, 2 clouds, lanes)
-__global__ void k_rab_scan(const __grid_constant__ Batch<RabArgs> B);    // grid (2 clouds, lanes)
-__global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B);    // grid (blocks, 2 clouds, lanes)
+template <int W> __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B);   // grid (blocks, 2 clouds, lanes)
+template <int W> __global__ void k_rab_scan(const __grid_constant__ Batch<RabArgs> B);    // grid (2 clouds, lanes)
+template <int W> __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B);    // grid (blocks, 2 clouds, lanes)
 
 // one residual block, ready for the LM kernel (doubles; built once per association like the Ceres cost functions)
 struct __align__(8) BlockRec {
@@ -86,8 +98,8 @@ struct OdomParams { double dist_sq_thresh; double nearby_scan; int distortion; /
 __global__ void k_transform_to_end(const Pt4* in, int n, const double* pose7, int distortion, Pt4* out);
 struct AssocArgs { const Pt4* sharp; const Pt4* flat; const int* feat_counts /*[4]*/; LastCloud corner, surf; const double* pose7;
                    BlockRec* blocks; int* corr /*[(n_sharp+n_flat)][4] a,b,c,valid ; may be null*/; };
-__global__ void k_odom_assoc(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp);   // grid (query groups, lanes)
-__global__ void k_knn_last(LastCloud cloud, const Pt4* queries, int nq, int* idx, float* sqd);
+template <int W> __global__ void k_odom_assoc(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp);   // grid (query groups, lanes)
+template <int W> __global__ void k_knn_last(LastCloud cloud, const Pt4* __restrict__ queries, int nq, int* __restrict__ idx, float* __restrict__ sqd);
 
 // ---- mapping.cu
 // hash grid over a map cloud = what replaces the kd-tree builds of laserMapping.cpp:558-559

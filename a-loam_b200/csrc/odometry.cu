@@ -2,8 +2,9 @@
 // :299-483 (the two association loops) and :567-568 (the kd-tree builds).
 //
 // Index = a dense (azimuth bucket x ring) table per "last" cloud instead of a kd-tree (k_rab_* kernels): a counting
-//   sort of the cloud into ALOAM_NB x 64 cells, bucket-major, so that "all rings of an azimuth bucket" and "rings
-//   rc-2..rc+2 of an azimuth bucket" are both contiguous slices of one float4 array (x, y, z, index<<6 | ring).
+//   sort of the cloud into ALOAM_NB x W cells, bucket-major (W = the context's ring width, 64 or 128: every kernel here is a
+//   template on it), so that "all rings of an azimuth bucket" and "rings rc-2..rc+2 of an azimuth bucket" are both contiguous
+//   slices of one float4 array (x, y, z, index << log2 W | ring).
 //   The order of points inside a cell depends on atomic timing, but every search below compares candidates on
 //   (distance, original index / visiting rank), so results are a pure function of the input.
 // Search = ONE WARP PER QUERY, exact.  The clouds live in the sensor frame of the last scan, so a point whose
@@ -22,7 +23,7 @@
 // section 3), so a cloud's int(intensity) is the physical ring or the one below and need not ascend: the invariant the search
 // relies on is only  int_i >= max_{j<i} int_j - 1.  Under it (and NEARBY_SCAN >= 1) the loops' break indices do not depend on
 // the closest point.  With up = the largest u with rc + u <= rc + NEARBY_SCAN and dn = the largest u with rc - u >=
-// rc - NEARBY_SCAN (both in double, as the reference's int-vs-double tests; at most 64) the forward break is the first index
+// rc - NEARBY_SCAN (both in double, as the reference's int-vs-double tests; at most W) the forward break is the first index
 // with int >= rc+up+1 and the backward break the last with int <= rc-dn-1, every candidate has int in rc-dn..rc+up, and the
 // class and visiting rank of a candidate follow from (index vs closest, int vs rc) alone.
 #include <climits>
@@ -34,12 +35,15 @@ namespace aloam {
 
 // validates a cloud handed in through the C ABI after its index is built: every int(intensity) is a legal ring and no
 // earlier point has a ring two or more above (fwd_end[r + 2] is the first index with ring >= r + 2)
+template <int W>
 __global__ void k_ring_offsets(const Pt4* __restrict__ pts, int n, const int* __restrict__ fwd_end, int* __restrict__ err) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int r = (int)pts[i].i;  // int(intensity) = scan line (laserOdometry.cpp:308,398)
-  if (r < 0 || r > 63 || fwd_end[min(r + 2, 64)] < i) atomicExch(err, 1);
+  if (r < 0 || r > W - 1 || fwd_end[min(r + 2, W)] < i) atomicExch(err, 1);
 }
+template __global__ void k_ring_offsets<64>(const Pt4* __restrict__ pts, int n, const int* __restrict__ fwd_end, int* __restrict__ err);
+template __global__ void k_ring_offsets<128>(const Pt4* __restrict__ pts, int n, const int* __restrict__ fwd_end, int* __restrict__ err);
 
 // ---------------------------------------------------------------------------------------------------------------
 // index build: counting sort of the cloud into (azimuth bucket, ring) cells, bucket-major
@@ -53,7 +57,11 @@ __device__ __forceinline__ int bucket_of(float x, float y) {
 }
 }  // namespace
 
+// log2 of the ring width: the ring bits of a packed word
+template <int W> struct RingBits { static constexpr int value = W == 64 ? 6 : 7; static_assert(W == 64 || W == 128, "ring width"); };
+
 // blockIdx.y selects the cloud (0 = a, 1 = b)
+template <int W>
 __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B) {
   pdl_launch_dependents();   // the next kernel of the stream may become resident (it blocks in pdl_wait())
   const RabArgs& A = B.a[blockIdx.z];
@@ -63,8 +71,8 @@ __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const Pt4 p = pts[i];
-  const int ring = min(max((int)p.i, 0), 63);
-  const int cell = bucket_of(p.x, p.y) * 64 + ring;
+  const int ring = min(max((int)p.i, 0), W - 1);
+  const int cell = bucket_of(p.x, p.y) * W + ring;
   g.cell_of[i] = cell;
   g.rank_of[i] = atomicAdd(&g.cnt[cell], 1);
   // first / last index of each ring: the lanes of a warp hold consecutive indices, so the lowest / highest lane of a ring's
@@ -74,18 +82,46 @@ __global__ void k_rab_count(const __grid_constant__ Batch<RabArgs> B) {
   if (lane == (unsigned)(__ffs(grp) - 1)) atomicMin(&g.first_of[ring], i);
   if (lane == 31u - __clz(grp)) atomicMax(&g.last_of[ring], i);
 }
+template __global__ void k_rab_count<64>(const __grid_constant__ Batch<RabArgs> B);
+template __global__ void k_rab_count<128>(const __grid_constant__ Batch<RabArgs> B);
 
-// one CTA per cloud: exclusive scan of the ALOAM_NB*64 cell counts -> start[], the break tables, and reset the scratch for
+// one CTA per cloud: exclusive scan of the ALOAM_NB*W cell counts -> start[], the break tables, and reset the scratch for
 // the next build
+template <int W>
 __global__ void __launch_bounds__(1024) k_rab_scan(const __grid_constant__ Batch<RabArgs> B) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
   const RabIndex& g = blockIdx.x == 0 ? B.a[blockIdx.y].a : B.a[blockIdx.y].b;
-  constexpr int NC = ALOAM_NB * 64, PER = NC / 1024;
+  constexpr int NC = ALOAM_NB * W, PER = NC / 1024;
   __shared__ int s_w[32];
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  // break tables, two ring entries per lane: warp 0 takes the suffix minima of first_of, warp 1 the prefix maxima of last_of
-  if (w == 0) {
+  // break tables, W / 32 ring entries per lane: warp 0 takes the suffix minima of first_of, warp 1 the prefix maxima of last_of
+  if (W == 128) {   // four entries per lane, entry 32 k + lane in slot k; the carry runs across the slots
+    if (w == 0) {
+      const int n = blockIdx.x == 0 ? *B.a[blockIdx.y].na : *B.a[blockIdx.y].nb;
+      int carry = n;   // min over the slots above, and n
+#pragma unroll
+      for (int k = W / 32 - 1; k >= 0; --k) {
+        int v = g.first_of[32 * k + lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_down_sync(0xffffffffu, v, d); if (lane + d < 32) v = min(v, u); }
+        g.fwd_end[32 * k + lane] = min(v, carry);
+        carry = min(carry, __shfl_sync(0xffffffffu, v, 0));
+      }
+      if (lane == 0) g.fwd_end[W] = n;
+    } else if (w == 1) {
+      int carry = -1;   // max over the slots below
+#pragma unroll
+      for (int k = 0; k < W / 32; ++k) {
+        int v = g.last_of[32 * k + lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v = max(v, u); }
+        g.bwd_begin[1 + 32 * k + lane] = max(v, carry) + 1;
+        carry = max(carry, __shfl_sync(0xffffffffu, v, 31));
+      }
+      if (lane == 0) g.bwd_begin[0] = 0;
+    }
+  } else if (w == 0) {   // W = 64: two entries per lane
     const int n = blockIdx.x == 0 ? *B.a[blockIdx.y].na : *B.a[blockIdx.y].nb;
     int lo = g.first_of[lane], hi = g.first_of[32 + lane];
 #pragma unroll
@@ -123,13 +159,16 @@ __global__ void __launch_bounds__(1024) k_rab_scan(const __grid_constant__ Batch
     s_w[lane] = inc - x;
   }
   __syncthreads();
-  if (t < 64) { g.first_of[t] = INT_MAX; g.last_of[t] = -1; }   // every reader of the scratch is past the barriers above
+  if (t < W) { g.first_of[t] = INT_MAX; g.last_of[t] = -1; }   // every reader of the scratch is past the barriers above
   int run = s_w[w] + incl - sum;
 #pragma unroll
   for (int k = 0; k < PER; ++k) { g.start[t * PER + k] = run; run += v[k]; }
   if (t == 1023) g.start[NC] = run;
 }
+template __global__ void k_rab_scan<64>(const __grid_constant__ Batch<RabArgs> B);
+template __global__ void k_rab_scan<128>(const __grid_constant__ Batch<RabArgs> B);
 
+template <int W>
 __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B) {
   pdl_launch_dependents();
   pdl_wait();   // launched with a programmatic dependency on the previous kernel of the stream
@@ -142,8 +181,11 @@ __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B) {
   const Pt4 p = pts[i];
   const int cell = g.cell_of[i];
   // index-major key: comparing keys compares indices, the reference's tie rule (the ring need not ascend with the index)
-  g.gpts[g.start[cell] + g.rank_of[i]] = make_float4(p.x, p.y, p.z, __int_as_float((i << 6) | (cell & 63)));
+  // (i < 2^24 at W = 128: aloam_create_wide bounds max_points, so the word stays non-negative)
+  g.gpts[g.start[cell] + g.rank_of[i]] = make_float4(p.x, p.y, p.z, __int_as_float((i << RingBits<W>::value) | (cell & (W - 1))));
 }
+template __global__ void k_rab_fill<64>(const __grid_constant__ Batch<RabArgs> B);
+template __global__ void k_rab_fill<128>(const __grid_constant__ Batch<RabArgs> B);
 
 // ---------------------------------------------------------------------------------------------------------------
 // search
@@ -175,26 +217,27 @@ __device__ __forceinline__ void visit_span(const float4* __restrict__ gpts, int 
 // whose first interval was not enough (2 % of the queries).  (A variant that doubles the interval per step -- one
 // delimiter round per step instead of two per bucket -- was tried: it shortens the rare far sweeps but its extra
 // bookkeeping on the common path made the average launch slower; bucket-by-bucket growth stays.)
-template <typename F>
+template <int W, typename F>
 __device__ __forceinline__ void visit_ring_step(const RabIndex& g, int bq, int k, int r_lo, int r_hi, F&& f) {
   const int b0 = (bq - k + ALOAM_NB) % ALOAM_NB, b1 = (bq + k) % ALOAM_NB;
 #pragma unroll 1
   for (int side = 0; side < 2; ++side) {
     if (side && b1 == b0) break;
     const int b = side ? b1 : b0;
-    visit_span<4>(g.gpts, g.start[b * 64 + r_lo], g.start[b * 64 + r_hi + 1], f);
+    visit_span<4>(g.gpts, g.start[b * W + r_lo], g.start[b * W + r_hi + 1], f);
   }
 }
 
 // All rings of the azimuth buckets lo..hi (lo <= hi, indices may run past either end of the circle) are at most two
 // contiguous slices of gpts: [a0, a1) and [b0, b1).  Their four delimiters are fetched in ONE round.
 struct Spans2 { int a0, a1, b0, b1; };
+template <int W>
 __device__ __forceinline__ Spans2 bucket_interval(const RabIndex& g, int lo, int hi) {
   int c0, c1, c2 = 0, c3 = 0;
-  if (hi - lo + 1 >= ALOAM_NB) { c0 = 0; c1 = ALOAM_NB * 64; }
-  else if (lo < 0) { c0 = (lo + ALOAM_NB) * 64; c1 = ALOAM_NB * 64; c3 = (hi + 1) * 64; }
-  else if (hi >= ALOAM_NB) { c0 = lo * 64; c1 = ALOAM_NB * 64; c3 = (hi - ALOAM_NB + 1) * 64; }
-  else { c0 = lo * 64; c1 = (hi + 1) * 64; }
+  if (hi - lo + 1 >= ALOAM_NB) { c0 = 0; c1 = ALOAM_NB * W; }
+  else if (lo < 0) { c0 = (lo + ALOAM_NB) * W; c1 = ALOAM_NB * W; c3 = (hi + 1) * W; }
+  else if (hi >= ALOAM_NB) { c0 = lo * W; c1 = ALOAM_NB * W; c3 = (hi - ALOAM_NB + 1) * W; }
+  else { c0 = lo * W; c1 = (hi + 1) * W; }
   const int lane = (int)lane_id();
   const int v = g.start[lane == 0 ? c0 : lane == 1 ? c1 : lane == 2 ? c2 : c3];
   Spans2 s;
@@ -206,14 +249,14 @@ __device__ __forceinline__ Spans2 bucket_interval(const RabIndex& g, int lo, int
 // Ring slice [r_lo, r_hi] of each of the buckets bq-k..bq+k (k <= kMaxK0): 2k+1 short slices.  One round for all the
 // delimiters, one round for the first 32 points of every slice, then whatever is left of slices longer than 32.
 constexpr int kMaxK0 = 3;
-template <typename F>
+template <int W, typename F>
 __device__ __forceinline__ void visit_ring_slices(const RabIndex& g, int bq, int k, int r_lo, int r_hi, F&& f) {
   const int lane = (int)lane_id();
   const int nb = 2 * k + 1;
   int v = 0;
   if (lane < 2 * nb) {
     const int b = (bq - k + (lane >> 1) + ALOAM_NB) % ALOAM_NB;
-    v = g.start[b * 64 + ((lane & 1) ? r_hi + 1 : r_lo)];
+    v = g.start[b * W + ((lane & 1) ? r_hi + 1 : r_lo)];
   }
   float4 p[2 * kMaxK0 + 1];
   unsigned valid = 0, longer = 0;
@@ -280,8 +323,9 @@ __device__ __forceinline__ void store_none(BlockRec* b, int* corr) {
 
 constexpr int kBig = 1 << 25;       // separates forward ranks [0, 2^24) from backward ranks
 
-// exact nearest neighbour of q with d2 < limit (strict); returns its packed word (index << 6 | ring) or -1, d2 in out_d,
+// exact nearest neighbour of q with d2 < limit (strict); returns its packed word (index << log2 W | ring) or -1, d2 in out_d,
 // the half-width of the bucket interval it had to read in k_out.  Ties -> smaller index (packed order == index order).
+template <int W>
 __device__ __forceinline__ int rab_nearest(const RabIndex& g, float qx, float qy, float qz, float limit, float& out_d, int& k_out) {
   const int bq = bucket_of(qx, qy);
   const float rho = sqrtf(qx * qx + qy * qy);
@@ -292,7 +336,7 @@ __device__ __forceinline__ int rab_nearest(const RabIndex& g, float qx, float qy
     if (d2 < best_d || (d2 == best_d && best_i != INT_MAX && packed < best_i)) { best_d = d2; best_i = packed; }
   };
   int k = first_halfwidth(rho);
-  const Spans2 sp = bucket_interval(g, bq - k, bq + k);
+  const Spans2 sp = bucket_interval<W>(g, bq - k, bq + k);
 #pragma unroll 1
   for (int side = 0; side < 2; ++side) visit_span<12>(g.gpts, side ? sp.b0 : sp.a0, side ? sp.b1 : sp.a1, f);
 #pragma unroll 1
@@ -302,7 +346,7 @@ __device__ __forceinline__ int rab_nearest(const RabIndex& g, float qx, float qy
     const float safe2 = safe_radius_sq(rho, k);
     if ((wi != INT_MAX && wd < safe2) || safe2 >= limit || 2 * (k + 1) > ALOAM_NB) break;
     ++k;
-    visit_ring_step(g, bq, k, 0, 63, f);
+    visit_ring_step<W>(g, bq, k, 0, W - 1, f);
   }
   k_out = k;
   out_d = wd;
@@ -311,7 +355,11 @@ __device__ __forceinline__ int rab_nearest(const RabIndex& g, float qx, float qy
 
 }  // namespace
 
-__global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp) {
+// W = 128 asks for one CTA per SM at least (minBlocks 1): without it ptxas keeps the 64-wide instance's 80 registers and spills
+// 104 bytes; with it the instance takes 95 registers and no spill.  (minBlocks 0 leaves the 64-wide instance as it was.)
+template <int W>
+__global__ void __launch_bounds__(256, W == 128 ? 1 : 0) k_odom_assoc(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp) {
+  constexpr int RB = RingBits<W>::value;
   pdl_launch_dependents();   // the LM solve that follows may become resident now; it blocks in its own pdl_wait()
   pdl_wait();                // the preceding LM solve (pose7 producer, blocks consumer) has completed
   const AssocArgs& A = B.a[blockIdx.y];   // blockIdx.y = trajectory of the batch
@@ -351,19 +399,19 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   // nearest neighbour (kdtree*Last->nearestKSearch(pointSel, 1, ...), :302,390) then `< DISTANCE_SQ_THRESHOLD`
   float d1;
   int k_nn;
-  const int packed1 = rab_nearest(g, qx, qy, qz, thr, d1, k_nn);
+  const int packed1 = rab_nearest<W>(g, qx, qy, qz, thr, d1, k_nn);
   if (packed1 < 0 || !((double)d1 < prm.dist_sq_thresh)) { if (lane == 0) store_none(out, co); return; }
-  const int closest = packed1 >> 6;
-  const int rc = packed1 & 63;   // closestPointScanID = int(intensity) of the closest point (k_rab_fill packs it)
+  const int closest = packed1 >> RB;
+  const int rc = packed1 & (W - 1);   // closestPointScanID = int(intensity) of the closest point (k_rab_fill packs it)
   // rings rc-dn .. rc+up survive the break tests `int > rc + NEARBY_SCAN` / `int < rc - NEARBY_SCAN` (:319,345,405,433),
   // evaluated in double as the reference does.  The two sides are counted separately: rc + N and rc - N need not round
-  // symmetrically (N = 3 - 2^-48 at rc = 32 keeps ring 35 but not ring 29).  64 rings cover 0..63 from any rc, so the
+  // symmetrically (N = 3 - 2^-48 at rc = 32 keeps ring 35 but not ring 29).  W rings cover 0..W-1 from any rc, so the
   // bound makes a huge or infinite NEARBY_SCAN mean "never break", as in the reference.
-  int up = 0; while (up < 64 && (double)(rc + up + 1) <= (double)rc + prm.nearby_scan) ++up;
-  int dn = 0; while (dn < 64 && (double)(rc - dn - 1) >= (double)rc - prm.nearby_scan) ++dn;
+  int up = 0; while (up < W && (double)(rc + up + 1) <= (double)rc + prm.nearby_scan) ++up;
+  int dn = 0; while (dn < W && (double)(rc - dn - 1) >= (double)rc - prm.nearby_scan) ++dn;
   // the loops' ranges: forward (closest, fwd_end), backward [bwd_begin, closest).  Issued together with the closest point;
   // aloam_create guarantees NEARBY_SCAN >= 1, hence up, dn >= 1, which puts both break indices on the right side of `closest`.
-  const int fwd_end = g.fwd_end[min(rc + up + 1, 64)], bwd_begin = g.bwd_begin[max(rc - dn, 0)];
+  const int fwd_end = g.fwd_end[min(rc + up + 1, W)], bwd_begin = g.bwd_begin[max(rc - dn, 0)];
   const Pt4 pc = L.pts[closest];   // issued now, consumed after the second search
 
   // second search: class 2 / class 3 minima in the reference's visiting order (forward ascending, then backward descending).
@@ -374,9 +422,9 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
   {
     const int bq = bucket_of(qx, qy);
     const float rho = sqrtf(qx * qx + qy * qy);
-    const int r_lo = max(rc - dn, 0), r_hi = min(rc + up, 63);
+    const int r_lo = max(rc - dn, 0), r_hi = min(rc + up, W - 1);
     auto f = [&](float x, float y, float z, int packed) {
-      const int idx = packed >> 6, ring = packed & 63;
+      const int idx = packed >> RB, ring = packed & (W - 1);
       if (idx == closest || idx >= fwd_end || idx < bwd_begin) return;
       const bool fwd = idx > closest;
       const bool same = fwd ? ring <= rc : ring >= rc;   // corner: skipped ; surf: class 2
@@ -387,7 +435,7 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
       else { if (d2 < b3 || (d2 == b3 && r3 != INT_MAX && rank < r3)) { b3 = d2; r3 = rank; } }
     };
     int k = min(k_nn, kMaxK0);
-    visit_ring_slices(g, bq, k, r_lo, r_hi, f);
+    visit_ring_slices<W>(g, bq, k, r_lo, r_hi, f);
 #pragma unroll 1
     for (;;) {
       w2 = r2 == INT_MAX ? FLT_MAX : b2; k2 = r2; warp_argmin(w2, k2);
@@ -399,7 +447,7 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
       }
       if (done || safe2 >= thr || 2 * (k + 1) > ALOAM_NB) break;
       ++k;
-      visit_ring_step(g, bq, k, r_lo, r_hi, f);
+      visit_ring_step<W>(g, bq, k, r_lo, r_hi, f);
     }
   }
   // rank -> index
@@ -440,6 +488,8 @@ __global__ void __launch_bounds__(256) k_odom_assoc(const __grid_constant__ Batc
     }
   }
 }
+template __global__ void k_odom_assoc<64>(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp);
+template __global__ void k_odom_assoc<128>(const __grid_constant__ Batch<AssocArgs> B, OdomParams prm, int max_sharp);
 
 // laserOdometry.cpp:133-148 TransformToEnd: undistort to the sweep start, then carry to the sweep end; the integer part of the
 // intensity is kept (dead code in the reference -- its call sites are under `if (0)`, :533-552 -- offered through aloam_transform_to_end)
@@ -467,6 +517,7 @@ __global__ void k_transform_to_end(const Pt4* __restrict__ in, int n, const doub
 }
 
 // exact 1-NN of arbitrary queries against a "last" cloud (aloam_knn, which = 0/1): no distance limit
+template <int W>
 __global__ void __launch_bounds__(256) k_knn_last(LastCloud cloud, const Pt4* __restrict__ queries, int nq,
                                                   int* __restrict__ idx, float* __restrict__ sqd) {
   const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -474,9 +525,11 @@ __global__ void __launch_bounds__(256) k_knn_last(LastCloud cloud, const Pt4* __
   const Pt4 q = queries[wid];
   float d;
   int k_used;
-  const int packed = rab_nearest(cloud.index, q.x, q.y, q.z, FLT_MAX, d, k_used);
-  const int j = packed < 0 ? -1 : (packed >> 6);
+  const int packed = rab_nearest<W>(cloud.index, q.x, q.y, q.z, FLT_MAX, d, k_used);
+  const int j = packed < 0 ? -1 : (packed >> RingBits<W>::value);
   if (lane_id() == 0) { idx[wid] = j; sqd[wid] = j < 0 ? __int_as_float(0x7f800000) : d; }
 }
+template __global__ void k_knn_last<64>(LastCloud cloud, const Pt4* __restrict__ queries, int nq, int* __restrict__ idx, float* __restrict__ sqd);
+template __global__ void k_knn_last<128>(LastCloud cloud, const Pt4* __restrict__ queries, int nq, int* __restrict__ idx, float* __restrict__ sqd);
 
 }  // namespace aloam

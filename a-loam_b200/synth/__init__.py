@@ -32,7 +32,21 @@ RING_SENSORS = {
     "R1": ((-4.0,), 1800),
     "R2": ((-8.0, 2.0), 1800),
 }
-RING_RANGES = (0.3, 0.2, 0.4)   # minimum_range, line_res, plane_res of every RING_SENSORS sensor
+# Driver-ring sensors of more than 64 beams, for contexts of aloam_create_wide (Aloam(..., wide=True)), in the layout of
+# RING_SENSORS.  Shaped like:
+#   OS128  an Ouster OS1-128: uniform +22.5 .. -22.5 deg, ring 0 the highest beam
+#   V128   a Velodyne VLS-128: non-uniform -25 .. +15 deg, 1.25 deg apart below -5 deg, 10/95 deg apart between -5 and +5,
+#          0.625 deg apart above; ring 0 the lowest beam
+#   L96    96 uniform beams -25 .. +15 deg (a width that is not a power of two), ring 0 the lowest
+#   E65    65 uniform beams +16 .. -16 deg, the narrowest table that needs the wide entry point, ring 0 the highest
+WIDE_RING_SENSORS = {
+    "OS128": (tuple(22.5 - k * 45.0 / 127 for k in range(128)), 1024),
+    "V128": (tuple(-25.0 + k * 1.25 for k in range(16)) + tuple(-5.0 + k * 10.0 / 95 for k in range(96)) +
+             tuple(5.625 + k * 0.625 for k in range(16)), 1800),
+    "L96": (tuple(-25.0 + k * 40.0 / 95 for k in range(96)), 1024),
+    "E65": (tuple(16.0 - k * 0.5 for k in range(65)), 1024),
+}
+RING_RANGES = (0.3, 0.2, 0.4)   # minimum_range, line_res, plane_res of every RING_SENSORS / WIDE_RING_SENSORS sensor
 
 
 def build(force=False):
@@ -155,11 +169,12 @@ def scan_beams(sensor, index, elevations_deg, z_offsets_m=None, cut=None, covera
 
 def scan_rings(sensor, index, reverse=False, cut=None, coverage=1.0, laser_major=False, ccw=False, seed=BASE_SEED, n_az=None,
                noise=0.02, max_range=120.0):
-    """Raw scan `index` of the trajectory from RING_SENSORS[sensor], with its driver ring: (n, 4) float32 x, y, z, ring.  The
+    """Raw scan `index` of the trajectory from RING_SENSORS[sensor] (or WIDE_RING_SENSORS[sensor]), with its driver ring: (n, 4)
+    float32 x, y, z, ring.  The
     ring of laser b is b, or n_beams - 1 - b with reverse (the other elevation order).  cut, coverage, laser_major and ccw as
     for scan_seam().  Raises SeamTooClose when a return that survives minimum_range (RING_RANGES) sits within 1e-5 rad of an
     azimuth threshold of the sweep walk: every such return takes part in it."""
-    elev, az = RING_SENSORS[sensor]
+    elev, az = RING_SENSORS[sensor] if sensor in RING_SENSORS else WIDE_RING_SENSORS[sensor]
     if n_az is not None:
         az = n_az
     el = np.ascontiguousarray(elev, np.float64)

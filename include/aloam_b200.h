@@ -31,13 +31,15 @@ extern "C" {
 #define ALOAM_OK 0
 #define ALOAM_ERR_INVALID_ARG (-1)
 #define ALOAM_ERR_UNSUPPORTED_SCANS (-2) /* scanRegistration.cpp:472-476: only 16, 32 or 64 scan lines under
-                                            ALOAM_RING_ELEVATION; 1..64 under ALOAM_RING_FIELD */
+                                            ALOAM_RING_ELEVATION; 1..64 under ALOAM_RING_FIELD (1..ALOAM_MAX_RINGS
+                                            through aloam_create_wide) */
 #define ALOAM_ERR_EMPTY_CLOUD (-3)       /* no point survives the NaN / minimum-range filter */
 #define ALOAM_ERR_CAPACITY (-4)          /* more points than the ctx was created for */
 #define ALOAM_ERR_CUDA (-5)
 #define ALOAM_ERR_NO_DEVICE (-6)
 #define ALOAM_ERR_RING_TOO_LARGE (-7)    /* a single ring holds more than ALOAM_MAX_RING_POINTS returns */
-#define ALOAM_ERR_NOT_RING_MAJOR (-8)    /* "last" cloud with an int(intensity) outside 0..63 or two or more below an earlier
+#define ALOAM_ERR_NOT_RING_MAJOR (-8)    /* "last" cloud with an int(intensity) outside 0..63 (0..127 in a context of
+                                            aloam_create_wide with n_scans > 64) or two or more below an earlier
                                             point's: every scanRegistration output has int_i >= max_{j<i} int_j - 1, and the
                                             association's break tables rely on it (laserOdometry.cpp:310-361,400-455) */
 #define ALOAM_ERR_STATE (-9)             /* call sequence error, e.g. register before set_last */
@@ -46,6 +48,7 @@ extern "C" {
                                             changes results (aloam_lane_restore, aloam_snapshot_check) */
 
 #define ALOAM_MAX_RING_POINTS 4096
+#define ALOAM_MAX_RINGS 128   /* the most rings a context takes: through aloam_create_wide, ALOAM_RING_FIELD only */
 #define ALOAM_MAX_BATCH 16
 #define ALOAM_MAX_CUBE_POINTS 262144   /* 2^18: the most points one map cube holds with cube growth on (aloam_set_cube_growth) */
 
@@ -81,7 +84,9 @@ typedef struct aloam_config {
                             aloam_scan_stream_lanes; 1..ALOAM_MAX_BATCH, default 1 */
   int distortion;        /* 0 (reference build) or 1: #define DISTORTION of laserOdometry.cpp:59 -- per-point interpolation ratio
                             s = (intensity - int(intensity)) / SCAN_PERIOD in TransformToStart (:113-118) and in the
-                            residual blocks (:376-379, 470-473; slerp inside the functors, lidarFactor.hpp:27-33) */
+                            residual blocks (:376-379, 470-473; slerp inside the functors, lidarFactor.hpp:27-33).
+                            intensity = ring + 0.1 relTime is the reference's float: on rings 64..127 its fraction, and so s, is
+                            quantised at 2^-17 instead of 2^-18, as scanRegistration.cpp's own float is */
   int max_ring_points;   /* capacity of one scan ring, multiple of 32, <= ALOAM_MAX_RING_POINTS (default).  Smaller rings take
                             less shared memory per ring CTA, so more of them are resident per SM (batched streams) */
   int mapping_skip_frame; /* mapping_skip_frame laserOdometry.cpp:191, launch/...:6 -- the mapped stream calls map every k-th scan
@@ -96,7 +101,8 @@ typedef struct aloam_config {
  *   ALOAM_RING_ELEVATION  the reference's elevation formula of the configured Velodyne (scanRegistration.cpp:166-205);
  *                         n_scans must be 16, 32 or 64.
  *   ALOAM_RING_FIELD      the sensor driver's ring: float 3 of every raw point (the 4th float, at stride 4 and 8 alike; the
- *                         reference never reads that slot of a raw scan).  n_scans may be 1..64.  After the NaN and
+ *                         reference never reads that slot of a raw scan).  n_scans may be 1..64, 1..128 through
+ *                         aloam_create_wide.  After the NaN and
  *                         minimum-range filters a return's ring is w = float 3 when w is finite, integral and 0 <= w < n_scans;
  *                         any other w drops the return as an out-of-range formula id does (it does not count in the sweep walk
  *                         either, scanRegistration.cpp:174-175).  Everything after the ring binning is unchanged: the azimuth
@@ -128,6 +134,22 @@ typedef struct aloam_stats {
 
 void aloam_default_config(aloam_config* cfg, int n_scans);
 int aloam_create(const aloam_config* cfg, aloam_ctx** out);
+/* aloam_create_wide: everything aloam_create accepts, giving the same context, and also ring_source = ALOAM_RING_FIELD with
+ * n_scans 65..ALOAM_MAX_RINGS (128-beam lidars: Ouster OS1/OS2-128, Velodyne VLS-128, Hesai Pandar128, RoboSense Ruby).
+ * Elevation rings stay 16 / 32 / 64 (ALOAM_ERR_UNSUPPORTED_SCANS, as 0 or 129 driver rings), a ring source other than 0 or 1
+ * stays ALOAM_ERR_INVALID_ARG.  With n_scans > 64:
+ *   - the context's ring-indexed tables are 128 wide: an int(intensity) of 0..127 is a ring of aloam_odometry_set_last's
+ *     clouds (ALOAM_ERR_NOT_RING_MAJOR above that);
+ *   - cfg.max_points > 2^24 is ALOAM_ERR_INVALID_ARG: the association index packs a point's index into 24 bits;
+ *   - every lane allocates 64 x (32 x (156 + max_ring_points) + 8 x (6 + ceil(max_points / 1024)) + 12 x 1040) bytes more
+ *     than at 64 rings (64 more rings of: two staging sets of 12 + 120 + 24 + max_ring_points points, the ring-binning
+ *     tables, and the twelve association indexes of 128 buckets): 9.7 MB per lane at max_ring_points = 4096 and
+ *     max_points = 400000, 5.5 MB at 2048 (arithmetic, not a measurement);
+ *   - 12 sharp and 24 flat query slots per ring: the fused paths' association covers 1536 + 3072 queries.
+ * Snapshots of a 128-ring context restore only into a context with the same n_scans (ALOAM_ERR_SNAPSHOT elsewhere, every
+ * context of aloam_create included).  Prior maps, relocalisation, recovery, cube growth, the registered sink and per-row
+ * records do not depend on rings and work unchanged.  The recommended max_ring_points for a 128-beam sensor is in README.md. */
+int aloam_create_wide(const aloam_config* cfg, aloam_ctx** out);
 int aloam_destroy(aloam_ctx* ctx);
 const char* aloam_strerror(int code);
 
