@@ -470,9 +470,9 @@ __device__ __forceinline__ void set_bits(unsigned* m, int lo, int hi) {  // sing
 }  // namespace
 
 // One sixth of a ring (:282-398 minus the sort): positions [sp, ep], lane owns positions sp + 32 s + lane.
-// spill_in : bit k set = position sp + k was marked in cloudNeighborPicked by the previous segment's picks (k < 5).
+// spill_in : bit k set = position sp + k was marked in cloudNeighborPicked by the picks of earlier segments (k < 5).
 // Results (warp-uniform): `less` = positions picked in the sharp walk in pick order (the first two are the sharp
-// points), `flat` = positions of the flat walk, spill_out = marks this segment leaves on positions ep+1 .. ep+5.
+// points), `flat` = positions of the flat walk, spill_out = marks this segment's picks leave on positions ep+1 .. ep+5.
 template <int NS>
 __device__ __forceinline__ void pick_segment(const float* curv, const unsigned char* fb, int sp, int ep, unsigned spill_in,
                                              unsigned short* less, int& n_less, unsigned short* flat, int& n_flat,
@@ -735,9 +735,11 @@ __device__ __forceinline__ void ring_features_body(const Batch<RingFeatArgs>& B,
   // greedy picks (:291-390).  std::sort + walk == repeatedly taking the arg-max (arg-min) of the still-eligible
   // points under the (curvature, index) order, so no sort is needed: one warp keeps a segment's curvatures in
   // registers (position sp + 32 s + lane in slot s) and performs <= 20 + 4 REDUX selections.
-  // The six segments of a ring depend on each other only through the <= 5 marks a segment spills onto the start of
-  // the next one (:319-330).  Six warps therefore process the six segments CONCURRENTLY assuming an empty spill;
-  // a segment is re-run (in order) only if a position actually spilled onto it is one of its own picks -- removing a
+  // The six segments of a ring share one cloudNeighborPicked array, and a pick marks at most 5 positions past itself
+  // (:319-330), so segment w depends on the segments before it only through the marks on its first 5 positions: those of
+  // segment w-1's own picks, and -- when segment w-1 is shorter than 5 positions (rings of 17..39 returns) -- the marks
+  // that came into w-1 and run past its end.  Six warps therefore process the six segments CONCURRENTLY assuming an
+  // empty spill; a segment is re-run only if a position actually spilled onto it is one of its own picks -- removing a
   // point that never wins a selection cannot change any selection, so otherwise the speculative result is exact.
   auto run_segment = [&](int w, unsigned spill_in) {
     const int sp = s_loc + span * w / 6, ep = s_loc + span * (w + 1) / 6 - 1;
@@ -753,33 +755,38 @@ __device__ __forceinline__ void ring_features_body(const Batch<RingFeatArgs>& B,
     run_segment(warp - 1, 0u);
     if (dbg8 && lane == 0) g_dbg_pick[9 + 2 * (warp - 1)] = clock64();
   }
-  if (tid < 6) s_in[tid] = 0u;   // the incoming spill every segment was walked with
+  if (tid < 6) s_in[tid] = 0u;   // the incoming spill every segment was walked with, or accepted without a walk
   if (dbg8 && tid == 0) g_dbg_pick[6] = clock64();
-  // Fixed-point rounds instead of a sequential sweep over the boundaries: every segment compares the spill its predecessor
-  // CURRENTLY reports (S) with the one it was walked with (A) and walks again, all such segments in parallel, if the difference
-  // can matter: a mark it assumed is not there (A & ~S), or a new mark sits on one of its own picks.  Otherwise its result is
-  // also the result for S.  When a round changes nothing every segment is consistent with its predecessor, and segment 0
-  // (no predecessor) is exact, so by induction all are; the lowest inconsistent segment becomes final in every round, hence
-  // at most five rounds -- typically one, where the sequential sweep paid one walk per conflict.
+  // Fixed-point rounds instead of a sequential sweep over the boundaries.  Segment w-1 PUBLISHES S = its own spill (s_spill)
+  // | the part of its accepted input that runs past its end (s_in >> length, non-zero only for segments shorter than 5).
+  // Every segment compares the S of its predecessor with the input it accepted (A) and walks again, all such segments in
+  // parallel, if the difference can matter: a mark it assumed is not there (A & ~S), or a new mark sits on one of its own
+  // picks.  Otherwise its picks are also the picks for S, and it accepts S without a walk -- which still changes what it
+  // publishes when S and A differ past its end, so such a segment keeps the rounds going as well.  When a round would change
+  // nothing every segment is consistent with its predecessor, and segment 0 (no predecessor) is exact, so by induction all
+  // are; the lowest inconsistent segment becomes final in every round, hence at most five rounds -- typically one, where
+  // the sequential sweep paid one walk per conflict.
   for (;;) {
     __syncthreads();
-    bool need = false;
+    bool need = false, moves = false;
     unsigned S = 0u;
     if (warp >= 2 && warp <= 6) {
       const int w = warp - 1;
-      S = s_spill[w - 1];
+      const int sp = s_loc + span * w / 6;
+      const int len_prev = sp - (s_loc + span * (w - 1) / 6), len = s_loc + span * (w + 1) / 6 - sp;
+      S = s_spill[w - 1] | (len_prev < 5 ? s_in[w - 1] >> len_prev : 0u);
       const unsigned Ain = s_in[w];
       if (S != Ain) {
-        const int sp = s_loc + span * w / 6;
         const int nl = s_nl[w], nf = s_nf[w];
         const unsigned fresh = S & ~Ain;
         bool hit = (Ain & ~S) != 0u;
         if (lane < nl) { const int k = (int)s_less[w][lane] - sp; hit = hit || (k < 5 && ((fresh >> k) & 1u)); }
         if (lane >= 24 && lane - 24 < nf) { const int k = (int)s_flat[w][lane - 24] - sp; hit = hit || (k < 5 && ((fresh >> k) & 1u)); }
         need = __any_sync(0xffffffffu, hit);
+        moves = len < 5 && ((S ^ Ain) >> len) != 0u;   // what it publishes changes
       }
     }
-    if (!__syncthreads_or(need ? 1 : 0)) break;   // (also orders this round's reads of s_spill / s_less before the walks' writes)
+    if (!__syncthreads_or(need || moves ? 1 : 0)) break;   // (also orders this round's reads of s_spill / s_in / s_less before the writes)
     if (warp >= 2 && warp <= 6) {
       const int w = warp - 1;
       if (need) run_segment(w, S);

@@ -283,16 +283,89 @@ def vlp16_elevation(ring):
     return -15.0 + 2.0 * ring                    # beam centres of scanRegistration.cpp's N_SCANS == 16 formula
 
 
-def room_scan(counts, dyadic=False, zigzag=(), far=(), shift=(0.0, 0.0), scale=1.0):
+def ring_elevation(ring, n_scans=16):
+    """degrees at the middle of `ring` of the elevation formula of n_scans (scanRegistration.cpp:166-205); for 64 rings the upper
+    block holds rings 0..32 and the lower block rings 33..50 (ring 0 and the block change sit on a decision: keep them empty)"""
+    if n_scans == 16:
+        return vlp16_elevation(ring)
+    if n_scans == 32:
+        return -92.0 / 3.0 + (4.0 * ring + 2.0) / 3.0
+    return 2.0 - ring / 3.0 if ring <= 32 else -8.83 - (ring - 32) / 2.0
+
+
+DENSE_STYLES = ("smooth", "zigzag", "dyadic")
+DENSE_STEP = 0.1    # metres between consecutive returns of a smooth or zigzag arc (the suppression break is sqrt(0.05) = 0.224 m)
+
+
+def dense_arc(n, phi, dist, style, z=0.0, el=None):
+    """n returns in firing order (clockwise) on a wall `dist` metres away across azimuth phi, consecutive returns less than
+    0.22 m apart, so that a pick marks 5 positions on either side -- a pole, a person or a car close to a beam that sees
+    nothing else.  style:
+      smooth  a concave corner: two walls at +-20 deg meeting at phi, 0.1 m steps (flat points, sharp ones at the corner)
+      zigzag  the same with the range alternating by +-6.25 cm (every point a corner candidate)
+      dyadic  a straight wall 0.125 m steps, its second half zigzagging by +-6.25 cm, coordinates multiples of 2^-10 m; with
+              phi in {0, +-pi/2} and constant z, equal geometry gives bit-equal curvatures (ties at 0 and at 0.5625)
+    z: height of every return; el (degrees): z = horizontal range * tan(el) instead (elevation-mode rings)."""
+    u = np.array([np.cos(phi), np.sin(phi)])
+    t = np.array([np.sin(phi), -np.cos(phi)])                     # clockwise along the wall
+    k = np.arange(n)
+    if style == "dyadic":
+        s = (k - n // 2) * 0.125
+        off = np.where(k >= n // 2, np.where(k % 2 == 0, 0.0625, -0.0625), 0.0)
+        xy = dist * u + s[:, None] * t + off[:, None] * u
+    else:
+        s = (k - (n - 1) / 2.0) * DENSE_STEP
+        xy = dist * u + s[:, None] * t - (np.abs(s) * np.tan(np.deg2rad(20.0)))[:, None] * u
+        if style == "zigzag":
+            xy = xy + np.where(k % 2 == 0, 0.0625, -0.0625)[:, None] * u
+    zz = np.hypot(xy[:, 0], xy[:, 1]) * np.tan(np.deg2rad(el)) if el is not None else np.full(n, float(z))
+    p = np.concatenate([xy, zz[:, None]], 1)
+    if style == "dyadic":
+        p = np.round(p * 1024.0) / 1024.0
+    return p
+
+
+def _dense_place(r, style):
+    """azimuth and wall distance of ring r's dense arc: spread round the sweep, away from its start and end at +-pi"""
+    if style == "dyadic":
+        return (np.pi / 2, 0.0, -np.pi / 2)[r % 3], 4.0 + r % 4
+    return -2.4 + 4.8 * ((0.618034 * r) % 1.0), 3.5 + (r % 5) * 0.75
+
+
+def _arc_key(p, r):
+    """fraction of the clockwise turn from azimuth pi at which a sensor fires the returns p of ring r"""
+    return (np.pi - np.arctan2(p[:, 1], p[:, 0])) / (2 * np.pi) + r * 1e-9
+
+
+def _firing_order(parts):
+    """[(xyz (n, 3), firing key (n,), ring value)] -> (n, 4) float32 in firing order, float 3 = the ring value"""
+    xyz = np.concatenate([p for p, _, _ in parts])
+    key = np.concatenate([k for _, k, _ in parts])
+    out = _pts(xyz)
+    out[:, 3] = np.concatenate([np.full(len(p), v, np.float64) for p, _, v in parts])
+    return out[np.argsort(key, kind="stable")]
+
+
+def room_scan(counts, dyadic=False, zigzag=(), far=(), shift=(0.0, 0.0), scale=1.0, dense=(), dense_style="smooth", n_scans=16):
     """A VLP-16 scan of a polygon room (walls meeting at corners: sharp features), points in firing order.
     counts[r] = returns of ring r (0 allowed).  zigzag: rings whose range alternates by +-0.0625 m (a two-letter
     curvature alphabet: every point is a corner candidate, picks crowd the segment boundaries).  far: (ring, first,
     count, range_m) blocks of consecutive returns on a wall `range_m` away.  dyadic: coordinates rounded to 2^-10 m, so
-    that equal geometry gives bit-equal curvatures."""
+    that equal geometry gives bit-equal curvatures.  dense: rings whose returns lie on a dense arc (dense_arc, in
+    `dense_style`) instead of the whole turn.  n_scans: 32 / 64 put ring r at the middle of that elevation formula's ring."""
     verts = _ROOM * scale - np.asarray(shift)
-    xyz, key = [], []
+    parts = []
     for r, n in enumerate(counts):
         if n == 0:
+            continue
+        el = ring_elevation(r, n_scans)
+        if r in dense:
+            phi, dist = _dense_place(r, dense_style)
+            p = dense_arc(n, phi, dist * scale, dense_style, el=el)
+            key = _arc_key(p, r)
+            if dyadic:
+                p = np.round(p * 1024.0) / 1024.0
+            parts.append((p, key, 0.0))
             continue
         k = np.arange(n)
         phi = np.pi - 2.0 * np.pi * (k + 0.37) / n                   # clockwise: -atan2(y, x) increases
@@ -302,13 +375,36 @@ def room_scan(counts, dyadic=False, zigzag=(), far=(), shift=(0.0, 0.0), scale=1
         for ring, first, cnt, rng_m in far:
             if ring == r:
                 rho[first:first + cnt] = rng_m
-        el = np.deg2rad(vlp16_elevation(r))
-        p = np.stack([rho * np.cos(phi), rho * np.sin(phi), rho * np.tan(el)], 1)
+        p = np.stack([rho * np.cos(phi), rho * np.sin(phi), rho * np.tan(np.deg2rad(el))], 1)
         if dyadic:
             p = np.round(p * 1024.0) / 1024.0
-        xyz.append(p); key.append((k + 0.37) / n + r * 1e-9)
-    xyz = np.concatenate(xyz); key = np.concatenate(key)
-    return _pts(xyz[np.argsort(key, kind="stable")])
+        parts.append((p, (k + 0.37) / n + r * 1e-9, 0.0))
+    return _firing_order(parts)
+
+
+def short_ring_scan(counts, style, shift=(0.0, 0.0)):
+    """A field-mode scan (ring id in float 3, aloam_config.ring_source = ALOAM_RING_FIELD): ring r holds counts[r] returns;
+    rings of fewer than 64 returns lie on a dense arc (dense_arc; style = one of DENSE_STYLES, or one per ring), the others
+    take the whole turn of the polygon room.  Heights are constant per ring.  shift: the sensor's position in the room
+    (rounded to 2^-10 m, so that dyadic arcs stay dyadic)."""
+    shift = np.round(np.asarray(shift, np.float64) * 1024.0) / 1024.0
+    parts = []
+    for r, n in enumerate(counts):
+        if n == 0:
+            continue
+        st = style if isinstance(style, str) else style[r]
+        z = np.round((-2.0 + 3.0 * r / len(counts)) * 1024.0) / 1024.0
+        if n < 64:
+            phi, dist = _dense_place(r, st)
+            p = dense_arc(n, phi, dist, st, z=z)
+            p[:, :2] -= shift
+            parts.append((p, _arc_key(p, r), float(r)))
+        else:
+            k = np.arange(n)
+            phi = np.pi - 2.0 * np.pi * (k + 0.37) / n
+            rho = _room_range(phi, _ROOM - shift)
+            parts.append((np.stack([rho * np.cos(phi), rho * np.sin(phi), np.full(n, z)], 1), (k + 0.37) / n + r * 1e-9, float(r)))
+    return _firing_order(parts)
 
 
 def suppression_reach(full):

@@ -98,6 +98,9 @@ def test_features_equal_the_wide_oracle(aloam, synth, sensor, reverse, laser_maj
     assert len(s) == ns and len(e) == ns
     assert_matches_oracle(got, curv, label, s, e, want, ns)
     assert len(want.sharp) > 0 and len(want.less_flat) > 0 and int(want.full[:, 3].max()) >= 64
+    if sensor == "OS128" and not laser_major:   # whole scans: the highest beams' rings of 17..39 returns are compared too
+        n = np.bincount(want.full[:, 3].astype(np.int64), minlength=ns)
+        assert ((n >= 17) & (n < 40)).any()
 
 
 def test_os128_at_2048_azimuth_steps(aloam, synth):
@@ -234,8 +237,15 @@ def test_sixteen_lanes_snapshots_and_a_64_ring_context(aloam, synth):
 def test_prior_map_relocalises_and_recovers_os128_scans(aloam, synth):
     runs = [WR.scan(synth, "OS128", k) for k in range(6)]
     mp = max(len(s) for s in runs) + 1024
+    import recovery_cases as RV
+    import track_cases as TC
+    # cube growth on: at one slab per cube this store overflows from the third frame on (flag 8), and the prior map built from
+    # the truncated store is not the oracle's
     m = _wide(aloam, 128, mp, max_map_points=200000)
+    m.set_cube_growth(True)
+    m.set_map_rows(True, TC.ISQ, TC.PTS)
     _, mapped = _run_lanes(m, [runs], [[START]] + [[SCAN]] * (len(runs) - 1))
+    assert not (m.map_rows(len(runs))["flags"] & aloam.FLAG_CUBE_OVERFLOW).any()
     blob = m.lane_save(0)
     m.close()
     split = aloam.snapshot_store_clouds(blob)
@@ -258,9 +268,8 @@ def test_prior_map_relocalises_and_recovers_os128_scans(aloam, synth):
     res, scores = c.prior_relocalise(np.array(hyps), f["less_sharp"], f["less_flat"], refine=1)
     assert res[0]["hyp"] == 13 and scores.argmax() == 13   # the undisplaced hypothesis
     assert np.abs(res[0]["pose"][4:] - true[4:]).max() < 0.05
-    # a recovery-armed localising lane started 1.5 m off re-seats on the prior map
-    import recovery_cases as RV
-    import track_cases as TC
+    # a recovery-armed localising lane started 1.5 m off re-seats on the prior map, adopting on its START row the candidate and
+    # score of the host model of recovery on the oracle's map (tests/recovery_cases.py via wide_ring_oracle.recovery_model)
     c.set_map_rows(True, TC.ISQ, TC.PTS)
     c.set_recovery(True, RV.TRIGGER, RV.ACCEPT, RV.deltas(aloam))
     start = mapped[2, 0].copy()
@@ -268,6 +277,10 @@ def test_prior_map_relocalises_and_recovers_os128_scans(aloam, synth):
     c.lane_localise(0, start[:4], start[4:])
     o, m2 = _run_lanes(c, [runs[2:]], [[START]] + [[SCAN]] * (len(runs) - 3))
     rec = c.recovery_rows(len(runs) - 2)
+    rows = c.map_rows(len(runs) - 2)
     c.close()
-    assert rec["adopted"].any()
+    _, want = WR.recovery_model(aloam, synth, (1.5, -1.5), frames=len(runs))
+    assert rec["adopted"].tolist() == [int(r["adopted"]) for r in want]
+    assert rec["best"].tolist() == [r["best"] for r in want] and rec["best_score"].tolist() == [r["best_score"] for r in want]
+    assert rows["score"][0] == want[0]["score"] and rows["n_score"][0] == want[0]["n_score"]
     assert np.abs(m2[-1, 0, 4:] - mapped[-1, 0, 4:]).max() < 0.1

@@ -1,9 +1,11 @@
 """CPU models of two re-formulations the ring feature kernel (a-loam_b200/csrc/features.cu) relies on.  They restate the ARGUMENT,
 not the kernel: the GPU parity tests compare the kernel itself with the oracle bit for bit.
 
-1. Greedy picks (scanRegistration.cpp:282-398): the six segments of a ring are walked in parallel assuming no marks spill in from
-   the previous segment, then re-walked in parallel fixed-point rounds.  Claim: the result equals the sequential sweep in which
-   every segment receives the exact spill of its predecessor.
+1. Greedy picks (scanRegistration.cpp:282-398): the reference walks the six segments of a ring one after the other with ONE
+   cloudNeighborPicked array (`sequential`).  The kernel walks them in parallel assuming no marks spill in from the previous
+   segment, then re-walks them in parallel fixed-point rounds (`fixed_point`), where what a segment passes on is the marks of its
+   own picks and the incoming marks that run past its end.  Claim: the two are equal.  `fixed_point_adjacent` passes on only a
+   segment's own marks; it is wrong exactly on rings with a segment shorter than 5 positions past segment 0 (17..39 returns).
 2. Per-ring VoxelGrid (scanRegistration.cpp:401-407): the kernel sorts EVERY in-range position by its absolute voxel coordinates
    before the picks are known and drops the picked positions afterwards.  Claim: the order equals PCL's sort by the voxel index
    relative to the bounding box of the surviving points (stable by position).
@@ -11,10 +13,12 @@ not the kernel: the GPU parity tests compare the kernel itself with the oracle b
 import numpy as np
 import pytest
 
+ALPHABET = np.array([0.0, 0.05, 0.1, 0.2, 0.5, 1.0, 3.0], np.float32)
+
 
 def walk_segment(curv, reach_b, reach_f, sp, ep, spill_in):
     """One segment: picks in the reference's order with `spill_in` (set of positions already marked).  Returns
-    (less_sharp picks, flat picks, set of marked positions beyond ep)."""
+    (less_sharp picks, flat picks, set of positions beyond ep marked by this segment's picks)."""
     picked = set(p for p in spill_in if sp <= p <= ep)
     spill_out = set()
 
@@ -52,71 +56,119 @@ def bounds(n, w):
 
 
 def sequential(curv, rb, rf):
+    """the reference: the six segments in order, one picked array for the whole ring"""
     n = len(curv)
-    out, spill = [], set()
+    out, marked = [], set()
     for w in range(6):
         sp, ep = bounds(n, w)
-        less, flat, spill = walk_segment(curv, rb, rf, sp, ep, spill)
+        less, flat, spill = walk_segment(curv, rb, rf, sp, ep, marked)
+        marked |= spill
         out.append((less, flat))
     return out
 
 
-def fixed_point(curv, rb, rf):
+def _rounds(curv, rb, rf, publish):
+    """the kernel's fixed-point rounds; publish(w, own, accepted) = the spill segment w passes on"""
     n = len(curv)
-    res, spill_out, assumed = [None] * 6, [set()] * 6, [set()] * 6
+    res, own, assumed = [None] * 6, [set()] * 6, [set()] * 6
     for w in range(6):                              # speculative pass: nothing spills in
         sp, ep = bounds(n, w)
         less, flat, so = walk_segment(curv, rb, rf, sp, ep, set())
-        res[w], spill_out[w] = (less, flat), so
+        res[w], own[w] = (less, flat), so
     rounds = 0
     while True:
         todo = []
         for w in range(1, 6):                       # all decisions of a round read the state of the previous round
-            S, A = spill_out[w - 1], assumed[w]
+            S, A = publish(w - 1, own[w - 1], assumed[w - 1]), assumed[w]
             if S == A:
                 continue
-            own = set(res[w][0]) | set(res[w][1])
-            hit = bool(A - S) or bool((S - A) & own)
-            todo.append((w, S, hit))
-        if not any(h for _, _, h in todo):
+            mine = set(res[w][0]) | set(res[w][1])
+            hit = bool(A - S) or bool((S - A) & mine)
+            moves = publish(w, own[w], S) != publish(w, own[w], A)   # accepting S without a walk changes what w passes on
+            todo.append((w, S, hit, moves))
+        if not any(h or m for _, _, h, m in todo):
             break
         rounds += 1
         new = {}
-        for w, S, hit in todo:
+        for w, S, hit, _ in todo:
             if hit:
                 sp, ep = bounds(n, w)
                 new[w] = walk_segment(curv, rb, rf, sp, ep, S)
-        for w, S, hit in todo:
+        for w, S, hit, _ in todo:
             assumed[w] = S
             if hit:
                 less, flat, so = new[w]
-                res[w], spill_out[w] = (less, flat), so
+                res[w], own[w] = (less, flat), so
         assert rounds <= 5
     return res, rounds
 
 
+def fixed_point(curv, rb, rf):
+    """the kernel: a segment passes on its own marks and the accepted incoming marks beyond its end"""
+    n = len(curv)
+    return _rounds(curv, rb, rf, lambda w, own, acc: own | {p for p in acc if p > bounds(n, w)[1]})
+
+
+def fixed_point_adjacent(curv, rb, rf):
+    """the kernel before marks passed through short segments: a segment passes on its own marks only"""
+    return _rounds(curv, rb, rf, lambda w, own, acc: own)
+
+
+def draw(seed, lo=17, hi=400, n=None):
+    """a ring of n (or lo..hi-1) positions: curvatures from a coarse alphabet (many ties, many picks next to the segment
+    boundaries) and random reaches of 0..5"""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(lo, hi)) if n is None else n
+    return rng.choice(ALPHABET, size=n), rng.integers(0, 6, size=n), rng.integers(0, 6, size=n)
+
+
 @pytest.mark.parametrize("seed", range(40))
 def test_parallel_rewalk_rounds_equal_the_sequential_sweep(seed):
-    rng = np.random.default_rng(seed)
-    n = int(rng.integers(60, 400))
-    # small segments and a coarse curvature alphabet: many ties, many picks next to the segment boundaries
-    curv = rng.choice(np.array([0.0, 0.05, 0.1, 0.2, 0.5, 1.0, 3.0], np.float32), size=n)
-    rb = rng.integers(0, 6, size=n)
-    rf = rng.integers(0, 6, size=n)
+    curv, rb, rf = draw(seed)
     want = sequential(curv, rb, rf)
     got, rounds = fixed_point(curv, rb, rf)
     assert got == want
+    if len(curv) >= 40:
+        assert fixed_point_adjacent(curv, rb, rf)[0] == want
 
 
 def test_the_rewalk_model_exercises_conflicts():
     hits = 0
     for seed in range(40):
-        rng = np.random.default_rng(seed)
-        n = int(rng.integers(60, 400))
-        curv = rng.choice(np.array([0.0, 0.05, 0.1, 0.2, 0.5, 1.0, 3.0], np.float32), size=n)
-        rb = rng.integers(0, 6, size=n); rf = rng.integers(0, 6, size=n)
+        curv, rb, rf = draw(seed, 60, 400)
         hits += fixed_point(curv, rb, rf)[1] > 0
     assert hits >= 10          # the equality above is not vacuous
+
+
+@pytest.mark.parametrize("n", range(17, 49))
+def test_short_rings_every_size(n):
+    """every ring of 17..48 returns (segments of 1..7 positions), 60 draws each: the pass-through rounds equal the sequential
+    sweep; passing on only a segment's own marks differs from it for some draw at every size up to 39 and never from 40 on
+    (from 40 every segment past the first holds at least 5 positions, so no mark runs past one)"""
+    lens = [bounds(n, w)[1] - bounds(n, w)[0] + 1 for w in range(6)]
+    assert (min(lens[1:]) < 5) == (n < 40)
+    differ = 0
+    for seed in range(60):
+        curv, rb, rf = draw(1000 * n + seed, n=n)
+        want = sequential(curv, rb, rf)
+        assert fixed_point(curv, rb, rf)[0] == want, seed
+        differ += fixed_point_adjacent(curv, rb, rf)[0] != want
+    if n < 40:
+        assert differ > 0
+    else:
+        assert differ == 0
+
+
+def test_marks_run_through_four_one_position_segments():
+    """17 returns: six segments of one position each.  A flat pick in segment 0 marks the next five positions, so the
+    reference picks nothing in segments 1..5; the adjacent-only model sees the marks in segment 1 only and picks again in 2 and 4"""
+    n = 17
+    curv = np.zeros(n, np.float32)
+    rb = np.zeros(n, int); rf = np.full(n, 5)
+    want = sequential(curv, rb, rf)
+    assert want == [([], [5])] + [([], [])] * 5
+    assert fixed_point(curv, rb, rf)[0] == want
+    assert fixed_point_adjacent(curv, rb, rf)[0] == [([], [5])] + [([], [])] + [([], [7])] + [([], [])] + [([], [9])] + [([], [])]
 
 
 @pytest.mark.parametrize("seed", range(10))

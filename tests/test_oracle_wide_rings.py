@@ -157,3 +157,37 @@ def test_snapshot_check_accepts_a_128_ring_header(aloam):
     struct.pack_into("<i", h, 36, 128)
     info = aloam.snapshot_info(bytes(h))
     assert info["n_scans"] == 128 and info["bytes"] == 256
+
+
+def test_os128_scans_hold_short_rings_that_need_the_pass_through(synth):
+    """the OS128 scans of the wide GPU tests are compared whole: their highest beams hold rings of 17..39 returns, on which
+    passing on only a segment's own marks gives other picks than the oracle (scan 2 is the one of the feature tests)"""
+    import short_ring_cases as SC
+    short, miss = [], []
+    for index in range(5):
+        raw = WR.scan(synth, "OS128", index)
+        n = np.bincount(raw[:, 3].astype(np.int64), minlength=128)
+        short.append(bool(((n >= 17) & (n < 40)).any()))
+        miss.append(bool(SC.adjacent_misses(WR.Features(raw, 128, synth.RING_RANGES[0]), 128)))
+    assert short[2] and miss[2] and sum(miss) >= 2, (short, miss)
+
+
+def test_only_the_os128_table_has_short_rings(synth):
+    """of the four wide tables only OS128's highest beams see little within range: V128, L96 and E65 hold over 500 returns on
+    every ring of every scan of the wide tests, so their whole scans have no ring of 17..39 returns"""
+    for sensor in ("V128", "L96", "E65"):
+        for index in range(6):
+            n = np.bincount(WR.scan(synth, sensor, index)[:, 3].astype(np.int64), minlength=WR.n_rings(synth, sensor))
+            assert n.min() > 500, (sensor, index)
+
+
+def test_recovery_model_reseats_from_every_corner_on_whole_os128_scans(aloam, synth):
+    """the host model of recovery (tests/recovery_cases.py) on the oracle's map of whole OS128 scans: a localising lane armed 1.5 m
+    off in x and y adopts a candidate on its START row from each of the four corners, stays within 0.1 m from the next row on and
+    ends within 1 cm; the GPU test holds the device to the model's candidate and score from (+1.5, -1.5)"""
+    for off in ((1.5, -1.5), (1.5, 1.5), (-1.5, 1.5), (-1.5, -1.5)):
+        poses, rows = WR.recovery_model(aloam, synth, off)
+        assert rows[0]["triggered"] and rows[0]["adopted"], off
+        assert not any(r["triggered"] for r in rows[1:]), off
+        err = [float(np.abs(r["pose"][4:] - poses[2 + j][4:]).max()) for j, r in enumerate(rows)]
+        assert max(err[1:]) < 0.1 and err[-1] < 0.01, (off, err)

@@ -71,18 +71,9 @@ def n_rings(synth, sensor):
     return len(synth.WIDE_RING_SENSORS[sensor][0]) if sensor in synth.WIDE_RING_SENSORS else len(synth.RING_SENSORS[sensor][0])
 
 
-SPARSE = 32
-
-
 def scan(synth, sensor, index, **kw):
-    """synth.scan_rings(sensor, index, **kw) without the returns of rings that hold fewer than SPARSE of them.  The highest beams
-    of these tables see little within range, and on a ring of about 20 returns the device's ring features and the oracle's
-    differ -- in a 64-wide context of aloam_create too, so it is not a matter of the ring width; the wide tests leave such rings
-    out rather than pin that difference here."""
-    raw = synth.scan_rings(sensor, index, **kw)
-    r = raw[:, 3].astype(np.int64)
-    cnt = np.bincount(r, minlength=MAX_RINGS)
-    return np.ascontiguousarray(raw[cnt[r] >= SPARSE])
+    """synth.scan_rings(sensor, index, **kw): the whole scan, the highest beams' short rings included"""
+    return synth.scan_rings(sensor, index, **kw)
 
 
 def odometry_chain(orc_mod, synth, sensor, frames, reverse=False, distortion=False, nearby_scan=2.5, n_az=None):
@@ -103,3 +94,34 @@ def odometry_chain(orc_mod, synth, sensor, frames, reverse=False, distortion=Fal
         od.set_last(f.less_sharp, f.less_flat)
         poses.append(np.concatenate([qw, tw]))
     return np.array(poses), counts
+
+
+def recovery_model(aloam, synth, offset, frames=6, start=2):
+    """tests/recovery_cases.recover_track on whole OS128 scans: the oracle maps scans 0 .. frames-1 (its store is the device's with
+    cube growth on), freezes the store, and runs a localising lane armed at the map pose of scan `start` moved by `offset` (x, y)
+    with recovery over RV.deltas.  Returns (map poses (frames, 7), the lane's rows)."""
+    import pyfrozen
+    import pyoracle
+    import recovery_cases as RV
+    import reloc_cases as RC
+    feats = [Features(scan(synth, "OS128", k), 128, synth.RING_RANGES[0]) for k in range(frames)]
+    od, cm = pyoracle.Odometry(), pyoracle.CubeMap()
+    q = np.array([0, 0, 0, 1.0]); t = np.zeros(3); qw = q.copy(); tw = t.copy()
+    poses = []
+    for k, f in enumerate(feats):
+        if k > 0:
+            q, t, _ = od.register(f.sharp, f.flat, q, t)
+            qw, tw = pyoracle.integrate_pose(qw, tw, q, t)
+        od.set_last(f.less_sharp, f.less_flat)
+        poses.append(cm.step(f.less_sharp, f.less_flat, qw, tw, *synth.RING_RANGES[1:])[0])
+    cubes = {}
+    for which in (0, 1):
+        for i in range(pyfrozen.NCUBE):
+            c = cm.cube(which, i)
+            if len(c):
+                cubes[(which, i)] = c
+    frozen = pyfrozen.FrozenMap.from_cubes(cm.state()["centre"], cubes)
+    init = np.array(poses[start], np.float64)
+    init[4:6] += offset
+    rows = RV.recover_track(frozen, RC.FrozenScorer(frozen), feats, init, start, frames, synth.RING_RANGES[1:], RV.deltas(aloam))
+    return np.array(poses), rows
