@@ -90,10 +90,11 @@ static int create_ctx(const aloam_config* cfg_in, aloam_ctx** out, int max_field
   if (cfg.ring_source == ALOAM_RING_FIELD ? cfg.n_scans < 1 || cfg.n_scans > max_field_rings : cfg.n_scans != 16 && cfg.n_scans != 32 && cfg.n_scans != 64)
     return ALOAM_ERR_UNSUPPORTED_SCANS;
   if (cfg.max_points <= 0 || cfg.outer_iters < 1 || cfg.outer_iters > 4 || cfg.inner_iters < 0) return ALOAM_ERR_INVALID_ARG;
-  // a 128-wide association index packs a point's index into 24 bits (index << 7 | ring), and aloam_odometry_set_last takes
-  // clouds of up to max_points
+  // the association index packs a point's index with its ring into a non-negative int (index << log2 W | ring) below INT_MAX,
+  // which the search keeps as its "no candidate" word, and aloam_odometry_set_last takes clouds of up to max_points: indices
+  // below 2^24 - 1 at W = 128, below 2^25 - 1 at W = 64
   const int ring_w = ring_width(cfg.n_scans);
-  if (ring_w > 64 && cfg.max_points > (1 << 24)) return ALOAM_ERR_INVALID_ARG;
+  if (cfg.max_points > (ring_w > 64 ? (1 << 24) - 1 : (1 << 25) - 1)) return ALOAM_ERR_INVALID_ARG;
   if (!(cfg.nearby_scan >= 1.0)) return ALOAM_ERR_INVALID_ARG;   // the association's break tables need a window of +-1 ring at least
   // HuberLoss(a) needs a > 0, and a VoxelGrid leaf <= 0 or NaN has no voxels
   if (!(cfg.huber > 0) || !(cfg.line_res > 0) || !(cfg.plane_res > 0)) return ALOAM_ERR_INVALID_ARG;

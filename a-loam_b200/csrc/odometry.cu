@@ -181,7 +181,8 @@ __global__ void k_rab_fill(const __grid_constant__ Batch<RabArgs> B) {
   const Pt4 p = pts[i];
   const int cell = g.cell_of[i];
   // index-major key: comparing keys compares indices, the reference's tie rule (the ring need not ascend with the index)
-  // (i < 2^24 at W = 128: aloam_create_wide bounds max_points, so the word stays non-negative)
+  // (i < 2^24 - 1 at W = 128, < 2^25 - 1 at W = 64: create_ctx bounds max_points, so the word stays below INT_MAX, the
+  // search's "no candidate")
   g.gpts[g.start[cell] + g.rank_of[i]] = make_float4(p.x, p.y, p.z, __int_as_float((i << RingBits<W>::value) | (cell & (W - 1))));
 }
 template __global__ void k_rab_fill<64>(const __grid_constant__ Batch<RabArgs> B);
@@ -321,7 +322,7 @@ __device__ __forceinline__ void store_none(BlockRec* b, int* corr) {
   if (corr) { corr[0] = -1; corr[1] = -1; corr[2] = -1; corr[3] = 0; }
 }
 
-constexpr int kBig = 1 << 25;       // separates forward ranks [0, 2^24) from backward ranks
+constexpr int kBig = 1 << 25;       // separates forward ranks [0, 2^25 - 1) from backward ranks (create_ctx bounds max_points)
 
 // exact nearest neighbour of q with d2 < limit (strict); returns its packed word (index << log2 W | ring) or -1, d2 in out_d,
 // the half-width of the bucket interval it had to read in k_out.  Ties -> smaller index (packed order == index order).

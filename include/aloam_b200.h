@@ -77,7 +77,9 @@ typedef struct aloam_config {
                             distance against this double */
   double nearby_scan;    /* 2.5 NEARBY_SCAN, laserOdometry.cpp:66; >= 1, may be +inf (the ring-window walks never break) */
   int device;            /* CUDA device ordinal */
-  int max_points;        /* capacity of one raw scan (reference: 400000 static arrays, scanRegistration.cpp:66-69) */
+  int max_points;        /* capacity of one raw scan (reference: 400000 static arrays, scanRegistration.cpp:66-69); 1 .. 2^25 - 1
+                            (2^24 - 1 above 64 rings, see aloam_create_wide): the association index packs a point's index and
+                            ring into one int.  Larger values are ALOAM_ERR_INVALID_ARG */
   int max_map_points;    /* capacity of the uploaded submap, per cloud type (0 = mapping not used); at most 2^30, larger
                             values are rejected by aloam_create with ALOAM_ERR_INVALID_ARG */
   int max_batch;         /* trajectories a context can advance in lockstep (aloam_scan_stream_batch), or lanes of
@@ -140,7 +142,8 @@ int aloam_create(const aloam_config* cfg, aloam_ctx** out);
  * stays ALOAM_ERR_INVALID_ARG.  With n_scans > 64:
  *   - the context's ring-indexed tables are 128 wide: an int(intensity) of 0..127 is a ring of aloam_odometry_set_last's
  *     clouds (ALOAM_ERR_NOT_RING_MAJOR above that);
- *   - cfg.max_points > 2^24 is ALOAM_ERR_INVALID_ARG: the association index packs a point's index into 24 bits;
+ *   - cfg.max_points > 2^24 - 1 is ALOAM_ERR_INVALID_ARG: the association index packs a point's index into 24 bits, and
+ *     index 2^24 - 1 on ring 127 would pack to INT_MAX, the search's "no candidate" word (2^25 - 1 at up to 64 rings);
  *   - every lane allocates 64 x (32 x (156 + max_ring_points) + 8 x (6 + ceil(max_points / 1024)) + 12 x 1040) bytes more
  *     than at 64 rings (64 more rings of: two staging sets of 12 + 120 + 24 + max_ring_points points, the ring-binning
  *     tables, and the twelve association indexes of 128 buckets): 9.7 MB per lane at max_ring_points = 4096 and

@@ -74,13 +74,14 @@ def associate(last, queries, thr, nearby, corner):
     return rows
 
 
-def window(rc, nearby):
-    """(dn, up) after the fix: the rings rc - dn .. rc + up pass the break tests `int < rc - N` / `int > rc + N`"""
+def window(rc, nearby, width=64):
+    """(dn, up) after the fix: the rings rc - dn .. rc + up pass the break tests `int < rc - N` / `int > rc + N`; both are
+    bounded by the context's ring width (64, or 128 in a context of aloam_create_wide above 64 rings)"""
     up = 0
-    while up < 64 and float(rc + up + 1) <= rc + nearby:
+    while up < width and float(rc + up + 1) <= rc + nearby:
         up += 1
     dn = 0
-    while dn < 64 and float(rc - dn - 1) >= rc - nearby:
+    while dn < width and float(rc - dn - 1) >= rc - nearby:
         dn += 1
     return dn, up
 
@@ -103,24 +104,26 @@ def _sorted(points):
     return np.ascontiguousarray(c[np.argsort(c[:, 3].astype(np.int32), kind="stable")])
 
 
-def window_scene(seed=0):
-    """(last, queries): per closest ring rc of WINDOW_RCS two clusters.  Around each query the closest point (ring rc, 5 cm),
-    a same-ring point (50 cm) and one point on every other ring.  Rings on one side sit nearer the farther they are from rc
-    (1.98 m at rc +- 1 down to 0.72 m at +- 64), the other side's 2 m farther still, so the 2nd (corner) and 3rd (surf) point
-    is the outermost in-window ring of the near side, and rings rc +- (up + 1) beyond it hold nearer points than every
-    candidate inside the window.  One cluster has the near side forward, the other backward."""
+def window_scene(seed=0, width=64, rcs=WINDOW_RCS):
+    """(last, queries): per closest ring rc of `rcs` two clusters.  Around each query the closest point (ring rc, 5 cm),
+    a same-ring point (50 cm) and one point on every other ring of 0 .. width - 1.  Rings on one side sit nearer the farther
+    they are from rc (1.98 m at rc +- 1 down to 0.72 m at +- width, in steps of 1.28 m / width), the other side's 2 m farther
+    still, so the 2nd (corner) and 3rd (surf) point is the outermost in-window ring of the near side, and rings rc +- (up + 1)
+    beyond it hold nearer points than every candidate inside the window.  One cluster has the near side forward, the other
+    backward."""
     rng = np.random.default_rng(seed)
-    cases = [(rc, side) for rc in WINDOW_RCS for side in (0, 1)]
+    step = 0.02 * 64 / width   # 0.02 exactly at 64 rings
+    cases = [(rc, side) for rc in rcs for side in (0, 1)]
     centres = _centres(len(cases), 90.0)
     pts, queries = [], []
     for (rc, side), q in zip(cases, centres):
         queries.append([q[0], q[1], 0.0, rc + 0.03])
         pts.append(list(q[:3] + 0.05 * _unit(rng)) + [rc + 0.01])
         pts.append(list(q[:3] + 0.5 * _unit(rng)) + [rc + 0.02])
-        for k in range(1, 65):
-            near, far = 2.0 - 0.02 * k, 4.0 - 0.02 * k
+        for k in range(1, width + 1):
+            near, far = 2.0 - step * k, 4.0 - step * k
             for r, dist in ((rc + k, near if side == 0 else far), (rc - k, far if side == 0 else near)):
-                if 0 <= r <= 63:
+                if 0 <= r <= width - 1:
                     pts.append(list(q[:3] + dist * _unit(rng)) + [r + 0.04])
     return _sorted(pts), np.array(queries, np.float32)
 

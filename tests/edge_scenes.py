@@ -168,32 +168,33 @@ def bucket_of(x, y, nb=128):
     return np.clip(((a + F32(np.pi)) * F32(nb / (2 * np.pi))).astype(np.int32), 0, nb - 1)
 
 
-def search_clouds(rng):
-    """non-lidar clouds for k-NN: {name: (cloud, queries)}"""
+def search_clouds(rng, width=64):
+    """non-lidar clouds for k-NN: {name: (cloud, queries)}, rings drawn from 0 .. width - 1 (the dense cells on rings 5 and
+    width - 24)"""
     out = {}
     n = 3000
     xyz = rng.uniform(-20, 20, (n, 3))
     q = np.concatenate([rng.uniform(-20, 20, (400, 3)), [[0, 0, 0], [0, 0, 7.5], [0, 0, -3], [-5, 0.0, 1], [-5, -0.0, 1],
                                                          [-12, -0.0, -2], [1e-30, 0, 0]]])
-    out["uniform"] = (ring_major(xyz, rng.integers(0, 64, n)), _pts(q))
+    out["uniform"] = (ring_major(xyz, rng.integers(0, width, n)), _pts(q))
     out["one_point"] = (ring_major([[3.0, -4.0, 0.5]], [17]), _pts(rng.uniform(-30, 30, (50, 3))))
     # everything at one azimuth, queries on the opposite side: the sweep must go round the whole circle
     phi = rng.uniform(0.30, 0.31, 400); rho = rng.uniform(3, 4, 400)
     c = np.stack([rho * np.cos(phi), rho * np.sin(phi), rng.uniform(-1, 1, 400)], 1)
     phq = rng.uniform(0.3, 0.31, 40) + np.pi; rq = rng.uniform(2, 8, 40)
-    out["one_azimuth"] = (ring_major(c, rng.integers(0, 64, 400)),
+    out["one_azimuth"] = (ring_major(c, rng.integers(0, width, 400)),
                           _pts(np.stack([rq * np.cos(phq), rq * np.sin(phq), rng.uniform(-1, 1, 40)], 1)))
     # dense cells: 40 and 1000 points in one (bucket, ring) cell, plus copies of points on other rings
     d1 = np.stack([10 + rng.uniform(0, 0.05, 40), rng.uniform(0, 0.05, 40), rng.uniform(0, 0.05, 40)], 1)
     d2 = np.stack([-10 + rng.uniform(0, 0.05, 1000), 3 + rng.uniform(0, 0.05, 1000), rng.uniform(0, 0.05, 1000)], 1)
     dup = np.repeat(d1[:5], 3, axis=0)
-    xyz = np.concatenate([d1, d2, dup]); rings = np.concatenate([np.full(40, 5), np.full(1000, 40), np.repeat([6, 7, 8], 5)])
+    xyz = np.concatenate([d1, d2, dup]); rings = np.concatenate([np.full(40, 5), np.full(1000, width - 24), np.repeat([6, 7, 8], 5)])
     qd = np.concatenate([d1 + rng.normal(0, 0.01, d1.shape), d2[:200] + rng.normal(0, 0.01, (200, 3)), d1[:5]])
     out["dense_cells"] = (ring_major(xyz, rings), _pts(qd))
     return out
 
 
-def assoc_scene(seed=0):
+def assoc_scene(seed=0, width=64):
     """A "last" corner / surf cloud (ring-major) of isolated sites in the sweep-start frame, and the start-frame positions
     of the queries meant for them.  Sites:
       tie    closest point A on ring rc; exact copies of one point B on rings rc+1 and rc-1 (2nd point: forward against
@@ -202,8 +203,9 @@ def assoc_scene(seed=0):
       far    points whose query lies 8.5-10 deg (3-3.5 buckets) away at 9-12 m (bucket-by-bucket growth)
       wrap   points at azimuth pi - 0.05 with their queries at -pi + 0.004 (the interval wraps past +-pi)
       near   sites at 2-5 m (the rho < 6.5 m first interval)
-      edge   sites on rings 0 and 63 only (clamped ring slices)
-    Returns (corner_last, surf_last, queries_start_frame (m, 3) float64, tags)."""
+      edge   sites on rings 0 and width - 1 only (clamped ring slices), and at width 128 also on rings 64 and 63 (either side
+             of the middle of the ring range)
+    Rings are those of a context of `width` rings (64, or 128 above 64 rings).  Returns (corner_last, surf_last, queries_start_frame (m, 3) float64, tags)."""
     rng = np.random.default_rng(seed)
     pts, rings, q, tags = [], [], [], []
 
@@ -215,19 +217,19 @@ def assoc_scene(seed=0):
         if with_ties:
             b = a + [0, 0, 0.25]
             c = a + 0.2 * tang + [0, 0, 0.0625]
-            up, dn = min(rc + 1, 63), max(rc - 1, 0)
+            up, dn = min(rc + 1, width - 1), max(rc - 1, 0)
             P = [a - 0.3 * tang, c, a, c, a + 0.3 * tang, b, b]; R = [rc, rc, rc, rc, rc, up, dn]
             if with_ties == "first":                       # a copy of A on the next ring: the 1st point ties instead
                 P.append(a); R.append(up)
         else:                                              # no copies; one point on the next ring makes a correspondence
-            P = [a - 0.3 * tang, a, a + 0.3 * tang, a + [0, 0, 0.25]]; R = [rc, rc, rc, min(rc + 1, 63)]
+            P = [a - 0.3 * tang, a, a + 0.3 * tang, a + [0, 0, 0.25]]; R = [rc, rc, rc, min(rc + 1, width - 1)]
         pts.extend(P); rings.extend(R)
         q.append(a + (offset if offset is not None else rng.normal(0, 0.02, 3))); tags.append(tag)
 
     for k in range(24):                                    # tie sites all round the circle, 12-20 m
         phi = -np.pi + (k + 0.5) * 2 * np.pi / 24
         rho = rng.uniform(12, 20)
-        site([rho * np.cos(phi), rho * np.sin(phi), rng.uniform(-2, 2)], int(rng.integers(2, 62)), "tie",
+        site([rho * np.cos(phi), rho * np.sin(phi), rng.uniform(-2, 2)], int(rng.integers(2, width - 2)), "tie",
              with_ties="first" if k % 4 == 3 else True)
     for k in range(6):                                     # queries 2-3 buckets from their only neighbours
         phi = 0.2 + k * 0.9; rho = rng.uniform(9, 12); dphi = np.deg2rad(rng.uniform(8.5, 10.0))
@@ -242,9 +244,10 @@ def assoc_scene(seed=0):
     for k in range(6):
         phi = 1.0 + k * 0.7; rho = 2 + 0.5 * k
         site([rho * np.cos(phi), rho * np.sin(phi), -0.5], 20 + k, "near")
-    for k in range(4):
+    edge = [width - 1, 0, width - 1, 0] + ([64, 63] if width > 64 else [])
+    for k, rc in enumerate(edge):
         phi = -2.5 + k * 0.3
-        site([15 * np.cos(phi), 15 * np.sin(phi), 3.0], 0 if k % 2 else 63, "edge")
+        site([15 * np.cos(phi), 15 * np.sin(phi), 3.0], rc, "edge")
     cloud = ring_major(pts, rings)
     return cloud, cloud.copy(), np.array(q), np.array(tags)
 

@@ -143,9 +143,15 @@ def test_create_wide_is_checked_before_the_device(aloam):
     assert _code(aloam, n_scans=0, ring_source=F) == -2 and _code(aloam, n_scans=129, ring_source=F) == -2
     assert _code(aloam, n_scans=40) == -2 and _code(aloam, n_scans=128) == -2   # elevation rings stay 16 / 32 / 64
     assert _code(aloam, n_scans=16, ring_source=2) == -1 and _code(aloam, n_scans=128, ring_source=2) == -1
-    # the packed index of a 128-wide association index has 24 bits
-    assert _code(aloam, n_scans=128, ring_source=F, max_points=(1 << 24) + 1) == -1
-    assert _code(aloam, n_scans=65, ring_source=F, max_points=(1 << 24) + 1) == -1
+    # the packed index of a 128-wide association index has 24 bits, and index 2^24 - 1 on ring 127 would pack to INT_MAX (the
+    # search's "no candidate"); at 64 rings index 2^25 - 1 on ring 63 would, and from 2^25 on the word turns negative
+    for mp in ((1 << 24) + 1, 1 << 24):
+        assert _code(aloam, n_scans=128, ring_source=F, max_points=mp) == -1
+        assert _code(aloam, n_scans=65, ring_source=F, max_points=mp) == -1
+    for mp in (1 << 25, (1 << 25) + 1, 1 << 30):
+        for ns, kw in ((64, {}), (16, {}), (64, dict(ring_source=F)), (40, dict(ring_source=F))):
+            assert _code(aloam, wide=False, n_scans=ns, max_points=mp, **kw) == -1, (ns, mp)
+            assert _code(aloam, n_scans=ns, max_points=mp, **kw) == -1, (ns, mp)
     # aloam_create is unchanged
     assert _code(aloam, wide=False, n_scans=65, ring_source=F) == -2 and _code(aloam, wide=False, n_scans=128, ring_source=F) == -2
     msg = aloam.lib().aloam_strerror(-2).decode()
