@@ -12,12 +12,14 @@
 //                                    gather (:392-398), pcl::VoxelGrid(0.2) (:401-407) -- all in shared memory
 //   k_compact    (CTA / ring)        ring-ordered concatenation of the four feature clouds (:304-310,356,407)
 //
-// Everything here is float32 with the reference's evaluation order (compiled -fmad=false); ties in the two
+// Everything here is float32 with the reference's evaluation order (compiled -fmad=false), and the azimuths of the sweep
+// walk and the elevation of :166 come out of libm_atan.cuh as the host's libm computes them; ties in the two
 // reference-internal unstable sorts are resolved by original index (SURVEY.md 8a note 4).
 #include <climits>
 #include <cfloat>
 #include "common.cuh"
 #include "kernels.h"
+#include "libm_atan.cuh"
 
 namespace aloam {
 
@@ -41,8 +43,9 @@ __device__ __forceinline__ bool point_ok(float x, float y, float z, float thres2
 
 // scanRegistration.cpp:166-205 ; returns -1 when the reference drops the return
 __device__ __forceinline__ int ring_of(float x, float y, float z, int n_scans) {
-  // :166 double atan / sqrt over float products, *180/M_PI in double, stored to float
-  float angle = (float)(atan((double)z / sqrt((double)(x * x + y * y))) * 180.0 / kPi);
+  // :166 double atan / sqrt over float products, *180/M_PI in double, stored to float; atan rounded as the host's libm
+  // rounds it wherever the float angle depends on it (libm_atan.cuh)
+  float angle = libm::elevation_deg(x, y, z);
   int id;
   if (n_scans == 16) {
     id = (int)((double)((angle + 15.0f) / 2.0f) + 0.5);
@@ -86,7 +89,7 @@ __device__ __forceinline__ void load_xyzw(const float* __restrict__ raw, int i, 
 
 // azimuth of a return before the halfPassed flip (:208-218)
 __device__ __forceinline__ float ori_first_half(float x, float y, float start_ori) {
-  float ori = -atan2f(y, x);
+  float ori = -libm::atan2f(y, x);
   if ((double)ori < (double)start_ori - kPi / 2) ori = (float)((double)ori + 2 * kPi);
   else if ((double)ori > (double)start_ori + kPi * 3 / 2) ori = (float)((double)ori - 2 * kPi);
   return ori;
@@ -129,7 +132,7 @@ __global__ void __launch_bounds__(CT) k_classify(const __grid_constant__ Batch<C
   float start_ori = 0.f;
   if (first != INT_MAX) {
     float x, y, z; load_xyz(raw, first, stride, x, y, z);
-    start_ori = -atan2f(y, x);  // :141
+    start_ori = -libm::atan2f(y, x);  // :141
   }
   int my_last = -1, my_half = INT_MAX;
 #pragma unroll
@@ -245,7 +248,7 @@ __global__ void __launch_bounds__(1024) k_ring_scan(const __grid_constant__ Batc
     if (sc->last_valid >= 0) {
       float x, y, z; load_xyz(raw, sc->last_valid, stride, x, y, z);
       const float start_ori = sc->start_ori;
-      end_ori = (float)((double)(-atan2f(y, x)) + 2 * kPi);  // :142-144
+      end_ori = (float)((double)(-libm::atan2f(y, x)) + 2 * kPi);  // :142-144
       if ((double)(end_ori - start_ori) > 3 * kPi) end_ori = (float)((double)end_ori - 2 * kPi);
       else if ((double)(end_ori - start_ori) < kPi) end_ori = (float)((double)end_ori + 2 * kPi);
     }
@@ -304,7 +307,7 @@ __global__ void __launch_bounds__(CT) k_scatter(const __grid_constant__ Batch<Sc
     if (i <= half_idx) {           // the flipping return itself still takes the first branch (:209-224)
       ori = ori_first_half(x, y, start_ori);
     } else {                       // :226-236
-      ori = (float)((double)(-atan2f(y, x)) + 2 * kPi);
+      ori = (float)((double)(-libm::atan2f(y, x)) + 2 * kPi);
       if ((double)ori < (double)end_ori - kPi * 3 / 2) ori = (float)((double)ori + 2 * kPi);
       else if ((double)ori > (double)end_ori + kPi / 2) ori = (float)((double)ori - 2 * kPi);
     }
