@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = [
     "aloam_lane_map_on_prior", "aloam_set_cube_growth",
     "aloam_io_unpack_points_ring",
     "aloam_create_wide",
+    "aloam_prior_map_digest", "aloam_lane_save_localising", "aloam_snapshot_localise_info",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -177,6 +178,9 @@ def lib():
         L.aloam_lane_save.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
         L.aloam_lane_restore.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
         L.aloam_snapshot_check.argtypes = [C.c_void_p, C.c_longlong, C.POINTER(SnapshotInfo)]
+        L.aloam_lane_save_localising.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
+        L.aloam_snapshot_localise_info.argtypes = [C.c_void_p, C.c_longlong, dp, C.POINTER(C.c_ulonglong), ip, C.POINTER(C.c_longlong)]
+        L.aloam_prior_map_digest.argtypes = [C.c_void_p, C.POINTER(C.c_ulonglong)]
         L.aloam_prior_map_load.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
         L.aloam_prior_map_clear.argtypes = [C.c_void_p]
         L.aloam_prior_map_build.argtypes = [C.c_void_p, cv, cv, ip, C.POINTER(C.c_longlong)]
@@ -240,12 +244,20 @@ def _blob(blob):
 
 def snapshot_info(blob):
     """checks a lane snapshot in host memory without a context or a GPU (aloam_snapshot_check) -> {version, mapped, n_scans,
-    scan_index, bytes, map_points, world}; raises AloamError(ERR_SNAPSHOT) when it is malformed"""
+    scan_index, bytes, map_points, world, localising}; a localising snapshot (format version 2) adds t_wmap_wodom (q xyzw, t),
+    map_digest, map_centre and map_points_prior (corner, surf) of the prior map it names (aloam_snapshot_localise_info).  Raises
+    AloamError(ERR_SNAPSHOT) when it is malformed"""
     ptr, n, keep = _blob(blob)
     info = SnapshotInfo()
     _check(lib().aloam_snapshot_check(ptr, n, C.byref(info)))
-    return {"version": info.version, "mapped": bool(info.mapped), "n_scans": info.n_scans, "scan_index": info.scan_index,
-            "bytes": info.bytes, "map_points": info.map_points, "world": np.array(info.world[:])}
+    out = {"version": info.version, "mapped": bool(info.mapped), "n_scans": info.n_scans, "scan_index": info.scan_index,
+           "bytes": info.bytes, "map_points": info.map_points, "world": np.array(info.world[:]), "localising": info.version == 2}
+    if out["localising"]:
+        t, digest, centre, points = (C.c_double * 7)(), C.c_ulonglong(0), (C.c_int * 3)(), (C.c_longlong * 2)()
+        _check(lib().aloam_snapshot_localise_info(ptr, n, t, C.byref(digest), centre, points))
+        out.update({"t_wmap_wodom": np.array(t[:]), "map_digest": int(digest.value), "map_centre": tuple(centre[:]),
+                    "map_points_prior": (int(points[0]), int(points[1]))})
+    return out
 
 
 def _cloud_view(a):
@@ -699,6 +711,20 @@ class Aloam:
         _check(lib().aloam_lane_save(self._h, int(lane), C.c_void_p(out.data_ptr()), out.numel(), C.byref(n)))
         return out.view(-1)[:n.value]
 
+    def lane_save_localising(self, lane, out=None):
+        """snapshot of the localising trajectory `lane` runs (aloam_lane_save_localising, format version 2: its odometry, its
+        T_wmap_wodom and the name of its prior map); `out` and the return value as for lane_save"""
+        n = C.c_longlong(0)
+        if out is None:
+            _check(lib().aloam_lane_save_localising(self._h, int(lane), None, 0, C.byref(n)))
+            arr = np.zeros(max(n.value, 1), np.uint8)
+            _check(lib().aloam_lane_save_localising(self._h, int(lane), arr.ctypes.data, arr.size, C.byref(n)))
+            return arr[:n.value]
+        if out.element_size() != 1 or not out.is_contiguous():
+            raise ValueError("out is a contiguous uint8 tensor")
+        _check(lib().aloam_lane_save_localising(self._h, int(lane), C.c_void_p(out.data_ptr()), out.numel(), C.byref(n)))
+        return out.view(-1)[:n.value]
+
     def lane_restore(self, lane, blob):
         """makes `lane` run the trajectory of a snapshot (aloam_lane_restore): a numpy array, bytes, or a torch tensor"""
         ptr, n, keep = _blob(blob)
@@ -725,6 +751,13 @@ class Aloam:
 
     def prior_map_clear(self):
         _check(lib().aloam_prior_map_clear(self._h))
+
+    def prior_map_digest(self):
+        """the 64-bit digest of the prior map (aloam_prior_map_digest; include/aloam_b200.h gives the formula), computed on the
+        device on first use and kept with the map"""
+        d = C.c_ulonglong(0)
+        _check(lib().aloam_prior_map_digest(self._h, C.byref(d)))
+        return int(d.value)
 
     def lane_localise(self, lane, q_init, t_init):
         """arms `lane`: its next LANE_START in a mapped scan_stream_lanes call begins a trajectory that registers against the

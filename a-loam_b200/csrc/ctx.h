@@ -211,6 +211,7 @@ struct PinnedScratch {
   double mapper_pose_in[7], mapper_pose_out[7];
   SnapHeader snap;          // aloam_lane_save / _restore: the snapshot's header
   int snap_counts[4];       //                             counts of the lane's "last" feature set
+  SnapLocalise snap_loc;    // aloam_lane_save_localising / _restore: the locator section of a format-2 snapshot
 };
 
 }  // namespace
@@ -343,11 +344,13 @@ namespace {
 
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
-       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE, KID_RECOVER_CAND, KID_RECOVER_ADOPT };
+       KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE, KID_RECOVER_CAND, KID_RECOVER_ADOPT,
+       KID_PRIOR_DIGEST };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
-    "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score", "k_recover_cand", "k_recover_adopt"};
+    "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score", "k_recover_cand", "k_recover_adopt",
+    "k_prior_digest"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -480,6 +483,14 @@ void mapper_run_orders(const aloam_ctx* c, bool growth, int ord[2]);
 int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head, int* growth);
 int mapper_store_points(aloam_ctx* c, int lane, long long n, char* dst, bool device);
 int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const char* pts, bool device, bool growth);
+// cubemap.cu: what names the context's prior map in a localising snapshot -- its centre offsets, its points per type and its
+// digest (aloam_prior_map_digest: computed on the first call, then kept with the map).  ALOAM_ERR_STATE without a prior map.
+int prior_map_identity(aloam_ctx* c, int cen[3], long long n[2], unsigned long long* digest);
+// cubemap.cu: the T_wmap_wodom of lane `lane`'s locator (it exists) into dst[7] (host memory: q xyzw, t), on c->stream, not
+// synchronised; and the locator's frame state set to what a fresh localising START leaves before its first frame, with
+// T_wmap_wodom = T[7] and the prior map's centre offsets (it exists), on c->stream
+int locator_map_pose(aloam_ctx* c, int lane, double* dst);
+int locator_restore(aloam_ctx* c, int lane, const double T[7]);
 int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf);
 int ensure_map_buffers(aloam_ctx* c);
 int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids = true);

@@ -120,6 +120,10 @@ struct aloam::PriorMap {
   // per type, from the cube table: the largest cube, the cubes that hold points and the slabs their runs take with cube growth
   // on -- whether a lane store can hold a copy of the map (aloam_lane_map_on_prior)
   int max_cube[2] = {0, 0}, n_cubes[2] = {0, 0}, run_slabs[2] = {0, 0};
+  // aloam_prior_map_digest: computed by the first call that needs it (k_prior_digest), kept until the map is released
+  bool have_digest = false;
+  unsigned long long digest = 0;
+  unsigned long long* d_digest = nullptr;
 };
 // what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
 // k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
@@ -387,6 +391,61 @@ __global__ void __launch_bounds__(256) k_locate_begin(const __grid_constant__ Ba
     for (int w = 0; w < ALOAM_WINDOW_CUBES; ++w)
       if (s_cnt[0][w] >= 0) S->valid[nv++] = cube_index(s_ctr[0] - 2 + w / 15, s_ctr[1] - 2 + (w / 3) % 5, s_ctr[2] - 1 + w % 3);
     S->n_valid = nv;
+  }
+}
+
+// grid (1), 256 threads, after a memset of the state: the frame state of a localising lane restored from a format-2 snapshot
+// (aloam_lane_restore) -- what a fresh localising START leaves before its first frame (k_locate_begin with `fresh`), with the
+// saved T_wmap_wodom and the prior map's centre offsets.  A later frame reads only T_wmap_wodom of it; everything else it
+// rewrites before reading.
+struct Pose7 { double v[7]; };
+__global__ void __launch_bounds__(256) k_locate_restore(MapperState* S, const __grid_constant__ Pose7 T, int cen0, int cen1, int cen2) {
+  mapper_fresh_state(S, 0, 0);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < 4; ++k) S->q_wmap_wodom[k] = T.v[k];
+    for (int k = 0; k < 3; ++k) S->t_wmap_wodom[k] = T.v[4 + k];
+    S->cen[0] = cen0; S->cen[1] = cen1; S->cen[2] = cen2;
+  }
+}
+
+// the digest of a prior map (aloam_prior_map_digest, include/aloam_b200.h): sum over k of mix(k, w_k) mod 2^64 for the word
+// sequence w = the three centre offsets, the cube-start tables cs[2][NCUBE + 1] (corner, then surf), the corner points, the surf
+// points (4 float bit patterns each, packed cube order); every word a 32-bit pattern, zero-extended.  mix: splitmix64's finaliser
+// of (k * golden gamma) ^ w.  Integer addition: the sum does not depend on how the words are split over threads.
+__host__ __device__ inline unsigned long long digest_mix(unsigned long long k, unsigned w) {
+  unsigned long long z = (k * 0x9E3779B97F4A7C15ull) ^ w;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+constexpr int kDigestThreads = 256;
+constexpr int kDigestHead = 3 + 2 * (NCUBE + 1);   // words before the points
+// grid-stride over the words, one 16-byte load per point; a warp-shuffle and shared-memory sum per CTA, one atomicAdd per CTA into
+// *out (zeroed before)
+__global__ void __launch_bounds__(kDigestThreads) k_prior_digest(int cen0, int cen1, int cen2, const int* __restrict__ cs, const float4* __restrict__ p0,
+                                                                 int n0, const float4* __restrict__ p1, int n1, unsigned long long* __restrict__ out) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  unsigned long long s = 0;
+  for (long long k = tid; k < kDigestHead; k += nt) {
+    const unsigned w = k == 0 ? (unsigned)cen0 : k == 1 ? (unsigned)cen1 : k == 2 ? (unsigned)cen2 : (unsigned)__ldg(cs + (k - 3));
+    s += digest_mix((unsigned long long)k, w);
+  }
+  const long long n = (long long)n0 + n1;
+  for (long long i = tid; i < n; i += nt) {
+    const float4 q = i < n0 ? __ldg(p0 + i) : __ldg(p1 + (i - n0));
+    const unsigned long long k = kDigestHead + 4ull * (unsigned long long)i;
+    s += digest_mix(k, __float_as_uint(q.x)) + digest_mix(k + 1, __float_as_uint(q.y)) + digest_mix(k + 2, __float_as_uint(q.z)) +
+         digest_mix(k + 3, __float_as_uint(q.w));
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  __shared__ unsigned long long ws[kDigestThreads / 32];
+  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    s = threadIdx.x < kDigestThreads / 32 ? ws[threadIdx.x] : 0ull;
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) atomicAdd(out, s);
   }
 }
 
@@ -1010,7 +1069,7 @@ int store_copy(aloam_ctx* c, const ExportLayout* L, long long n, char* mem, bool
 void prior_free(PriorMap* p) {
   if (!p) return;
   for (int t = 0; t < 2; ++t) { cudaFree(p->pts[t]); cudaFree(p->grid[t].slots); cudaFree(p->grid[t].dyn); cudaFree(p->grid[t].gpts); }
-  cudaFree(p->d_cube_start); cudaFree(p->d_n); cudaFree(p->d_layout);
+  cudaFree(p->d_cube_start); cudaFree(p->d_n); cudaFree(p->d_layout); cudaFree(p->d_digest);
   delete p;
 }
 // the one place a context's prior map is released: aloam_prior_map_clear, a load that replaces it, aloam_destroy
@@ -1763,6 +1822,55 @@ int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps) {
   return ALOAM_OK;
 }
 
+// the digest of the context's prior map (it exists): on the first call one k_prior_digest launch over the whole map and one
+// synchronisation, then the value kept with the map
+static int prior_map_digest(aloam_ctx* c, unsigned long long* out) {
+  PriorMap* P = c->prior;
+  if (!P->have_digest) {
+    if (!P->d_digest && cudaMalloc(&P->d_digest, sizeof(unsigned long long)) != cudaSuccess) { cudaGetLastError(); P->d_digest = nullptr; return ALOAM_ERR_CUDA; }
+    const long long n = (long long)P->n[0] + P->n[1];
+    const int blocks = (int)std::max<long long>(1, std::min<long long>((n + kDigestThreads - 1) / kDigestThreads, (long long)c->sms * 8));
+    CUDA_CHECK_RET(cudaMemsetAsync(P->d_digest, 0, sizeof(unsigned long long), c->stream));
+    LAUNCH(c, KID_PRIOR_DIGEST, k_prior_digest, blocks, kDigestThreads, 0, P->cen[0], P->cen[1], P->cen[2], (const int*)P->d_cube_start,
+           reinterpret_cast<const float4*>(P->pts[0]), P->n[0], reinterpret_cast<const float4*>(P->pts[1]), P->n[1], P->d_digest);
+    unsigned long long d = 0;
+    CUDA_CHECK_RET(cudaMemcpyAsync(&d, P->d_digest, sizeof(d), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+    CUDA_CHECK_RET(cudaGetLastError());
+    prof_collect(c);
+    P->digest = d;
+    P->have_digest = true;
+  }
+  *out = P->digest;
+  return ALOAM_OK;
+}
+
+int prior_map_identity(aloam_ctx* c, int cen[3], long long n[2], unsigned long long* digest) {
+  const PriorMap* P = c->prior;
+  if (!P) return ALOAM_ERR_STATE;
+  for (int a = 0; a < 3; ++a) cen[a] = P->cen[a];
+  for (int t = 0; t < 2; ++t) n[t] = P->n[t];
+  return prior_map_digest(c, digest);
+}
+
+int locator_map_pose(aloam_ctx* c, int lane, double* dst) {
+  const MapperState* S = c->lanes[lane].locator->d_state;
+  CUDA_CHECK_RET(cudaMemcpyAsync(dst, S->q_wmap_wodom, 4 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(dst + 4, S->t_wmap_wodom, 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  return ALOAM_OK;
+}
+
+int locator_restore(aloam_ctx* c, int lane, const double T[7]) {
+  const PriorMap* P = c->prior;
+  MapperState* S = c->lanes[lane].locator->d_state;
+  Pose7 p;
+  for (int k = 0; k < 7; ++k) p.v[k] = T[k];
+  CUDA_CHECK_RET(cudaMemsetAsync(S, 0, sizeof(MapperState), c->stream));
+  LAUNCH(c, KID_CUBES, k_locate_restore, 1, 256, 0, S, p, P->cen[0], P->cen[1], P->cen[2]);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return ALOAM_OK;
+}
+
 extern "C" {
 
 int aloam_prior_map_load(aloam_ctx* c, const void* blob, long long n_bytes) {
@@ -1842,6 +1950,13 @@ int aloam_prior_map_build(aloam_ctx* c, aloam_cloud_view corner, aloam_cloud_vie
   if (rc) return rc;
   if (dropped) { dropped[0] = drop[0]; dropped[1] = drop[1]; }
   return ALOAM_OK;
+}
+
+int aloam_prior_map_digest(aloam_ctx* c, unsigned long long* out) {
+  if (!c || !out) return ALOAM_ERR_INVALID_ARG;
+  if (!c->prior) return ALOAM_ERR_STATE;
+  CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
+  return prior_map_digest(c, out);
 }
 
 int aloam_prior_map_clear(aloam_ctx* c) {

@@ -1,5 +1,6 @@
-// Internal: lane snapshot format v1 (aloam_lane_save / aloam_lane_restore / aloam_snapshot_check), shared by snapshot.cu and
-// cubemap.cu.  include/aloam_b200.h documents the same layout for callers: little-endian, every section 16-byte aligned.
+// Internal: lane snapshot formats v1 (aloam_lane_save / aloam_lane_restore / aloam_snapshot_check) and v2 (a localising lane:
+// aloam_lane_save_localising), shared by snapshot.cu and cubemap.cu.  include/aloam_b200.h documents the same layouts for callers:
+// little-endian, every section 16-byte aligned.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -7,6 +8,7 @@
 namespace aloam {
 
 constexpr int kSnapVersion = 1;
+constexpr int kSnapVersionLocalise = 2;   // the v1 header (mapped 0, cube_growth 0), the "last" clouds, then SnapLocalise
 constexpr int kSnapCubes = 4851;   // 21 x 21 x 11 cubes of the mapper's ring buffer
 constexpr int kSnapValid = 128;
 constexpr int kSnapPool = 1024;    // slabs per cloud type: the runs of a type's cubes take at most this many
@@ -51,5 +53,18 @@ struct SnapStore {
 static_assert(sizeof(SnapStore) == 39424, "snapshot store table");
 static_assert(offsetof(SnapStore, frames) == 528 && offsetof(SnapStore, q_wmap_wodom) == 536 && offsetof(SnapStore, count) == 592 &&
               offsetof(SnapStore, n_points) == 39408, "snapshot store table layout");
+
+// section 3 of a format-2 snapshot (a localising lane), at S = 256 + 16 (n_less_sharp + n_less_flat): the lane's T_wmap_wodom
+// and what names the prior map it localises against
+struct SnapLocalise {
+  double q_wmap_wodom[4], t_wmap_wodom[3];
+  uint64_t digest;                     // aloam_prior_map_digest of the map
+  int32_t centre[3], zero0;            // its centre offsets
+  int64_t map_points[2];               // its corner / surf points
+  char zero1[32];
+};
+static_assert(sizeof(SnapLocalise) == 128, "localising snapshot section");
+static_assert(offsetof(SnapLocalise, t_wmap_wodom) == 32 && offsetof(SnapLocalise, digest) == 56 && offsetof(SnapLocalise, centre) == 64 &&
+              offsetof(SnapLocalise, map_points) == 80, "localising snapshot section layout");
 
 }  // namespace aloam

@@ -353,15 +353,50 @@ int aloam_reset_odometry(aloam_ctx* ctx); /* forget pose, warm start and "last" 
  *      S+39400 zero   S+39408 int64 n_points (the sum of the counts >= 0)   S+39416 zero
  *      S+39424 n_points points of 4 floats in ALOAM_EXPORT_MAP order: corner cube i, then surf cube i, for i = 0 .. 4850
  *   total_bytes = S, or S + 39424 + 16 n_points for a mapped snapshot.  Which slabs a cube held is not saved: only which cubes hold
- *   a run, and the points, change results. */
+ *   a run, and the points, change results.
+ *
+ * Snapshot format, version 2 -- a LOCALISING lane (aloam_lane_save_localising), which owns no cube store: the trajectory's state
+ * is its odometry and its T_wmap_wodom, and it depends on a prior map the snapshot does not hold but names.
+ *   1. the header of version 1 with version = 2, mapped = 0 and cube_growth = 0 (magic "ALOAMLS1"; the configuration fields as
+ *      version 1 writes them)
+ *   2. at 256: the "last" clouds, as version 1
+ *   3. at S = 256 + 16 (n_less_sharp + n_less_flat), 128 bytes:
+ *      S+0 double q_wmap_wodom[4]   S+32 double t_wmap_wodom[3] (the lane's T_wmap_wodom after its last registered scan and any
+ *      recovery it adopted)   S+56 uint64 digest (aloam_prior_map_digest of the map)   S+64 int32 centre[3] (its centre offsets)
+ *      S+76 zero   S+80 int64 map_points[2] (its corner / surf points)   S+96 zero to S+128
+ *   total_bytes = S + 128.
+ * aloam_lane_restore of a version-2 snapshot ends the lane first, as for version 1, then: ALOAM_ERR_STATE without a prior map (and,
+ * as for version 1, on a rank of a sharded job or an emulating context); ALOAM_ERR_SNAPSHOT for the version-1 header checks, a size
+ * other than S + 128, mapped or cube_growth not 0, a non-finite T_wmap_wodom or a zero quaternion, a centre offset outside
+ * -2^20 .. 2^20, a negative point count, a map position T_wmap_wodom * world (translation) whose (x + 25.0) / 50.0 is not finite or
+ * lies beyond int (or whose centre cube int((x + 25.0) / 50.0) + centre[a] does), cfg.max_map_points = 0, a configuration that
+ * differs -- the odometry fields of version 1 and line_res, plane_res and mapping_skip_frame; the slab capacities and
+ * max_map_points do not count --, and a map whose centre offsets, point counts or digest differ from the context's prior map.
+ * ALOAM_ERR_CAPACITY / ALOAM_ERR_NOT_RING_MAJOR for the "last" clouds as for version 1; ALOAM_ERR_CUDA when the lane's locator cannot
+ * be created (created if needed, as at a localising START).  On success the lane runs a localising trajectory at the saved scan
+ * index, its frame state that of a fresh localising START with the saved T_wmap_wodom; a mapped lanes call that continues it with
+ * ALOAM_LANE_SCAN gives exactly what the uninterrupted trajectory would have (odometry and map poses, row records and scores,
+ * recovery, registered clouds).  The lane's arming is left alone, and aloam_prior_map_load / _build / _clear are refused while it
+ * localises, as for any localising lane.  aloam_snapshot_check accepts a well-formed version-2 snapshot (info->version = 2,
+ * mapped = 0, map_points = 0); aloam_prior_map_load refuses it with ALOAM_ERR_SNAPSHOT (it holds no store).
+ * aloam_lane_save_localising writes the version-2 snapshot of a localising lane under the buffer rules of aloam_lane_save
+ * (device, pinned or pageable memory; out = NULL with capacity = 0 for the size; ALOAM_ERR_CAPACITY).  ALOAM_ERR_STATE unless the
+ * context runs lanes and `lane` runs a localising trajectory; aloam_lane_save of a localising lane stays ALOAM_ERR_STATE.  The
+ * first save (or restore) against a map computes the map's digest (one launch over the map, one synchronisation).
+ * aloam_snapshot_localise_info describes a version-2 snapshot in host memory without a context or a GPU, after the checks of
+ * aloam_snapshot_check: t_wmap_wodom (q xyzw, t), the digest, centre offsets and point counts of its map (each output may be NULL).
+ * ALOAM_ERR_SNAPSHOT for anything but a well-formed version-2 snapshot. */
 typedef struct aloam_snapshot_info {
   int version, mapped, n_scans, scan_index;
   long long bytes, map_points;
   double world[7];
 } aloam_snapshot_info;
 int aloam_lane_save(aloam_ctx* ctx, int lane, void* out, long long capacity, long long* n_bytes);
+int aloam_lane_save_localising(aloam_ctx* ctx, int lane, void* out, long long capacity, long long* n_bytes);
 int aloam_lane_restore(aloam_ctx* ctx, int lane, const void* blob, long long n_bytes);
 int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapshot_info* info);
+int aloam_snapshot_localise_info(const void* host_blob, long long n_bytes, double t_wmap_wodom[7], unsigned long long* digest, int centre[3],
+                                 long long map_points[2]);
 
 /* ---- localisation against a prior map: vehicles register their scans against ONE saved map that no frame changes.
  * aloam_prior_map_load makes the cube store of a MAPPED lane snapshot (format v1; blob in device, pinned or pageable memory, as
@@ -401,7 +436,10 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  * its frame state, 5-NN records and residual blocks for 2 x cfg.max_points queries, the two filtered stacks and the stack filter's
  * sort buffers -- about 450 B per point of cfg.max_points, 0.18 GB at 400 000 and 27 MB at 60 000 (arithmetic from the buffer
  * sizes, not measured), against about 1.75 GB for a mapping lane -- and no cube store if the lane never maps.
- * Limits, each ALOAM_ERR_STATE: aloam_lane_save of a localising lane (snapshot format v1 has no section for it); sharded jobs.
+ * A localising lane is suspended and resumed with aloam_lane_save_localising / aloam_lane_restore (snapshot format version 2,
+ * above): its snapshot names the prior map by centre offsets, point counts and digest, and restores only against that map.
+ * Limits, each ALOAM_ERR_STATE: aloam_lane_save of a localising lane (format version 1 has no section for it: use
+ * aloam_lane_save_localising); sharded jobs.
  * The lockstep stream calls and aloam_mapper_step never localise.
  *
  * aloam_prior_map_build makes the prior map from two clouds in the MAP frame (the frame of aloam_lane_localise's q_init / t_init):
@@ -427,6 +465,18 @@ int aloam_snapshot_check(const void* host_blob, long long n_bytes, aloam_snapsho
  *   - state rules are aloam_prior_map_load's: ALOAM_ERR_STATE while any lane is localising, on a rank of a sharded job and on an
  *     emulating context; the new map is built beside the old one, which is replaced only on success; armings survive;
  *     aloam_prior_map_clear and aloam_destroy release it.  Two host synchronisations: one to learn the map's sizes, one at the end. */
+/* aloam_prior_map_digest: a 64-bit digest of everything a localising frame reads of the context's prior map, which localising
+ * snapshots (format version 2) carry to name their map.  Words w_k, each a 32-bit pattern zero-extended to 64 bits: the three centre
+ * offsets; both types' cube-start tables cs[t][0 .. 4851] (cube i of type t holds the packed points cs[t][i] .. cs[t][i + 1] - 1;
+ * corner table, then surf table); the corner points, then the surf points, 4 float bit patterns each (x, y, z, intensity), in the
+ * packed cube order of the ALOAM_EXPORT_MAP export.  digest = sum over k of mix(k, w_k) mod 2^64, with
+ *   mix(k, w) = f(k * 0x9E3779B97F4A7C15 ^ w) mod 2^64,  f(z) = splitmix64's finaliser:
+ *   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  f = z ^ (z >> 31).
+ * Maps loaded or built from the same store agree on it; a changed point bit, cube count or centre offset changes it (up to
+ * collisions of a 64-bit sum).  Computed on the device by the first call that needs it (this call, or a localising save or
+ * restore: one launch over the map and one synchronisation), then kept with the map; aloam_prior_map_load and _build issue no
+ * digest launch.  ALOAM_ERR_STATE without a prior map. */
+int aloam_prior_map_digest(aloam_ctx* ctx, unsigned long long* out);
 #define ALOAM_PRIOR_MAP (-1)
 int aloam_prior_map_load(aloam_ctx* ctx, const void* blob, long long n_bytes);
 int aloam_prior_map_build(aloam_ctx* ctx, aloam_cloud_view corner_map, aloam_cloud_view surf_map, const int centre[3], long long dropped[2]);
