@@ -35,6 +35,8 @@ EXPORTED_SYMBOLS = [
     "aloam_io_unpack_points_ring",
     "aloam_create_wide",
     "aloam_prior_map_digest", "aloam_lane_save_localising", "aloam_snapshot_localise_info",
+    "aloam_set_place", "aloam_place_rows", "aloam_place_keyframes", "aloam_place_db_load", "aloam_place_db_clear",
+    "aloam_place_describe", "aloam_place_query",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -44,6 +46,12 @@ ROW_IDLE, ROW_MAPPED, ROW_LOCALISED, ROW_SKIPPED = 0, 1, 2, 3   # aloam_map_row.
 RING_ELEVATION, RING_FIELD = 0, 1   # aloam_config.ring_source: the elevation formula, or the driver's ring in float 3 of a raw point
 MAX_RINGS = 128   # ALOAM_MAX_RINGS: the most rings a context takes (Aloam(..., wide=True), driver rings only)
 MAX_CUBE_POINTS = 262144   # ALOAM_MAX_CUBE_POINTS: the most points one map cube holds with cube growth on (set_cube_growth)
+PLACE_RINGS, PLACE_SECTORS, PLACE_MAX_K = 20, 60, 64   # the Scan Context grid and the most matches a query returns
+# one keyframe record (ALOAM_PLACE_RECORD_BYTES, little-endian): the row's map pose (q xyzw, t), its scan index in its trajectory,
+# its lane, the descriptor parameters and the ring-major descriptor
+PLACE_RECORD_DTYPE = np.dtype([("pose", "<f8", (7,)), ("scan_index", "<i4"), ("lane", "<i4"), ("max_range", "<f4"), ("z_offset", "<f4"),
+                               ("pad", "<i4", (2,)), ("desc", "<f4", (PLACE_RINGS * PLACE_SECTORS,))])
+assert PLACE_RECORD_DTYPE.itemsize == 4880, "aloam place record layout"
 
 
 class Config(C.Structure):
@@ -106,6 +114,19 @@ class RecoveryOpts(C.Structure):
 
 class RecoveryRow(C.Structure):
     _fields_ = [("triggered", C.c_int), ("best", C.c_int), ("best_score", C.c_int), ("adopted", C.c_int), ("pose", C.c_double * 7)]
+
+
+class PlaceOpts(C.Structure):
+    _fields_ = [("max_range", C.c_float), ("z_offset", C.c_float), ("keyframe_gap", C.c_double), ("exclude_recent", C.c_int),
+                ("max_keyframes", C.c_int)]
+
+
+class PlaceRow(C.Structure):
+    _fields_ = [("keyframe", C.c_int), ("loop", C.c_int), ("shift", C.c_int), ("full", C.c_int), ("distance", C.c_double)]
+
+
+class PlaceMatch(C.Structure):
+    _fields_ = [("keyframe", C.c_int), ("shift", C.c_int), ("distance", C.c_double)]
 
 
 class AloamError(RuntimeError):
@@ -194,6 +215,13 @@ def lib():
         L.aloam_set_recovery.argtypes = [C.c_void_p, C.c_int, C.POINTER(RecoveryOpts), dp, C.c_int]
         L.aloam_recovery_rows.argtypes = [C.c_void_p, C.POINTER(RecoveryRow), C.c_int]
         L.aloam_debug_recovery_scores.argtypes = [C.c_void_p, C.c_int, ip, C.c_int]
+        L.aloam_set_place.argtypes = [C.c_void_p, C.c_int, C.POINTER(PlaceOpts)]
+        L.aloam_place_rows.argtypes = [C.c_void_p, C.POINTER(PlaceRow), C.c_int]
+        L.aloam_place_keyframes.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
+        L.aloam_place_db_load.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        L.aloam_place_db_clear.argtypes = [C.c_void_p]
+        L.aloam_place_describe.argtypes = [C.c_void_p, cv, cv, C.c_void_p]
+        L.aloam_place_query.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(PlaceMatch)]
         _LIB = L
     return _LIB
 
@@ -313,6 +341,27 @@ def pose_grid(q_base, t_centre, half_extent_xy, step_xy, yaws):
     out[:, 5] = np.repeat(t0[1] + gy.ravel(), len(yaws))
     out[:, 6] = t0[2]
     return out
+
+
+def place_hypotheses(matches, records, half_extent_xy, step_xy, yaw_half, yaw_step):
+    """relocalisation hypotheses from place matches: for every match (a dict or structured array with keyframe and shift, as
+    Aloam.place_query returns) a pose_grid around q_kf * Rz(shift * 2 pi / 60), t_kf of its keyframe record (records: a
+    PLACE_RECORD_DTYPE array, the database the query ran against), with headings yaw_half apart at most in steps of yaw_step
+    (radians) -> (n, 7) float64, ready for Aloam.prior_relocalise"""
+    kf = np.atleast_1d(np.asarray(matches["keyframe"])).ravel()
+    sh = np.atleast_1d(np.asarray(matches["shift"])).ravel()
+    k = int(np.floor(yaw_half / yaw_step + 1e-9)) if yaw_step > 0 else 0
+    yaws = np.arange(-k, k + 1) * float(yaw_step)
+    out = []
+    for j, s in zip(kf, sh):
+        if j < 0:
+            continue
+        x, y, z, w = records["pose"][int(j)][:4]
+        a = float(s) * 2.0 * np.pi / PLACE_SECTORS
+        sz, cz = np.sin(a / 2), np.cos(a / 2)   # q_kf * (0, 0, sz, cz)
+        q = np.array([x * cz + y * sz, y * cz - x * sz, z * cz + w * sz, w * cz - z * sz])
+        out.append(pose_grid(q, records["pose"][int(j)][4:], half_extent_xy, step_xy, yaws))
+    return np.concatenate(out) if out else np.zeros((0, 7))
 
 
 def default_config(n_scans):
@@ -804,6 +853,64 @@ class Aloam:
         res = [{"hyp": r.hyp, "score": r.score, "refined_score": r.refined_score, "flags": r.flags, "pose": np.array(r.pose[:])}
                for r in out[:int(refine)]]
         return res, (sc[:h.shape[0]] if scores else None)
+
+    # --- place recognition (Scan Context)
+    def set_place(self, on=True, max_range=80.0, z_offset=2.0, keyframe_gap=0.0, exclude_recent=0, max_keyframes=4096):
+        """sets the descriptor parameters and turns keyframe recording of the mapped stream calls on or off (aloam_set_place); every
+        call clears every lane's keyframe table"""
+        o = PlaceOpts(float(max_range), float(z_offset), float(keyframe_gap), int(exclude_recent), int(max_keyframes))
+        _check(lib().aloam_set_place(self._h, int(on), C.byref(o)))
+
+    def place_describe(self, less_sharp=None, less_flat=None, raw=None):
+        """the (1200,) float32 Scan Context descriptor of one scan (ring-major), from its less_sharp / less_flat clouds or from a raw
+        scan whose features are extracted first"""
+        if raw is not None:
+            f = self.extract_features(raw)
+            less_sharp, less_flat = f["less_sharp"], f["less_flat"]
+        a, ka = _view(less_sharp)
+        b, kb = _view(less_flat)
+        out = np.zeros(PLACE_RINGS * PLACE_SECTORS, np.float32)
+        _check(lib().aloam_place_describe(self._h, a, b, C.c_void_p(out.ctypes.data)))
+        return out
+
+    def place_keyframes(self, lane=0):
+        """lane `lane`'s keyframe records (aloam_place_keyframes) as a PLACE_RECORD_DTYPE array"""
+        n = C.c_longlong(0)
+        _check(lib().aloam_place_keyframes(self._h, int(lane), None, 0, C.byref(n)))
+        out = np.zeros(max(n.value, 1), PLACE_RECORD_DTYPE)
+        _check(lib().aloam_place_keyframes(self._h, int(lane), C.c_void_p(out.ctypes.data), out.shape[0], C.byref(n)))
+        return out[:n.value]
+
+    def place_db_load(self, records):
+        """makes `records` (a PLACE_RECORD_DTYPE array, or raw bytes of concatenated records) the context's database"""
+        r = np.ascontiguousarray(records if isinstance(records, np.ndarray) else np.frombuffer(records, np.uint8))
+        if r.nbytes % 4880:
+            raise ValueError("records are 4880 bytes each")
+        _check(lib().aloam_place_db_load(self._h, C.c_void_p(r.ctypes.data), r.nbytes // 4880))
+
+    def place_db_clear(self):
+        _check(lib().aloam_place_db_clear(self._h))
+
+    def place_query(self, descs, k=1):
+        """the k best database keyframes of every descriptor of descs ((n, 1200) float32) -> dict of (n, k) arrays keyframe,
+        shift, distance"""
+        d = np.ascontiguousarray(descs, np.float32).reshape(-1, PLACE_RINGS * PLACE_SECTORS)
+        out = (PlaceMatch * (d.shape[0] * int(k)))()
+        _check(lib().aloam_place_query(self._h, C.c_void_p(d.ctypes.data), d.shape[0], int(k), out))
+        n = d.shape[0]
+        return {"keyframe": np.array([m.keyframe for m in out], np.int32).reshape(n, k),
+                "shift": np.array([m.shift for m in out], np.int32).reshape(n, k),
+                "distance": np.array([m.distance for m in out], np.float64).reshape(n, k)}
+
+    def place_rows(self, rows):
+        """the place rows of the `rows` = n_scans x batch rows (scan-major) of the last mapped stream call (aloam_place_rows) -> dict
+        of (rows,) arrays keyframe, loop, shift, full (-1 where there is none) and distance (-1.0)"""
+        out = (PlaceRow * max(int(rows), 1))()
+        _check(lib().aloam_place_rows(self._h, out, int(rows)))
+        out = out[:int(rows)]
+        d = {k: np.array([getattr(r, k) for r in out], np.int32) for k in ("keyframe", "loop", "shift", "full")}
+        d["distance"] = np.array([r.distance for r in out], np.float64)
+        return d
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

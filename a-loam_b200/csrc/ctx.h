@@ -95,6 +95,7 @@ struct Locator;        // cubemap.cu: the frame state and registration buffers o
 struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexed
 struct Relocaliser;    // reloc.cu: the scratch of aloam_prior_relocalise
 struct Recovery;       // recover.cu: the setting and buffers of aloam_set_recovery
+struct Place;          // place.cu: the keyframe tables, database and scratch of place recognition (aloam_set_place)
 }  // namespace aloam
 
 using namespace aloam;
@@ -139,6 +140,7 @@ struct MappedCall {
   bool registered = false;       // aloam_registered_rows may read the table and reg_count
   bool records = false;          // aloam_map_rows and aloam_recovery_rows may read the table and the pinned row table h_rows
   bool recovered = false;        // the call ran recovery (aloam_set_recovery)
+  bool places = false;           // aloam_place_rows may read the table and the pinned place rows (the call recorded keyframes)
   // a reader's check: ALOAM_ERR_STATE while its flag is off, ALOAM_ERR_INVALID_ARG for a row count other than the call's
   int check(bool readable, int rows) const { return !readable ? ALOAM_ERR_STATE : rows != n_scans * nb ? ALOAM_ERR_INVALID_ARG : ALOAM_OK; }
 };
@@ -286,6 +288,10 @@ struct aloam_ctx {
   // recovery of localising lanes (aloam_set_recovery, recover.cu): on only while rows are scored; its buffers, created on first use
   bool rec_on = false;
   Recovery* recover = nullptr;
+  // place recognition (aloam_set_place, place.cu): keyframes recorded by the mapped stream calls while place_on; the tables,
+  // database and scratch, created on first use
+  bool place_on = false;
+  Place* place = nullptr;
   MappedCall last_mapped;   // the rows of the last mapped stream call and which of its readers may read them
   // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
   // memory, created on first use
@@ -345,12 +351,12 @@ namespace {
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
        KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE, KID_RECOVER_CAND, KID_RECOVER_ADOPT,
-       KID_PRIOR_DIGEST };
+       KID_PRIOR_DIGEST, KID_PLACE_GATE, KID_PLACE_DIST, KID_PLACE_BEST };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
     "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score", "k_recover_cand", "k_recover_adopt",
-    "k_prior_digest"};
+    "k_prior_digest", "k_place_gate(describe)", "k_place_dist", "k_place_best"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -425,6 +431,13 @@ int reloc_score_ctas(aloam_ctx* c, int n_hyp);
 int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows);
 int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, const double* const* cand,
                          const unsigned long long* const* best, float accept_frac);
+// place recognition (place.cu): after the mapping frame of nb records just issued, the keyframe gate, descriptor and loop query of
+// each (scan[l]: its scan index, start[l]: it STARTs a trajectory, which clears its lane's table first; rows[l]: its place row);
+// and the clearing of lane `lane`'s table (-1: every lane), on c->stream
+int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows);
+int place_clear(aloam_ctx* c, int lane);
+aloam_place_row* place_rows_device(aloam_ctx* c);
+aloam_place_row* place_rows_host(aloam_ctx* c);
 // which lanes' candidate scores belong to a triggered row of the last mapped stream call (recover.cu; none while its records
 // cannot be read or it ran no recovery)
 void recover_call_done(aloam_ctx* c);

@@ -20,7 +20,7 @@
 
 #ifdef __CUDACC__
 #define LIBM_HD __host__ __device__ __forceinline__
-#define LIBM_HD_NOINLINE __host__ __device__ __noinline__
+#define LIBM_HD_NOINLINE static __host__ __device__ __noinline__   // internal linkage: several translation units include this header
 #else
 #define LIBM_HD inline
 #define LIBM_HD_NOINLINE inline

@@ -359,6 +359,7 @@ int aloam_lane_restore(aloam_ctx* c, int lane, const void* blob, long long n_byt
   Lane& L = c->lanes[lane];
   c->lanes_mode = true;
   L.sched.running = L.sched.localising = false;
+  if (const int rc = place_clear(c, lane)) return rc;   // keyframes are not part of snapshots
   // ---- validation, on the host, before anything is written to the device
   const char* b = static_cast<const char*>(blob);
   const SnapHeader& h = c->pin->snap;

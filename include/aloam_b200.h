@@ -813,6 +813,88 @@ typedef struct aloam_recovery_row {
 } aloam_recovery_row;
 int aloam_recovery_rows(aloam_ctx* ctx, aloam_recovery_row* out, int rows);
 int aloam_debug_recovery_scores(aloam_ctx* ctx, int lane, int* scores, int n);
+/* ---- place recognition: the Scan Context descriptor (G. Kim and A. Kim, "Scan Context: Egocentric Spatial Descriptor for Place
+ * Recognition within 3D Point Cloud Map", IROS 2018), for loop candidates of mapping lanes and for relocalisation without a pose guess.
+ * Search is the paper's exact definition: brute force over every keyframe and every column shift (no ring-key tree).
+ * Descriptor of a scan: its less_sharp then less_flat clouds in the sensor frame (as aloam_mapper_step takes them).  For every point
+ * (float x, y, z), float operations without contraction:
+ *   r = sqrtf(x*x + y*y); the point is skipped unless r < max_range;  ring = min(19, (int)((r * 20.0f) / max_range));
+ *   a = atan2f(y, x) (glibc's float atan2f), a = a + 6.28318548f when a < 0;  sector = min(59, (int)((a * 60.0f) / 6.28318548f));
+ *   v = z + z_offset.  Bin (ring, sector) holds the maximum v of its points in the total order of IEEE bit patterns (-0 < +0, so
+ *   the result does not depend on point order); an empty bin holds +0.0f.  Storage is ring-major: bin (r, s) at r * 60 + s.
+ * Distance, in double, one IEEE operation at a time (no FMA), sums in ascending index order:
+ *   column norm n[c] = sqrt(sum_r d[r][c]^2);  for a shift s visit c = 0 .. 59 with c' = (c + s) mod 60, skip the column when
+ *   n_q[c] == 0 or n_d[c'] == 0, else dot = sum_r q[r][c] * d[r][c'], sim += dot / (n_q[c] * n_d[c']), cnt += 1;
+ *   dist(s) = cnt ? 1 - sim / cnt : 1.0;  D = min_s dist(s), the smallest s on ties: the match's `shift`.
+ *   Heading: q_query ~ q_keyframe * Rz(shift * 2 pi / 60).  Matches rank by (D ascending, keyframe index ascending).
+ * Keyframe record, ALOAM_PLACE_RECORD_BYTES, little-endian: 0 double pose[7] (the row's map pose, q xyzw, t)  56 int32 scan_index
+ * (the row's scan j in its trajectory)  60 int32 lane  64 float max_range  68 float z_offset  72 zero  80 float desc[1200].
+ * Records concatenate: keyframes of several lanes or sessions form one database by appending.
+ *
+ * aloam_set_place(ctx, on, opts): opts->max_range and opts->z_offset are the descriptor parameters of every call below (80 and 2.0
+ * before any call).  on = 1 records keyframes in the mapped stream calls from the next call on, on = 0 stops.  Every call clears
+ * every lane's keyframe table.  Errors, with nothing changed: ALOAM_ERR_INVALID_ARG for on outside {0, 1}, a NULL opts, non-finite
+ * values, max_range <= 0, keyframe_gap < 0, exclude_recent < 0 or max_keyframes outside 1 .. 65536; ALOAM_ERR_STATE on a rank of a
+ * sharded job or an emulating context (aloam_comm_init and aloam_debug_shard_emulate turn recording off); ALOAM_ERR_CUDA when the
+ * tables cannot be allocated.
+ * Recording: ALOAM_ROW_MAPPED rows of aloam_scan_stream_mapped, _mapped_batch and _lanes (seeded aloam_lane_map_on_prior lanes
+ * included); skipped rows, localising rows, odometry-only lanes and aloam_mapper_step record nothing.  A mapped row is a keyframe
+ * when its lane's table is empty or when (dx*dx + dy*dy) + dz*dz (double) between the row's map translation and the lane's last
+ * keyframe's is >= keyframe_gap^2: its record is appended to the lane's table, then it is queried against the lane's keyframes
+ * 0 .. n - 1 - exclude_recent (n: its own index); the best match is the row's loop candidate.  A full table records nothing and
+ * sets the row's `full`.  A lane's table is cleared by every mapping START (seeded STARTs included), aloam_reset_odometry and
+ * aloam_lane_restore (keyframes are not part of snapshots).  All of it is decided on the device without a host synchronisation:
+ * 3 launches per mapping frame (k_place_gate, k_place_dist, k_place_best) and one device-to-host copy of the call's place rows.
+ * With recording off the stream calls issue exactly what they issue without this feature.
+ * aloam_place_rows mirrors aloam_map_rows: the same row count, scan-major order, state rules, and readability after
+ * ALOAM_ERR_CAPACITY / ALOAM_ERR_COMM (ALOAM_ERR_STATE when the last mapped call ran with recording off).  Fields are -1 / -1.0
+ * where there is none; `full` is 0 or 1.
+ * aloam_place_keyframes exports lane `lane`'s records to device, pinned or pageable memory, with the size rules of
+ * aloam_mapper_export counted in records: *n_out is always set; out = NULL with capacity = 0 asks for the size; capacity < *n_out is
+ * ALOAM_ERR_CAPACITY and writes nothing.  ALOAM_ERR_INVALID_ARG for a bad lane, ALOAM_ERR_STATE before recording was ever turned on.
+ * aloam_place_db_load replaces the context's database with n_records records (host or device memory), checked on the device before
+ * anything changes: ALOAM_ERR_INVALID_ARG when a record's max_range / z_offset differ bit for bit from the context's, a pose or
+ * descriptor value is not finite, or n_records is outside 1 .. 2^20.  Column norms are computed on load.  aloam_place_db_clear
+ * releases it.
+ * aloam_place_describe: the descriptor of one scan into desc (host or device memory); ALOAM_ERR_CAPACITY above cfg.max_points.
+ * aloam_place_query: n_query descriptors (n_query x 1200 floats, host or device memory) against the database; out = n_query x k
+ * matches, the k best per query in rank order.  ALOAM_ERR_STATE without a database; ALOAM_ERR_INVALID_ARG unless
+ * 1 <= k <= min(ALOAM_PLACE_MAX_K, M) and n_query >= 1.
+ * Memory, arithmetic from the buffer sizes: recording on allocates max_keyframes x (4880 + 480) B for each of cfg.max_batch lanes and
+ * a 4096-row place-row table (24 B per row, device and pinned), kept until aloam_destroy (a larger max_keyframes replaces them); the
+ * database M x 5360 B; aloam_place_describe two staging clouds of 16 B x cfg.max_points; aloam_place_query the queries (4.8 kB each)
+ * and 12 B per (query, keyframe) pair of up to 2^24 pairs at a time. */
+#define ALOAM_PLACE_RINGS 20
+#define ALOAM_PLACE_SECTORS 60
+#define ALOAM_PLACE_MAX_K 64
+#define ALOAM_PLACE_RECORD_BYTES 4880
+typedef struct aloam_place_opts {
+  float max_range;      /* > 0 (m): points at r >= max_range are skipped; default 80 */
+  float z_offset;       /* added to z before the maximum; default 2.0 */
+  double keyframe_gap;  /* >= 0 (m): the least distance from the lane's last keyframe to a new one */
+  int exclude_recent;   /* >= 0: the newest keyframes a loop query leaves out */
+  int max_keyframes;    /* 1 .. 65536: the capacity of each lane's table */
+} aloam_place_opts;
+typedef struct aloam_place_row {
+  int keyframe;         /* the row's index in its lane's table, -1 when it is not a keyframe */
+  int loop;             /* the best match among the lane's older keyframes, -1 when none */
+  int shift;            /* its column shift, -1 when none */
+  int full;             /* 1 when the row would have been a keyframe but the table was full */
+  double distance;      /* its distance, -1.0 when none */
+} aloam_place_row;
+typedef struct aloam_place_match {
+  int keyframe;         /* index into the database */
+  int shift;
+  double distance;
+} aloam_place_match;
+int aloam_set_place(aloam_ctx* ctx, int on, const aloam_place_opts* opts);
+int aloam_place_rows(aloam_ctx* ctx, aloam_place_row* out, int rows);
+int aloam_place_keyframes(aloam_ctx* ctx, int lane, void* out, long long capacity, long long* n_out);
+int aloam_place_db_load(aloam_ctx* ctx, const void* records, int n_records);
+int aloam_place_db_clear(aloam_ctx* ctx);
+int aloam_place_describe(aloam_ctx* ctx, aloam_cloud_view less_sharp, aloam_cloud_view less_flat, float* desc);
+int aloam_place_query(aloam_ctx* ctx, const float* descs, int n_query, int k, aloam_place_match* out);
+
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
