@@ -37,6 +37,7 @@ EXPORTED_SYMBOLS = [
     "aloam_prior_map_digest", "aloam_lane_save_localising", "aloam_snapshot_localise_info",
     "aloam_set_place", "aloam_place_rows", "aloam_place_keyframes", "aloam_place_db_load", "aloam_place_db_clear",
     "aloam_place_describe", "aloam_place_query",
+    "aloam_set_loops", "aloam_loop_rows", "aloam_loop_verify", "aloam_place_keyframe_cloud",
 ]
 ERR_SNAPSHOT = -11
 LANE_IDLE, LANE_SCAN, LANE_START = 0, 1, 2
@@ -127,6 +128,21 @@ class PlaceRow(C.Structure):
 
 class PlaceMatch(C.Structure):
     _fields_ = [("keyframe", C.c_int), ("shift", C.c_int), ("distance", C.c_double)]
+
+
+class LoopOpts(C.Structure):
+    _fields_ = [("max_distance", C.c_double), ("window", C.c_int), ("cloud_points", C.c_int), ("outer_iters", C.c_int),
+                ("inlier_sq", C.c_float)]
+
+
+class LoopRow(C.Structure):
+    _fields_ = [("query", C.c_int), ("cand", C.c_int), ("verified", C.c_int), ("shift", C.c_int), ("n_sub", C.c_int * 2),
+                ("score", C.c_int), ("n_score", C.c_int), ("stats", Stats), ("pose", C.c_double * 7), ("rel", C.c_double * 7)]
+
+    def as_dict(self):
+        return {"query": self.query, "cand": self.cand, "verified": self.verified, "shift": self.shift, "n_sub": tuple(self.n_sub),
+                "score": self.score, "n_score": self.n_score, "stats": self.stats.as_dict(), "pose": np.array(self.pose[:]),
+                "rel": np.array(self.rel[:])}
 
 
 class AloamError(RuntimeError):
@@ -222,6 +238,10 @@ def lib():
         L.aloam_place_db_clear.argtypes = [C.c_void_p]
         L.aloam_place_describe.argtypes = [C.c_void_p, cv, cv, C.c_void_p]
         L.aloam_place_query.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(PlaceMatch)]
+        L.aloam_set_loops.argtypes = [C.c_void_p, C.c_int, C.POINTER(LoopOpts)]
+        L.aloam_loop_rows.argtypes = [C.c_void_p, C.POINTER(LoopRow), C.c_int]
+        L.aloam_loop_verify.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(LoopRow)]
+        L.aloam_place_keyframe_cloud.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
         _LIB = L
     return _LIB
 
@@ -911,6 +931,42 @@ class Aloam:
         d = {k: np.array([getattr(r, k) for r in out], np.int32) for k in ("keyframe", "loop", "shift", "full")}
         d["distance"] = np.array([r.distance for r in out], np.float64)
         return d
+
+    # --- loop verification
+    def set_loops(self, on=True, max_distance=0.3, window=10, cloud_points=1000, outer_iters=4, inlier_sq=1.0):
+        """turns loop verification of the mapped stream calls on or off (aloam_set_loops; needs set_place on): every mapped keyframe
+        row whose place-row distance is <= max_distance (default 0.3) is registered against the submap of its candidate's keyframes
+        within `window` (default 10) on each side, each keyframe keeping at most cloud_points (default 1000) points per type of its
+        filtered stacks, in outer_iters (default 4) rounds; the score counts inliers at float d^2 < inlier_sq (default 1.0 m^2).
+        Every call clears every lane's keyframe table"""
+        o = LoopOpts(float(max_distance), int(window), int(cloud_points), int(outer_iters), float(inlier_sq))
+        _check(lib().aloam_set_loops(self._h, int(on), C.byref(o)))
+
+    def loop_rows(self, rows):
+        """the loop rows of the `rows` = n_scans x batch rows (scan-major) of the last mapped stream call (aloam_loop_rows) -> list
+        of dicts query, cand, verified, shift, n_sub, score, n_score, stats, pose, rel (query / cand / shift -1 where not verified)"""
+        out = (LoopRow * max(int(rows), 1))()
+        _check(lib().aloam_loop_rows(self._h, out, int(rows)))
+        return [r.as_dict() for r in out[:int(rows)]]
+
+    def loop_verify(self, lane, query, cand, shift=None, init=None):
+        """one verification (aloam_loop_verify) of keyframe `query` of lane `lane` against the submap of keyframe `cand`: from
+        q_cand * Rz(shift * 2 pi / 60), t_cand (shift default 0), or from the pose init (q xyzw, t) when given -> the row's dict"""
+        out = LoopRow()
+        x = None if init is None else np.ascontiguousarray(init, np.float64)
+        if x is not None and x.shape != (7,):
+            raise ValueError("init is a pose (q xyzw, t) of 7 doubles")
+        _check(lib().aloam_loop_verify(self._h, int(lane), int(query), int(cand), -1 if shift is None and x is not None else int(shift or 0),
+                                       None if x is None else _dp(x), C.byref(out)))
+        return out.as_dict()
+
+    def keyframe_cloud(self, lane, k):
+        """keyframe k's stored clouds of lane `lane` (aloam_place_keyframe_cloud; loops on) -> (corner, surf), (n, 4) float32"""
+        n = (C.c_longlong * 2)()
+        _check(lib().aloam_place_keyframe_cloud(self._h, int(lane), int(k), None, 0, n))
+        out = np.zeros((max(n[0] + n[1], 1), 4), np.float32)
+        _check(lib().aloam_place_keyframe_cloud(self._h, int(lane), int(k), C.c_void_p(out.ctypes.data), out.shape[0], n))
+        return out[:n[0]].copy(), out[n[0]:n[0] + n[1]].copy()
 
     def transform_to_end(self, cloud, q, t, distortion=True):
         v, keep = _view(cloud)

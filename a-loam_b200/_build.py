@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libaloam_b200.so")
-SOURCES = ["features.cu", "odometry.cu", "lm.cu", "mapping.cu", "comm.cu", "voxel.cu", "cubemap.cu", "reloc.cu", "rows.cu", "recover.cu", "place.cu", "capi.cu", "snapshot.cu", "io.cu"]
+SOURCES = ["features.cu", "odometry.cu", "lm.cu", "mapping.cu", "comm.cu", "voxel.cu", "cubemap.cu", "reloc.cu", "rows.cu", "recover.cu", "place.cu", "loop.cu", "capi.cu", "snapshot.cu", "io.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # float32 decision kernels must not contract a*b+c (bit parity with an x86-64 no-FMA build of the reference);

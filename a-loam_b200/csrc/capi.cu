@@ -577,10 +577,12 @@ struct StreamSwitches {
   bool rec, score;
   bool recov;          // recovery of localising lanes (aloam_set_recovery, recover.cu): four more launches after every scored localising frame
   bool place;          // keyframes (aloam_set_place, place.cu): three more launches after every mapping frame, one copy of the place rows
+  bool loop;           // loop verification (aloam_set_loops, loop.cu): keyframe clouds after every mapping frame and the verification of
+                       // its triggered rows, one copy of the loop rows
   bool reset_stores;   // a START also resets its lane's cube store
   StreamSwitches(const aloam_ctx* c, bool mapped, bool reset)
       : map(mapped), sink(map && c->reg_sink), rec(map && c->rows_on), score(rec && c->rows_max_score > 0), recov(score && c->rec_on),
-        place(map && c->place_on), reset_stores(reset) {}
+        place(map && c->place_on), loop(place && c->loop_on), reset_stores(reset) {}
 };
 #define STREAM_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[aloam_b200] CUDA error %s at %s:%d\n", cudaGetErrorName(_e), __FILE__, __LINE__); return ALOAM_ERR_CUDA; } } while (0)
 
@@ -630,7 +632,9 @@ static int map_stage(aloam_ctx* c, const StreamSwitches& w, const StreamRow* row
         const StreamRow& R = row[in[j].lane];
         scan[j] = R.scan; start[j] = R.op == ALOAM_LANE_START; prow[j] = place_rows_device(c) + r0 + in[j].lane;
       }
-      rc = place_record_device(c, n, in, scan, start, prow); if (rc) return rc;
+      int n_upper = 0;
+      rc = place_record_device(c, n, in, scan, start, prow, &n_upper); if (rc) return rc;
+      if (w.loop) { rc = loop_record_device(c, n, in, prow, r0, n_upper); if (rc) return rc; }
     }
     for (int j = 0; loc && j < n; ++j) c->lanes[in[j].lane].window = true;
     // /velodyne_cloud_registered of the frame's rows, before the lanes' next frame replaces the refined pose
@@ -763,6 +767,7 @@ static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const Stream
     STREAM_TRY(cudaMemcpyAsync(c->h_poses + (size_t)kMaxStreamScans * 7, c->d_map_poses, total * 56, cudaMemcpyDeviceToHost, s_main));
     if (w.rec) STREAM_TRY(cudaMemcpyAsync(c->h_rows, c->d_rows, total * sizeof(MapRowRec), cudaMemcpyDeviceToHost, s_main));
     if (w.place) STREAM_TRY(cudaMemcpyAsync(place_rows_host(c), place_rows_device(c), total * sizeof(aloam_place_row), cudaMemcpyDeviceToHost, s_main));
+    if (w.loop) STREAM_TRY(cudaMemcpyAsync(loop_rows_host(c), loop_rows_device(c), total * loop_row_bytes(), cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) {
       c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
       if (c->lanes[l].mapper) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
@@ -805,7 +810,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, StreamTab
   MappedCall& M = c->last_mapped;
   if (w.map) {   // this call's rows replace the last mapped call's, unreadable until the call has drained
     M.table = std::move(table); M.n_scans = n_scans; M.nb = nb;
-    M.registered = M.records = M.places = false; M.recovered = w.recov;
+    M.registered = M.records = M.places = M.loops = false; M.recovered = w.recov;
     recover_call_done(c);   // no lane's candidate scores belong to this call yet
   }
   const StreamTable& t = w.map ? M.table : table;
@@ -836,7 +841,7 @@ static int scan_stream_run(aloam_ctx* c, const aloam_cloud_view* raws, StreamTab
   if (w.map) {   // the call's rows are readable (after ALOAM_ERR_CAPACITY and ALOAM_ERR_COMM below too: they name the row that was hit)
     M.reg_count.resize(total);
     for (size_t r = 0; r < total; ++r) M.reg_count[r] = w.sink && t.rows[r].mapped ? c->h_scan_nfull[r] : 0;
-    M.registered = true; M.records = w.rec; M.places = w.place;
+    M.registered = true; M.records = w.rec; M.places = w.place; M.loops = w.loop;
     recover_call_done(c);
     // as aloam_mapper_step: a voxel index range beyond the key width in any frame of any lane means its map results would be wrong
     c->pin->mapper_err = 0;
@@ -936,7 +941,7 @@ int aloam_scan_stream_lanes(aloam_ctx* c, const aloam_cloud_view* raws, const in
   }
   if (map && c->reg_sink && t.reg_total > c->reg_cap) return ALOAM_ERR_CAPACITY;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  if (run_err) { if (map) c->last_mapped.records = c->last_mapped.places = false; aloam_reset_odometry(c); return run_err; }
+  if (run_err) { if (map) c->last_mapped.records = c->last_mapped.places = c->last_mapped.loops = false; aloam_reset_odometry(c); return run_err; }
   for (int l = 0; map && l < batch; ++l) {   // creates the cube stores and locators this call needs: a lane that only localises gets no cube store
     int rc = localises[l] ? locator_ensure(c, l) : ALOAM_OK; if (rc) return rc;
     rc = maps[l] || !localises[l] ? mapper_ensure(c, l) : ALOAM_OK; if (rc) return rc;

@@ -218,7 +218,7 @@ int aloam_debug_shard_emulate(aloam_ctx* c, int rank, int world, int exchange, i
   const int new_rank = world ? rank : 0, new_count = world ? world : 1;
   if (new_rank != c->shard_rank || new_count != c->shard_count) c->have_map = false;   // the map was cut for another rank
   c->shard_rank = new_rank; c->shard_count = new_count; c->shard_exchange = world ? exchange : -1;
-  if (world > 0) c->rows_on = c->rec_on = c->place_on = false;   // per-row records, recovery and keyframes serve unsharded contexts only
+  if (world > 0) c->rows_on = c->rec_on = c->place_on = c->loop_on = false;   // per-row records, recovery and keyframes serve unsharded contexts only
   return ALOAM_OK;
 }
 
@@ -251,7 +251,7 @@ int aloam_comm_init(aloam_ctx* c, int rank, int world, const char id128[128]) {
   own(c, [comm] { g_nccl.CommDestroy(comm); });   // an earlier communicator of this context lives on until aloam_destroy
   const int rc = lm_exchange_alloc(c); if (rc) return rc;
   c->shard_rank = rank; c->shard_count = world;
-  c->rows_on = c->rec_on = c->place_on = false;   // per-row records, recovery and keyframes serve unsharded contexts only
+  c->rows_on = c->rec_on = c->place_on = c->loop_on = false;   // per-row records, recovery and keyframes serve unsharded contexts only
   // the 256-byte exchange of every LM evaluation goes through NVLink peer memory inside the solve kernel when the ranks can map
   // each other's memory (all ranks decide alike: the outcome of the handle exchange is the same everywhere ... see below)
   peer_drop(c);   // the peer path of an earlier communicator

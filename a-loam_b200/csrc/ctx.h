@@ -96,6 +96,7 @@ struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexe
 struct Relocaliser;    // reloc.cu: the scratch of aloam_prior_relocalise
 struct Recovery;       // recover.cu: the setting and buffers of aloam_set_recovery
 struct Place;          // place.cu: the keyframe tables, database and scratch of place recognition (aloam_set_place)
+struct Loop;           // loop.cu: the setting, keyframe clouds and registration sets of loop verification (aloam_set_loops)
 }  // namespace aloam
 
 using namespace aloam;
@@ -141,6 +142,7 @@ struct MappedCall {
   bool records = false;          // aloam_map_rows and aloam_recovery_rows may read the table and the pinned row table h_rows
   bool recovered = false;        // the call ran recovery (aloam_set_recovery)
   bool places = false;           // aloam_place_rows may read the table and the pinned place rows (the call recorded keyframes)
+  bool loops = false;            // aloam_loop_rows may read the table and the pinned loop rows (the call verified loops)
   // a reader's check: ALOAM_ERR_STATE while its flag is off, ALOAM_ERR_INVALID_ARG for a row count other than the call's
   int check(bool readable, int rows) const { return !readable ? ALOAM_ERR_STATE : rows != n_scans * nb ? ALOAM_ERR_INVALID_ARG : ALOAM_OK; }
 };
@@ -292,6 +294,10 @@ struct aloam_ctx {
   // database and scratch, created on first use
   bool place_on = false;
   Place* place = nullptr;
+  // loop verification (aloam_set_loops, loop.cu): keyframe clouds and in-stream verification while loop_on (only with place_on);
+  // its buffers, created by the call that turns it on
+  bool loop_on = false;
+  Loop* loop = nullptr;
   MappedCall last_mapped;   // the rows of the last mapped stream call and which of its readers may read them
   // exports of a lane's store (aloam_mapper_export, lane snapshots): the layout of the last one and the staging buffer of host
   // memory, created on first use
@@ -351,12 +357,12 @@ namespace {
 enum { KID_CLASSIFY = 0, KID_RING_SCAN, KID_SCATTER, KID_RING_FEATURES, KID_COMPACT, KID_GRID_BUILD, KID_ODOM_ASSOC, KID_LM_SOLVE,
        KID_RING_OFFSETS, KID_KNN_LAST, KID_PACK_BLOCKS, KID_MAP_GRID, KID_MAP_KNN5, KID_VOXEL, KID_MAP_KNN, KID_MAP_FIT, KID_CUBES, KID_LM_SHARD, KID_MAP_KNN5_PRIOR,
        KID_PRIOR_BUILD, KID_RELOC, KID_RELOC_TOPK, KID_MAP_ROWS, KID_TRACK_SCORE, KID_RECOVER_CAND, KID_RECOVER_ADOPT,
-       KID_PRIOR_DIGEST, KID_PLACE_GATE, KID_PLACE_DIST, KID_PLACE_BEST };
+       KID_PRIOR_DIGEST, KID_PLACE_GATE, KID_PLACE_DIST, KID_PLACE_BEST, KID_LOOP_KEEP, KID_LOOP_VERIFY };
 const char* const kKernelNames[ALOAM_N_KERNEL_IDS] = {"k_classify", "k_ring_scan", "k_scatter", "k_ring_features", "k_compact",
     "k_rab_build(3 launches)", "k_odom_assoc", "k_lm_solve", "k_ring_offsets", "k_knn_last", "k_pack_blocks", "k_map_grid(4 launches)", "k_map_knn5",
     "k_voxel", "k_map_knn", "k_map_fit", "k_cube_store", "k_lm_shard", "k_map_knn5_prior",
     "k_prior_build", "k_reloc_score", "k_reloc_topk", "k_map_rows", "k_track_score", "k_recover_cand", "k_recover_adopt",
-    "k_prior_digest", "k_place_gate(describe)", "k_place_dist", "k_place_best"};
+    "k_prior_digest", "k_place_gate(describe)", "k_place_dist", "k_place_best", "k_loop_keep", "k_loop_gather/score/finish"};
 
 inline void prof_begin(aloam_ctx* c, int kid) {
   ++c->launches;
@@ -434,10 +440,26 @@ int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* co
 // place recognition (place.cu): after the mapping frame of nb records just issued, the keyframe gate, descriptor and loop query of
 // each (scan[l]: its scan index, start[l]: it STARTs a trajectory, which clears its lane's table first; rows[l]: its place row);
 // and the clearing of lane `lane`'s table (-1: every lane), on c->stream
-int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows);
+// (*n_upper, when not null: the host bound on the keyframes any record's loop query searches; <= 0 when no record can have one)
+int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows,
+                        int* n_upper = nullptr);
 int place_clear(aloam_ctx* c, int lane);
 aloam_place_row* place_rows_device(aloam_ctx* c);
 aloam_place_row* place_rows_host(aloam_ctx* c);
+// lane `lane`'s keyframe table (place recording has been on): its records and count on the device, the keyframes it takes and the
+// loop query's exclude_recent
+struct PlaceTable { const char* rec; const int* count; int cap; int exclude; };
+PlaceTable place_table(aloam_ctx* c, int lane);
+// loop verification (loop.cu): after place_record_device of the mapping frame of nb records, the keyframe clouds of its keyframe
+// rows and the verification of its triggered rows (prow[l]: record l's place row; n_upper: the bound place_record_device returned),
+// on c->stream; the clearing of lane `lane`'s clouds goes with its place table (nothing to do on the device)
+int loop_record_device(aloam_ctx* c, int nb, const MapperIn* in, const aloam_place_row* const* prow, size_t r0, int n_upper);
+void* loop_rows_device(aloam_ctx* c);
+void* loop_rows_host(aloam_ctx* c);
+size_t loop_row_bytes();
+// the stacks a lane's latest mapping frame registered (sensor frame) and their sizes (counts[0], counts[1]), from its cube store
+struct MapperStacks { const Pt4* stack[2]; const int* counts; };
+MapperStacks mapper_stacks(const aloam_ctx* c, int lane);
 // which lanes' candidate scores belong to a triggered row of the last mapped stream call (recover.cu; none while its records
 // cannot be read or it ran no recovery)
 void recover_call_done(aloam_ctx* c);
@@ -509,7 +531,8 @@ int ensure_map_buffers(aloam_ctx* c);
 int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids = true);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
-int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, const PriorSearch* prior = nullptr);
+// rounds: outer iterations of association + solve (cfg.outer_iters for every mapping and localising frame)
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, int rounds, const PriorSearch* prior = nullptr);
 namespace {
 
 // a rank of a sharded job: joined to a world of several ranks by a communicator, or emulating a rank (aloam_debug_shard_emulate)

@@ -1547,7 +1547,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- optimisation (:554-733)
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  rc = map_register_device(c, nb, io, nq_upper); if (rc) return rc;
+  rc = map_register_device(c, nb, io, nq_upper, c->cfg.outer_iters); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   // ---- insertion (:736-767)
   const int up = std::max(n_upper_c, n_upper_s);
@@ -1752,6 +1752,11 @@ LocatorFrame locator_frame(const Locator* m) {
   return LocatorFrame{{m->reg.stack[0], m->reg.stack[1]}, S->stack_counts, &S->flags};
 }
 
+MapperStacks mapper_stacks(const aloam_ctx* c, int lane) {
+  const Mapper* m = c->lanes[lane].mapper;
+  return MapperStacks{{m->reg->stack[0], m->reg->stack[1]}, m->d_state->stack_counts};
+}
+
 PriorGrid prior_grid(const aloam_ctx* c) { return PriorGrid{c->prior->grid[0], c->prior->grid[1]}; }
 
 int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_upper_c, int n_upper_s) {
@@ -1804,7 +1809,7 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const*
   CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_stack_join, 0));   // join: the filtered stacks are ready
   launch_ex(c, KID_CUBES, k_mapper_prep, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   const int nq_upper = std::min(n_upper_c + n_upper_s, 2 * c->max_points);
-  rc = map_register_device(c, nb, io, nq_upper, &ps); if (rc) return rc;
+  rc = map_register_device(c, nb, io, nq_upper, c->cfg.outer_iters, &ps); if (rc) return rc;
   launch_ex(c, KID_CUBES, k_mapper_update, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   launch_ex(c, KID_CUBES, k_mapper_finish, dim3(1, 1, nb), dim3(32), 0, 1, true, B);
   CUDA_CHECK_RET(cudaGetLastError());

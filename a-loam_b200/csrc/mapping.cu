@@ -778,11 +778,12 @@ void map_associate_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_uppe
 }
 }  // namespace
 
-// outer_iters x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers its stacks against io[l].reg
-// (see map_associate_device) and refines io[l].pose.  A sharded job's solves exchange their normal equations (one lane).
-int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, const PriorSearch* prior) {
+// rounds x (5-NN + fits + LM) of nb lanes, each launch covering all of them: lane l registers its stacks against io[l].reg
+// (see map_associate_device) and refines io[l].pose; round it leaves its summary in io[l].reg.summary[it & 3].  A sharded job's
+// solves exchange their normal equations (one lane).
+int map_register_device(aloam_ctx* c, int nb, const MapLaneIO* io, int nq_upper, int rounds, const PriorSearch* prior) {
   const LmParams lp = lm_params(c->cfg);
-  for (int it = 0; it < c->cfg.outer_iters; ++it) {
+  for (int it = 0; it < rounds; ++it) {
     map_associate_device(c, nb, io, nq_upper, it > 0, nullptr, prior);
     Batch<LmArgs> lm = {};
     for (int l = 0; l < nb; ++l) lm.a[l] = LmArgs{io[l].reg.blocks, io[l].counts3 + 2, 0, io[l].pose, io[l].reg.summary + (it & 3), nullptr, nullptr};
@@ -948,7 +949,7 @@ int aloam_mapping_register(aloam_ctx* c, aloam_cloud_view corner_stack, aloam_cl
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_map_pose, c->pin->pose_in, 56, cudaMemcpyHostToDevice, c->stream));
   rc = peer_err_reset(c); if (rc) return rc;
   const MapLaneIO io = {c->map, {nullptr, nullptr}, c->d_stack_counts, c->d_map_pose};
-  rc = map_register_device(c, 1, &io, corner_stack.n + surf_stack.n); if (rc) return rc;
+  rc = map_register_device(c, 1, &io, corner_stack.n + surf_stack.n, c->cfg.outer_iters); if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->pose_out, c->d_map_pose, 56, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, c->map.summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
   rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;

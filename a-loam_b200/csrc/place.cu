@@ -319,7 +319,13 @@ int place_clear(aloam_ctx* c, int lane) {
 aloam_place_row* place_rows_device(aloam_ctx* c) { return c->place->d_rows; }
 aloam_place_row* place_rows_host(aloam_ctx* c) { return c->place->h_rows; }
 
-int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows) {
+PlaceTable place_table(aloam_ctx* c, int lane) {
+  const Place* P = c->place;
+  return PlaceTable{P->d_rec + (size_t)lane * P->alloc * kRec, P->d_count + lane, P->cap, P->opt.exclude_recent};
+}
+
+int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows, int* n_upper_out) {
+  if (n_upper_out) *n_upper_out = 0;
   Place* P = c->place;
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || !P->d_count) return ALOAM_ERR_STATE;
   Batch<PlaceGate> G = {};
@@ -338,6 +344,7 @@ int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* sca
   const double gap2 = P->opt.keyframe_gap * P->opt.keyframe_gap;
   LAUNCH(c, KID_PLACE_GATE, k_place_gate, nb, kDescThreads, 0, G, P->cap, P->opt.max_range, P->opt.z_offset, gap2);
   CUDA_CHECK_RET(cudaGetLastError());
+  if (n_upper_out) *n_upper_out = n_upper;
   if (n_upper <= 0) return ALOAM_OK;   // no record has an older keyframe to query: the rows keep the gate's -1 fields
   S.exclude = P->opt.exclude_recent; S.stream = true;
   S.dist = P->d_dist; S.shift = P->d_shift; S.stride = P->alloc;
@@ -388,6 +395,7 @@ int aloam_set_place(aloam_ctx* c, int on, const aloam_place_opts* opts) {
   }
   P->opt = o;
   P->cap = std::min(o.max_keyframes, P->alloc);
+  c->loop_on = false;   // the keyframe clouds belong to the tables this call clears (aloam_set_loops turns them on again)
   if (P->d_count) {
     CUDA_CHECK_RET(cudaMemsetAsync(P->d_count, 0, c->n_lanes * sizeof(int), c->stream));
     CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));

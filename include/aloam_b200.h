@@ -895,6 +895,80 @@ int aloam_place_db_clear(aloam_ctx* ctx);
 int aloam_place_describe(aloam_ctx* ctx, aloam_cloud_view less_sharp, aloam_cloud_view less_flat, float* desc);
 int aloam_place_query(aloam_ctx* ctx, const float* descs, int n_query, int k, aloam_place_match* out);
 
+/* ---- loop verification: the geometric half of loop closure (the registration step SC-A-LOAM runs after Scan Context detection).
+ * A place row's loop candidate is a hypothesis; verification registers the query keyframe against a submap made of the candidate's
+ * neighbouring keyframes and returns the refined pose, its inlier score and the relative-pose constraint a pose-graph optimiser takes.
+ *
+ * aloam_set_loops(ctx, on, opts): needs place recording on (aloam_set_place; ALOAM_ERR_STATE otherwise) and clears every lane's
+ * keyframe table.  aloam_set_place turns loops off.  While loops are on:
+ *   Keyframe clouds: every keyframe a mapping row appends also stores its frame's filtered corner and surf stacks in the sensor
+ *   frame (the clouds the frame registered, aloam_map_row.n_stack points each).  Per type, with n stack points and
+ *   m = min(n, cloud_points), stored point i is stack point floor(i * n / m) (64-bit integers): the relocaliser's scoring-point
+ *   rule.  Clouds are cleared with their table (a mapping START, aloam_reset_odometry, aloam_lane_restore, aloam_set_place,
+ *   aloam_set_loops); neither they nor keyframes are part of snapshots.
+ *   Verification of (lane, query q, candidate c, shift s), n the lane's keyframe count and e = exclude_recent: it requires q < n
+ *   and 0 <= c <= q - 1 - e.
+ *     window W = [max(0, c - window), min(c + window, q - 1 - e)]: the keyframes the loop query itself searched, so the current
+ *       pass through the place never enters the submap;
+ *     submap, per type: the concatenation over k in W (ascending) of keyframe k's stored cloud in stored order, every point moved by
+ *       pointAssociateToMap at record k's pose (double, stored as float, intensity kept -- the rule of the registered clouds);
+ *     initial pose: q0 = q_c * (0, 0, sz, cz) written as (x cz + y sz, y cz - x sz, z cz + w sz, w cz - z sz) with
+ *       (sz, cz) = (sin, cos)(a / 2), a = ((s * 2.0) * pi) / 60 (the C library's sin / cos on the host), then normalised as
+ *       aloam_lane_localise normalises (|q|^2 summed in index order, q / sqrt); t0 = t_c.  aloam_loop_verify takes `init` instead
+ *       when it is not NULL (normalised the same way; `shift` is ignored and the row's shift is -1);
+ *     registration: with <= 10 corner or <= 50 surf submap points no round runs, the pose stays the initial pose and the row is
+ *       flagged ALOAM_FLAG_MAP_TOO_THIN.  Otherwise outer_iters rounds of the mapper's association and solve run with the query
+ *       keyframe's stored clouds as the stacks.  The result is, bit for bit, what a context of the same configuration with
+ *       outer_iters = 1 computes with one aloam_map_upload of the submap and outer_iters successive aloam_mapping_register calls
+ *       from the initial pose: the pose and the last call's stats (ms_total = 0);
+ *     score: the relocaliser's inlier rule -- a stored point of the query keyframe moved by `pose` is an inlier when a submap point
+ *       of its type lies at float ((dx*dx + dy*dy) + dz*dz) < inlier_sq.  An integer count; there is no accept threshold, the caller
+ *       judges score / n_score;
+ *     constraint: rel = T_c^-1 * pose in Eigen's operation order, (q_c.conjugate() * q, q_c.conjugate() * (t - t_c)).
+ *   In the stream: every ALOAM_ROW_MAPPED keyframe row of aloam_scan_stream_mapped, _mapped_batch and _lanes whose place row has
+ *   loop >= 0 and distance <= max_distance (double compare) is verified at its own step on the mapper stream with (its lane, its
+ *   keyframe, its loop, its shift), without a host synchronisation.  Launches per mapping frame: 1 (k_loop_keep); when some record
+ *   can have a candidate (the bound place recognition uses to size its query), 8 + 3 outer_iters more (k_loop_gather, k_grid_setup,
+ *   the 4 index-build launches, outer_iters x (k_map_knn5, k_map_fit, k_lm_solve), k_loop_score, k_loop_finish); one device-to-host
+ *   copy of the loop rows per call.  With loops off the stream calls issue exactly what they issue without this feature.
+ * aloam_loop_rows mirrors aloam_place_rows: the same row count, scan-major order, state rules, and readability after
+ * ALOAM_ERR_CAPACITY / ALOAM_ERR_COMM (ALOAM_ERR_STATE when the last mapped call ran with loops off).  Fields are -1 / 0 where a row
+ * was not verified.
+ * aloam_loop_verify runs one verification on the context's stream and synchronises once; ALOAM_ERR_STATE while loops are off.
+ * aloam_place_keyframe_cloud exports keyframe `keyframe` of lane `lane`: corner points then surf points, 4 floats each, to device,
+ * pinned or pageable memory with the size rules of aloam_place_keyframes counted in points (n_out[0], n_out[1] always set).
+ * ALOAM_ERR_INVALID_ARG for a bad lane or a keyframe outside the lane's table, ALOAM_ERR_STATE while loops are off.
+ * Errors, each leaving nothing changed: ALOAM_ERR_INVALID_ARG for on outside {0, 1}, a NULL or out-of-range option, a bad lane,
+ * query, cand or shift (0 .. 59), a non-finite init or a zero quaternion; ALOAM_ERR_CAPACITY when (2 window + 1) x cloud_points >
+ * cfg.max_map_points (the submap bound, so no frame truncates a submap); ALOAM_ERR_STATE on a rank of a sharded job or an emulating
+ * context (aloam_comm_init and aloam_debug_shard_emulate turn loops off), for aloam_loop_verify while loops are off and for
+ * aloam_loop_rows after a call made with loops off; ALOAM_ERR_CUDA when the buffers cannot be allocated.
+ * Memory, per lane of cfg.max_batch lanes, with K = the place table's max_keyframes, P = cloud_points, B = (2 window + 1) P and
+ * S = the power of two >= 1.25 B (at least 1024): the cloud pool K x 2 x P x 16 B + K x 8 B; the registration set 2 x (S x 16 B +
+ * B x 16 B) grids, 2P x 80 B neighbours, 2P x 96 B residual blocks, 2P x 16 B query stacks and 4 solve summaries; the two submap
+ * buffers 2 x B x 16 B; plus a 4096-row loop-row table (device and pinned). */
+typedef struct aloam_loop_opts {
+  double max_distance;  /* >= 0: a keyframe row whose place-row distance is <= this (double compare) is verified */
+  int window;           /* 0 .. 64: keyframes on each side of the candidate that form its submap */
+  int cloud_points;     /* 1 .. cfg.max_points: per type, the most points a keyframe keeps of its frame's filtered stack */
+  int outer_iters;      /* 1 .. 16: association + solve rounds of a verification */
+  float inlier_sq;      /* 0 < . <= 1 (m^2): the relocaliser's inlier rule, for the score */
+} aloam_loop_opts;
+typedef struct aloam_loop_row {
+  int query, cand;      /* the row's keyframe and its candidate; -1 when the row was not verified */
+  int verified;         /* 1 when verification ran */
+  int shift;            /* the place row's shift used for the initial heading; -1 when not verified */
+  int n_sub[2];         /* corner / surf points of the candidate submap */
+  int score, n_score;   /* inliers of the query keyframe's stored points at `pose`, out of n_score (its stored corner + surf) */
+  aloam_stats stats;    /* the last round's stats as aloam_mapping_register returns them, ms_total = 0; MAP_TOO_THIN for a thin submap */
+  double pose[7];       /* the query keyframe's refined pose in the map frame of the candidate's submap (q xyzw, t) */
+  double rel[7];        /* the constraint: that pose in the candidate keyframe's frame, T_cand^-1 * pose */
+} aloam_loop_row;
+int aloam_set_loops(aloam_ctx* ctx, int on, const aloam_loop_opts* opts);
+int aloam_loop_rows(aloam_ctx* ctx, aloam_loop_row* out, int rows);
+int aloam_loop_verify(aloam_ctx* ctx, int lane, int query, int cand, int shift, const double init[7], aloam_loop_row* out);
+int aloam_place_keyframe_cloud(aloam_ctx* ctx, int lane, int keyframe, float* out, long long capacity, long long n_out[2]);
+
 /* the segmented VoxelGrid of the mapper (tests): n_segs clouds, each with its own cubic leaf, filtered by one pass with
  * idx_bits voxel-index bits in the 32-bit sort key (the segments go in windows of 2^(32 - idx_bits) when they do not fit
  * beside the index), exactly as the per-cube re-filter runs.  out: room for the sum of segs[s].n points; segment s is
