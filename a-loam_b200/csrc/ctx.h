@@ -89,6 +89,32 @@ struct TrackArgs {
   const double* pose;
   MapRowRec* row;
 };
+// Buffers that a later call replaces as a whole (a larger table, a new map): a replacement group is filled on the side and
+// swapped in only when every allocation in it succeeded; the group it replaces is freed as a whole by its destructor.  Nothing
+// here synchronises: an owner drains the work that reads a group's buffers before it frees them.
+class BufGroup {
+ public:
+  BufGroup() = default;
+  BufGroup(BufGroup&& o) noexcept { swap(o); }
+  BufGroup& operator=(BufGroup&& o) noexcept { BufGroup t(std::move(o)); swap(t); return *this; }
+  ~BufGroup() {
+    for (void* p : dev_) cudaFree(p);
+    for (void* p : pinned_) cudaFreeHost(p);
+  }
+  // n elements of T in device / page-locked host memory, recorded in the group; false (the error cleared, *p null) on failure
+  template <typename T> bool dev(T** p, size_t n) { return keep(cudaMalloc((void**)p, n * sizeof(T)), (void**)p, dev_); }
+  template <typename T> bool pinned(T** p, size_t n) { return keep(cudaMallocHost((void**)p, n * sizeof(T)), (void**)p, pinned_); }
+  void swap(BufGroup& o) noexcept { dev_.swap(o.dev_); pinned_.swap(o.pinned_); }
+  bool empty() const { return dev_.empty() && pinned_.empty(); }
+
+ private:
+  static bool keep(cudaError_t e, void** p, std::vector<void*>& list) {
+    if (e != cudaSuccess) { cudaGetLastError(); *p = nullptr; return false; }
+    list.push_back(*p);
+    return true;
+  }
+  std::vector<void*> dev_, pinned_;
+};
 struct ExportLayout;   // cubemap.cu: where the segments of a store export are in the export and in the store
 struct Mapper;         // cubemap.cu: a lane's cube store
 struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
@@ -528,7 +554,7 @@ int locator_map_pose(aloam_ctx* c, int lane, double* dst);
 int locator_restore(aloam_ctx* c, int lane, const double T[7]);
 int index_last_clouds(aloam_ctx* c, int lane, int slot, int n_ls, int n_lf);
 int ensure_map_buffers(aloam_ctx* c);
-int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids = true);
+int map_reg_alloc(BufGroup& g, MapReg* r, size_t queries, size_t bound, unsigned slots);
 void map_index_build(aloam_ctx* c, int nb, const MapLaneIO* io, int n_upper);
 int map_shard_index_device(aloam_ctx* c, Pt4* const sub[2], const int* n_sub, int n_upper, int* err_word);
 // rounds: outer iterations of association + solve (cfg.outer_iters for every mapping and localising frame)
@@ -562,6 +588,11 @@ template <typename T> cudaError_t halloc(aloam_ctx* c, T** p, size_t n) {
   const cudaError_t e = cudaMallocHost((void**)p, n * sizeof(T));
   if (e == cudaSuccess) { void* q = *p; own(c, [q] { cudaFreeHost(q); }); }
   return e;
+}
+// a finished group handed to the context: released by aloam_destroy
+inline void own(aloam_ctx* c, BufGroup&& g) {
+  BufGroup* q = new BufGroup(std::move(g));
+  own(c, [q] { delete q; });
 }
 inline cudaError_t screate(aloam_ctx* c, cudaStream_t* s) {
   const cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);

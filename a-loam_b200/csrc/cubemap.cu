@@ -107,9 +107,10 @@ struct aloam::Mapper {
 
 // The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
 // exclusive prefix of the snapshot's counts) and a hash grid over ALL of them, built once by prior_index; the centre offsets of
-// the store, which never change (no localising frame shifts the ring buffer); the layout of its ALOAM_EXPORT_MAP export.  Plain
-// cudaMalloc, freed by prior_map_release.
+// the store, which never change (no localising frame shifts the ring buffer); the layout of its ALOAM_EXPORT_MAP export.  Its
+// buffers, the digest's included, are one group, freed with the map by prior_map_release.
 struct aloam::PriorMap {
+  BufGroup mem;
   Pt4* pts[2] = {nullptr, nullptr};
   int n[2] = {0, 0};
   int cen[3] = {0, 0, 0};
@@ -1066,15 +1067,9 @@ int store_copy(aloam_ctx* c, const ExportLayout* L, long long n, char* mem, bool
 
 // ---- localisation: the prior map of a context and the lanes that register against it
 
-void prior_free(PriorMap* p) {
-  if (!p) return;
-  for (int t = 0; t < 2; ++t) { cudaFree(p->pts[t]); cudaFree(p->grid[t].slots); cudaFree(p->grid[t].dyn); cudaFree(p->grid[t].gpts); }
-  cudaFree(p->d_cube_start); cudaFree(p->d_n); cudaFree(p->d_layout); cudaFree(p->d_digest);
-  delete p;
-}
 // the one place a context's prior map is released: aloam_prior_map_clear, a load that replaces it, aloam_destroy
 void prior_map_release(aloam_ctx* c) {
-  prior_free(c->prior);
+  delete c->prior;
   c->prior = nullptr;
   for (Lane& L : c->lanes) L.window = false;   // the windows were cut from this map
 }
@@ -1121,17 +1116,15 @@ template <typename Fill> int prior_install(aloam_ctx* c, const int cen[3], const
     }
   }
   for (int a = 0; a < 3; ++a) p->cen[a] = cen[a];
-  bool ok = cudaMalloc(&p->d_cube_start, cs.size() * sizeof(int)) == cudaSuccess && cudaMalloc(&p->d_n, 2 * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&p->d_layout, sizeof(ExportLayout)) == cudaSuccess;
+  bool ok = p->mem.dev(&p->d_cube_start, cs.size()) && p->mem.dev(&p->d_n, 2) && p->mem.dev(&p->d_layout, 1);
   for (int t = 0; t < 2 && ok; ++t) {
     GridTable& g = p->grid[t];
     g.cap_slots = grid_mask_for(p->n[t], 1u << 30) + 1;
     g.cs = kMapCell; g.inv_cs = 1.0f / g.cs;
     const size_t n1 = (size_t)std::max(p->n[t], 1);
-    ok = cudaMalloc(&p->pts[t], n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&g.gpts, n1 * sizeof(float4)) == cudaSuccess &&
-         cudaMalloc(&g.slots, (size_t)g.cap_slots * sizeof(uint4)) == cudaSuccess && cudaMalloc(&g.dyn, sizeof(GridDyn)) == cudaSuccess;
+    ok = p->mem.dev(&p->pts[t], n1) && p->mem.dev(&g.gpts, n1) && p->mem.dev(&g.slots, (size_t)g.cap_slots) && p->mem.dev(&g.dyn, 1);
   }
-  auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); prior_free(p); return code; };
+  auto fail = [&](int code) { cudaStreamSynchronize(c->stream); cudaGetLastError(); delete p; return code; };
   if (!ok) return fail(ALOAM_ERR_CUDA);
   // the ALOAM_EXPORT_MAP layout of the packed clouds: segment 2 i + t is cube i of cloud t
   std::unique_ptr<ExportLayout> L(new (std::nothrow) ExportLayout());
@@ -1352,9 +1345,10 @@ __global__ void __launch_bounds__(kBuildTile) k_build_emit(const Pt4* __restrict
   *dst = o;
 }
 
-// the build's scratch, plain cudaMalloc: freed (after the stream has drained) when the call returns
+// the build's scratch, one group: freed (after the stream has drained) when the call returns
 struct BuildScratch {
   cudaStream_t stream;
+  BufGroup mem;
   Pt4* pts = nullptr;
   int *seg = nullptr, *cnt = nullptr, *bbox = nullptr, *dropped = nullptr, *off = nullptr, *vals[2] = {nullptr, nullptr}, *hist = nullptr;
   int *tile_heads = nullptr, *total = nullptr, *rank = nullptr, *n_dev = nullptr;
@@ -1362,25 +1356,16 @@ struct BuildScratch {
   unsigned char* head = nullptr;
   BuildSeg* par = nullptr;
   explicit BuildScratch(cudaStream_t s) : stream(s) {}
-  ~BuildScratch() {
+  ~BuildScratch() {   // runs before `mem` is freed
     cudaStreamSynchronize(stream);
     cudaGetLastError();
-    for (void* q : {(void*)pts, (void*)seg, (void*)cnt, (void*)bbox, (void*)dropped, (void*)off, (void*)vals[0], (void*)vals[1], (void*)hist,
-                    (void*)tile_heads, (void*)total, (void*)rank, (void*)n_dev, (void*)vox, (void*)keys[0], (void*)keys[1], (void*)head, (void*)par})
-      cudaFree(q);
   }
   bool alloc(size_t n, int tiles) {
     const size_t n1 = std::max<size_t>(n, 1);
-    return cudaMalloc(&pts, n1 * sizeof(Pt4)) == cudaSuccess && cudaMalloc(&seg, n1 * sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&cnt, kBuildSegs * sizeof(int)) == cudaSuccess && cudaMalloc(&bbox, 6 * kBuildSegs * sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&dropped, 2 * sizeof(int)) == cudaSuccess && cudaMalloc(&off, (kBuildSegs + 1) * sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&vals[0], n1 * sizeof(int)) == cudaSuccess && cudaMalloc(&vals[1], n1 * sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&hist, vox_radix_hist_ints((int)n1) * sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&tile_heads, (size_t)std::max(tiles, 1) * sizeof(int)) == cudaSuccess && cudaMalloc(&total, sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&rank, (kBuildSegs + 1) * sizeof(int)) == cudaSuccess && cudaMalloc(&n_dev, sizeof(int)) == cudaSuccess &&
-           cudaMalloc(&vox, n1 * sizeof(unsigned)) == cudaSuccess && cudaMalloc(&keys[0], n1 * sizeof(unsigned)) == cudaSuccess &&
-           cudaMalloc(&keys[1], n1 * sizeof(unsigned)) == cudaSuccess && cudaMalloc(&head, n1) == cudaSuccess &&
-           cudaMalloc(&par, kBuildSegs * sizeof(BuildSeg)) == cudaSuccess;
+    return mem.dev(&pts, n1) && mem.dev(&seg, n1) && mem.dev(&cnt, kBuildSegs) && mem.dev(&bbox, 6 * kBuildSegs) && mem.dev(&dropped, 2) &&
+           mem.dev(&off, kBuildSegs + 1) && mem.dev(&vals[0], n1) && mem.dev(&vals[1], n1) && mem.dev(&hist, vox_radix_hist_ints((int)n1)) &&
+           mem.dev(&tile_heads, (size_t)std::max(tiles, 1)) && mem.dev(&total, 1) && mem.dev(&rank, kBuildSegs + 1) && mem.dev(&n_dev, 1) &&
+           mem.dev(&vox, n1) && mem.dev(&keys[0], n1) && mem.dev(&keys[1], n1) && mem.dev(&head, n1) && mem.dev(&par, kBuildSegs);
   }
 };
 
@@ -1714,11 +1699,15 @@ int mapper_ensure(aloam_ctx* c, int lane) {
   // created here, after the context's (which fixes the table size)
   m->reg = lane == 0 ? &c->map : new (std::nothrow) MapReg();
   if (lane > 0 && m->reg) own(c, [r = m->reg] { delete r; });
-  ok = ok && m->reg && (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK && map_reg_alloc(c, m->reg) == ALOAM_OK));
-  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy
+  BufGroup g;
+  ok = ok && m->reg &&
+       (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK &&
+                      map_reg_alloc(g, m->reg, (size_t)2 * c->max_points, (size_t)c->max_map, (unsigned)c->map_slots) == ALOAM_OK));
+  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy, the set's group is freed
     cudaGetLastError();
     return ALOAM_ERR_CUDA;
   }
+  own(c, std::move(g));
   const int rc = reset_lane(c, m);   // a lane is published with the state of a fresh trajectory, never uninitialised
   if (rc) return rc;
   c->lanes[lane].mapper = m;
@@ -1732,10 +1721,12 @@ int locator_create(aloam_ctx* c, Locator** out) {
   Locator* m = new (std::nothrow) Locator();
   if (!m) return ALOAM_ERR_CUDA;
   own(c, [m] { delete m; });
+  BufGroup g;
   bool ok = dalloc(c, &m->d_state, 1) == cudaSuccess && halloc(c, &m->h_state, 1) == cudaSuccess;
-  ok = ok && map_reg_alloc(c, &m->reg, false) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
+  ok = ok && map_reg_alloc(g, &m->reg, (size_t)2 * c->max_points, 0, 0) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
   ok = ok && cudaMemset(m->d_state, 0, sizeof(MapperState)) == cudaSuccess;
   if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+  own(c, std::move(g));
   *out = m;
   return ALOAM_OK;
 }
@@ -1832,7 +1823,7 @@ int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps) {
 static int prior_map_digest(aloam_ctx* c, unsigned long long* out) {
   PriorMap* P = c->prior;
   if (!P->have_digest) {
-    if (!P->d_digest && cudaMalloc(&P->d_digest, sizeof(unsigned long long)) != cudaSuccess) { cudaGetLastError(); P->d_digest = nullptr; return ALOAM_ERR_CUDA; }
+    if (!P->d_digest && !P->mem.dev(&P->d_digest, 1)) return ALOAM_ERR_CUDA;
     const long long n = (long long)P->n[0] + P->n[1];
     const int blocks = (int)std::max<long long>(1, std::min<long long>((n + kDigestThreads - 1) / kDigestThreads, (long long)c->sms * 8));
     CUDA_CHECK_RET(cudaMemsetAsync(P->d_digest, 0, sizeof(unsigned long long), c->stream));

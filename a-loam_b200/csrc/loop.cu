@@ -58,7 +58,7 @@ struct aloam::Loop {
   aloam_loop_opts opt = {0.0, 0, 1, 1, 1.f};
   int cap = 0, bound = 0;                  // keyframes per lane in the pools; submap points per type, (2 window + 1) P
   std::vector<LoopLane> lanes;             // [n_lanes]
-  std::vector<void*> mem;                  // the per-lane buffers of the current setting
+  BufGroup mem;                            // the per-lane buffers of the current setting
   double* d_rz = nullptr;                  // [60][2]: sin, cos of s * pi / 60, from the host's libm
   LoopRowRec* d_rows = nullptr;            // [kMaxStreamScans], and its pinned copy
   LoopRowRec* h_rows = nullptr;
@@ -279,12 +279,6 @@ int verify_device(aloam_ctx* c, int nb, const Batch<LoopRec>& B, const int* lane
   return ALOAM_OK;
 }
 
-void loop_free(Loop* Lp) {
-  for (void* p : Lp->mem) cudaFree(p);
-  Lp->mem.clear();
-  Lp->lanes.clear();
-}
-
 // the context's Loop with its row tables and heading table, created on first use and released by aloam_destroy
 int loop_ensure(aloam_ctx* c) {
   if (c->loop) return ALOAM_OK;
@@ -295,19 +289,13 @@ int loop_ensure(aloam_ctx* c) {
     const double a = (double)s * 2.0 * M_PI / ALOAM_PLACE_SECTORS;
     rz[2 * s] = std::sin(a / 2); rz[2 * s + 1] = std::cos(a / 2);
   }
-  const bool ok = cudaMalloc((void**)&Lp->d_rz, sizeof(rz)) == cudaSuccess && cudaMemcpy(Lp->d_rz, rz, sizeof(rz), cudaMemcpyHostToDevice) == cudaSuccess &&
-                  cudaMalloc((void**)&Lp->d_rows, kMaxStreamScans * sizeof(LoopRowRec)) == cudaSuccess &&
-                  cudaMallocHost((void**)&Lp->h_rows, kMaxStreamScans * sizeof(LoopRowRec)) == cudaSuccess &&
-                  cudaMalloc((void**)&Lp->d_vrow, sizeof(LoopRowRec)) == cudaSuccess && cudaMallocHost((void**)&Lp->h_vrow, sizeof(LoopRowRec)) == cudaSuccess;
-  auto release = [Lp] {
-    loop_free(Lp);
-    for (void* p : {(void*)Lp->d_rz, (void*)Lp->d_rows, (void*)Lp->d_vrow}) if (p) cudaFree(p);
-    for (void* p : {(void*)Lp->h_rows, (void*)Lp->h_vrow}) if (p) cudaFreeHost(p);
-    delete Lp;
-  };
-  if (!ok) { cudaGetLastError(); release(); return ALOAM_ERR_CUDA; }
+  BufGroup g;
+  const bool ok = g.dev(&Lp->d_rz, 2 * ALOAM_PLACE_SECTORS) && cudaMemcpy(Lp->d_rz, rz, sizeof(rz), cudaMemcpyHostToDevice) == cudaSuccess &&
+                  g.dev(&Lp->d_rows, kMaxStreamScans) && g.pinned(&Lp->h_rows, kMaxStreamScans) && g.dev(&Lp->d_vrow, 1) && g.pinned(&Lp->h_vrow, 1);
+  if (!ok) { cudaGetLastError(); delete Lp; return ALOAM_ERR_CUDA; }
+  own(c, std::move(g));
+  own(c, [Lp] { delete Lp; });
   c->loop = Lp;
-  own(c, release);
   return ALOAM_OK;
 }
 
@@ -315,39 +303,18 @@ int loop_ensure(aloam_ctx* c) {
 // failure nothing of the old setting has changed
 int loop_alloc(aloam_ctx* c, int cap, int P, int bound) {
   Loop* Lp = c->loop;
-  std::vector<void*> mem;
+  BufGroup g;
   std::vector<LoopLane> lanes(c->n_lanes);
-  auto get = [&](void** p, size_t bytes) {
-    if (cudaMalloc(p, bytes) != cudaSuccess) return false;
-    mem.push_back(*p);
-    return true;
-  };
   unsigned slots = 1024;
   while (slots < (unsigned)bound + ((unsigned)bound >> 2)) slots <<= 1;
-  bool ok = true;
   for (LoopLane& L : lanes) {
     L = LoopLane{};
-    ok = ok && get((void**)&L.pool, (size_t)cap * 2 * P * sizeof(Pt4)) && get((void**)&L.pool_n, (size_t)cap * 2 * sizeof(int)) &&
-         get((void**)&L.sub[0], (size_t)bound * sizeof(Pt4)) && get((void**)&L.sub[1], (size_t)bound * sizeof(Pt4)) &&
-         get((void**)&L.st, sizeof(LoopState)) && get((void**)&L.reg.nbr, (size_t)2 * P * 5 * sizeof(float4)) &&
-         get((void**)&L.reg.blocks, (size_t)2 * P * sizeof(BlockRec)) && get((void**)&L.reg.summary, 4 * sizeof(LmSummary)) &&
-         get((void**)&L.reg.stack[0], (size_t)P * sizeof(Pt4)) && get((void**)&L.reg.stack[1], (size_t)P * sizeof(Pt4));
-    for (int t = 0; t < 2 && ok; ++t) {
-      GridTable& g = (t ? L.reg.surf : L.reg.corner).grid;
-      ok = get((void**)&g.slots, (size_t)slots * sizeof(uint4)) && get((void**)&g.dyn, sizeof(GridDyn)) && get((void**)&g.gpts, (size_t)bound * sizeof(float4));
-      g.cap_slots = slots; g.cs = kMapCell; g.inv_cs = 1.0f / g.cs;
-    }
-    if (ok) ok = cudaMemset(L.st, 0, sizeof(LoopState)) == cudaSuccess && cudaMemset(L.reg.corner.grid.dyn, 0, sizeof(GridDyn)) == cudaSuccess &&
-                 cudaMemset(L.reg.surf.grid.dyn, 0, sizeof(GridDyn)) == cudaSuccess;
-    if (!ok) break;
+    const bool ok = g.dev(&L.pool, (size_t)cap * 2 * P) && g.dev(&L.pool_n, (size_t)cap * 2) && g.dev(&L.sub[0], (size_t)bound) &&
+                    g.dev(&L.sub[1], (size_t)bound) && g.dev(&L.st, 1) && map_reg_alloc(g, &L.reg, (size_t)2 * P, (size_t)bound, slots) == ALOAM_OK &&
+                    cudaMemset(L.st, 0, sizeof(LoopState)) == cudaSuccess;
+    if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
   }
-  if (!ok) {
-    cudaGetLastError();
-    for (void* p : mem) cudaFree(p);
-    return ALOAM_ERR_CUDA;
-  }
-  loop_free(Lp);   // no frame reads the old buffers: every stream call drains before it returns
-  Lp->mem = std::move(mem);
+  Lp->mem.swap(g);   // no frame reads the old buffers: every stream call drains before it returns
   Lp->lanes = std::move(lanes);
   Lp->cap = cap;
   Lp->bound = bound;

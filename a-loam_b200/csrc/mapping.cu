@@ -699,22 +699,20 @@ bool is_device_ptr(const void* p) {
 }
 }  // namespace
 
-// the buffers of one registration set, its two grid tables (`grids`: a localising lane searches the prior map's and has none) sized for cfg.max_map_points (c->map_slots, fixed by
-// ensure_map_buffers, which creates the context's set before any other).  On failure what was acquired belongs to the context
-// until aloam_destroy.
-int map_reg_alloc(aloam_ctx* c, MapReg* r, bool grids) {
-  for (int t = 0; t < 2 && grids; ++t) {
-    GridTable& g = (t ? r->surf : r->corner).grid;
-    if (dalloc(c, &g.slots, (size_t)c->map_slots) != cudaSuccess || dalloc(c, &g.dyn, 1) != cudaSuccess || dalloc(c, &g.gpts, (size_t)c->max_map) != cudaSuccess ||
-        cudaMemset(g.dyn, 0, sizeof(GridDyn)) != cudaSuccess)
+// the buffers of one registration set in g: the 5-NN records and residual blocks of `queries` points, the two stacks of
+// queries / 2 points each and, with slots > 0, the two grid tables over submaps of up to `bound` points per type (`slots` slots
+// each; a localising lane searches the prior map's and passes 0)
+int map_reg_alloc(BufGroup& g, MapReg* r, size_t queries, size_t bound, unsigned slots) {
+  for (int t = 0; t < 2 && slots > 0; ++t) {
+    GridTable& gt = (t ? r->surf : r->corner).grid;
+    if (!g.dev(&gt.slots, slots) || !g.dev(&gt.dyn, 1) || !g.dev(&gt.gpts, bound) || cudaMemset(gt.dyn, 0, sizeof(GridDyn)) != cudaSuccess)
       return ALOAM_ERR_CUDA;
-    g.cap_slots = (unsigned)c->map_slots;
-    g.cs = kMapCell;
-    g.inv_cs = 1.0f / g.cs;
+    gt.cap_slots = slots;
+    gt.cs = kMapCell;
+    gt.inv_cs = 1.0f / gt.cs;
   }
-  const size_t mp = (size_t)c->max_points;
-  if (dalloc(c, &r->nbr, 2 * mp * 5) != cudaSuccess || dalloc(c, &r->blocks, 2 * mp) != cudaSuccess || dalloc(c, &r->summary, 4) != cudaSuccess ||
-      dalloc(c, &r->stack[0], mp) != cudaSuccess || dalloc(c, &r->stack[1], mp) != cudaSuccess)
+  if (!g.dev(&r->nbr, queries * 5) || !g.dev(&r->blocks, queries) || !g.dev(&r->summary, 4) || !g.dev(&r->stack[0], queries / 2) ||
+      !g.dev(&r->stack[1], queries / 2))
     return ALOAM_ERR_CUDA;
   return ALOAM_OK;
 }
@@ -729,9 +727,13 @@ int ensure_map_buffers(aloam_ctx* c) {
   while (slots < (unsigned)c->max_map + ((unsigned)c->max_map >> 2)) slots <<= 1;   // ends: aloam_create bounds max_map_points by 2^30
   c->map_slots = (int)slots;
   const size_t mm = (size_t)c->max_map, mp = (size_t)c->max_points;
-  if (dalloc(c, &c->d_map_pts[0], mm) != cudaSuccess || dalloc(c, &c->d_map_pts[1], mm) != cudaSuccess || map_reg_alloc(c, &c->map) != ALOAM_OK ||
+  BufGroup g;
+  MapReg r = {};
+  if (dalloc(c, &c->d_map_pts[0], mm) != cudaSuccess || dalloc(c, &c->d_map_pts[1], mm) != cudaSuccess || map_reg_alloc(g, &r, 2 * mp, mm, slots) != ALOAM_OK ||
       dalloc(c, &c->d_stack_counts, 4) != cudaSuccess || dalloc(c, &c->d_map_pose, 8) != cudaSuccess || dalloc(c, &c->d_fits, 2 * mp * 14) != cudaSuccess)
     return ALOAM_ERR_CUDA;
+  own(c, std::move(g));
+  c->map = r;
   c->map_ready = true;
   return ALOAM_OK;
 }

@@ -26,20 +26,25 @@ struct aloam::Place {
   aloam_place_opts opt = {80.f, 2.f, 0.0, 0, 1};
   int cap = 0;                                  // keyframes per lane the tables take (opt.max_keyframes)
   int alloc = 0;                                // keyframes per lane the tables have room for: the lanes' stride
+  BufGroup tables;                              // d_rec, d_norm: empty while recording has never been on
   char* d_rec = nullptr;                        // [n_lanes][alloc] records
   double* d_norm = nullptr;                     // [n_lanes][alloc][60]
   int* d_count = nullptr;                       // [n_lanes]
   int upper[ALOAM_MAX_BATCH] = {};              // host bound on each lane's count (the mapped rows since its table was cleared)
   aloam_place_row* d_rows = nullptr;            // [kMaxStreamScans], and its pinned copy
   aloam_place_row* h_rows = nullptr;
-  char* d_db = nullptr;                         // the database: M records and their norms
+  BufGroup db;                                  // the database: M records and their norms
+  char* d_db = nullptr;
   double* d_db_norm = nullptr;
   int db_n = 0;
-  Pt4* d_cloud[2] = {};                         // aloam_place_describe: the two uploaded clouds, and the descriptor
+  BufGroup describe;                            // aloam_place_describe: the two uploaded clouds, and the descriptor
+  Pt4* d_cloud[2] = {};
   float* d_desc = nullptr;
-  float* d_q = nullptr; long long q_cap = 0;    // aloam_place_query: the queries, the pairs' D and shift, the matches
-  double* d_dist = nullptr; int* d_shift = nullptr; long long pair_cap = 0;
+  BufGroup query;                               // aloam_place_query: the queries and the matches
+  float* d_q = nullptr; long long q_cap = 0;
   aloam_place_match* d_match = nullptr; long long match_cap = 0;
+  BufGroup pairs;                               // the pairs' D and shift, of the loop query and the database query
+  double* d_dist = nullptr; int* d_shift = nullptr; long long pair_cap = 0;
   int* d_err = nullptr;
 };
 
@@ -269,33 +274,32 @@ __global__ void k_place_load(const char* rec, double* norm, unsigned range_bits,
 
 unsigned bits_of(float f) { unsigned u; std::memcpy(&u, &f, 4); return u; }
 
-// the context's Place, created on first use and released by aloam_destroy
+// the context's Place with its error word, keyframe counts and row tables, created on first use and released by aloam_destroy
 int place_ensure(aloam_ctx* c) {
   if (c->place) return ALOAM_OK;
+  if (cudaFuncSetAttribute(k_place_dist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)place_dist_smem()) != cudaSuccess) {
+    cudaGetLastError(); return ALOAM_ERR_CUDA;
+  }
   Place* P = new (std::nothrow) Place();
   if (!P) return ALOAM_ERR_CUDA;
-  if (cudaMalloc((void**)&P->d_err, sizeof(int)) != cudaSuccess) { cudaGetLastError(); delete P; return ALOAM_ERR_CUDA; }
-  if (cudaFuncSetAttribute(k_place_dist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)place_dist_smem()) != cudaSuccess) {
-    cudaGetLastError(); cudaFree(P->d_err); delete P; return ALOAM_ERR_CUDA;
+  BufGroup g;
+  if (!g.dev(&P->d_err, 1) || !g.dev(&P->d_count, c->n_lanes) || !g.dev(&P->d_rows, kMaxStreamScans) || !g.pinned(&P->h_rows, kMaxStreamScans)) {
+    delete P; return ALOAM_ERR_CUDA;
   }
+  own(c, std::move(g));
+  own(c, [P] { delete P; });
   c->place = P;
-  own(c, [P] {
-    for (void* p : {(void*)P->d_err, (void*)P->d_rec, (void*)P->d_norm, (void*)P->d_count, (void*)P->d_rows, (void*)P->d_db, (void*)P->d_db_norm,
-                    (void*)P->d_cloud[0], (void*)P->d_cloud[1], (void*)P->d_desc, (void*)P->d_q, (void*)P->d_dist, (void*)P->d_shift, (void*)P->d_match})
-      if (p) cudaFree(p);
-    if (P->h_rows) cudaFreeHost(P->h_rows);
-    delete P;
-  });
   return ALOAM_OK;
 }
 
-// *p grown to n elements of T (its content is not kept)
-template <typename T> int grow(T** p, long long* cap, long long n) {
-  if (*cap >= n) return ALOAM_OK;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  if (cudaMalloc((void**)p, (size_t)n * sizeof(T)) != cudaSuccess) { cudaGetLastError(); *p = nullptr; return ALOAM_ERR_CUDA; }
-  *cap = n;
+// room for n pairs in the pair scratch: a smaller one is replaced (the caller has drained the stream); a failure leaves it as it was
+int pairs_reserve(Place* P, long long n) {
+  if (P->pair_cap >= n) return ALOAM_OK;
+  BufGroup g;
+  double* dist; int* shift;
+  if (!g.dev(&dist, (size_t)n) || !g.dev(&shift, (size_t)n)) return ALOAM_ERR_CUDA;
+  P->pairs.swap(g);
+  P->d_dist = dist; P->d_shift = shift; P->pair_cap = n;
   return ALOAM_OK;
 }
 
@@ -309,7 +313,7 @@ PlaceSets db_sets(const Place* P) {
 
 int place_clear(aloam_ctx* c, int lane) {
   Place* P = c->place;
-  if (!P || !P->d_count) return ALOAM_OK;
+  if (!P || P->tables.empty()) return ALOAM_OK;
   const int l0 = lane < 0 ? 0 : lane, nl = lane < 0 ? c->n_lanes : 1;
   CUDA_CHECK_RET(cudaMemsetAsync(P->d_count + l0, 0, nl * sizeof(int), c->stream));
   for (int l = l0; l < l0 + nl; ++l) P->upper[l] = 0;
@@ -327,7 +331,7 @@ PlaceTable place_table(aloam_ctx* c, int lane) {
 int place_record_device(aloam_ctx* c, int nb, const MapperIn* in, const int* scan, const bool* start, aloam_place_row* const* rows, int* n_upper_out) {
   if (n_upper_out) *n_upper_out = 0;
   Place* P = c->place;
-  if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || !P->d_count) return ALOAM_ERR_STATE;
+  if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || P->tables.empty()) return ALOAM_ERR_STATE;
   Batch<PlaceGate> G = {};
   PlaceSets S = {};
   int n_upper = 0;   // the most candidates a record can query: its new keyframe's index is at most its lane's bound
@@ -366,37 +370,21 @@ int aloam_set_place(aloam_ctx* c, int on, const aloam_place_opts* opts) {
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (int rc = place_ensure(c)) return rc;
   Place* P = c->place;
-  if (on && P->alloc < o.max_keyframes) {   // the tables of every lane, the row table and the loop query's pairs
+  if (on && P->alloc < o.max_keyframes) {   // the tables of every lane, and the loop query's pairs
     const size_t L = c->n_lanes, K = o.max_keyframes;
-    char* rec = nullptr; double* norm = nullptr; int* count = P->d_count;
-    aloam_place_row *drows = P->d_rows, *hrows = P->h_rows;
-    long long cd = P->pair_cap, cs = P->pair_cap;
-    bool ok = cudaMalloc((void**)&rec, L * K * kRec) == cudaSuccess && cudaMalloc((void**)&norm, L * K * kSectors * sizeof(double)) == cudaSuccess;
-    if (ok && !count) ok = cudaMalloc((void**)&count, L * sizeof(int)) == cudaSuccess;
-    if (ok && !drows) ok = cudaMalloc((void**)&drows, kMaxStreamScans * sizeof(aloam_place_row)) == cudaSuccess;
-    if (ok && !hrows) ok = cudaMallocHost((void**)&hrows, kMaxStreamScans * sizeof(aloam_place_row)) == cudaSuccess;
-    if (ok) {   // the loop query's pairs share the database query's scratch (nothing runs on it between calls)
-      CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-      ok = !grow(&P->d_dist, &cd, (long long)(L * K)) && !grow(&P->d_shift, &cs, (long long)(L * K));
-      P->pair_cap = std::min(cd, cs);
-    }
-    if (!ok) {
-      cudaGetLastError();
-      if (rec) cudaFree(rec);
-      if (norm) cudaFree(norm);
-      if (count && count != P->d_count) cudaFree(count);
-      if (drows && drows != P->d_rows) cudaFree(drows);
-      if (hrows && hrows != P->h_rows) cudaFreeHost(hrows);
-      return ALOAM_ERR_CUDA;
-    }
-    if (P->d_rec) cudaFree(P->d_rec);   // no frame reads the old tables: every stream call drains before it returns
-    if (P->d_norm) cudaFree(P->d_norm);
-    P->d_rec = rec; P->d_norm = norm; P->d_count = count; P->d_rows = drows; P->h_rows = hrows; P->alloc = o.max_keyframes;
+    BufGroup tables;
+    char* rec; double* norm;
+    if (!tables.dev(&rec, L * K * kRec) || !tables.dev(&norm, L * K * kSectors)) return ALOAM_ERR_CUDA;
+    // the loop query's pairs share the database query's scratch (nothing runs on it between calls)
+    CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
+    if (int rc = pairs_reserve(P, (long long)(L * K))) return rc;
+    P->tables.swap(tables);   // no frame reads the old tables: every stream call drains before it returns
+    P->d_rec = rec; P->d_norm = norm; P->alloc = o.max_keyframes;
   }
   P->opt = o;
   P->cap = std::min(o.max_keyframes, P->alloc);
   c->loop_on = false;   // the keyframe clouds belong to the tables this call clears (aloam_set_loops turns them on again)
-  if (P->d_count) {
+  if (!P->tables.empty()) {
     CUDA_CHECK_RET(cudaMemsetAsync(P->d_count, 0, c->n_lanes * sizeof(int), c->stream));
     CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
     for (int& u : P->upper) u = 0;
@@ -417,7 +405,7 @@ int aloam_place_rows(aloam_ctx* c, aloam_place_row* out, int rows) {
 int aloam_place_keyframes(aloam_ctx* c, int lane, void* out, long long capacity, long long* n_out) {
   if (!c || !n_out || lane < 0 || lane >= c->n_lanes || capacity < 0 || (capacity > 0 && !out)) return ALOAM_ERR_INVALID_ARG;
   const Place* P = c->place;
-  if (!P || !P->d_count) return ALOAM_ERR_STATE;
+  if (!P || P->tables.empty()) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   int n = 0;
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
@@ -434,11 +422,9 @@ int aloam_place_db_load(aloam_ctx* c, const void* records, int n_records) {
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (int rc = place_ensure(c)) return rc;
   Place* P = c->place;
-  char* rec = nullptr; double* norm = nullptr;
-  if (cudaMalloc((void**)&rec, (size_t)n_records * kRec) != cudaSuccess ||
-      cudaMalloc((void**)&norm, (size_t)n_records * kSectors * sizeof(double)) != cudaSuccess) {
-    cudaGetLastError(); if (rec) cudaFree(rec); return ALOAM_ERR_CUDA;
-  }
+  BufGroup db;
+  char* rec; double* norm;
+  if (!db.dev(&rec, (size_t)n_records * kRec) || !db.dev(&norm, (size_t)n_records * kSectors)) return ALOAM_ERR_CUDA;
   int err = 0;
   cudaError_t e = cudaMemcpyAsync(rec, records, (size_t)n_records * kRec, cudaMemcpyDefault, c->stream);
   if (e == cudaSuccess) e = cudaMemsetAsync(P->d_err, 0, sizeof(int), c->stream);
@@ -446,11 +432,10 @@ int aloam_place_db_load(aloam_ctx* c, const void* records, int n_records) {
   if (e == cudaSuccess) e = cudaMemcpyAsync(&err, P->d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess || err) {
-    cudaGetLastError(); cudaFree(rec); cudaFree(norm);
+    cudaGetLastError();
     return e != cudaSuccess ? ALOAM_ERR_CUDA : ALOAM_ERR_INVALID_ARG;
   }
-  if (P->d_db) cudaFree(P->d_db);
-  if (P->d_db_norm) cudaFree(P->d_db_norm);
+  P->db.swap(db);
   P->d_db = rec; P->d_db_norm = norm; P->db_n = n_records;
   return ALOAM_OK;
 }
@@ -461,7 +446,7 @@ int aloam_place_db_clear(aloam_ctx* c) {
   if (!P || !P->d_db) return ALOAM_OK;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  cudaFree(P->d_db); cudaFree(P->d_db_norm);
+  P->db = BufGroup();
   P->d_db = nullptr; P->d_db_norm = nullptr; P->db_n = 0;
   return ALOAM_OK;
 }
@@ -474,10 +459,12 @@ int aloam_place_describe(aloam_ctx* c, aloam_cloud_view less_sharp, aloam_cloud_
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   if (int rc = place_ensure(c)) return rc;
   Place* P = c->place;
-  if (!P->d_desc) {
-    long long cap0 = 0, cap1 = 0, capd = 0;
-    if (grow(&P->d_cloud[0], &cap0, c->max_points) || grow(&P->d_cloud[1], &cap1, c->max_points) || grow(&P->d_desc, &capd, (long long)kBins))
-      return ALOAM_ERR_CUDA;
+  if (P->describe.empty()) {
+    BufGroup g;
+    Pt4* cloud[2]; float* desc;
+    if (!g.dev(&cloud[0], c->max_points) || !g.dev(&cloud[1], c->max_points) || !g.dev(&desc, kBins)) return ALOAM_ERR_CUDA;
+    P->describe.swap(g);
+    P->d_cloud[0] = cloud[0]; P->d_cloud[1] = cloud[1]; P->d_desc = desc;
   }
   if (int rc = upload_cloud(c, less_sharp, P->d_cloud[0], c->max_points)) return rc;
   if (int rc = upload_cloud(c, less_flat, P->d_cloud[1], c->max_points)) return rc;
@@ -497,12 +484,18 @@ int aloam_place_query(aloam_ctx* c, const float* descs, int n_query, int k, aloa
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   const int M = P->db_n;
   const int chunk = (int)std::max(1LL, std::min((long long)n_query, kMaxPairs / M));   // queries per launch pair
-  if (grow(&P->d_q, &P->q_cap, (long long)n_query * kBins) || grow(&P->d_match, &P->match_cap, (long long)n_query * k)) return ALOAM_ERR_CUDA;
+  const long long need_q = (long long)n_query * kBins, need_m = (long long)n_query * k;
+  if (P->q_cap < need_q || P->match_cap < need_m) {   // either buffer grown to what this call needs, the other kept at its size
+    BufGroup g;
+    const long long q_cap = std::max(P->q_cap, need_q), match_cap = std::max(P->match_cap, need_m);
+    float* q; aloam_place_match* match;
+    if (!g.dev(&q, (size_t)q_cap) || !g.dev(&match, (size_t)match_cap)) return ALOAM_ERR_CUDA;
+    P->query.swap(g);
+    P->d_q = q; P->q_cap = q_cap; P->d_match = match; P->match_cap = match_cap;
+  }
   if (P->pair_cap < (long long)chunk * M) {
     CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-    long long cd = P->pair_cap, cs = P->pair_cap;
-    if (grow(&P->d_dist, &cd, (long long)chunk * M) || grow(&P->d_shift, &cs, (long long)chunk * M)) { P->pair_cap = 0; return ALOAM_ERR_CUDA; }
-    P->pair_cap = (long long)chunk * M;
+    if (int rc = pairs_reserve(P, (long long)chunk * M)) return rc;
   }
   CUDA_CHECK_RET(cudaMemcpyAsync(P->d_q, descs, (size_t)n_query * kBins * sizeof(float), cudaMemcpyDefault, c->stream));
   for (int q0 = 0; q0 < n_query; q0 += chunk) {

@@ -13,12 +13,13 @@
 #include "ctx.h"
 #include "quat.cuh"
 
-// the setting and the buffers, created by the first aloam_set_recovery that turns recovery on and grown by later ones (plain
-// cudaMalloc, freed by recover_free); per lane l a slice of `cap` candidates, scores, ctas x kRelocTop CTA keys and kRelocTop best keys
+// the setting and the buffers, created by the first aloam_set_recovery that turns recovery on and replaced by larger ones as later
+// calls need (one group); per lane l a slice of `cap` candidates, scores, ctas x kRelocTop CTA keys and kRelocTop best keys
 struct aloam::Recovery {
   float trigger_frac = 0.f, accept_frac = 0.f;
   int n_delta = 0, cap = 0;
   int ctas = 0, ctas_cap = 0;                // CTAs of a record's k_reloc_score launch; the key slices are sized for ctas_cap
+  BufGroup mem;
   double* d_delta = nullptr;                 // [cap][7] normalised deltas
   double* d_cand = nullptr;                  // [ALOAM_MAX_BATCH][cap][7]
   int* d_score = nullptr;                    // [ALOAM_MAX_BATCH][cap]
@@ -62,35 +63,26 @@ __global__ void __launch_bounds__(kCandThreads) k_recover_cand(const __grid_cons
   for (int k = 0; k < 3; ++k) o[4 + k] = P[4 + k] + d[4 + k];
 }
 
-void recover_free(Recovery* R) {
-  cudaFree(R->d_delta); cudaFree(R->d_cand); cudaFree(R->d_score); cudaFree(R->d_part); cudaFree(R->d_best);
-  delete R;
-}
-
 // room for n candidates and `ctas` CTA key lists per lane (a failure leaves the buffers as they were)
 int recover_ensure(aloam_ctx* c, int n, int ctas) {
   if (!c->recover) {
     Recovery* R = new (std::nothrow) Recovery();
     if (!R) return ALOAM_ERR_CUDA;
-    own(c, [R] { recover_free(R); });
+    own(c, [R] { delete R; });
     c->recover = R;
   }
   Recovery* R = c->recover;
   if (n <= R->cap && ctas <= R->ctas_cap) return ALOAM_OK;
   const int cap = std::max(n, R->cap), ctas_cap = std::max(ctas, R->ctas_cap);
-  double *delta = nullptr, *cand = nullptr;
-  int* score = nullptr;
-  unsigned long long *part = nullptr, *best = nullptr;
+  BufGroup g;
+  double *delta, *cand;
+  int* score;
+  unsigned long long *part, *best;
   const size_t L = ALOAM_MAX_BATCH;
-  const bool ok = cudaMalloc(&delta, (size_t)cap * 7 * sizeof(double)) == cudaSuccess &&
-                  cudaMalloc(&cand, L * cap * 7 * sizeof(double)) == cudaSuccess && cudaMalloc(&score, L * cap * sizeof(int)) == cudaSuccess &&
-                  cudaMalloc(&part, L * ctas_cap * kRelocTop * sizeof(unsigned long long)) == cudaSuccess &&
-                  cudaMalloc(&best, L * kRelocTop * sizeof(unsigned long long)) == cudaSuccess;
-  if (!ok) {
-    cudaFree(delta); cudaFree(cand); cudaFree(score); cudaFree(part); cudaFree(best); cudaGetLastError();
+  if (!g.dev(&delta, (size_t)cap * 7) || !g.dev(&cand, L * cap * 7) || !g.dev(&score, L * cap) || !g.dev(&part, L * ctas_cap * kRelocTop) ||
+      !g.dev(&best, L * kRelocTop))
     return ALOAM_ERR_CUDA;
-  }
-  cudaFree(R->d_delta); cudaFree(R->d_cand); cudaFree(R->d_score); cudaFree(R->d_part); cudaFree(R->d_best);
+  R->mem.swap(g);
   R->d_delta = delta; R->d_cand = cand; R->d_score = score; R->d_part = part; R->d_best = best;
   R->cap = cap; R->ctas_cap = ctas_cap;
   return ALOAM_OK;

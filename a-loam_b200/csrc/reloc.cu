@@ -29,8 +29,9 @@ constexpr int kMaxHyp = 1 << 24;
 
 // The relocaliser's scratch, created on first use: the K locators (a localising lane's registration set each, context-owned,
 // created as calls need them), the uploaded clouds and the per-call buffers.  The hypothesis buffers grow with the largest call
-// and are plain cudaMalloc, freed by reloc_free.
+// (group `hyps`); the others are group `mem`.
 struct aloam::Relocaliser {
+  BufGroup mem, hyps;
   Locator* loc[ALOAM_MAX_BATCH] = {};
   int n_loc = 0;
   Pt4* d_in[2] = {nullptr, nullptr};
@@ -182,26 +183,22 @@ int reloc_score_ctas(aloam_ctx* c, int n_hyp) {
 
 namespace {
 
-void reloc_free(Relocaliser* R) {
-  cudaFree(R->d_hyp);
-  cudaFree(R->d_score);
-  delete R;
-}
-
-// the relocaliser with at least `k` locators and room for n_hyp hypotheses (a failure leaves what exists as it was)
+// the relocaliser with at least `k` locators and room for n_hyp hypotheses (a failure leaves what exists as it was); it is
+// published only complete, a failed first attempt freed at once
 int reloc_ensure(aloam_ctx* c, int k, int n_hyp) {
   if (!c->reloc) {
     Relocaliser* R = new (std::nothrow) Relocaliser();
     if (!R) return ALOAM_ERR_CUDA;
-    own(c, [R] { reloc_free(R); });
     int per_sm = 0;
     bool ok = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reloc_score, kRelocWarps * 32, 0) == cudaSuccess;
     R->ctas = c->sms * std::max(per_sm, 1);
-    ok = ok && dalloc(c, &R->d_in[0], (size_t)c->max_points) == cudaSuccess && dalloc(c, &R->d_in[1], (size_t)c->max_points) == cudaSuccess;
-    ok = ok && dalloc(c, &R->d_n, 2) == cudaSuccess && dalloc(c, &R->d_part, (size_t)R->ctas * kTop) == cudaSuccess;
-    ok = ok && dalloc(c, &R->d_best, kTop) == cudaSuccess && dalloc(c, &R->d_pose, kTop * 7) == cudaSuccess;
-    ok = ok && dalloc(c, &R->d_rscore, kTop) == cudaSuccess && halloc(c, &R->h, 1) == cudaSuccess;
-    if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+    BufGroup& g = R->mem;
+    ok = ok && g.dev(&R->d_in[0], (size_t)c->max_points) && g.dev(&R->d_in[1], (size_t)c->max_points);
+    ok = ok && g.dev(&R->d_n, 2) && g.dev(&R->d_part, (size_t)R->ctas * kTop);
+    ok = ok && g.dev(&R->d_best, kTop) && g.dev(&R->d_pose, kTop * 7);
+    ok = ok && g.dev(&R->d_rscore, kTop) && g.pinned(&R->h, 1);
+    if (!ok) { cudaGetLastError(); delete R; return ALOAM_ERR_CUDA; }
+    own(c, [R] { delete R; });
     c->reloc = R;
   }
   Relocaliser* R = c->reloc;
@@ -210,13 +207,11 @@ int reloc_ensure(aloam_ctx* c, int k, int n_hyp) {
     ++R->n_loc;
   }
   if (n_hyp > R->cap) {
-    double* hyp = nullptr;
-    int* sc = nullptr;
-    if (cudaMalloc(&hyp, (size_t)n_hyp * 7 * sizeof(double)) != cudaSuccess || cudaMalloc(&sc, (size_t)n_hyp * sizeof(int)) != cudaSuccess) {
-      cudaFree(hyp); cudaFree(sc); cudaGetLastError();
-      return ALOAM_ERR_CUDA;
-    }
-    cudaFree(R->d_hyp); cudaFree(R->d_score);
+    BufGroup g;
+    double* hyp;
+    int* sc;
+    if (!g.dev(&hyp, (size_t)n_hyp * 7) || !g.dev(&sc, (size_t)n_hyp)) return ALOAM_ERR_CUDA;
+    R->hyps.swap(g);
     R->d_hyp = hyp; R->d_score = sc; R->cap = n_hyp;
   }
   return ALOAM_OK;
