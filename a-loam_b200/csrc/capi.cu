@@ -572,7 +572,7 @@ struct StreamSwitches {
   // registered clouds (aloam_set_registered_sink): every mapped row's ring-major cloud is stashed with its feature slot by stage C
   // and moved into the world by k_register_full after the row's mapper frame; without a sink none of this is issued
   bool sink;
-  // per-row records (aloam_set_map_rows): k_map_rows after every frame, k_track_score after every localising frame when scoring is
+  // per-row records (aloam_set_map_rows): k_map_rows after every frame, the tracking score after every localising frame when scoring is
   // on; without recording none of this is issued
   bool rec, score;
   bool recov;          // recovery of localising lanes (aloam_set_recovery, recover.cu): four more launches after every scored localising frame

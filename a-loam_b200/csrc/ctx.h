@@ -59,10 +59,11 @@ struct LmHead {
   int n_edge, n_plane;
   double initial_cost, final_cost;
 };
-// one row of a mapped stream call as k_map_rows (cubemap.cu) and k_track_score (rows.cu) leave it on the device: the frame's
-// flags and error word, its window and stack sizes, the summaries of its outer iterations and its prior-map inlier score (-1: not
-// scored; k_track_score adds to 0).  With recovery on (aloam_set_recovery), a localising row also holds what its recovery did:
-// k_recover_cand (recover.cu) sets rec_triggered, k_recover_adopt (cubemap.cu) the rest of a triggered row.
+// one row of a mapped stream call as k_map_rows (cubemap.cu) and the tracking score (rows.cu, k_inlier_score in reloc.cu) leave it
+// on the device: the frame's flags and error word, its window and stack sizes, the summaries of its outer iterations and its
+// prior-map inlier score (-1: not scored; k_inlier_score adds to 0).  With recovery on (aloam_set_recovery), a localising row also
+// holds what its recovery did: k_recover_cand (recover.cu) sets rec_triggered, k_recover_adopt (cubemap.cu) the rest of a
+// triggered row.
 struct MapRowRec {
   int flags, err, n_valid, n_sub[2], n_stack[2], score, n_score, pad;
   LmHead lm[4];
@@ -70,8 +71,9 @@ struct MapRowRec {
   double rec_pose[7];
 };
 // one hypothesis set of k_reloc_score / k_reloc_topk (reloc.cu): n_hyp normalised poses (7 doubles each) scored against the
-// stacks (sizes counts[0], counts[1]) into score[h]; part (may be null): the CTAs' best keys, kRelocTop per CTA; best: the best
-// keys of the set; gate (may be null): the set is ranked only when *gate != 0 -- its CTAs leave at once otherwise
+// stacks (sizes counts[0], counts[1]) into score[h] through warp_inliers (grid.cuh), as inlier_score_device scores one pose;
+// part (may be null): the CTAs' best keys, kRelocTop per CTA; best: the best keys of the set; gate (may be null): the set is
+// ranked only when *gate != 0 -- its CTAs leave at once otherwise
 struct RelocRec {
   const double* hyp;
   int n_hyp;
@@ -82,12 +84,14 @@ struct RelocRec {
   unsigned long long* best;
   const int* gate;
 };
-// one record of k_track_score: the localising frame's filtered stacks and their sizes, the row's map pose and its row slot
-struct TrackArgs {
+// one record of k_inlier_score (reloc.cu): stacks of sizes counts[0], counts[1] scored at one pose against the corner and surf
+// grids; the count is added to *score
+struct ScoreRec {
   const Pt4* stack[2];
   const int* counts;
   const double* pose;
-  MapRowRec* row;
+  GridTable grid[2];
+  int* score;
 };
 // Buffers that a later call replaces as a whole (a larger table, a new map): a replacement group is filled on the side and
 // swapped in only when every allocation in it succeeded; the group it replaces is freed as a whole by its destructor.  Nothing
@@ -458,6 +462,10 @@ int track_score_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* cons
 void reloc_score_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int max_pts, float inlier_sq);
 void reloc_topk_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int rounds);
 int reloc_score_ctas(aloam_ctx* c, int n_hyp);
+// one pose per record (reloc.cu): k_inlier_score under profile id kid over records B.a[0 .. nb-1], parallel over the scoring
+// points (max_pts per type; m_upper: the host's bound on any record's scoring points sizes the grid), inliers at float d2 <
+// inlier_sq added to each record's *score; tracking scores (rows.cu) and loop verification (loop.cu) launch it
+void inlier_score_device(aloam_ctx* c, int kid, int nb, const Batch<ScoreRec>& B, long long m_upper, int max_pts, float inlier_sq);
 // recovery of localising lanes (recover.cu): after track_score_device, the recovery of the frame's nb localising records, whose
 // scored rows are rows[l]; and its last kernel (cubemap.cu), which adopts record l's best candidate (of cand[l], best key *best[l])
 int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows);

@@ -32,6 +32,7 @@
 #include <memory>
 #include "common.cuh"
 #include "ctx.h"
+#include "grid.cuh"
 #include "quat.cuh"
 
 namespace {
@@ -1586,8 +1587,8 @@ struct MapRowLane {
 };
 
 // the rows of a frame's records, grid (1, 1, records) x 32 threads, after the frame's last kernel: thread t < outer copies the head
-// of outer iteration t's summary, thread 0 the frame's flags, error word and sizes.  A scored row starts its count at 0 for
-// k_track_score and records the scoring points it covers.
+// of outer iteration t's summary, thread 0 the frame's flags, error word and sizes.  A scored row starts its count at 0 for the
+// tracking score (k_inlier_score) and records the scoring points it covers.
 __global__ void __launch_bounds__(32) k_map_rows(const __grid_constant__ Batch<MapRowLane> B, int outer) {
   const MapRowLane& a = B.a[blockIdx.z];
   const MapperState* S = a.S;
@@ -1600,7 +1601,7 @@ __global__ void __launch_bounds__(32) k_map_rows(const __grid_constant__ Batch<M
   if (t == 0) {
     r->flags = S->flags; r->err = S->frame_err; r->n_valid = S->n_valid;
     for (int k = 0; k < 2; ++k) { r->n_sub[k] = S->n_sub[k]; r->n_stack[k] = S->stack_counts[k]; }
-    const int m = a.max_score > 0 ? min(S->stack_counts[0], a.max_score) + min(S->stack_counts[1], a.max_score) : 0;
+    const int m = a.max_score > 0 ? scoring_points(S->stack_counts[0], S->stack_counts[1], a.max_score) : 0;
     r->score = a.max_score > 0 ? 0 : -1;
     r->n_score = m;
   }

@@ -1,6 +1,7 @@
-// The map hash grid's cell keys and probes, shared by the scan-to-map search (mapping.cu), the relocaliser's scoring (reloc.cu)
-// and the tracking score of per-row records (rows.cu): all must find a point's cell under the same key and hash, and the two
-// scores must pick and test their points alike.
+// The map hash grid's cell keys and probes, shared by the scan-to-map search (mapping.cu) and every prior-map or keyframe inlier
+// score (reloc.cu: k_reloc_score, k_inlier_score): all must find a point's cell under the same key and hash.  Every score picks
+// its points with scoring_point / scoring_points and counts a warp's moved points with warp_inliers, so scores of one pose taken
+// by different kernels are equal (recovery compares a candidate's k_reloc_score count with its row's k_inlier_score count).
 #pragma once
 #include "kernels.h"
 
@@ -72,10 +73,31 @@ __device__ __forceinline__ bool any_in_block27(const GridTable& g, unsigned mask
   return false;
 }
 
+// the scoring points of stacks of n_c corner and n_s surf points: at most max_pts of each type, m_c = min(n_c, max_pts) corner
+// points first
+__device__ __forceinline__ int scoring_points(int n_c, int n_s, int max_pts) { return min(n_c, max_pts) + min(n_s, max_pts); }
+
 // scoring point i (< m_c + m_s): corner stack point floor(i n_c / m_c), or surf stack point floor((i - m_c) n_s / m_s)
 __device__ __forceinline__ float4 scoring_point(const Pt4* __restrict__ corner, const Pt4* __restrict__ surf, int n_c, int m_c, int n_s, int m_s, int i) {
   const Pt4 p = i < m_c ? corner[(long long)i * n_c / m_c] : surf[(long long)(i - m_c) * n_s / m_s];
   return make_float4(p.x, p.y, p.z, p.i);
+}
+
+// cnt plus the inliers among scoring points p0 .. p0 + np - 1 (np <= 32) once moved: lane j holds point p0 + j at (qx, qy, qz);
+// points below m_c are corner points.  The warp walks the points in turn, each through any_in_block27 over its type's grid (mask:
+// the grid's dyn->mask, hoisted by the caller), and a point is an inlier when some map point lies at float d2 < inlier_sq: it
+// needs a map point, not the nearest one.  Warp-uniform; every lane takes part and gets the count.  (The running count goes in
+// rather than being added to the result: k_reloc_score then keeps its 55 registers.)
+__device__ __forceinline__ int warp_inliers(int cnt, float qx, float qy, float qz, int p0, int np, int m_c, const GridTable& corner,
+                                            unsigned mask_c, const GridTable& surf, unsigned mask_s, float inlier_sq) {
+  for (int j = 0; j < np; ++j) {
+    const float px = __shfl_sync(0xffffffffu, qx, j), py = __shfl_sync(0xffffffffu, qy, j), pz = __shfl_sync(0xffffffffu, qz, j);
+    const bool is_corner = p0 + j < m_c;
+    const bool in = any_in_block27(is_corner ? corner : surf, is_corner ? mask_c : mask_s, px, py, pz,
+                                   [&](float u, float v, float w) { return sqdist3(u, v, w, px, py, pz) < inlier_sq; });
+    cnt += in ? 1 : 0;
+  }
+  return cnt;
 }
 
 }  // namespace aloam

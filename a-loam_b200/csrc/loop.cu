@@ -11,11 +11,11 @@
 //     does, so the solve leaves the pose alone) and the initial pose.  An untriggered record writes zero sizes.
 //   * then the mapper's own code: k_grid_setup + the K0 index build over the lanes' loop sets, map_register_device with the
 //     verification's round count.
-//   * k_loop_score: the relocaliser's inlier count of the query's stored points at the refined pose, through the 27-cell walk of
-//     grid.cuh over each record's own grid -- one warp per 32 points, one atomic per warp: an integer, independent of order.
+//   * the score: the relocaliser's inlier count of the query's stored points at the refined pose against the lane's registration
+//     set's own grids, one launch of k_inlier_score (reloc.cu) with max_pts = cloud_points.  A stored cloud holds at most
+//     cloud_points points per type, so every stored point is a scoring point, taken once.
 //   * k_loop_finish: the constraint T_c^-1 * pose in Eigen's operation order, and the row (sizes, score, last round's summary head).
 #include "ctx.h"
-#include "grid.cuh"
 #include "quat.cuh"
 
 namespace {
@@ -23,7 +23,6 @@ constexpr int kRec = ALOAM_PLACE_RECORD_BYTES;
 constexpr int kMaxWindow = 64, kMaxSpan = 2 * kMaxWindow + 1;
 constexpr int kMaxRounds = 16;
 constexpr int kLoopThreads = 256;
-constexpr int kScoreWarps = 8;
 
 // what a verification leaves on the device for the kernels after k_loop_gather (one per lane)
 struct LoopState {
@@ -108,7 +107,6 @@ struct LoopRec {
   LoopState* st;
   LoopRowRec* row;
   const LmSummary* summary;
-  GridTable grid[2];
   int q, c, s, has_init;
   double init[7];
 };
@@ -189,35 +187,6 @@ __global__ void __launch_bounds__(kLoopThreads) k_loop_gather(const __grid_const
   }
 }
 
-// grid (CTAs, 1, records), kScoreWarps warps: warp w of CTA b takes the query points 32 (b kScoreWarps + w) .. + 31
-__global__ void __launch_bounds__(kScoreWarps * 32, 4) k_loop_score(const __grid_constant__ Batch<LoopRec> B, float inlier_sq) {
-  const LoopRec& a = B.a[blockIdx.z];
-  LoopState* st = a.st;
-  const int n_c = st->n_q[0], m = n_c + st->n_q[1];
-  const int p0 = (blockIdx.x * kScoreWarps + (threadIdx.x >> 5)) * 32;
-  if (p0 >= m) return;   // warp-uniform
-  const unsigned lane = lane_id();
-  float qx = 0.f, qy = 0.f, qz = 0.f;
-  if (p0 + (int)lane < m) {
-    const int i = p0 + (int)lane;
-    const Pt4 p = i < n_c ? a.stack[0][i] : a.stack[1][i - n_c];
-    const double* x = st->pose;
-    const Pt4 r = point_associate_to_map(p, x[0], x[1], x[2], x[3], x[4], x[5], x[6]);
-    qx = r.x; qy = r.y; qz = r.z;
-  }
-  const unsigned mask_c = a.grid[0].dyn->mask, mask_s = a.grid[1].dyn->mask;
-  const int np = min(32, m - p0);
-  int cnt = 0;
-  for (int j = 0; j < np; ++j) {
-    const float px = __shfl_sync(0xffffffffu, qx, j), py = __shfl_sync(0xffffffffu, qy, j), pz = __shfl_sync(0xffffffffu, qz, j);
-    const bool is_corner = p0 + j < n_c;
-    const bool in = any_in_block27(a.grid[is_corner ? 0 : 1], is_corner ? mask_c : mask_s, px, py, pz,
-                                   [&](float u, float v, float w) { return sqdist3(u, v, w, px, py, pz) < inlier_sq; });
-    cnt += in ? 1 : 0;
-  }
-  if (lane == 0 && cnt) atomicAdd(&st->score, cnt);
-}
-
 // grid (records), 32 threads
 __global__ void __launch_bounds__(32) k_loop_finish(const __grid_constant__ Batch<LoopRec> B, int last_round) {
   const LoopRec& a = B.a[blockIdx.x];
@@ -251,7 +220,6 @@ LoopRec lane_rec(aloam_ctx* c, int lane) {
   r.stack[0] = L.reg.stack[0]; r.stack[1] = L.reg.stack[1];
   r.sub[0] = L.sub[0]; r.sub[1] = L.sub[1];
   r.st = L.st; r.summary = L.reg.summary;
-  r.grid[0] = L.reg.corner.grid; r.grid[1] = L.reg.surf.grid;
   return r;
 }
 
@@ -265,15 +233,17 @@ int verify_device(aloam_ctx* c, int nb, const Batch<LoopRec>& B, const int* lane
          (const double*)Lp->d_rz);
   MapLaneIO io[ALOAM_MAX_BATCH];
   Batch<GridArgs> gs = {};
+  Batch<ScoreRec> S = {};
   for (int l = 0; l < nb; ++l) {
     const LoopLane& L = Lp->lanes[lanes[l]];
     io[l] = MapLaneIO{L.reg, {L.sub[0], L.sub[1]}, L.st->counts3, L.st->pose};
     gs.a[l] = GridArgs{L.reg.corner.grid, L.sub[0], &L.st->n_sub[0], L.reg.surf.grid, L.sub[1], &L.st->n_sub[1]};
+    S.a[l] = ScoreRec{{L.reg.stack[0], L.reg.stack[1]}, L.st->n_q, L.st->pose, {L.reg.corner.grid, L.reg.surf.grid}, &L.st->score};
   }
   launch_ex(c, KID_MAP_GRID, k_grid_setup, dim3(1, 1, nb), dim3(32), 0, 1, true, gs);
   map_index_build(c, nb, io, Lp->bound);
   if (const int rc = map_register_device(c, nb, io, 2 * P, o.outer_iters)) return rc;
-  LAUNCH(c, KID_LOOP_VERIFY, k_loop_score, dim3((2 * P + kScoreWarps * 32 - 1) / (kScoreWarps * 32), 1, nb), kScoreWarps * 32, 0, B, o.inlier_sq);
+  inlier_score_device(c, KID_LOOP_VERIFY, nb, S, 2LL * P, P, o.inlier_sq);
   LAUNCH(c, KID_LOOP_VERIFY, k_loop_finish, nb, 32, 0, B, o.outer_iters - 1);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;

@@ -1,13 +1,15 @@
 // Recovery of localising lanes inside the mapped stream calls (aloam_set_recovery, aloam_recovery_rows): when a localising row's
-// prior-map inlier score (k_track_score, rows.cu) falls below trigger_frac of its scoring points, the same stream scores pose
+// prior-map inlier score (the tracking score, rows.cu) falls below trigger_frac of its scoring points, the same stream scores pose
 // candidates around the row's map pose and, when the best one is clearly better, re-seats the lane's T_wmap_wodom.  The lane's next
 // registered frame refines from there; its odometry goes on untouched.  Four launches per localising frame, whether or not a row
-// triggers, all on the mapper stream right after k_track_score and decided on the device:
+// triggers, all on the mapper stream right after the tracking score and decided on the device:
 //   * k_recover_cand: per record the trigger test on its row (rec_triggered), then, for a triggered row only, candidate h =
 //     (normalise(q_delta_h * q_P), t_P + t_delta_h) around the row's map pose P into the lane's slice -- an untriggered record's
 //     CTAs leave at once;
 //   * k_reloc_score / k_reloc_topk (reloc.cu), gated on rec_triggered: the candidates' coarse scores on the frame's filtered
-//     stacks at the rows' scoring setting, and each set's best key, ranking by (score descending, h ascending);
+//     stacks at the rows' scoring setting, and each set's best key, ranking by (score descending, h ascending).  The row's score
+//     (k_inlier_score) and the candidates' count their points through the same walk (warp_inliers, grid.cuh), so a candidate at
+//     the row's own pose ties with the row and the adoption's strict comparison never takes it;
 //   * k_recover_adopt (cubemap.cu): the accept test and transformUpdate at the best candidate with the frame's odometry pose.
 // Everything of a lane lives in the lane's slice of the buffers, so the scores of its latest triggered row stay readable.
 #include "ctx.h"
@@ -91,7 +93,7 @@ int recover_ensure(aloam_ctx* c, int n, int ctas) {
 }  // namespace
 
 // the recovery of the nb localising records of the frame just issued on the current stream (the mapper stream), after
-// k_track_score has scored their rows rows[l]: four launches whatever the rows hold
+// the tracking score has scored their rows rows[l]: four launches whatever the rows hold
 int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows) {
   const Recovery* R = c->recover;
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !R || !c->prior) return ALOAM_ERR_STATE;

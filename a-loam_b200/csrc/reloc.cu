@@ -1,13 +1,18 @@
 // Relocalisation against the prior map (aloam_prior_relocalise): score many pose hypotheses of one scan against the whole prior
-// map, keep the best K on the device, refine those with one batched localising frame.
+// map, keep the best K on the device, refine those with one batched localising frame.  Every inlier score of the library is
+// taken here, by the two kernels below, and both count a warp's moved points with warp_inliers (grid.cuh).
 //   * k_reloc_score: one warp per hypothesis, grid-stride over the hypotheses.  The scoring points (the frame's filtered stacks,
 //     subsampled) are staged per CTA in shared memory with plain loads: they are a few KB read once per CTA, so a TMA bulk copy
 //     would save nothing and needs a contiguous source, which the subsample is not.  Lane j moves point p0 + j by the warp's
-//     hypothesis (pointAssociateToMap in double, once per point instead of 32 times), then the warp probes the 32 moved points in
-//     turn through the cooperative 27-cell walk of k_map_knn5 (lanes 0-26 probe one cell each, the candidates split over the
-//     lanes 32 at a time), stopping after the first chunk in which some lane has a candidate inside inlier_sq: an inlier needs a
-//     map point, not the nearest one.  The count stays in a register; lane 0 writes it, and the warp keeps its 16 best keys
-//     (score << 32 | ~index) in lanes 0-15, merged per CTA at the end.
+//     hypothesis (pointAssociateToMap in double, once per point instead of 32 times), then warp_inliers walks the 32 moved points
+//     in turn through the cooperative 27-cell walk of k_map_knn5 (lanes 0-26 probe one cell each, the candidates split over the
+//     lanes 32 at a time), stopping after the first chunk in which some lane has a candidate inside inlier_sq.  The count stays
+//     in a register; lane 0 writes it, and the warp keeps its 16 best keys (score << 32 | ~index) in lanes 0-15, merged per CTA
+//     at the end.
+//   * k_inlier_score: one pose per record (ScoreRec), parallel over the scoring points rather than the records -- the tracking
+//     score of localising rows (rows.cu) and the score of a verified loop (loop.cu).  Grid (CTAs per record, 1, records), each
+//     warp moves 32 scoring points of its record by the record's pose, counts them with warp_inliers and adds the count to the
+//     record's score with one atomic: an integer sum, so the score does not depend on the order the warps finish in.
 //   * k_reloc_topk: one CTA merges the per-CTA lists into the 16 best keys: ranking by (score descending, index ascending).
 //   * both take one hypothesis set per record (RelocRec, blockIdx.z), with an optional device gate word: aloam_prior_relocalise is
 //     the one-record, ungated case; the recovery of localising lanes (recover.cu) scores every localising record of a stream step
@@ -22,6 +27,8 @@
 namespace {
 constexpr int kRelocWarps = 8;                 // warps (hypotheses in flight) per CTA of k_reloc_score, 4 CTAs per SM (55 registers:
                                                // without the bound ptxas aims for 5 and spills the key list)
+constexpr int kScoreWarps = 8;                 // warps per CTA of k_inlier_score: 256 scoring points per CTA (4 CTAs per SM:
+                                               // 46 registers, no spills)
 constexpr int kRelocStage = 2048;              // scoring points staged in shared memory at once (32 KB)
 constexpr int kTop = kRelocTop;                // best keys kept per CTA and returned: the largest K
 constexpr int kMaxHyp = 1 << 24;
@@ -66,7 +73,7 @@ __global__ void __launch_bounds__(kRelocWarps * 32, 4) k_reloc_score(const __gri
   __shared__ float4 s_pts[kRelocStage];
   __shared__ unsigned long long s_top[kRelocWarps * kTop], s_out[kTop];
   const int n_c = counts[0], n_s = counts[1];
-  const int m_c = min(n_c, max_pts), m_s = min(n_s, max_pts), m = m_c + m_s;
+  const int m_c = min(n_c, max_pts), m = scoring_points(n_c, n_s, max_pts), m_s = m - m_c;
   const unsigned lane = lane_id();
   const int warp = threadIdx.x >> 5;
   const unsigned mask_c = G.corner.dyn->mask, mask_s = G.surf.dyn->mask;
@@ -98,14 +105,7 @@ __global__ void __launch_bounds__(kRelocWarps * 32, 4) k_reloc_score(const __gri
           const Pt4 q = point_associate_to_map(Pt4{s.x, s.y, s.z, s.w}, x[0], x[1], x[2], x[3], x[4], x[5], x[6]);
           qx = q.x; qy = q.y; qz = q.z;
         }
-        const int np = min(32, c1 - p0);
-        for (int j = 0; j < np; ++j) {
-          const float px = __shfl_sync(0xffffffffu, qx, j), py = __shfl_sync(0xffffffffu, qy, j), pz = __shfl_sync(0xffffffffu, qz, j);
-          const bool is_corner = p0 + j < m_c;
-          const bool in = any_in_block27(is_corner ? G.corner : G.surf, is_corner ? mask_c : mask_s, px, py, pz,
-                                         [&](float a, float b, float c) { return sqdist3(a, b, c, px, py, pz) < inlier_sq; });
-          cnt += in ? 1 : 0;
-        }
+        cnt = warp_inliers(cnt, qx, qy, qz, p0, min(32, c1 - p0), m_c, G.corner, mask_c, G.surf, mask_s, inlier_sq);
       }
     }
     if (!live) continue;
@@ -130,6 +130,28 @@ __global__ void __launch_bounds__(kRelocWarps * 32, 4) k_reloc_score(const __gri
   }
   __syncthreads();
   if (threadIdx.x < kTop) best[(size_t)blockIdx.x * kTop + threadIdx.x] = s_out[threadIdx.x];
+}
+
+// scores of the records (ScoreRec): *score += the scoring points of the record's stacks (sizes counts[0], counts[1]; at most
+// max_pts of each type) that have a map point of their type at float d2 < inlier_sq once moved by the record's pose.  Warp w of
+// CTA b takes scoring points 32 (b kScoreWarps + w) .. + 31; warps past the record's scoring points return at once.
+__global__ void __launch_bounds__(kScoreWarps * 32, 4) k_inlier_score(const __grid_constant__ Batch<ScoreRec> B, int max_pts, float inlier_sq) {
+  const ScoreRec& a = B.a[blockIdx.z];
+  const int n_c = a.counts[0], n_s = a.counts[1];
+  const int m_c = min(n_c, max_pts), m = scoring_points(n_c, n_s, max_pts), m_s = m - m_c;
+  const int p0 = (blockIdx.x * kScoreWarps + (threadIdx.x >> 5)) * 32;
+  if (p0 >= m) return;   // warp-uniform
+  const unsigned lane = lane_id();
+  float qx = 0.f, qy = 0.f, qz = 0.f;
+  if (p0 + (int)lane < m) {
+    const float4 s = scoring_point(a.stack[0], a.stack[1], n_c, m_c, n_s, m_s, p0 + (int)lane);
+    const double* x = a.pose;
+    const Pt4 q = point_associate_to_map(Pt4{s.x, s.y, s.z, s.w}, x[0], x[1], x[2], x[3], x[4], x[5], x[6]);
+    qx = q.x; qy = q.y; qz = q.z;
+  }
+  const unsigned mask_c = a.grid[0].dyn->mask, mask_s = a.grid[1].dyn->mask;
+  const int cnt = warp_inliers(0, qx, qy, qz, p0, min(32, m - p0), m_c, a.grid[0], mask_c, a.grid[1], mask_s, inlier_sq);
+  if (lane == 0 && cnt) atomicAdd(a.score, cnt);
 }
 
 __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
@@ -172,6 +194,11 @@ void reloc_score_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ct
 
 void reloc_topk_device(aloam_ctx* c, int nrec, const Batch<RelocRec>& B, int ctas, int rounds) {
   LAUNCH(c, KID_RELOC_TOPK, k_reloc_topk, dim3(1, 1, nrec), 1024, 0, B, ctas * kTop, rounds);
+}
+
+void inlier_score_device(aloam_ctx* c, int kid, int nb, const Batch<ScoreRec>& B, long long m_upper, int max_pts, float inlier_sq) {
+  const int ctas = (int)std::max(1LL, (m_upper + kScoreWarps * 32 - 1) / (kScoreWarps * 32));
+  LAUNCH(c, kid, k_inlier_score, dim3(ctas, 1, nb), kScoreWarps * 32, 0, B, max_pts, inlier_sq);
 }
 
 // one resident wave of k_reloc_score, at most one warp per hypothesis

@@ -2,65 +2,25 @@
 // for a localising row how well its scan still fits the prior map at the row's map pose.
 //   * k_map_rows (cubemap.cu): one launch per frame, right after it on the mapper stream -- each record copies its frame's flags,
 //     error word, window and stack sizes and the heads of its solve summaries into the row's slot of the device row table.
-//   * k_track_score: the prior-map inlier score of aloam_prior_relocalise at the row's map pose, one launch per localising frame.
-//     Parallel over the scoring points, not over records: grid (CTAs per record, 1, records), each warp takes 32 scoring points of
-//     its record, lane j moves point j by the row's map pose (pointAssociateToMap in double), the warp walks the 32 moved points
-//     through the cooperative 27-cell walk k_reloc_score uses (any_in_block27, grid.cuh) and adds its count to the row's score
-//     with one atomic: an integer sum, so the score does not depend on the order the warps finish in.
+//   * the tracking score: the prior-map inlier score of aloam_prior_relocalise at the row's map pose, one launch of
+//     k_inlier_score (reloc.cu) per localising frame, which counts the row's scoring points as k_reloc_score counts a hypothesis'.
 //   * the host turns the rows into aloam_map_row after the call's final synchronise; skipped and idle rows cost no device work.
 #include "ctx.h"
-#include "grid.cuh"
 
-namespace {
-constexpr int kTrackWarps = 8;   // warps per CTA of k_track_score: 256 scoring points per CTA (at least 4 CTAs per SM: 46 registers, no spills)
-
-// scores of the records' rows: row->score += the scoring points of the record's stacks (sizes counts[0], counts[1]; at most max_pts
-// of each type, picked as k_reloc_score picks them) that have a prior-map point of their type at float d2 < inlier_sq once moved by
-// the record's map pose.  Warps past the record's scoring points return at once.
-__global__ void __launch_bounds__(kTrackWarps * 32, 4) k_track_score(const __grid_constant__ Batch<TrackArgs> B, int max_pts, float inlier_sq,
-                                                                  const __grid_constant__ PriorGrid G) {
-  const TrackArgs& a = B.a[blockIdx.z];
-  const int n_c = a.counts[0], n_s = a.counts[1];
-  const int m_c = min(n_c, max_pts), m_s = min(n_s, max_pts), m = m_c + m_s;
-  const int p0 = (blockIdx.x * kTrackWarps + (threadIdx.x >> 5)) * 32;
-  if (p0 >= m) return;   // warp-uniform
-  const unsigned lane = lane_id();
-  float qx = 0.f, qy = 0.f, qz = 0.f;
-  if (p0 + (int)lane < m) {
-    const float4 s = scoring_point(a.stack[0], a.stack[1], n_c, m_c, n_s, m_s, p0 + (int)lane);
-    const double* x = a.pose;
-    const Pt4 q = point_associate_to_map(Pt4{s.x, s.y, s.z, s.w}, x[0], x[1], x[2], x[3], x[4], x[5], x[6]);
-    qx = q.x; qy = q.y; qz = q.z;
-  }
-  const unsigned mask_c = G.corner.dyn->mask, mask_s = G.surf.dyn->mask;
-  const int np = min(32, m - p0);
-  int cnt = 0;
-  for (int j = 0; j < np; ++j) {
-    const float px = __shfl_sync(0xffffffffu, qx, j), py = __shfl_sync(0xffffffffu, qy, j), pz = __shfl_sync(0xffffffffu, qz, j);
-    const bool is_corner = p0 + j < m_c;
-    const bool in = any_in_block27(is_corner ? G.corner : G.surf, is_corner ? mask_c : mask_s, px, py, pz,
-                                   [&](float u, float v, float w) { return sqdist3(u, v, w, px, py, pz) < inlier_sq; });
-    cnt += in ? 1 : 0;
-  }
-  if (lane == 0 && cnt) atomicAdd(&a.row->score, cnt);
-}
-
-}  // namespace
-
-// k_track_score over the nb localising records of the frame just issued on the current stream, after k_map_rows has set their
-// rows' counts to 0: record l scores rows[l] at its map pose in[l].out7 with its locator's filtered stacks.  The grid is sized
-// from the host's bound on the scoring points, min(max_score, n_upper) per type.
+// the tracking score over the nb localising records of the frame just issued on the current stream, after k_map_rows has set
+// their rows' counts to 0: record l scores rows[l] at its map pose in[l].out7 with its locator's filtered stacks against the prior
+// map.  The grid is sized from the host's bound on the scoring points, min(max_score, n_upper) per type.
 int track_score_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* rows, int n_upper_c, int n_upper_s) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !c->prior) return ALOAM_ERR_STATE;
-  Batch<TrackArgs> B = {};
+  const PriorGrid G = prior_grid(c);
+  Batch<ScoreRec> B = {};
   for (int l = 0; l < nb; ++l) {
     const LocatorFrame F = locator_frame(c->lanes[in[l].lane].locator);
-    B.a[l] = TrackArgs{{F.stack[0], F.stack[1]}, F.counts, in[l].out7, rows[l]};
+    B.a[l] = ScoreRec{{F.stack[0], F.stack[1]}, F.counts, in[l].out7, {G.corner, G.surf}, &rows[l]->score};
   }
   const int max_pts = c->rows_max_score;
   const long long m_upper = (long long)std::min(max_pts, std::max(n_upper_c, 0)) + std::min(max_pts, std::max(n_upper_s, 0));
-  const int ctas = (int)std::max(1LL, (m_upper + kTrackWarps * 32 - 1) / (kTrackWarps * 32));
-  LAUNCH(c, KID_TRACK_SCORE, k_track_score, dim3(ctas, 1, nb), kTrackWarps * 32, 0, B, max_pts, c->rows_inlier_sq, prior_grid(c));
+  inlier_score_device(c, KID_TRACK_SCORE, nb, B, m_upper, max_pts, c->rows_inlier_sq);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }

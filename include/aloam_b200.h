@@ -727,7 +727,7 @@ int aloam_registered_rows(aloam_ctx* ctx, long long* begin, int* count, int rows
  * outside {0, 1}, max_score_points < 0, or max_score_points > 0 with inlier_sq outside (0, 1] (the 27 cells of the 1.00001 m
  * grid hold every point that close, as for aloam_prior_relocalise); max_score_points = 0 records rows without scoring.
  * ALOAM_ERR_STATE on a rank of a sharded job and on an emulating context; aloam_comm_init and aloam_debug_shard_emulate with
- * world > 0 turn recording off.  Cost with recording on: one launch (k_map_rows) per frame, one more (k_track_score) per
+ * world > 0 turn recording off.  Cost with recording on: one launch (k_map_rows) per frame, one more (k_inlier_score) per
  * localising frame when scoring, one device-to-host copy of the call's rows.
  * aloam_map_rows copies the `rows` = n_scans x batch rows of the last mapped stream call, scan-major like map_poses (it mirrors
  * aloam_registered_rows).  ALOAM_ERR_INVALID_ARG when out is NULL or `rows` is not that call's row count; ALOAM_ERR_STATE before
@@ -929,7 +929,7 @@ int aloam_place_query(aloam_ctx* ctx, const float* descs, int n_query, int k, al
  *   loop >= 0 and distance <= max_distance (double compare) is verified at its own step on the mapper stream with (its lane, its
  *   keyframe, its loop, its shift), without a host synchronisation.  Launches per mapping frame: 1 (k_loop_keep); when some record
  *   can have a candidate (the bound place recognition uses to size its query), 8 + 3 outer_iters more (k_loop_gather, k_grid_setup,
- *   the 4 index-build launches, outer_iters x (k_map_knn5, k_map_fit, k_lm_solve), k_loop_score, k_loop_finish); one device-to-host
+ *   the 4 index-build launches, outer_iters x (k_map_knn5, k_map_fit, k_lm_solve), k_inlier_score, k_loop_finish); one device-to-host
  *   copy of the loop rows per call.  With loops off the stream calls issue exactly what they issue without this feature.
  * aloam_loop_rows mirrors aloam_place_rows: the same row count, scan-major order, state rules, and readability after
  * ALOAM_ERR_CAPACITY / ALOAM_ERR_COMM (ALOAM_ERR_STATE when the last mapped call ran with loops off).  Fields are -1 / 0 where a row

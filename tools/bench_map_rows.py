@@ -5,7 +5,7 @@ prior map of a mapping lane that ran the same scans.  One process, one context p
 alternate --repeats times:
   off      recording off;
   rows     rows only (k_map_rows after every frame);
-  s256     rows and scores at 256 scoring points per type (k_track_score after every localising frame);
+  s256     rows and scores at 256 scoring points per type (k_inlier_score after every localising frame);
   s1024    rows and scores at 1 024 points per type.
 inlier_sq = 0.25.  Per (B, k) and arm one JSON line: median and range of ms per step (host clock around the synchronous call) and
 launches per step.  The GPU's name and power limit are read in the same run.  Needs a GPU: without one it fails.
