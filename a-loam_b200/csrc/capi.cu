@@ -614,7 +614,7 @@ static int map_stage(aloam_ctx* c, const StreamSwitches& w, const StreamRow* row
     if (n == 0) continue;
     MapRowRec* rows[ALOAM_MAX_BATCH] = {};                    // the row slots of the frame's records
     const Pt4* src[ALOAM_MAX_BATCH] = {}; const int* nf[ALOAM_MAX_BATCH] = {}; Pt4* dst[ALOAM_MAX_BATCH] = {};   // their registered clouds
-    Locator* lp[ALOAM_MAX_BATCH] = {}; const double* init[ALOAM_MAX_BATCH] = {};                                    // their locators
+    LaneFrame* lp[ALOAM_MAX_BATCH] = {}; const double* init[ALOAM_MAX_BATCH] = {};                                    // their locators
     for (int j = 0; j < n; ++j) {
       Lane& L = c->lanes[in[j].lane];
       if (w.rec) rows[j] = c->d_rows + r0 + in[j].lane;
@@ -651,10 +651,9 @@ static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const Stream
   const cudaStream_t s_main = c->stream;
   const auto host_t0 = std::chrono::steady_clock::now();
   if (w.map) {
-    for (int l = 0; l < nb; ++l) {   // the mappers' error bits of this call (a lane that only localises has no cube store)
-      if (c->lanes[l].mapper) STREAM_TRY(cudaMemsetAsync(mapper_err_acc(c, l), 0, sizeof(int), s_main));
-      if (c->lanes[l].locator) STREAM_TRY(cudaMemsetAsync(locator_err_acc(c, l), 0, sizeof(int), s_main));
-    }
+    for (int l = 0; l < nb; ++l)   // every frame's error bits of this call (a lane that only localises has no cube store)
+      for (int loc = 0; loc < 2; ++loc)
+        if (const LaneFrame* f = lane_frame(c, l, loc)) STREAM_TRY(cudaMemsetAsync(frame_view(f).err_acc, 0, sizeof(int), s_main));
     const int rc = peer_err_reset(c); if (rc) return rc;
   }
   STREAM_TRY(cudaEventRecord(c->ev0, s_main));
@@ -769,9 +768,10 @@ static int stream_issue(aloam_ctx* c, const aloam_cloud_view* raws, const Stream
     if (w.place) STREAM_TRY(cudaMemcpyAsync(place_rows_host(c), place_rows_device(c), total * sizeof(aloam_place_row), cudaMemcpyDeviceToHost, s_main));
     if (w.loop) STREAM_TRY(cudaMemcpyAsync(loop_rows_host(c), loop_rows_device(c), total * loop_row_bytes(), cudaMemcpyDeviceToHost, s_main));
     for (int l = 0; l < nb; ++l) {
-      c->pin->mapper_err_lane[l] = c->pin->locate_err_lane[l] = 0;
-      if (c->lanes[l].mapper) STREAM_TRY(cudaMemcpyAsync(&c->pin->mapper_err_lane[l], mapper_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
-      if (c->lanes[l].locator) STREAM_TRY(cudaMemcpyAsync(&c->pin->locate_err_lane[l], locator_err_acc(c, l), sizeof(int), cudaMemcpyDeviceToHost, s_main));
+      int* dst[2] = {&c->pin->mapper_err_lane[l], &c->pin->locate_err_lane[l]};
+      *dst[0] = *dst[1] = 0;
+      for (int loc = 0; loc < 2; ++loc)
+        if (const LaneFrame* f = lane_frame(c, l, loc)) STREAM_TRY(cudaMemcpyAsync(dst[loc], frame_view(f).err_acc, sizeof(int), cudaMemcpyDeviceToHost, s_main));
     }
     const int rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;
   }

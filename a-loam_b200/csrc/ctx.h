@@ -120,8 +120,8 @@ class BufGroup {
   std::vector<void*> dev_, pinned_;
 };
 struct ExportLayout;   // cubemap.cu: where the segments of a store export are in the export and in the store
-struct Mapper;         // cubemap.cu: a lane's cube store
-struct Locator;        // cubemap.cu: the frame state and registration buffers of a lane that localises
+struct LaneFrame;      // cubemap.cu: what a scan-to-map frame runs on -- frame state, registration set, stack filter
+struct Mapper;         // cubemap.cu: a lane's cube store, one frame and the store's buffers
 struct PriorMap;       // cubemap.cu: the context's prior map, frozen and indexed
 struct Relocaliser;    // reloc.cu: the scratch of aloam_prior_relocalise
 struct Recovery;       // recover.cu: the setting and buffers of aloam_set_recovery
@@ -194,10 +194,10 @@ struct LaneSched {
 // aloam_scan_stream_batch drives lanes 0 .. batch-1 in lockstep with shared launches.
 struct Lane {
   LaneSched sched;
-  // its cube store and its locator (cubemap.cu), each created on first use: lane 0's store serves the host API and both mapped
-  // stream calls; a lane that only localises has no store
+  // its cube store and its locator, the frame its localising trajectories run on (cubemap.cu), each created on first use: lane
+  // 0's store serves the host API and both mapped stream calls; a lane that only localises has no store
   Mapper* mapper = nullptr;
-  Locator* locator = nullptr;
+  LaneFrame* locator = nullptr;
   double init[7] = {};   // the T_wmap_wodom an armed START starts from (aloam_lane_localise, aloam_lane_map_on_prior)
   // the locator holds the window of a localising frame against the current prior map (aloam_debug_prior_associate); set by the
   // frame, cleared when the prior map is released
@@ -293,10 +293,9 @@ struct aloam_ctx {
   int* d_stack_counts = nullptr;  // [4] {n_corner, n_surf, total} of the host API's stacks
   double* d_map_pose = nullptr;   // [7] host API: scan-to-map pose being refined (parameters[7], laserMapping.cpp:110)
   double* d_fits = nullptr;       // [queries][14] debug / test records of the line / plane fits
-  // aloam_voxel_filter (voxel.cu): a segmented filter of its own (cap = max_points), created on first use
+  // aloam_voxel_filter (voxel.cu): a segmented filter of its own (cap = max_points), created on first use, published complete
   SegBuffers vox_seg;
   int* d_seg_io = nullptr;        // [3] the segment's size, its filtered size, the filter's error word
-  bool vox_seg_ready = false;     // every buffer of this group is allocated
   // pipelined scan stream: ring binning on s_exa, per-ring features on s_ext, compaction + index on s_idx, association + LM
   // on `stream`, host->device copies of the raw scans on s_h2d, scan-to-map on s_map; all chained by events
   cudaStream_t s_ext = nullptr, s_exa = nullptr, s_idx = nullptr, s_h2d = nullptr, s_map = nullptr;
@@ -444,7 +443,7 @@ int launch_lm_batch(aloam_ctx* c, bool pdl, const aloam::Batch<aloam::LmArgs>& a
 int peer_err_reset(aloam_ctx* c);
 int peer_err_fetch(aloam_ctx* c, int* dst);
 void vox_seg_filter(aloam_ctx* c, int nb, const aloam::SegFilter* f, aloam::SegBuffers* const* b, int S_upper, int n_upper, int per_seg_upper);
-int vox_seg_alloc(aloam_ctx* c, aloam::SegBuffers& b, size_t cap);
+int vox_seg_alloc(aloam_ctx* c, BufGroup& g, aloam::SegBuffers& b, size_t cap);
 // voxel.cu: the segmented filter's stable radix sort over one key array of up to n_upper keys (the prior-map build), and the ints
 // of histogram it needs for n keys
 int vox_radix_sort(aloam_ctx* c, int kid, unsigned* k0, int* v0, unsigned* k1, int* v1, const int* n_dev, int n_upper, int bits, int* hist);
@@ -491,9 +490,6 @@ int loop_record_device(aloam_ctx* c, int nb, const MapperIn* in, const aloam_pla
 void* loop_rows_device(aloam_ctx* c);
 void* loop_rows_host(aloam_ctx* c);
 size_t loop_row_bytes();
-// the stacks a lane's latest mapping frame registered (sensor frame) and their sizes (counts[0], counts[1]), from its cube store
-struct MapperStacks { const Pt4* stack[2]; const int* counts; };
-MapperStacks mapper_stacks(const aloam_ctx* c, int lane);
 // which lanes' candidate scores belong to a triggered row of the last mapped stream call (recover.cu; none while its records
 // cannot be read or it ran no recovery)
 void recover_call_done(aloam_ctx* c);
@@ -501,21 +497,22 @@ void recover_call_done(aloam_ctx* c);
 int mapper_ensure(aloam_ctx* c, int lane);
 // the layouts of seeded STARTs (aloam_ctx::d_seed_layout), created on first use
 int mapper_seed_ensure(aloam_ctx* c);
-int* mapper_err_acc(aloam_ctx* c, int lane);
+// the frame lane `lane` runs on in mode `localise`: its locator, else its cube store's frame; null when the lane has none
+LaneFrame* lane_frame(const aloam_ctx* c, int lane, bool localise);
+// what frame f's latest run left on the device: its filtered corner / surf stacks (sensor frame), their sizes (counts[0],
+// counts[1]), its flags followed by its error word (2 ints) and its solve summaries; and the OR of its error words over one
+// mapped stream call
+struct FrameView { const Pt4* stack[2]; const int* counts; const int* flags; const LmSummary* summary; int* err_acc; };
+FrameView frame_view(const LaneFrame* f);
 // localisation against the prior map (cubemap.cu): a new locator; a lane's locator, created on first use; one frame of nb
 // localising records on the current stream, record l on locator loc[l] (in[l].fresh: it starts a trajectory with this frame,
-// from T_wmap_wodom init[l]); a lane's per-call error word
-int locator_create(aloam_ctx* c, Locator** out);
+// from T_wmap_wodom init[l])
+int locator_create(aloam_ctx* c, LaneFrame** out);
 int locator_ensure(aloam_ctx* c, int lane);
-int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const* loc, const double* const* init, int n_upper_c, int n_upper_s);
-int* locator_err_acc(aloam_ctx* c, int lane);
-// what a locator's latest frame left on the device: its filtered corner / surf stacks, their sizes (counts[0], counts[1]) and
-// its flags followed by its error word (2 ints)
-struct LocatorFrame { const Pt4* stack[2]; const int* counts; const int* flags; };
-LocatorFrame locator_frame(const Locator* m);
-// the stack filters of a localising frame alone, for locator m on the clouds of `in`, joined to the current stream: the
-// filtered stacks and their sizes as locator_frame reports them (a stack filter's error bit joins the locator's next frame)
-int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_upper_c, int n_upper_s);
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, LaneFrame* const* loc, const double* const* init, int n_upper_c, int n_upper_s);
+// the stack filters of a localising frame alone, for locator f on the clouds of `in`, joined to the current stream: the
+// filtered stacks and their sizes as frame_view reports them (a stack filter's error bit joins the locator's next frame)
+int locator_stacks_device(aloam_ctx* c, LaneFrame* f, const MapperIn& in, int n_upper_c, int n_upper_s);
 // the hash grids of the context's prior map (it exists)
 PriorGrid prior_grid(const aloam_ctx* c);
 // the checks and normalisation of an initial T_wmap_wodom (aloam_lane_localise, aloam_prior_relocalise): false for a non-finite

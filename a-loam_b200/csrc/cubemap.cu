@@ -88,22 +88,37 @@ struct MapperState {
 
 }  // namespace
 
+// What a scan-to-map frame runs on, mapping or localising: the frame state on the device and its pinned mirror (debug / host API
+// read-back), the registration set and the segmented filter of the stack filters.  Every kernel of a frame takes the state the same
+// way for both modes; a localising frame leaves the slab tables unused and keeps its window tables in sub_off.  The frame owns its
+// buffers in `mem`, except lane 0 of the mapper, which registers with the context's set c->map, shared with the host API.
+struct aloam::LaneFrame {
+  BufGroup mem;
+  MapperState* d_state = nullptr;
+  MapperState* h_state = nullptr;
+  MapReg* reg = nullptr;   // &set, or the context's set
+  MapReg set = {};
+  SegBuffers buf;
+};
+
+// A lane's cube store: its frame (whose filter also runs the per-cube re-filter) and the store's buffers, in `mem`
 struct aloam::Mapper {
+  LaneFrame frame;
+  BufGroup mem;
   int cap[2] = {0, 0};
   Pt4* d_pts[2] = {nullptr, nullptr};       // [kPool * cap] slabs
   Pt4* d_sub[2] = {nullptr, nullptr};       // gathered submap
   Pt4* d_in[2] = {nullptr, nullptr};        // host API: uploaded less-sharp / less-flat clouds
   Pt4* d_world = nullptr;                   // insertion scratch: transformed stack points
   int* d_cube = nullptr;                    //                    their cube index (-1 = outside the ring buffer)
-  MapperState* d_state = nullptr;
-  MapperState* h_state = nullptr;           // pinned mirror (debug / host API read-back)
-  SegBuffers buf;                           // the segmented filter of the stack filters and the per-cube re-filter
   double* d_pose_io = nullptr;              // [14] host API: odometry pose in, refined pose out
-  Pt4* d_dbg_pts = nullptr;                 // aloam_debug_seg_voxel_filter: segments back to back [buf.cap] ...
-  int* d_dbg_counts = nullptr;              //                                their sizes [ALOAM_MAX_SEGS]
-  int* d_dbg_err = nullptr;                 //                                private error word
+  // aloam_debug_seg_voxel_filter, created on first use: segments back to back [frame.buf.cap], their sizes [ALOAM_MAX_SEGS] and a
+  // private error word, one group
+  BufGroup dbg;
+  Pt4* d_dbg_pts = nullptr;
+  int* d_dbg_counts = nullptr;
+  int* d_dbg_err = nullptr;
   int max_sub = 0;
-  MapReg* reg = nullptr;                    // registration set: lane 0 shares the context's with the host API, the others own one
 };
 
 // The prior map: the store of a mapped lane snapshot, frozen.  Per cloud type the points packed in cube order (cube_start = the
@@ -126,15 +141,6 @@ struct aloam::PriorMap {
   bool have_digest = false;
   unsigned long long digest = 0;
   unsigned long long* d_digest = nullptr;
-};
-// what a localising lane owns: the state its frames write (a MapperState whose slab tables stay unused: k_mapper_prep,
-// k_mapper_update, k_mapper_finish, k_mapper_high_freq, k_register_full and the debug read-back work on it unchanged; sub_off
-// holds the window tables), a registration set without grid tables, and a segmented filter sized for the two scan stacks
-struct aloam::Locator {
-  MapperState* d_state = nullptr;
-  MapperState* h_state = nullptr;
-  MapReg reg = {};
-  SegBuffers buf;
 };
 
 namespace {
@@ -1000,8 +1006,8 @@ size_t refilter_bound(const Mapper* m, const aloam_ctx* c) {
 int reset_lane(aloam_ctx* c, Mapper* m) {
   int ord[2];
   mapper_run_orders(c, c->cube_growth, ord);
-  CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
-  LAUNCH(c, KID_CUBES, k_mapper_reset, 1, 1024, 0, m->d_state, ord[0], ord[1]);
+  CUDA_CHECK_RET(cudaMemsetAsync(m->frame.d_state, 0, sizeof(MapperState), c->stream));
+  LAUNCH(c, KID_CUBES, k_mapper_reset, 1, 1024, 0, m->frame.d_state, ord[0], ord[1]);
   CUDA_CHECK_RET(cudaGetLastError());
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   return ALOAM_OK;
@@ -1036,7 +1042,7 @@ int stack_filters_fork(aloam_ctx* c, int nb, const Batch<MapperLane>& B, const S
 // Synchronises.
 int export_sizes(aloam_ctx* c, const Mapper* m, int what, long long* n) {
   if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
-  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->d_state, what, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->d_export_layout);
+  LAUNCH(c, KID_CUBES, k_export_sizes, 1, 1024, 0, m->frame.d_state, what, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], c->d_export_layout);
   CUDA_CHECK_RET(cudaMemcpyAsync(&c->pin->export_total, &c->d_export_layout->total, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1075,10 +1081,18 @@ void prior_map_release(aloam_ctx* c) {
   for (Lane& L : c->lanes) L.window = false;   // the windows were cut from this map
 }
 
-// the frame state of the lane a record runs on: its locator's when it localises, else its cube store's
-MapperState* lane_state(const aloam_ctx* c, const MapperIn& in) {
-  const Lane& L = c->lanes[in.lane];
-  return in.localise ? L.locator->d_state : L.mapper->d_state;
+// The record of frame f for `in` with the fields every frame fills -- state, poses, input clouds and sizes, stacks, segment
+// descriptors -- and the stack filter of f into *stack_f / *buf; a mapping frame adds its store's fields
+MapperLane frame_record(LaneFrame* f, const MapperIn& in, SegFilter* stack_f, SegBuffers** buf) {
+  MapperState* S = f->d_state;
+  *stack_f = seg_filter(f->buf, 31, &S->err);
+  *buf = &f->buf;
+  MapperLane a = {};
+  a.S = S; a.odom7 = in.odom7; a.out7 = in.out7;
+  a.in[0] = in.corner; a.in[1] = in.surf; a.n_in[0] = in.nc; a.n_in[1] = in.ns;
+  a.stack[0] = f->reg->stack[0]; a.stack[1] = f->reg->stack[1];
+  a.segs = f->buf.segs; a.n_seg = f->buf.n_seg;
+  return a;
 }
 
 // the persistent index: the k_grid_* chain of mapping.cu once over both packed clouds, then the cube tags
@@ -1396,9 +1410,9 @@ void mapper_run_orders(const aloam_ctx* c, bool growth, int ord[2]) {
 // exists.  Synchronises.
 int mapper_store_tables(aloam_ctx* c, int lane, SnapStore* head, int* growth) {
   Mapper* m = c->lanes[lane].mapper;
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->frame.h_state, m->frame.d_state, sizeof(MapperState), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
-  const MapperState* S = m->h_state;
+  const MapperState* S = m->frame.h_state;
   std::memset(head, 0, sizeof(*head));
   for (int a = 0; a < 3; ++a) head->cen[a] = S->cen[a];
   head->n_valid = S->n_valid;
@@ -1438,8 +1452,8 @@ int mapper_store_restore(aloam_ctx* c, int lane, const SnapStore* head, const ch
   if (!c->d_export_layout) CUDA_CHECK_RET(dalloc(c, &c->d_export_layout, 1));
   if (!c->d_snap_store) CUDA_CHECK_RET(dalloc(c, &c->d_snap_store, 1));
   CUDA_CHECK_RET(cudaMemcpyAsync(c->d_snap_store, head, sizeof(SnapStore), cudaMemcpyHostToDevice, c->stream));
-  CUDA_CHECK_RET(cudaMemsetAsync(m->d_state, 0, sizeof(MapperState), c->stream));
-  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->d_state, c->d_snap_store, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], ord[0], ord[1],
+  CUDA_CHECK_RET(cudaMemsetAsync(m->frame.d_state, 0, sizeof(MapperState), c->stream));
+  LAUNCH(c, KID_CUBES, k_store_import_tables, 1, 1024, 0, m->frame.d_state, c->d_snap_store, m->d_pts[0], m->d_pts[1], m->cap[0], m->cap[1], ord[0], ord[1],
          c->d_export_layout);
   if (head->n_points > 0) { const int rc = store_copy(c, c->d_export_layout, head->n_points, const_cast<char*>(pts), device, true); if (rc) return rc; }
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
@@ -1457,7 +1471,7 @@ static int seed_stores(aloam_ctx* c, int nb, const MapperIn* in) {
     if (!in[l].seed) continue;
     const Lane& L = c->lanes[in[l].lane];
     const Mapper* m = L.mapper;
-    B.a[n] = SeedLane{m->d_state, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, c->d_seed_layout + n, {}};
+    B.a[n] = SeedLane{m->frame.d_state, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, c->d_seed_layout + n, {}};
     for (int k = 0; k < 7; ++k) B.a[n].init[k] = L.init[k];
     ++n;
   }
@@ -1496,19 +1510,19 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     while (cube_bits < 31 && (double)(1ull << cube_bits) < cells) ++cube_bits; }
   for (int l = 0; l < nb; ++l) {   // record l runs on the store of lane in[l].lane
     Mapper* m = c->lanes[in[l].lane].mapper;
-    MapperState* S = m->d_state;
-    const MapReg& reg = *m->reg;
-    B.a[l] = MapperLane{S, in[l].odom7, in[l].out7, {m->d_pts[0], m->d_pts[1]}, {m->cap[0], m->cap[1]}, {m->d_sub[0], m->d_sub[1]}, {in[l].corner, in[l].surf},
-                        {in[l].nc, in[l].ns}, {reg.stack[0], reg.stack[1]}, m->d_world, m->d_cube, m->buf.segs, m->buf.n_seg};
+    MapperState* S = m->frame.d_state;
+    const MapReg& reg = *m->frame.reg;
+    MapperLane& a = B.a[l];
+    a = frame_record(&m->frame, in[l], &stack_f[l], &bufs[l]);
+    for (int t = 0; t < 2; ++t) { a.pts[t] = m->d_pts[t]; a.cap[t] = m->cap[t]; a.sub[t] = m->d_sub[t]; }
+    a.world = m->d_world; a.cube = m->d_cube;
     if (in[l].fresh) fresh |= 1u << l;
     io[l] = MapLaneIO{reg, {m->d_sub[0], m->d_sub[1]}, S->stack_counts, S->x};
     gs.a[l] = GridArgs{reg.corner.grid, m->d_sub[0], &S->n_sub[0], reg.surf.grid, m->d_sub[1], &S->n_sub[1]};
-    stack_f[l] = seg_filter(m->buf, 31, &S->err);
-    cube_f[l] = seg_filter(m->buf, cube_bits, &S->err);
-    bufs[l] = &m->buf;
+    cube_f[l] = seg_filter(m->frame.buf, cube_bits, &S->err);
   }
   const int max_sub = m0->max_sub, cap1 = m0->cap[1];
-  const int refilter_cap = (int)m0->buf.cap;   // refilter_bound: the same for every lane
+  const int refilter_cap = (int)m0->frame.buf.cap;   // refilter_bound: the same for every lane
   int ord[2];                                  // the runs of the lanes that start a trajectory with this frame
   mapper_run_orders(c, c->cube_growth, ord);
   // ---- seeded STARTs: their stores become copies of the prior map, in order on this stream after the lanes' previous frames and
@@ -1522,7 +1536,7 @@ int mapper_step_device(aloam_ctx* c, int nb, const MapperIn* in, int n_upper_c, 
     // A rank of a sharded job keeps the WHOLE cube store (the insertions below are replicated: the refined pose is bit-identical
     // on every rank) but indexes and searches only its x-slabs (+ halo) of the submap; the ranks meet in the all-reduce of the
     // normal equations inside the solve.  The too-thin test of k_mapper_prep is on the whole submap, the same on every rank.
-    MapperState* S = m0->d_state;
+    MapperState* S = m0->frame.d_state;
     rc = map_shard_index_device(c, m0->d_sub, S->n_sub, max_sub, &S->err); if (rc) return rc;
   } else {
     launch_ex(c, KID_MAP_GRID, k_grid_setup, dim3(1, 1, nb), dim3(32), 0, 1, true, gs);
@@ -1554,7 +1568,7 @@ int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<MapperLane> B = {};
   for (int l = 0; l < nb; ++l) {
-    B.a[l].S = lane_state(c, in[l]);
+    B.a[l].S = lane_frame(c, in[l].lane, in[l].localise)->d_state;
     B.a[l].odom7 = in[l].odom7;
     B.a[l].out7 = in[l].out7;
   }
@@ -1569,7 +1583,7 @@ int mapper_high_freq_device(aloam_ctx* c, int nb, const MapperIn* in) {
 int mapper_register_full_device(aloam_ctx* c, int nb, const MapperIn* in, const Pt4* const* src, const int* const* n_full, Pt4* const* dst, int n_upper) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<RegFullLane> B = {};
-  for (int l = 0; l < nb; ++l) B.a[l] = RegFullLane{lane_state(c, in[l]), src[l], n_full[l], dst[l]};
+  for (int l = 0; l < nb; ++l) B.a[l] = RegFullLane{lane_frame(c, in[l].lane, in[l].localise)->d_state, src[l], n_full[l], dst[l]};
   const int blocks = std::max(1, std::min((n_upper + 255) / 256, std::max(1, c->sms * 2 / nb)));
   launch_ex(c, KID_CUBES, k_register_full, dim3(blocks, 1, nb), dim3(256), 0, 1, false, B);
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1614,8 +1628,8 @@ int map_rows_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* 
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<MapRowLane> B = {};
   for (int l = 0; l < nb; ++l) {
-    const Lane& L = c->lanes[in[l].lane];
-    B.a[l] = MapRowLane{lane_state(c, in[l]), in[l].localise ? L.locator->reg.summary : L.mapper->reg->summary, rows[l], in[l].localise ? max_score : 0};
+    const LaneFrame* f = lane_frame(c, in[l].lane, in[l].localise);
+    B.a[l] = MapRowLane{f->d_state, f->reg->summary, rows[l], in[l].localise ? max_score : 0};
   }
   LAUNCH(c, KID_MAP_ROWS, k_map_rows, dim3(1, 1, nb), 32, 0, B, std::min(c->cfg.outer_iters, 4));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -1660,75 +1674,69 @@ int recover_adopt_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* co
                          const unsigned long long* const* best, float accept_frac) {
   if (nb < 1 || nb > ALOAM_MAX_BATCH) return ALOAM_ERR_STATE;
   Batch<RecoverAdopt> B = {};
-  for (int l = 0; l < nb; ++l) B.a[l] = RecoverAdopt{lane_state(c, in[l]), rows[l], cand[l], best[l]};
+  for (int l = 0; l < nb; ++l) B.a[l] = RecoverAdopt{lane_frame(c, in[l].lane, in[l].localise)->d_state, rows[l], cand[l], best[l]};
   LAUNCH(c, KID_RECOVER_ADOPT, k_recover_adopt, 1, 32, 0, B, nb, accept_frac);
   CUDA_CHECK_RET(cudaGetLastError());
   return ALOAM_OK;
 }
-
-// the per-call error accumulation of a mapped stream call (device word; the lane's mapper must exist)
-int* mapper_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].mapper->d_state->err_acc; }
 
 int mapper_seed_ensure(aloam_ctx* c) {
   if (!c->d_seed_layout) CUDA_CHECK_RET(dalloc(c, &c->d_seed_layout, (size_t)c->n_lanes));
   return ALOAM_OK;
 }
 
-int mapper_ensure(aloam_ctx* c, int lane) {
-  if (c->lanes[lane].mapper) return ALOAM_OK;
-  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
-  Mapper* m = new (std::nothrow) Mapper();
-  if (!m) return ALOAM_ERR_CUDA;
-  own(c, [m] { delete m; });
-  mapper_slab_caps(c, m->cap);
-  m->max_sub = c->cfg.max_map_points;
-  bool ok = true;
-  for (int t = 0; t < 2 && ok; ++t) {
-    ok = ok && dalloc(c, &m->d_pts[t], (size_t)kPool * m->cap[t]) == cudaSuccess;
-    ok = ok && dalloc(c, &m->d_sub[t], (size_t)m->max_sub) == cudaSuccess;
-    ok = ok && dalloc(c, &m->d_in[t], (size_t)c->max_points) == cudaSuccess;
-  }
-  ok = ok && dalloc(c, &m->d_world, (size_t)2 * c->max_points) == cudaSuccess;   // both stacks side by side
-  ok = ok && dalloc(c, &m->d_cube, (size_t)2 * c->max_points) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_state, 1) == cudaSuccess;
-  ok = ok && halloc(c, &m->h_state, 1) == cudaSuccess;
-  ok = ok && dalloc(c, &m->d_pose_io, 16) == cudaSuccess;
-  ok = ok && stack_stream_ensure(c) == cudaSuccess;
-  ok = ok && cudaFuncSetAttribute(k_cube_insert, cudaFuncAttributeMaxDynamicSharedMemorySize, kInsertSmem) == cudaSuccess;
-  ok = ok && vox_seg_alloc(c, m->buf, refilter_bound(m, c)) == ALOAM_OK;
-  // lane 0's set is the context's, whose buffers ensure_map_buffers creates when they are first needed; another lane's set is
-  // created here, after the context's (which fixes the table size)
-  m->reg = lane == 0 ? &c->map : new (std::nothrow) MapReg();
-  if (lane > 0 && m->reg) own(c, [r = m->reg] { delete r; });
+// Fills frame f of a new cube store or locator: its state and pinned mirror, a stack filter of filter_cap points and, unless it
+// registers with `shared`, a registration set of `queries` points with grid tables of `slots` slots over submaps of `bound`
+// points per type (map_reg_alloc; 0 slots: none).  f.mem takes the buffers only when every allocation succeeded; on a failure
+// they are freed at once and f is to be discarded.
+static int frame_alloc(aloam_ctx* c, LaneFrame& f, MapReg* shared, size_t queries, size_t bound, unsigned slots, size_t filter_cap) {
   BufGroup g;
-  ok = ok && m->reg &&
-       (lane == 0 || (ensure_map_buffers(c) == ALOAM_OK &&
-                      map_reg_alloc(g, m->reg, (size_t)2 * c->max_points, (size_t)c->max_map, (unsigned)c->map_slots) == ALOAM_OK));
-  if (!ok) {   // publish nothing half-built: what was acquired belongs to the context until aloam_destroy, the set's group is freed
-    cudaGetLastError();
-    return ALOAM_ERR_CUDA;
-  }
-  own(c, std::move(g));
-  const int rc = reset_lane(c, m);   // a lane is published with the state of a fresh trajectory, never uninitialised
-  if (rc) return rc;
-  c->lanes[lane].mapper = m;
+  bool ok = stack_stream_ensure(c) == cudaSuccess && g.dev(&f.d_state, 1) && g.pinned(&f.h_state, 1);
+  ok = ok && (shared || map_reg_alloc(g, &f.set, queries, bound, slots) == ALOAM_OK) && vox_seg_alloc(c, g, f.buf, filter_cap) == ALOAM_OK;
+  if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+  f.mem = std::move(g);
+  f.reg = shared ? shared : &f.set;
   return ALOAM_OK;
 }
 
-// a new locator in *out, published only when fully allocated (what was acquired before a failure belongs to the context until
-// aloam_destroy)
-int locator_create(aloam_ctx* c, Locator** out) {
-  if (stack_stream_ensure(c) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
-  Locator* m = new (std::nothrow) Locator();
+int mapper_ensure(aloam_ctx* c, int lane) {
+  if (c->lanes[lane].mapper) return ALOAM_OK;
+  if (c->cfg.max_map_points <= 0) return ALOAM_ERR_CAPACITY;
+  // lane 0 registers with the context's set, whose buffers ensure_map_buffers creates when they are first needed; another lane's
+  // set is sized by the context's, which is created first
+  if (lane > 0 && ensure_map_buffers(c) != ALOAM_OK) return ALOAM_ERR_CUDA;
+  std::unique_ptr<Mapper> m(new (std::nothrow) Mapper());
   if (!m) return ALOAM_ERR_CUDA;
-  own(c, [m] { delete m; });
-  BufGroup g;
-  bool ok = dalloc(c, &m->d_state, 1) == cudaSuccess && halloc(c, &m->h_state, 1) == cudaSuccess;
-  ok = ok && map_reg_alloc(g, &m->reg, (size_t)2 * c->max_points, 0, 0) == ALOAM_OK && vox_seg_alloc(c, m->buf, (size_t)2 * c->max_points) == ALOAM_OK;
-  ok = ok && cudaMemset(m->d_state, 0, sizeof(MapperState)) == cudaSuccess;
+  mapper_slab_caps(c, m->cap);
+  m->max_sub = c->cfg.max_map_points;
+  const size_t mp = (size_t)c->max_points;
+  BufGroup& g = m->mem;
+  bool ok = true;
+  for (int t = 0; t < 2 && ok; ++t) ok = g.dev(&m->d_pts[t], (size_t)kPool * m->cap[t]) && g.dev(&m->d_sub[t], (size_t)m->max_sub) && g.dev(&m->d_in[t], mp);
+  ok = ok && g.dev(&m->d_world, 2 * mp) && g.dev(&m->d_cube, 2 * mp) && g.dev(&m->d_pose_io, 16);   // d_world: both stacks side by side
+  ok = ok && cudaFuncSetAttribute(k_cube_insert, cudaFuncAttributeMaxDynamicSharedMemorySize, kInsertSmem) == cudaSuccess;
   if (!ok) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
-  own(c, std::move(g));
-  *out = m;
+  int rc = frame_alloc(c, m->frame, lane == 0 ? &c->map : nullptr, 2 * mp, (size_t)c->max_map, (unsigned)c->map_slots, refilter_bound(m.get(), c));
+  if (rc) return rc;
+  rc = reset_lane(c, m.get());   // a lane is published with the state of a fresh trajectory, never uninitialised
+  if (rc) return rc;
+  Mapper* p = m.release();
+  own(c, [p] { delete p; });
+  c->lanes[lane].mapper = p;
+  return ALOAM_OK;
+}
+
+// a new locator in *out, its state zeroed, published only when complete: a registration set without grid tables and a filter
+// for the two scan stacks
+int locator_create(aloam_ctx* c, LaneFrame** out) {
+  std::unique_ptr<LaneFrame> f(new (std::nothrow) LaneFrame());
+  if (!f) return ALOAM_ERR_CUDA;
+  const size_t q = (size_t)2 * c->max_points;
+  const int rc = frame_alloc(c, *f, nullptr, q, 0, 0, q); if (rc) return rc;
+  if (cudaMemset(f->d_state, 0, sizeof(MapperState)) != cudaSuccess) { cudaGetLastError(); return ALOAM_ERR_CUDA; }
+  LaneFrame* p = f.release();
+  own(c, [p] { delete p; });
+  *out = p;
   return ALOAM_OK;
 }
 
@@ -1737,30 +1745,24 @@ int locator_ensure(aloam_ctx* c, int lane) {
   return c->lanes[lane].locator ? ALOAM_OK : locator_create(c, &c->lanes[lane].locator);
 }
 
-int* locator_err_acc(aloam_ctx* c, int lane) { return &c->lanes[lane].locator->d_state->err_acc; }
-
-LocatorFrame locator_frame(const Locator* m) {
-  const MapperState* S = m->d_state;
-  return LocatorFrame{{m->reg.stack[0], m->reg.stack[1]}, S->stack_counts, &S->flags};
+LaneFrame* lane_frame(const aloam_ctx* c, int lane, bool localise) {
+  const Lane& L = c->lanes[lane];
+  return localise ? L.locator : L.mapper ? &L.mapper->frame : nullptr;
 }
 
-MapperStacks mapper_stacks(const aloam_ctx* c, int lane) {
-  const Mapper* m = c->lanes[lane].mapper;
-  return MapperStacks{{m->reg->stack[0], m->reg->stack[1]}, m->d_state->stack_counts};
+FrameView frame_view(const LaneFrame* f) {
+  MapperState* S = f->d_state;
+  return FrameView{{f->reg->stack[0], f->reg->stack[1]}, S->stack_counts, &S->flags, f->reg->summary, &S->err_acc};
 }
 
 PriorGrid prior_grid(const aloam_ctx* c) { return PriorGrid{c->prior->grid[0], c->prior->grid[1]}; }
 
-int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_upper_c, int n_upper_s) {
+int locator_stacks_device(aloam_ctx* c, LaneFrame* f, const MapperIn& in, int n_upper_c, int n_upper_s) {
   Batch<MapperLane> B = {};
-  MapperState* S = m->d_state;
-  B.a[0].S = S;
-  B.a[0].in[0] = in.corner; B.a[0].in[1] = in.surf; B.a[0].n_in[0] = in.nc; B.a[0].n_in[1] = in.ns;
-  B.a[0].stack[0] = m->reg.stack[0]; B.a[0].stack[1] = m->reg.stack[1];
-  B.a[0].segs = m->buf.segs; B.a[0].n_seg = m->buf.n_seg;
-  const SegFilter f = seg_filter(m->buf, 31, &S->err);
-  SegBuffers* bufs[1] = {&m->buf};
-  const int rc = stack_filters_fork(c, 1, B, &f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
+  SegFilter sf;
+  SegBuffers* bufs[1];
+  B.a[0] = frame_record(f, in, &sf, &bufs[0]);
+  const int rc = stack_filters_fork(c, 1, B, &sf, bufs, n_upper_c, n_upper_s); if (rc) return rc;
   CUDA_CHECK_RET(cudaStreamWaitEvent(c->stream, c->ev_stack_join, 0));
   return ALOAM_OK;
 }
@@ -1771,7 +1773,7 @@ int locator_stacks_device(aloam_ctx* c, Locator* m, const MapperIn& in, int n_up
 // doubles, host memory).  Every launch covers all records: the stack filters (forked, as the mapping frame's), k_locate_begin,
 // the thin-map test, outer_iters x (k_map_knn5_prior, k_map_fit, LM), k_mapper_update, k_mapper_finish (the stack filter's error
 // bit).
-int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const* loc, const double* const* init, int n_upper_c, int n_upper_s) {
+int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, LaneFrame* const* loc, const double* const* init, int n_upper_c, int n_upper_s) {
   const PriorMap* P = c->prior;
   if (nb < 1 || nb > ALOAM_MAX_BATCH || !P || sharded_job(c)) return ALOAM_ERR_STATE;
   Batch<MapperLane> B = {};
@@ -1782,18 +1784,12 @@ int locate_step_device(aloam_ctx* c, int nb, const MapperIn* in, Locator* const*
   PriorSearch ps = {};
   ps.grid = PriorGrid{P->grid[0], P->grid[1]};
   for (int l = 0; l < nb; ++l) {
-    Locator* m = loc[l];
-    MapperState* S = m->d_state;
-    B.a[l].S = S; B.a[l].odom7 = in[l].odom7; B.a[l].out7 = in[l].out7;
-    B.a[l].in[0] = in[l].corner; B.a[l].in[1] = in[l].surf; B.a[l].n_in[0] = in[l].nc; B.a[l].n_in[1] = in[l].ns;
-    B.a[l].stack[0] = m->reg.stack[0]; B.a[l].stack[1] = m->reg.stack[1];
-    B.a[l].segs = m->buf.segs; B.a[l].n_seg = m->buf.n_seg;
+    MapperState* S = loc[l]->d_state;
+    B.a[l] = frame_record(loc[l], in[l], &stack_f[l], &bufs[l]);
     L.a[l].S = S; L.a[l].odom7 = in[l].odom7; L.a[l].fresh = in[l].fresh;
     for (int k = 0; k < 7; ++k) L.a[l].init[k] = init[l][k];
-    io[l] = MapLaneIO{m->reg, {nullptr, nullptr}, S->stack_counts, S->x};
+    io[l] = MapLaneIO{*loc[l]->reg, {nullptr, nullptr}, S->stack_counts, S->x};
     ps.win[l][0] = S->sub_off[0]; ps.win[l][1] = S->sub_off[1]; ps.ctr[l] = S->ctr;
-    stack_f[l] = seg_filter(m->buf, 31, &S->err);
-    bufs[l] = &m->buf;
   }
   // the stack filters share s_stack with the mapping frame's: this fork is recorded after the whole mapping frame of the step
   int rc = stack_filters_fork(c, nb, B, stack_f, bufs, n_upper_c, n_upper_s); if (rc) return rc;
@@ -1812,7 +1808,7 @@ int locator_prior_search(aloam_ctx* c, int lane, PriorSearch* ps) {
   const PriorMap* P = c->prior;
   const Lane& L = c->lanes[lane];
   if (!P || !L.window) return ALOAM_ERR_STATE;
-  MapperState* S = L.locator->d_state;
+  MapperState* S = lane_frame(c, lane, true)->d_state;
   *ps = {};
   ps->grid = PriorGrid{P->grid[0], P->grid[1]};
   ps->win[0][0] = S->sub_off[0]; ps->win[0][1] = S->sub_off[1]; ps->ctr[0] = S->ctr;
@@ -1851,7 +1847,7 @@ int prior_map_identity(aloam_ctx* c, int cen[3], long long n[2], unsigned long l
 }
 
 int locator_map_pose(aloam_ctx* c, int lane, double* dst) {
-  const MapperState* S = c->lanes[lane].locator->d_state;
+  const MapperState* S = lane_frame(c, lane, true)->d_state;
   CUDA_CHECK_RET(cudaMemcpyAsync(dst, S->q_wmap_wodom, 4 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(dst + 4, S->t_wmap_wodom, 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   return ALOAM_OK;
@@ -1859,7 +1855,7 @@ int locator_map_pose(aloam_ctx* c, int lane, double* dst) {
 
 int locator_restore(aloam_ctx* c, int lane, const double T[7]) {
   const PriorMap* P = c->prior;
-  MapperState* S = c->lanes[lane].locator->d_state;
+  MapperState* S = lane_frame(c, lane, true)->d_state;
   Pose7 p;
   for (int k = 0; k < 7; ++k) p.v[k] = T[k];
   CUDA_CHECK_RET(cudaMemsetAsync(S, 0, sizeof(MapperState), c->stream));
@@ -2032,18 +2028,18 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   rc = upload_cloud(c, corner_last, m->d_in[0], c->max_points); if (rc) return rc;
   rc = upload_cloud(c, surf_last, m->d_in[1], c->max_points); if (rc) return rc;
   c->pin->mapper_counts[0] = corner_last.n; c->pin->mapper_counts[1] = surf_last.n;
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->d_state->in_counts, c->pin->mapper_counts, 8, cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->frame.d_state->in_counts, c->pin->mapper_counts, 8, cudaMemcpyHostToDevice, c->stream));
   for (int k = 0; k < 4; ++k) c->pin->mapper_pose_in[k] = q_wodom_curr[k];
   for (int k = 0; k < 3; ++k) c->pin->mapper_pose_in[4 + k] = t_wodom_curr[k];
   CUDA_CHECK_RET(cudaMemcpyAsync(m->d_pose_io, c->pin->mapper_pose_in, 56, cudaMemcpyHostToDevice, c->stream));
-  const MapperIn one{m->d_in[0], &m->d_state->in_counts[0], m->d_in[1], &m->d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7, 0, 0};
+  const MapperIn one{m->d_in[0], &m->frame.d_state->in_counts[0], m->d_in[1], &m->frame.d_state->in_counts[1], m->d_pose_io, m->d_pose_io + 7, 0, 0};
   rc = peer_err_reset(c); if (rc) return rc;
   rc = mapper_step_device(c, 1, &one, corner_last.n, surf_last.n);
   if (rc) return rc;
   CUDA_CHECK_RET(cudaMemcpyAsync(c->pin->mapper_pose_out, m->d_pose_io + 7, 56, cudaMemcpyDeviceToHost, c->stream));
   rc = peer_err_fetch(c, &c->pin->peer_err); if (rc) return rc;
-  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, m->reg->summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_CHECK_RET(cudaMemcpyAsync(&m->h_state->flags, &m->d_state->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(c->h_summary, m->frame.reg->summary, sizeof(LmSummary) * 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(&m->frame.h_state->flags, &m->frame.d_state->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaEventRecord(c->ev1, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
@@ -2051,8 +2047,8 @@ int aloam_mapper_step(aloam_ctx* c, aloam_cloud_view corner_last, aloam_cloud_vi
   for (int k = 0; k < 4; ++k) q_w_curr[k] = c->pin->mapper_pose_out[k];
   for (int k = 0; k < 3; ++k) t_w_curr[k] = c->pin->mapper_pose_out[4 + k];
   float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-  frame_stats_from(c->h_summary, stats, c->cfg.outer_iters, m->h_state->flags, ms);
-  if (m->h_state->frame_err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
+  frame_stats_from(c->h_summary, stats, c->cfg.outer_iters, m->frame.h_state->flags, ms);
+  if (m->frame.h_state->frame_err & 1) return ALOAM_ERR_CAPACITY;   // a voxel index range beyond the key width: results would be wrong
   if (c->pin->peer_err) return ALOAM_ERR_COMM;                // a peer did not answer: the pose rests on a partial sum
   return ALOAM_OK;
 }
@@ -2065,12 +2061,11 @@ int aloam_mapper_debug_state_lane(aloam_ctx* c, int lane, int centre[3], int* n_
   // a lane whose trajectory localises answers from its locator, with the totals of the prior map it reads
   const Lane& L = c->lanes[lane];
   const bool loc = L.sched.localising && L.locator && c->prior;
-  if (!loc && !L.mapper) return ALOAM_ERR_STATE;
-  MapperState* d_state = loc ? L.locator->d_state : L.mapper->d_state;
-  MapperState* h_state = loc ? L.locator->h_state : L.mapper->h_state;
+  const LaneFrame* f = lane_frame(c, lane, loc);
+  if (!f) return ALOAM_ERR_STATE;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  CUDA_CHECK_RET(cudaMemcpy(h_state, d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
-  const MapperState* h = h_state;
+  CUDA_CHECK_RET(cudaMemcpy(f->h_state, f->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
+  const MapperState* h = f->h_state;
   if (centre) for (int a = 0; a < 3; ++a) centre[a] = h->cen[a];
   if (n_valid) *n_valid = h->n_valid;
   if (valid) for (int i = 0; i < h->n_valid && i < 125; ++i) valid[i] = h->valid[i];
@@ -2095,9 +2090,9 @@ int aloam_mapper_debug_cube_lane(aloam_ctx* c, int lane, int which, int cube, al
   if (lane >= c->n_lanes || !c->lanes[lane].mapper) return ALOAM_ERR_STATE;
   Mapper* m = c->lanes[lane].mapper;
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
-  CUDA_CHECK_RET(cudaMemcpy(m->h_state, m->d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
-  const int s = m->h_state->slab_of[which][cube];
-  const int n = s < 0 ? 0 : m->h_state->cnt[which][s];
+  CUDA_CHECK_RET(cudaMemcpy(m->frame.h_state, m->frame.d_state, sizeof(MapperState), cudaMemcpyDeviceToHost));
+  const int s = m->frame.h_state->slab_of[which][cube];
+  const int n = s < 0 ? 0 : m->frame.h_state->cnt[which][s];
   // a cube beyond max_points (cube growth) is read into a pinned buffer of ALOAM_MAX_CUBE_POINTS points, created on first use
   if (n > c->max_points && !c->h_cube) CUDA_CHECK_RET(halloc(c, &c->h_cube, (size_t)ALOAM_MAX_CUBE_POINTS));
   Pt4* h = n > c->max_points ? c->h_cube : c->h_out[4];
@@ -2154,11 +2149,14 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
   CUDA_CHECK_RET(cudaSetDevice(c->cfg.device));
   int rc = mapper_ensure(c, 0); if (rc) return rc;
   Mapper* m = c->lanes[0].mapper;
-  if (total > m->buf.cap) return ALOAM_ERR_CAPACITY;
-  if (!m->d_dbg_err) {   // first use; the pointer that marks the group as ready is allocated last
-    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_pts, m->buf.cap));
-    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_counts, ALOAM_MAX_SEGS));
-    CUDA_CHECK_RET(dalloc(c, &m->d_dbg_err, 1));
+  if (total > m->frame.buf.cap) return ALOAM_ERR_CAPACITY;
+  if (!m->d_dbg_err) {   // first use: the group is published complete
+    BufGroup g;
+    Pt4* pts;
+    int *counts, *e;
+    if (!g.dev(&pts, m->frame.buf.cap) || !g.dev(&counts, ALOAM_MAX_SEGS) || !g.dev(&e, 1)) return ALOAM_ERR_CUDA;
+    m->dbg = std::move(g);
+    m->d_dbg_pts = pts; m->d_dbg_counts = counts; m->d_dbg_err = e;
   }
   // the segments back to back, filtered in place like the cubes of the re-filter; the mapper state is not touched (the
   // descriptors, offsets and sort buffers are scratch that every frame rewrites before use)
@@ -2166,20 +2164,20 @@ int aloam_debug_seg_voxel_filter(aloam_ctx* c, const aloam_cloud_view* segs, con
   int counts[ALOAM_MAX_SEGS];
   size_t off = 0;
   for (int s = 0; s < n_segs; ++s) {
-    rc = upload_cloud(c, segs[s], m->d_dbg_pts + off, (int)(m->buf.cap - off)); if (rc) return rc;
+    rc = upload_cloud(c, segs[s], m->d_dbg_pts + off, (int)(m->frame.buf.cap - off)); if (rc) return rc;
     desc[s] = SegDesc{m->d_dbg_pts + off, m->d_dbg_counts + s, leaves[s], m->d_dbg_pts + off, m->d_dbg_counts + s};
     counts[s] = segs[s].n;
     off += (size_t)segs[s].n;
   }
   if (n_segs > 0) {
-    CUDA_CHECK_RET(cudaMemcpyAsync(m->buf.segs, desc, sizeof(SegDesc) * n_segs, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK_RET(cudaMemcpyAsync(m->frame.buf.segs, desc, sizeof(SegDesc) * n_segs, cudaMemcpyHostToDevice, c->stream));
     CUDA_CHECK_RET(cudaMemcpyAsync(m->d_dbg_counts, counts, sizeof(int) * n_segs, cudaMemcpyHostToDevice, c->stream));
   }
-  CUDA_CHECK_RET(cudaMemcpyAsync(m->buf.n_seg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CUDA_CHECK_RET(cudaMemcpyAsync(m->frame.buf.n_seg, &n_segs, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_CHECK_RET(cudaMemsetAsync(m->d_dbg_err, 0, sizeof(int), c->stream));
   if (n_segs > 0) {
-    const SegFilter f = seg_filter(m->buf, idx_bits, m->d_dbg_err);
-    SegBuffers* bp = &m->buf;
+    const SegFilter f = seg_filter(m->frame.buf, idx_bits, m->d_dbg_err);
+    SegBuffers* bp = &m->frame.buf;
     vox_seg_filter(c, 1, &f, &bp, n_segs, (int)std::max<size_t>(total, 1), std::max(per_seg, 1));
   }
   CUDA_CHECK_RET(cudaGetLastError());

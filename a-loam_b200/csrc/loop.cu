@@ -317,7 +317,7 @@ int loop_record_device(aloam_ctx* c, int nb, const MapperIn* in, const aloam_pla
   for (int l = 0; l < nb; ++l) {
     const int lane = in[l].lane;
     const LoopLane& L = Lp->lanes[lane];
-    const MapperStacks S = mapper_stacks(c, lane);
+    const FrameView S = frame_view(lane_frame(c, lane, false));
     LoopRowRec* row = Lp->d_rows + r0 + lane;
     K.a[l] = LoopKeep{prow[l], row, {S.stack[0], S.stack[1]}, S.counts, L.pool, L.pool_n};
     B.a[l] = lane_rec(c, lane);

@@ -104,7 +104,7 @@ int recover_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* const* r
   for (int l = 0; l < nb; ++l) {
     const int lane = in[l].lane;
     double* cs = R->d_cand + (size_t)lane * R->cap * 7;
-    const LocatorFrame F = locator_frame(c->lanes[lane].locator);
+    const FrameView F = frame_view(lane_frame(c, lane, true));
     C.a[l] = RecoverCand{rows[l], in[l].out7, cs};
     S.a[l] = RelocRec{cs, R->n_delta, {F.stack[0], F.stack[1]}, F.counts, R->d_score + (size_t)lane * R->cap,
                       R->d_part + (size_t)lane * R->ctas_cap * kRelocTop, R->d_best + (size_t)lane * kRelocTop, &rows[l]->rec_triggered};

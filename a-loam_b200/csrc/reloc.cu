@@ -39,7 +39,7 @@ constexpr int kMaxHyp = 1 << 24;
 // (group `hyps`); the others are group `mem`.
 struct aloam::Relocaliser {
   BufGroup mem, hyps;
-  Locator* loc[ALOAM_MAX_BATCH] = {};
+  LaneFrame* loc[ALOAM_MAX_BATCH] = {};
   int n_loc = 0;
   Pt4* d_in[2] = {nullptr, nullptr};
   int* d_n = nullptr;                       // [2] the clouds' sizes
@@ -246,7 +246,7 @@ int reloc_ensure(aloam_ctx* c, int k, int n_hyp) {
 
 // the one-record, ungated set of aloam_prior_relocalise: n poses at d_pose scored on its stacks into d_score, best keys per CTA into
 // part when it is set
-RelocRec reloc_set(const Relocaliser* R, const LocatorFrame& F, const double* d_pose, int n, int* d_score, unsigned long long* part) {
+RelocRec reloc_set(const Relocaliser* R, const FrameView& F, const double* d_pose, int n, int* d_score, unsigned long long* part) {
   return RelocRec{d_pose, n, {F.stack[0], F.stack[1]}, F.counts, d_score, part, R->d_best, nullptr};
 }
 
@@ -280,7 +280,7 @@ extern "C" int aloam_prior_relocalise(aloam_ctx* c, aloam_cloud_view less_sharp,
   MapperIn rec[ALOAM_MAX_BATCH];
   for (int r = 0; r < K; ++r) rec[r] = MapperIn{R->d_in[0], R->d_n, R->d_in[1], R->d_n + 1, c->d_ident, R->d_pose + 7 * r, 0, 1, 1};
   rc = locator_stacks_device(c, R->loc[0], rec[0], n_up_c, n_up_s); if (rc) return rc;
-  const LocatorFrame F = locator_frame(R->loc[0]);
+  const FrameView F = frame_view(R->loc[0]);
   // ---- coarse scores and the K best
   const int ctas = std::max(1, std::min(R->ctas, (n_hyp + kRelocWarps - 1) / kRelocWarps));
   Batch<RelocRec> B = {};
@@ -291,7 +291,7 @@ extern "C" int aloam_prior_relocalise(aloam_ctx* c, aloam_cloud_view less_sharp,
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   int win[ALOAM_MAX_BATCH], win_score[ALOAM_MAX_BATCH];
-  Locator* lp[ALOAM_MAX_BATCH];
+  LaneFrame* lp[ALOAM_MAX_BATCH];
   const double* init[ALOAM_MAX_BATCH];
   for (int r = 0; r < K; ++r) {
     win[r] = (int)~(unsigned)(H->best[r] & 0xffffffffull);
@@ -305,7 +305,7 @@ extern "C" int aloam_prior_relocalise(aloam_ctx* c, aloam_cloud_view less_sharp,
   reloc_score_device(c, 1, B, (K + kRelocWarps - 1) / kRelocWarps, o.max_score_points, o.inlier_sq);
   CUDA_CHECK_RET(cudaMemcpyAsync(H->pose, R->d_pose, sizeof(double) * 7 * K, cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaMemcpyAsync(H->rscore, R->d_rscore, sizeof(int) * K, cudaMemcpyDeviceToHost, c->stream));
-  for (int r = 0; r < K; ++r) CUDA_CHECK_RET(cudaMemcpyAsync(H->flags[r], locator_frame(R->loc[r]).flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  for (int r = 0; r < K; ++r) CUDA_CHECK_RET(cudaMemcpyAsync(H->flags[r], frame_view(R->loc[r]).flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_CHECK_RET(cudaStreamSynchronize(c->stream));
   CUDA_CHECK_RET(cudaGetLastError());
   if (scores) CUDA_CHECK_RET(cudaMemcpy(scores, R->d_score, (size_t)n_hyp * sizeof(int), cudaMemcpyDeviceToHost));

@@ -15,7 +15,7 @@ int track_score_device(aloam_ctx* c, int nb, const MapperIn* in, MapRowRec* cons
   const PriorGrid G = prior_grid(c);
   Batch<ScoreRec> B = {};
   for (int l = 0; l < nb; ++l) {
-    const LocatorFrame F = locator_frame(c->lanes[in[l].lane].locator);
+    const FrameView F = frame_view(lane_frame(c, in[l].lane, true));
     B.a[l] = ScoreRec{{F.stack[0], F.stack[1]}, F.counts, in[l].out7, {G.corner, G.surf}, &rows[l]->score};
   }
   const int max_pts = c->rows_max_score;

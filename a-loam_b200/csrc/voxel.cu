@@ -491,20 +491,16 @@ int vox_radix_sort(aloam_ctx* c, int kid, unsigned* k0, int* v0, unsigned* k1, i
 }
 size_t vox_radix_hist_ints(int n) { return (size_t)std::max(1, (n + VCH - 1) / VCH) * 256; }
 
-int vox_seg_alloc(aloam_ctx* c, SegBuffers& b, size_t cap) {
+int vox_seg_alloc(aloam_ctx* c, BufGroup& g, SegBuffers& b, size_t cap) {
   const size_t nb = (cap + VCH - 1) / VCH + 1;
   int per_sm = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort_all, VT, 0);
   b.cap = cap;
   b.coop_grid = std::max(1, std::min(c->sms, per_sm * c->sms));
-  if (dalloc(c, &b.segs, ALOAM_MAX_SEGS) != cudaSuccess || dalloc(c, &b.n_seg, 1) != cudaSuccess ||
-      dalloc(c, &b.off, ALOAM_MAX_SEGS + 8) != cudaSuccess || dalloc(c, &b.rank0, ALOAM_MAX_SEGS + 8) != cudaSuccess ||
-      dalloc(c, &b.bbox, ALOAM_MAX_SEGS * 6) != cudaSuccess || dalloc(c, &b.total, 1) != cudaSuccess ||
-      dalloc(c, &b.pass, ALOAM_MAX_SEGS) != cudaSuccess ||
-      dalloc(c, &b.keys[0], cap) != cudaSuccess || dalloc(c, &b.keys[1], cap) != cudaSuccess ||
-      dalloc(c, &b.vals[0], cap) != cudaSuccess || dalloc(c, &b.vals[1], cap) != cudaSuccess ||
-      dalloc(c, &b.hist, nb * 256) != cudaSuccess || dalloc(c, &b.block_heads, nb) != cudaSuccess ||
-      dalloc(c, &b.heads_total, 1) != cudaSuccess || dalloc(c, &b.tmp, cap) != cudaSuccess)
+  if (!g.dev(&b.segs, ALOAM_MAX_SEGS) || !g.dev(&b.n_seg, 1) || !g.dev(&b.off, ALOAM_MAX_SEGS + 8) || !g.dev(&b.rank0, ALOAM_MAX_SEGS + 8) ||
+      !g.dev(&b.bbox, ALOAM_MAX_SEGS * 6) || !g.dev(&b.total, 1) || !g.dev(&b.pass, ALOAM_MAX_SEGS) || !g.dev(&b.keys[0], cap) ||
+      !g.dev(&b.keys[1], cap) || !g.dev(&b.vals[0], cap) || !g.dev(&b.vals[1], cap) || !g.dev(&b.hist, nb * 256) ||
+      !g.dev(&b.block_heads, nb) || !g.dev(&b.heads_total, 1) || !g.dev(&b.tmp, cap))
     return ALOAM_ERR_CUDA;
   return ALOAM_OK;
 }
@@ -520,12 +516,14 @@ extern "C" int aloam_voxel_filter(aloam_ctx* c, aloam_cloud_view in, float leaf,
   if (!c->h_vox_out) CUDA_CHECK_RET(halloc(c, &c->h_vox_out, (size_t)c->max_points));
   out->data = reinterpret_cast<const float*>(c->h_vox_out); out->n = 0; out->stride_floats = 4;
   if (in.n == 0) return ALOAM_OK;
-  if (!c->vox_seg_ready) {   // publish nothing half-built: what a failed attempt acquired belongs to the context until aloam_destroy
-    if (dalloc(c, &c->d_seg_io, 3) != cudaSuccess || vox_seg_alloc(c, c->vox_seg, (size_t)c->max_points) != ALOAM_OK) {
-      cudaGetLastError();
-      return ALOAM_ERR_CUDA;
-    }
-    c->vox_seg_ready = true;
+  if (!c->d_seg_io) {   // first use: the filter and its io words, one group published complete
+    BufGroup g;
+    SegBuffers b;
+    int* io;
+    if (!g.dev(&io, 3) || vox_seg_alloc(c, g, b, (size_t)c->max_points) != ALOAM_OK) return ALOAM_ERR_CUDA;
+    own(c, std::move(g));
+    c->vox_seg = b;
+    c->d_seg_io = io;
   }
   Pt4* d_in = c->d_query;        // staging buffers that already exist in the context
   Pt4* d_out = c->lanes[0].d_full[0];
